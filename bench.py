@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Benchmark of the contrastive training step (BASELINE.json metric: 3 s-segments/sec).
 
-    python bench.py --gpus N --steps K --warmup W [--config cfg2|cfg3|cfg4|cfg5]   # B200 arm (this repo's CUDA path)
+    python bench.py --gpus N --steps K --warmup W [--config cfg2|cfg3|cfg4|cfg5]   # this repo's CUDA path
+                    [--dump-outputs DIR]                                           # + what the last timed step computed
     python bench.py --impl reference --gpus N --steps K --warmup W                 # reference arm: the reference's OWN
                                                                                    # modules on the host cores
 
@@ -52,7 +53,7 @@ def load_peaks():
             p = json.load(f)
         return dict(hbm_gbs=p["hbm_gbs"], bf16_tflops=p["bf16_tflops"],
                     bf16_tflops_sustained=p.get("bf16_tflops_sustained", p["bf16_tflops"]), source="measured")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, bf16_tflops_sustained=1400.0, source="fallback")
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, bf16_tflops_sustained=989.0, source="H100 SXM data sheet (not measured)")
 
 
 def host_threads() -> int:
@@ -143,7 +144,7 @@ def run_b200(args):
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
-    assert torch.cuda.is_available(), "bench.py needs a CUDA device (no CPU fallback for the B200 arm)"
+    assert torch.cuda.is_available(), "bench.py needs a CUDA device (no CPU fallback for the CUDA arm)"
     torch.cuda.set_device(local_rank)
     dev = torch.device("cuda", local_rank)
     if world > 1:
@@ -179,6 +180,8 @@ def run_b200(args):
     def make_batch(meg_d, subj_d, subj_h):
         return synthetic.SyntheticBatch(meg_d, subj_d, [recs[s] for s in subj_h])
 
+    last = {}                                   # the most recent step's estimate and loss (--dump-outputs)
+
     def step(meg_d, feats_d, subj_d, subj_h):
         opt.zero_grad(set_to_none=True)
         batch = make_batch(meg_d, subj_d, subj_h)
@@ -189,6 +192,7 @@ def run_b200(args):
         if world > 1 and diag_step != "no_allreduce":      # (BM_STEP_DIAG: diagnostic only)
             distrib.sync_gradients(model.parameters())
         opt.step()
+        last["estimate"], last["loss"] = est, loss
         return loss
 
     def barrier():
@@ -243,6 +247,8 @@ def run_b200(args):
     host_ms_value = host_ms[0]        # >= ms_per_step would mean the host, not the GPU, paces the step
     clocks = sampler.stop() if rank == 0 else None
     ms_per_step = ms_total / args.steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last, model)
     value = world * B / (ms_per_step / 1e3)
 
     # ---- end to end through the public API with HOST buffers (`e2e`) ------------------------------------
@@ -378,15 +384,38 @@ def run_b200(args):
         ms_per_step=ms_per_step, higher_is_better=True, scaling=scaling, vs_baseline=None, dtype="f32", data="synthetic",
         config=dict(workload=cfg["name"], batch_per_gpu=B, global_batch=B * world, sensors=C, T=T, F=F,
                     subjects=S, model="clip_conv (random init)", negatives="global (all-gather)" if world > 1 else "local",
-                    arithmetic="fp32-faithful (parity 1e-4): every product = 3 tensor-core MMAs over two-piece operands, fp32 "
-                               "accumulation in tensor memory -- fp16 pieces on tcgen05 kind::f16 (convs, weight gradients), "
-                               "tf32 pieces on kind::tf32 (CLIP, grouped / per-sample 1x1); elementwise in fp32",
-                    l2=f"per-step working set (inputs {h2d / 1e6:.0f} MB + ~{act_gb:.1f} GB saved activations) >> 126 MB L2; "
+                    arithmetic="fp32-faithful (parity 1e-4): every product = 3 wgmma tf32 MMAs over two-piece operands, "
+                               "each 32-wide K block accumulated into a round-to-nearest fp32 sum; elementwise in fp32",
+                    l2=f"per-step working set (inputs {h2d / 1e6:.0f} MB + ~{act_gb:.1f} GB saved activations) >> 50 MB L2; "
                        "two input batches rotate",
                     last_loss=last_loss[0]),
         host_enqueue_ms_per_step=host_ms_value, step_ms=step_ms,
         clocks=clocks, e2e=e2e, gpu_launches=int(launches), roofline=roofline, cpu_baseline=cpu_baseline, also=also)
     emit(json.dumps(out))
+
+
+def dump_outputs(out_dir, last, model, budget_bytes=64 << 20, sample=1 << 20):
+    """Writes what the last timed step returned to its caller -- the loss, the estimate and every parameter's gradient (the
+    Adam update is a function of these) -- as float32 .npy files.  A tensor above `sample` elements is represented by a
+    fixed sample of its flattened elements (indices drawn from a generator seeded by the tensor's name, identical from run
+    to run and build to build), so that the files stay under `budget_bytes` in all."""
+    import zlib
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = [("loss", last["loss"]), ("estimate", last["estimate"])]
+    arrays += [("grad." + n, p.grad) for n, p in model.named_parameters() if p.grad is not None]
+    total = 0
+    for name, t in arrays:
+        flat = t.detach().reshape(-1)
+        if flat.numel() > sample:
+            g = torch.Generator().manual_seed(zlib.crc32(name.encode()))
+            idx = torch.randint(0, flat.numel(), (sample,), generator=g).sort().values.to(flat.device)
+            flat, name = flat[idx], name + ".sample"
+        a = flat.float().cpu().numpy().reshape(t.shape if flat.numel() == t.numel() else (-1,))
+        total += a.nbytes
+        if total > budget_bytes:
+            raise RuntimeError(f"--dump-outputs: more than {budget_bytes} bytes")
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def also_measured(cfg, model, clip, make_batch, resident, host, n_host, mask, dev, B, iters=5):
@@ -481,7 +510,7 @@ def ncu_traffic_bytes(pattern):
 def _time_kernel(fns, flush=None, iters=24, skip=4):
     """Mean duration of one launch, the way the training step runs it: back to back on the launching stream, CUDA events
     around `iters` launches.  `fns` = the same launch over ROTATING operand sets whose combined footprint is several times
-    the 126 MB L2 (timing rule: inputs larger than L2), so no launch finds its operands cached by the previous one."""
+    the 50 MB L2 (timing rule: inputs larger than L2), so no launch finds its operands cached by the previous one."""
     if callable(fns):
         fns = [fns]
     for i in range(skip):
@@ -526,20 +555,20 @@ def kernel_rooflines(dev, B, T, F, Bc, H=320, Kw=3):
     stats = torch.empty(2 * H, device=dev, dtype=torch.float64)
 
     def tensor_entry(kernel, ms, flops, alg_bytes, traffic, pipe="tf32"):
-        """`frac` is against the measured dense bf16 peak.  An fp32-faithful product needs three MMAs (hi*hi + lo*hi + hi*lo):
-        on kind::tf32 (half the bf16 rate) the ceiling of `frac` is 1/6, on kind::f16 it is 1/3 -- `frac_of_scheme_ceiling`."""
+        """`frac` is against the dense bf16 peak.  An fp32-faithful product needs three MMAs (hi*hi + lo*hi + hi*lo): on
+        tf32 (half the bf16 rate) the ceiling of `frac` is 1/6 -- `frac_of_scheme_ceiling`."""
         ach = flops / (ms / 1e3) / 1e12
         ceil = peak_tf / (6 if pipe == "tf32" else 3)
         return dict(kernel=kernel, bound="tensor", achieved=ach, peak=peak_tf, unit="TFLOP/s", frac=ach / peak_tf,
                     traffic=traffic, algorithmic_bytes=alg_bytes, ms_per_launch=ms,
-                    peak_source=src + " cuBLAS bf16 burst (MEASURED_PEAKS.json)", pipe="kind::" + pipe,
+                    peak_source=src + " (dense bf16)", pipe="wgmma " + pipe,
                     executed_tflops_bf16_equivalent=(6 if pipe == "tf32" else 3) * ach, frac_of_scheme_ceiling=ach / ceil)
 
     def hbm_entry(kernel, ms, alg_bytes, traffic):
         ach = alg_bytes / (ms / 1e3) / 1e9
         return dict(kernel=kernel, bound="hbm", achieved=ach, peak=peak_gb, unit="GB/s", frac=ach / peak_gb,
                     traffic=traffic, algorithmic_bytes=alg_bytes, ms_per_launch=ms,
-                    peak_source=src + " copy bandwidth (MEASURED_PEAKS.json)")
+                    peak_source=src + " (HBM bandwidth)")
 
     def f16_weights(w_op):
         amax = torch.empty(1, device=dev)
@@ -554,7 +583,7 @@ def kernel_rooflines(dev, B, T, F, Bc, H=320, Kw=3):
         call("bm_amax", ptr(t), t.numel(), ptr(cell), st)
         return cell
 
-    # the kernels the training step runs: the persistent CTA-pair conv on the F16 pipe (bm_tc_conv1d_f16)
+    # the conv through the fp16-piece entry point (bm_tc_conv1d_f16; the same engine as the fp32 entry point below)
     fh, fl, fa = f16_weights(f)
     gh, gl, ga = f16_weights(g)
     fgh, fgl, fga = f16_weights(fg)
@@ -563,29 +592,28 @@ def kernel_rooflines(dev, B, T, F, Bc, H=320, Kw=3):
     ms = _time_kernel([lambda x=x, y=y, a=a: call("bm_tc_conv1d_f16", ptr(x), ptr(a), ptr(fh), ptr(fl), ptr(fa), ptr(bias), 0, B, T,
                                                   H, H, Kw, 4, 1, 0, 0, 0, ptr(y), None, None, ptr(stats), None, ptr(status), st)
                        for x, y, a in zip(xs, ys, xa)])
-    main = tensor_entry("conv_hp_kernel via bm_tc_conv1d_f16 (K3: Conv1d 320->320 k3 d4 + BatchNorm statistics; persistent CTA "
-                        "pairs, tcgen05 cta_group::2 kind::f16, fp32 operands as fp16 hi/lo pieces)", ms,
-                        2.0 * H * H * Kw * T * B, 2.0 * B * T * H * 4, ncu_traffic_bytes("convh"), pipe="f16")
+    main = tensor_entry("hg_gemm_kernel<ConvOp> via bm_tc_conv1d_f16 (K3: Conv1d 320->320 k3 d4 + BatchNorm statistics; "
+                        "wgmma 3xTF32, weights as fp16 hi/lo pieces)", ms,
+                        2.0 * H * H * Kw * T * B, 2.0 * B * T * H * 4, ncu_traffic_bytes("convh"))
     main["note"] = ("achieved = ALGORITHMIC fp32 FLOPs (2*320*320*3*T*B per launch) / time; fp32-faithful parity (1e-4) takes "
-                    "three MMAs per product, so the ceiling of `frac` is 1/3 on kind::f16 (1/6 on kind::tf32): see "
-                    "frac_of_scheme_ceiling")
+                    "three tf32 MMAs per product, so the ceiling of `frac` is 1/6: see frac_of_scheme_ceiling")
     others = []
     try:
         ms = _time_kernel([lambda x=x, y=y, a=a: call("bm_tc_conv1d_f16", ptr(x), ptr(a), ptr(fgh), ptr(fgl), ptr(fga), None, 0,
                                                       B, T, H, 2 * H, Kw, 1, 1, 1, 0, 0, ptr(h), None, ptr(y), None,
                                                       ptr(out_amax), ptr(status), st) for x, y, a in zip(xs, ys, xa)])
-        others.append(tensor_entry("conv_hp_kernel GLU mode (K4: Conv1d 320->640 k3 + GLU, h saved, max |out| reported)", ms,
-                                   4.0 * H * H * Kw * T * B, 4.0 * B * T * H * 4, ncu_traffic_bytes("convh_glu"), pipe="f16"))
+        others.append(tensor_entry("hg_gemm_kernel<ConvOp> GLU mode (K4: Conv1d 320->640 k3 + GLU, h saved, max |out| reported)", ms,
+                                   4.0 * H * H * Kw * T * B, 4.0 * B * T * H * 4, ncu_traffic_bytes("convh_glu")))
         ms = _time_kernel([lambda x=x, y=y, a=a: call("bm_tc_conv1d_f16", ptr(x), ptr(a), ptr(gh), ptr(gl), ptr(ga), None, 1, B,
                                                       T, H, H, Kw, 4, -1, 0, 0, 0, ptr(y), None, None, None, None, ptr(status),
                                                       st) for x, y, a in zip(xs, ys, xa)])
-        others.append(tensor_entry("conv_hp_kernel data gradient, y += tile (TMA reduce-add)", ms, 2.0 * H * H * Kw * T * B,
-                                   3.0 * B * T * H * 4, ncu_traffic_bytes("convh_acc"), pipe="f16"))
-        # the 3xTF32 variant of the same kernel (round 2's first half; still what runs where USE_CONV_F16 is off)
+        others.append(tensor_entry("hg_gemm_kernel<ConvOp> data gradient, y += tile (in-place add)", ms, 2.0 * H * H * Kw * T * B,
+                                   3.0 * B * T * H * 4, ncu_traffic_bytes("convh_acc")))
+        # the same conv through the fp32-weight entry point: what the training step runs (functional.USE_CONV_F16 off)
         ms = _time_kernel([lambda x=x, y=y: call("bm_tc_conv1d_persistent", ptr(x), ptr(f), ptr(bias), 0, B, T, H, H, Kw, 4, 1,
                                                  0, 0, 0, ptr(y), None, None, ptr(stats), ptr(status), st)
                            for x, y in zip(xs, ys)])
-        others.append(tensor_entry("conv_pp_kernel via bm_tc_conv1d_persistent (K3 on kind::tf32, 3xTF32: for comparison)", ms,
+        others.append(tensor_entry("hg_gemm_kernel<ConvOp> via bm_tc_conv1d_persistent (K3, fp32 weights: for comparison)", ms,
                                    2.0 * H * H * Kw * T * B, 2.0 * B * T * H * 4, ncu_traffic_bytes("convp")))
         # K6: CLIP scores + candidate norms + softmax / CE / mean at the training shape (Bn = local rows, Bc = global rows)
         KT = F * T
@@ -596,8 +624,8 @@ def kernel_rooflines(dev, B, T, F, Bc, H=320, Kw=3):
         ws = torch.empty(max(int(lib.bm_clip_workspace(B, Bc, KT)), 2), device=dev)
         ms = _time_kernel(lambda: call("bm_clip_loss_fwd", ptr(est), ptr(cand), B, Bc, KT, 0, ptr(inv), ptr(sc), ptr(pr),
                                        ptr(rl), ptr(loss), ptr(ws), ws.numel(), ptr(status), st))
-        e = tensor_entry(f"clip_scores_kernel + clip_finalize_kernel via bm_clip_loss_fwd (K6: {B} x {Bc} x {KT}, norms and "
-                         "softmax/CE fused; split-K CTA pairs, bounded accumulation chains)", ms, 2.0 * B * Bc * KT,
+        e = tensor_entry(f"hg_gemm_kernel<ClipOp> + clip_finalize_kernel via bm_clip_loss_fwd (K6: {B} x {Bc} x {KT}, norms, "
+                         "softmax/CE; split-K, per-block fp32 accumulation)", ms, 2.0 * B * Bc * KT,
                          4.0 * KT * (B + Bc), ncu_traffic_bytes("clip"))
         hbm = 4.0 * KT * (B + Bc) / (ms / 1e3) / 1e9
         e["hbm_view"] = dict(achieved=hbm, peak=peak_gb, unit="GB/s", frac=hbm / peak_gb,
@@ -609,18 +637,19 @@ def kernel_rooflines(dev, B, T, F, Bc, H=320, Kw=3):
         dys = [torch.randn(B, T, H, device=dev) for _ in range(NSETS)]
         dy = dys[0]
         dw = torch.empty(H, H, Kw, device=dev)
-        # the kernel the training step uses for this layer (functional.tc_wgrad's choice): CTA pairs, rows = (tap, x channel)
+        # the weight-gradient GEMM the training step uses for this layer (functional.tc_wgrad): rows = (tap, x channel);
+        # the step calls the fp32 entry point (bm_tc_wgrad_conv), both are timed
         assert lib.bm_tc_wgrad_conv_supported(T, H, H, Kw)
         wsg = torch.empty(int(lib.bm_tc_wgrad_conv_workspace(B, T, H, H, Kw)), device=dev)
         dya = [amax_of(dy) for dy in dys]
         ms = _time_kernel([lambda x=x, dy=dy, a=a, b=b: call("bm_tc_wgrad_conv_f16", ptr(dy), ptr(b), ptr(x), ptr(a), B, T, H, H, H,
                                                              Kw, 4, ptr(wsg), ptr(dw), ptr(status), st)
                            for x, dy, a, b in zip(xs, dys, xa, dya)])
-        others.append(tensor_entry("wgrad_hp_kernel (+reduce) via bm_tc_wgrad_conv_f16 (weight gradient of K3, kind::f16)", ms,
-                                   2.0 * H * H * Kw * T * B, 2.0 * B * T * H * 4, ncu_traffic_bytes("wgradh"), pipe="f16"))
+        others.append(tensor_entry("hg_gemm_kernel<WgradPOp> (+reduce) via bm_tc_wgrad_conv_f16 (weight gradient of K3)", ms,
+                                   2.0 * H * H * Kw * T * B, 2.0 * B * T * H * 4, ncu_traffic_bytes("wgradh")))
         ms = _time_kernel([lambda x=x, dy=dy: call("bm_tc_wgrad_conv", ptr(dy), ptr(x), B, T, H, H, H, Kw, 4, ptr(wsg), ptr(dw),
                                                    ptr(status), st) for x, dy in zip(xs, dys)])
-        others.append(tensor_entry("wgrad_pp_kernel (+reduce) via bm_tc_wgrad_conv (the same on kind::tf32: for comparison)", ms,
+        others.append(tensor_entry("hg_gemm_kernel<WgradPOp> (+reduce) via bm_tc_wgrad_conv (the same entry without amax: for comparison)", ms,
                                    2.0 * H * H * Kw * T * B, 2.0 * B * T * H * 4, ncu_traffic_bytes("wgrad")))
         del wsg
         # ... and of the GLU conv (640 x 320 x 3): the second-largest share of the step after the convs
@@ -630,8 +659,8 @@ def kernel_rooflines(dev, B, T, F, Bc, H=320, Kw=3):
         wsg = torch.empty(int(lib.bm_tc_wgrad_conv_workspace(B, T, 2 * H, H, Kw)), device=dev)
         ms = _time_kernel([lambda x=x, a=a: call("bm_tc_wgrad_conv_f16", ptr(dy2), ptr(dy2a), ptr(x), ptr(a), B, T, 2 * H, H, H,
                                                  Kw, 1, ptr(wsg), ptr(dw2), ptr(status), st) for x, a in zip(xs, xa)])
-        others.append(tensor_entry("wgrad_hp_kernel (+reduce) via bm_tc_wgrad_conv_f16 (weight gradient of K4)", ms,
-                                   2.0 * 2 * H * H * Kw * T * B, 3.0 * B * T * H * 4, None, pipe="f16"))
+        others.append(tensor_entry("hg_gemm_kernel<WgradPOp> (+reduce) via bm_tc_wgrad_conv_f16 (weight gradient of K4)", ms,
+                                   2.0 * 2 * H * H * Kw * T * B, 3.0 * B * T * H * 4, None))
         del wsg, dy2, dw2
         # HBM-bound: BatchNorm + GELU (+skip) backward and forward
         gam, bet = torch.ones(H, device=dev), torch.zeros(H, device=dev)
@@ -639,7 +668,7 @@ def kernel_rooflines(dev, B, T, F, Bc, H=320, Kw=3):
         sums = torch.empty(2 * H, device=dev, dtype=torch.float64)
         dgam, dbet = torch.empty(H, device=dev), torch.empty(H, device=dev)
         rows = B * T
-        amax = torch.empty(1, device=dev)                     # max |output| for the F16-pipe conv downstream, as in the step
+        amax = torch.empty(1, device=dev)                     # max |output| for the fp16-piece conv downstream, as in the step
         ms = _time_kernel([lambda x=x, dy=dy, gy=gy: call("bm_bn_gelu_skip_bwd", ptr(dy), ptr(x), ptr(mean), ptr(invstd),
                                                           ptr(gam), ptr(bet), 1, rows, H, ptr(sums), ptr(gy), ptr(dgam),
                                                           ptr(dbet), ptr(amax), st) for x, dy, gy in zip(xs, dys, ys)])
@@ -658,12 +687,12 @@ def kernel_rooflines(dev, B, T, F, Bc, H=320, Kw=3):
                                 ncu_traffic_bytes("bn_fwd")))
     except Exception as exc:
         others.append(dict(error=f"{type(exc).__name__}: {exc}"))
-    assert int(status.item()) == 0, "a tcgen05 kernel reported a pipeline timeout"
+    assert int(status.item()) == 0, "a tensor-core kernel reported a pipeline timeout"
     return main, others
 
 
 # ------------------------------------------------------------------------------------------------------
-# CPU arm: the reference's own modules (staged under baseline/_ref by oracle/stage_reference.py) on the host cores
+# CPU arm: the reference's own modules (staged under oracle/_ref by build(), oracle/stage_reference.py) on the host cores
 # ------------------------------------------------------------------------------------------------------
 def run_cpu(cfg, steps, warmup, batch, threads):
     """A bounded sample of the workload on the host: `steps` training steps of `batch` segments at the configuration's
@@ -689,7 +718,7 @@ def run_cpu(cfg, steps, warmup, batch, threads):
         def one():
             return tr.step(d["meg"], d["rec_positions"], d["rec_of_sample"], d["subject_index"], d["candidates"], d["ban_centre"])
         kind = "port"
-        what = "oracle/bm_oracle.py CpuTrainer (baseline/_ref not staged), fwd+loss+bwd+Adam"
+        what = "oracle/bm_oracle.py CpuTrainer (oracle/_ref not staged), fwd+loss+bwd+Adam"
     for _ in range(warmup):
         one()
     per = []
@@ -726,8 +755,10 @@ def run_reference(args):
         dtype="f32", data="synthetic",
         config=dict(workload=cfg["name"], batch_per_step=batch, sensors=cfg["C"], T=cfg["T"], F=cfg["F"],
                     subjects=cfg["S"], model="clip_conv (random init)",
-                    note="the reference's own SimpleConv + ClipLoss (unmodified files staged under baseline/_ref by "
-                         "oracle/stage_reference.py) under the restated Solver step; bounded sample of B=64 per step, "
+                    note=("the reference's own SimpleConv + ClipLoss (unmodified files staged under oracle/_ref by build(), "
+                          "oracle/stage_reference.py)" if res["kind"] == "reference" else
+                          "the reference is not staged: the oracle restatement (kind 'port')") +
+                         " under the restated Solver step; bounded sample of B=64 per step, "
                          f"{threads} threads set with torch.set_num_threads (also under torchrun)"),
         cpu_baseline=res, also=also,
         e2e=dict(value=res["value"], unit="segments/s", h2d_bytes_per_step=0, d2h_bytes_per_step=0))
@@ -768,6 +799,8 @@ def main():
     ap.add_argument("--batch", type=int, default=0, help="override the batch per GPU (default: the configuration's)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--lean", action="store_true", help="skip the `also` extras (forward-only, eager-PyTorch bar, B=256 CPU step)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default="",
+                    help="after the timed steps, write what the last one computed (loss, estimate, gradients) as DIR/<name>.npy")
     ap.add_argument("--next-rows", action="store_true",
                     help="instead of the headline step: the SURVEY 8(f) rows (batch preparation, retrieval evaluation, "
                          "DeepMel), each beside a bounded CPU sample of its oracle; one GPU")

@@ -1,4 +1,4 @@
-"""brainmagick_b200: B200-native (sm_100a) drop-in for brainmagick's contrastive training step --
+"""brainmagick_b200: H100-native (sm_90a) drop-in for brainmagick's contrastive training step --
 `SimpleConv` (bm/models/simpleconv.py) and `ClipLoss` (bm/losses.py) behind the reference's module surface -- and for the
 callers either side of it: batch preparation (`norm`: bm/norm.py), the DeepMel feature model (`features`:
 bm/models/features.py) and the retrieval evaluation (`retrieval`: scripts/run_eval_probs.py, bm/wer.py)."""

@@ -96,7 +96,7 @@ def load():
     if not os.path.isfile(LIB_PATH):
         raise BmB200Error(
             f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). brainmagick_b200 has no CPU or PyTorch fallback.")
+            "(nvcc, sm_90a). brainmagick_b200 has no CPU or PyTorch fallback.")
     lib = ctypes.CDLL(LIB_PATH)
     lib.bm_last_error.restype = ctypes.c_char_p
     lib.bm_last_error.argtypes = []

@@ -1,4 +1,4 @@
-"""Builds libbm_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU)."""
+"""Builds libbm_b200.so in-tree with nvcc for sm_90a (H100) (cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import hashlib
@@ -11,7 +11,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbm_b200.so")
 STAMP = LIB + ".sha256"        # digest of the sources the library was built from (git-ignored, travels with the .so)
 SOURCES = ["bm_api.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-shared", "--expt-relaxed-constexpr"]
 
 

@@ -28,7 +28,7 @@ def _require_cuda_fp32(x: torch.Tensor, who: str) -> None:
     if x.dtype != torch.float32:
         raise TypeError(f"brainmagick_b200.{who} computes in fp32, got {x.dtype}")
     if not x.is_cuda:
-        raise RuntimeError(f"brainmagick_b200.{who} runs on CUDA (sm_100a) only; there is no CPU fallback")
+        raise RuntimeError(f"brainmagick_b200.{who} runs on CUDA (sm_90a) only; there is no CPU fallback")
 
 
 class PositionGetter:

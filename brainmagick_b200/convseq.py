@@ -1,6 +1,6 @@
 """Stand-alone `ConvSequence.forward` (reference: bm/models/common.py:142-151) as ONE autograd function over the same
-CUDA kernels the brain encoder uses (tcgen05 implicit-GEMM convolutions with fused BatchNorm statistics / GLU, tensor-core
-weight gradients, FP32-FMA kernels for shapes outside the tcgen05 tiling) -- the `DeepMel` feature model
+CUDA kernels the brain encoder uses (tensor-core implicit-GEMM convolutions with fused BatchNorm statistics / GLU, tensor-core
+weight gradients, FP32-FMA kernels for shapes outside the tensor-core tiling) -- the `DeepMel` feature model
 (bm/models/features.py:15-35) is exactly this.
 
 x [B, C0, T] (channel-major, like every tensor the reference hands to a model) is transposed once to channels-last, the
@@ -221,7 +221,7 @@ class _ConvSequenceFn(torch.autograd.Function):
 
 def _require_cuda(x: torch.Tensor) -> None:
     if not x.is_cuda:
-        raise RuntimeError("brainmagick_b200.ConvSequence runs on CUDA (sm_100a) only; there is no CPU fallback")
+        raise RuntimeError("brainmagick_b200.ConvSequence runs on CUDA (sm_90a) only; there is no CPU fallback")
 
 
 def conv_sequence(module, x: torch.Tensor) -> torch.Tensor:

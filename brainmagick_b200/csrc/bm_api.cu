@@ -9,7 +9,6 @@
 #include "tc_clip.cuh"
 #include "tc_convp.cuh"
 #include "tc_convh.cuh"
-#include "tc_wgradh.cuh"
 #include "tc_wgradp.cuh"
 #include "tc_gemm_nt.cuh"
 #include "retrieval.cuh"
@@ -649,9 +648,7 @@ extern "C" int bm_clip_loss_bwd(const float* probs, const float* inv_norm, const
     BM_CHECK_ARG(KT < (1ll << 31));
     cudaStream_t st = ST(stream);
     if (tc::gemm_nt_pp_supported(Bn, (int)KT, Bc) && Bn >= 192) {
-        // persistent CTA pairs (csrc/tc_gemm_nt.cuh): dE = G C with G [Bn][Bc], C [Bc][KT].  Its M tile is 256 rows: with
-        // fewer than 192 estimates (cfg3 / cfg5 per-rank batches of 64 / 128) the padding costs more than the single-CTA
-        // kernel below loses (measured 0.47 vs 0.32 ms at 64 x 512, 0.75 vs 0.59 ms at 128 x 1024)
+        // csrc/tc_gemm_nt.cuh: dE = G C with G [Bn][Bc], C [Bc][KT]; smaller batches take the weight-gradient form below
         clip_ce_bwd_kernel<<<ew_grid((long long)Bn * Bc), 256, 0, st>>>(probs, inv_norm, gout, Bn, Bc, target_offset, G, 0);
         BM_CHECK_LAUNCH();
         return tc::launch_gemm_nt_pp(G, cand, dest, Bn, (int)KT, Bc, status, st);
@@ -722,7 +719,7 @@ extern "C" int bm_clip_loss_bwd_cand(const float* probs, const float* scores, co
     BM_CHECK_LAUNCH();
     // dcand[o][k] = sum_b G[b][o] est[b][k]
     if (tc::gemm_nt_pp_supported(Bc, (int)KT, Bn)) {
-        // persistent CTA pairs (csrc/tc_gemm_nt.cuh): A = G^T [Bc][Bn] (rewritten into the same scratch), B = est [Bn][KT]
+        // csrc/tc_gemm_nt.cuh: A = G^T [Bc][Bn] (rewritten into the same scratch), B = est [Bn][KT]
         clip_ce_bwd_kernel<<<ew_grid((long long)Bn * Bc), 256, 0, st>>>(probs, inv_norm, gout, Bn, Bc, target_offset, G, 1);
         BM_CHECK_LAUNCH();
         int rc = tc::launch_gemm_nt_pp(G, est, dcand, Bc, (int)KT, Bn, status, st);
@@ -831,7 +828,7 @@ extern "C" int bm_gather_rows(const float* x, const int* rows, int n_rows, long 
 }
 
 // =================================================================================================
-// tcgen05 (tensor-core) versions of K3/K4
+// tensor-core (wgmma) versions of K3/K4
 // =================================================================================================
 extern "C" int bm_tc_conv_supported(int T, int Cin, int Ntot, int Kw, int glu) {
     return tc::conv_tc_supported(T, Cin, Ntot, Kw, glu) ? 1 : 0;
@@ -851,7 +848,7 @@ extern "C" int bm_tc_conv1d(const float* x, const float* w_hi, const float* w_lo
                             const float* addend, int B, int T, int Cin, int Ntot, int Kw, int dilation, int sign,
                             int glu, int act, int out_tmajor, float* y, float* aux, float* glu_out, double* stats,
                             int* status, bm_stream_t stream) {
-    BM_CHECK_ARG(stats == nullptr);      // only the CTA-pair kernel produces BatchNorm statistics in its epilogue
+    BM_CHECK_ARG(stats == nullptr);      // BatchNorm statistics in the epilogue: bm_tc_conv1d_persistent / bm_tc_conv1d_f16
     BM_CHECK_ARG(x && w_hi && w_lo && B > 0 && T > 0 && dilation >= 1 && (sign == 1 || sign == -1));
     BM_CHECK_ARG(glu ? (glu_out != nullptr) : (y != nullptr));
     BM_CHECK_ARG(B <= 65535);
@@ -860,12 +857,12 @@ extern "C" int bm_tc_conv1d(const float* x, const float* w_hi, const float* w_lo
     tc::ConvTcP p;
     p.B = B; p.T = T; p.Cin = Cin; p.Ntot = Ntot; p.taps = Kw; p.dilation = dilation; p.sign = sign; p.glu = glu;
     p.bias = bias; p.addend = addend; p.y = y; p.glu_out = glu_out; p.err = status;
-    p.act = act; p.out_tmajor = out_tmajor; p.aux = aux; p.bn = 0; p.wsel = nullptr; p.n_wsets = 1;
+    p.act = act; p.out_tmajor = out_tmajor; p.aux = aux; p.wsel = nullptr; p.n_wsets = 1;
     BM_CHECK_ARG(!(glu && (act || out_tmajor || aux)));
     return tc::launch_conv_tc(x, w_hi, w_lo, p, ST(stream));
 }
 
-// per-column sum / sum of squares of a channels-last matrix (BatchNorm batch statistics after the tcgen05 conv)
+// per-column sum / sum of squares of a channels-last matrix (BatchNorm batch statistics after bm_tc_conv1d)
 extern "C" int bm_col_stats(const float* y, long long rows, int C, double* stats, bm_stream_t stream) {
     BM_CHECK_ARG(y && stats && rows > 0 && C > 0);
     cudaStream_t st = ST(stream);
@@ -918,7 +915,7 @@ extern "C" int bm_tc_wgrad(const float* dy, const float* x, int B, int T, int M,
     return tc::launch_wgrad_tc(dy, x, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, status, ST(stream), dbias);
 }
 
-// CTA-pair weight gradient of a k-tap conv (csrc/tc_wgradp.cuh): output rows = (tap, x channel), reduction over the
+// weight gradient of a k-tap conv (csrc/tc_wgradp.cuh): output rows = (tap, x channel), reduction over the
 // flattened rows; no bias gradient (use bm_col_sum on dy where the layer's bias gradient is not exactly zero)
 extern "C" int bm_tc_wgrad_conv_supported(int T, int M, int N, int Kw) {
     return tc::wgradp_supported(T, M, N, Kw) ? 1 : 0;
@@ -933,7 +930,7 @@ extern "C" int bm_tc_wgrad_conv(const float* dy, const float* x, int B, int T, i
     return tc::launch_wgrad_pp(dy, x, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, status, ST(stream));
 }
 
-// the same weight gradient on the F16 pipe (csrc/tc_wgradh.cuh): dy_amax / x_amax = device floats with max |dy|, max |x|
+// the same weight gradient for callers that hold the operands' amax (csrc/tc_wgradp.cuh): dy_amax / x_amax = device floats with max |dy|, max |x|
 // (bm_amax, or the amax_out of the kernels that produced the tensors); same shape gate and workspace as bm_tc_wgrad_conv
 extern "C" int bm_tc_wgrad_conv_f16(const float* dy, const float* dy_amax, const float* x, const float* x_amax, int B, int T,
                                     int M, int N, int Ntrue, int Kw, int dilation, float* workspace, float* dw, int* status,
@@ -970,7 +967,7 @@ extern "C" int bm_gelu_bwd(const float* dq, const float* h, long long n, float* 
 extern "C" int bm_tc_conv1d_persistent_supported(int T, int Cin, int Ntot, int Kw, int glu) {
     return tc::conv_pp_supported(T, Cin, Ntot, Kw, glu) ? 1 : 0;
 }
-// persistent CTA-pair kernel (csrc/tc_convp.cuh): w_raw = the RAW fp32 weights re-laid K-major [Kw][Ntot][Cin]
+// csrc/tc_convp.cuh: w_raw = the RAW fp32 weights re-laid K-major [Kw][Ntot][Cin]
 // (bm_tc_weight_split with f_lo / g_lo = NULL); accumulate=1: y += conv (in place, TMA reduce-add)
 extern "C" int bm_tc_conv1d_persistent(const float* x, const float* w_raw, const float* bias, int accumulate, int B, int T,
                                        int Cin, int Ntot, int Kw, int dilation, int sign, int glu, int act,
@@ -986,7 +983,7 @@ extern "C" int bm_tc_conv1d_persistent(const float* x, const float* w_raw, const
     return tc::launch_conv_pp(a, ST(stream));
 }
 
-// ---- the same conv on the F16 tensor pipe (csrc/tc_convh.cuh): fp32 operands as two fp16 pieces of a power-of-two-scaled
+// ---- the same conv with fp16-piece weights (csrc/tc_convh.cuh): fp32 weights as two fp16 pieces of a power-of-two-scaled
 // tensor.  bm_amax writes the largest magnitude of a tensor into a device float; bm_f16_split prepares the weights
 // (w_raw [Kw][Ntot][Cin] -> fp16 hi / lo copies of w_raw * scale(amax)); the kernel scales x itself.
 extern "C" int bm_amax(const float* x, long long n, float* amax, bm_stream_t stream) {
@@ -1034,7 +1031,7 @@ extern "C" int bm_tc_pointwise_sel(const float* x, const float* w_hi, const floa
     tc::ConvTcP p;
     p.B = B; p.T = T; p.Cin = Cin; p.Ntot = Ntot; p.taps = 1; p.dilation = 1; p.sign = 1; p.glu = 0;
     p.bias = nullptr; p.addend = nullptr; p.y = y; p.glu_out = nullptr; p.err = status;
-    p.act = 0; p.out_tmajor = 0; p.aux = nullptr; p.bn = 0; p.wsel = wsel; p.n_wsets = n_sets;
+    p.act = 0; p.out_tmajor = 0; p.aux = nullptr; p.wsel = wsel; p.n_wsets = n_sets;
     return tc::launch_conv_tc(x, w_hi, w_lo, p, ST(stream));
 }
 

@@ -1,4 +1,4 @@
-// Shared device/host helpers for the brainmagick_b200 kernels (sm_100a only).
+// Shared device/host helpers for the brainmagick_b200 kernels (sm_90a).
 #pragma once
 #include <cuda_runtime.h>
 #include <cstdint>
@@ -9,8 +9,8 @@ namespace bm {
 
 // ---- error plumbing (C-ABI returns an int, message kept for bm_last_error()) -------------------
 extern thread_local char g_last_error[512];
-extern int g_debug_flags;               // bm_set_debug_flags(): experiment switches (bit 0: wgrad keeps X raw as hi)
-extern long long* g_debug_buf;           // bm_set_debug_buffer(): device scratch some kernels fill with cycle counters
+extern int g_debug_flags;               // bm_set_debug_flags(): experiment switches (none defined: every kernel ignores them)
+extern long long* g_debug_buf;           // bm_set_debug_buffer(): device scratch for cycle counters (no kernel records any)
 extern unsigned long long g_launches;   // kernels launched by this library since load (bm_launch_count())
 inline int set_error(int code, const char* fmt, const char* a = "", const char* b = "") {
     snprintf(g_last_error, sizeof(g_last_error), fmt, a, b);

@@ -1,6 +1,6 @@
-// Generic FP32-FMA tiled GEMM for sm_100a: the workhorse for every *small* contraction of the hot path
-// (spatial attention, sensor chain, per-subject layers, parameter gradients) and the parity-grade fallback
-// body for the big ones while their tcgen05 versions are brought up.
+// Generic FP32-FMA tiled GEMM: the workhorse for every *small* contraction of the hot path (spatial attention, sensor
+// chain, per-subject layers, parameter gradients) and for the shapes outside the tensor-core shape gates (the small unit-test
+// models).
 //
 //   D[g][m][n] (+)= epi( sum_{z in seg(g)} sum_{tap} sum_{k in krange} A(z, m + a_shift_m[tap], k) * B(bz(z), tap, n, k + b_shift_k[tap]) )
 //

@@ -1,310 +1,56 @@
-// K6: ClipLoss.get_scores (bm/losses.py:91-94) as ONE split-K tensor-core GEMM on CTA pairs, with the candidate norms
-// computed on the way, followed by ONE finalize kernel (split reduction + 1/norm scale + row softmax / cross-entropy +
-// batch mean, bm/losses.py:97-114).
+// K6: ClipLoss.get_scores (bm/losses.py:91-94) as ONE split-K tensor-core GEMM (3xTF32 wgmma engine of tc_common.cuh)
+// followed by ONE finalize kernel (split reduction + 1/norm scale + row softmax / cross-entropy + batch mean,
+// bm/losses.py:97-114).
 //
 //     S[b][o] = sum_k E[b][k] C[o][k]          E = estimates [Bn][K], C = candidates [Bc][K], K = F*T (368 640)
 //
-// Why a kernel of its own (round 1 ran this on the conv kernel with 37-74 K slices): the tensor core's fp32 accumulator
-// TRUNCATES.  One accumulator that chains ~3 700 tcgen05.mma additions of same-signed products (a self dot product, or any
-// well-trained estimate/candidate pair) comes out 1.1e-4 low -- measured: 2.9e-8 relative per addition.  Here a chain is
-// at most CL_CHAIN chunks (128 K-steps, 384 additions; the expected truncation gain is compensated, tc_common.cuh, which
-// leaves <= 5e-6); four "drain" warps add each finished chain into an fp32 running sum (round-to-nearest, kept in tensor
-// memory as well) -- a ~3 % pause of the MMA stream per chain.  (A first version alternated two chain accumulators and left
-// only two tensor-memory slots for the A operand: the converter <-> MMA hand-shake latency was then exposed on every chunk
-// and the MMA thread waited 31 % of the time; four slots and two alternating converter warp sets hide it.)
-//
-//   cluster = 2 CTAs = 256 candidate rows (M side, through TMEM) x NT (64 or 128) estimate rows (N side, smem)
-//   per K chunk of 32, per CTA:  candidates 128 x 32 (16 KB) by TMA -> 4 converter warps: tf32 hi/lo -> TMEM, and the
-//                                row's sum of squares (the 1/||c|| of losses.py:91) for free;
-//                                estimates NT/2 x 32 raw (the tensor core's own truncation is the `hi`), 2 warps write
-//                                lo = x - trunc(x) beside it
-//   leader CTA, one thread:      12 x tcgen05.mma.cta_group::2.kind::tf32 (M = 256, N = NT, K = 8; 3xTF32)
-//   outputs: partial scores [ks][Bn][Bc] (transposed store is the coalesced one: lane = candidate) and [ks][Bc] fp64
-//   partial sums of squares; `clip_finalize_kernel` reduces both in a fixed order (deterministic).
+// K is long: a self dot product chained through the tensor core's truncating accumulator would come out ~1e-4 low; the
+// engine adds every 32-wide K block into a round-to-nearest fp32 sum instead.  The candidate norms (the 1/||c|| of
+// losses.py:91) come from a fp64 row sum of squares beside the GEMM.
+//   grid: 128-estimate x 128-candidate tiles x K slices; outputs: partial scores [ks][Bn][Bc] and [ks][Bc] fp64 partial sums
+//   of squares (slice 0 holds the full sums); `clip_finalize_kernel` reduces both in a fixed order (deterministic).
 #pragma once
-#include "tc_pair.cuh"
+#include "tc_common.cuh"
+#include "elementwise.cuh"
 
 namespace bm {
 namespace tc {
 
-constexpr int CL_BM = 128, CL_BK = 32, CL_STAGES = 6, CL_TSLOTS = 4, CL_THREADS = 512;
-constexpr int CL_CHAIN = 32;                                      // chunks per accumulation chain
-constexpr int CL_PF_CHUNKS = 8;                                   // K chunks covered by one L2 prefetch box (256 floats = 1 KB per row)
-constexpr int CL_A_BYTES = CL_BM * CL_BK * 4;                     // 16 KB
-constexpr int CL_BH_BYTES = 64 * CL_BK * 4;                       // 8 KB: NT/2 <= 64 estimate rows
-constexpr int CL_STAGE_BYTES = CL_A_BYTES + 2 * CL_BH_BYTES;      // 32 KB
-constexpr int CL_SMEM_BYTES = CL_STAGES * CL_STAGE_BYTES + 1024;
-constexpr int CL_PART_COLS = 128;                                 // TMEM: chain accumulator | running sum | A slots 0..3 (six smem stages)
-constexpr int CL_RUN_COL = CL_PART_COLS;
-constexpr int CL_A_COL = 2 * CL_PART_COLS, CL_A_COLS = 2 * CL_BK;
+constexpr int CL_BK = HG_BK;
 
-struct ClipP {
-    int Bn, Bc;               // estimates, candidates
-    int nt;                   // estimate rows per tile: 64 or 128
-    int mtiles, ntiles, ks;   // 256-candidate tiles, NT-estimate tiles, K slices
-    int chunks, per_split;    // K chunks of 32 in total / per slice
-    float* P;                 // [ks][Bn][Bc]
-    double* ssp;              // [ks][Bc] or null
-    int* err;
-    long long* dbg;           // debug only (bm_set_debug_buffer): per CTA 8 cycle counters
+struct ClipOp {
+    static constexpr bool A_KCONTIG = true, B_KCONTIG = true;
+    const float* E; const float* C;
+    int Bn, Bc, chunks, per_split;
+    long long KT;
+    float* P;                   // [ks][Bn][Bc]
+    struct Cta { int m0, n0, c0, c1; };
+    __device__ Cta cta() const {
+        Cta c;
+        c.n0 = blockIdx.x * HG_BN;
+        c.m0 = blockIdx.y * HG_BM;
+        c.c0 = blockIdx.z * per_split;
+        c.c1 = min(chunks, c.c0 + per_split);
+        return c;
+    }
+    __device__ int kblocks(const Cta& c) const { return max(0, c.c1 - c.c0); }
+    __device__ float4 a4(const Cta& c, int kb, int r, int q) const {
+        const int m = c.m0 + r;
+        const long long k = (long long)(c.c0 + kb) * HG_BK + 4 * q;
+        if (m >= Bn || k >= KT) return make_float4(0.f, 0.f, 0.f, 0.f);
+        return __ldg(reinterpret_cast<const float4*>(E + m * KT + k));
+    }
+    __device__ float4 b4(const Cta& c, int kb, int r, int q) const {
+        const int n = c.n0 + r;
+        const long long k = (long long)(c.c0 + kb) * HG_BK + 4 * q;
+        if (n >= Bc || k >= KT) return make_float4(0.f, 0.f, 0.f, 0.f);
+        return __ldg(reinterpret_cast<const float4*>(C + n * KT + k));
+    }
+    __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+        HgStore s{P + (long long)blockIdx.z * Bn * Bc, Bc, Bn, Bc};
+        s.store(acc, c.m0 + m0, c.n0);
+    }
 };
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(CL_THREADS, 1)
-clip_scores_kernel(const __grid_constant__ CUtensorMap tmC, const __grid_constant__ CUtensorMap tmE,
-                   const __grid_constant__ CUtensorMap tmCp, const __grid_constant__ CUtensorMap tmEp, const ClipP p) {
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[CL_STAGES], conv_bar[CL_STAGES], empty_bar[CL_STAGES];
-    __shared__ __align__(8) uint64_t part_full, part_empty;
-    __shared__ double ssq_sh[CL_BM];
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ int prior_error;
-
-    if (threadIdx.x == 0) prior_error = p.err ? *reinterpret_cast<volatile int*>(p.err) : 0;
-    __syncthreads();
-    const bool skip = prior_error != 0;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
-
-    // pair -> (K slice, candidate tile, estimate tile); the estimate tiles of one (slice, candidate tile) are neighbours,
-    // so the candidate stream they share is an L2 hit for all but the first
-    int pair = blockIdx.x >> 1;
-    const int n_tile = pair % p.ntiles; pair /= p.ntiles;
-    const int m_tile = pair % p.mtiles;
-    const int ksl = pair / p.mtiles;
-    const int it_begin = ksl * p.per_split;
-    const int total = skip ? 0 : max(0, min(p.chunks, it_begin + p.per_split) - it_begin);
-    const int nchains = (total + CL_CHAIN - 1) / CL_CHAIN;
-    const int nt = p.nt, nq = nt / 2;
-    const int m0 = m_tile * 2 * CL_BM + (int)rank * CL_BM;        // first candidate row of this CTA
-    const int n0 = n_tile * nt;                                   // first estimate row of the tile
-    const uint32_t bh_bytes = (uint32_t)(nq * CL_BK * 4);
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < CL_STAGES; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&conv_bar[s], 2 * (4 + 2));                 // one elected lane per converter warp of both CTAs (LEADER's copy)
-            mbar_init(&empty_bar[s], 1);
-        }
-        mbar_init(&part_full, 1);
-        mbar_init(&part_empty, 2 * 4);                            // one elected lane per drain warp of both CTAs
-        fence_barrier_init();
-    }
-    if (warp == 1) tmem_alloc_2sm<512>(&tmem_base_smem);
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_smem;
-
-    if (warp == 0) {
-        // ------------------------------------------------ TMA producer ------------------------------------------------
-        if (lane == 0) {
-            prefetch_tmap(&tmC);
-            prefetch_tmap(&tmE);
-            prefetch_tmap(&tmCp);
-            prefetch_tmap(&tmEp);
-            // The operand rows are F*T*4 = 1.4 MB apart, and a K chunk takes only 128 bytes of each: fetched on demand, every
-            // row piece is its own DRAM page activation (measured: the converters waited for the TMA 68 % of the time at
-            // 2.3 TB/s).  So the rows are pulled into L2 one kilobyte at a time, eight chunks ahead, by wide L2-prefetch boxes
-            // (cp.async.bulk.prefetch.tensor); the narrow 128-byte-swizzled loads below then hit L2.
-            auto l2_prefetch = [&](int group) {
-                const int k0 = (it_begin + group * CL_PF_CHUNKS) * CL_BK;
-                if (group * CL_PF_CHUNKS < total) {
-                    tma_prefetch_2d(&tmCp, k0, m0);
-                    tma_prefetch_2d(&tmEp, k0, n0 + (int)rank * nq);
-                }
-            };
-            l2_prefetch(0);
-            l2_prefetch(1);
-            for (int it = 0; it < total; ++it) {
-                const int s = it % CL_STAGES;
-                const uint32_t ph = (it / CL_STAGES) & 1;
-                if (it % CL_PF_CHUNKS == 0) l2_prefetch(it / CL_PF_CHUNKS + 2);
-                if (!mbar_wait(&empty_bar[s], ph ^ 1, p.err, 61)) break;
-                const int k0 = (it_begin + it) * CL_BK;
-                uint8_t* st = smem + s * CL_STAGE_BYTES;
-                mbar_expect_tx(&full_bar[s], CL_A_BYTES + bh_bytes);
-                tma_load_2d(st, &tmC, &full_bar[s], k0, m0);
-                tma_load_2d(st + CL_A_BYTES, &tmE, &full_bar[s], k0, n0 + (int)rank * nq);
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------ MMA issuer (leader): the whole warp walks the loop, one elected
-        // lane issues (see elect_one) ------------------------------------------------------------------------------------
-        if (leader) {
-            const uint32_t idesc = umma_idesc_tf32(2 * CL_BM, nt);
-            bool ok = true;
-            long long t_conv = 0, t_drain = 0, t_begin = clock64();
-            for (int it = 0; it < total && ok; ++it) {
-                const int s = it % CL_STAGES;
-                const uint32_t ph = (it / CL_STAGES) & 1;
-                const int c = it / CL_CHAIN;
-                const bool first = (it - c * CL_CHAIN) == 0;
-                long long c0 = clock64();
-                if (first && c >= 1) {                            // the drain of the previous chain has read the accumulator
-                    ok = mbar_wait(&part_empty, (uint32_t)(c - 1) & 1, p.err, 62);
-                    t_drain += clock64() - c0;
-                    c0 = clock64();
-                }
-                ok = ok && mbar_wait(&conv_bar[s], ph, p.err, 63);
-                ok = __all_sync(0xffffffffu, ok);
-                t_conv += clock64() - c0;
-                if (!ok) break;
-                tc_fence_after();
-                if (elect_one()) {
-                    const uint32_t b_hi = smem_base + s * CL_STAGE_BYTES + CL_A_BYTES, b_lo = b_hi + CL_BH_BYTES;
-                    const uint32_t a_hi = tmem + CL_A_COL + (it % CL_TSLOTS) * CL_A_COLS, a_lo = a_hi + CL_BK;
-                    const uint64_t dbh0 = umma_desc_k_sw128(b_hi), dbl0 = umma_desc_k_sw128(b_lo);
-#pragma unroll
-                    for (int kk = 0; kk < CL_BK / 8; ++kk) {
-                        const uint64_t dbh = dbh0 + (uint64_t)(kk * 2), dbl = dbl0 + (uint64_t)(kk * 2);   // +32 bytes >> 4
-                        umma_tf32_ts_2sm(tmem, a_lo + kk * 8, dbh, idesc, (first && kk == 0) ? 0u : 1u);
-                        umma_tf32_ts_2sm(tmem, a_hi + kk * 8, dbl, idesc, 1);
-                        umma_tf32_ts_2sm(tmem, a_hi + kk * 8, dbh, idesc, 1);
-                    }
-                    umma_commit_2sm(&empty_bar[s]);
-                    if (it + 1 == total || (it + 1) % CL_CHAIN == 0) umma_commit_2sm(&part_full);
-                }
-                __syncwarp();
-            }
-            if (p.dbg && lane == 0) {
-                p.dbg[blockIdx.x * 8 + 0] = t_conv; p.dbg[blockIdx.x * 8 + 1] = clock64() - t_begin; p.dbg[blockIdx.x * 8 + 6] = t_drain;
-            }
-        }
-    } else if (warp < 4) {
-        // ------------------------------------------------ estimate tile: lo = x - trunc_tf32(x) -----------------------
-        const int ct = (warp - 2) * 32 + lane;                    // 0..63
-        const int nvec = (int)(bh_bytes / 16);
-        bool ok = true;
-        for (int it = 0; it < total && ok; ++it) {
-            const int s = it % CL_STAGES;
-            const uint32_t ph = (it / CL_STAGES) & 1;
-            ok = mbar_wait(&full_bar[s], ph, p.err, 64);
-            const float4* bh = reinterpret_cast<const float4*>(smem + s * CL_STAGE_BYTES + CL_A_BYTES);
-            float4* bl = reinterpret_cast<float4*>(smem + s * CL_STAGE_BYTES + CL_A_BYTES + CL_BH_BYTES);
-#pragma unroll 4
-            for (int idx = ct; idx < nvec; idx += 64) {
-                const float4 v = bh[idx];
-                float4 l;
-                l.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-                l.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-                l.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-                l.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-                bl[idx] = l;
-            }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&conv_bar[s]), 0));
-        }
-    } else if (warp < 12) {
-        // ------------------------------------------------ candidate rows -> TMEM (hi | lo), sum of squares -------------
-        // two sets of four warps take alternate chunks (a set's ~780 cycles per chunk would otherwise equal the MMA time)
-        const int set = (warp - 4) >> 2;
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16);
-        double ssq = 0.0;
-        bool ok = true;
-        long long t_full = 0, t_slot = 0, t_work = 0;
-        for (int it = set; it < total && ok; it += 2) {
-            const int s = it % CL_STAGES;
-            const uint32_t ph = (it / CL_STAGES) & 1;
-            const long long c0 = clock64();
-            ok = mbar_wait(&full_bar[s], ph, p.err, 65);
-            const long long c1 = clock64();
-            t_full += c1 - c0;
-            const uint8_t* arow = smem + s * CL_STAGE_BYTES + row * 128;
-            float hi[CL_BK], lo[CL_BK];
-            float sq = 0.f;
-#pragma unroll
-            for (int c = 0; c < 8; ++c) {
-                const float4 v = *reinterpret_cast<const float4*>(arow + ((c ^ (row & 7)) << 4));
-                tf32_split(v.x, hi[4 * c + 0], lo[4 * c + 0]); tf32_split(v.y, hi[4 * c + 1], lo[4 * c + 1]);
-                tf32_split(v.z, hi[4 * c + 2], lo[4 * c + 2]); tf32_split(v.w, hi[4 * c + 3], lo[4 * c + 3]);
-                sq = fmaf(v.x, v.x, sq); sq = fmaf(v.y, v.y, sq); sq = fmaf(v.z, v.z, sq); sq = fmaf(v.w, v.w, sq);
-            }
-            ssq += (double)sq;
-            const long long c2 = clock64();
-            if (it >= CL_TSLOTS) {            // tensor-memory slot it % 4 is free once the MMAs of chunk it-4 have completed
-                const int i4 = it - CL_TSLOTS;
-                ok = ok && mbar_wait(&empty_bar[i4 % CL_STAGES], (uint32_t)(i4 / CL_STAGES) & 1, p.err, 66);
-            }
-            tc_fence_after();
-            const long long c3 = clock64();
-            t_slot += c3 - c2;
-            tmem_st32(tq + CL_A_COL + (it % CL_TSLOTS) * CL_A_COLS, hi);
-            tmem_st32(tq + CL_A_COL + (it % CL_TSLOTS) * CL_A_COLS + CL_BK, lo);
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&conv_bar[s]), 0));
-            t_work += (c2 - c1) + (clock64() - c3);
-        }
-        if (p.dbg && warp == 4 && lane == 0) {
-            p.dbg[blockIdx.x * 8 + 2] = t_full; p.dbg[blockIdx.x * 8 + 3] = t_slot; p.dbg[blockIdx.x * 8 + 4] = t_work;
-        }
-        // the two sets each hold half of the row's sum of squares: set 1 hands its half over through shared memory
-        if (set == 1) ssq_sh[row] = ssq;
-        asm volatile("bar.sync 1, 256;" ::: "memory");           // the eight converter warps
-        const int o = m0 + row;
-        if (set == 0 && p.ssp && n_tile == 0 && o < p.Bc) p.ssp[(long long)ksl * p.Bc + o] = ssq + ssq_sh[row];
-    } else {
-        // ------------------------------------------------ drain: running += finished chain (fp32, RN); final store -----
-        const int q = warp & 3;
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16);
-        const int o = m0 + q * 32 + lane;                         // candidate (column of the score matrix)
-        float* dst = p.P + ((long long)ksl * p.Bn + n0) * p.Bc + o;
-        if (nchains == 0) {
-            if (o < p.Bc)
-                for (int j = 0; j < nt; ++j)
-                    if (n0 + j < p.Bn) dst[(long long)j * p.Bc] = 0.f;
-        }
-        bool ok = true;
-        for (int c = 0; c < nchains && ok; ++c) {
-            ok = mbar_wait(&part_full, (uint32_t)c & 1, p.err, 67);
-            tc_fence_after();
-            const bool last = c + 1 == nchains;
-            const float comp = acc_trunc_comp(min(CL_CHAIN, total - c * CL_CHAIN) * (CL_BK / 8) * 3);
-#pragma unroll 1
-            for (int j = 0; j < nt / 32; ++j) {
-                float a[32];
-                tmem_ld32(tq + j * 32, a);
-#pragma unroll
-                for (int i = 0; i < 32; ++i) a[i] *= comp;
-                if (c > 0) {
-                    float r[32];
-                    tmem_ld32(tq + CL_RUN_COL + j * 32, r);
-#pragma unroll
-                    for (int i = 0; i < 32; ++i) a[i] += r[i];
-                }
-                if (!last) {
-                    tmem_st32(tq + CL_RUN_COL + j * 32, a);
-                } else if (o < p.Bc) {
-#pragma unroll
-                    for (int i = 0; i < 32; ++i)
-                        if (n0 + j * 32 + i < p.Bn) dst[(long long)(j * 32 + i) * p.Bc] = a[i];
-                }
-            }
-            if (!last) {
-                tmem_st_wait();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&part_empty), 0));
-            }
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_2sm<512>(tmem);
-    }
-}
 
 // ---- finalize: fixed-order reduction of the K slices, 1/norm, scores, optional softmax / cross-entropy / batch mean ----
 // one block per estimate row b.  `counter` (zeroed by the launcher) elects the last block, which averages row_loss in a
@@ -389,19 +135,16 @@ __global__ void clip_finalize_kernel(const float* __restrict__ P, const double* 
 }
 
 // ---- geometry / workspace -------------------------------------------------------------------------------------------
-struct ClipGeom { int nt, mtiles, ntiles, ks, chunks, per_split; };
+struct ClipGeom { int ks, chunks, per_split; };
 
 inline bool clip_tc_supported(int Bn, int Bc, long long KT) {
     return Bn > 0 && Bc > 0 && KT >= CL_BK && KT % 4 == 0 && KT < (1ll << 31);
 }
 inline ClipGeom clip_geometry(int Bn, int Bc, long long KT) {
     ClipGeom g;
-    g.nt = Bn <= 64 ? 64 : 128;
-    g.mtiles = (Bc + 2 * CL_BM - 1) / (2 * CL_BM);
-    g.ntiles = (Bn + g.nt - 1) / g.nt;
     g.chunks = (int)((KT + CL_BK - 1) / CL_BK);
-    const int tiles = g.mtiles * g.ntiles, pairs = num_sms() / 2;
-    int ks = pairs / tiles;                                       // one wave of CTA pairs
+    const int tiles = ((Bc + HG_BN - 1) / HG_BN) * ((Bn + HG_BM - 1) / HG_BM);
+    int ks = num_sms() / tiles;                                   // one wave of 128 x 128 tiles
     if (ks < 1) ks = 1;
     if (ks > g.chunks) ks = g.chunks;
     g.per_split = (g.chunks + ks - 1) / ks;
@@ -420,52 +163,33 @@ inline long long clip_ws_floats(int Bn, int Bc, long long KT) {
 inline int launch_clip_scores(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
                               int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss,
                               float* loss, float* ws, int* err, cudaStream_t st) {
+    (void)err;
     const ClipGeom g = clip_geometry(Bn, Bc, KT);
-    CUtensorMap tmC, tmE;
-    {
-        uint64_t dims[2] = {(uint64_t)KT, (uint64_t)Bc};
-        uint64_t str[1] = {(uint64_t)KT * 4};
-        uint32_t box[2] = {CL_BK, CL_BM};
-        if (!make_tmap_f32(&tmC, cand, 2, dims, str, box)) return set_error(4, "%s: cuTensorMapEncodeTiled(C) failed%s", __func__);
-    }
-    {
-        uint64_t dims[2] = {(uint64_t)KT, (uint64_t)Bn};
-        uint64_t str[1] = {(uint64_t)KT * 4};
-        uint32_t box[2] = {CL_BK, (uint32_t)(g.nt / 2)};
-        if (!make_tmap_f32(&tmE, est, 2, dims, str, box)) return set_error(4, "%s: cuTensorMapEncodeTiled(E) failed%s", __func__);
-    }
-    CUtensorMap tmCp, tmEp;                                       // the same tensors with 1 KB-wide boxes, for the L2 prefetches
-    {
-        uint64_t dims[2] = {(uint64_t)KT, (uint64_t)Bc};
-        uint64_t str[1] = {(uint64_t)KT * 4};
-        uint32_t box[2] = {CL_PF_CHUNKS * CL_BK, CL_BM};
-        uint64_t dimse[2] = {(uint64_t)KT, (uint64_t)Bn};
-        uint32_t boxe[2] = {CL_PF_CHUNKS * CL_BK, (uint32_t)(g.nt / 2)};
-        if (!make_tmap_f32(&tmCp, cand, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE) ||
-            !make_tmap_f32(&tmEp, est, 2, dimse, str, boxe, CU_TENSOR_MAP_SWIZZLE_NONE))
-            return set_error(4, "%s: cuTensorMapEncodeTiled(prefetch) failed%s", __func__);
-    }
-    int rc = ensure_dyn_smem(reinterpret_cast<const void*>(clip_scores_kernel), CL_SMEM_BYTES);
-    if (rc) return rc;
     long long nP = (long long)g.ks * Bn * Bc;
     nP += nP & 1;
-    ClipP p;
-    p.Bn = Bn; p.Bc = Bc; p.nt = g.nt; p.mtiles = g.mtiles; p.ntiles = g.ntiles; p.ks = g.ks; p.chunks = g.chunks;
-    p.per_split = g.per_split; p.P = ws; p.ssp = norms_given ? nullptr : reinterpret_cast<double*>(ws + nP); p.err = err;
-    p.dbg = g_debug_buf;
+    double* ssp = norms_given ? nullptr : reinterpret_cast<double*>(ws + nP);
     unsigned int* counter = reinterpret_cast<unsigned int*>(ws + nP + 2ll * g.ks * Bc);
     if (loss) {
         cudaError_t em = cudaMemsetAsync(counter, 0, sizeof(unsigned int), st);
         if (em != cudaSuccess) return set_error(3, "%s: memset: %s", __func__, cudaGetErrorString(em));
     }
-    clip_scores_kernel<<<2 * g.mtiles * g.ntiles * g.ks, CL_THREADS, CL_SMEM_BYTES, st>>>(tmC, tmE, tmCp, tmEp, p);
-    ++g_launches;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", __func__, cudaGetErrorString(e));
-    clip_finalize_kernel<<<Bn, 256, 0, st>>>(ws, p.ssp, g.ks, Bn, Bc, target_offset, inv_norm, scores, probs, row_loss,
+    if (ssp) {
+        cudaError_t em = cudaMemsetAsync(ssp, 0, sizeof(double) * g.ks * Bc, st);
+        if (em != cudaSuccess) return set_error(3, "%s: memset: %s", __func__, cudaGetErrorString(em));
+        int splits = (int)((KT + 65535) / 65536);
+        if (splits > 32) splits = 32;
+        row_sumsq_kernel<<<dim3(Bc, splits), 256, 0, st>>>(cand, ssp, KT);
+        ++g_launches;
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return set_error(3, "%s: norm launch failed: %s", __func__, cudaGetErrorString(e));
+    }
+    ClipOp o;
+    o.E = est; o.C = cand; o.Bn = Bn; o.Bc = Bc; o.chunks = g.chunks; o.per_split = g.per_split; o.KT = KT; o.P = ws;
+    if (int rc = hg_launch(o, dim3((Bc + HG_BN - 1) / HG_BN, (Bn + HG_BM - 1) / HG_BM, g.ks), st, __func__)) return rc;
+    clip_finalize_kernel<<<Bn, 256, 0, st>>>(ws, ssp, g.ks, Bn, Bc, target_offset, inv_norm, scores, probs, row_loss,
                                              loss, counter);
     ++g_launches;
-    e = cudaGetLastError();
+    cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(3, "%s: finalize launch failed: %s", __func__, cudaGetErrorString(e));
     return 0;
 }

@@ -1,238 +1,25 @@
-// Blackwell (sm_100a) primitives used by the tensor-core kernels: mbarrier, TMA (cp.async.bulk.tensor),
-// tcgen05 (alloc / mma / commit / ld / st / fences) as inline PTX, UMMA descriptors, and host-side tensor-map
-// creation through the runtime's driver entry point (no link-time dependency on libcuda).
+// Hopper (sm_90a) tensor-core engine shared by the conv / weight-gradient / CLIP kernels: one 3xTF32 wgmma GEMM
+//
+//     D[m][n] = sum_k A[m][k] * B[n][k]        (fp32 operands, fp32-faithful result)
+//
+// whose operands and epilogue are supplied by an "op" (see the tc_*.cuh launchers), so that every contraction keeps its own
+// addressing (tap shifts with per-sample zero padding, position-major weight-gradient operands, K slices) and its own fused
+// epilogue without a copy of the pipeline.
+//
+// One CTA = two warpgroups = one 128 x 128 output tile (warpgroup g owns rows [64 g, 64 g + 64)).  Per K block of 32:
+//   * every thread loads its share of the A and B tiles from global memory into registers one block AHEAD (the loads of
+//     block kb+1 are in flight while the tensor cores work on block kb), splits each fp32 value x into tf32 pieces
+//     hi = rna_tf32(x), lo = x - hi, and writes hi and lo into the 128-byte-swizzled K-major layout wgmma reads;
+//     operands whose contiguous dimension is M/N (the position-major weight gradients) are transposed on that store;
+//   * 4 x 3 wgmma.m64n128k8.f32.tf32 per warpgroup: lo*hi + hi*lo + hi*hi (the lo*lo term is below fp32 resolution);
+//   * the block's products are accumulated in a fresh register tile and then added into the running fp32 sum with
+//     ordinary round-to-nearest FADDs.  The tensor core's internal accumulation truncates; chaining at most 12 MMAs per
+//     block keeps that bias below 1e-7 relative however long K is, with no correction factor to calibrate per GPU.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
 
 namespace bm {
-namespace tc {
-
-// ---------------------------------------------------------------------------------------------------
-// device: shared-memory addresses, mbarrier
-// ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-}
-__device__ __forceinline__ void fence_barrier_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
-    uint32_t ok;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(ok)
-        : "r"(smem_u32(bar)), "r"(parity)
-        : "memory");
-    return ok != 0;
-}
-// Bounded wait: a mis-programmed pipeline must never hang the GPU.  On timeout the error word is set and the
-// caller carries on (results are garbage, the host reports the failure).
-__device__ __forceinline__ bool mbar_wait(uint64_t* bar, uint32_t parity, int* err, int code) {
-    for (uint32_t i = 0; i < (1u << 24); ++i) {
-        if (mbar_try_wait(bar, parity)) return true;
-        if (i > 64) __nanosleep(32);
-    }
-    if (err) atomicExch(err, code);
-    return false;
-}
-
-// ---------------------------------------------------------------------------------------------------
-// device: TMA
-// ---------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void prefetch_tmap(const CUtensorMap* m) {
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(m)) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1)
-        : "memory");
-}
-// pulls a box into L2 only (no shared-memory destination, no completion to wait for)
-__device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* m, int c0, int c1) {
-    asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_load_3d(void* dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
-    asm volatile(
-        "cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
-        ::"r"(smem_u32(dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2)
-        : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------------
-// device: tcgen05
-// ---------------------------------------------------------------------------------------------------
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* dst_smem) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(NCOLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-
-// One lane of a CONVERGED warp (elect.sync).  Issuing tcgen05.mma from `if (lane == 0)` code makes ptxas wrap every MMA in
-// an ELECT / BRA.U.ANY loop over the active lanes (~45 cycles per instruction: the 12 MMAs of a 768-cycle K chunk of the
-// CLIP kernel then cost 1 000 cycles to issue); with the whole warp in the loop and only the issue under this predicate the
-// MMAs are plainly predicated instructions.
-__device__ __forceinline__ bool elect_one() {
-    uint32_t pred = 0;
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "elect.sync _|p, 0xFFFFFFFF;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(pred)::"memory");
-    return pred != 0;
-}
-
-// D[tmem] (+)= A[smem] * B[smem]^T, tf32 inputs, fp32 accumulate; issued by ONE thread.
-__device__ __forceinline__ void umma_tf32_ss(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// A operand from tensor memory (lane = row, 32-bit column = k)
-__device__ __forceinline__ void umma_tf32_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                             uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrives on the mbarrier once every previously issued tcgen05.mma of this thread has completed
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-                 : "memory");
-}
-
-// 32 lanes x 32 consecutive 32-bit columns: thread i of the warp receives columns [c, c+32) of TMEM lane base+i
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, float* v) {
-    uint32_t r[32];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-          "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-          "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 32; ++i) v[i] = __uint_as_float(r[i]);
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float* v) {
-    uint32_t r[16];
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-          "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr)
-        : "memory");
-    asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-    for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
-}
-
-// ---------------------------------------------------------------------------------------------------
-// UMMA descriptors (bit layouts as in cute/arch/mma_sm100_desc.hpp)
-// ---------------------------------------------------------------------------------------------------
-// K-major operand tile, rows of exactly 128 bytes (32 fp32), SWIZZLE_128B, 8-row atoms 1024 B apart.
-__device__ __forceinline__ uint64_t umma_desc_k_sw128(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);        // start address  [0,14)
-    d |= (uint64_t)1 << 16;                              // leading byte offset (unused for swizzled K-major)
-    d |= (uint64_t)(1024 >> 4) << 32;                    // stride byte offset: next 8-row group
-    d |= (uint64_t)1 << 46;                              // descriptor version 1 (sm_100)
-    d |= (uint64_t)2 << 61;                              // SWIZZLE_128B
-    return d;
-}
-// instruction descriptor: tf32 x tf32 -> f32, both operands K-major
-__host__ __device__ constexpr uint32_t umma_idesc_tf32(int M, int N) {
-    return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// The tensor core's fp32 accumulator TRUNCATES toward zero on every tcgen05.mma addition.  Measured on B200
-// (profiles/accumulator_gain_probe.py, kind::tf32, 3xTF32 chains of 120 ... 720 additions, random-sign and all-positive
-// data alike): the result is the true sum times (1 - 1.66e-8 * n_additions) plus a residual half that size -- a systematic
-// GAIN, which compounds through the ~25 chained contractions of a backward pass (8.7e-5 on the deepest gradients).  Every
-// epilogue multiplies the accumulator it drains by acc_trunc_comp(n_additions), the inverse of that expected gain.
-constexpr float TC_ACC_TRUNC_PER_ADD = 1.66e-8f;
-__host__ __device__ __forceinline__ float acc_trunc_comp(int n_additions) { return 1.0f + TC_ACC_TRUNC_PER_ADD * (float)n_additions; }
-
-// fp32 -> (hi, lo) with hi = rna_tf32(x) and lo = rna_tf32(x - hi): x*y ~= hi*hi' + lo*hi' + hi*lo' to ~2^-21
-__device__ __forceinline__ float tf32_rna(float x) {
-    uint32_t r;
-    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
-    return __uint_as_float(r);
-}
-
-// The same split with full-rate integer/FP32 instructions (cvt.rna.tf32 issues at a fraction of the FMA rate and made
-// the converter warps the bottleneck): hi = round-to-nearest(ties away) of x to 10 mantissa bits = (bits + 0x1000) &
-// ~0x1FFF, lo = x - hi exactly (the tensor core ignores lo's 13 low mantissa bits: error <= 2^-21 |x|).
-__device__ __forceinline__ void tf32_split(float x, float& hi, float& lo) {
-    hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
-    lo = x - hi;
-}
-
-}  // namespace tc
-
-// ---------------------------------------------------------------------------------------------------
-// host: tensor maps
-// ---------------------------------------------------------------------------------------------------
-typedef CUresult (*PFN_bm_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                       const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                       CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-inline PFN_bm_encodeTiled get_encode_tiled() {
-    static PFN_bm_encodeTiled fn = nullptr;
-    if (!fn) {
-        void* p = nullptr;
-        cudaDriverEntryPointQueryResult q;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
-            q == cudaDriverEntryPointSuccess)
-            fn = reinterpret_cast<PFN_bm_encodeTiled>(p);
-    }
-    return fn;
-}
-
-// fp32 tensor, innermost dimension first; strides in BYTES for dims 1..rank-1; SWIZZLE_128B; OOB reads give 0.
-inline bool make_tmap_f32(CUtensorMap* m, const void* base, int rank, const uint64_t* dims, const uint64_t* strides_b,
-                          const uint32_t* box, CUtensorMapSwizzle swizzle = CU_TENSOR_MAP_SWIZZLE_128B) {
-    PFN_bm_encodeTiled enc = get_encode_tiled();
-    if (!enc) return false;
-    cuuint64_t gd[5], gs[5];
-    cuuint32_t bx[5], es[5];
-    for (int i = 0; i < rank; ++i) { gd[i] = dims[i]; bx[i] = box[i]; es[i] = 1; }
-    for (int i = 0; i + 1 < rank; ++i) gs[i] = strides_b[i];
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, (cuuint32_t)rank, const_cast<void*>(base), gd, gs, bx, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
-}
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device): the attribute is per device, so a
 // process-wide flag would leave a second device of the same process without it.
@@ -255,5 +42,222 @@ inline int ensure_dyn_smem(const void* func, int bytes) {
     if (dev >= 0 && dev < kMaxDev) done[f][dev] = true;
     return 0;
 }
+
+
+namespace tc {
+
+__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+
+// fp32 -> (hi, lo) with hi = rna_tf32(x) and lo = rna_tf32(x - hi): x*y ~= hi*hi' + lo*hi' + hi*lo' to ~2^-21
+__device__ __forceinline__ float tf32_rna(float x) {
+    uint32_t r;
+    asm("cvt.rna.tf32.f32 %0, %1;" : "=r"(r) : "f"(x));
+    return __uint_as_float(r);
+}
+// the same split with integer arithmetic: hi = x rounded to 10 mantissa bits (ties away), lo = x - hi exactly (the tensor
+// core reads only lo's upper 19 bits: error <= 2^-21 |x|)
+__device__ __forceinline__ void tf32_split(float x, float& hi, float& lo) {
+    hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
+    lo = x - hi;
+}
+
+// ---------------------------------------------------------------------------------------------------
+// wgmma
+// ---------------------------------------------------------------------------------------------------
+// K-major operand tile, rows of exactly 128 bytes (32 fp32), 128-byte swizzle, 8-row groups 1024 B apart (sm_90 layout)
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);        // start address
+    d |= (uint64_t)1 << 16;                              // leading byte offset (unused for swizzled K-major)
+    d |= (uint64_t)(1024 >> 4) << 32;                    // stride byte offset: next 8-row group
+    d |= (uint64_t)1 << 62;                              // SWIZZLE_128B
+    return d;
+}
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+
+// d (+)= A[smem] * B[smem]^T, M = 64, N = 128, K = 8, tf32 inputs, fp32 accumulators in registers
+__device__ __forceinline__ void wgmma_tf32_m64n128(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+
+// ---------------------------------------------------------------------------------------------------
+// the GEMM engine
+// ---------------------------------------------------------------------------------------------------
+constexpr int HG_BM = 128, HG_BN = 128, HG_BK = 32, HG_THREADS = 256;
+constexpr int HG_TILE_BYTES = 128 * HG_BK * 4;                        // 16 KB: 128 rows x 32 fp32
+constexpr int HG_STAGE_BYTES = 4 * HG_TILE_BYTES;                     // A hi | A lo | B hi | B lo
+constexpr int HG_SMEM_BYTES = 2 * HG_STAGE_BYTES + 1024;              // double-buffered, 1 KB alignment slack
+
+// Operand fetch, per 128-row tile and K block (ops implement a4 / b4 with the signature below):
+//   K-contiguous operand (Op::A_KCONTIG / B_KCONTIG):  v4(cta, kb, row, q) = elements k = 4q .. 4q+3 of tile row `row`
+//   M/N-contiguous operand:                            v4(cta, kb, k, q)   = tile rows 4q .. 4q+3 at reduction index k
+// Out-of-range elements (padding, tails, other samples) are returned as zeros.
+template <bool KCONTIG>
+struct HgSlot {
+    // the 4 float4 this thread moves per 128 x 32 tile: (i, q) = (row, k quad) or (k, row quad)
+    __device__ static void coords(int tid, int j, int& i, int& q) {
+        const int idx = tid + HG_THREADS * j;
+        if (KCONTIG) { i = idx >> 3; q = idx & 7; }
+        else {                                   // lanes: 8 k x 4 row quads (64 B contiguous per k, 2-way bank conflicts)
+            const int lane = idx & 31, w = idx >> 5;
+            i = (w & 3) * 8 + (lane & 7);
+            q = (w >> 2) * 4 + (lane >> 3);
+        }
+    }
+    __device__ static void store(uint8_t* hi, uint8_t* lo, int i, int q, float4 v) {
+        if (KCONTIG) {
+            float4 h, l;
+            tf32_split(v.x, h.x, l.x); tf32_split(v.y, h.y, l.y); tf32_split(v.z, h.z, l.z); tf32_split(v.w, h.w, l.w);
+            const int off = i * 128 + ((q ^ (i & 7)) << 4);
+            *reinterpret_cast<float4*>(hi + off) = h;
+            *reinterpret_cast<float4*>(lo + off) = l;
+        } else {
+            const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+            for (int c = 0; c < 4; ++c) {
+                const int r = 4 * q + c;
+                const int off = r * 128 + (((i >> 2) ^ (r & 7)) << 4) + (i & 3) * 4;
+                float h, l;
+                tf32_split(e[c], h, l);
+                *reinterpret_cast<float*>(hi + off) = h;
+                *reinterpret_cast<float*>(lo + off) = l;
+            }
+        }
+    }
+};
+
+// Accumulator fragment of warpgroup g (m64n128): element i of thread (warp w of the group, lane) is
+//   row 64 g + 16 w + lane/4 + 8 ((i >> 1) & 1),  column 8 (i >> 2) + 2 (lane & 3) + (i & 1)
+__device__ __forceinline__ int hg_row(int i) {
+    const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+    return 16 * w + (lane >> 2) + 8 * ((i >> 1) & 1);
+}
+__device__ __forceinline__ int hg_col(int i) { return 8 * (i >> 2) + 2 * (threadIdx.x & 3) + (i & 1); }
+
+template <class Op>
+__global__ void __launch_bounds__(HG_THREADS, 1) hg_gemm_kernel(const __grid_constant__ Op op) {
+    extern __shared__ uint8_t smem_raw[];
+    const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
+    const int tid = threadIdx.x, wg = tid >> 7;
+    using SA = HgSlot<Op::A_KCONTIG>;
+    using SB = HgSlot<Op::B_KCONTIG>;
+
+    const typename Op::Cta cta = op.cta();
+    const int nkb = op.kblocks(cta);
+    float4 ra[4], rb[4];
+    auto fetch = [&](int kb) {
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            int i, q;
+            SA::coords(tid, j, i, q);
+            ra[j] = op.a4(cta, kb, i, q);
+            SB::coords(tid, j, i, q);
+            rb[j] = op.b4(cta, kb, i, q);
+        }
+    };
+    auto stash = [&](int s) {
+        uint8_t* st = smem + s * HG_STAGE_BYTES;
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            int i, q;
+            SA::coords(tid, j, i, q);
+            SA::store(st, st + HG_TILE_BYTES, i, q, ra[j]);
+            SB::coords(tid, j, i, q);
+            SB::store(st + 2 * HG_TILE_BYTES, st + 3 * HG_TILE_BYTES, i, q, rb[j]);
+        }
+    };
+
+    float acc[64], part[64];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    if (nkb > 0) {
+        fetch(0);
+        stash(0);
+        fence_proxy_async();
+        __syncthreads();
+    }
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb & 1;
+        if (kb + 1 < nkb) fetch(kb + 1);
+        const uint32_t st = base_u32 + s * HG_STAGE_BYTES;
+        const uint32_t a_hi = st + wg * (HG_TILE_BYTES / 2), a_lo = a_hi + HG_TILE_BYTES;
+        const uint32_t b_hi = st + 2 * HG_TILE_BYTES, b_lo = b_hi + HG_TILE_BYTES;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < HG_BK / 8; ++kk) {
+            const uint32_t off = kk * 32;                  // 8 tf32 = 32 bytes along K inside the swizzle span
+            const uint64_t dah = wgmma_desc_k_sw128(a_hi + off), dal = wgmma_desc_k_sw128(a_lo + off);
+            const uint64_t dbh = wgmma_desc_k_sw128(b_hi + off), dbl = wgmma_desc_k_sw128(b_lo + off);
+            wgmma_tf32_m64n128(part, dal, dbh, kk != 0);
+            wgmma_tf32_m64n128(part, dah, dbl, 1);
+            wgmma_tf32_m64n128(part, dah, dbh, 1);
+        }
+        wgmma_commit();
+        if (kb + 1 < nkb) stash(s ^ 1);                    // the other stage's MMAs completed in the previous iteration
+        wgmma_wait_all();
+#pragma unroll
+        for (int i = 0; i < 64; ++i) acc[i] += part[i];
+        fence_proxy_async();
+        __syncthreads();
+    }
+    op.epilogue(cta, acc, 64 * wg);
+}
+
+template <class Op>
+inline int hg_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) {
+    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hg_gemm_kernel<Op>), HG_SMEM_BYTES)) return rc;
+    if (grid.x == 0 || grid.y == 0 || grid.z == 0) return 0;
+    if (grid.y > 65535 || grid.z > 65535) return set_error(2, "%s: grid too large%s", who);
+    hg_gemm_kernel<Op><<<grid, HG_THREADS, HG_SMEM_BYTES, st>>>(op);
+    ++g_launches;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", who, cudaGetErrorString(e));
+    return 0;
+}
+
+// the plain epilogue: D[z plane][row][col] = acc for rows < rows, cols < cols (row-major, leading dimension ld)
+struct HgStore {
+    float* D;
+    long long ld;
+    int rows, cols;
+    __device__ void store(const float* acc, int m0, int n0) const {
+#pragma unroll
+        for (int i = 0; i < 64; i += 2) {
+            const int r = m0 + hg_row(i), c = n0 + hg_col(i);
+            if (r >= rows) continue;
+            float* d = D + (long long)r * ld + c;
+            if (c + 1 < cols && ((reinterpret_cast<uintptr_t>(d) & 7) == 0)) {
+                *reinterpret_cast<float2*>(d) = make_float2(acc[i], acc[i + 1]);
+            } else {
+                if (c < cols) d[0] = acc[i];
+                if (c + 1 < cols) d[1] = acc[i + 1];
+            }
+        }
+    }
+};
+
+}  // namespace tc
 
 }  // namespace bm

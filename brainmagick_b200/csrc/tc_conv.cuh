@@ -1,244 +1,206 @@
-// K3/K4 on the 5th-generation tensor cores: dilated Conv1d as an implicit GEMM with 3xTF32 error compensation.
+// K3/K4/K5 on the Hopper tensor cores: dilated Conv1d (and its data gradient, and the 1x1 head / subject layers) as an
+// implicit GEMM on the 3xTF32 wgmma engine of tc_common.cuh.
 //
-//   y[b, t, n] = bias[n] + sum_{tap} sum_{k} x[b, t + shift(tap), k] * W[tap][n][k]      (channels-last x, y)
+//   y[b, t, n] = bias[n] + sum_{tap} sum_{k} x[b, t + shift(tap), k] * W[wset(b)][tap][n][k]      (channels-last x, y)
 //
-// Roles inside one CTA (192 threads), one 128(t) x 160(n) output tile per CTA:
-//   warp 0    TMA producer: per (tap, 32-wide k chunk) one 3-D box of x (rows shifted by the tap; rows outside
-//             [0,T) are zero-filled by TMA = the conv's zero padding) and the matching rows of W_hi / W_lo,
-//             all in the 128-byte-swizzled K-major layout tcgen05 reads.
-//   warps 2-5 split the fp32 x tile in shared memory into tf32 hi and lo parts (in place + a second buffer),
-//             then act as the epilogue: TMEM -> registers -> bias / skip-gradient add / GLU -> global.
-//   warp 1    one thread issues tcgen05.mma (kind::tf32, M=128, N=160, K=8): hi*hi + lo*hi + hi*lo into an
-//             fp32 accumulator in tensor memory; tcgen05.commit releases the stage back to the producer.
-// Every mbarrier wait is bounded (tc_common.cuh) so a pipeline bug reports an error instead of hanging the GPU.
+// shift(tap) = sign * (tap - taps/2) * dilation; a shifted time outside [0, T) reads zeros (the conv's zero padding, never
+// the neighbouring sample).  One CTA = 128 times of one sample x 128 output columns (GLU: 64 'a' columns and the 64 gate
+// columns they pair with, so that a * sigmoid(gate) is formed in registers).  The weights arrive either as fp32
+// [sets][taps][Ntot][Cin] or as the two fp16 pieces of a power-of-two-scaled copy (bm_tc_weight_split_f16), which are
+// summed back on load (~22 significant bits of the weight: the precision the pieces carry).  Fused epilogue: bias, addend (skip gradient / in-place accumulate),
+// pre-activation copy, exact GELU, channel-major store, GLU, BatchNorm column statistics (fp64), max |output|.
 #pragma once
+#include <cuda_fp16.h>
+#include <cstring>
 #include "tc_common.cuh"
 
 namespace bm {
 namespace tc {
 
-constexpr int CV_BM = 128, CV_BN = 160, CV_BK = 32, CV_STAGES = 3, CV_THREADS = 192;
-constexpr int CV_A_BYTES = CV_BM * CV_BK * 4;       // 16 KB
-constexpr int CV_B_BYTES = CV_BN * CV_BK * 4;       // 20 KB
-constexpr int CV_STAGE_BYTES = 2 * CV_A_BYTES + 2 * CV_B_BYTES;
-constexpr int CV_SMEM_BYTES = CV_STAGES * CV_STAGE_BYTES + 1024;
+constexpr int HP_TARGET_EXP = 14;                                    // scaled maximum in [2^14, 2^15)
 
-struct ConvTcP {
-    int B, T, Cin, Ntot;      // Ntot = output channels of the GEMM (2H for the GLU conv)
-    int taps, dilation, sign;
-    int glu;                  // 1: tile = 80 'a' columns + 80 gate columns, out = a * sigmoid(gate)
-    int bn;                   // N tile (multiple of 16, <= 160; 160 when glu)
-    int act;                  // 1: exact GELU on the output (after bias/addend); `aux` receives the pre-activation
-    int out_tmajor;           // 1: y is [B, Ntot, T] (channel-major, the encoder's output layout)
-    const float* bias;        // [Ntot] or null
-    const float* addend;      // [B,T,Ntot] or null
-    float* y;                 // [B,T,Ntot] (pre-GLU h when glu; may be null then)
-    float* aux;               // [B,T,Ntot] or null
-    float* glu_out;           // [B,T,Ntot/2]
-    int n_wsets;              // number of weight sets when wsel != null
-    const int* wsel;          // per-sample weight set (SubjectLayers): weight rows are offset by wsel[b]*taps*Ntot; or null
+// The power of two that puts a tensor whose largest magnitude is `amax` into [2^14, 2^15) (where both fp16 pieces of a
+// value are exact); 1 for an all-zero / non-finite tensor.  Identical on every thread that evaluates it (bit arithmetic).
+__host__ __device__ __forceinline__ float f16_scale_of(float amax) {
+#ifdef __CUDA_ARCH__
+    const uint32_t bits = __float_as_uint(amax);
+#else
+    uint32_t bits; memcpy(&bits, &amax, 4);
+#endif
+    const int e = (int)((bits >> 23) & 0xFF);
+    if (e == 0 || e == 255) return 1.0f;
+    int se = 127 + HP_TARGET_EXP - (e - 127);             // exponent field of the scale
+    se = se < 1 ? 1 : (se > 254 ? 254 : se);
+    const uint32_t sb = (uint32_t)se << 23;
+#ifdef __CUDA_ARCH__
+    return __uint_as_float(sb);
+#else
+    float s; memcpy(&s, &sb, 4); return s;
+#endif
+}
+
+struct ConvOp {
+    static constexpr bool A_KCONTIG = true, B_KCONTIG = true;
+    const float* x;                       // [B, T, Cin]
+    const float* w;                       // fp32 weights [sets][taps][Ntot][Cin], or null: fp16 pieces below
+    const float* w_lo32;                  // nullable: second tf32 piece of w (bm_tc_weight_split), added back on load
+    const __half* w_hi; const __half* w_lo; const float* w_amax;
+    int B, T, Cin, Ntot, taps, dilation, sign, glu, ttiles;
+    int n_wsets; const int* wsel;         // per-sample weight set (SubjectLayers) or null
+    const float* bias;                    // [Ntot] or null
+    const float* addend;                  // [B,T,Ntot] or null (may alias y: in-place accumulate)
+    float* y;                             // [B,T,Ntot], [B,Ntot,T] when out_tmajor; GLU: the pre-GLU h (nullable)
+    float* aux;                           // pre-activation copy or null
+    float* glu_out;                       // GLU: [B,T,Ntot/2]
+    double* stats;                        // [2*Ntot] column sum / sum of squares of y (zeroed by the launcher) or null
+    unsigned int* out_amax;               // max |GELU / GLU output| (float bits) or null
+    int act, out_tmajor;
     int* err;
-};
 
-__global__ void __launch_bounds__(CV_THREADS, 1)
-conv_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBhi,
-               const __grid_constant__ CUtensorMap tmBlo, const ConvTcP p) {
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[CV_STAGES], conv_bar[CV_STAGES], empty_bar[CV_STAGES], tmem_full_bar;
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ int prior_error;
-
-    // a previous CTA already reported a pipeline failure: do not spend another timeout on it
-    if (threadIdx.x == 0) prior_error = p.err ? *reinterpret_cast<volatile int*>(p.err) : 0;
-    __syncthreads();
-    if (prior_error) return;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
-
-    const int n_tile = blockIdx.x, t0 = blockIdx.y * CV_BM, b = blockIdx.z;
-    const int kchunks = p.Cin / CV_BK;
-    const int total = p.taps * kchunks;
-    const int H = p.Ntot / 2;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < CV_STAGES; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&conv_bar[s], 128);
-            mbar_init(&empty_bar[s], 1);
+    struct Cta { int b, t0, n_tile, wbase; float w_inv; };
+    __device__ Cta cta() const {
+        Cta c;
+        c.b = blockIdx.x / ttiles;
+        c.t0 = (blockIdx.x - c.b * ttiles) * HG_BM;
+        c.n_tile = blockIdx.y;
+        int s = wsel ? wsel[c.b] : 0;
+        if (s < 0 || s >= n_wsets) {                 // a subject / recording index outside the weight sets: report it like
+            if (err && threadIdx.x == 0) atomicCAS(err, 0, 900);     // the reference's gather would raise
+            s = 0;
         }
-        mbar_init(&tmem_full_bar, 1);
-        fence_barrier_init();
+        c.wbase = s * taps;
+        c.w_inv = w ? 1.f : 1.f / f16_scale_of(__ldg(w_amax));
+        return c;
     }
-    if (warp == 1) tmem_alloc<256>(&tmem_base_smem);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_smem;
+    __device__ int kblocks(const Cta&) const { return taps * (Cin / HG_BK); }
+    __device__ float4 a4(const Cta& c, int kb, int r, int q) const {
+        const int kch = Cin / HG_BK, tap = kb / kch, k0 = (kb - tap * kch) * HG_BK;
+        const int t = c.t0 + r, ts = t + sign * (tap - taps / 2) * dilation;
+        if (t >= T || ts < 0 || ts >= T) return make_float4(0.f, 0.f, 0.f, 0.f);
+        return __ldg(reinterpret_cast<const float4*>(x + ((long long)c.b * T + ts) * Cin + k0) + q);
+    }
+    // output column of tile column j (GLU: j < 64 'a' columns, j >= 64 their gates), -1 past the end
+    __device__ int col_of(const Cta& c, int j) const {
+        if (glu) {
+            const int H = Ntot / 2, cc = c.n_tile * 64 + (j & 63);
+            return cc < H ? cc + (j >= 64 ? H : 0) : -1;
+        }
+        const int n = c.n_tile * HG_BN + j;
+        return n < Ntot ? n : -1;
+    }
+    __device__ float4 b4(const Cta& c, int kb, int j, int q) const {
+        const int n = col_of(c, j);
+        if (n < 0) return make_float4(0.f, 0.f, 0.f, 0.f);
+        const int kch = Cin / HG_BK, tap = kb / kch, k0 = (kb - tap * kch) * HG_BK;
+        const long long off = ((long long)(c.wbase + tap) * Ntot + n) * Cin + k0 + 4 * q;
+        if (w) {
+            float4 v = __ldg(reinterpret_cast<const float4*>(w + off));
+            if (w_lo32) {
+                const float4 l = __ldg(reinterpret_cast<const float4*>(w_lo32 + off));
+                v.x += l.x; v.y += l.y; v.z += l.z; v.w += l.w;
+            }
+            return v;
+        }
+        const uint2 h = __ldg(reinterpret_cast<const uint2*>(w_hi + off)), l = __ldg(reinterpret_cast<const uint2*>(w_lo + off));
+        const float2 h0 = __half22float2(*reinterpret_cast<const __half2*>(&h.x)), h1 = __half22float2(*reinterpret_cast<const __half2*>(&h.y));
+        const float2 l0 = __half22float2(*reinterpret_cast<const __half2*>(&l.x)), l1 = __half22float2(*reinterpret_cast<const __half2*>(&l.y));
+        return make_float4((h0.x + l0.x) * c.w_inv, (h0.y + l0.y) * c.w_inv, (h1.x + l1.x) * c.w_inv, (h1.y + l1.y) * c.w_inv);
+    }
 
-    if (warp == 0) {
-        if (lane == 0) {
-            prefetch_tmap(&tmA);
-            prefetch_tmap(&tmBhi);
-            prefetch_tmap(&tmBlo);
-            int wsel = p.wsel ? p.wsel[b] : 0;
-            if (wsel < 0 || wsel >= p.n_wsets) {             // a subject / recording index outside the weight sets: the TMA would
-                if (p.err) atomicCAS(p.err, 0, 900);         // zero-fill silently; report it like the reference's gather would raise
-                wsel = 0;
-            }
-            const int wsel_base = wsel * p.taps;
-            for (int it = 0; it < total; ++it) {
-                const int s = it % CV_STAGES;
-                const uint32_t ph = (it / CV_STAGES) & 1;
-                if (!mbar_wait(&empty_bar[s], ph ^ 1, p.err, 1)) break;
-                const int tap = it / kchunks, k0 = (it - tap * kchunks) * CV_BK;
-                const int shift = p.sign * (tap - p.taps / 2) * p.dilation;
-                uint8_t* st = smem + s * CV_STAGE_BYTES;
-                mbar_expect_tx(&full_bar[s], CV_A_BYTES + 2 * p.bn * CV_BK * 4);
-                tma_load_3d(st, &tmA, &full_bar[s], k0, t0 + shift, b);
-                uint8_t* bh = st + 2 * CV_A_BYTES;
-                uint8_t* bl = bh + CV_B_BYTES;
-                if (!p.glu) {
-                    const int row = (wsel_base + tap) * p.Ntot + n_tile * p.bn;
-                    tma_load_2d(bh, &tmBhi, &full_bar[s], k0, row);
-                    tma_load_2d(bl, &tmBlo, &full_bar[s], k0, row);
-                } else {
-                    const int ra = tap * p.Ntot + n_tile * (CV_BN / 2), rg = ra + H;
-                    tma_load_2d(bh, &tmBhi, &full_bar[s], k0, ra);
-                    tma_load_2d(bh + CV_B_BYTES / 2, &tmBhi, &full_bar[s], k0, rg);
-                    tma_load_2d(bl, &tmBlo, &full_bar[s], k0, ra);
-                    tma_load_2d(bl + CV_B_BYTES / 2, &tmBlo, &full_bar[s], k0, rg);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc_tf32(CV_BM, p.bn);
-            bool ok = true;
-            for (int it = 0; it < total && ok; ++it) {
-                const int s = it % CV_STAGES;
-                const uint32_t ph = (it / CV_STAGES) & 1;
-                ok = mbar_wait(&full_bar[s], ph, p.err, 2) && mbar_wait(&conv_bar[s], ph, p.err, 3);
-                if (!ok) break;
-                tc_fence_after();
-                const uint32_t a_hi = smem_base + s * CV_STAGE_BYTES;
-                const uint32_t a_lo = a_hi + CV_A_BYTES;
-                const uint32_t b_hi = a_lo + CV_A_BYTES;
-                const uint32_t b_lo = b_hi + CV_B_BYTES;
+    __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+        __shared__ double col_sums[2 * HG_BN];
+        float am = 0.f;
+        if (glu) {
+            const int H = Ntot / 2;
 #pragma unroll
-                for (int kk = 0; kk < CV_BK / 8; ++kk) {
-                    const uint32_t off = kk * 32;      // 8 tf32 = 32 bytes along K inside the 128-byte swizzle span
-                    const uint64_t dah = umma_desc_k_sw128(a_hi + off), dal = umma_desc_k_sw128(a_lo + off);
-                    const uint64_t dbh = umma_desc_k_sw128(b_hi + off), dbl = umma_desc_k_sw128(b_lo + off);
-                    umma_tf32_ss(tmem, dal, dbh, idesc, (it | kk) != 0);
-                    umma_tf32_ss(tmem, dah, dbl, idesc, 1);
-                    umma_tf32_ss(tmem, dah, dbh, idesc, 1);
-                }
-                umma_commit(&empty_bar[s]);
-            }
-            umma_commit(&tmem_full_bar);
-        }
-    } else {
-        // ---- converter: split the x tile into tf32 hi (in place) and lo ----
-        const int ct = (warp - 2) * 32 + lane;          // 0..127
-        bool ok = true;
-        for (int it = 0; it < total && ok; ++it) {
-            const int s = it % CV_STAGES;
-            const uint32_t ph = (it / CV_STAGES) & 1;
-            ok = mbar_wait(&full_bar[s], ph, p.err, 4);
-            float4* hi = reinterpret_cast<float4*>(smem + s * CV_STAGE_BYTES);
-            float4* lo = reinterpret_cast<float4*>(smem + s * CV_STAGE_BYTES + CV_A_BYTES);
-#pragma unroll
-            for (int j = 0; j < CV_A_BYTES / 16 / 128; ++j) {
-                const int idx = ct + 128 * j;
-                float4 v = hi[idx], h, l;
-                tf32_split(v.x, h.x, l.x); tf32_split(v.y, h.y, l.y); tf32_split(v.z, h.z, l.z); tf32_split(v.w, h.w, l.w);
-                hi[idx] = h;
-                lo[idx] = l;
-            }
-            fence_proxy_async();
-            mbar_arrive(&conv_bar[s]);
-        }
-        // ---- epilogue ----
-        mbar_wait(&tmem_full_bar, 0, p.err, 5);
-        tc_fence_after();
-        const int q = warp & 3;                          // TMEM lane quarter this warp may access
-        const int t = t0 + q * 32 + lane;
-        const bool valid = t < p.T;
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16);
-        const float comp = acc_trunc_comp(total * (CV_BK / 8) * 3);          // additions chained into the accumulator
-        if (!p.glu) {
-            const int n0 = n_tile * p.bn;
-            const long long off = ((long long)b * p.T + t) * p.Ntot + n0;
-#pragma unroll 1
-            for (int c = 0; c < p.bn / 16; ++c) {
-                float v[16];
-                tmem_ld16(tq + c * 16, v);
-#pragma unroll
-                for (int j = 0; j < 16; ++j) v[j] *= comp;
-                if (valid) {
-#pragma unroll
-                    for (int j = 0; j < 16; j += 4) {
-                        float4 o = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-                        if (p.bias) {
-                            float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + c * 16 + j);
-                            o.x += bb.x; o.y += bb.y; o.z += bb.z; o.w += bb.w;
-                        }
-                        if (p.addend) {
-                            float4 aa = *reinterpret_cast<const float4*>(p.addend + off + c * 16 + j);
-                            o.x += aa.x; o.y += aa.y; o.z += aa.z; o.w += aa.w;
-                        }
-                        if (p.aux) *reinterpret_cast<float4*>(p.aux + off + c * 16 + j) = o;
-                        if (p.act) { o.x = gelu_f(o.x); o.y = gelu_f(o.y); o.z = gelu_f(o.z); o.w = gelu_f(o.w); }
-                        if (!p.out_tmajor) {
-                            *reinterpret_cast<float4*>(p.y + off + c * 16 + j) = o;
-                        } else {
-                            float* yt = p.y + ((long long)b * p.Ntot + n0 + c * 16 + j) * p.T + t;
-                            yt[0] = o.x; yt[p.T] = o.y; yt[2 * (long long)p.T] = o.z; yt[3 * (long long)p.T] = o.w;
-                        }
-                    }
-                }
+            for (int i = 0; i < 32; ++i) {               // tile columns 0..63; the gate of column j is column j + 64
+                const int t = c.t0 + m0 + hg_row(i), cc = c.n_tile * 64 + hg_col(i);
+                if (t >= T || cc >= H) continue;
+                const long long row = (long long)c.b * T + t;
+                float a = acc[i], g = acc[i + 32];
+                if (bias) { a += bias[cc]; g += bias[H + cc]; }
+                if (y) { y[row * Ntot + cc] = a; y[row * Ntot + H + cc] = g; }
+                const float o = a * sigmoid_f(g);
+                glu_out[row * H + cc] = o;
+                am = fmaxf(am, fabsf(o));
             }
         } else {
-            const int c0 = n_tile * (CV_BN / 2);
-            const long long row = (long long)b * p.T + t;
-#pragma unroll 1
-            for (int c = 0; c < (CV_BN / 2) / 16; ++c) {
-                float a[16], g[16];
-                tmem_ld16(tq + c * 16, a);
-                tmem_ld16(tq + CV_BN / 2 + c * 16, g);
+            if (stats) {
+                for (int i = threadIdx.x; i < 2 * HG_BN; i += HG_THREADS) col_sums[i] = 0.0;
+                __syncthreads();
+            }
 #pragma unroll
-                for (int j = 0; j < 16; ++j) { a[j] *= comp; g[j] *= comp; }
-                if (valid) {
+            for (int g = 0; g < 16; ++g) {
 #pragma unroll
-                    for (int j = 0; j < 16; j += 4) {
-                        float4 av = make_float4(a[j], a[j + 1], a[j + 2], a[j + 3]);
-                        float4 gv = make_float4(g[j], g[j + 1], g[j + 2], g[j + 3]);
-                        if (p.bias) {
-                            float4 ba = *reinterpret_cast<const float4*>(p.bias + c0 + c * 16 + j);
-                            float4 bg = *reinterpret_cast<const float4*>(p.bias + H + c0 + c * 16 + j);
-                            av.x += ba.x; av.y += ba.y; av.z += ba.z; av.w += ba.w;
-                            gv.x += bg.x; gv.y += bg.y; gv.z += bg.z; gv.w += bg.w;
+                for (int e = 0; e < 2; ++e) {
+                    float s1 = 0.f, s2 = 0.f;
+                    const int j = 8 * g + 2 * (threadIdx.x & 3) + e, n = c.n_tile * HG_BN + j;
+#pragma unroll
+                    for (int h = 0; h < 2; ++h) {
+                        const int i = 4 * g + 2 * h + e;
+                        const int t = c.t0 + m0 + hg_row(i);
+                        if (t >= T || n >= Ntot) continue;
+                        const long long row = (long long)c.b * T + t;
+                        float v = acc[i];
+                        if (bias) v += bias[n];
+                        if (addend) v += addend[row * Ntot + n];
+                        if (aux) aux[row * Ntot + n] = v;
+                        if (act) { v = gelu_f(v); am = fmaxf(am, fabsf(v)); }
+                        if (out_tmajor) y[((long long)c.b * Ntot + n) * T + t] = v;
+                        else y[row * Ntot + n] = v;
+                        s1 += v;
+                        s2 = fmaf(v, v, s2);
+                    }
+                    if (stats) {
+#pragma unroll
+                        for (int o = 4; o < 32; o <<= 1) {
+                            s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+                            s2 += __shfl_xor_sync(0xffffffffu, s2, o);
                         }
-                        if (p.y) {
-                            *reinterpret_cast<float4*>(p.y + row * p.Ntot + c0 + c * 16 + j) = av;
-                            *reinterpret_cast<float4*>(p.y + row * p.Ntot + H + c0 + c * 16 + j) = gv;
+                        if ((threadIdx.x & 31) < 4 && n < Ntot) {
+                            atomicAdd(&col_sums[j], (double)s1);
+                            atomicAdd(&col_sums[HG_BN + j], (double)s2);
                         }
-                        float4 o = make_float4(av.x * sigmoid_f(gv.x), av.y * sigmoid_f(gv.y), av.z * sigmoid_f(gv.z),
-                                               av.w * sigmoid_f(gv.w));
-                        *reinterpret_cast<float4*>(p.glu_out + row * H + c0 + c * 16 + j) = o;
+                    }
+                }
+            }
+            if (stats) {
+                __syncthreads();
+                for (int j = threadIdx.x; j < HG_BN; j += HG_THREADS) {
+                    const int n = c.n_tile * HG_BN + j;
+                    if (n < Ntot) {
+                        atomicAdd(stats + n, col_sums[j]);
+                        atomicAdd(stats + Ntot + n, col_sums[HG_BN + j]);
                     }
                 }
             }
         }
-        tc_fence_before();
+        if (out_amax) {
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, o));
+            if ((threadIdx.x & 31) == 0 && am > 0.f) atomicMax(out_amax, __float_as_uint(am));
+        }
     }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<256>(tmem);
+};
+
+inline ConvOp conv_op_defaults() {
+    ConvOp o;
+    memset(&o, 0, sizeof(o));
+    o.n_wsets = 1;
+    return o;
+}
+
+inline int launch_conv_op(ConvOp o, cudaStream_t st, const char* who) {
+    if ((long long)o.B * o.T >= (1ll << 31)) return set_error(2, "%s: too many rows%s", who);
+    o.ttiles = (o.T + HG_BM - 1) / HG_BM;
+    const long long ctas = (long long)o.B * o.ttiles;
+    if (ctas >= (1ll << 31)) return set_error(2, "%s: too many rows%s", who);
+    const int ntiles = o.glu ? (o.Ntot / 2 + 63) / 64 : (o.Ntot + HG_BN - 1) / HG_BN;
+    if (o.stats) {
+        cudaError_t em = cudaMemsetAsync(o.stats, 0, sizeof(double) * 2 * o.Ntot, st);
+        if (em != cudaSuccess) return set_error(3, "%s: memset: %s", who, cudaGetErrorString(em));
     }
+    return hg_launch(o, dim3((unsigned)ctas, (unsigned)ntiles, 1), st, who);
 }
 
 // W[o][i][j] (nn.Conv1d layout) -> tf32-split K-major operands:
@@ -260,44 +222,32 @@ __global__ void weight_split_kernel(const float* __restrict__ W, float* __restri
     }
 }
 
-// N tile for a GEMM with Ntot output columns: the largest multiple of 16 <= 160 that divides Ntot (0: unsupported)
-inline int conv_tc_pick_bn(int Ntot, int glu) {
-    if (glu) return (Ntot % 2 == 0 && (Ntot / 2) % (CV_BN / 2) == 0) ? CV_BN : 0;
-    for (int bn = CV_BN; bn >= 64; bn -= 16)
-        if (Ntot % bn == 0) return bn;
-    return 0;
-}
+// Shape gate of bm_tc_conv1d / bm_tc_pointwise_sel: Ntot a multiple of 16 with a divisor in [64, 160] (GLU: H a multiple
+// of 80), K chunks of 32 input channels.  The kernel itself handles any N; the gate is the library's published contract.
 inline bool conv_tc_supported(int T, int Cin, int Ntot, int Kw, int glu) {
     if (Kw < 1 || Kw > 3 || (Kw & 1) == 0) return false;
-    if (Cin % CV_BK != 0) return false;
-    return conv_tc_pick_bn(Ntot, glu) != 0;
+    if (Cin % HG_BK != 0) return false;
+    if (glu) return Ntot % 2 == 0 && (Ntot / 2) % 80 == 0;
+    for (int bn = 160; bn >= 64; bn -= 16)
+        if (Ntot % bn == 0) return true;
+    return false;
 }
 
-// x [B,T,Cin]; w_hi/w_lo [Kw][Ntot][Cin]
-inline int launch_conv_tc(const float* x, const float* w_hi, const float* w_lo, ConvTcP p, cudaStream_t st) {
-    p.bn = conv_tc_pick_bn(p.Ntot, p.glu);
-    if (p.bn == 0) return set_error(2, "%s: unsupported N%s", __func__);
-    CUtensorMap tmA, tmBh, tmBl;
-    {
-        uint64_t dims[3] = {(uint64_t)p.Cin, (uint64_t)p.T, (uint64_t)p.B};
-        uint64_t str[2] = {(uint64_t)p.Cin * 4, (uint64_t)p.T * p.Cin * 4};
-        uint32_t box[3] = {CV_BK, CV_BM, 1};
-        if (!make_tmap_f32(&tmA, x, 3, dims, str, box)) return set_error(4, "%s: cuTensorMapEncodeTiled(A) failed%s", __func__);
-    }
-    {
-        uint64_t dims[2] = {(uint64_t)p.Cin, (uint64_t)p.taps * p.Ntot * (uint64_t)(p.wsel ? p.n_wsets : 1)};
-        uint64_t str[1] = {(uint64_t)p.Cin * 4};
-        uint32_t box[2] = {CV_BK, (uint32_t)(p.glu ? CV_BN / 2 : p.bn)};
-        if (!make_tmap_f32(&tmBh, w_hi, 2, dims, str, box) || !make_tmap_f32(&tmBl, w_lo, 2, dims, str, box))
-            return set_error(4, "%s: cuTensorMapEncodeTiled(B) failed%s", __func__);
-    }
-    if (int rc_ = ensure_dyn_smem(reinterpret_cast<const void*>(conv_tc_kernel), CV_SMEM_BYTES)) return rc_;
-    dim3 grid(p.glu ? (p.Ntot / 2) / (CV_BN / 2) : p.Ntot / p.bn, (p.T + CV_BM - 1) / CV_BM, p.B);
-    conv_tc_kernel<<<grid, CV_THREADS, CV_SMEM_BYTES, st>>>(tmA, tmBh, tmBl, p);
-    ++g_launches;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", __func__, cudaGetErrorString(e));
-    return 0;
+// x [B,T,Cin]; w_hi / w_lo [Kw][Ntot][Cin] (wsel: [n_wsets][Kw][Ntot][Cin]), the tf32 pieces of bm_tc_weight_split
+struct ConvTcP {
+    int B, T, Cin, Ntot, taps, dilation, sign, glu, act, out_tmajor;
+    const float* bias; const float* addend;
+    float* y; float* aux; float* glu_out;
+    int n_wsets; const int* wsel;
+    int* err;
+};
+inline int launch_conv_tc(const float* x, const float* w_hi, const float* w_lo, const ConvTcP& p, cudaStream_t st) {
+    ConvOp o = conv_op_defaults();
+    o.x = x; o.w = w_hi; o.w_lo32 = w_lo; o.B = p.B; o.T = p.T; o.Cin = p.Cin; o.Ntot = p.Ntot; o.taps = p.taps; o.dilation = p.dilation;
+    o.sign = p.sign; o.glu = p.glu; o.n_wsets = p.wsel ? p.n_wsets : 1; o.wsel = p.wsel; o.bias = p.bias;
+    o.addend = p.addend; o.y = p.y; o.aux = p.aux; o.glu_out = p.glu_out; o.act = p.act; o.out_tmajor = p.out_tmajor;
+    o.err = p.err;
+    return launch_conv_op(o, st, __func__);
 }
 
 }  // namespace tc

@@ -1,410 +1,13 @@
-// K3/K4/K5 on the F16 tensor pipe: the persistent CTA-pair conv of tc_convp.cuh with fp32 operands carried as TWO FP16 PIECES
-// (x*s = hi + lo, 11 + 11 significant bits) instead of two TF32 pieces.
-//
-// Why.  conv_pp_kernel runs at 93-98 % of what 3xTF32 can give: three kind::tf32 MMAs per product at half the f16 rate is a
-// ceiling of peak/6.  kind::f16 consumes the same operand BYTES per instruction for twice the K (16 instead of 8), so the
-// same three products (hi*hi + lo*hi + hi*lo) cost half the tensor-pipe time: ceiling peak/3.  The operand precision is the
-// same 22 bits (tf32: 11 + 11, f16: 11 + 11), rounded to nearest here rather than truncated.
-//
-// What FP16 needs that TF32 did not: range.  An fp16 piece is exact only inside [2^-14, 2^16); each operand TENSOR is
-// therefore scaled by a power of two that puts its largest magnitude in [2^14, 2^15) (bm_amax: one HBM pass, or the
-// producer's epilogue) and the epilogue multiplies the accumulator by the inverse (exact).  Elements more than 2^17 below
-// the tensor's maximum lose low bits gradually (fp16 subnormals): their absolute error is <= 2^-25 of the scaled maximum,
-// i.e. 2^-40 relative to the tensor's largest element -- invisible next to fp32's own rounding of the sums they enter.
-//
-//   per K chunk (32 input channels of one tap), per CTA:
-//     x rows 128 x 32 fp32 (16 KB, 2-D TMA, SWIZZLE_128B)  -> 4 converter warps: *s, fp16 hi/lo, packed pairs -> TMEM (32 cols)
-//     weight rows [rank*nh/2, +nh/2) of both column halves, PRE-SPLIT fp16 hi and lo (4 x 5 KB, 2-D TMA, SWIZZLE_64B):
-//       the weights change once per step, so bm_f16_split prepares them once and no warp converts them here
-//     leader CTA, one elected lane: 12 x tcgen05.mma.cta_group::2.kind::f16 (M = 256, N = nh <= 160, K = 16; A from TMEM)
-//   TMEM: [0, 320) accumulator (two column halves of nh), [320 + 32 s, +32) x stage s (hi pairs | lo pairs).
+// The conv of tc_convp.cuh with the weights given as TWO FP16 PIECES of a power-of-two-scaled copy (w*s = hi + lo, 11 + 11
+// significant bits, s from the tensor's largest magnitude: bm_amax + bm_f16_split / bm_tc_weight_split_f16).  The pieces
+// are summed back on load (~22 significant bits, the pieces' precision) and the GEMM runs on the same 3xTF32 engine; x_amax is accepted for the ABI and
+// not needed.  The epilogue can also report max |output| (amax_out) for the conv that consumes the tensor next.
 #pragma once
 #include <cuda_fp16.h>
-#include <cstring>
 #include "tc_convp.cuh"
 
 namespace bm {
 namespace tc {
-
-constexpr int HP_BM = 128, HP_BK = 32, HP_STAGES = 5, HP_THREADS = 448;
-constexpr int HP_A_BYTES = HP_BM * HP_BK * 4;                        // 16 KB fp32
-constexpr int HP_BQ_BYTES = (PP_MAX_NH / 2) * HP_BK * 2;             // 5 KB: half of one column half, fp16
-constexpr int HP_STAGE_BYTES = HP_A_BYTES + 4 * HP_BQ_BYTES;         // 36 KB: x | hi h0 | hi h1 | lo h0 | lo h1
-constexpr int HP_SMEM_BYTES = HP_STAGES * HP_STAGE_BYTES + PP_EPI_WARPS * PP_EPI_BUF + PP_STATS_BYTES + 1024;
-constexpr int HP_ACC_COLS = 2 * PP_MAX_NH, HP_A_COLS = HP_BK;        // 16 packed hi columns + 16 packed lo columns
-constexpr int HP_TARGET_EXP = 14;                                    // scaled maximum in [2^14, 2^15)
-
-// K-major operand tile, rows of exactly 64 bytes (32 fp16), SWIZZLE_64B, 8-row atoms 512 B apart.
-__device__ __forceinline__ uint64_t umma_desc_k_sw64(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(512 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)4 << 61;                              // SWIZZLE_64B
-    return d;
-}
-// instruction descriptor: f16 x f16 -> f32, both operands K-major
-__host__ __device__ constexpr uint32_t umma_idesc_f16(int M, int N) {
-    return (1u << 4) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_f16_ts_2sm(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                                uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st32u(uint32_t taddr, const uint32_t* r) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-          "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]),
-          "r"(r[18]), "r"(r[19]), "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]),
-          "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]), "r"(r[31])
-        : "memory");
-}
-
-// The power of two that puts a tensor whose largest magnitude is `amax` into [2^14, 2^15); 1 for an all-zero / non-finite
-// tensor.  Identical on every thread that evaluates it (pure bit arithmetic).
-__host__ __device__ __forceinline__ float f16_scale_of(float amax) {
-#ifdef __CUDA_ARCH__
-    const uint32_t bits = __float_as_uint(amax);
-#else
-    uint32_t bits; memcpy(&bits, &amax, 4);
-#endif
-    const int e = (int)((bits >> 23) & 0xFF);
-    if (e == 0 || e == 255) return 1.0f;
-    int se = 127 + HP_TARGET_EXP - (e - 127);             // exponent field of the scale
-    se = se < 1 ? 1 : (se > 254 ? 254 : se);
-    const uint32_t sb = (uint32_t)se << 23;
-#ifdef __CUDA_ARCH__
-    return __uint_as_float(sb);
-#else
-    float s; memcpy(&s, &sb, 4); return s;
-#endif
-}
-// two scaled fp32 values -> packed fp16 pairs: hi = rn(v), lo = rn(v - hi); element k in the LOW half, k+1 in the high half
-__device__ __forceinline__ void f16_split2(float a, float b, uint32_t& hi, uint32_t& lo) {
-    const __half2 h = __floats2half2_rn(a, b);
-    const float2 hf = __half22float2(h);
-    const __half2 l = __floats2half2_rn(a - hf.x, b - hf.y);
-    hi = *reinterpret_cast<const uint32_t*>(&h);
-    lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-
-struct ConvHP {
-    ConvPP c;                   // geometry, epilogue mode and outputs as in conv_pp_kernel
-    const float* x_amax;        // device scalars: largest |x|, largest |w| (what bm_amax wrote)
-    const float* w_amax;
-    unsigned int* out_amax;     // nullable: max |glu_out| (mode 3) / max |y| (mode 2) for the conv that consumes it next
-    int comp_off;               // debug: leave the accumulator's truncation gain uncorrected (profiles/accumulator_gain_probe.py)
-};
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(HP_THREADS, 1)
-conv_hp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmBh,
-               const __grid_constant__ CUtensorMap tmBl, const __grid_constant__ CUtensorMap tmY,
-               const __grid_constant__ CUtensorMap tmO, const ConvHP hp) {
-    const ConvPP& p = hp.c;
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[HP_STAGES], conv_bar[HP_STAGES], empty_bar[HP_STAGES];
-    __shared__ __align__(8) uint64_t acc_full, acc_empty;
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ int prior_error;
-
-    if (threadIdx.x == 0) prior_error = p.err ? *reinterpret_cast<volatile int*>(p.err) : 0;
-    __syncthreads();
-    const bool skip = prior_error != 0;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
-    uint8_t* epi_smem = smem + HP_STAGES * HP_STAGE_BYTES;
-    double* stats_smem = reinterpret_cast<double*>(epi_smem + PP_EPI_WARPS * PP_EPI_BUF);
-
-    const int npairs = gridDim.x >> 1, pair = blockIdx.x >> 1;
-    const int ntiles = skip ? 0 : p.mtiles * p.ntn;
-    const int kchunks = p.Cin / HP_BK;
-    const int per_tile = p.taps * kchunks;
-    const int nh = p.nh, nq = nh / 2;
-    const int H = p.Ntot / 2;
-    const bool glu = p.mode == 3;
-    const uint32_t bq_bytes = (uint32_t)(nq * HP_BK * 2);
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < HP_STAGES; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&conv_bar[s], 2 * 4);                     // one elected lane per converter warp of both CTAs (LEADER's copy)
-            mbar_init(&empty_bar[s], 1);
-        }
-        mbar_init(&acc_full, 1);
-        mbar_init(&acc_empty, 2 * PP_EPI_WARPS);
-        fence_barrier_init();
-    }
-    if (p.stats)
-        for (int i = threadIdx.x; i < 4 * PP_MAX_NH; i += HP_THREADS) stats_smem[i] = 0.0;
-    if (warp == 1) tmem_alloc_2sm<512>(&tmem_base_smem);
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_smem;
-
-    if (warp == 0) {
-        // ------------------------------------------------ TMA producer ------------------------------------------------
-        if (lane == 0) {
-            prefetch_tmap(&tmA);
-            prefetch_tmap(&tmBh);
-            prefetch_tmap(&tmBl);
-            int git = 0;
-            bool ok = true;
-            for (int tile = pair; tile < ntiles && ok; tile += npairs) {
-                const int n_tile = tile % p.ntn, m_tile = tile / p.ntn;
-                const int row0 = m_tile * 2 * HP_BM + (int)rank * HP_BM;
-                const int rowbase0 = (glu ? n_tile * nh : n_tile * 2 * nh) + (int)rank * nq;
-                const int rowbase1 = (glu ? H + n_tile * nh : n_tile * 2 * nh + nh) + (int)rank * nq;
-                for (int it = 0; it < per_tile; ++it, ++git) {
-                    const int s = git % HP_STAGES;
-                    const uint32_t ph = (git / HP_STAGES) & 1;
-                    ok = mbar_wait(&empty_bar[s], ph ^ 1, p.err, 91);
-                    if (!ok) break;
-                    const int tap = it / kchunks, k0 = (it - tap * kchunks) * HP_BK;
-                    const int shift = p.sign * (tap - p.taps / 2) * p.dilation;
-                    uint8_t* st = smem + s * HP_STAGE_BYTES;
-                    mbar_expect_tx(&full_bar[s], HP_A_BYTES + 4 * bq_bytes);
-                    tma_load_2d(st, &tmA, &full_bar[s], k0, row0 + shift);
-                    uint8_t* b = st + HP_A_BYTES;
-                    tma_load_2d(b, &tmBh, &full_bar[s], k0, tap * p.Ntot + rowbase0);
-                    tma_load_2d(b + HP_BQ_BYTES, &tmBh, &full_bar[s], k0, tap * p.Ntot + rowbase1);
-                    tma_load_2d(b + 2 * HP_BQ_BYTES, &tmBl, &full_bar[s], k0, tap * p.Ntot + rowbase0);
-                    tma_load_2d(b + 3 * HP_BQ_BYTES, &tmBl, &full_bar[s], k0, tap * p.Ntot + rowbase1);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------ MMA issuer (leader): whole warp in the loop, one elected lane issues
-        if (leader) {
-            const uint32_t idesc = umma_idesc_f16(2 * HP_BM, nh);
-            int git = 0, tcount = 0;
-            bool ok = true;
-            for (int tile = pair; tile < ntiles && ok; tile += npairs, ++tcount) {
-                if (tcount > 0) {                                // the previous tile's accumulator has been read out
-                    ok = mbar_wait(&acc_empty, (uint32_t)(tcount - 1) & 1, p.err, 92);
-                    ok = __all_sync(0xffffffffu, ok);
-                    if (!ok) break;
-                    tc_fence_after();
-                }
-                for (int it = 0; it < per_tile; ++it, ++git) {
-                    const int s = git % HP_STAGES;
-                    const uint32_t ph = (git / HP_STAGES) & 1;
-                    ok = mbar_wait(&conv_bar[s], ph, p.err, 93);
-                    ok = __all_sync(0xffffffffu, ok);
-                    if (!ok) break;
-                    tc_fence_after();
-                    if (elect_one()) {
-                        const uint32_t bq = smem_base + s * HP_STAGE_BYTES + HP_A_BYTES;
-                        const uint32_t a_hi = tmem + HP_ACC_COLS + s * HP_A_COLS, a_lo = a_hi + HP_BK / 2;
-#pragma unroll
-                        for (int kk = 0; kk < HP_BK / 16; ++kk) {
-#pragma unroll
-                            for (int half = 0; half < 2; ++half) {
-                                const uint64_t dbh = umma_desc_k_sw64(bq + half * HP_BQ_BYTES + kk * 32);
-                                const uint64_t dbl = umma_desc_k_sw64(bq + (2 + half) * HP_BQ_BYTES + kk * 32);
-                                const uint32_t d = tmem + half * nh;
-                                umma_f16_ts_2sm(d, a_lo + kk * 8, dbh, idesc, (it | kk) != 0);
-                                umma_f16_ts_2sm(d, a_hi + kk * 8, dbl, idesc, 1);
-                                umma_f16_ts_2sm(d, a_hi + kk * 8, dbh, idesc, 1);
-                            }
-                        }
-                        umma_commit_2sm(&empty_bar[s]);
-                        if (it + 1 == per_tile) umma_commit_2sm(&acc_full);
-                    }
-                    __syncwarp();
-                }
-            }
-        }
-    } else if (warp < 6) {
-        // ------------------------------------------------ x rows * s -> TMEM (fp16 hi pairs | lo pairs); sample edges = 0 ---
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16);
-        const float sx = f16_scale_of(__ldg(hp.x_amax));
-        int git = 0;
-        bool ok = true;
-        for (int tile = pair; tile < ntiles && ok; tile += npairs) {
-            const int m_tile = tile / p.ntn;
-            const int prow = m_tile * 2 * HP_BM + (int)rank * HP_BM + row;      // flattened row b*T + t
-            const int t = prow % p.T;
-            for (int it = 0; it < per_tile && ok; ++it, ++git) {
-                const int s = git % HP_STAGES;
-                const uint32_t ph = (git / HP_STAGES) & 1;
-                const int tap = it / kchunks;
-                const int ts = t + p.sign * (tap - p.taps / 2) * p.dilation;
-                const float m = (ts >= 0 && ts < p.T) ? sx : 0.f;       // else: the conv's zero padding
-                ok = mbar_wait(&full_bar[s], ph, p.err, 94);
-                const uint8_t* arow = smem + s * HP_STAGE_BYTES + row * 128;
-                uint32_t r[HP_BK];                                       // [0,16) hi pairs, [16,32) lo pairs
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    const float4 v = *reinterpret_cast<const float4*>(arow + ((c ^ (row & 7)) << 4));
-                    f16_split2(v.x * m, v.y * m, r[2 * c], r[16 + 2 * c]);
-                    f16_split2(v.z * m, v.w * m, r[2 * c + 1], r[16 + 2 * c + 1]);
-                }
-                tmem_st32u(tq + HP_ACC_COLS + s * HP_A_COLS, r);
-                tmem_st_wait();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&conv_bar[s]), 0));
-            }
-        }
-    } else {
-        // ------------------------------------------------ epilogue: two warps per TMEM lane quarter ---------------------
-        const int ew = warp - 6;                                     // 0..7
-        const int q = warp & 3, cset = ew >> 2;
-        const int row = q * 32 + lane;
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16);
-        uint8_t* buf = epi_smem + ew * PP_EPI_BUF;
-        if (lane == 0) { prefetch_tmap(&tmY); prefetch_tmap(&tmO); }
-        // undo the operand scales (exact powers of two) and the accumulator's truncation gain in one factor
-        const float comp = (hp.comp_off ? 1.0f : acc_trunc_comp(per_tile * (HP_BK / 16) * 3)) *
-                           (1.0f / f16_scale_of(__ldg(hp.x_amax))) * (1.0f / f16_scale_of(__ldg(hp.w_amax)));
-        int tcount = 0;
-        bool ok = true;
-        float am = 0.f;                                               // max |output| this thread has produced
-        for (int tile = pair; tile < ntiles && ok; tile += npairs, ++tcount) {
-            const int n_tile = tile % p.ntn, m_tile = tile / p.ntn;
-            const int row0 = m_tile * 2 * HP_BM + (int)rank * HP_BM;  // this CTA's first row
-            const int r32 = row0 + q * 32;                            // this warp's first row
-            const bool row_live = row0 + row < p.R;                   // rows past the end are computed from zero-filled x
-            ok = mbar_wait(&acc_full, (uint32_t)tcount & 1, p.err, 96);
-            tc_fence_after();
-            if (glu) {
-                const int nch = nh / 32;
-                const int ch_begin = cset == 0 ? 0 : (nch + 1) / 2, ch_end = cset == 0 ? (nch + 1) / 2 : nch;
-                const int c0 = n_tile * nh;
-#pragma unroll 1
-                for (int c = ch_begin; c < ch_end; ++c) {
-                    float a[32], g[32];
-                    tmem_ld32(tq + c * 32, a);
-                    tmem_ld32(tq + nh + c * 32, g);
-                    if (c + 1 == ch_end) {                            // last TMEM read of this thread: release the accumulator
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&acc_empty), 0));
-                    }
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) { a[j] *= comp; g[j] *= comp; }
-                    if (p.bias) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            const float4 ba = *reinterpret_cast<const float4*>(p.bias + c0 + c * 32 + j);
-                            const float4 bg = *reinterpret_cast<const float4*>(p.bias + H + c0 + c * 32 + j);
-                            a[j] += ba.x; a[j + 1] += ba.y; a[j + 2] += ba.z; a[j + 3] += ba.w;
-                            g[j] += bg.x; g[j + 1] += bg.y; g[j + 2] += bg.z; g[j + 3] += bg.w;
-                        }
-                    }
-                    if (p.save_h) {
-                        pp_stage_store(buf, a, lane, &tmY, c0 + c * 32, r32, false);
-                        pp_stage_store(buf, g, lane, &tmY, H + c0 + c * 32, r32, false);
-                    }
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) a[j] *= sigmoid_f(g[j]);
-                    if (hp.out_amax && row_live) {
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) am = fmaxf(am, fabsf(a[j]));
-                    }
-                    pp_stage_store(buf, a, lane, &tmO, c0 + c * 32, r32, false);
-                }
-            } else {
-                const int ncol0 = cset * nh;
-                const int n0 = n_tile * 2 * nh + ncol0;
-                const int nch = nh / 32;
-                const int prow = row0 + row;
-#pragma unroll 1
-                for (int c = 0; c < nch; ++c) {
-                    float v[32];
-                    tmem_ld32(tq + ncol0 + c * 32, v);
-                    if (c + 1 == nch) {
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&acc_empty), 0));
-                    }
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] *= comp;
-                    if (p.bias) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            const float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + c * 32 + j);
-                            v[j] += bb.x; v[j + 1] += bb.y; v[j + 2] += bb.z; v[j + 3] += bb.w;
-                        }
-                    }
-                    if (p.mode == 4) {
-                        if (prow < p.R) {
-                            const int b = prow / p.T, t = prow - b * p.T;
-                            float* yt = p.y + ((long long)b * p.Ntot + n0 + c * 32) * p.T + t;
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) yt[(long long)j * p.T] = v[j];
-                        }
-                        continue;
-                    }
-                    if (p.mode == 2) {
-                        if (p.save_aux) pp_stage_store(buf, v, lane, &tmO, n0 + c * 32, r32, false);
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) v[j] = gelu_f(v[j]);
-                        if (hp.out_amax && row_live) {
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) am = fmaxf(am, fabsf(v[j]));
-                        }
-                    }
-                    pp_stage_store(buf, v, lane, &tmY, n0 + c * 32, r32, p.mode == 1);
-                    if (p.stats) {
-                        const int nrows = min(32, p.R - r32);
-                        float s1 = 0.f, s2 = 0.f;
-                        for (int r = 0; r < nrows; ++r) {
-                            const float x = *reinterpret_cast<const float*>(buf + r * 128 + (((lane >> 2) ^ (r & 7)) << 4) +
-                                                                              (lane & 3) * 4);
-                            s1 += x;
-                            s2 = fmaf(x, x, s2);
-                        }
-                        if (nrows > 0) {
-                            atomicAdd(stats_smem + ncol0 + c * 32 + lane, (double)s1);
-                            atomicAdd(stats_smem + 2 * PP_MAX_NH + ncol0 + c * 32 + lane, (double)s2);
-                        }
-                    }
-                }
-            }
-        }
-        if (hp.out_amax) {
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, o));
-            if (lane == 0 && am > 0.f) atomicMax(hp.out_amax, __float_as_uint(am));
-        }
-        if (lane == 0) bulk_wait<0>();
-        __syncwarp();
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (p.stats && !skip) {
-        for (int i = threadIdx.x; i < 2 * nh; i += HP_THREADS) {
-            const double s1 = stats_smem[i], s2 = stats_smem[2 * PP_MAX_NH + i];
-            if (s1 != 0.0 || s2 != 0.0) {
-                atomicAdd(p.stats + i, s1);
-                atomicAdd(p.stats + p.Ntot + i, s2);
-            }
-        }
-    }
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_2sm<512>(tmem);
-    }
-}
 
 // ---- operand preparation ---------------------------------------------------------------------------------------------
 // largest |x| of a tensor into `cell` (a float whose bits compare like an unsigned integer because it is non-negative);
@@ -465,18 +68,6 @@ __global__ void __launch_bounds__(256) weight_split_f16_kernel(const float* __re
     }
 }
 
-inline bool make_tmap_f16(CUtensorMap* m, const void* base, const uint64_t* dims, const uint64_t* strides_b,
-                          const uint32_t* box, CUtensorMapSwizzle swizzle) {
-    PFN_bm_encodeTiled enc = get_encode_tiled();
-    if (!enc) return false;
-    cuuint64_t gd[2] = {dims[0], dims[1]}, gs[1] = {strides_b[0]};
-    cuuint32_t bx[2] = {box[0], box[1]}, es[2] = {1, 1};
-    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), gd, gs, bx, es,
-                     CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS;
-}
-
 struct ConvHPArgs {
     ConvPPArgs c;                    // c.w_raw unused
     const float* x_amax; const void* w_hi; const void* w_lo; const float* w_amax;
@@ -485,73 +76,19 @@ struct ConvHPArgs {
 
 inline int launch_conv_hp(const ConvHPArgs& h, cudaStream_t st) {
     const ConvPPArgs& a = h.c;
-    ConvHP hp;
-    ConvPP& p = hp.c;
-    p.R = a.B * a.T; p.T = a.T; p.Cin = a.Cin; p.Ntot = a.Ntot; p.taps = a.taps; p.dilation = a.dilation; p.sign = a.sign;
-    p.nh = conv_pp_pick_nh(a.Ntot, a.glu);
-    if (p.nh == 0 || p.nh % 32 != 0) return set_error(2, "%s: unsupported N%s", __func__);
-    if ((long long)a.B * a.T >= (1ll << 31)) return set_error(2, "%s: too many rows%s", __func__);
-    p.ntn = a.glu ? (a.Ntot / 2) / p.nh : a.Ntot / (2 * p.nh);
-    p.mtiles = (p.R + 2 * HP_BM - 1) / (2 * HP_BM);
-    p.bias = a.bias; p.y = a.y; p.stats = a.stats; p.err = a.err;
-    p.save_h = (a.glu && a.y) ? 1 : 0;
-    p.save_aux = (a.act && a.aux) ? 1 : 0;
-    if (a.glu) p.mode = 3;
-    else if (a.out_tmajor) p.mode = 4;
-    else if (a.act) p.mode = 2;
-    else if (a.accumulate) p.mode = 1;
-    else p.mode = 0;
-    if (a.stats && (p.mode != 0 || p.ntn != 1)) return set_error(2, "%s: statistics need a plain single-N-tile conv%s", __func__);
+    const int nh = conv_pp_pick_nh(a.Ntot, a.glu);
+    if (nh == 0 || nh % 32 != 0) return set_error(2, "%s: unsupported N%s", __func__);
+    const int ntn = a.glu ? (a.Ntot / 2) / nh : a.Ntot / (2 * nh);
+    if (a.stats && (a.glu || a.out_tmajor || a.act || a.accumulate || ntn != 1))
+        return set_error(2, "%s: statistics need a plain single-N-tile conv%s", __func__);
     if (a.glu && (a.act || a.out_tmajor || a.aux || a.accumulate)) return set_error(2, "%s: GLU excludes the other epilogues%s", __func__);
     if (a.out_tmajor && (a.act || a.accumulate)) return set_error(2, "%s: channel-major output is a plain store%s", __func__);
     if (a.act && a.accumulate) return set_error(2, "%s: accumulate excludes the activation%s", __func__);
-    hp.x_amax = h.x_amax; hp.w_amax = h.w_amax; hp.out_amax = reinterpret_cast<unsigned int*>(h.out_amax);
-    hp.comp_off = (g_debug_flags & 2) ? 1 : 0;
-
-    CUtensorMap tmA, tmBh, tmBl, tmY, tmO;
-    {
-        uint64_t dims[2] = {(uint64_t)a.Cin, (uint64_t)p.R};
-        uint64_t str[1] = {(uint64_t)a.Cin * 4};
-        uint32_t box[2] = {HP_BK, HP_BM};
-        if (!make_tmap_f32(&tmA, a.x, 2, dims, str, box)) return set_error(4, "%s: cuTensorMapEncodeTiled(A) failed%s", __func__);
-    }
-    {
-        uint64_t dims[2] = {(uint64_t)a.Cin, (uint64_t)a.taps * a.Ntot};
-        uint64_t str[1] = {(uint64_t)a.Cin * 2};
-        uint32_t box[2] = {HP_BK, (uint32_t)(p.nh / 2)};
-        if (!make_tmap_f16(&tmBh, h.w_hi, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B) ||
-            !make_tmap_f16(&tmBl, h.w_lo, dims, str, box, CU_TENSOR_MAP_SWIZZLE_64B))
-            return set_error(4, "%s: cuTensorMapEncodeTiled(B) failed%s", __func__);
-    }
-    auto out_map = [&](CUtensorMap* m, const float* base, int width) {
-        uint64_t dims[2] = {(uint64_t)width, (uint64_t)p.R};
-        uint64_t str[1] = {(uint64_t)width * 4};
-        uint32_t box[2] = {32, 32};
-        return make_tmap_f32(m, base, 2, dims, str, box);
-    };
-    bool okm = true;
-    if (p.mode == 3) {
-        okm = out_map(&tmO, a.glu_out, a.Ntot / 2) && (a.y ? out_map(&tmY, a.y, a.Ntot) : out_map(&tmY, a.x, a.Cin));
-    } else if (p.mode == 4) {
-        okm = out_map(&tmY, a.x, a.Cin);
-        tmO = tmY;
-    } else {
-        okm = out_map(&tmY, a.y, a.Ntot) && (p.save_aux ? out_map(&tmO, a.aux, a.Ntot) : out_map(&tmO, a.x, a.Cin));
-    }
-    if (!okm) return set_error(4, "%s: cuTensorMapEncodeTiled(out) failed%s", __func__);
-    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(conv_hp_kernel), HP_SMEM_BYTES)) return rc;
-    if (a.stats) {
-        cudaError_t em = cudaMemsetAsync(a.stats, 0, sizeof(double) * 2 * a.Ntot, st);
-        if (em != cudaSuccess) return set_error(3, "%s: memset: %s", __func__, cudaGetErrorString(em));
-    }
-    int pairs = num_sms() / 2;
-    const int tiles = p.mtiles * p.ntn;
-    if (pairs > tiles) pairs = tiles;
-    conv_hp_kernel<<<2 * pairs, HP_THREADS, HP_SMEM_BYTES, st>>>(tmA, tmBh, tmBl, tmY, tmO, hp);
-    ++g_launches;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", __func__, cudaGetErrorString(e));
-    return 0;
+    ConvOp o = conv_pp_op(a);
+    o.w = nullptr;
+    o.w_hi = reinterpret_cast<const __half*>(h.w_hi); o.w_lo = reinterpret_cast<const __half*>(h.w_lo); o.w_amax = h.w_amax;
+    o.out_amax = reinterpret_cast<unsigned int*>(h.out_amax);
+    return launch_conv_op(o, st, __func__);
 }
 
 inline int launch_amax(const float* x, long long n, float* cell, cudaStream_t st) {

@@ -1,396 +1,17 @@
-// K3/K4/K5 (dilated Conv1d / Conv1d+GLU / head 1x1, forward and data gradient): PERSISTENT CTA pairs on tcgen05.
+// K3/K4/K5 (dilated Conv1d / Conv1d+GLU / head 1x1, forward and data gradient) with the RAW fp32 weights re-laid K-major
+// [Kw][Ntot][Cin] (bm_tc_weight_split with NULL lo pointers): the ConvOp GEMM of tc_conv.cuh, splitting both operands into
+// tf32 pieces on their way into shared memory.
 //
 //   y[p, n] = bias[n] + sum_tap sum_k x[p + shift(tap), k] * W[tap][n][k]        p = b*T + t (channels-last rows)
 //
-// What round 1's pair kernel (one CTA pair per tile; removed) lost, and what changes here:
-//   * one CTA pair per 256-row tile, 384 tiles on 74 SM pairs = 5.19 waves (13 % idle) and every tile paid the launch,
-//     TMEM allocation, pipeline fill and a fully exposed epilogue        -> the grid is ONE CTA pair per SM pair; each loops
-//     over its tiles with the pipeline (TMA producer, converters) running ahead across tile boundaries, and dedicated
-//     epilogue warps drain the accumulator while the next tile's operands are already staged; the MMA thread only waits
-//     for the drain's TMEM reads (the stores go through a staging buffer + TMA afterwards);
-//   * tiles were per sample (T = 360 -> 3 x 128 rows, the last 81 % full) -> tiles cover the FLATTENED rows b*T + t
-//     (92 160 rows = exactly 360 tiles at B = 256); a tap shift that would read across a sample boundary is the conv's
-//     zero padding: the converter thread that owns the row writes zeros to tensor memory instead;
-//   * the weights came pre-split as tf32 hi and lo copies (2 x 20 KB per K chunk per CTA from L2; the kernel asked 68 % of
-//     the L2 slice throughput)                                          -> ONE raw fp32 copy is loaded; the tensor core's own
-//     truncation of the raw operand IS the `hi`, and two warps write lo = w - trunc(w) beside it in shared memory;
-//   * BatchNorm statistics cost 2 560 fp64 global atomics per tile       -> accumulated in shared memory across the CTA's
-//     tiles, flushed once per CTA.
-//
-//   per K chunk (32 input channels of one tap), per CTA:
-//     x rows 128 x 32 (16 KB, 2-D TMA, negative / past-the-end rows zero-filled) -> 4 converter warps: tf32 hi/lo -> TMEM
-//     weight rows [rank*nh/2, +nh/2) of both column halves, raw (2 x 10 KB) -> 2 warps write the lo copy (2 x 10 KB)
-//     leader CTA, one thread: 24 x tcgen05.mma.cta_group::2.kind::tf32 (M = 256, N = nh <= 160, K = 8; A from TMEM)
-//   TMEM: [0, 320) accumulator (two column halves of nh), [320 + 64 s, +64) x stage s (hi | lo).
-//   Accumulation chain per tile: taps * Cin/8 * 3 MMAs (360 at K = 960): the accumulator's truncation stays < 1e-5.
+// Epilogue modes: store y | y += conv (accumulate, in place) | aux = pre-activation (nullable), y = GELU |
+// GLU: y = h (nullable), glu_out = a * sigmoid(gate) | y channel-major [B][Ntot][T]; BatchNorm statistics of y (plain store).
 #pragma once
+#include "tc_conv.cuh"
 #include "tc_pair.cuh"
 
 namespace bm {
 namespace tc {
-
-constexpr int PP_BM = 128, PP_BK = 32, PP_STAGES = 3, PP_THREADS = 512;
-constexpr int PP_MAX_NH = 160;
-constexpr int PP_A_BYTES = PP_BM * PP_BK * 4;                        // 16 KB
-constexpr int PP_BQ_BYTES = (PP_MAX_NH / 2) * PP_BK * 4;             // 10 KB: half of one column half
-constexpr int PP_STAGE_BYTES = PP_A_BYTES + 4 * PP_BQ_BYTES;         // 56 KB: x | raw h0 | raw h1 | lo h0 | lo h1
-constexpr int PP_EPI_WARPS = 8, PP_EPI_BUF = 4096;
-constexpr int PP_STATS_BYTES = 2 * 2 * PP_MAX_NH * 8;                // fp64 sum / sum of squares of 320 columns
-constexpr int PP_SMEM_BYTES = PP_STAGES * PP_STAGE_BYTES + PP_EPI_WARPS * PP_EPI_BUF + PP_STATS_BYTES + 1024;
-constexpr int PP_ACC_COLS = 2 * PP_MAX_NH, PP_A_COLS = 2 * PP_BK;
-
-struct ConvPP {
-    int R, T, Cin, Ntot;        // R = B*T rows
-    int taps, dilation, sign;
-    int mode;                   // 0 store y | 1 y += tile (TMA reduce-add) | 2 aux = pre-activation (nullable), y = GELU
-                                // 3 GLU: y = h (nullable), glu_out = a * sigmoid(g) | 4 y channel-major [B][Ntot][T]
-    int nh, ntn;                // column half (<= 160), N tiles
-    int mtiles;                 // 256-row tiles
-    const float* bias;
-    float* y;                   // mode 4 only (the other modes store through tensor maps)
-    double* stats;              // mode 0: [2*Ntot] sum / sum of squares per output column (zeroed by the launcher) or null
-    int save_h;                 // mode 3: h wanted
-    int save_aux;               // mode 2: pre-activation wanted
-    int* err;
-};
-
-__device__ __forceinline__ void tma_store_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_2d(const CUtensorMap* m, const void* src, int c0, int c1) {
-    asm volatile("cp.reduce.async.bulk.tensor.2d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1) : "memory");
-}
-
-// one warp: 32 rows x 32 columns (thread = row, v = its 32 columns) -> 128B-swizzled staging block -> TMA store / reduce.
-// The block is the warp's only one: the previous store must have READ it before it is overwritten.
-__device__ __forceinline__ void pp_stage_store(uint8_t* buf, const float* v, int lane, const CUtensorMap* m, int col,
-                                               int row, bool reduce) {
-    if (lane == 0) bulk_wait_read<0>();
-    __syncwarp();
-#pragma unroll
-    for (int j = 0; j < 8; ++j)
-        *reinterpret_cast<float4*>(buf + lane * 128 + ((j ^ (lane & 7)) << 4)) =
-            make_float4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]);
-    fence_proxy_async();
-    __syncwarp();
-    if (lane == 0) {
-        if (reduce) tma_reduce_add_2d(m, buf, col, row);
-        else tma_store_2d(m, buf, col, row);
-        bulk_commit();
-    }
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(PP_THREADS, 1)
-conv_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-               const __grid_constant__ CUtensorMap tmY, const __grid_constant__ CUtensorMap tmO, const ConvPP p) {
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[PP_STAGES], conv_bar[PP_STAGES], empty_bar[PP_STAGES];
-    __shared__ __align__(8) uint64_t acc_full, acc_empty;
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ int prior_error;
-
-    if (threadIdx.x == 0) prior_error = p.err ? *reinterpret_cast<volatile int*>(p.err) : 0;
-    __syncthreads();
-    const bool skip = prior_error != 0;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
-    uint8_t* epi_smem = smem + PP_STAGES * PP_STAGE_BYTES;
-    double* stats_smem = reinterpret_cast<double*>(epi_smem + PP_EPI_WARPS * PP_EPI_BUF);
-
-    const int npairs = gridDim.x >> 1, pair = blockIdx.x >> 1;
-    const int ntiles = skip ? 0 : p.mtiles * p.ntn;
-    const int kchunks = p.Cin / PP_BK;
-    const int per_tile = p.taps * kchunks;
-    const int nh = p.nh, nq = nh / 2;
-    const int H = p.Ntot / 2;
-    const bool glu = p.mode == 3;
-    const uint32_t bq_bytes = (uint32_t)(nq * PP_BK * 4);
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < PP_STAGES; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&conv_bar[s], 2 * (4 + 2));               // one elected lane per converter warp of both CTAs (LEADER's copy)
-            mbar_init(&empty_bar[s], 1);
-        }
-        mbar_init(&acc_full, 1);
-        mbar_init(&acc_empty, 2 * PP_EPI_WARPS);                // one elected lane per epilogue warp of both CTAs
-        fence_barrier_init();
-    }
-    if (p.stats)
-        for (int i = threadIdx.x; i < 4 * PP_MAX_NH; i += PP_THREADS) stats_smem[i] = 0.0;
-    if (warp == 1) tmem_alloc_2sm<512>(&tmem_base_smem);
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_smem;
-
-    if (warp == 0) {
-        // ------------------------------------------------ TMA producer ------------------------------------------------
-        if (lane == 0) {
-            prefetch_tmap(&tmA);
-            prefetch_tmap(&tmB);
-            int git = 0;
-            bool ok = true;
-            for (int tile = pair; tile < ntiles && ok; tile += npairs) {
-                const int n_tile = tile % p.ntn, m_tile = tile / p.ntn;
-                const int row0 = m_tile * 2 * PP_BM + (int)rank * PP_BM;
-                const int rowbase0 = (glu ? n_tile * nh : n_tile * 2 * nh) + (int)rank * nq;
-                const int rowbase1 = (glu ? H + n_tile * nh : n_tile * 2 * nh + nh) + (int)rank * nq;
-                for (int it = 0; it < per_tile; ++it, ++git) {
-                    const int s = git % PP_STAGES;
-                    const uint32_t ph = (git / PP_STAGES) & 1;
-                    ok = mbar_wait(&empty_bar[s], ph ^ 1, p.err, 71);
-                    if (!ok) break;
-                    const int tap = it / kchunks, k0 = (it - tap * kchunks) * PP_BK;
-                    const int shift = p.sign * (tap - p.taps / 2) * p.dilation;
-                    uint8_t* st = smem + s * PP_STAGE_BYTES;
-                    mbar_expect_tx(&full_bar[s], PP_A_BYTES + 2 * bq_bytes);
-                    tma_load_2d(st, &tmA, &full_bar[s], k0, row0 + shift);
-                    tma_load_2d(st + PP_A_BYTES, &tmB, &full_bar[s], k0, tap * p.Ntot + rowbase0);
-                    tma_load_2d(st + PP_A_BYTES + PP_BQ_BYTES, &tmB, &full_bar[s], k0, tap * p.Ntot + rowbase1);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------ MMA issuer (leader) -----------------------------------------
-        if (leader && lane == 0) {
-            const uint32_t idesc = umma_idesc_tf32(2 * PP_BM, nh);
-            int git = 0, tcount = 0;
-            bool ok = true;
-            for (int tile = pair; tile < ntiles && ok; tile += npairs, ++tcount) {
-                if (tcount > 0) {                                // the previous tile's accumulator has been read out
-                    ok = mbar_wait(&acc_empty, (uint32_t)(tcount - 1) & 1, p.err, 72);
-                    if (!ok) break;
-                    tc_fence_after();
-                }
-                for (int it = 0; it < per_tile; ++it, ++git) {
-                    const int s = git % PP_STAGES;
-                    const uint32_t ph = (git / PP_STAGES) & 1;
-                    ok = mbar_wait(&conv_bar[s], ph, p.err, 73);
-                    if (!ok) break;
-                    tc_fence_after();
-                    const uint32_t bq = smem_base + s * PP_STAGE_BYTES + PP_A_BYTES;
-                    const uint32_t a_hi = tmem + PP_ACC_COLS + s * PP_A_COLS, a_lo = a_hi + PP_BK;
-#pragma unroll
-                    for (int kk = 0; kk < PP_BK / 8; ++kk) {
-#pragma unroll
-                        for (int half = 0; half < 2; ++half) {
-                            const uint64_t dbh = umma_desc_k_sw128(bq + half * PP_BQ_BYTES + kk * 32);
-                            const uint64_t dbl = umma_desc_k_sw128(bq + (2 + half) * PP_BQ_BYTES + kk * 32);
-                            const uint32_t d = tmem + half * nh;
-                            umma_tf32_ts_2sm(d, a_lo + kk * 8, dbh, idesc, (it | kk) != 0);
-                            umma_tf32_ts_2sm(d, a_hi + kk * 8, dbl, idesc, 1);
-                            umma_tf32_ts_2sm(d, a_hi + kk * 8, dbh, idesc, 1);
-                        }
-                    }
-                    umma_commit_2sm(&empty_bar[s]);
-                }
-                if (ok) umma_commit_2sm(&acc_full);
-            }
-        }
-    } else if (warp < 6) {
-        // ------------------------------------------------ x rows -> TMEM (hi | lo); rows across a sample edge = 0 -------
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16);
-        int git = 0;
-        bool ok = true;
-        for (int tile = pair; tile < ntiles && ok; tile += npairs) {
-            const int m_tile = tile / p.ntn;
-            const int prow = m_tile * 2 * PP_BM + (int)rank * PP_BM + row;      // flattened row b*T + t
-            const int t = prow % p.T;
-            for (int it = 0; it < per_tile && ok; ++it, ++git) {
-                const int s = git % PP_STAGES;
-                const uint32_t ph = (git / PP_STAGES) & 1;
-                const int tap = it / kchunks;
-                const int ts = t + p.sign * (tap - p.taps / 2) * p.dilation;
-                const bool inside = ts >= 0 && ts < p.T;            // else: the conv's zero padding
-                ok = mbar_wait(&full_bar[s], ph, p.err, 74);
-                const uint8_t* arow = smem + s * PP_STAGE_BYTES + row * 128;
-                float hi[PP_BK], lo[PP_BK];
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    float4 v = *reinterpret_cast<const float4*>(arow + ((c ^ (row & 7)) << 4));
-                    if (!inside) v = make_float4(0.f, 0.f, 0.f, 0.f);
-                    tf32_split(v.x, hi[4 * c + 0], lo[4 * c + 0]); tf32_split(v.y, hi[4 * c + 1], lo[4 * c + 1]);
-                    tf32_split(v.z, hi[4 * c + 2], lo[4 * c + 2]); tf32_split(v.w, hi[4 * c + 3], lo[4 * c + 3]);
-                }
-                tmem_st32(tq + PP_ACC_COLS + s * PP_A_COLS, hi);
-                tmem_st32(tq + PP_ACC_COLS + s * PP_A_COLS + PP_BK, lo);
-                tmem_st_wait();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&conv_bar[s]), 0));
-            }
-        }
-    } else if (warp < 8) {
-        // ------------------------------------------------ weights: lo = w - trunc_tf32(w) ------------------------------
-        const int ct = (warp - 6) * 32 + lane;                       // 0..63
-        const int nvec = (int)(bq_bytes / 16);                       // float4 per quarter tile
-        int git = 0;
-        bool ok = true;
-        for (int tile = pair; tile < ntiles && ok; tile += npairs) {
-            for (int it = 0; it < per_tile && ok; ++it, ++git) {
-                const int s = git % PP_STAGES;
-                const uint32_t ph = (git / PP_STAGES) & 1;
-                ok = mbar_wait(&full_bar[s], ph, p.err, 75);
-                uint8_t* st = smem + s * PP_STAGE_BYTES + PP_A_BYTES;
-#pragma unroll
-                for (int half = 0; half < 2; ++half) {
-                    const float4* bh = reinterpret_cast<const float4*>(st + half * PP_BQ_BYTES);
-                    float4* bl = reinterpret_cast<float4*>(st + (2 + half) * PP_BQ_BYTES);
-#pragma unroll 5
-                    for (int idx = ct; idx < nvec; idx += 64) {
-                        const float4 v = bh[idx];
-                        float4 l;
-                        l.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-                        l.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-                        l.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-                        l.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-                        bl[idx] = l;
-                    }
-                }
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&conv_bar[s]), 0));
-            }
-        }
-    } else {
-        // ------------------------------------------------ epilogue: two warps per TMEM lane quarter ---------------------
-        const int ew = warp - 8;                                     // 0..7
-        const int q = warp & 3, cset = ew >> 2;
-        const int row = q * 32 + lane;
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16);
-        uint8_t* buf = epi_smem + ew * PP_EPI_BUF;
-        if (lane == 0) { prefetch_tmap(&tmY); prefetch_tmap(&tmO); }
-        const float comp = acc_trunc_comp(per_tile * (PP_BK / 8) * 3);       // additions chained into this accumulator
-        int tcount = 0;
-        bool ok = true;
-        for (int tile = pair; tile < ntiles && ok; tile += npairs, ++tcount) {
-            const int n_tile = tile % p.ntn, m_tile = tile / p.ntn;
-            const int row0 = m_tile * 2 * PP_BM + (int)rank * PP_BM;  // this CTA's first row
-            const int r32 = row0 + q * 32;                            // this warp's first row
-            ok = mbar_wait(&acc_full, (uint32_t)tcount & 1, p.err, 76);
-            tc_fence_after();
-            if (glu) {
-                // column chunk c: a = acc[c*32 ..], gate = acc[nh + c*32 ..]; h (when saved) and out through the staging block
-                const int nch = nh / 32;
-                const int ch_begin = cset == 0 ? 0 : (nch + 1) / 2, ch_end = cset == 0 ? (nch + 1) / 2 : nch;
-                const int c0 = n_tile * nh;
-#pragma unroll 1
-                for (int c = ch_begin; c < ch_end; ++c) {
-                    float a[32], g[32];
-                    tmem_ld32(tq + c * 32, a);
-                    tmem_ld32(tq + nh + c * 32, g);
-                    if (c + 1 == ch_end) {                            // last TMEM read of this thread: release the accumulator
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&acc_empty), 0));
-                    }
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) { a[j] *= comp; g[j] *= comp; }
-                    if (p.bias) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            const float4 ba = *reinterpret_cast<const float4*>(p.bias + c0 + c * 32 + j);
-                            const float4 bg = *reinterpret_cast<const float4*>(p.bias + H + c0 + c * 32 + j);
-                            a[j] += ba.x; a[j + 1] += ba.y; a[j + 2] += ba.z; a[j + 3] += ba.w;
-                            g[j] += bg.x; g[j + 1] += bg.y; g[j + 2] += bg.z; g[j + 3] += bg.w;
-                        }
-                    }
-                    if (p.save_h) {
-                        pp_stage_store(buf, a, lane, &tmY, c0 + c * 32, r32, false);
-                        pp_stage_store(buf, g, lane, &tmY, H + c0 + c * 32, r32, false);
-                    }
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) a[j] *= sigmoid_f(g[j]);
-                    pp_stage_store(buf, a, lane, &tmO, c0 + c * 32, r32, false);
-                }
-            } else {
-                const int ncol0 = cset * nh;
-                const int n0 = n_tile * 2 * nh + ncol0;
-                const int nch = nh / 32;
-                const int prow = row0 + row;
-#pragma unroll 1
-                for (int c = 0; c < nch; ++c) {
-                    float v[32];
-                    tmem_ld32(tq + ncol0 + c * 32, v);
-                    if (c + 1 == nch) {
-                        tc_fence_before();
-                        __syncwarp();
-                        if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&acc_empty), 0));
-                    }
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] *= comp;
-                    if (p.bias) {
-#pragma unroll
-                        for (int j = 0; j < 32; j += 4) {
-                            const float4 bb = *reinterpret_cast<const float4*>(p.bias + n0 + c * 32 + j);
-                            v[j] += bb.x; v[j + 1] += bb.y; v[j + 2] += bb.z; v[j + 3] += bb.w;
-                        }
-                    }
-                    if (p.mode == 4) {
-                        // channel-major output y[b][n][t]: lanes are consecutive t, so each column is one coalesced row piece
-                        if (prow < p.R) {
-                            const int b = prow / p.T, t = prow - b * p.T;
-                            float* yt = p.y + ((long long)b * p.Ntot + n0 + c * 32) * p.T + t;
-#pragma unroll
-                            for (int j = 0; j < 32; ++j) yt[(long long)j * p.T] = v[j];
-                        }
-                        continue;
-                    }
-                    if (p.mode == 2) {
-                        if (p.save_aux) pp_stage_store(buf, v, lane, &tmO, n0 + c * 32, r32, false);
-#pragma unroll
-                        for (int j = 0; j < 32; ++j) v[j] = gelu_f(v[j]);
-                    }
-                    pp_stage_store(buf, v, lane, &tmY, n0 + c * 32, r32, p.mode == 1);
-                    if (p.stats) {
-                        // column sums of the staged 32x32 block (lane = column) into the CTA's shared accumulators
-                        const int nrows = min(32, p.R - r32);
-                        float s1 = 0.f, s2 = 0.f;
-                        for (int r = 0; r < nrows; ++r) {
-                            const float x = *reinterpret_cast<const float*>(buf + r * 128 + (((lane >> 2) ^ (r & 7)) << 4) +
-                                                                              (lane & 3) * 4);
-                            s1 += x;
-                            s2 = fmaf(x, x, s2);
-                        }
-                        if (nrows > 0) {
-                            atomicAdd(stats_smem + ncol0 + c * 32 + lane, (double)s1);
-                            atomicAdd(stats_smem + 2 * PP_MAX_NH + ncol0 + c * 32 + lane, (double)s2);
-                        }
-                    }
-                }
-            }
-        }
-        if (lane == 0) bulk_wait<0>();
-        __syncwarp();
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (p.stats && !skip) {
-        // ntn == 1 when statistics are requested (launcher), so shared column j is output column j
-        for (int i = threadIdx.x; i < 2 * nh; i += PP_THREADS) {
-            const double s1 = stats_smem[i], s2 = stats_smem[2 * PP_MAX_NH + i];
-            if (s1 != 0.0 || s2 != 0.0) {
-                atomicAdd(p.stats + i, s1);
-                atomicAdd(p.stats + p.Ntot + i, s2);
-            }
-        }
-    }
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_2sm<512>(tmem);
-    }
-}
 
 inline int conv_pp_pick_nh(int Ntot, int glu) { return pair_pick_nh(Ntot, glu); }
 inline bool conv_pp_supported(int T, int Cin, int Ntot, int Kw, int glu) { return pair_conv_supported(T, Cin, Ntot, Kw, glu); }
@@ -403,70 +24,26 @@ struct ConvPPArgs {
     float* y; float* aux; float* glu_out; double* stats; int* err;
 };
 
+inline ConvOp conv_pp_op(const ConvPPArgs& a) {
+    ConvOp o = conv_op_defaults();
+    o.x = a.x; o.w = a.w_raw; o.bias = a.bias; o.B = a.B; o.T = a.T; o.Cin = a.Cin; o.Ntot = a.Ntot; o.taps = a.taps;
+    o.dilation = a.dilation; o.sign = a.sign; o.glu = a.glu; o.act = a.act; o.out_tmajor = a.out_tmajor;
+    o.addend = a.accumulate ? a.y : nullptr; o.y = a.y; o.aux = a.act ? a.aux : nullptr; o.glu_out = a.glu_out;
+    o.stats = a.stats; o.err = a.err;
+    return o;
+}
+
 inline int launch_conv_pp(const ConvPPArgs& a, cudaStream_t st) {
-    ConvPP p;
-    p.R = a.B * a.T; p.T = a.T; p.Cin = a.Cin; p.Ntot = a.Ntot; p.taps = a.taps; p.dilation = a.dilation; p.sign = a.sign;
-    p.nh = conv_pp_pick_nh(a.Ntot, a.glu);
-    if (p.nh == 0 || p.nh % 32 != 0) return set_error(2, "%s: unsupported N%s", __func__);
-    if ((long long)a.B * a.T >= (1ll << 31)) return set_error(2, "%s: too many rows%s", __func__);
-    p.ntn = a.glu ? (a.Ntot / 2) / p.nh : a.Ntot / (2 * p.nh);
-    p.mtiles = (p.R + 2 * PP_BM - 1) / (2 * PP_BM);
-    p.bias = a.bias; p.y = a.y; p.stats = a.stats; p.err = a.err;
-    p.save_h = (a.glu && a.y) ? 1 : 0;
-    p.save_aux = (a.act && a.aux) ? 1 : 0;
-    if (a.glu) p.mode = 3;
-    else if (a.out_tmajor) p.mode = 4;
-    else if (a.act) p.mode = 2;
-    else if (a.accumulate) p.mode = 1;
-    else p.mode = 0;
-    if (a.stats && (p.mode != 0 || p.ntn != 1)) return set_error(2, "%s: statistics need a plain single-N-tile conv%s", __func__);
+    const int nh = conv_pp_pick_nh(a.Ntot, a.glu);
+    if (nh == 0 || nh % 32 != 0) return set_error(2, "%s: unsupported N%s", __func__);
+    const int ntn = a.glu ? (a.Ntot / 2) / nh : a.Ntot / (2 * nh);
+    if (a.stats && (a.glu || a.out_tmajor || a.act || a.accumulate || ntn != 1))
+        return set_error(2, "%s: statistics need a plain single-N-tile conv%s", __func__);
     if (a.glu && (a.act || a.out_tmajor || a.aux || a.accumulate)) return set_error(2, "%s: GLU excludes the other epilogues%s", __func__);
     if (a.out_tmajor && (a.act || a.accumulate)) return set_error(2, "%s: channel-major output is a plain store%s", __func__);
     if (a.act && a.accumulate) return set_error(2, "%s: accumulate excludes the activation%s", __func__);
 
-    CUtensorMap tmA, tmB, tmY, tmO;
-    {
-        uint64_t dims[2] = {(uint64_t)a.Cin, (uint64_t)p.R};
-        uint64_t str[1] = {(uint64_t)a.Cin * 4};
-        uint32_t box[2] = {PP_BK, PP_BM};
-        if (!make_tmap_f32(&tmA, a.x, 2, dims, str, box)) return set_error(4, "%s: cuTensorMapEncodeTiled(A) failed%s", __func__);
-    }
-    {
-        uint64_t dims[2] = {(uint64_t)a.Cin, (uint64_t)a.taps * a.Ntot};
-        uint64_t str[1] = {(uint64_t)a.Cin * 4};
-        uint32_t box[2] = {PP_BK, (uint32_t)(p.nh / 2)};
-        if (!make_tmap_f32(&tmB, a.w_raw, 2, dims, str, box)) return set_error(4, "%s: cuTensorMapEncodeTiled(B) failed%s", __func__);
-    }
-    auto out_map = [&](CUtensorMap* m, const float* base, int width) {
-        uint64_t dims[2] = {(uint64_t)width, (uint64_t)p.R};
-        uint64_t str[1] = {(uint64_t)width * 4};
-        uint32_t box[2] = {32, 32};
-        return make_tmap_f32(m, base, 2, dims, str, box);
-    };
-    // tmY: y (modes 0/1/2) or h (mode 3);  tmO: aux (mode 2) or glu_out (mode 3).  Unused maps point at x (never issued).
-    bool okm = true;
-    if (p.mode == 3) {
-        okm = out_map(&tmO, a.glu_out, a.Ntot / 2) && (a.y ? out_map(&tmY, a.y, a.Ntot) : out_map(&tmY, a.x, a.Cin));
-    } else if (p.mode == 4) {
-        okm = out_map(&tmY, a.x, a.Cin);
-        tmO = tmY;
-    } else {
-        okm = out_map(&tmY, a.y, a.Ntot) && (p.save_aux ? out_map(&tmO, a.aux, a.Ntot) : out_map(&tmO, a.x, a.Cin));
-    }
-    if (!okm) return set_error(4, "%s: cuTensorMapEncodeTiled(out) failed%s", __func__);
-    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(conv_pp_kernel), PP_SMEM_BYTES)) return rc;
-    if (a.stats) {
-        cudaError_t em = cudaMemsetAsync(a.stats, 0, sizeof(double) * 2 * a.Ntot, st);
-        if (em != cudaSuccess) return set_error(3, "%s: memset: %s", __func__, cudaGetErrorString(em));
-    }
-    int pairs = num_sms() / 2;
-    const int tiles = p.mtiles * p.ntn;
-    if (pairs > tiles) pairs = tiles;
-    conv_pp_kernel<<<2 * pairs, PP_THREADS, PP_SMEM_BYTES, st>>>(tmA, tmB, tmY, tmO, p);
-    ++g_launches;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", __func__, cudaGetErrorString(e));
-    return 0;
+    return launch_conv_op(conv_pp_op(a), st, __func__);
 }
 
 }  // namespace tc

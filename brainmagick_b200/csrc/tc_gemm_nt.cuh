@@ -1,238 +1,37 @@
-// ClipLoss backward contractions (bm/losses.py:91-114 differentiated, SURVEY.md A.6) on persistent CTA pairs:
+// ClipLoss backward contractions (bm/losses.py:91-114 differentiated, SURVEY.md A.6) on the 3xTF32 wgmma engine:
 //
 //     D[m][n] = sum_k A[m][k] * B[k][n]        A [M][K] row-major (K contiguous), B [K][N] row-major (N contiguous)
 //
 //   dE = G C      (M = estimates, K = candidates,  N = F*T = 368 640):  A = G   [Bn][Bc], B = candidates [Bc][F*T]
 //   dC = G^T E    (M = candidates, K = estimates,  N = F*T):            A = G^T [Bc][Bn], B = estimates  [Bn][F*T]
-//
-// Round 1 ran these on the weight-gradient kernel in "direct" mode: one CTA per 128 x 320 output tile with a K loop of
-// Bc/32 = 8 chunks at B = 256 -- prologue and epilogue dominated (95 TFLOP/s algorithmic at 256 x 256, 0.51 ms).  Here the
-// grid is one CTA pair per SM pair looping over the 256 x 256 output tiles (1 440 of them at F*T = 368 640), the operand
-// pipeline runs ahead across tile boundaries and eight epilogue warps store tile i through the TMA while tile i+1 is being
-// multiplied.
-//   per K chunk of 32, per CTA:  A rows 128 x 32 (16 KB, K-major, TMA) -> 4 converter warps: tf32 hi/lo -> TMEM slot
-//                                B [32 k][128 n] as four MN-major SWIZZLE_128B_ATOM_32B blocks (16 KB), raw = the tensor
-//                                core's `hi`; 2 warps write lo = x - trunc(x) beside it
-//   leader CTA, one thread:      12 x tcgen05.mma.cta_group::2.kind::tf32 (M = 256, N = 256, K = 8; A from TMEM)
-//   TMEM: [0, 256) accumulator, [256 + 64 s, +64) A slot of stage s (4 stages).
 #pragma once
-#include "tc_wgrad.cuh"
-#include "tc_convp.cuh"
+#include "tc_common.cuh"
 
 namespace bm {
 namespace tc {
 
-constexpr int GN_BM = 128, GN_BN = 256, GN_BK = 32, GN_STAGES = 4, GN_THREADS = 512;
-constexpr int GN_A_BYTES = GN_BM * GN_BK * 4;                       // 16 KB
-constexpr int GN_BLK_BYTES = 32 * 32 * 4;
-constexpr int GN_B_BYTES = (GN_BN / 2 / 32) * GN_BLK_BYTES;         // 16 KB: this CTA's half of the N tile
-constexpr int GN_STAGE_BYTES = GN_A_BYTES + 2 * GN_B_BYTES;         // 48 KB
-constexpr int GN_EPI_WARPS = 8, GN_EPI_BUF = 4096;
-constexpr int GN_SMEM_BYTES = GN_STAGES * GN_STAGE_BYTES + GN_EPI_WARPS * GN_EPI_BUF + 1024;
-constexpr int GN_ACC_COLS = GN_BN, GN_A_COLS = 2 * GN_BK;
-
-struct GemmNT {
+struct GemmNTOp {
+    static constexpr bool A_KCONTIG = true, B_KCONTIG = false;
+    const float* A; const float* B; float* D;
     int M, N, K;
-    int mtiles, ntiles, kchunks;
-    int* err;
+    struct Cta { int m0, n0; };
+    __device__ Cta cta() const { return Cta{(int)blockIdx.y * HG_BM, (int)blockIdx.x * HG_BN}; }
+    __device__ int kblocks(const Cta&) const { return (K + HG_BK - 1) / HG_BK; }
+    __device__ float4 a4(const Cta& c, int kb, int r, int q) const {
+        const int m = c.m0 + r, k = kb * HG_BK + 4 * q;
+        if (m >= M || k >= K) return make_float4(0.f, 0.f, 0.f, 0.f);
+        return __ldg(reinterpret_cast<const float4*>(A + (long long)m * K + k));
+    }
+    __device__ float4 b4(const Cta& c, int kb, int k, int q) const {
+        const int kk = kb * HG_BK + k, n = c.n0 + 4 * q;
+        if (kk >= K || n >= N) return make_float4(0.f, 0.f, 0.f, 0.f);
+        return __ldg(reinterpret_cast<const float4*>(B + (long long)kk * N + n));
+    }
+    __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+        HgStore s{D, N, M, N};
+        s.store(acc, c.m0 + m0, c.n0);
+    }
 };
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GN_THREADS, 1)
-gemm_nt_pp_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                  const __grid_constant__ CUtensorMap tmD, const GemmNT p) {
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[GN_STAGES], conv_bar[GN_STAGES], empty_bar[GN_STAGES];
-    __shared__ __align__(8) uint64_t acc_full, acc_empty;
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ int prior_error;
-
-    if (threadIdx.x == 0) prior_error = p.err ? *reinterpret_cast<volatile int*>(p.err) : 0;
-    __syncthreads();
-    const bool skip = prior_error != 0;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
-    uint8_t* epi_smem = smem + GN_STAGES * GN_STAGE_BYTES;
-
-    const int npairs = gridDim.x >> 1, pair = blockIdx.x >> 1;
-    const int ntiles = skip ? 0 : p.mtiles * p.ntiles;
-    const int per_tile = p.kchunks;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < GN_STAGES; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&conv_bar[s], 2 * (4 + 2));
-            mbar_init(&empty_bar[s], 1);
-        }
-        mbar_init(&acc_full, 1);
-        mbar_init(&acc_empty, 2 * GN_EPI_WARPS);
-        fence_barrier_init();
-    }
-    if (warp == 1) tmem_alloc_2sm<512>(&tmem_base_smem);
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_smem;
-
-    if (warp == 0) {
-        // ------------------------------------------------ TMA producer ------------------------------------------------
-        if (lane == 0) {
-            prefetch_tmap(&tmA);
-            prefetch_tmap(&tmB);
-            int git = 0;
-            bool ok = true;
-            for (int tile = pair; tile < ntiles && ok; tile += npairs) {
-                const int m_tile = tile % p.mtiles, n_tile = tile / p.mtiles;       // the M tiles of one N tile share B in L2
-                const int row0 = m_tile * 2 * GN_BM + (int)rank * GN_BM;
-                const int col0 = n_tile * GN_BN + (int)rank * (GN_BN / 2);
-                for (int it = 0; it < per_tile; ++it, ++git) {
-                    const int s = git % GN_STAGES;
-                    const uint32_t ph = (git / GN_STAGES) & 1;
-                    ok = mbar_wait(&empty_bar[s], ph ^ 1, p.err, 91);
-                    if (!ok) break;
-                    uint8_t* st = smem + s * GN_STAGE_BYTES;
-                    mbar_expect_tx(&full_bar[s], GN_A_BYTES + GN_B_BYTES);
-                    tma_load_2d(st, &tmA, &full_bar[s], it * GN_BK, row0);
-#pragma unroll
-                    for (int k = 0; k < GN_BN / 2 / 32; ++k)
-                        tma_load_2d(st + GN_A_BYTES + k * GN_BLK_BYTES, &tmB, &full_bar[s], col0 + 32 * k, it * GN_BK);
-                }
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------ MMA issuer (leader) -----------------------------------------
-        if (leader && lane == 0) {
-            const uint32_t idesc = umma_idesc_tf32_bmn(2 * GN_BM, GN_BN);
-            int git = 0, tcount = 0;
-            bool ok = true;
-            for (int tile = pair; tile < ntiles && ok; tile += npairs, ++tcount) {
-                if (tcount > 0) {
-                    ok = mbar_wait(&acc_empty, (uint32_t)(tcount - 1) & 1, p.err, 92);
-                    if (!ok) break;
-                    tc_fence_after();
-                }
-                for (int it = 0; it < per_tile; ++it, ++git) {
-                    const int s = git % GN_STAGES;
-                    const uint32_t ph = (git / GN_STAGES) & 1;
-                    ok = mbar_wait(&conv_bar[s], ph, p.err, 93);
-                    if (!ok) break;
-                    tc_fence_after();
-                    const uint32_t b_hi = smem_base + s * GN_STAGE_BYTES + GN_A_BYTES, b_lo = b_hi + GN_B_BYTES;
-                    const uint32_t a_hi = tmem + GN_ACC_COLS + s * GN_A_COLS, a_lo = a_hi + GN_BK;
-#pragma unroll
-                    for (int kk = 0; kk < GN_BK / 8; ++kk) {
-                        const uint64_t dbh = umma_desc_mn_sw128(b_hi + kk * 1024, GN_BLK_BYTES);
-                        const uint64_t dbl = umma_desc_mn_sw128(b_lo + kk * 1024, GN_BLK_BYTES);
-                        umma_tf32_ts_2sm(tmem, a_lo + kk * 8, dbh, idesc, (it | kk) != 0);
-                        umma_tf32_ts_2sm(tmem, a_hi + kk * 8, dbl, idesc, 1);
-                        umma_tf32_ts_2sm(tmem, a_hi + kk * 8, dbh, idesc, 1);
-                    }
-                    umma_commit_2sm(&empty_bar[s]);
-                }
-                if (ok) umma_commit_2sm(&acc_full);
-            }
-        }
-    } else if (warp < 6) {
-        // ------------------------------------------------ A rows -> TMEM (hi | lo) --------------------------------------
-        const int q = warp & 3;
-        const int row = q * 32 + lane;
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16);
-        int git = 0;
-        bool ok = true;
-        for (int tile = pair; tile < ntiles && ok; tile += npairs) {
-            for (int it = 0; it < per_tile && ok; ++it, ++git) {
-                const int s = git % GN_STAGES;
-                const uint32_t ph = (git / GN_STAGES) & 1;
-                ok = mbar_wait(&full_bar[s], ph, p.err, 94);
-                const uint8_t* arow = smem + s * GN_STAGE_BYTES + row * 128;
-                float hi[GN_BK], lo[GN_BK];
-#pragma unroll
-                for (int c = 0; c < 8; ++c) {
-                    const float4 v = *reinterpret_cast<const float4*>(arow + ((c ^ (row & 7)) << 4));
-                    tf32_split(v.x, hi[4 * c + 0], lo[4 * c + 0]); tf32_split(v.y, hi[4 * c + 1], lo[4 * c + 1]);
-                    tf32_split(v.z, hi[4 * c + 2], lo[4 * c + 2]); tf32_split(v.w, hi[4 * c + 3], lo[4 * c + 3]);
-                }
-                tc_fence_after();
-                tmem_st32(tq + GN_ACC_COLS + s * GN_A_COLS, hi);
-                tmem_st32(tq + GN_ACC_COLS + s * GN_A_COLS + GN_BK, lo);
-                tmem_st_wait();
-                tc_fence_before();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&conv_bar[s]), 0));
-            }
-        }
-    } else if (warp < 8) {
-        // ------------------------------------------------ B: lo = x - trunc_tf32(x) -----------------------------------
-        const int ct = (warp - 6) * 32 + lane;
-        int git = 0;
-        bool ok = true;
-        for (int tile = pair; tile < ntiles && ok; tile += npairs) {
-            for (int it = 0; it < per_tile && ok; ++it, ++git) {
-                const int s = git % GN_STAGES;
-                const uint32_t ph = (git / GN_STAGES) & 1;
-                ok = mbar_wait(&full_bar[s], ph, p.err, 95);
-                const float4* bh = reinterpret_cast<const float4*>(smem + s * GN_STAGE_BYTES + GN_A_BYTES);
-                float4* bl = reinterpret_cast<float4*>(smem + s * GN_STAGE_BYTES + GN_A_BYTES + GN_B_BYTES);
-#pragma unroll 4
-                for (int idx = ct; idx < GN_B_BYTES / 16; idx += 64) {
-                    const float4 v = bh[idx];
-                    float4 l;
-                    l.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-                    l.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-                    l.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-                    l.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-                    bl[idx] = l;
-                }
-                fence_proxy_async();
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&conv_bar[s]), 0));
-            }
-        }
-    } else {
-        // ------------------------------------------------ epilogue: two warps per TMEM lane quarter ---------------------
-        const int ew = warp - 8;
-        const int q = warp & 3, cset = ew >> 2;
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16);
-        uint8_t* buf = epi_smem + ew * GN_EPI_BUF;
-        if (lane == 0) prefetch_tmap(&tmD);
-        const float comp = acc_trunc_comp(per_tile * (GN_BK / 8) * 3);
-        int tcount = 0;
-        bool ok = true;
-        for (int tile = pair; tile < ntiles && ok; tile += npairs, ++tcount) {
-            const int m_tile = tile % p.mtiles, n_tile = tile / p.mtiles;
-            const int r32 = m_tile * 2 * GN_BM + (int)rank * GN_BM + q * 32;
-            const int c0 = n_tile * GN_BN + cset * (GN_BN / 2);
-            ok = mbar_wait(&acc_full, (uint32_t)tcount & 1, p.err, 96);
-            tc_fence_after();
-#pragma unroll 1
-            for (int c = 0; c < GN_BN / 2 / 32; ++c) {
-                float v[32];
-                tmem_ld32(tq + cset * (GN_BN / 2) + c * 32, v);
-                if (c + 1 == GN_BN / 2 / 32) {                       // last TMEM read of this thread: release the accumulator
-                    tc_fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&acc_empty), 0));
-                }
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] *= comp;
-                pp_stage_store(buf, v, lane, &tmD, c0 + c * 32, r32, false);
-            }
-        }
-        if (lane == 0) bulk_wait<0>();
-        __syncwarp();
-        tc_fence_before();
-    }
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_2sm<512>(tmem);
-    }
-}
 
 inline bool gemm_nt_pp_supported(int M, int N, int K) {
     return M > 0 && N >= 32 && K >= 8 && K % 4 == 0 && N % 4 == 0;
@@ -240,41 +39,9 @@ inline bool gemm_nt_pp_supported(int M, int N, int K) {
 
 // D [M][N] = A [M][K] * B [K][N], all row-major fp32
 inline int launch_gemm_nt_pp(const float* A, const float* B, float* D, int M, int N, int K, int* err, cudaStream_t st) {
-    CUtensorMap tmA, tmB, tmD;
-    {
-        uint64_t dims[2] = {(uint64_t)K, (uint64_t)M};
-        uint64_t str[1] = {(uint64_t)K * 4};
-        uint32_t box[2] = {GN_BK, GN_BM};
-        if (!make_tmap_f32(&tmA, A, 2, dims, str, box)) return set_error(4, "%s: cuTensorMapEncodeTiled(A) failed%s", __func__);
-    }
-    {
-        uint64_t dims[2] = {(uint64_t)N, (uint64_t)K};
-        uint64_t str[1] = {(uint64_t)N * 4};
-        uint32_t box[2] = {32, 32};
-        if (!make_tmap_f32(&tmB, B, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B))
-            return set_error(4, "%s: cuTensorMapEncodeTiled(B) failed%s", __func__);
-    }
-    {
-        uint64_t dims[2] = {(uint64_t)N, (uint64_t)M};
-        uint64_t str[1] = {(uint64_t)N * 4};
-        uint32_t box[2] = {32, 32};
-        if (!make_tmap_f32(&tmD, D, 2, dims, str, box)) return set_error(4, "%s: cuTensorMapEncodeTiled(D) failed%s", __func__);
-    }
-    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(gemm_nt_pp_kernel), GN_SMEM_BYTES)) return rc;
-    GemmNT p;
-    p.M = M; p.N = N; p.K = K;
-    p.mtiles = (M + 2 * GN_BM - 1) / (2 * GN_BM);
-    p.ntiles = (N + GN_BN - 1) / GN_BN;
-    p.kchunks = (K + GN_BK - 1) / GN_BK;
-    p.err = err;
-    int pairs = num_sms() / 2;
-    const long long tiles = (long long)p.mtiles * p.ntiles;
-    if (pairs > tiles) pairs = (int)tiles;
-    gemm_nt_pp_kernel<<<2 * pairs, GN_THREADS, GN_SMEM_BYTES, st>>>(tmA, tmB, tmD, p);
-    ++g_launches;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", __func__, cudaGetErrorString(e));
-    return 0;
+    (void)err;
+    GemmNTOp o{A, B, D, M, N, K};
+    return hg_launch(o, dim3((N + HG_BN - 1) / HG_BN, (M + HG_BM - 1) / HG_BM, 1), st, __func__);
 }
 
 }  // namespace tc

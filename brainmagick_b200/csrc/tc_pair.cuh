@@ -1,77 +1,10 @@
-// Shared pieces of the CTA-pair (tcgen05 cta_group::2) kernels: cluster rank / sync / remote mbarrier arrive, 2-SM tensor
-// memory allocation, the 2-SM MMA and commit wrappers, TMA store / reduce-add of staged epilogue blocks, and the N-tile rule.
+// Shape gate shared by the persistent conv entry points (bm_tc_conv1d_persistent, bm_tc_conv1d_f16): the column-half
+// rule nh in {160, 128} of the library's published contract.
 #pragma once
 #include "tc_common.cuh"
 
 namespace bm {
 namespace tc {
-
-// smem (128B-swizzled 32x32 fp32 block) -> global through the TMA: full-line, asynchronous stores; rows/samples outside
-// the tensor are clipped by the hardware.
-__device__ __forceinline__ void tma_store_3d(const CUtensorMap* m, const void* src, int c0, int c1, int c2) {
-    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* m, const void* src, int c0, int c1, int c2) {
-    asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];"
-                 ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait() { asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory"); }
-
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-    asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// address of the same shared-memory object in CTA `rank` of the cluster
-__device__ __forceinline__ uint32_t mapa_u32(uint32_t local_addr, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
-    return r;
-}
-// Arrive on an mbarrier of another CTA of the cluster.  Default semantics (.release.cta), NOT .release.cluster: ptxas lowers
-// a cluster-scope release to MEMBAR.ALL.GPU + ERRBAR, which cost the converter warps ~1 300 cycles per K chunk (measured
-// with the cycle counters of tc_wgradp.cuh: the MMA thread waited for the converters 53 % of the time).  What the consumer
-// reads is ordered by other means: tensor memory by the tcgen05.fence::before/after_thread_sync pair around this arrive,
-// shared memory written through the generic proxy by the fence.proxy.async before it (the pattern of CUTLASS's
-// ClusterBarrier::arrive(cta_id)).
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t* dst_smem) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(dst_smem)), "n"(NCOLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS) : "memory");
-}
-__device__ __forceinline__ void umma_tf32_ts_2sm(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc,
-                                                 uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::tf32 [%0], [%1], %2, %3, p;\n\t}"
-        ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// arrives on the barrier at this smem offset in BOTH CTAs of the pair when the issued MMAs are complete
-__device__ __forceinline__ void umma_commit_2sm(uint64_t* bar) {
-    asm volatile(
-        "tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-        ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-        : "memory");
-}
 
 inline int pair_pick_nh(int Ntot, int glu) {
     if (glu && (Ntot % 2)) return 0;
@@ -87,7 +20,6 @@ inline bool pair_conv_supported(int T, int Cin, int Ntot, int Kw, int glu) {
     if (Cin % 32 != 0) return false;
     return pair_pick_nh(Ntot, glu) != 0;
 }
-
 
 }  // namespace tc
 }  // namespace bm

@@ -1,266 +1,20 @@
-// Weight gradients on the tensor cores (3xTF32):  for one tap shift s
+// Weight gradients on the tensor cores (3xTF32 wgmma engine of tc_common.cuh):  for one tap shift s
 //
 //     P[ks][m][n] = sum_{b in split ks} sum_t  dY[b, t, m] * X[b, t + s, n]          (dY, X channels-last)
 //
-// i.e. a GEMM whose reduction runs over POSITIONS, so both operands are "MN-major" in memory (the contraction
-// index is the slow one).  Per CTA: one 128(m) x 2*NH(n) output tile for one tap and one slice of the batch.
-//   * A = dY^T goes through REGISTERS into TENSOR MEMORY: thread m of the 4 converter warps loads dY[b, t, m0+m]
-//     for 32 positions (each warp-load is one coalesced 128-byte row piece), splits hi/lo, and writes its TMEM
-//     lane with tcgen05.st -- the transpose costs nothing and A never touches shared memory (tcgen05 "TS" form).
-//   * B = X tile via TMA as MN-major SWIZZLE_128B_BASE32B blocks ([32 positions] x [32 channels] = 4 KB each; rows outside
-//     [0,T) are zero-filled = the conv padding); the converter warps split it in place into hi and a lo copy.
-//   * one thread issues tcgen05.mma kind::tf32 (A from TMEM, B from smem, M=128, N=NH) x 3 passes x 2 halves.
-//   * epilogue: TMEM -> registers -> partial tile in the workspace; `wgrad_reduce_kernel` sums the batch slices in a
-//     fixed order (deterministic) and scatters into the nn.Conv1d weight layout [m][n][tap].
+// i.e. a GEMM whose reduction runs over POSITIONS, so both operands are M/N-contiguous in memory; the engine transposes
+// them on their way into its K-major shared-memory tiles.  Per CTA: one 128(m) x 128(n) tile for one tap and one slice of
+// the batch (X rows shifted outside [0,T) are zeros = the conv padding).  The partial tiles go to the workspace and
+// `wgrad_reduce_kernel` sums the batch slices in a fixed order (deterministic) into the nn.Conv1d layout [m][n][tap];
+// "direct" calls (one tap, one slice) write the output itself, and the grouped form writes one plane per group.
 #pragma once
 #include "tc_common.cuh"
+#include "elementwise.cuh"
 
 namespace bm {
 namespace tc {
 
-constexpr int WG_BM = 128, WG_BK = 32, WG_STAGES = 2, WG_THREADS = 192;
-constexpr int WG_MAX_NH = 160;
-constexpr int WG_BLK_BYTES = 32 * 32 * 4;                       // one [32 pos][32 ch] block
-constexpr int WG_B_BYTES_MAX = 2 * WG_MAX_NH * WG_BK * 4;       // 40 KB
-constexpr int WG_STAGE_BYTES = 2 * WG_B_BYTES_MAX;              // hi + lo
-constexpr int WG_SMEM_BYTES = WG_STAGES * WG_STAGE_BYTES + 1024;
-constexpr int WG_ACC_COLS = 2 * WG_MAX_NH;                      // 320
-constexpr int WG_A_COLS = 2 * WG_BK;                            // hi 32 + lo 32 per stage
-
-struct WgradP {
-    int B, T, M, N;             // M = dY channels, N = X channels
-    int nh;                     // half N tile (N tile = 2*nh), multiple of 32, <= 160
-    int taps, dilation;         // blockIdx.x = tap * ntiles + n_tile; X rows shifted by (tap - taps/2)*dilation
-    int ksplit, bchunk;         // batch slices: slice ks covers samples [ks*bchunk, min(B, (ks+1)*bchunk))
-    const float* dY;            // [B,T,M]
-    float* P;                   // [taps][ksplit][Mpad][N] partial tiles, Mpad = gridDim.y*128
-    int* err;
-    int direct;                 // 1 (taps == 1, ksplit == 1): P IS the output [M][N]; rows >= M are not written
-    const int* zlist;           // grouped mode (per-subject gradients): slice ks = samples zlist[seg_off[ks] .. seg_off[ks+1])
-    const int* seg_off;         //   and P [ksplit][Mpad][N] is the per-group output (no reduction)
-    float* dbias;               // [M] or null: bias gradient sum_{b,t} dY[b,t,m], accumulated for free from the dY values the
-                                //   converter threads already hold (atomicAdd; zeroed by the launcher)
-    int trunc_hi;               // 1: leave X raw in smem as the hi operand (the tensor core ignores the 13 low mantissa
-                                //    bits) and write only lo = x - trunc(x): one third less converter smem traffic
-};
-
-// MN-major tf32 operand: the only legal shared-memory layout is SWIZZLE_128B_BASE32B (cutlass sm100_common.inl:92):
-// rows of 128 bytes (32 elements along MN), 4-row atoms along K whose 32-byte chunks are XOR-swizzled with the row
-// index -- what TMA writes with CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);
-    d |= (uint64_t)(lbo_bytes >> 4) << 16;               // next 32-element block along MN
-    d |= (uint64_t)(512 >> 4) << 32;                     // next 4-row atom along K
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)1 << 61;                              // SWIZZLE_128B_BASE32B
-    return d;
-}
-__host__ __device__ constexpr uint32_t umma_idesc_tf32_bmn(int M, int N) {
-    return umma_idesc_tf32(M, N) | (1u << 16);           // B operand MN-major
-}
-
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const float* v) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, "
-        "%17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-        ::"r"(taddr), "r"(__float_as_uint(v[0])), "r"(__float_as_uint(v[1])), "r"(__float_as_uint(v[2])),
-        "r"(__float_as_uint(v[3])), "r"(__float_as_uint(v[4])), "r"(__float_as_uint(v[5])), "r"(__float_as_uint(v[6])),
-        "r"(__float_as_uint(v[7])), "r"(__float_as_uint(v[8])), "r"(__float_as_uint(v[9])), "r"(__float_as_uint(v[10])),
-        "r"(__float_as_uint(v[11])), "r"(__float_as_uint(v[12])), "r"(__float_as_uint(v[13])),
-        "r"(__float_as_uint(v[14])), "r"(__float_as_uint(v[15])), "r"(__float_as_uint(v[16])),
-        "r"(__float_as_uint(v[17])), "r"(__float_as_uint(v[18])), "r"(__float_as_uint(v[19])),
-        "r"(__float_as_uint(v[20])), "r"(__float_as_uint(v[21])), "r"(__float_as_uint(v[22])),
-        "r"(__float_as_uint(v[23])), "r"(__float_as_uint(v[24])), "r"(__float_as_uint(v[25])),
-        "r"(__float_as_uint(v[26])), "r"(__float_as_uint(v[27])), "r"(__float_as_uint(v[28])),
-        "r"(__float_as_uint(v[29])), "r"(__float_as_uint(v[30])), "r"(__float_as_uint(v[31]))
-        : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-__global__ void __launch_bounds__(WG_THREADS, 1)
-wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmX, const WgradP p) {
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[WG_STAGES], conv_bar[WG_STAGES], empty_bar[WG_STAGES], tmem_full_bar;
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ int prior_error;
-
-    if (threadIdx.x == 0) prior_error = p.err ? *reinterpret_cast<volatile int*>(p.err) : 0;
-    __syncthreads();
-    if (prior_error) return;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
-
-    const int ntiles = p.N / (2 * p.nh);
-    const int tap = blockIdx.x / ntiles;
-    const int shift = (tap - p.taps / 2) * p.dilation;
-    const int n0 = (blockIdx.x - tap * ntiles) * 2 * p.nh, m0 = blockIdx.y * WG_BM, ks = blockIdx.z;
-    const int b_begin = p.seg_off ? p.seg_off[ks] : ks * p.bchunk;
-    const int b_end = p.seg_off ? p.seg_off[ks + 1] : min(p.B, b_begin + p.bchunk);
-    const int tchunks = (p.T + WG_BK - 1) / WG_BK;
-    const int total = max(0, b_end - b_begin) * tchunks;
-    const int nblk = 2 * p.nh / 32;                          // 32-channel blocks in the B tile
-    const uint32_t b_bytes = (uint32_t)nblk * WG_BLK_BYTES;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < WG_STAGES; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&conv_bar[s], 128);
-            mbar_init(&empty_bar[s], 1);
-        }
-        mbar_init(&tmem_full_bar, 1);
-        fence_barrier_init();
-    }
-    if (warp == 1) tmem_alloc<512>(&tmem_base_smem);
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_smem;
-
-    if (warp == 0) {
-        if (lane == 0) {
-            prefetch_tmap(&tmX);
-            for (int it = 0; it < total; ++it) {
-                const int s = it % WG_STAGES;
-                const uint32_t ph = (it / WG_STAGES) & 1;
-                if (!mbar_wait(&empty_bar[s], ph ^ 1, p.err, 11)) break;
-                int b = b_begin + it / tchunks;
-                if (p.zlist) b = p.zlist[b];
-                const int t0 = (it % tchunks) * WG_BK;
-                uint8_t* st = smem + s * WG_STAGE_BYTES;
-                mbar_expect_tx(&full_bar[s], b_bytes);
-                for (int k = 0; k < nblk; ++k)
-                    tma_load_3d(st + k * WG_BLK_BYTES, &tmX, &full_bar[s], n0 + 32 * k, t0 + shift, b);
-            }
-        }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = umma_idesc_tf32_bmn(WG_BM, p.nh);
-            bool ok = true;
-            for (int it = 0; it < total && ok; ++it) {
-                const int s = it % WG_STAGES;
-                const uint32_t ph = (it / WG_STAGES) & 1;
-                ok = mbar_wait(&conv_bar[s], ph, p.err, 13);
-                if (!ok) break;
-                tc_fence_after();
-                const uint32_t b_hi = smem_base + s * WG_STAGE_BYTES, b_lo = b_hi + WG_B_BYTES_MAX;
-                const uint32_t a_hi = tmem + WG_ACC_COLS + s * WG_A_COLS, a_lo = a_hi + WG_BK;
-#pragma unroll
-                for (int kk = 0; kk < WG_BK / 8; ++kk) {
-#pragma unroll
-                    for (int half = 0; half < 2; ++half) {
-                        const uint32_t boff = kk * 1024 + half * (p.nh / 32) * WG_BLK_BYTES;
-                        const uint64_t dbh = umma_desc_mn_sw128(b_hi + boff, WG_BLK_BYTES);
-                        const uint64_t dbl = umma_desc_mn_sw128(b_lo + boff, WG_BLK_BYTES);
-                        const uint32_t d = tmem + half * p.nh;
-                        umma_tf32_ts(d, a_lo + kk * 8, dbh, idesc, (it | kk) != 0);
-                        umma_tf32_ts(d, a_hi + kk * 8, dbl, idesc, 1);
-                        umma_tf32_ts(d, a_hi + kk * 8, dbh, idesc, 1);
-                    }
-                }
-                umma_commit(&empty_bar[s]);
-            }
-            umma_commit(&tmem_full_bar);
-        }
-    } else {
-        const int q = warp & 3;                              // TMEM lane quarter of this warp
-        const int m = m0 + q * 32 + lane;                    // the dY channel (= output row) this thread owns
-        const bool m_ok = m < p.M;
-        const int ct = (warp - 2) * 32 + lane;
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16);
-        float nxt[WG_BK];
-        auto load_a = [&](int it) {
-            int b = b_begin + it / tchunks;
-            if (p.zlist) b = p.zlist[b];
-            const int t0 = (it % tchunks) * WG_BK;
-            const float* src = p.dY + ((long long)b * p.T + t0) * p.M + m;
-#pragma unroll
-            for (int j = 0; j < WG_BK; ++j) nxt[j] = (m_ok && t0 + j < p.T) ? __ldg(src + (long long)j * p.M) : 0.f;
-        };
-        if (total > 0) load_a(0);
-        bool ok = true;
-        float bias_acc = 0.f;
-        for (int it = 0; it < total && ok; ++it) {
-            const int s = it % WG_STAGES;
-            const uint32_t ph = (it / WG_STAGES) & 1;
-            float hi[WG_BK], lo[WG_BK];
-#pragma unroll
-            for (int j = 0; j < WG_BK; ++j) {
-                tf32_split(nxt[j], hi[j], lo[j]);
-                bias_acc += nxt[j];
-            }
-            if (it + 1 < total) load_a(it + 1);              // prefetch the next chunk's dY column
-            // the TMEM A slot and the smem stage are free once the MMAs of iteration it-STAGES have completed
-            ok = mbar_wait(&empty_bar[s], ph ^ 1, p.err, 14);
-            tc_fence_after();
-            tmem_st32(tq + WG_ACC_COLS + s * WG_A_COLS, hi);
-            tmem_st32(tq + WG_ACC_COLS + s * WG_A_COLS + WG_BK, lo);
-            tmem_st_wait();
-            ok = ok && mbar_wait(&full_bar[s], ph, p.err, 15);
-            float4* bh = reinterpret_cast<float4*>(smem + s * WG_STAGE_BYTES);
-            float4* bl = reinterpret_cast<float4*>(smem + s * WG_STAGE_BYTES + WG_B_BYTES_MAX);
-            const int nvec = (int)(b_bytes / 16);
-            if (p.trunc_hi) {
-#pragma unroll 4
-                for (int idx = ct; idx < nvec; idx += 128) {
-                    const float4 v = bh[idx];
-                    float4 l;
-                    l.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-                    l.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-                    l.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-                    l.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-                    bl[idx] = l;
-                }
-            } else {
-#pragma unroll 2
-                for (int idx = ct; idx < nvec; idx += 128) {
-                    float4 v = bh[idx], h, l;
-                    tf32_split(v.x, h.x, l.x); tf32_split(v.y, h.y, l.y); tf32_split(v.z, h.z, l.z); tf32_split(v.w, h.w, l.w);
-                    bh[idx] = h;
-                    bl[idx] = l;
-                }
-            }
-            fence_proxy_async();
-            tc_fence_before();
-            mbar_arrive(&conv_bar[s]);
-        }
-        if (p.dbias && m_ok && tap == p.taps / 2 && n0 == 0) atomicAdd(p.dbias + m, bias_acc);
-        // ---- epilogue: partial tile -> workspace ----
-        mbar_wait(&tmem_full_bar, 0, p.err, 16);
-        tc_fence_after();
-        const int Mpad = p.direct ? p.M : gridDim.y * WG_BM;
-        const bool row_ok = !p.direct || m_ok;
-        float* dst = p.P + (((long long)tap * p.ksplit + ks) * Mpad + (m0 + q * 32 + lane)) * p.N + n0;
-#pragma unroll 1
-        for (int c = 0; c < 2 * p.nh / 32; ++c) {
-            float v[32];
-            tmem_ld32(tq + c * 32, v);
-            {
-                const float comp = acc_trunc_comp(total * (WG_BK / 8) * 3);
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] *= comp;
-            }
-            if (total == 0) {
-#pragma unroll
-                for (int j = 0; j < 32; ++j) v[j] = 0.f;
-            }
-            if (row_ok) {
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    *reinterpret_cast<float4*>(dst + c * 32 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-            }
-        }
-        tc_fence_before();
-    }
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc<512>(tmem);
-    }
-}
+constexpr int WG_BM = HG_BM;
 
 // dW[m][n][tap] = sum_ks P[tap][ks][m][n]   (fixed summation order => deterministic), n < Ntrue only
 __global__ void wgrad_reduce_kernel(const float* __restrict__ P, float* __restrict__ dW, int taps, int ksplit, int Mpad,
@@ -288,7 +42,7 @@ inline bool wgrad_tc_supported(int M, int N) { return wgrad_pick_nh(N) != 0 && M
 inline void wgrad_geometry(int B, int M, int N, int taps, int* nh, int* mblocks, int* ksplit, int* bchunk) {
     *nh = wgrad_pick_nh(N);
     *mblocks = (M + WG_BM - 1) / WG_BM;
-    int tiles = (*mblocks) * (N / (2 * *nh)) * taps;
+    int tiles = (*mblocks) * ((N + HG_BN - 1) / HG_BN) * taps;
     int want = num_sms() / tiles;                 // floor: the whole grid must fit in ONE wave (1 CTA per SM)
     if (want < 1) want = 1;
     if (want > B) want = B;
@@ -301,42 +55,82 @@ inline size_t wgrad_workspace_floats(int B, int M, int N, int taps) {
     return (size_t)taps * ks * mb * WG_BM * N;
 }
 
+struct WgradOp {
+    static constexpr bool A_KCONTIG = false, B_KCONTIG = false;
+    int B, T, M, N, taps, dilation, ntiles;
+    int bchunk;                 // batch slices: slice ks covers samples [ks*bchunk, min(B, (ks+1)*bchunk))
+    const int* zlist;           // grouped mode: slice ks = samples zlist[seg_off[ks] .. seg_off[ks+1])
+    const int* seg_off;
+    const float* dY;            // [B,T,M]
+    const float* X;             // [B,T,N]
+    float* P;                   // output planes
+    long long plane;            // floats per (tap, slice) plane of P
+    int rows;                   // rows of a plane that are written
+    int ksplit;
+
+    struct Cta { int tap, shift, m0, n0, ks, b_begin, b_end, tchunks; };
+    __device__ Cta cta() const {
+        Cta c;
+        c.tap = blockIdx.x / ntiles;
+        c.shift = (c.tap - taps / 2) * dilation;
+        c.n0 = (blockIdx.x - c.tap * ntiles) * HG_BN;
+        c.m0 = blockIdx.y * HG_BM;
+        c.ks = blockIdx.z;
+        c.b_begin = seg_off ? seg_off[c.ks] : c.ks * bchunk;
+        c.b_end = seg_off ? seg_off[c.ks + 1] : min(B, c.b_begin + bchunk);
+        c.tchunks = (T + HG_BK - 1) / HG_BK;
+        return c;
+    }
+    __device__ int kblocks(const Cta& c) const { return max(0, c.b_end - c.b_begin) * c.tchunks; }
+    __device__ int sample(const Cta& c, int kb) const {
+        const int b = c.b_begin + kb / c.tchunks;
+        return zlist ? zlist[b] : b;
+    }
+    __device__ float4 a4(const Cta& c, int kb, int k, int q) const {         // dY^T: rows m, reduction over positions
+        const int t = (kb % c.tchunks) * HG_BK + k, m = c.m0 + 4 * q;
+        if (t >= T || m >= M) return make_float4(0.f, 0.f, 0.f, 0.f);
+        return __ldg(reinterpret_cast<const float4*>(dY + ((long long)sample(c, kb) * T + t) * M + m));
+    }
+    __device__ float4 b4(const Cta& c, int kb, int k, int q) const {         // X^T shifted by the tap, zeros across the edges
+        const int t = (kb % c.tchunks) * HG_BK + k, ts = t + c.shift, n = c.n0 + 4 * q;
+        if (t >= T || ts < 0 || ts >= T || n >= N) return make_float4(0.f, 0.f, 0.f, 0.f);
+        return __ldg(reinterpret_cast<const float4*>(X + ((long long)sample(c, kb) * T + ts) * N + n));
+    }
+    __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+        HgStore s{P + ((long long)c.tap * ksplit + c.ks) * plane, N, rows, N};
+        s.store(acc, c.m0 + m0, c.n0);
+    }
+};
+
 // dY [B,T,M], X [B,T,N] -> dW [M][Ntrue][taps]; ws: wgrad_workspace_floats() floats
 inline int launch_wgrad_tc(const float* dY, const float* X, int B, int T, int M, int N, int Ntrue, int taps,
                            int dilation, float* ws, float* dW, int* err, cudaStream_t st, float* dbias = nullptr) {
+    (void)err;
     int nh, mblocks, ksplit, bchunk;
     wgrad_geometry(B, M, N, taps, &nh, &mblocks, &ksplit, &bchunk);
     if (nh == 0) return set_error(2, "%s: unsupported N%s", __func__);
-    CUtensorMap tmX;
-    {
-        uint64_t dims[3] = {(uint64_t)N, (uint64_t)T, (uint64_t)B};
-        uint64_t str[2] = {(uint64_t)N * 4, (uint64_t)T * N * 4};
-        uint32_t box[3] = {32, 32, 1};
-        if (!make_tmap_f32(&tmX, X, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B)) return set_error(4, "%s: cuTensorMapEncodeTiled failed%s", __func__);
-    }
-    if (int rc_ = ensure_dyn_smem(reinterpret_cast<const void*>(wgrad_tc_kernel), WG_SMEM_BYTES)) return rc_;
     const int Mpad = mblocks * WG_BM;
-    WgradP p;
-    p.B = B; p.T = T; p.M = M; p.N = N; p.nh = nh; p.taps = taps; p.dilation = dilation;
-    p.ksplit = ksplit; p.bchunk = bchunk; p.dY = dY; p.err = err; p.P = ws;
-    p.direct = (taps == 1 && ksplit == 1 && Ntrue == N) ? 1 : 0;
-    p.zlist = nullptr; p.seg_off = nullptr;
-    p.dbias = dbias;
-    if (dbias) {
+    const bool direct = taps == 1 && ksplit == 1 && Ntrue == N;
+    WgradOp o;
+    o.B = B; o.T = T; o.M = M; o.N = N; o.taps = taps; o.dilation = dilation; o.ntiles = (N + HG_BN - 1) / HG_BN;
+    o.bchunk = bchunk; o.zlist = nullptr; o.seg_off = nullptr; o.dY = dY; o.X = X; o.ksplit = ksplit;
+    o.P = direct ? dW : ws;
+    o.plane = (long long)(direct ? M : Mpad) * N;
+    o.rows = direct ? M : Mpad;
+    if (int rc = hg_launch(o, dim3(o.ntiles * taps, mblocks, ksplit), st, __func__)) return rc;
+    if (dbias) {               // bias gradient sum_{b,t} dY[b,t,m]
         cudaError_t em = cudaMemsetAsync(dbias, 0, sizeof(float) * M, st);
         if (em != cudaSuccess) return set_error(3, "%s: memset: %s", __func__, cudaGetErrorString(em));
+        const long long rows = (long long)B * T;
+        colsum_cl_kernel<<<dim3((unsigned)((rows + 255) / 256), (M + 127) / 128), 128, 0, st>>>(dY, dbias, rows, M, 256);
+        ++g_launches;
+        cudaError_t e = cudaGetLastError();
+        if (e != cudaSuccess) return set_error(3, "%s: bias launch failed: %s", __func__, cudaGetErrorString(e));
     }
-    if (p.direct) p.P = dW;
-    p.trunc_hi = (g_debug_flags & 1) ? 0 : 1;     // default ON; debug bit 0 restores the explicit rna split
-    dim3 grid(N / (2 * nh) * taps, mblocks, ksplit);
-    wgrad_tc_kernel<<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(tmX, p);
-    ++g_launches;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", __func__, cudaGetErrorString(e));
-    if (p.direct) return 0;
+    if (direct) return 0;
     wgrad_reduce_kernel<<<ew_grid((long long)M * Ntrue * taps), 256, 0, st>>>(ws, dW, taps, ksplit, Mpad, M, N, Ntrue);
     ++g_launches;
-    e = cudaGetLastError();
+    cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(3, "%s: reduce launch failed: %s", __func__, cudaGetErrorString(e));
     return 0;
 }
@@ -345,29 +139,15 @@ inline int launch_wgrad_tc(const float* dY, const float* X, int B, int T, int M,
 // Mpad = ceil(M/128)*128 (rows >= M are zero); groups given as CSR (zlist, seg_off[G+1]) over the samples.
 inline int launch_wgrad_tc_grouped(const float* dY, const float* X, const int* zlist, const int* seg_off, int G, int B,
                                    int T, int M, int N, float* out, int* err, cudaStream_t st) {
-    const int nh = wgrad_pick_nh(N);
-    if (nh == 0) return set_error(2, "%s: unsupported N%s", __func__);
-    CUtensorMap tmX;
-    {
-        uint64_t dims[3] = {(uint64_t)N, (uint64_t)T, (uint64_t)B};
-        uint64_t str[2] = {(uint64_t)N * 4, (uint64_t)T * N * 4};
-        uint32_t box[3] = {32, 32, 1};
-        if (!make_tmap_f32(&tmX, X, 3, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B))
-            return set_error(4, "%s: cuTensorMapEncodeTiled failed%s", __func__);
-    }
-    if (int rc_ = ensure_dyn_smem(reinterpret_cast<const void*>(wgrad_tc_kernel), WG_SMEM_BYTES)) return rc_;
-    WgradP p;
-    p.B = B; p.T = T; p.M = M; p.N = N; p.nh = nh; p.taps = 1; p.dilation = 1;
-    p.ksplit = G; p.bchunk = 0; p.dY = dY; p.err = err; p.P = out; p.direct = 0;
-    p.zlist = zlist; p.seg_off = seg_off; p.dbias = nullptr;
-    p.trunc_hi = (g_debug_flags & 1) ? 0 : 1;
-    dim3 grid(N / (2 * nh), (M + WG_BM - 1) / WG_BM, G);
+    (void)err;
+    if (wgrad_pick_nh(N) == 0) return set_error(2, "%s: unsupported N%s", __func__);
     if (G > 65535) return set_error(2, "%s: too many groups%s", __func__);
-    wgrad_tc_kernel<<<grid, WG_THREADS, WG_SMEM_BYTES, st>>>(tmX, p);
-    ++g_launches;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", __func__, cudaGetErrorString(e));
-    return 0;
+    const int mblocks = (M + WG_BM - 1) / WG_BM;
+    WgradOp o;
+    o.B = B; o.T = T; o.M = M; o.N = N; o.taps = 1; o.dilation = 1; o.ntiles = (N + HG_BN - 1) / HG_BN;
+    o.bchunk = 0; o.zlist = zlist; o.seg_off = seg_off; o.dY = dY; o.X = X; o.ksplit = G;
+    o.P = out; o.plane = (long long)mblocks * WG_BM * N; o.rows = mblocks * WG_BM;
+    return hg_launch(o, dim3(o.ntiles, mblocks, G), st, __func__);
 }
 
 }  // namespace tc

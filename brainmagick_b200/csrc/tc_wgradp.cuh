@@ -1,4 +1,4 @@
-// Weight gradient of a (dilated) k-tap conv on CTA PAIRS (3xTF32):
+// Weight gradient of a (dilated) k-tap conv (3xTF32 wgmma engine of tc_common.cuh):
 //
 //     dW[m][n][tap] = sum_p dY[p, m] * X[p + shift(tap), n]          p = b*T + t flattened rows, channels-last operands
 //
@@ -6,292 +6,51 @@
 //
 //     G[(tap, n)][m] = sum_p Xs[p, (tap, n)] * dY[p, m],     Xs[p, (tap, n)] = X[p + shift(tap), n] (0 across a sample edge)
 //
-// Why (round 1's wgrad_tc_kernel, 28 % of the step at 54-64 % of the 3xTF32 ceiling):
-//   * it tiled the dY channels in blocks of 128: 320 channels = 3 blocks = 384 rows, 20 % of its MMAs were padding, per tap.
-//     Here the 3 x 320 = 960 (tap, n) rows are tiled together: 4 pair-tiles of 256 = 1024 rows, 6 % padding;
-//   * it reduced per sample in chunks of 32 positions (T = 360 -> 12 chunks, the last one 25 % full).  dY is not shifted
-//     here (the shift moved to the X side), so the reduction runs over the flattened rows in exact chunks of 32;
-//   * one CTA multiplied a 128-row block against all 320 columns: every B byte was read from shared memory three times by
-//     the MMAs plus once by the splitter -- 125 B/cycle of the SM's 128.  A CTA pair (cta_group::2, M = 256) holds HALF of
-//     the dY tile per CTA: 62 B/cycle.
-// Operands:  A = Xs^T: per converter warp one TMA box [32 positions][32 x-channels] at row p + shift(tap) (un-swizzled: the
-//            warp reads it column-wise, lane = channel, conflict-free) in a SIX-deep ring -- X is an activation saved by the
-//            forward pass and comes from HBM; per-thread loads one or two chunks ahead left the MMA thread waiting 47-53 %
-//            of the time (cycle counters, bm_set_debug_buffer).  Thread r owns row (tap, n): positions whose shifted time
-//            falls outside [0, T) are zeros (the conv padding); split hi/lo, tcgen05.st into tensor memory;
-//            B = dY tile by TMA as MN-major SWIZZLE_128B_ATOM_32B blocks ([32 positions] x [32 channels], 4 KB), raw =
-//            the tensor core's `hi`; two warps write lo = x - trunc(x) beside it.
-// One CTA pair = one (256-row tile, N tile, K slice); partial tiles go to the workspace and `wgradp_reduce_kernel` sums the
-// K slices in a fixed order (deterministic) while scattering into the nn.Conv1d layout [m][n][tap].
+// so the taps share one tile grid (3 x 320 rows = 7.5 tiles of 128 instead of 3 x 3) and the reduction runs over the
+// flattened rows in exact blocks of 32.  One CTA = one (128-row tile, 128-column tile, K slice); partial tiles go to the
+// workspace and `wgradp_reduce_kernel` sums the K slices in a fixed order (deterministic) while scattering into the
+// nn.Conv1d layout [m][n][tap].
 #pragma once
 #include "tc_wgrad.cuh"
-#include "tc_pair.cuh"
 
 namespace bm {
 namespace tc {
 
-constexpr int WP_BK = 32, WP_STAGES = 3, WP_ASTAGES = 6, WP_THREADS = 288;
-constexpr int WP_BLK_BYTES = 32 * 32 * 4;                    // one [32 positions][32 channels] block
-constexpr int WP_MAX_BLKS = 5;                               // per CTA: half of an N tile of <= 320 channels
-constexpr int WP_B_BYTES = WP_MAX_BLKS * WP_BLK_BYTES;       // 20 KB
-constexpr int WP_STAGE_BYTES = 2 * WP_B_BYTES;               // raw + lo
-constexpr int WP_ATILE_BYTES = 4 * WP_BLK_BYTES;             // X tile of one chunk: per converter warp [32 positions][32 rows]
-constexpr int WP_SMEM_BYTES = WP_STAGES * WP_STAGE_BYTES + WP_ASTAGES * WP_ATILE_BYTES + 1024;
-constexpr int WP_ACC_COLS = 320, WP_A_COLS = 2 * WP_BK;
+struct WgradPOp {
+    static constexpr bool A_KCONTIG = false, B_KCONTIG = false;
+    int R, T, Mdy, Nx, taps, dilation, rows, per_split, chunks;
+    const float* dY; const float* X;
+    float* P;                   // [ks][rows_pad][Mdy]
+    int rows_pad;
 
-struct WgradPP {
-    int R, T, Mdy, Nx;          // flattened rows, samples' length, dY channels, X channels
-    int taps, dilation;
-    int rows;                   // taps * Nx output rows
-    int mtiles, ntiles, ks;     // 256-row tiles, N tiles, K slices
-    int nt, h0, h1;             // N tile and its two MMA halves (h1 may be 0); each a multiple of 64
-    int chunks, per_split;
-    float* P;                   // [ks][mtiles*256][Mdy]
-    int* err;
-    long long* dbg;             // debug only (bm_set_debug_buffer): per CTA 8 cycle counters, see the kernel
+    struct Cta { int m0, n0, c0, c1; };
+    __device__ Cta cta() const {
+        Cta c;
+        c.n0 = blockIdx.x * HG_BN;
+        c.m0 = blockIdx.y * HG_BM;
+        c.c0 = blockIdx.z * per_split;
+        c.c1 = min(chunks, c.c0 + per_split);
+        return c;
+    }
+    __device__ int kblocks(const Cta& c) const { return max(0, c.c1 - c.c0); }
+    __device__ float4 a4(const Cta& c, int kb, int k, int q) const {         // Xs^T: rows (tap, n), 4 never straddle a tap
+        const int r = c.m0 + 4 * q, p = (c.c0 + kb) * HG_BK + k;
+        if (r >= rows || p >= R) return make_float4(0.f, 0.f, 0.f, 0.f);
+        const int tap = r / Nx, n = r - tap * Nx;
+        const int b = p / T, t = p - b * T, ts = t + (tap - taps / 2) * dilation;
+        if (ts < 0 || ts >= T) return make_float4(0.f, 0.f, 0.f, 0.f);
+        return __ldg(reinterpret_cast<const float4*>(X + ((long long)b * T + ts) * Nx + n));
+    }
+    __device__ float4 b4(const Cta& c, int kb, int k, int q) const {         // dY^T
+        const int m = c.n0 + 4 * q, p = (c.c0 + kb) * HG_BK + k;
+        if (m >= Mdy || p >= R) return make_float4(0.f, 0.f, 0.f, 0.f);
+        return __ldg(reinterpret_cast<const float4*>(dY + (long long)p * Mdy + m));
+    }
+    __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+        HgStore s{P + (long long)blockIdx.z * rows_pad * Mdy, Mdy, rows_pad, Mdy};
+        s.store(acc, c.m0 + m0, c.n0);
+    }
 };
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(WP_THREADS, 1)
-wgrad_pp_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, const WgradPP p) {
-    extern __shared__ uint8_t smem_raw[];
-    __shared__ __align__(8) uint64_t full_bar[WP_STAGES], conv_bar[WP_STAGES], empty_bar[WP_STAGES], tmem_full_bar;
-    __shared__ __align__(8) uint64_t afull_bar[WP_ASTAGES], aempty_bar[WP_ASTAGES];
-    __shared__ uint32_t tmem_base_smem;
-    __shared__ int prior_error;
-
-    if (threadIdx.x == 0) prior_error = p.err ? *reinterpret_cast<volatile int*>(p.err) : 0;
-    __syncthreads();
-    const bool skip = prior_error != 0;
-
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const uint32_t rank = cluster_ctarank();
-    const bool leader = rank == 0;
-    const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-    uint8_t* smem = smem_raw + (smem_base - smem_u32(smem_raw));
-
-    int pair = blockIdx.x >> 1;
-    const int n_tile = pair % p.ntiles; pair /= p.ntiles;
-    const int m_tile = pair % p.mtiles;
-    const int ksl = pair / p.mtiles;
-    const int it_begin = ksl * p.per_split;
-    const int total = skip ? 0 : max(0, min(p.chunks, it_begin + p.per_split) - it_begin);
-    const int n0 = n_tile * p.nt;                                  // first dY channel of the N tile
-    // this CTA's dY channels: [n0 + rank*h0/2, +h0/2) and [n0 + h0 + rank*h1/2, +h1/2)
-    const int blk0 = p.h0 / 64, blk1 = p.h1 / 64;                   // 32-channel blocks per CTA in each half
-    const uint32_t b_bytes = (uint32_t)(blk0 + blk1) * WP_BLK_BYTES;
-
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < WP_STAGES; ++s) {
-            mbar_init(&full_bar[s], 1);
-            mbar_init(&conv_bar[s], 2 * (4 + 2));                   // one elected lane per converter warp of both CTAs (LEADER's copy)
-            mbar_init(&empty_bar[s], 1);
-        }
-        for (int s = 0; s < WP_ASTAGES; ++s) {
-            mbar_init(&afull_bar[s], 1);
-            mbar_init(&aempty_bar[s], 4);                           // one elected lane per converter warp (this CTA)
-        }
-        mbar_init(&tmem_full_bar, 1);
-        fence_barrier_init();
-    }
-    if (warp == 1) tmem_alloc_2sm<512>(&tmem_base_smem);
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_smem;
-
-    if (warp == 0) {
-        // ------------------------------------------------ TMA producer: this CTA's half of the dY tile ----------------
-        if (lane == 0) {
-            prefetch_tmap(&tmDY);
-            for (int it = 0; it < total; ++it) {
-                const int s = it % WP_STAGES;
-                const uint32_t ph = (it / WP_STAGES) & 1;
-                if (!mbar_wait(&empty_bar[s], ph ^ 1, p.err, 81)) break;
-                const int p0 = (it_begin + it) * WP_BK;
-                uint8_t* st = smem + s * WP_STAGE_BYTES;
-                mbar_expect_tx(&full_bar[s], b_bytes);
-                for (int k = 0; k < blk0; ++k)
-                    tma_load_2d(st + k * WP_BLK_BYTES, &tmDY, &full_bar[s], n0 + (int)rank * (p.h0 / 2) + 32 * k, p0);
-                for (int k = 0; k < blk1; ++k)
-                    tma_load_2d(st + (blk0 + k) * WP_BLK_BYTES, &tmDY, &full_bar[s],
-                                n0 + p.h0 + (int)rank * (p.h1 / 2) + 32 * k, p0);
-            }
-        }
-    } else if (warp == 1) {
-        // ------------------------------------------------ MMA issuer (leader) -----------------------------------------
-        if (leader && lane == 0) {
-            const uint32_t idesc0 = umma_idesc_tf32_bmn(256, p.h0);
-            const uint32_t idesc1 = p.h1 ? umma_idesc_tf32_bmn(256, p.h1) : 0u;
-            bool ok = true;
-            long long t_wait = 0, t_begin = clock64();
-            for (int it = 0; it < total && ok; ++it) {
-                const int s = it % WP_STAGES;
-                const uint32_t ph = (it / WP_STAGES) & 1;
-                const long long c0 = clock64();
-                ok = mbar_wait(&conv_bar[s], ph, p.err, 83);
-                t_wait += clock64() - c0;
-                if (!ok) break;
-                tc_fence_after();
-                const uint32_t b_hi = smem_base + s * WP_STAGE_BYTES, b_lo = b_hi + WP_B_BYTES;
-                const uint32_t a_hi = tmem + WP_ACC_COLS + s * WP_A_COLS, a_lo = a_hi + WP_BK;
-#pragma unroll
-                for (int kk = 0; kk < WP_BK / 8; ++kk) {
-                    {
-                        const uint32_t boff = kk * 1024;
-                        const uint64_t dbh = umma_desc_mn_sw128(b_hi + boff, WP_BLK_BYTES);
-                        const uint64_t dbl = umma_desc_mn_sw128(b_lo + boff, WP_BLK_BYTES);
-                        umma_tf32_ts_2sm(tmem, a_lo + kk * 8, dbh, idesc0, (it | kk) != 0);
-                        umma_tf32_ts_2sm(tmem, a_hi + kk * 8, dbl, idesc0, 1);
-                        umma_tf32_ts_2sm(tmem, a_hi + kk * 8, dbh, idesc0, 1);
-                    }
-                    if (p.h1) {
-                        const uint32_t boff = kk * 1024 + blk0 * WP_BLK_BYTES;
-                        const uint64_t dbh = umma_desc_mn_sw128(b_hi + boff, WP_BLK_BYTES);
-                        const uint64_t dbl = umma_desc_mn_sw128(b_lo + boff, WP_BLK_BYTES);
-                        const uint32_t d = tmem + p.h0;
-                        umma_tf32_ts_2sm(d, a_lo + kk * 8, dbh, idesc1, (it | kk) != 0);
-                        umma_tf32_ts_2sm(d, a_hi + kk * 8, dbl, idesc1, 1);
-                        umma_tf32_ts_2sm(d, a_hi + kk * 8, dbh, idesc1, 1);
-                    }
-                }
-                umma_commit_2sm(&empty_bar[s]);
-            }
-            umma_commit_2sm(&tmem_full_bar);
-            if (p.dbg) { p.dbg[blockIdx.x * 8 + 0] = t_wait; p.dbg[blockIdx.x * 8 + 1] = clock64() - t_begin; }
-        }
-    } else if (warp < 6) {
-        // ------------------------------------------------ A: shifted X rows -> TMEM; then the epilogue ------------------
-        const int q = warp & 3;
-        const uint32_t tq = tmem + ((uint32_t)(q * 32) << 16);
-        const int grow = m_tile * 256 + (int)rank * 128 + q * 32 + lane;      // output row (tap, n)
-        const bool row_ok = grow < p.rows;
-        const int tap = row_ok ? grow / p.Nx : 0;
-        const int shift = (tap - p.taps / 2) * p.dilation;
-        uint8_t* a_ring = smem + WP_STAGES * WP_STAGE_BYTES;
-        bool ok = true;
-        long long t_split = 0, t_empty = 0, t_st = 0;
-        for (int it = 0; it < total && ok; ++it) {
-            const int s = it % WP_STAGES, sa = it % WP_ASTAGES;
-            const uint32_t ph = (it / WP_STAGES) & 1, pha = (it / WP_ASTAGES) & 1;
-            const long long c0 = clock64();
-            ok = mbar_wait(&afull_bar[sa], pha, p.err, 87);              // this chunk's X boxes have landed
-            const float* col = reinterpret_cast<const float*>(a_ring + sa * WP_ATILE_BYTES + q * WP_BLK_BYTES) + lane;
-            const int p0 = (it_begin + it) * WP_BK;
-            int t = p0 % p.T;                                            // time of the chunk's first row in its sample
-            float hi[WP_BK], lo[WP_BK];
-#pragma unroll
-            for (int j = 0; j < WP_BK; ++j) {
-                const int ts = t + shift;
-                float v = col[j * 32];
-                if (!(row_ok && ts >= 0 && ts < p.T)) v = 0.f;           // across a sample edge: the conv's zero padding
-                tf32_split(v, hi[j], lo[j]);
-                if (++t == p.T) t = 0;
-            }
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&aempty_bar[sa]);                 // the ring slot can be refilled
-            const long long c1 = clock64();
-            ok = ok && mbar_wait(&empty_bar[s], ph ^ 1, p.err, 84);      // the MMAs of chunk it-STAGES have left this slot
-            const long long c2 = clock64();
-            t_split += c1 - c0; t_empty += c2 - c1;
-            tc_fence_after();
-            tmem_st32(tq + WP_ACC_COLS + s * WP_A_COLS, hi);
-            tmem_st32(tq + WP_ACC_COLS + s * WP_A_COLS + WP_BK, lo);
-            tmem_st_wait();
-            tc_fence_before();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&conv_bar[s]), 0));
-            t_st += clock64() - c2;
-        }
-        if (p.dbg && warp == 2 && lane == 0) {
-            p.dbg[blockIdx.x * 8 + 2] = t_split; p.dbg[blockIdx.x * 8 + 3] = t_empty; p.dbg[blockIdx.x * 8 + 4] = t_st;
-        }
-        // ---- epilogue: partial tile -> workspace [ks][mtiles*256][Mdy] ----
-        if (!skip) {
-            if (total > 0) mbar_wait(&tmem_full_bar, 0, p.err, 86);
-            tc_fence_after();
-            float* dst = p.P + (((long long)ksl * p.mtiles * 256) + grow) * p.Mdy + n0;
-#pragma unroll 1
-            for (int c = 0; c < p.nt / 32; ++c) {
-                float v[32];
-                if (total > 0) {
-                    tmem_ld32(tq + c * 32, v);
-                    const float comp = acc_trunc_comp(total * (WP_BK / 8) * 3);
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] *= comp;
-                } else {
-#pragma unroll
-                    for (int j = 0; j < 32; ++j) v[j] = 0.f;
-                }
-#pragma unroll
-                for (int j = 0; j < 32; j += 4)
-                    *reinterpret_cast<float4*>(dst + c * 32 + j) = make_float4(v[j], v[j + 1], v[j + 2], v[j + 3]);
-            }
-            tc_fence_before();
-        }
-    } else if (warp < 8) {
-        // ------------------------------------------------ B: lo = dy - trunc_tf32(dy) ---------------------------------
-        const int ct = (warp - 6) * 32 + lane;                           // 0..63
-        const int nvec = (int)(b_bytes / 16);
-        bool ok = true;
-        long long t_full = 0;
-        for (int it = 0; it < total && ok; ++it) {
-            const int s = it % WP_STAGES;
-            const uint32_t ph = (it / WP_STAGES) & 1;
-            const long long c0 = clock64();
-            ok = mbar_wait(&full_bar[s], ph, p.err, 85);
-            t_full += clock64() - c0;
-            const float4* bh = reinterpret_cast<const float4*>(smem + s * WP_STAGE_BYTES);
-            float4* bl = reinterpret_cast<float4*>(smem + s * WP_STAGE_BYTES + WP_B_BYTES);
-#pragma unroll 4
-            for (int idx = ct; idx < nvec; idx += 64) {
-                const float4 v = bh[idx];
-                float4 l;
-                l.x = v.x - __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
-                l.y = v.y - __uint_as_float(__float_as_uint(v.y) & 0xFFFFE000u);
-                l.z = v.z - __uint_as_float(__float_as_uint(v.z) & 0xFFFFE000u);
-                l.w = v.w - __uint_as_float(__float_as_uint(v.w) & 0xFFFFE000u);
-                bl[idx] = l;
-            }
-            fence_proxy_async();
-            __syncwarp();
-            if (lane == 0) mbar_arrive_cluster(mapa_u32(smem_u32(&conv_bar[s]), 0));
-        }
-        if (p.dbg && warp == 6 && lane == 0) p.dbg[blockIdx.x * 8 + 5] = t_full;
-    } else {
-        // ------------------------------------------------ TMA producer of the X ring: 4 boxes (one per converter warp) ---
-        if (lane == 0) {
-            prefetch_tmap(&tmX);
-            uint8_t* a_ring = smem + WP_STAGES * WP_STAGE_BYTES;
-            int nq[4], sh[4];
-#pragma unroll
-            for (int w = 0; w < 4; ++w) {
-                const int wrow = m_tile * 256 + (int)rank * 128 + w * 32;   // first (tap, n) row of converter quarter w
-                const bool okw = wrow < p.rows;                             // Nx % 32 == 0: a quarter never straddles a tap
-                const int tapw = okw ? wrow / p.Nx : 0;
-                nq[w] = okw ? wrow - tapw * p.Nx : -1;
-                sh[w] = (tapw - p.taps / 2) * p.dilation;
-            }
-            for (int it = 0; it < total; ++it) {
-                const int sa = it % WP_ASTAGES;
-                const uint32_t pha = (it / WP_ASTAGES) & 1;
-                if (!mbar_wait(&aempty_bar[sa], pha ^ 1, p.err, 88)) break;
-                const int p0 = (it_begin + it) * WP_BK;
-                uint8_t* dst = a_ring + sa * WP_ATILE_BYTES;
-                mbar_expect_tx(&afull_bar[sa], WP_ATILE_BYTES);
-#pragma unroll
-                for (int w = 0; w < 4; ++w)        // padding quarters read past the end of the tensor: zero-filled
-                    tma_load_2d(dst + w * WP_BLK_BYTES, &tmX, &afull_bar[sa], nq[w] < 0 ? 0 : nq[w], nq[w] < 0 ? p.R : p0 + sh[w]);
-            }
-        }
-    }
-    __syncthreads();
-    cluster_sync_all();
-    if (warp == 1) {
-        tc_fence_after();
-        tmem_dealloc_2sm<512>(tmem);
-    }
-}
 
 // dW[m][n][tap] = sum_ks P[ks][tap*Nx + n][m]   (fixed order => deterministic), n < Ntrue only
 __global__ void wgradp_reduce_kernel(const float* __restrict__ P, float* __restrict__ dW, int taps, int ks, int rows_pad,
@@ -323,7 +82,7 @@ inline bool wgradp_pick_nt(int Mdy, int* nt, int* h0, int* h1) {
 }
 inline bool wgradp_supported(int T, int Mdy, int Nx, int taps) {
     int nt, h0, h1;
-    return T >= WP_BK && Nx % 32 == 0 && Nx >= 32 && taps >= 1 && taps <= 3 && wgradp_pick_nt(Mdy, &nt, &h0, &h1);
+    return T >= HG_BK && Nx % 32 == 0 && Nx >= 32 && taps >= 1 && taps <= 3 && wgradp_pick_nt(Mdy, &nt, &h0, &h1);
 }
 inline WgradPPGeom wgradp_geometry(int B, int T, int Mdy, int Nx, int taps) {
     WgradPPGeom g;
@@ -332,9 +91,9 @@ inline WgradPPGeom wgradp_geometry(int B, int T, int Mdy, int Nx, int taps) {
     g.mtiles = (g.rows + 255) / 256;
     g.ntiles = Mdy / g.nt;
     const long long R = (long long)B * T;
-    g.chunks = (int)((R + WP_BK - 1) / WP_BK);
-    const int tiles = g.mtiles * g.ntiles, pairs = num_sms() / 2;
-    int ks = pairs / tiles;                                  // one wave of CTA pairs
+    g.chunks = (int)((R + HG_BK - 1) / HG_BK);
+    const int tiles = 2 * g.mtiles * ((Mdy + HG_BN - 1) / HG_BN);
+    int ks = num_sms() / tiles;                              // one wave of 128 x 128 tiles
     if (ks < 1) ks = 1;
     if (ks > g.chunks) ks = g.chunks;
     g.per_split = (g.chunks + ks - 1) / ks;
@@ -349,40 +108,28 @@ inline size_t wgradp_workspace_floats(int B, int T, int Mdy, int Nx, int taps) {
 // dY [B,T,Mdy], X [B,T,Nx] channels-last -> dW [Mdy][Ntrue][taps]; ws: wgradp_workspace_floats() floats
 inline int launch_wgrad_pp(const float* dY, const float* X, int B, int T, int Mdy, int Nx, int Ntrue, int taps,
                            int dilation, float* ws, float* dW, int* err, cudaStream_t st) {
+    (void)err;
     const WgradPPGeom g = wgradp_geometry(B, T, Mdy, Nx, taps);
     const long long R = (long long)B * T;
     if (R >= (1ll << 31)) return set_error(2, "%s: too many rows%s", __func__);
-    CUtensorMap tmDY;
-    {
-        uint64_t dims[2] = {(uint64_t)Mdy, (uint64_t)R};
-        uint64_t str[1] = {(uint64_t)Mdy * 4};
-        uint32_t box[2] = {32, 32};
-        if (!make_tmap_f32(&tmDY, dY, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B))
-            return set_error(4, "%s: cuTensorMapEncodeTiled failed%s", __func__);
-    }
-    CUtensorMap tmX;
-    {
-        uint64_t dims[2] = {(uint64_t)Nx, (uint64_t)R};
-        uint64_t str[1] = {(uint64_t)Nx * 4};
-        uint32_t box[2] = {32, 32};
-        if (!make_tmap_f32(&tmX, X, 2, dims, str, box, CU_TENSOR_MAP_SWIZZLE_NONE))
-            return set_error(4, "%s: cuTensorMapEncodeTiled(X) failed%s", __func__);
-    }
-    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(wgrad_pp_kernel), WP_SMEM_BYTES)) return rc;
-    WgradPP p;
-    p.R = (int)R; p.T = T; p.Mdy = Mdy; p.Nx = Nx; p.taps = taps; p.dilation = dilation; p.rows = g.rows;
-    p.mtiles = g.mtiles; p.ntiles = g.ntiles; p.ks = g.ks; p.nt = g.nt; p.h0 = g.h0; p.h1 = g.h1;
-    p.chunks = g.chunks; p.per_split = g.per_split; p.P = ws; p.err = err; p.dbg = g_debug_buf;
-    wgrad_pp_kernel<<<2 * g.mtiles * g.ntiles * g.ks, WP_THREADS, WP_SMEM_BYTES, st>>>(tmDY, tmX, p);
-    ++g_launches;
-    cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", __func__, cudaGetErrorString(e));
-    wgradp_reduce_kernel<<<ew_grid((long long)Mdy * Ntrue * taps), 256, 0, st>>>(ws, dW, taps, g.ks, g.mtiles * 256, Mdy, Nx,
+    WgradPOp o;
+    o.R = (int)R; o.T = T; o.Mdy = Mdy; o.Nx = Nx; o.taps = taps; o.dilation = dilation; o.rows = g.rows;
+    o.per_split = g.per_split; o.chunks = g.chunks; o.dY = dY; o.X = X; o.P = ws; o.rows_pad = g.mtiles * 256;
+    if (int rc = hg_launch(o, dim3((Mdy + HG_BN - 1) / HG_BN, o.rows_pad / HG_BM, g.ks), st, __func__)) return rc;
+    wgradp_reduce_kernel<<<ew_grid((long long)Mdy * Ntrue * taps), 256, 0, st>>>(ws, dW, taps, g.ks, o.rows_pad, Mdy, Nx,
                                                                                 Ntrue);
     ++g_launches;
-    e = cudaGetLastError();
+    cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(3, "%s: reduce launch failed: %s", __func__, cudaGetErrorString(e));
     return 0;
+}
+
+// the entry point that takes max |dy| and max |x| (bm_tc_wgrad_conv_f16): the operands are read as fp32 and split on the
+// engine's 3xTF32 path, so the scales are not needed
+inline int launch_wgrad_hp(const float* dY, const float* dy_amax, const float* X, const float* x_amax, int B, int T, int Mdy,
+                           int Nx, int Ntrue, int taps, int dilation, float* ws, float* dW, int* err, cudaStream_t st) {
+    (void)dy_amax; (void)x_amax;
+    return launch_wgrad_pp(dY, X, B, T, Mdy, Nx, Ntrue, taps, dilation, ws, dW, err, st);
 }
 
 }  // namespace tc

@@ -7,8 +7,8 @@ like the reference which never converts to SyncBatchNorm), then
   * `all_gather_candidates_with_grad`: the same exchange when a trainable feature model produced the candidates --
     its backward is the reduce-scatter(sum) of the candidate gradients;
   * `sync_gradients`: the reference's gradient all-reduce(avg) (flashy.distrib.sync_model, bm/solver.py:386),
-    done on one flat bucket AFTER the backward pass: the backward's kernels are persistent and own every SM, so an NCCL
-    kernel overlapped with them would push CTA pairs into a second round (see the candidate gather below), costing more
+    done on one flat bucket AFTER the backward pass: the backward's kernels fill every SM, so an NCCL
+    kernel overlapped with them would push CTAs into a second round (see the candidate gather below), costing more
     than the ~0.3 ms the 36-80 MB all-reduce takes on its own.
 """
 from __future__ import annotations
@@ -122,10 +122,10 @@ def all_gather_candidates_with_grad(candidate: torch.Tensor, uniform: bool = Fal
 # ---------------------------------------------------------------------------------------------------------------------
 # Candidate all-gather over NVLink peer memory, driven by the COPY ENGINES (no SMs)
 # ---------------------------------------------------------------------------------------------------------------------
-# The conv / weight-gradient / CLIP kernels are persistent: one CTA (pair) per SM, all registers and shared memory of the
-# SM.  An NCCL all-gather kernel that runs beside them for milliseconds (3 GB at N = 8) takes a handful of SMs for that
-# whole time, and every persistent launch in that window finds fewer SMs than CTA pairs: the leftover pairs wait for a
-# whole pair to finish its tiles -- a second round, up to 2x per kernel.  So the gather is done without SMs: every rank
+# The conv / weight-gradient / CLIP kernels run one CTA per SM (all of the SM's shared memory) in waves sized to the SM
+# count.  An NCCL all-gather kernel that runs beside them for milliseconds (3 GB at N = 8) takes a handful of SMs for that
+# whole time, and every launch in that window finds fewer SMs than it was sized for: the leftover CTAs wait for a
+# whole CTA to finish its tile -- a second round, up to 2x per kernel.  So the gather is done without SMs: every rank
 # copies its block into a symmetric-memory buffer (torch.distributed._symmetric_memory: cuMem allocations mapped into
 # every peer), and after a barrier PULLS the other ranks' blocks with cudaMemcpyAsync device-to-device copies, which the
 # copy engines execute over NVLink.  A second barrier tells the owners that their buffer may be overwritten by the next

@@ -5,7 +5,7 @@ autograd node: its backward launches the hand-written gradient kernels in revers
 leaves ordinary dense `.grad` tensors on every parameter (what bm/solver.py:384-387 and
 flashy.distrib.sync_model expect).  `clip_loss` / `clip_scores` are ClipLoss (bm/losses.py:77-114).
 
-Kernel selection is by shape only: contractions whose channel counts fit the tcgen05 tiling (K % 32 == 0 and an
+Kernel selection is by shape only: contractions whose channel counts fit the tensor-core tiling (K % 32 == 0 and an
 N tile of 64..160 dividing N -- every layer of the real clip_conv model) run on the tensor-core kernels
 (3xTF32, `bm_tc_*`); other shapes (the tiny unit-test models) run on the FP32-FMA kernels of the same library.
 """
@@ -59,7 +59,7 @@ _status: tp.Dict[torch.device, torch.Tensor] = {}
 
 
 def tc_status_tensor(device) -> torch.Tensor:
-    """Device int32 word the tcgen05 kernels set if their bounded pipeline waits ever time out."""
+    """Device int32 word the tensor-core kernels set if their bounded pipeline waits ever time out."""
     device = torch.device(device)
     if device not in _status:
         _status[device] = torch.zeros(1, dtype=torch.int32, device=device)
@@ -76,11 +76,11 @@ def check_tc_status(device=None) -> None:
                 raise IndexError(f"a subject / recording index is outside the weight sets of the per-sample 1x1 layer on {dev} "
                                  "(bm/models/common.py:57 raises there too)")
             if code != 0:
-                raise _lib.BmB200Error(f"a tcgen05 kernel reported a pipeline timeout (barrier code {code}) on {dev}")
+                raise _lib.BmB200Error(f"a tensor-core kernel reported a pipeline timeout (barrier code {code}) on {dev}")
 
 
 OVERLAP_WGRAD = True   # weight-gradient kernels on a side stream, concurrent with the data-gradient kernels of the layer
-USE_CONV_PP = True     # persistent CTA-pair kernel (tc_convp.cuh, tcgen05 cta_group::2) where its tiling fits
+USE_CONV_PP = True     # raw-weight conv entry point (tc_convp.cuh) where its shape gate fits
 
 
 _side_streams: tp.Dict[torch.device, torch.cuda.Stream] = {}
@@ -97,15 +97,18 @@ def _round_up(n, m):
     return (n + m - 1) // m * m
 
 
-USE_CONV_F16 = True    # the persistent conv on the F16 tensor pipe (tc_convh.cuh: fp16 hi/lo pieces, twice the MMA rate of 3xTF32)
-USE_WGRAD_F16 = True   # ... and the CTA-pair weight gradient (tc_wgradh.cuh)
-USE_WGRAD_PP = True    # CTA-pair weight-gradient kernel (tc_wgradp.cuh) where its 256-row tiling wastes < 10 %
+# The fp16-piece entry points (bm_tc_conv1d_f16, bm_tc_wgrad_conv_f16: operands as fp16 hi/lo pieces of power-of-two-scaled
+# tensors, with their amax) compute on the same 3xTF32 engine as the fp32 ones, so on this GPU they would only add the amax
+# passes and the fp16 weight preparation to every step: off by default, kept switchable for the ABI's callers.
+USE_CONV_F16 = False
+USE_WGRAD_F16 = False
+USE_WGRAD_PP = True    # all-taps weight-gradient GEMM (tc_wgradp.cuh) where its 256-row padding wastes < 10 %
 
 
 def tc_wgrad(dy, x, B, T, M, N, Ntrue, kw, dilation, status, dbias=None, dy_amax=None, x_amax=None):
     """dw[m][n][tap] = sum_{b,t} dy[b,t,m] x[b,t+(tap-kw//2)*dilation,n] on the tensor cores -> [M, Ntrue, kw];
-    `dbias` [M] (optional) receives sum_{b,t} dy[b,t,m].  `dy_amax` / `x_amax` (F16 pipe): device floats with max |dy| /
-    max |x| when their producers reported them, else a bm_amax pass here."""
+    `dbias` [M] (optional) receives sum_{b,t} dy[b,t,m].  `dy_amax` / `x_amax` (USE_WGRAD_F16 only): device floats with
+    max |dy| / max |x| when their producers reported them, else a bm_amax pass here."""
     lib = _lib.load()
     dw = _empty((M, Ntrue, kw), dy)
     rows = kw * N                                       # output rows of the pair kernel, tiled in blocks of 256
@@ -170,7 +173,7 @@ class _Conv:
         st = stream()
         lib = _lib.load()
         g = 1 if glu else 0
-        # persistent CTA-pair kernel (csrc/tc_convp.cuh) where its tiling fits, else the single-CTA tensor-core kernel,
+        # raw-weight entry point (csrc/tc_convp.cuh) where its shape gate fits, else the pre-split one (tc_conv.cuh),
         # else FP32 FMA
         self.fwd_pp = allow_tc and USE_CONV_PP and bool(lib.bm_tc_conv1d_persistent_supported(T, self.cin, self.cout, self.kw, g))
         self.bwd_pp = allow_tc and USE_CONV_PP and bool(lib.bm_tc_conv1d_persistent_supported(T, self.cout, self.cin, self.kw, 0))

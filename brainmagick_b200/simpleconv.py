@@ -3,7 +3,7 @@
 Same constructor signature, submodule/parameter names (=> interchangeable `state_dict`), construction order
 (=> identical parameters for a given `torch.manual_seed`), `forward(inputs, batch) -> [B, F, T]`, train/eval
 semantics (BatchNorm running statistics, one spatial-dropout centre per training forward).  The arithmetic runs in
-hand-written sm_100a CUDA through the C ABI (`functional.encoder_forward`); there is no PyTorch/CPU fallback.
+hand-written sm_90a CUDA through the C ABI (`functional.encoder_forward`); there is no PyTorch/CPU fallback.
 
 Accelerated configuration = the `clip_conv` family of conf/model/clip_conv.yaml (merger + initial_linear +
 subject_layers + ConvSequence(batch_norm) + head), with or without `skip`, with any `glu` period, with GELU or
@@ -27,7 +27,7 @@ from .common import ChannelMerger, ConvSequence, ScaledEmbedding, SubjectLayers,
 
 def _require_cuda(meg: torch.Tensor) -> None:
     if not meg.is_cuda:
-        raise RuntimeError("brainmagick_b200.SimpleConv runs on CUDA (sm_100a) only; there is no CPU fallback")
+        raise RuntimeError("brainmagick_b200.SimpleConv runs on CUDA (sm_90a) only; there is no CPU fallback")
 
 
 class SimpleConv(nn.Module):

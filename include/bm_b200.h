@@ -1,4 +1,4 @@
-/* brainmagick_b200 -- C ABI of the B200-native contrastive training step (SimpleConv + ClipLoss).
+/* brainmagick_b200 -- C ABI of the H100-native (sm_90a) contrastive training step (SimpleConv + ClipLoss).
  *
  * The reference (facebookresearch/brainmagick) has no FFI: its boundary for this path is the Python object
  * surface of `bm.models.SimpleConv` (bm/models/simpleconv.py:22-249) and `bm.losses.ClipLoss`
@@ -28,12 +28,11 @@ const char* bm_last_error(void);
 int bm_abi_version(void);
 /* number of CUDA kernels this library has launched since it was loaded (bench.py's `gpu_launches`). */
 unsigned long long bm_launch_count(void);
-/* experiment switches (returns the previous value).  By default bm_tc_wgrad keeps X raw in shared memory as the tf32
- * `hi` operand (the tensor core ignores the 13 low mantissa bits) and only writes `lo = x - trunc(x)`; bit 0 restores
- * the explicit round-to-nearest hi/lo split (one third more shared-memory traffic). */
+/* experiment switches (returns the previous value).  No switch is defined: every kernel ignores the flags (kept for
+ * ABI compatibility). */
 int bm_set_debug_flags(int flags);
-/* profiling aid (process-wide, NOT part of the product path): device buffer of >= 8 * gridDim long longs that the CTA-pair
- * weight-gradient kernel fills with per-CTA cycle counters (barrier waits per warp role); NULL (default) disables it. */
+/* profiling aid (process-wide, NOT part of the product path): device buffer for per-CTA cycle counters; the current
+ * kernels record none.  NULL (default). */
 int bm_set_debug_buffer(long long* buf);
 
 /* ---- K1: spatial-attention weights, once per recording ------------------------------------------------
@@ -149,11 +148,10 @@ int bm_head_bwd_params(const float* dest, const float* x, const float* h1, const
  * bm_clip_scores = ClipLoss.get_scores (+ get_probabilities when probs != NULL):
  *   inv_norm[o] = 1/(1e-8+||cand_o||), scores[b,o] = inv_norm[o] <est_b, cand_o>, probs = softmax_o(scores).
  *   norms_given = 1: inv_norm is an INPUT (a fixed candidate set is normed once, see bm_candidate_inv_norms).
- * One split-K tcgen05 GEMM on CTA pairs (3xTF32; every accumulation chain is bounded to 64 K-steps and drained into an
- * fp32 round-to-nearest running sum, because the tensor core's accumulator truncates) that also produces the candidate
- * norms, + one finalize kernel (slice reduction in a fixed order, norm scale, row softmax / cross-entropy / batch mean).
+ * One split-K wgmma GEMM (3xTF32; every 32-wide K block is accumulated into an fp32 round-to-nearest running sum,
+ * because the tensor core's accumulator truncates), a row sum of squares for the candidate norms, + one finalize kernel (slice reduction in a fixed order, norm scale, row softmax / cross-entropy / batch mean).
  * workspace: bm_clip_workspace(Bn,Bc,KT) floats of caller-owned scratch, 8-byte aligned; status: device int set on a
- * pipeline timeout (never hangs).  KT % 4 != 0 (no TMA row pitch) falls to the FP32-FMA GEMM of this library. */
+ * kernel failure (reserved; never hangs).  KT % 4 != 0 (no 16-byte row pitch) falls to the FP32-FMA GEMM of this library. */
 long long bm_clip_workspace(int Bn, int Bc, long long KT);
 int bm_clip_scores(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given, float* inv_norm,
                    float* scores, float* probs, float* workspace, long long workspace_floats, int* status,
@@ -233,9 +231,9 @@ int bm_reject_compact(const unsigned int* peak_bits, const unsigned char* mask, 
                       int B, unsigned char* keep, int* keep_rows, int* n_keep, bm_stream_t stream);
 int bm_gather_rows(const float* x, const int* rows, int n_rows, long long row_elems, float* y, bm_stream_t stream);
 
-/* ---- tcgen05 (5th-gen tensor core) versions of K3/K4: 3xTF32 implicit-GEMM conv ---------------------------
+/* ---- tensor-core (wgmma) versions of K3/K4: 3xTF32 implicit-GEMM conv ------------------------------------
  * Same arithmetic contract as bm_conv1d_fwd / bm_conv1d_bwd_data / bm_conv1d_glu_fwd (fp32-faithful: every
- * product is hi*hi + lo*hi + hi*lo of tf32 splits, fp32 accumulation in tensor memory).
+ * product is hi*hi + lo*hi + hi*lo of tf32 splits, fp32 accumulation per 32-wide K block).
  * bm_tc_weight_split: w [Cout,Cin,Kw] -> forward operand f_hi/f_lo [Kw,Cout,Cin] and data-gradient operand
  * g_hi/g_lo [Kw,Cin,Cout] (either pair may be NULL).
  * bm_tc_conv1d: x [B,T,Cin], w_hi/w_lo [Kw,Ntot,Cin]; sign=+1 forward taps, -1 data gradient; glu=1: Ntot = 2H,
@@ -252,24 +250,23 @@ int bm_tc_conv1d(const float* x, const float* w_hi, const float* w_lo, const flo
  * channel-major `estimate`).  With Kw=1 this is the pointwise (1x1) contraction of the head (K5).
  * bm_col_stats: stats[0:C] = sum_r y[r,c], stats[C:2C] = sum_r y[r,c]^2 (fp64), the BatchNorm batch statistics. */
 int bm_col_stats(const float* y, long long rows, int C, double* stats, bm_stream_t stream);
-/* PERSISTENT CTA-pair kernel (csrc/tc_convp.cuh): one CTA pair per SM pair loops over 256-row tiles of the flattened
- * rows b*T + t (taps that would cross a sample edge read zeros = the conv padding), epilogue warps drain tile i while the
- * operands of tile i+1 are staged.  w_raw: RAW fp32 weights re-laid K-major [Kw][Ntot][Cin] (bm_tc_weight_split with
- * f_lo / g_lo = NULL) -- the tensor core's truncation of the raw operand is the tf32 `hi`, the kernel derives `lo`.
- * accumulate=1: y += conv(x) in place (the skip-path gradient; TMA reduce-add).  glu / act / out_tmajor / aux / glu_out as
+/* csrc/tc_convp.cuh: the same conv from the RAW fp32 weights re-laid K-major [Kw][Ntot][Cin] (bm_tc_weight_split with
+ * f_lo / g_lo = NULL); the kernel splits them into tf32 pieces itself (taps that would cross a sample edge read zeros =
+ * the conv padding).  accumulate=1: y += conv(x) in place (the skip-path gradient).  glu / act / out_tmajor / aux / glu_out as
  * bm_tc_conv1d.  stats (nullable; plain forward only): BatchNorm batch statistics stats[0:Ntot] = sum(y), stats[Ntot:2Ntot]
- * = sum(y^2) (fp64, zeroed by the call) accumulated in shared memory across the CTA's tiles -- replaces bm_col_stats.
+ * = sum(y^2) (fp64, zeroed by the call) reduced per tile in shared memory -- replaces bm_col_stats.
  * Shape gate (bm_tc_conv1d_persistent_supported): Cin % 32 == 0 and Ntot % 320 == 0 or Ntot % 256 == 0 (GLU: halves). */
 int bm_tc_conv1d_persistent_supported(int T, int Cin, int Ntot, int Kw, int glu);
 int bm_tc_conv1d_persistent(const float* x, const float* w_raw, const float* bias, int accumulate, int B, int T, int Cin,
                             int Ntot, int Kw, int dilation, int sign, int glu, int act, int out_tmajor, float* y,
                             float* aux, float* glu_out, double* stats, int* status, bm_stream_t stream);
 
-/* The same conv on the F16 tensor pipe (csrc/tc_convh.cuh; replaces the same reference lines as bm_tc_conv1d_persistent:
- * nn.Conv1d / GLU in bm/models/common.py:107-151, the head's 1x1 convs simpleconv.py:153-168).  Each fp32 operand is
- * carried as two fp16 pieces (11 + 11 significant bits, like the two tf32 pieces) of the tensor times a power of two that
- * puts its largest magnitude in [2^14, 2^15): three kind::f16 MMAs per product cost half the tensor-pipe time of three
- * kind::tf32 MMAs.  bm_amax: amax[0] = max |x[i]| (device float; one HBM pass).  bm_f16_split: hi/lo = fp16 pieces of
+/* The same conv with the weights as fp16 pieces (csrc/tc_convh.cuh; replaces the same reference lines as
+ * bm_tc_conv1d_persistent: nn.Conv1d / GLU in bm/models/common.py:107-151, the head's 1x1 convs simpleconv.py:153-168).
+ * The weights are carried as two fp16 pieces (11 + 11 significant bits) of the tensor times a power of two that puts its
+ * largest magnitude in [2^14, 2^15); the kernel sums the pieces back (hi + lo: ~22 significant bits of the weight, the
+ * precision of the pieces) and runs the same 3xTF32 GEMM (x_amax is accepted and not needed).  bm_amax: amax[0] =
+ * max |x[i]| (device float; one HBM pass).  bm_f16_split: hi/lo = fp16 pieces of
  * src * scale(amax[0]) in the same element order (the weights, once per step, from bm_tc_weight_split's raw K-major
  * re-layout).  bm_tc_conv1d_f16: arguments as bm_tc_conv1d_persistent with (w_hi, w_lo, w_amax) in place of w_raw and
  * x_amax = the device float bm_amax wrote for x; same shape gate. */
@@ -290,22 +287,21 @@ int bm_tc_conv1d_f16(const float* x, const float* x_amax, const void* w_hi, cons
  * for n < Ntrue (x may be channel-padded to N); dy [B,T,M], x [B,T,N] channels-last; dw in nn.Conv1d layout
  * [M][Ntrue][Kw].  workspace: bm_tc_wgrad_workspace() floats (per-batch-slice partial tiles, reduced in a fixed
  * order => deterministic).  dbias (nullable) [M] receives the bias gradient sum_{b,t} dy[b,t,m], accumulated from the dy
- * values the kernel already holds in registers.  bm_col_sum: out[c] = sum_r x[r,c] (other bias gradients). */
+ * values (one column-sum pass).  bm_col_sum: out[c] = sum_r x[r,c] (other bias gradients). */
 int bm_tc_wgrad_supported(int M, int N);
 long long bm_tc_wgrad_workspace(int B, int M, int N, int Kw);
 int bm_tc_wgrad(const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw, int dilation,
                 float* workspace, float* dw, float* dbias, int* status, bm_stream_t stream);
-/* bm_tc_wgrad_conv: the same weight gradient on CTA PAIRS (csrc/tc_wgradp.cuh): ONE GEMM whose output rows are the
- * (tap, x-channel) pairs (3 x 320 = 960 rows in 4 pair-tiles instead of 3 x 384 padded rows), reduced over the flattened
- * rows b*T + t in exact chunks of 32 (the tap shift is applied to the x side; a shifted row across a sample edge reads 0),
- * each CTA holding half of the dy tile.  No dbias output.  T >= 32; M % 64 == 0; N % 4 == 0. */
+/* bm_tc_wgrad_conv: the same weight gradient as ONE GEMM (csrc/tc_wgradp.cuh) whose output rows are the (tap, x-channel)
+ * pairs, reduced over the flattened rows b*T + t in exact chunks of 32 (the tap shift is applied to the x side; a shifted
+ * row across a sample edge reads 0).  No dbias output.  T >= 32; M % 64 == 0; N % 4 == 0. */
 int bm_tc_wgrad_conv_supported(int T, int M, int N, int Kw);
 long long bm_tc_wgrad_conv_workspace(int B, int T, int M, int N, int Kw);
 int bm_tc_wgrad_conv(const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw, int dilation,
                      float* workspace, float* dw, int* status, bm_stream_t stream);
-/* bm_tc_wgrad_conv_f16: the same on the F16 pipe (csrc/tc_wgradh.cuh; see bm_tc_conv1d_f16 for the arithmetic): both
- * operands as fp16 hi/lo pieces of the tensors scaled by powers of two from dy_amax / x_amax (device floats: bm_amax or a
- * producer's amax_out); the dY tile is transposed to K-major rows while it is split.  Same gate and workspace. */
+/* bm_tc_wgrad_conv_f16: the same for callers that hold dy_amax / x_amax (device floats: bm_amax or a producer's
+ * amax_out); the result is bm_tc_wgrad_conv's (the amax values are not needed by the 3xTF32 arithmetic).  Same gate and
+ * workspace. */
 int bm_tc_wgrad_conv_f16(const float* dy, const float* dy_amax, const float* x, const float* x_amax, int B, int T, int M,
                          int N, int Ntrue, int Kw, int dilation, float* workspace, float* dw, int* status,
                          bm_stream_t stream);

@@ -3,6 +3,7 @@
 inputs, in this build container (the reference tree does not travel to the GPU box; the fixtures do).
 
     python oracle/make_golden.py            # rewrites tests/golden/
+    python oracle/make_golden.py --check    # regenerates into a temporary directory and compares with tests/golden/
 
 Each fixture holds: the configuration, the reference state_dict (`p.<key>`), the inputs, and the reference's
 outputs: estimate, scores, loss, probabilities, every parameter gradient (`g.<key>`), and BN running stats after
@@ -318,9 +319,34 @@ def run_ablation(name, change):
     print(f"{name}: loss={loss.item():.6f} est.std={est.std().item():.4f} params={sum(v.numel() for v in state.values())}")
 
 
-if __name__ == "__main__":
-    torch.set_num_threads(1)
-    wanted = sys.argv[1:]
+def check(wanted):
+    """Regenerates the fixtures into a temporary directory and compares them with the committed ones: the committed
+    fixtures must be exactly what this generator produces from the reference today.  Returns the names that differ."""
+    import tempfile
+    global OUT
+    committed_dir, bad = OUT, []
+    with tempfile.TemporaryDirectory() as tmp:
+        OUT = tmp
+        try:
+            generate(wanted)
+        finally:
+            OUT = committed_dir
+        for f in sorted(os.listdir(tmp)):
+            fresh, committed = np.load(os.path.join(tmp, f)), np.load(os.path.join(committed_dir, f))
+            same = sorted(fresh.files) == sorted(committed.files)
+            for k in committed.files if same else []:
+                a, b = fresh[k], committed[k]
+                if a.shape != b.shape or not (np.allclose(a, b, rtol=1e-5, atol=1e-7, equal_nan=True)
+                                              if a.dtype.kind == "f" else np.array_equal(a, b)):
+                    same = False
+                    break
+            print(f"{f}: {'same' if same else 'DIFFERS'}")
+            if not same:
+                bad.append(f)
+    return bad
+
+
+def generate(wanted):
     for name, c in CASES.items():
         if not wanted or name in wanted:
             run_case(name, c)
@@ -334,3 +360,11 @@ if __name__ == "__main__":
     for name, change in ABLATIONS.items():
         if not wanted or name in wanted:
             run_ablation(name, change)
+
+
+if __name__ == "__main__":
+    torch.set_num_threads(1)
+    args = sys.argv[1:]
+    if args[:1] == ["--check"]:
+        sys.exit(1 if check(args[1:]) else 0)
+    generate(args)

@@ -1,8 +1,8 @@
 """TEST INFRASTRUCTURE ONLY -- loads the *verbatim* brainmagick hot-path modules from /root/reference (build container) or
-from the unmodified copy staged under baseline/_ref/ by oracle/stage_reference.py (GPU box; `bench.py --impl reference`).
+from the unmodified copy build() stages under oracle/_ref/ (oracle/stage_reference.py; `bench.py --impl reference`).
 
-Used by `oracle/make_golden.py` (fixture generation) and by `tests/test_oracle_vs_reference.py`
-(which skips when /root/reference is absent, i.e. on the GPU box).  `load_reference_norm()` adds the verbatim
+Used by the fixture generators (`oracle/make_golden.py`, incl. its `--check`, and `oracle/make_live_golden.py`); the
+tests read what they stored and use only `clip_conv_kwargs`; they never load the reference.  `load_reference_norm()` adds the verbatim
 `bm/norm.py`; `bm/models/features.py` (DeepMel) is loaded by the generator the same way.  Nothing in the product package
 (`brainmagick_b200/`) imports this file.
 
@@ -19,11 +19,11 @@ import types
 
 import numpy as np
 
-_STAGED = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "baseline", "_ref")
+_STAGED = os.path.join(os.path.dirname(os.path.abspath(__file__)), "_ref")
 
 
 def _find_root() -> str:
-    """/root/reference in the build container; on the GPU box the copy staged by oracle/stage_reference.py."""
+    """The reference source tree where present, else the copy build() staged under oracle/_ref (oracle/stage_reference.py)."""
     env = os.environ.get("BM_REFERENCE_ROOT")
     if env:
         return env
@@ -34,7 +34,7 @@ def _find_root() -> str:
 
 REF_ROOT = _find_root()
 REF = os.path.join(REF_ROOT, "bm")
-REF_KIND = "source tree" if REF_ROOT == "/root/reference" else "staged copy (baseline/_ref)"
+REF_KIND = "source tree" if REF_ROOT == "/root/reference" else "staged copy (oracle/_ref)"
 
 
 def reference_available() -> bool:

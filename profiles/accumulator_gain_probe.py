@@ -1,4 +1,7 @@
-"""Measures whether the tensor-core accumulation error of the 3xTF32 kernels is a systematic GAIN (the fp32 accumulator truncates\ntoward zero on every tcgen05.mma addition) or noise: for each kernel, total relative error vs fp64, the fitted gain <y,ref>/<ref,ref>-1\nand the residual once the gain is removed.      python profiles/accumulator_gain_probe.py"""
+"""Measures whether the tensor-core accumulation error of the 3xTF32 kernels is a systematic GAIN (the tensor core's fp32
+accumulation truncates; the engine adds every 32-wide K block into a round-to-nearest fp32 sum to bound it) or noise: for each
+kernel, total relative error vs fp64, the fitted gain <y,ref>/<ref,ref>-1 and the residual once the gain is removed.
+    python profiles/accumulator_gain_probe.py"""
 import sys, os, torch
 sys.path.insert(0, os.getcwd())
 from brainmagick_b200 import _lib
@@ -27,15 +30,14 @@ for (B,T,Cin,Cout,Kw,label) in [(8,360,320,320,3,"K3 fwd n_adds=360"),(8,360,640
         torch.cuda.synchronize()
         ref=torch.nn.functional.conv1d(x.double().permute(0,2,1), w.double(), None, padding=Kw//2).permute(0,2,1)
         probe(label+" "+dist, y, ref)
-# the same conv on the F16 pipe (fp16 pieces), compensation switched off (debug flag 2): gain per tcgen05.mma addition
+# the same conv through the fp16-piece entry point
 lib=_lib.load()
 def f16_ops(x, f):
     amax=torch.empty(2,device=dev)
     call("bm_amax", ptr(x), x.numel(), ptr(amax[0:1]), stream()); call("bm_amax", ptr(f), f.numel(), ptr(amax[1:2]), stream())
     hi=torch.empty(f.shape,device=dev,dtype=torch.float16); lo=torch.empty(f.shape,device=dev,dtype=torch.float16)
     call("bm_f16_split", ptr(f), f.numel(), ptr(amax[1:2]), ptr(hi), ptr(lo), stream()); return amax,hi,lo
-for flags,tag in ((2,"uncompensated"),(0,"compensated")):
-    lib.bm_set_debug_flags(flags)
+for tag in ("fp16-piece weights",):
     for (B,T,Cin,Cout,Kw,label) in [(8,360,320,320,3,"f16 K=960 n_adds=180"),(8,360,640,320,3,"f16 K=1920 n_adds=360"),(8,360,320,640,1,"f16 1x1 K=320 n_adds=60"),(8,360,1024,640,1,"f16 1x1 K=1024 n_adds=192")]:
         for dist in ("randn","gelu-like"):
             x=torch.randn(B,T,Cin,device=dev)
@@ -48,7 +50,6 @@ for flags,tag in ((2,"uncompensated"),(0,"compensated")):
             torch.cuda.synchronize()
             ref=torch.nn.functional.conv1d(x.double().permute(0,2,1), w.double(), None, padding=Kw//2).permute(0,2,1)
             probe(tag+" "+label+" "+dist, y, ref)
-lib.bm_set_debug_flags(0)
 # wgrad pair
 B,T,M,N,Kw=64,360,320,320,3
 dy=torch.randn(B,T,M,device=dev); x=torch.randn(B,T,N,device=dev)

@@ -1,6 +1,6 @@
 """Micro-benchmarks of the SURVEY 8(f) rows built after the training step (batch preparation, retrieval evaluation,
 DeepMel feature model), each beside a bounded CPU sample of its oracle.  Not the headline metric (that is bench.py);
-run on one B200 as a leg of bench.py (the oracle imports below are that leg's `cpu_baseline`):
+run on one GPU as a leg of bench.py (the oracle imports below are that leg's `cpu_baseline`):
 
     python bench.py --next-rows                   # writes gpurun_out/next_rows.json and prints it
 

@@ -1,6 +1,6 @@
 #!/bin/bash
-# SASS evidence that the hot kernels use tcgen05 / TMA: per kernel, the count of each tensor-core / TMA / TMEM mnemonic in
-# the built library.   bash profiles/sass_listing.sh > profiles/r2_sass_mnemonics.txt
+# SASS evidence that the hot kernels use the tensor cores: per kernel, the count of each tensor-core / memory mnemonic in
+# the built library (wgmma appears as HGMMA).   bash profiles/sass_listing.sh
 cuobjdump -sass brainmagick_b200/libbm_b200.so 2>/dev/null | awk '
 /Function :/ {name=$3}
 /UTCHMMA|UTCQMMA|UTMALDG|UTMASTG|UTMAREDG|UTMAPF|UTCBAR|LDTM|STTM|UTCCP|ELECT/ {

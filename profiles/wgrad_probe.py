@@ -1,4 +1,4 @@
-"""Where does the CTA-pair weight-gradient kernel wait?  Three launch patterns at the K3 shape (B=256, T=360, 320x320, k3 d4):
+"""How does the all-taps weight-gradient kernel behave?  Three launch patterns at the K3 shape (B=256, T=360, 320x320, k3 d4):
 isolated launches after an L2 flush, back-to-back launches on the same operands, back-to-back over rotating operand sets
 (> L2), each with the kernel's cycle counters (bm_set_debug_buffer).   python profiles/wgrad_probe.py"""
 import os

@@ -2,7 +2,7 @@
 
 Purpose: the host side (which entry points are called, with which buffers, leading dimensions, strides and in which order,
 and where each gradient ends up) is Python that changes between GPU sessions.  The CUDA kernels behind the entry points
-below are verified on a B200 (`-m gpu` tests) but new COMPOSITIONS of them cannot be when no GPU is at hand.  This module
+below are verified on an H100 (`-m gpu` tests) but new COMPOSITIONS of them cannot be when no GPU is at hand.  This module
 implements each entry point's documented contract with torch CPU ops on the very buffers the host code passes, so the whole
 drop-in can be run here against the verbatim-reference fixtures:
   * the fixtures the GPU path is known to pass must also pass on the emulator (that validates the emulator's reading of the

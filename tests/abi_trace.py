@@ -19,7 +19,7 @@ sys.path.insert(0, ROOT)
 
 
 CONFIGS = {   # B, C, T, F, S, hidden, merger_channels, initial_linear, pos_dim
-    "full": (4, 208, 360, 1024, 27, 320, 270, 270, 2048),       # BASELINE widths: every contraction on tcgen05
+    "full": (4, 208, 360, 1024, 27, 320, 270, 270, 2048),       # BASELINE widths: every contraction on the tensor cores
     "mid": (8, 40, 130, 128, 3, 160, 48, 24, 128),              # mixed tensor-core / FP32-FMA kernels
     "small": (6, 10, 24, 8, 3, 16, 12, 12, 32),                 # the fixtures' size: FP32-FMA kernels only
 }

@@ -14,7 +14,7 @@ GOLDEN_CASES = ["train_small", "eval_small", "train_padded_negs", "train_depth4"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):

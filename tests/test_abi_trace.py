@@ -5,7 +5,27 @@ import pytest
 import abi_trace
 
 
-def test_full_size_step_runs_on_tensor_cores_only():
+@pytest.fixture
+def f16_pieces(monkeypatch):
+    """The fp16-piece host path (functional.USE_CONV_F16 / USE_WGRAD_F16, off by default) switched on."""
+    from brainmagick_b200 import functional
+    monkeypatch.setattr(functional, "USE_CONV_F16", True)
+    monkeypatch.setattr(functional, "USE_WGRAD_F16", True)
+
+
+def test_default_step_prepares_no_fp16_pieces():
+    """By default the step runs the fp32 entry points: no amax pass, no fp16 operand preparation, one weight re-layout
+    launch per prepared weight set (the forward and data-gradient operands of a layer in the same launch)."""
+    calls = abi_trace.simpleconv_step(abi_trace.CONFIGS["full"], True)
+    names = [c[0] for c in calls]
+    assert {"bm_tc_conv1d_persistent", "bm_tc_wgrad_conv", "bm_tc_pointwise_sel", "bm_tc_wgrad_grouped"} <= set(names)
+    assert not set(names) & {"bm_amax", "bm_f16_split", "bm_tc_weight_split_f16", "bm_tc_conv1d_f16", "bm_tc_wgrad_conv_f16"}
+    assert names.count("bm_tc_conv1d_persistent") >= 30 and names.count("bm_tc_weight_split") >= 17
+    producers = [c for c in calls if c[0] in ("bm_bn_gelu_skip_fwd", "bm_bn_gelu_skip_bwd", "bm_glu_bwd")]
+    assert producers and all(c[-2] is False for c in producers)          # amax_out == NULL: no max |output| reductions
+
+
+def test_full_size_step_runs_on_tensor_cores_only(f16_pieces):
     """At the BASELINE widths no FP32-FMA contraction is left in the step."""
     names = {c[0] for c in abi_trace.simpleconv_step(abi_trace.CONFIGS["full"], True)}
     assert not names & {"bm_conv1d_fwd", "bm_conv1d_bwd_data", "bm_conv1d_bwd_weight", "bm_conv1d_glu_fwd", "bm_head_fwd",
@@ -66,7 +86,7 @@ def test_group_layout_matches_bincount_without_a_sync():
             assert (idx[order.long()[off[s]:off[s + 1]]] == s).all()
 
 
-def test_weight_preparation_is_two_launches_per_layer():
+def test_weight_preparation_is_two_launches_per_layer(f16_pieces):
     """F16 pipe: per conv layer and step, one bm_amax over the nn.Conv1d weight and ONE re-layout-and-split launch."""
     calls = abi_trace.simpleconv_step(abi_trace.CONFIGS["full"], True)
     names = [c[0] for c in calls]

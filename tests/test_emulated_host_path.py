@@ -199,7 +199,7 @@ def test_batch_preparation_host_path_on_the_emulator(clip, excl):
 
 
 @pytest.mark.parametrize("shape", [
-    # the "tcgen05-eligible widths" case of tests/test_gpu_parity.py (mixed tensor-core / FMA kernels)
+    # the "tensor-core-eligible widths" case of tests/test_gpu_parity.py (mixed tensor-core / FMA kernels)
     dict(B=8, C=40, T=130, F=128, S=3, hidden=160, MC=48, IL=24, P=128, n_valid=()),
     # BASELINE widths (every contraction through a tensor-core entry point), short and narrow in batch/time only
     dict(B=3, C=208, T=48, F=1024, S=4, hidden=320, MC=270, IL=270, P=2048, n_valid=(208, 150, 208, 97)),

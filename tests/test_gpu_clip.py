@@ -1,4 +1,4 @@
-"""GPU: the ClipLoss kernels (csrc/tc_clip.cuh: split-K CTA-pair score GEMM with bounded accumulation chains + fused
+"""GPU: the ClipLoss kernels (csrc/tc_clip.cuh: split-K score GEMM with per-K-block fp32 accumulation + fused
 finalize) against fp64 references (torch, test-only) of bm/losses.py:77-114, through the C ABI.
 
 The case that matters most is the SAME-SIGNED one: the tensor core's fp32 accumulator truncates, so a long accumulation of

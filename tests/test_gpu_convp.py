@@ -1,5 +1,5 @@
-"""GPU: the persistent CTA-pair conv kernels -- 3xTF32 (csrc/tc_convp.cuh, bm_tc_conv1d_persistent) and the fp16-pieces
-variant on the F16 pipe (csrc/tc_convh.cuh, bm_tc_conv1d_f16) -- in every epilogue mode against torch's fp64 conv (test-only
+"""GPU: the conv entry points -- fp32 weights (csrc/tc_convp.cuh, bm_tc_conv1d_persistent) and fp16-piece weights
+(csrc/tc_convh.cuh, bm_tc_conv1d_f16), both on the 3xTF32 wgmma engine -- in every epilogue mode against torch's fp64 conv (test-only
 reference), at the real layer shapes, incl. the flattened-row tiling across sample edges (odd batch sizes, T not a multiple
 of anything) and the BatchNorm statistics out of the epilogue."""
 import pytest
@@ -73,7 +73,7 @@ def _run(x, w_op, bias, accumulate, B, T, Cin, Ntot, Kw, dil, sign, glu, act, tm
         call("bm_tc_conv1d_persistent", ptr(x), ptr(w_op), ptr(bias), accumulate, B, T, Cin, Ntot, Kw, dil, sign, glu, act,
              tmajor, ptr(y), ptr(aux), ptr(glu_out), ptr(stats), ptr(status), stream())
     torch.cuda.synchronize()
-    assert int(status.item()) == 0, f"tcgen05 pipeline timed out at barrier code {int(status.item())}"
+    assert int(status.item()) == 0, f"tensor-core kernel timed out at barrier code {int(status.item())}"
 
 
 @pytest.mark.parametrize("xs,ws,spread", [(1e-6, 1e-3, 0), (3e4, 50.0, 0), (1.0, 1.0, 12), (1e-30, 1e30, 6)])
@@ -281,7 +281,7 @@ def test_speed_report(capsys):
                 times.append(e0.elapsed_time(e1))
         ms = sum(times) / len(times)
         lines.append(f"[{name}] {ms:.4f} ms/launch = {flops / ms / 1e9:.1f} algorithmic TFLOP/s (min {min(times):.4f} ms)")
-    # time = fixed + rounds * per-tile: T = 256 makes one 256-row tile per sample, so B = 74 k gives k tiles per CTA pair
+    # time = fixed + per-tile work: T = 256 makes two 128-row tiles per sample, so the tile count grows linearly with B
     Tt = 256
     xs = torch.randn(370, Tt, C, device=DEV)
     ys = torch.empty(370, Tt, C, device=DEV)

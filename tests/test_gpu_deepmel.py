@@ -78,7 +78,7 @@ def _oracle_step(spec, params, mel, est, training=True):
 
 
 @pytest.mark.parametrize("cfg", [
-    # tcgen05-eligible widths (N tiles of 160 / 256 / 320), mel channels padded 40 -> 64; input gradient requested
+    # tensor-core-eligible widths (N tiles of 160 / 256 / 320), mel channels padded 40 -> 64; input gradient requested
     dict(n_in=40, hidden=160, layers=4, out=320, B=4, T=72, act=None),
     dict(n_in=64, hidden=256, layers=3, out=256, B=3, T=130, act="gelu"),
 ])

@@ -86,7 +86,7 @@ def test_drop_in_matches_reference_golden(name):
 @pytest.mark.parametrize("shape", [
     dict(B=16, C=64, T=120, F=40, S=4, hidden=64, MC=48, IL=56, P=288, n_valid=()),          # cfg1-like (mock, 64 sensors)
     dict(B=12, C=37, T=91, F=33, S=5, hidden=40, MC=30, IL=34, P=128, n_valid=(37, 20, 11)),   # ragged / padded
-    dict(B=8, C=40, T=130, F=128, S=3, hidden=160, MC=48, IL=24, P=128, n_valid=()),           # tcgen05-eligible widths
+    dict(B=8, C=40, T=130, F=128, S=3, hidden=160, MC=48, IL=24, P=128, n_valid=()),           # tensor-core-eligible widths
 ])
 @pytest.mark.parametrize("train", [True, False])
 def test_drop_in_matches_oracle(shape, train):
@@ -188,7 +188,7 @@ def test_baseline_shapes_match_oracle(case):
 
 @pytest.mark.parametrize("Bn,Bc", [(256, 256), (64, 512), (100, 256)])
 def test_clip_tensor_core_shapes_match_oracle(Bn, Bc):
-    """ClipLoss at tcgen05-eligible candidate counts (B' % 256 == 0, F*T % 320 == 0), incl. ragged row counts and the
+    """ClipLoss at tensor-core-eligible candidate counts (B' % 256 == 0, F*T % 320 == 0), incl. ragged row counts and the
     multi-GPU target offset, against the CPU oracle (F*T kept small so the oracle is instant)."""
     import brainmagick_b200.functional as BF
     from oracle import bm_oracle

@@ -235,7 +235,7 @@ def _retrieval_task(n, m, F, T, n_words, signal, seed):
 
 
 def test_retrieval_tensor_core_path():
-    """Candidate axis padded to the tcgen05 tile (1000 -> 1024), K = F*T = 2048: scores against the oracle, the fused
+    """Candidate axis padded to the tensor-core tile (1000 -> 1024), K = F*T = 2048: scores against the oracle, the fused
     top-k against torch.topk on the very same scores, accuracies against the oracle's."""
     trues, seg, preds, labels, _ = _retrieval_task(n=300, m=1000, F=16, T=128, n_words=0 + 1, signal=0.06, seed=11)
     clip = ClipLoss().eval()

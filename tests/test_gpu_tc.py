@@ -1,4 +1,4 @@
-"""GPU: the tcgen05 (3xTF32) conv kernels against the FP32-FMA kernels of the same library and against torch's
+"""GPU: the tensor-core (3xTF32) conv kernels against the FP32-FMA kernels of the same library and against torch's
 fp64 conv (test-only reference), at the real layer shapes.  Tolerance 3e-5 relative to fp64: the 3xTF32 scheme
 must stay fp32-faithful, inside the 1e-4 parity bar (measured ~1e-5 at K=1920: the tensor-core fp32 accumulator
 truncates, so the error grows with the accumulation length)."""
@@ -27,8 +27,8 @@ _FN = {1: "bm_tc_conv1d"}
 
 
 def _gen_flags(gen):
-    """generation 1 = single-CTA kernel (still used with per-sample weight sets); the persistent CTA-pair kernel has its own
-    file, tests/test_gpu_convp.py."""
+    """generation 1 = the pre-split-weight entry point (bm_tc_conv1d, still used with per-sample weight sets); the raw-weight
+    entry point has its own file, tests/test_gpu_convp.py."""
     from brainmagick_b200 import _lib
     _lib.load().bm_set_debug_flags(0)
 
@@ -60,7 +60,7 @@ def test_tc_conv_forward(dilation, T, gen):
     call(_FN[gen], ptr(x), ptr(fh), ptr(fl), ptr(bias), None, B, T, Cin, Cout, Kw, dilation, 1, 0, 0, 0, ptr(y), None, None,
          None, ptr(status), stream())
     torch.cuda.synchronize()
-    assert int(status.item()) == 0, f"tcgen05 pipeline timed out at barrier code {int(status.item())}"
+    assert int(status.item()) == 0, f"tensor-core kernel timed out at barrier code {int(status.item())}"
     ref = _ref_conv(x, w, bias, dilation)
     err = rel_err(y.cpu(), ref.cpu())
     print(f'[tc gen{gen} fwd d={dilation} T={T}] rel_err vs fp64 = {err:.2e}')
@@ -143,6 +143,8 @@ def test_tc_conv_speed_report(capsys, gen):
         print(f"\n[tc gen{gen} conv 320->320 k3 B=256 T=360] {ms:.3f} ms/launch = {tf:.1f} algorithmic TFLOP/s")
 
 
+# `trunc` sets bm_set_debug_flags, which the ABI still accepts and no kernel reads any more: both settings must give the
+# same, correct result.
 @pytest.mark.parametrize("trunc", [0, 1])
 @pytest.mark.parametrize("case", [
     dict(B=5, T=360, M=320, N=320, Kw=3, dil=1),
@@ -167,7 +169,7 @@ def test_tc_wgrad(case, trunc):
     torch.cuda.synchronize()
     _lib.load().bm_set_debug_flags(0)
     assert rel_err(db.cpu(), dy.double().sum(dim=(0, 1)).cpu()) < 1e-5
-    assert int(status.item()) == 0, f"tcgen05 pipeline timed out at barrier code {int(status.item())}"
+    assert int(status.item()) == 0, f"tensor-core kernel timed out at barrier code {int(status.item())}"
     # fp64 reference: dw[m,n,j] = sum_{b,t} dy[b,t,m] x[b,t+(j-Kw//2)*dil,n]
     ref = torch.zeros(M, N, Kw, dtype=torch.float64, device=dev)
     xd, dyd = x.double(), dy.double()
@@ -219,8 +221,8 @@ def test_tc_wgrad_speed_report(capsys, trunc):
 ])
 @pytest.mark.parametrize("pipe", ["tf32", "f16"])
 def test_tc_wgrad_pair_kernel(case, pipe):
-    """bm_tc_wgrad_conv (csrc/tc_wgradp.cuh) and bm_tc_wgrad_conv_f16 (csrc/tc_wgradh.cuh): rows = (tap, x channel), flattened
-    reduction, CTA pairs."""
+    """bm_tc_wgrad_conv and bm_tc_wgrad_conv_f16 (the entry point that also takes the operands' amax; csrc/tc_wgradp.cuh):
+    rows = (tap, x channel), flattened reduction."""
     call, ptr, stream = _call()
     from brainmagick_b200 import _lib
     torch.manual_seed(11)
@@ -246,7 +248,7 @@ def test_tc_wgrad_pair_kernel(case, pipe):
             call("bm_tc_wgrad_conv", ptr(dy), ptr(x), B, T, M, N, N, Kw, dil, ptr(ws), ptr(out), ptr(status), stream())
     run(dw)
     torch.cuda.synchronize()
-    assert int(status.item()) == 0, f"tcgen05 pipeline timed out at barrier code {int(status.item())}"
+    assert int(status.item()) == 0, f"tensor-core kernel timed out at barrier code {int(status.item())}"
     ref = torch.zeros(M, N, Kw, dtype=torch.float64, device=dev)
     xd, dyd = x.double(), dy.double()
     for j in range(Kw):
