@@ -25,9 +25,9 @@ struct ClipOp {
     long long KT;
     float* P;                   // [ks][Bn][Bc]
     struct Cta { int m0, n0, c0, c1; };
-    __device__ Cta cta() const {
+    template <int BN> __device__ Cta cta() const {
         Cta c;
-        c.n0 = blockIdx.x * HG_BN;
+        c.n0 = blockIdx.x * BN;
         c.m0 = blockIdx.y * HG_BM;
         c.c0 = blockIdx.z * per_split;
         c.c1 = min(chunks, c.c0 + per_split);
@@ -46,9 +46,9 @@ struct ClipOp {
         if (n >= Bc || k >= KT) return make_float4(0.f, 0.f, 0.f, 0.f);
         return __ldg(reinterpret_cast<const float4*>(C + n * KT + k));
     }
-    __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+    template <int BN> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
         HgStore s{P + (long long)blockIdx.z * Bn * Bc, Bc, Bn, Bc};
-        s.store(acc, c.m0 + m0, c.n0);
+        s.store<BN>(acc, c.m0 + m0, c.n0);
     }
 };
 
@@ -185,7 +185,7 @@ inline int launch_clip_scores(const float* est, const float* cand, int Bn, int B
     }
     ClipOp o;
     o.E = est; o.C = cand; o.Bn = Bn; o.Bc = Bc; o.chunks = g.chunks; o.per_split = g.per_split; o.KT = KT; o.P = ws;
-    if (int rc = hg_launch(o, dim3((Bc + HG_BN - 1) / HG_BN, (Bn + HG_BM - 1) / HG_BM, g.ks), st, __func__)) return rc;
+    if (int rc = hg_launch<HG_BN>(o, dim3((Bc + HG_BN - 1) / HG_BN, (Bn + HG_BM - 1) / HG_BM, g.ks), st, __func__)) return rc;
     clip_finalize_kernel<<<Bn, 256, 0, st>>>(ws, ssp, g.ks, Bn, Bc, target_offset, inv_norm, scores, probs, row_loss,
                                              loss, counter);
     ++g_launches;

@@ -6,12 +6,13 @@
 // addressing (tap shifts with per-sample zero padding, position-major weight-gradient operands, K slices) and its own fused
 // epilogue without a copy of the pipeline.
 //
-// One CTA = two warpgroups = one 128 x 128 output tile (warpgroup g owns rows [64 g, 64 g + 64)).  Per K block of 32:
+// One CTA = two warpgroups = one 128 x BN output tile (warpgroup g owns rows [64 g, 64 g + 64)); BN = 128, or for the weight
+// gradients 160 where the output width asks for it (hg_pick_bn).  Per K block of 32:
 //   * every thread loads its share of the A and B tiles from global memory into registers one block AHEAD (the loads of
 //     block kb+1 are in flight while the tensor cores work on block kb), splits each fp32 value x into tf32 pieces
 //     hi = rna_tf32(x), lo = x - hi, and writes hi and lo into the 128-byte-swizzled K-major layout wgmma reads;
 //     operands whose contiguous dimension is M/N (the position-major weight gradients) are transposed on that store;
-//   * 4 x 3 wgmma.m64n128k8.f32.tf32 per warpgroup: lo*hi + hi*lo + hi*hi (the lo*lo term is below fp32 resolution);
+//   * 4 x 3 wgmma.m64nBNk8.f32.tf32 per warpgroup: lo*hi + hi*lo + hi*hi (the lo*lo term is below fp32 resolution);
 //   * the block's products are accumulated in a fresh register tile and then added into the running fp32 sum with
 //     ordinary round-to-nearest FADDs.  The tensor core's internal accumulation truncates; chaining at most 12 MMAs per
 //     block keeps that bias below 1e-7 relative however long K is, with no correction factor to calibrate per GPU.
@@ -100,22 +101,62 @@ __device__ __forceinline__ void wgmma_tf32_m64n128(float* d, uint64_t adesc, uin
         : "l"(adesc), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
+// the same with N = 160
+__device__ __forceinline__ void wgmma_tf32_m64n160(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %82, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n160k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
+        "%80, %81, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]),
+          "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]),
+          "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+    static_assert(BN == 128 || BN == 160, "engine tile widths: 128, 160");
+    if constexpr (BN == 128) wgmma_tf32_m64n128(d, adesc, bdesc, accumulate);
+    else wgmma_tf32_m64n160(d, adesc, bdesc, accumulate);
+}
 
 // ---------------------------------------------------------------------------------------------------
 // the GEMM engine
 // ---------------------------------------------------------------------------------------------------
 constexpr int HG_BM = 128, HG_BN = 128, HG_BK = 32, HG_THREADS = 256;
 constexpr int HG_TILE_BYTES = 128 * HG_BK * 4;                        // 16 KB: 128 rows x 32 fp32
-constexpr int HG_STAGE_BYTES = 4 * HG_TILE_BYTES;                     // A hi | A lo | B hi | B lo
-constexpr int HG_SMEM_BYTES = 2 * HG_STAGE_BYTES + 1024;              // double-buffered, 1 KB alignment slack
+// one stage: A hi | A lo (128 rows each) | B hi | B lo (BN rows each); double-buffered, 1 KB alignment slack
+template <int BN> constexpr int hg_stage_bytes() { return 2 * HG_TILE_BYTES + 2 * BN * HG_BK * 4; }
+template <int BN> constexpr int hg_smem_bytes() { return 2 * hg_stage_bytes<BN>() + 1024; }
 
-// Operand fetch, per 128-row tile and K block (ops implement a4 / b4 with the signature below):
+// The tile width for an output of n columns: 160 where it pads no more columns than 128 (320 columns: 2 exact tiles instead
+// of 3 with 64 padding columns), else 128.
+inline int hg_pick_bn(long long n) {
+    const long long p128 = (n + 127) / 128 * 128, p160 = (n + 159) / 160 * 160;
+    return p160 <= p128 ? 160 : 128;
+}
+
+// Operand fetch, per tile of ROWS rows (128 for A, BN for B) and K block (ops implement a4 / b4 with the signature below):
 //   K-contiguous operand (Op::A_KCONTIG / B_KCONTIG):  v4(cta, kb, row, q) = elements k = 4q .. 4q+3 of tile row `row`
 //   M/N-contiguous operand:                            v4(cta, kb, k, q)   = tile rows 4q .. 4q+3 at reduction index k
 // Out-of-range elements (padding, tails, other samples) are returned as zeros.
-template <bool KCONTIG>
+template <bool KCONTIG, int ROWS>
 struct HgSlot {
-    // the 4 float4 this thread moves per 128 x 32 tile: (i, q) = (row, k quad) or (k, row quad)
+    static constexpr int N4 = ROWS / 32;       // float4 moved per thread per tile
+    // the N4 float4 this thread moves per ROWS x 32 tile: (i, q) = (row, k quad) or (k, row quad)
     __device__ static void coords(int tid, int j, int& i, int& q) {
         const int idx = tid + HG_THREADS * j;
         if (KCONTIG) { i = idx >> 3; q = idx & 7; }
@@ -147,7 +188,8 @@ struct HgSlot {
     }
 };
 
-// Accumulator fragment of warpgroup g (m64n128): element i of thread (warp w of the group, lane) is
+// Accumulator fragment of warpgroup g (m64nBN, BN / 2 elements per thread): element i of thread (warp w of the group,
+// lane) is
 //   row 64 g + 16 w + lane/4 + 8 ((i >> 1) & 1),  column 8 (i >> 2) + 2 (lane & 3) + (i & 1)
 __device__ __forceinline__ int hg_row(int i) {
     const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
@@ -155,43 +197,52 @@ __device__ __forceinline__ int hg_row(int i) {
 }
 __device__ __forceinline__ int hg_col(int i) { return 8 * (i >> 2) + 2 * (threadIdx.x & 3) + (i & 1); }
 
-template <class Op>
+template <class Op, int BN>
 __global__ void __launch_bounds__(HG_THREADS, 1) hg_gemm_kernel(const __grid_constant__ Op op) {
+    constexpr int NACC = BN / 2, STAGE = hg_stage_bytes<BN>(), B_TILE = BN * HG_BK * 4;
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
     const int tid = threadIdx.x, wg = tid >> 7;
-    using SA = HgSlot<Op::A_KCONTIG>;
-    using SB = HgSlot<Op::B_KCONTIG>;
+    using SA = HgSlot<Op::A_KCONTIG, HG_BM>;
+    using SB = HgSlot<Op::B_KCONTIG, BN>;
 
-    const typename Op::Cta cta = op.cta();
+    const typename Op::Cta cta = op.template cta<BN>();
     const int nkb = op.kblocks(cta);
-    float4 ra[4], rb[4];
+    float4 ra[SA::N4], rb[SB::N4];
     auto fetch = [&](int kb) {
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
+        for (int j = 0; j < SA::N4; ++j) {
             int i, q;
             SA::coords(tid, j, i, q);
             ra[j] = op.a4(cta, kb, i, q);
+        }
+#pragma unroll
+        for (int j = 0; j < SB::N4; ++j) {
+            int i, q;
             SB::coords(tid, j, i, q);
             rb[j] = op.b4(cta, kb, i, q);
         }
     };
     auto stash = [&](int s) {
-        uint8_t* st = smem + s * HG_STAGE_BYTES;
+        uint8_t* st = smem + s * STAGE;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
+        for (int j = 0; j < SA::N4; ++j) {
             int i, q;
             SA::coords(tid, j, i, q);
             SA::store(st, st + HG_TILE_BYTES, i, q, ra[j]);
+        }
+#pragma unroll
+        for (int j = 0; j < SB::N4; ++j) {
+            int i, q;
             SB::coords(tid, j, i, q);
-            SB::store(st + 2 * HG_TILE_BYTES, st + 3 * HG_TILE_BYTES, i, q, rb[j]);
+            SB::store(st + 2 * HG_TILE_BYTES, st + 2 * HG_TILE_BYTES + B_TILE, i, q, rb[j]);
         }
     };
 
-    float acc[64], part[64];
+    float acc[NACC], part[NACC];
 #pragma unroll
-    for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+    for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
     if (nkb > 0) {
         fetch(0);
         stash(0);
@@ -201,40 +252,45 @@ __global__ void __launch_bounds__(HG_THREADS, 1) hg_gemm_kernel(const __grid_con
     for (int kb = 0; kb < nkb; ++kb) {
         const int s = kb & 1;
         if (kb + 1 < nkb) fetch(kb + 1);
-        const uint32_t st = base_u32 + s * HG_STAGE_BYTES;
+        const uint32_t st = base_u32 + s * STAGE;
         const uint32_t a_hi = st + wg * (HG_TILE_BYTES / 2), a_lo = a_hi + HG_TILE_BYTES;
-        const uint32_t b_hi = st + 2 * HG_TILE_BYTES, b_lo = b_hi + HG_TILE_BYTES;
+        const uint32_t b_hi = st + 2 * HG_TILE_BYTES, b_lo = b_hi + B_TILE;
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < HG_BK / 8; ++kk) {
             const uint32_t off = kk * 32;                  // 8 tf32 = 32 bytes along K inside the swizzle span
             const uint64_t dah = wgmma_desc_k_sw128(a_hi + off), dal = wgmma_desc_k_sw128(a_lo + off);
             const uint64_t dbh = wgmma_desc_k_sw128(b_hi + off), dbl = wgmma_desc_k_sw128(b_lo + off);
-            wgmma_tf32_m64n128(part, dal, dbh, kk != 0);
-            wgmma_tf32_m64n128(part, dah, dbl, 1);
-            wgmma_tf32_m64n128(part, dah, dbh, 1);
+            wgmma_tf32<BN>(part, dal, dbh, kk != 0);
+            wgmma_tf32<BN>(part, dah, dbl, 1);
+            wgmma_tf32<BN>(part, dah, dbh, 1);
         }
         wgmma_commit();
         if (kb + 1 < nkb) stash(s ^ 1);                    // the other stage's MMAs completed in the previous iteration
         wgmma_wait_all();
 #pragma unroll
-        for (int i = 0; i < 64; ++i) acc[i] += part[i];
+        for (int i = 0; i < NACC; ++i) acc[i] += part[i];
         fence_proxy_async();
         __syncthreads();
     }
-    op.epilogue(cta, acc, 64 * wg);
+    op.template epilogue<BN>(cta, acc, 64 * wg);
 }
 
-template <class Op>
+template <int BN, class Op>
 inline int hg_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) {
-    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hg_gemm_kernel<Op>), HG_SMEM_BYTES)) return rc;
+    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hg_gemm_kernel<Op, BN>), hg_smem_bytes<BN>())) return rc;
     if (grid.x == 0 || grid.y == 0 || grid.z == 0) return 0;
     if (grid.y > 65535 || grid.z > 65535) return set_error(2, "%s: grid too large%s", who);
-    hg_gemm_kernel<Op><<<grid, HG_THREADS, HG_SMEM_BYTES, st>>>(op);
+    hg_gemm_kernel<Op, BN><<<grid, HG_THREADS, hg_smem_bytes<BN>(), st>>>(op);
     ++g_launches;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", who, cudaGetErrorString(e));
     return 0;
+}
+// the same with the tile width of hg_pick_bn
+template <class Op>
+inline int hg_launch_bn(int bn, const Op& op, dim3 grid, cudaStream_t st, const char* who) {
+    return bn == 160 ? hg_launch<160>(op, grid, st, who) : hg_launch<128>(op, grid, st, who);
 }
 
 // the plain epilogue: D[z plane][row][col] = acc for rows < rows, cols < cols (row-major, leading dimension ld)
@@ -242,9 +298,10 @@ struct HgStore {
     float* D;
     long long ld;
     int rows, cols;
+    template <int BN>
     __device__ void store(const float* acc, int m0, int n0) const {
 #pragma unroll
-        for (int i = 0; i < 64; i += 2) {
+        for (int i = 0; i < BN / 2; i += 2) {
             const int r = m0 + hg_row(i), c = n0 + hg_col(i);
             if (r >= rows) continue;
             float* d = D + (long long)r * ld + c;

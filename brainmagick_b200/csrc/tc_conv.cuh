@@ -58,7 +58,10 @@ struct ConvOp {
     int* err;
 
     struct Cta { int b, t0, n_tile, wbase; float w_inv; };
-    __device__ Cta cta() const {
+    // 128 columns: with the engine's current main loop (every thread stages its operands through registers), 160-wide
+    // tiles run the 320-wide conv slower than 128-wide ones although they skip the 64 padding columns
+    template <int BN> __device__ Cta cta() const {
+        static_assert(BN == HG_BN, "ConvOp tiles are 128 columns wide");
         Cta c;
         c.b = blockIdx.x / ttiles;
         c.t0 = (blockIdx.x - c.b * ttiles) * HG_BM;
@@ -107,7 +110,7 @@ struct ConvOp {
         return make_float4((h0.x + l0.x) * c.w_inv, (h0.y + l0.y) * c.w_inv, (h1.x + l1.x) * c.w_inv, (h1.y + l1.y) * c.w_inv);
     }
 
-    __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+    template <int BN> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
         __shared__ double col_sums[2 * HG_BN];
         float am = 0.f;
         if (glu) {
@@ -200,7 +203,7 @@ inline int launch_conv_op(ConvOp o, cudaStream_t st, const char* who) {
         cudaError_t em = cudaMemsetAsync(o.stats, 0, sizeof(double) * 2 * o.Ntot, st);
         if (em != cudaSuccess) return set_error(3, "%s: memset: %s", who, cudaGetErrorString(em));
     }
-    return hg_launch(o, dim3((unsigned)ctas, (unsigned)ntiles, 1), st, who);
+    return hg_launch<HG_BN>(o, dim3((unsigned)ctas, (unsigned)ntiles, 1), st, who);
 }
 
 // W[o][i][j] (nn.Conv1d layout) -> tf32-split K-major operands:

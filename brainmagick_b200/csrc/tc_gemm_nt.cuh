@@ -15,7 +15,7 @@ struct GemmNTOp {
     const float* A; const float* B; float* D;
     int M, N, K;
     struct Cta { int m0, n0; };
-    __device__ Cta cta() const { return Cta{(int)blockIdx.y * HG_BM, (int)blockIdx.x * HG_BN}; }
+    template <int BN> __device__ Cta cta() const { return Cta{(int)blockIdx.y * HG_BM, (int)blockIdx.x * BN}; }
     __device__ int kblocks(const Cta&) const { return (K + HG_BK - 1) / HG_BK; }
     __device__ float4 a4(const Cta& c, int kb, int r, int q) const {
         const int m = c.m0 + r, k = kb * HG_BK + 4 * q;
@@ -27,9 +27,9 @@ struct GemmNTOp {
         if (kk >= K || n >= N) return make_float4(0.f, 0.f, 0.f, 0.f);
         return __ldg(reinterpret_cast<const float4*>(B + (long long)kk * N + n));
     }
-    __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+    template <int BN> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
         HgStore s{D, N, M, N};
-        s.store(acc, c.m0 + m0, c.n0);
+        s.store<BN>(acc, c.m0 + m0, c.n0);
     }
 };
 
@@ -41,7 +41,7 @@ inline bool gemm_nt_pp_supported(int M, int N, int K) {
 inline int launch_gemm_nt_pp(const float* A, const float* B, float* D, int M, int N, int K, int* err, cudaStream_t st) {
     (void)err;
     GemmNTOp o{A, B, D, M, N, K};
-    return hg_launch(o, dim3((N + HG_BN - 1) / HG_BN, (M + HG_BM - 1) / HG_BM, 1), st, __func__);
+    return hg_launch<HG_BN>(o, dim3((N + HG_BN - 1) / HG_BN, (M + HG_BM - 1) / HG_BM, 1), st, __func__);
 }
 
 }  // namespace tc

@@ -42,7 +42,8 @@ inline bool wgrad_tc_supported(int M, int N) { return wgrad_pick_nh(N) != 0 && M
 inline void wgrad_geometry(int B, int M, int N, int taps, int* nh, int* mblocks, int* ksplit, int* bchunk) {
     *nh = wgrad_pick_nh(N);
     *mblocks = (M + WG_BM - 1) / WG_BM;
-    int tiles = (*mblocks) * ((N + HG_BN - 1) / HG_BN) * taps;
+    const int bn = hg_pick_bn(N);
+    int tiles = (*mblocks) * ((N + bn - 1) / bn) * taps;
     int want = num_sms() / tiles;                 // floor: the whole grid must fit in ONE wave (1 CTA per SM)
     if (want < 1) want = 1;
     if (want > B) want = B;
@@ -69,11 +70,11 @@ struct WgradOp {
     int ksplit;
 
     struct Cta { int tap, shift, m0, n0, ks, b_begin, b_end, tchunks; };
-    __device__ Cta cta() const {
+    template <int BN> __device__ Cta cta() const {
         Cta c;
         c.tap = blockIdx.x / ntiles;
         c.shift = (c.tap - taps / 2) * dilation;
-        c.n0 = (blockIdx.x - c.tap * ntiles) * HG_BN;
+        c.n0 = (blockIdx.x - c.tap * ntiles) * BN;
         c.m0 = blockIdx.y * HG_BM;
         c.ks = blockIdx.z;
         c.b_begin = seg_off ? seg_off[c.ks] : c.ks * bchunk;
@@ -96,9 +97,9 @@ struct WgradOp {
         if (t >= T || ts < 0 || ts >= T || n >= N) return make_float4(0.f, 0.f, 0.f, 0.f);
         return __ldg(reinterpret_cast<const float4*>(X + ((long long)sample(c, kb) * T + ts) * N + n));
     }
-    __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+    template <int BN> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
         HgStore s{P + ((long long)c.tap * ksplit + c.ks) * plane, N, rows, N};
-        s.store(acc, c.m0 + m0, c.n0);
+        s.store<BN>(acc, c.m0 + m0, c.n0);
     }
 };
 
@@ -112,12 +113,13 @@ inline int launch_wgrad_tc(const float* dY, const float* X, int B, int T, int M,
     const int Mpad = mblocks * WG_BM;
     const bool direct = taps == 1 && ksplit == 1 && Ntrue == N;
     WgradOp o;
-    o.B = B; o.T = T; o.M = M; o.N = N; o.taps = taps; o.dilation = dilation; o.ntiles = (N + HG_BN - 1) / HG_BN;
+    const int bn = hg_pick_bn(N);
+    o.B = B; o.T = T; o.M = M; o.N = N; o.taps = taps; o.dilation = dilation; o.ntiles = (N + bn - 1) / bn;
     o.bchunk = bchunk; o.zlist = nullptr; o.seg_off = nullptr; o.dY = dY; o.X = X; o.ksplit = ksplit;
     o.P = direct ? dW : ws;
     o.plane = (long long)(direct ? M : Mpad) * N;
     o.rows = direct ? M : Mpad;
-    if (int rc = hg_launch(o, dim3(o.ntiles * taps, mblocks, ksplit), st, __func__)) return rc;
+    if (int rc = hg_launch_bn(bn, o, dim3(o.ntiles * taps, mblocks, ksplit), st, __func__)) return rc;
     if (dbias) {               // bias gradient sum_{b,t} dY[b,t,m]
         cudaError_t em = cudaMemsetAsync(dbias, 0, sizeof(float) * M, st);
         if (em != cudaSuccess) return set_error(3, "%s: memset: %s", __func__, cudaGetErrorString(em));
@@ -147,7 +149,9 @@ inline int launch_wgrad_tc_grouped(const float* dY, const float* X, const int* z
     o.B = B; o.T = T; o.M = M; o.N = N; o.taps = 1; o.dilation = 1; o.ntiles = (N + HG_BN - 1) / HG_BN;
     o.bchunk = 0; o.zlist = zlist; o.seg_off = seg_off; o.dY = dY; o.X = X; o.ksplit = G;
     o.P = out; o.plane = (long long)mblocks * WG_BM * N; o.rows = mblocks * WG_BM;
-    return hg_launch(o, dim3(o.ntiles, mblocks, G), st, __func__);
+    // 128 columns: one CTA per (tile, group) and no K-slice count to raise, so fewer, wider tiles fill the waves worse
+    // (27 groups of 320 x 320: 162 CTAs at 160, a second wave of 30 on 132 SMs, ran slower than 243 at 128)
+    return hg_launch<HG_BN>(o, dim3(o.ntiles, mblocks, G), st, __func__);
 }
 
 }  // namespace tc

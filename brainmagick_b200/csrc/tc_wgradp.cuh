@@ -7,7 +7,7 @@
 //     G[(tap, n)][m] = sum_p Xs[p, (tap, n)] * dY[p, m],     Xs[p, (tap, n)] = X[p + shift(tap), n] (0 across a sample edge)
 //
 // so the taps share one tile grid (3 x 320 rows = 7.5 tiles of 128 instead of 3 x 3) and the reduction runs over the
-// flattened rows in exact blocks of 32.  One CTA = one (128-row tile, 128-column tile, K slice); partial tiles go to the
+// flattened rows in exact blocks of 32.  One CTA = one (128-row tile, 128- or 160-column tile, K slice); partial tiles go to the
 // workspace and `wgradp_reduce_kernel` sums the K slices in a fixed order (deterministic) while scattering into the
 // nn.Conv1d layout [m][n][tap].
 #pragma once
@@ -24,9 +24,9 @@ struct WgradPOp {
     int rows_pad;
 
     struct Cta { int m0, n0, c0, c1; };
-    __device__ Cta cta() const {
+    template <int BN> __device__ Cta cta() const {
         Cta c;
-        c.n0 = blockIdx.x * HG_BN;
+        c.n0 = blockIdx.x * BN;
         c.m0 = blockIdx.y * HG_BM;
         c.c0 = blockIdx.z * per_split;
         c.c1 = min(chunks, c.c0 + per_split);
@@ -46,9 +46,9 @@ struct WgradPOp {
         if (m >= Mdy || p >= R) return make_float4(0.f, 0.f, 0.f, 0.f);
         return __ldg(reinterpret_cast<const float4*>(dY + (long long)p * Mdy + m));
     }
-    __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+    template <int BN> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
         HgStore s{P + (long long)blockIdx.z * rows_pad * Mdy, Mdy, rows_pad, Mdy};
-        s.store(acc, c.m0 + m0, c.n0);
+        s.store<BN>(acc, c.m0 + m0, c.n0);
     }
 };
 
@@ -70,7 +70,7 @@ __global__ void wgradp_reduce_kernel(const float* __restrict__ P, float* __restr
     }
 }
 
-struct WgradPPGeom { int nt, h0, h1, mtiles, ntiles, ks, chunks, per_split, rows; };
+struct WgradPPGeom { int nt, h0, h1, mtiles, ntiles, ks, chunks, per_split, rows, bn; };
 
 inline bool wgradp_pick_nt(int Mdy, int* nt, int* h0, int* h1) {
     if (Mdy % 320 == 0) { *nt = 320; *h0 = 192; *h1 = 128; return true; }
@@ -92,8 +92,9 @@ inline WgradPPGeom wgradp_geometry(int B, int T, int Mdy, int Nx, int taps) {
     g.ntiles = Mdy / g.nt;
     const long long R = (long long)B * T;
     g.chunks = (int)((R + HG_BK - 1) / HG_BK);
-    const int tiles = 2 * g.mtiles * ((Mdy + HG_BN - 1) / HG_BN);
-    int ks = num_sms() / tiles;                              // one wave of 128 x 128 tiles
+    g.bn = hg_pick_bn(Mdy);
+    const int tiles = 2 * g.mtiles * ((Mdy + g.bn - 1) / g.bn);
+    int ks = num_sms() / tiles;                              // one wave of 128 x bn tiles
     if (ks < 1) ks = 1;
     if (ks > g.chunks) ks = g.chunks;
     g.per_split = (g.chunks + ks - 1) / ks;
@@ -115,7 +116,8 @@ inline int launch_wgrad_pp(const float* dY, const float* X, int B, int T, int Md
     WgradPOp o;
     o.R = (int)R; o.T = T; o.Mdy = Mdy; o.Nx = Nx; o.taps = taps; o.dilation = dilation; o.rows = g.rows;
     o.per_split = g.per_split; o.chunks = g.chunks; o.dY = dY; o.X = X; o.P = ws; o.rows_pad = g.mtiles * 256;
-    if (int rc = hg_launch(o, dim3((Mdy + HG_BN - 1) / HG_BN, o.rows_pad / HG_BM, g.ks), st, __func__)) return rc;
+    const dim3 grid((Mdy + g.bn - 1) / g.bn, o.rows_pad / HG_BM, g.ks);
+    if (int rc = hg_launch_bn(g.bn, o, grid, st, __func__)) return rc;
     wgradp_reduce_kernel<<<ew_grid((long long)Mdy * Ntrue * taps), 256, 0, st>>>(ws, dW, taps, g.ks, o.rows_pad, Mdy, Nx,
                                                                                 Ntrue);
     ++g_launches;
