@@ -28,6 +28,7 @@ SIGNATURES = {
     "bm_subject_layers_bwd": [P, I, P, I, P, P, P, P, I, I, I, I, I, I, P, P, P],
     "bm_initial_linear_bwd": [P, I, P, I, P, I, I, I, I, I, P, P, P, P],
     "bm_sensor_mix_bwd": [P, I, P, P, P, I, I, I, I, I, P, P],
+    "bm_sensor_mix_bwd_data": [P, I, P, P, P, I, I, I, I, P, P],
     "bm_conv_weight_prep": [P, I, I, I, P, P, P],
     "bm_conv1d_fwd": [P, P, P, I, I, I, I, I, I, P, P, P],
     "bm_bn_stats_finalize": [P, L, F, F, P, P, P, P, I, P],
@@ -67,6 +68,7 @@ SIGNATURES = {
     "bm_col_sum": [P, L, I, P, P],
     "bm_tc_pointwise_sel": [P, P, P, P, I, I, I, I, I, P, P, P],
     "bm_tc_wgrad_grouped": [P, P, P, P, I, I, I, I, I, P, P, P],
+    "bm_tc_sensor_mix_bwd_data": [P, P, P, P, I, P, I, I, I, I, I, P, P, P],
     "bm_gelu_bwd": [P, P, L, P, P],
     "bm_candidate_inv_norms": [P, I, L, P, P, P],
     "bm_retrieval_topk": [P, L, I, I, P, I, I, I, P, P, P, P, P, P, P, P, P, P],
@@ -79,6 +81,7 @@ SIGNATURES = {
     "bm_bn_act_skip_fwd": [P, P, P, P, P, P, P, L, I, I, F, P],
     "bm_bn_act_skip_bwd": [P, P, P, P, P, P, I, L, I, I, F, P, P, P, P, P],
     "bm_clip_loss_bwd_cand": [P, P, P, P, P, P, I, I, L, I, P, P, P, P, P],
+    "bm_clip_scores_bwd": [P, P, P, P, P, I, I, L, P, P, P, P, P, P],
 }
 
 _lib = None

@@ -226,6 +226,21 @@ extern "C" int bm_sensor_mix_bwd(const float* du, int ld_du, const float* meg, c
     return 0;
 }
 
+extern "C" int bm_sensor_mix_bwd_data(const float* du, int ld_du, const float* weights, const int* rec_of_sample,
+                                      const float* mask, int B, int C, int T, int O, float* dmeg, bm_stream_t stream) {
+    BM_CHECK_ARG(du && weights && rec_of_sample && dmeg && ld_du >= O && B > 0 && C > 0 && T > 0 && O > 0);
+    // dmeg[b][c][t] = mask[c] sum_o du[b][t][o] w[rec_b][o][c]
+    GemmP g = gemm_defaults();
+    g.M = T; g.N = C; g.K = O; g.kchunk = O;
+    g.Z = B; g.nseg = B; g.zchunk = 1;
+    g.A = du; g.lda_z = (long long)T * ld_du; g.lda_m = ld_du; g.lda_k = 1;
+    g.B = weights; g.bsel = rec_of_sample; g.ldb_z = (long long)O * C; g.ldb_n = 1; g.ldb_k = C; g.b_ncontig = 1;
+    g.D = dmeg; g.ldd_z = (long long)C * T; g.ldd_m = 1; g.ldd_n = T;
+    g.colscale = mask;
+    BM_CUDA(launch_gemm(g, ST(stream)));
+    return 0;
+}
+
 extern "C" int bm_sensor_chain_bwd(const float* dx0, const float* meg, const float* il_w, const float* subj_w,
                                    const int* subject, const float* u, const float* v, const int* subj_order,
                                    const int* subj_off, const int* rec_order, const int* rec_off, int B, int C,
@@ -641,26 +656,23 @@ extern "C" int bm_clip_loss_fwd(const float* est, const float* cand, int Bn, int
                         workspace_floats, status, ST(stream));
 }
 
-extern "C" int bm_clip_loss_bwd(const float* probs, const float* inv_norm, const float* cand, const float* gout,
-                                int Bn, int Bc, long long KT, int target_offset, float* G, float* dest,
-                                int* status, bm_stream_t stream) {
-    BM_CHECK_ARG(probs && inv_norm && cand && gout && G && dest && Bn > 0 && Bc > 0 && KT > 0);
-    BM_CHECK_ARG(KT < (1ll << 31));
-    cudaStream_t st = ST(stream);
+namespace {
+// dest = G @ cand, the GEMM of the CLIP backward.  fill(transposed) writes G [Bn][Bc] (transposed: [Bc][Bn]) in the layout
+// the chosen GEMM reads.
+template <class Fill>
+int clip_dest_gemm(Fill fill, const float* cand, int Bn, int Bc, long long KT, float* G, float* dest, int* status,
+                   cudaStream_t st) {
     if (tc::gemm_nt_pp_supported(Bn, (int)KT, Bc) && Bn >= 192) {
         // csrc/tc_gemm_nt.cuh: dE = G C with G [Bn][Bc], C [Bc][KT]; smaller batches take the weight-gradient form below
-        clip_ce_bwd_kernel<<<ew_grid((long long)Bn * Bc), 256, 0, st>>>(probs, inv_norm, gout, Bn, Bc, target_offset, G, 0);
-        BM_CHECK_LAUNCH();
+        if (int rc = fill(0)) return rc;
         return tc::launch_gemm_nt_pp(G, cand, dest, Bn, (int)KT, Bc, status, st);
     }
     if (tc::wgrad_tc_supported(Bn, (int)KT)) {
         // tensor cores: dE[b][k] = sum_o G^T[o][b] C[o][k]  == weight-gradient GEMM with "positions" = candidates
-        clip_ce_bwd_kernel<<<ew_grid((long long)Bn * Bc), 256, 0, st>>>(probs, inv_norm, gout, Bn, Bc, target_offset, G, 1);
-        BM_CHECK_LAUNCH();
+        if (int rc = fill(1)) return rc;
         return tc::launch_wgrad_tc(G, cand, 1, Bc, Bn, (int)KT, (int)KT, 1, 1, dest, dest, status, st);   // direct mode: no workspace
     }
-    clip_ce_bwd_kernel<<<ew_grid((long long)Bn * Bc), 256, 0, st>>>(probs, inv_norm, gout, Bn, Bc, target_offset, G, 0);
-    BM_CHECK_LAUNCH();
+    if (int rc = fill(0)) return rc;
     GemmP g = gemm_defaults();
     g.M = Bn; g.N = (int)KT; g.K = Bc; g.kchunk = Bc;
     g.A = G; g.lda_m = Bc; g.lda_k = 1;
@@ -668,6 +680,51 @@ extern "C" int bm_clip_loss_bwd(const float* probs, const float* inv_norm, const
     g.D = dest; g.ldd_m = KT; g.ldd_n = 1;
     BM_CUDA(launch_gemm(g, st));
     return 0;
+}
+
+// dcand[o] = sum_b G[b][o] est[b] - coef[o] cand[o] (see clip_cand_coef_kernel); fill as in clip_dest_gemm
+template <class Fill>
+int clip_dcand_gemm(Fill fill, const float* scores, const float* inv_norm, const float* est, const float* cand, int Bn, int Bc,
+                    long long KT, float* G, float* coef, float* dcand, int* status, cudaStream_t st) {
+    if (int rc = fill(0)) return rc;
+    clip_cand_coef_kernel<<<(Bc + 127) / 128, 128, 0, st>>>(G, scores, inv_norm, Bn, Bc, coef);     // needs G as [Bn][Bc]
+    BM_CHECK_LAUNCH();
+    // dcand[o][k] = sum_b G[b][o] est[b][k]
+    if (tc::gemm_nt_pp_supported(Bc, (int)KT, Bn)) {
+        // csrc/tc_gemm_nt.cuh: A = G^T [Bc][Bn] (rewritten into the same scratch), B = est [Bn][KT]
+        if (int rc = fill(1)) return rc;
+        int rc = tc::launch_gemm_nt_pp(G, est, dcand, Bc, (int)KT, Bn, status, st);
+        if (rc) return rc;
+    } else if (tc::wgrad_tc_supported(Bc, (int)KT)) {
+        int rc = tc::launch_wgrad_tc(G, est, 1, Bn, Bc, (int)KT, (int)KT, 1, 1, dcand, dcand, status, st);   // direct mode
+        if (rc) return rc;
+    } else {
+        GemmP g = gemm_defaults();
+        g.M = Bc; g.N = (int)KT; g.K = Bn; g.kchunk = Bn;
+        g.A = G; g.lda_m = 1; g.lda_k = Bc; g.a_mcontig = 1;
+        g.B = est; g.ldb_n = 1; g.ldb_k = KT; g.b_ncontig = 1;
+        g.D = dcand; g.ldd_m = KT; g.ldd_n = 1;
+        BM_CUDA(launch_gemm(g, st));
+    }
+    clip_cand_correct_kernel<<<ew_grid((long long)Bc * KT), 256, 0, st>>>(cand, coef, KT, (long long)Bc * KT, dcand);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+}  // namespace
+
+extern "C" int bm_clip_loss_bwd(const float* probs, const float* inv_norm, const float* cand, const float* gout,
+                                int Bn, int Bc, long long KT, int target_offset, float* G, float* dest,
+                                int* status, bm_stream_t stream) {
+    BM_CHECK_ARG(probs && inv_norm && cand && gout && G && dest && Bn > 0 && Bc > 0 && KT > 0);
+    BM_CHECK_ARG(KT < (1ll << 31));
+    cudaStream_t st = ST(stream);
+    auto fill = [&](int transposed) {
+        clip_ce_bwd_kernel<<<ew_grid((long long)Bn * Bc), 256, 0, st>>>(probs, inv_norm, gout, Bn, Bc, target_offset, G,
+                                                                        transposed);
+        BM_CHECK_LAUNCH();
+        return 0;
+    };
+    return clip_dest_gemm(fill, cand, Bn, Bc, KT, G, dest, status, st);
 }
 
 // =================================================================================================
@@ -713,30 +770,30 @@ extern "C" int bm_clip_loss_bwd_cand(const float* probs, const float* scores, co
     BM_CHECK_ARG(probs && scores && inv_norm && est && cand && gout && G && coef && dcand);
     BM_CHECK_ARG(Bn > 0 && Bc > 0 && KT > 0 && KT < (1ll << 31));
     cudaStream_t st = ST(stream);
-    clip_ce_bwd_kernel<<<ew_grid((long long)Bn * Bc), 256, 0, st>>>(probs, inv_norm, gout, Bn, Bc, target_offset, G, 0);
-    BM_CHECK_LAUNCH();
-    clip_cand_coef_kernel<<<(Bc + 127) / 128, 128, 0, st>>>(G, scores, inv_norm, Bn, Bc, coef);     // needs G as [Bn][Bc]
-    BM_CHECK_LAUNCH();
-    // dcand[o][k] = sum_b G[b][o] est[b][k]
-    if (tc::gemm_nt_pp_supported(Bc, (int)KT, Bn)) {
-        // csrc/tc_gemm_nt.cuh: A = G^T [Bc][Bn] (rewritten into the same scratch), B = est [Bn][KT]
-        clip_ce_bwd_kernel<<<ew_grid((long long)Bn * Bc), 256, 0, st>>>(probs, inv_norm, gout, Bn, Bc, target_offset, G, 1);
+    auto fill = [&](int transposed) {
+        clip_ce_bwd_kernel<<<ew_grid((long long)Bn * Bc), 256, 0, st>>>(probs, inv_norm, gout, Bn, Bc, target_offset, G,
+                                                                        transposed);
         BM_CHECK_LAUNCH();
-        int rc = tc::launch_gemm_nt_pp(G, est, dcand, Bc, (int)KT, Bn, status, st);
-        if (rc) return rc;
-    } else if (tc::wgrad_tc_supported(Bc, (int)KT)) {
-        int rc = tc::launch_wgrad_tc(G, est, 1, Bn, Bc, (int)KT, (int)KT, 1, 1, dcand, dcand, status, st);   // direct mode
-        if (rc) return rc;
-    } else {
-        GemmP g = gemm_defaults();
-        g.M = Bc; g.N = (int)KT; g.K = Bn; g.kchunk = Bn;
-        g.A = G; g.lda_m = 1; g.lda_k = Bc; g.a_mcontig = 1;
-        g.B = est; g.ldb_n = 1; g.ldb_k = KT; g.b_ncontig = 1;
-        g.D = dcand; g.ldd_m = KT; g.ldd_n = 1;
-        BM_CUDA(launch_gemm(g, st));
-    }
-    clip_cand_correct_kernel<<<ew_grid((long long)Bc * KT), 256, 0, st>>>(cand, coef, KT, (long long)Bc * KT, dcand);
-    BM_CHECK_LAUNCH();
+        return 0;
+    };
+    return clip_dcand_gemm(fill, scores, inv_norm, est, cand, Bn, Bc, KT, G, coef, dcand, status, st);
+}
+
+extern "C" int bm_clip_scores_bwd(const float* dscores, const float* scores, const float* inv_norm, const float* est,
+                                  const float* cand, int Bn, int Bc, long long KT, float* G, float* coef, float* dest,
+                                  float* dcand, int* status, bm_stream_t stream) {
+    BM_CHECK_ARG(dscores && inv_norm && cand && G && Bn > 0 && Bc > 0 && KT > 0 && KT < (1ll << 31));
+    BM_CHECK_ARG(!dcand || (scores && est && coef));
+    cudaStream_t st = ST(stream);
+    auto fill = [&](int transposed) {
+        clip_scores_grad_kernel<<<ew_grid((long long)Bn * Bc), 256, 0, st>>>(dscores, inv_norm, Bn, Bc, G, transposed);
+        BM_CHECK_LAUNCH();
+        return 0;
+    };
+    if (dest)
+        if (int rc = clip_dest_gemm(fill, cand, Bn, Bc, KT, G, dest, status, st)) return rc;
+    if (dcand)
+        if (int rc = clip_dcand_gemm(fill, scores, inv_norm, est, cand, Bn, Bc, KT, G, coef, dcand, status, st)) return rc;
     return 0;
 }
 
@@ -1033,6 +1090,16 @@ extern "C" int bm_tc_pointwise_sel(const float* x, const float* w_hi, const floa
     p.bias = nullptr; p.addend = nullptr; p.y = y; p.glu_out = nullptr; p.err = status;
     p.act = 0; p.out_tmajor = 0; p.aux = nullptr; p.wsel = wsel; p.n_wsets = n_sets;
     return tc::launch_conv_tc(x, w_hi, w_lo, p, ST(stream));
+}
+
+// data gradient of the sensor mix on the tensor cores (ChannelMerger, common.py:358):
+//   dmeg[b,c,t] = mask[c] sum_o du[b,t,o] W[wsel[b]][c][o], c < C;  w_hi / w_lo: tf32-split transposed weight sets [S][Cp][Op]
+extern "C" int bm_tc_sensor_mix_bwd_data(const float* du, const float* w_hi, const float* w_lo, const int* wsel, int n_sets,
+                                         const float* mask, int B, int T, int Op, int Cp, int C, float* dmeg, int* status,
+                                         bm_stream_t stream) {
+    BM_CHECK_ARG(du && w_hi && w_lo && wsel && dmeg && n_sets > 0 && B > 0 && T > 0 && C > 0 && C <= Cp);
+    BM_CHECK_ARG(tc::conv_tc_supported(T, Op, Cp, 1, 0));
+    return tc::launch_sensor_mix_bwd_tc(du, w_hi, w_lo, wsel, n_sets, mask, B, T, Op, Cp, C, dmeg, status, ST(stream));
 }
 
 // per-group pointwise weight gradient (SubjectLayers: dM[s] = sum over the samples of subject s), tensor cores:

@@ -403,6 +403,20 @@ __global__ void clip_ce_bwd_kernel(const float* __restrict__ probs, const float*
     }
 }
 
+// G[b][o] = dscores[b][o] * inv_norm[o]: the same G for an arbitrary upstream gradient of the scores (get_scores backward);
+// transposed as in clip_ce_bwd_kernel
+__global__ void clip_scores_grad_kernel(const float* __restrict__ dscores, const float* __restrict__ inv_norm, int Bn, int Bc,
+                                        float* __restrict__ G, int transposed) {
+    long long total = (long long)Bn * Bc;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        int b = (int)(i / Bc), o = (int)(i - (long long)b * Bc);
+        float v = dscores[i] * inv_norm[o];
+        if (transposed) G[(long long)o * Bn + b] = v;
+        else G[i] = v;
+    }
+}
+
 // y[b][c][t] = x[b][c][t] * mask[c]   (simpleconv.py:200-203: `subsample_meg_channels` zeroes the sensors not drawn)
 __global__ void channel_mask_kernel(const float* __restrict__ x, const float* __restrict__ mask, float* __restrict__ y,
                                     int C, int T, long long total) {

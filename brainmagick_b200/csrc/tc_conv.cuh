@@ -186,6 +186,32 @@ struct ConvOp {
     }
 };
 
+// Data gradient of the sensor mix (ChannelMerger, common.py:358) as a pointwise ConvOp with one weight set per recording:
+//   dmeg[b, c, t] = mask[c] * sum_o du[b, t, o] * W[wsel[b]][c][o]
+// x = du [B,T,Cin=Op], w = the transposed attention weights [R][Ntot=Cp][Op].  Its own epilogue stores only the C live sensor
+// rows, channel-major [B,C,T], times the channel mask (nullable); the ConvOp epilogue itself is untouched.
+struct SensorMixBwdOp : ConvOp {
+    int C;
+    const float* mask;
+    template <int BN> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+#pragma unroll
+        for (int g = 0; g < 16; ++g) {
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int n = c.n_tile * HG_BN + 8 * g + 2 * (threadIdx.x & 3) + e;
+                if (n >= C) continue;
+                const float m = mask ? mask[n] : 1.f;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int i = 4 * g + 2 * h + e;
+                    const int t = c.t0 + m0 + hg_row(i);
+                    if (t < T) y[((long long)c.b * C + n) * T + t] = acc[i] * m;
+                }
+            }
+        }
+    }
+};
+
 inline ConvOp conv_op_defaults() {
     ConvOp o;
     memset(&o, 0, sizeof(o));
@@ -251,6 +277,20 @@ inline int launch_conv_tc(const float* x, const float* w_hi, const float* w_lo, 
     o.addend = p.addend; o.y = p.y; o.aux = p.aux; o.glu_out = p.glu_out; o.act = p.act; o.out_tmajor = p.out_tmajor;
     o.err = p.err;
     return launch_conv_op(o, st, __func__);
+}
+
+// du [B,T,Op]; w_hi / w_lo [n_sets][Cp][Op] (tf32 pieces); dmeg [B,C,T] with C <= Cp; mask [C] or null
+inline int launch_sensor_mix_bwd_tc(const float* du, const float* w_hi, const float* w_lo, const int* wsel, int n_sets,
+                                    const float* mask, int B, int T, int Op, int Cp, int C, float* dmeg, int* err,
+                                    cudaStream_t st) {
+    SensorMixBwdOp o;
+    memset(&o, 0, sizeof(o));
+    o.x = du; o.w = w_hi; o.w_lo32 = w_lo; o.B = B; o.T = T; o.Cin = Op; o.Ntot = Cp; o.taps = 1; o.dilation = 1; o.sign = 1;
+    o.n_wsets = n_sets; o.wsel = wsel; o.y = dmeg; o.err = err; o.C = C; o.mask = mask;
+    if ((long long)B * T >= (1ll << 31)) return set_error(2, "%s: too many rows%s", __func__);
+    o.ttiles = (T + HG_BM - 1) / HG_BM;
+    return hg_launch<HG_BN>(o, dim3((unsigned)((long long)B * o.ttiles), (unsigned)((Cp + HG_BN - 1) / HG_BN), 1), st,
+                            __func__);
 }
 
 }  // namespace tc

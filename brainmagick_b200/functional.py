@@ -3,7 +3,8 @@
 `encoder_forward` is SimpleConv.forward at the clip_conv configuration (bm/models/simpleconv.py:198-249) as ONE
 autograd node: its backward launches the hand-written gradient kernels in reverse order, so `loss.backward()`
 leaves ordinary dense `.grad` tensors on every parameter (what bm/solver.py:384-387 and
-flashy.distrib.sync_model expect).  `clip_loss` / `clip_scores` are ClipLoss (bm/losses.py:77-114).
+flashy.distrib.sync_model expect), and on `meg` when it requires grad (gradient-based attribution).  `clip_loss` /
+`clip_scores` / `clip_scores_grad` are ClipLoss (bm/losses.py:77-114).
 
 Kernel selection is by shape only: contractions whose channel counts fit the tensor-core tiling (K % 32 == 0 and an
 N tile of 64..160 dividing N -- every layer of the real clip_conv model) run on the tensor-core kernels
@@ -49,6 +50,8 @@ class EncoderPlan:
     staged: bool = False                   # a sensor-chain stage is missing (merger / initial_linear / subject_layers
                                            # ablations) or a subject embedding is appended: run the chain stage by stage
     has_sub_emb: bool = False              # the last tensor argument is the [B, E] subject-embedding rows
+    channel_mask: tp.Optional[torch.Tensor] = None   # [C] subsample_meg_channels mask (simpleconv.py:200-203), or None
+    masked_meg: tp.Optional[torch.Tensor] = None     # [B,C,T] buffer that receives meg * channel_mask
 
 
 def _empty(shape, like, dtype=torch.float32):
@@ -350,8 +353,9 @@ def _staged_front_forward(plan: "EncoderPlan", meg, heads, il_w, il_b, subj_w, s
     return x, saved
 
 
-def _staged_front_backward(plan: "EncoderPlan", saved, g, heads, il_w, subj_w, sub_emb):
-    """g = dL/dx [B,T,D_total] -> (dheads, d_il_w, d_il_b, d_subj, d_sub_emb); None where the stage is absent."""
+def _staged_front_backward(plan: "EncoderPlan", saved, g, heads, il_w, subj_w, sub_emb, want_dmeg=False):
+    """g = dL/dx [B,T,D_total] -> (dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg); None where the stage is absent or
+    (dmeg) not wanted."""
     st = stream()
     meg = saved["meg"]
     B, C, T = meg.shape
@@ -388,7 +392,40 @@ def _staged_front_backward(plan: "EncoderPlan", saved, g, heads, il_w, subj_w, s
         dheads = _empty((O, P), meg)
         call("bm_attention_weights_bwd", ptr(d_att), ptr(saved["att"]), ptr(saved["emb"]), R, C, O, P, ptr(dscores),
              ptr(dheads), st)
-    return dheads, d_il_w, d_il_b, d_subj, d_sub_emb
+    dmeg = None
+    if want_dmeg:
+        # g is now the gradient at the first stage present: the mix output, or the raw sensors transposed (merger=False)
+        dmeg = _empty((B, C, T), meg)
+        if heads is not None:
+            call("bm_sensor_mix_bwd_data", ptr(g), g.shape[2], ptr(saved["att"]), ptr(plan.rec_of_sample),
+                 ptr(plan.channel_mask), B, C, T, heads.shape[0], ptr(dmeg), st)
+        else:
+            call("bm_transpose_nt", ptr(g), B, T, C, ptr(dmeg), st)
+            if plan.channel_mask is not None:
+                call("bm_channel_mask", ptr(dmeg), ptr(plan.channel_mask), B, C, T, ptr(dmeg), st)
+    return dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg
+
+
+def _sensor_mix_bwd_data(plan: "EncoderPlan", s, du, dims, status) -> torch.Tensor:
+    """dmeg [B,C,T] = mask[c] * sum_o att[rec_b][o][c] du[b,t,o] for the fused sensor chain; du [B,T,O or Op].  On the tensor
+    cores when the mix ran there and the transposed contraction fits their shape gate, else the FP32-FMA stage kernel."""
+    B, C, T, R, O = dims[:5]
+    st = stream()
+    meg, att = s["meg"], s["att"]
+    dmeg = _empty((B, C, T), meg)
+    Op = du.shape[2]
+    Cp = s["megT"].shape[2] if s["megT"] is not None else 0
+    if Cp and bool(_lib.load().bm_tc_conv_supported(T, Op, Cp, 1, 0)):
+        att_t = torch.zeros((R, Cp, Op), device=meg.device)           # weight set r: [c][o], zero-padded
+        att_t[:, :C, :O] = att.transpose(1, 2)
+        w_hi, w_lo = _empty((R * Cp, Op), meg), _empty((R * Cp, Op), meg)
+        call("bm_tc_weight_split", ptr(att_t), R * Cp, Op, 1, ptr(w_hi), ptr(w_lo), None, None, st)
+        call("bm_tc_sensor_mix_bwd_data", ptr(du), ptr(w_hi), ptr(w_lo), ptr(plan.rec_of_sample), R, ptr(plan.channel_mask),
+             B, T, Op, Cp, C, ptr(dmeg), ptr(status), st)
+    else:
+        call("bm_sensor_mix_bwd_data", ptr(du), Op, ptr(att), ptr(plan.rec_of_sample), ptr(plan.channel_mask), B, C, T, O,
+             ptr(dmeg), st)
+    return dmeg
 
 
 class _EncoderFn(torch.autograd.Function):
@@ -411,6 +448,10 @@ class _EncoderFn(torch.autograd.Function):
         st = stream()
         meg = meg.contiguous()
         B, C, T = meg.shape
+        if plan.channel_mask is not None:
+            # inside the node, so that the gradient reaches the caller's unmasked tensor (the backward applies the mask)
+            call("bm_channel_mask", ptr(meg), ptr(plan.channel_mask), B, C, T, ptr(plan.masked_meg), st)
+            meg = plan.masked_meg
         R = plan.rec_positions.shape[0]
         O, P = heads.shape if heads is not None else (0, 0)
         IL = il_w.shape[0] if il_w is not None else 0
@@ -815,8 +856,8 @@ class _EncoderFn(torch.autograd.Function):
         keep_alive.clear()
         if plan.staged:
             heads_p, il_w_p, subj_w_p, sub_emb_p = s["params"]
-            dheads, d_il_w, d_il_b, d_subj, d_sub_emb = _staged_front_backward(plan, s["front"], g, heads_p, il_w_p,
-                                                                               subj_w_p, sub_emb_p)
+            dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg = _staged_front_backward(
+                plan, s["front"], g, heads_p, il_w_p, subj_w_p, sub_emb_p, want_dmeg=ctx.needs_input_grad[1])
         else:
             d_sub_emb = None
             # ---- sensor chain + attention ----
@@ -865,6 +906,7 @@ class _EncoderFn(torch.autograd.Function):
                 call("bm_sensor_chain_bwd", ptr(g), ptr(meg), ptr(s["il_w2"]), ptr(s["subj_w"]), ptr(plan.subject),
                      ptr(s["u"]), ptr(s["v"]), ptr(subj_order), ptr(subj_off), ptr(plan.rec_order), ptr(plan.rec_off),
                      B, C, T, O, IL, D, Dp, S, R, ptr(dv), ptr(du), ptr(d_subj), ptr(d_il_w), ptr(d_il_b), ptr(d_att), st)
+            dmeg = _sensor_mix_bwd_data(plan, s, du, ctx.dims, status) if ctx.needs_input_grad[1] else None
             dscores = _empty((R, O, C), meg)
             if s["heads_tc"]:
                 Opad = _round_up(O, 64)
@@ -880,9 +922,9 @@ class _EncoderFn(torch.autograd.Function):
         if d_il_w is not None:
             d_il_w = d_il_w.reshape(s["il_shape"])
         if plan.bare_last:
-            grads = [None, None, dheads, d_il_w, d_il_b, d_subj, None, None, None, None]
+            grads = [None, dmeg, dheads, d_il_w, d_il_b, d_subj, None, None, None, None]
         else:
-            grads = [None, None, dheads, d_il_w, d_il_b, d_subj,
+            grads = [None, dmeg, dheads, d_il_w, d_il_b, d_subj,
                      dw0.reshape(s["w0_shape"]), db0, dw2.reshape(s["w2_shape"]), db2]
         for k in range(depth):
             grads.extend(layer_grads[k])
@@ -928,7 +970,8 @@ def _check_clip_operands(est: torch.Tensor, cand: torch.Tensor) -> None:
 
 
 def clip_scores(estimates: torch.Tensor, candidates: torch.Tensor, want_probs: bool = False):
-    """ClipLoss.get_scores / get_probabilities (bm/losses.py:77-102); no autograd."""
+    """ClipLoss.get_scores / get_probabilities (bm/losses.py:77-102) without autograd (evaluation, retrieval); see
+    `clip_scores_grad` for the differentiable form."""
     est = estimates.detach().contiguous().float()
     cand = candidates.detach().contiguous().float()
     Bn, Bc = est.shape[0], cand.shape[0]
@@ -941,6 +984,52 @@ def clip_scores(estimates: torch.Tensor, candidates: torch.Tensor, want_probs: b
     call("bm_clip_scores", ptr(est), ptr(cand), Bn, Bc, KT, 0, ptr(inv), ptr(scores), ptr(probs), ptr(ws), ws.numel(),
          ptr(tc_status_tensor(est.device)), stream())
     return probs if want_probs else scores
+
+
+class _ClipScoresFn(torch.autograd.Function):
+    """get_scores / get_probabilities with a backward to the estimates and the candidates (gradient-based attribution).
+    The forward is clip_scores' bm_clip_scores call, so the values are the same."""
+
+    @staticmethod
+    def forward(ctx, estimate, candidate, want_probs: bool):
+        _check_clip_operands(estimate, candidate)
+        est, cand = estimate.contiguous(), candidate.contiguous()
+        Bn, Bc = est.shape[0], cand.shape[0]
+        KT = est[0].numel()
+        assert cand[0].numel() == KT
+        inv = _empty((Bc,), est)
+        scores = _empty((Bn, Bc), est)
+        probs = _empty((Bn, Bc), est) if want_probs else None
+        ws = _clip_workspace(est, Bn, Bc, KT)
+        call("bm_clip_scores", ptr(est), ptr(cand), Bn, Bc, KT, 0, ptr(inv), ptr(scores), ptr(probs), ptr(ws), ws.numel(),
+             ptr(tc_status_tensor(est.device)), stream())
+        ctx.save_for_backward(est, cand, inv, scores, probs)
+        ctx.meta = (Bn, Bc, KT, estimate.shape, candidate.shape)
+        return probs if want_probs else scores
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gout):
+        est, cand, inv, scores, probs = ctx.saved_tensors
+        Bn, Bc, KT, est_shape, cand_shape = ctx.meta
+        st = stream()
+        dscores = gout.contiguous().float()
+        if probs is not None:                    # get_probabilities: through the row softmax first
+            ds = _empty((Bn, Bc), est)
+            call("bm_softmax_bwd", ptr(probs), ptr(dscores), Bn, Bc, ptr(ds), st)
+            dscores = ds
+        dest = _empty(est_shape, est) if ctx.needs_input_grad[0] else None
+        dcand = _empty(cand_shape, est) if ctx.needs_input_grad[1] else None
+        G = _empty((Bn, Bc), est)
+        coef = _empty((Bc,), est) if dcand is not None else None
+        call("bm_clip_scores_bwd", ptr(dscores), ptr(scores), ptr(inv), ptr(est), ptr(cand), Bn, Bc, KT, ptr(G), ptr(coef),
+             ptr(dest), ptr(dcand), ptr(tc_status_tensor(est.device)), st)
+        return dest, dcand, None
+
+
+def clip_scores_grad(estimates: torch.Tensor, candidates: torch.Tensor, want_probs: bool = False):
+    """clip_scores as an autograd node: scores (or probabilities) whose backward reaches the estimates and candidates."""
+    return _ClipScoresFn.apply(estimates, candidates, want_probs)
 
 
 def candidate_inv_norms(candidates: torch.Tensor) -> torch.Tensor:
@@ -1022,7 +1111,7 @@ def clip_loss(estimate, candidate, target_offset: int = 0):
 # ----------------------------------------------------------------------------------------------------
 # Stand-alone ChannelMerger.forward / SubjectLayers.forward (bm/models/common.py:334-362, 55-58): inside SimpleConv both are
 # fused into the encoder; called on their own (analysis notebooks, user code) they run the same stage kernels.  Channel-major
-# tensors in and out, like the reference; gradients flow to the parameters (and to `x` for SubjectLayers), not to `meg`.
+# tensors in and out, like the reference; gradients flow to the parameters and to the input (`meg` / `x`).
 # ----------------------------------------------------------------------------------------------------
 class _MergerFn(torch.autograd.Function):
     @staticmethod
@@ -1039,14 +1128,14 @@ class _MergerFn(torch.autograd.Function):
         call("bm_sensor_mix_fwd", ptr(meg), ptr(att), ptr(rec_of_sample), B, C, T, O, O, ptr(u), st)
         out = _empty((B, O, T), meg)
         call("bm_transpose_nt", ptr(u), B, T, O, ptr(out), st)
-        ctx.save_for_backward(meg, emb, att, rec_order, rec_off)
+        ctx.save_for_backward(meg, emb, att, rec_of_sample, rec_order, rec_off)
         ctx.dims = (B, C, T, R, O, P)
         return out
 
     @staticmethod
     @torch.autograd.function.once_differentiable
     def backward(ctx, gout):
-        meg, emb, att, rec_order, rec_off = ctx.saved_tensors
+        meg, emb, att, rec_of_sample, rec_order, rec_off = ctx.saved_tensors
         B, C, T, R, O, P = ctx.dims
         st = stream()
         g = _empty((B, T, O), meg)
@@ -1054,7 +1143,11 @@ class _MergerFn(torch.autograd.Function):
         d_att, dscores, dheads = _empty((R, O, C), meg), _empty((R, O, C), meg), _empty((O, P), meg)
         call("bm_sensor_mix_bwd", ptr(g), O, ptr(meg), ptr(rec_order), ptr(rec_off), B, C, T, O, R, ptr(d_att), st)
         call("bm_attention_weights_bwd", ptr(d_att), ptr(att), ptr(emb), R, C, O, P, ptr(dscores), ptr(dheads), st)
-        return None, dheads, None, None, None, None, None, None, None
+        dmeg = None
+        if ctx.needs_input_grad[0]:
+            dmeg = _empty((B, C, T), meg)
+            call("bm_sensor_mix_bwd_data", ptr(g), O, ptr(att), ptr(rec_of_sample), None, B, C, T, O, ptr(dmeg), st)
+        return dmeg, dheads, None, None, None, None, None, None, None
 
 
 def channel_merger_forward(meg, heads, positions, rec_of_sample, rec_order, rec_off, freq, ban_centre, radius):

@@ -1,6 +1,7 @@
 """Drop-in `ClipLoss` (reference: bm/losses.py:29-114): same constructor, `forward(estimate, candidate, mask)`,
-`get_scores`, `get_probabilities`, `trim_samples`.  Scores, softmax / cross-entropy and their gradient run in
-CUDA through the C ABI (`functional.clip_loss`, `functional.clip_scores`).
+`get_scores`, `get_probabilities`, `trim_samples`.  Scores, softmax / cross-entropy and their gradients run in
+CUDA through the C ABI (`functional.clip_loss`, `functional.clip_scores`, and `functional.clip_scores_grad` when the
+scores are differentiated, e.g. for gradient-based attribution).
 
 Reference semantics kept on purpose: only the CANDIDATES are L2-normalised (losses.py:91-94), no temperature,
 the `linear` projection is constructed but never applied (losses.py:35,82), targets are the first B candidates.
@@ -17,6 +18,10 @@ import torch
 
 from . import functional as BF
 from . import distrib
+
+
+def _wants_grad(estimates, candidates) -> bool:
+    return torch.is_grad_enabled() and (estimates.requires_grad or candidates.requires_grad)
 
 
 class ClipLoss(torch.nn.Module):
@@ -71,12 +76,17 @@ class ClipLoss(torch.nn.Module):
         return estimates, candidates
 
     def get_scores(self, estimates: torch.Tensor, candidates: torch.Tensor):
-        """[B, C, T] x [B', C, T] -> [B, B'] matching scores (no autograd; use forward() for training)."""
+        """[B, C, T] x [B', C, T] -> [B, B'] matching scores.  Differentiable when an input requires grad (gradient-based
+        attribution); otherwise no autograd node is recorded."""
         estimates, candidates = self._prepare(estimates, candidates)
+        if _wants_grad(estimates, candidates):
+            return BF.clip_scores_grad(estimates, candidates)
         return BF.clip_scores(estimates, candidates)
 
     def get_probabilities(self, estimates, candidates):
         estimates, candidates = self._prepare(estimates, candidates)
+        if _wants_grad(estimates, candidates):
+            return BF.clip_scores_grad(estimates, candidates, want_probs=True)
         return BF.clip_scores(estimates, candidates, want_probs=True)
 
     def prefetch_candidates(self, candidate: torch.Tensor) -> None:

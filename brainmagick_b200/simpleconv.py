@@ -2,8 +2,9 @@
 
 Same constructor signature, submodule/parameter names (=> interchangeable `state_dict`), construction order
 (=> identical parameters for a given `torch.manual_seed`), `forward(inputs, batch) -> [B, F, T]`, train/eval
-semantics (BatchNorm running statistics, one spatial-dropout centre per training forward).  The arithmetic runs in
-hand-written sm_90a CUDA through the C ABI (`functional.encoder_forward`); there is no PyTorch/CPU fallback.
+semantics (BatchNorm running statistics, one spatial-dropout centre per training forward), and the same autograd
+behaviour: gradients reach every parameter and, when it requires grad, the tensor passed as `inputs["meg"]`.
+The arithmetic runs in hand-written sm_90a CUDA through the C ABI (`functional.encoder_forward`); there is no PyTorch/CPU fallback.
 
 Accelerated configuration = the `clip_conv` family of conf/model/clip_conv.yaml (merger + initial_linear +
 subject_layers + ConvSequence(batch_norm) + head), with or without `skip`, with any `glu` period, with GELU or
@@ -219,17 +220,14 @@ class SimpleConv(nn.Module):
             raise TypeError("brainmagick_b200.SimpleConv computes in fp32, like the reference")
         assert meg.shape[1] == self.n_input_channels, "number of MEG channels differs from in_channels['meg']"
         length = meg.shape[-1]
-        if self.subsampled_meg_channels is not None:         # simpleconv.py:200-203
+        plan = self._plan(meg, batch)
+        if self.subsampled_meg_channels is not None:         # simpleconv.py:200-203, applied inside the encoder node
             if self._channel_mask is None or self._channel_mask.device != meg.device:
                 mask = torch.zeros(self.n_input_channels)
                 mask[self.subsampled_meg_channels] = 1.
                 self._channel_mask = mask.to(meg.device)
-            meg = meg.contiguous()
-            masked = torch.empty_like(meg)
-            BF.call("bm_channel_mask", BF.ptr(meg), BF.ptr(self._channel_mask), meg.shape[0], meg.shape[1], meg.shape[2],
-                    BF.ptr(masked), BF.stream())
-            meg = inputs["meg"] = masked
-        plan = self._plan(meg, batch)
+            plan.channel_mask = self._channel_mask
+            plan.masked_meg = inputs["meg"] = torch.empty(meg.shape, device=meg.device)
         heads = None if self.merger is None else self.merger.heads
         il_w, il_b = (None, None) if self.initial_linear is None else \
             (self.initial_linear[0].weight, self.initial_linear[0].bias)

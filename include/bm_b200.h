@@ -88,6 +88,12 @@ int bm_initial_linear_bwd(const float* dv, int ld_dv, const float* u, int ld_u, 
                           int IL, int ld_du, float* du, float* d_il_w, float* d_il_b, bm_stream_t stream);
 int bm_sensor_mix_bwd(const float* du, int ld_du, const float* meg, const int* rec_order, const int* rec_off, int B, int C,
                       int T, int O, int R, float* d_weights, bm_stream_t stream);
+/* Data gradient of the sensor mix, for callers that backpropagate to `meg` (gradient-based attribution, input
+ * optimisation): dmeg[b,c,t] = mask[c] * sum_o weights[rec[b],o,c] du[b,t,o].  du [B,T,ld_du]; weights [R,O,C]; mask [C]
+ * (nullable = all ones: SimpleConv's subsample_meg_channels mask, simpleconv.py:200-203); dmeg [B,C,T] channel-major.
+ * Sensors with attention weight 0 (INVALID / banned) receive exactly 0. */
+int bm_sensor_mix_bwd_data(const float* du, int ld_du, const float* weights, const int* rec_of_sample, const float* mask, int B,
+                           int C, int T, int O, float* dmeg, bm_stream_t stream);
 
 /* ---- K3: dilated Conv1d + train-mode BatchNorm + GELU + skip (ConvSequence, common.py:98-151) ------------
  * w [Cout,Cin,Kw] -> wf [Kw,Cin,Cout] (forward operand), wb [Kw,Cout,Cin] (data-gradient operand). */
@@ -186,6 +192,14 @@ int bm_bn_act_skip_bwd(const float* g, const float* y, const float* mean, const 
 int bm_clip_loss_bwd_cand(const float* probs, const float* scores, const float* inv_norm, const float* est,
                           const float* cand, const float* gout, int Bn, int Bc, long long KT, int target_offset,
                           float* G, float* coef, float* dcand, int* status, bm_stream_t stream);
+/* Backward of ClipLoss.get_scores (losses.py:91-94) for an arbitrary upstream gradient dscores [Bn,Bc]: with
+ * G = dscores * inv_norm (per column), dest [Bn,KT] = G @ cand and dcand [Bc,KT] = G^T est - coef * cand, coef as in
+ * bm_clip_loss_bwd_cand (0 for a zero candidate, as autograd's norm backward defines it).  The same GEMMs as
+ * bm_clip_loss_bwd / bm_clip_loss_bwd_cand.  dest and dcand are each nullable; scores [Bn,Bc], est and coef [Bc] (scratch)
+ * are needed for dcand only.  G [Bn,Bc]: scratch.  get_probabilities: dscores = bm_softmax_bwd(probs, dprobs) first. */
+int bm_clip_scores_bwd(const float* dscores, const float* scores, const float* inv_norm, const float* est, const float* cand,
+                       int Bn, int Bc, long long KT, float* G, float* coef, float* dest, float* dcand, int* status,
+                       bm_stream_t stream);
 
 /* ---- Retrieval evaluation (SURVEY 8(f) row 1): scripts/run_eval_probs.py:237-307, bm/wer.py:80-116 ---------
  * The score matrix comes from bm_clip_scores (queries x candidates, candidate axis optionally zero-padded to the
@@ -314,6 +328,13 @@ int bm_tc_pointwise_sel(const float* x, const float* w_hi, const float* w_lo, co
                         int Cin, int Ntot, float* y, int* status, bm_stream_t stream);
 int bm_tc_wgrad_grouped(const float* dy, const float* x, const int* order, const int* seg_off, int G, int B, int T, int M,
                         int N, float* out, int* status, bm_stream_t stream);
+/* bm_sensor_mix_bwd_data on the tensor cores: the pointwise contraction of bm_tc_pointwise_sel with du [B,T,Op] as x and
+ * the TRANSPOSED attention weights as the per-recording weight sets, w_hi/w_lo [S][Cp][Op] (tf32 pieces, zero-padded;
+ * wsel = rec_of_sample).  The epilogue stores only the C <= Cp live sensor rows, channel-major dmeg [B,C,T], times mask [C]
+ * (nullable).  Shape gate: bm_tc_conv_supported(T, Op, Cp, 1, 0). */
+int bm_tc_sensor_mix_bwd_data(const float* du, const float* w_hi, const float* w_lo, const int* wsel, int n_sets,
+                              const float* mask, int B, int T, int Op, int Cp, int C, float* dmeg, int* status,
+                              bm_stream_t stream);
 /* dh = dq * GELU'(h), elementwise over n values (dh may alias dq): the head's activation backward. */
 int bm_gelu_bwd(const float* dq, const float* h, long long n, float* dh, bm_stream_t stream);
 /* y[b,c,t] = x[b,c,t] * mask[c]: SimpleConv(subsample_meg_channels=n) keeps n sensors drawn with random.Random(1234)
