@@ -6,8 +6,12 @@
 // addressing (tap shifts with per-sample zero padding, position-major weight-gradient operands, K slices) and its own fused
 // epilogue without a copy of the pipeline.
 //
-// One CTA = two warpgroups = one 128 x BN output tile (warpgroup g owns rows [64 g, 64 g + 64)); BN = 128, or for the weight
-// gradients 160 where the output width asks for it (hg_pick_bn).  Per K block of 32:
+// Two main loops share the wgmma wrappers, the tile layout and the numerics below: hc_conv_kernel (further down: TMA-fed,
+// warp-specialised) for the conv ops, whose A operand is a K-contiguous activation tile, and hg_gemm_kernel (register-staged)
+// for the weight gradients and the CLIP GEMMs, whose M/N-contiguous operands are transposed on their way into shared memory.
+//
+// hg_gemm_kernel: one CTA = two warpgroups = one 128 x BN output tile (warpgroup g owns rows [64 g, 64 g + 64)); BN = 128,
+// or 160 where the output width asks for it (hg_pick_bn).  Per K block of 32:
 //   * every thread loads its share of the A and B tiles from global memory into registers one block AHEAD (the loads of
 //     block kb+1 are in flight while the tensor cores work on block kb), splits each fp32 value x into tf32 pieces
 //     hi = rna_tf32(x), lo = x - hi, and writes hi and lo into the 128-byte-swizzled K-major layout wgmma reads;
@@ -18,6 +22,7 @@
 //     block keeps that bias below 1e-7 relative however long K is, with no correction factor to calibrate per GPU.
 #pragma once
 #include <cuda.h>
+#include <type_traits>
 #include "common.cuh"
 
 namespace bm {
@@ -131,6 +136,103 @@ __device__ __forceinline__ void wgmma_tf32(float* d, uint64_t adesc, uint64_t bd
     static_assert(BN == 128 || BN == 160, "engine tile widths: 128, 160");
     if constexpr (BN == 128) wgmma_tf32_m64n128(d, adesc, bdesc, accumulate);
     else wgmma_tf32_m64n160(d, adesc, bdesc, accumulate);
+}
+
+// d (+)= A[registers] * B[smem]^T, M = 64, N = 128, K = 8: a = this thread's 4 tf32 values of the 64 x 8 A fragment
+// (warp w of the group holds rows 16 w + lane/4 (+8 for a[1], a[3]), columns lane%4 (+4 for a[2], a[3]))
+__device__ __forceinline__ void wgmma_tf32_rs_m64n128(float* d, const float* a, uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])),
+          "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+// the same with N = 160
+__device__ __forceinline__ void wgmma_tf32_rs_m64n160(float* d, const float* a, uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %85, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n160k8.f32.tf32.tf32 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
+        "{%80, %81, %82, %83}, %84, p, 1, 1;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]),
+          "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]),
+          "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
+        : "r"(__float_as_uint(a[0])), "r"(__float_as_uint(a[1])), "r"(__float_as_uint(a[2])), "r"(__float_as_uint(a[3])),
+          "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+template <int BN>
+__device__ __forceinline__ void wgmma_tf32_rs(float* d, const float* a, uint64_t bdesc, int accumulate) {
+    static_assert(BN == 128 || BN == 160, "engine tile widths: 128, 160");
+    if constexpr (BN == 128) wgmma_tf32_rs_m64n128(d, a, bdesc, accumulate);
+    else wgmma_tf32_rs_m64n160(d, a, bdesc, accumulate);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// mbarrier / TMA
+// ---------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void mbar_init(uint32_t bar, int count) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, int bytes) {
+    asm volatile("mbarrier.expect_tx.relaxed.cta.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
+    uint32_t done;
+    asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+                 : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+    return done != 0;
+}
+__device__ __forceinline__ uint64_t globaltimer_ns() {
+    uint64_t t;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+    return t;
+}
+// Waits for the phase of `parity` to complete; false after HC_TIMEOUT_NS.  A correct pipeline waits microseconds at most,
+// so a timeout means a lost arrival: the kernel reports it and exits instead of hanging the GPU.
+constexpr uint64_t HC_TIMEOUT_NS = 4000000000ull;
+__device__ __forceinline__ bool mbar_wait(uint32_t bar, uint32_t parity) {
+    if (mbar_try_wait(bar, parity)) return true;
+    const uint64_t t0 = globaltimer_ns();
+    while (!mbar_try_wait(bar, parity))
+        if (globaltimer_ns() - t0 > HC_TIMEOUT_NS) return false;
+    return true;
+}
+// box (c0, c1, c2) of a 3D tensor map into shared memory; completes `bytes` on the mbarrier (out-of-bounds elements: 0)
+__device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4}], [%5];"
+                 ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(bar)
+                 : "memory");
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -291,6 +393,189 @@ inline int hg_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) 
 template <class Op>
 inline int hg_launch_bn(int bn, const Op& op, dim3 grid, cudaStream_t st, const char* who) {
     return bn == 160 ? hg_launch<160>(op, grid, st, who) : hg_launch<128>(op, grid, st, who);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// the conv engine: the same 3xTF32 GEMM, warp-specialised and fed by TMA
+// ---------------------------------------------------------------------------------------------------
+// For ops whose A operand is a K-contiguous activation tile [1 sample][128 times][32 channels] of x [B][T][Cin] (ConvOp
+// and its variants).  One CTA = one producer warpgroup + two consumer warpgroups, HC_STAGES stages, each with a full and
+// an empty mbarrier:
+//   * producer: thread 0 loads the A tile with TMA (op.a_box: the tap shift is in the t coordinate, and TMA's zero fill
+//     outside [0, T) is the conv's zero padding); all 128 threads fetch B through op.b4 into registers, split it into tf32
+//     hi/lo and store both into the stage (128-byte-swizzled K-major, as in hg_gemm_kernel);
+//   * consumers: warpgroup g reads its 64 raw fp32 A rows from the stage, splits them in registers with tf32_split and
+//     issues 4 x 3 wgmma with A from registers: lo*hi + hi*lo + hi*hi per k8 into a fresh `part` tile, which is added into
+//     `acc` with round-to-nearest FADDs per K block -- the pieces, MMA order and per-block adds of hg_gemm_kernel.
+// Shared-memory traffic per K block at BN = 160: A 16 KB written by TMA + 16 KB read, B hi/lo 40 KB written + 120 KB
+// read by the wgmmas (the register-staged loop also wrote A hi/lo and read A twice per MMA).
+constexpr int HC_THREADS = 384, HC_CONSUMERS = 256, HC_STAGES = 3;
+constexpr int HC_PRODUCER_REGS = 104, HC_CONSUMER_REGS = 200;    // 104 * 128 + 200 * 256 = 168 * 384 registers
+constexpr int HC_ERR_FULL = 901, HC_ERR_EMPTY = 902;           // status codes of a timed-out consumer / producer wait
+// one stage: A raw fp32 (128 rows) | B hi | B lo (BN rows each), every tile 1 KB-aligned for the 128-byte swizzle
+template <int BN> constexpr int hc_stage_bytes() { return HG_TILE_BYTES + 2 * BN * HG_BK * 4; }
+template <int BN> constexpr int hc_smem_bytes() { return HC_STAGES * hc_stage_bytes<BN>() + 1024; }
+
+// index of a consumer thread in [0, 256) and a barrier over the consumer warpgroups only (the producer has exited)
+__device__ __forceinline__ int hc_consumer_tid() { return threadIdx.x - (HC_THREADS - HC_CONSUMERS); }
+__device__ __forceinline__ void hc_consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(HC_CONSUMERS) : "memory"); }
+
+template <class Op, int BN>
+__global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_constant__ Op op,
+                                                               const __grid_constant__ CUtensorMap xmap) {
+    constexpr int NACC = BN / 2, STAGE = hc_stage_bytes<BN>(), B_TILE = BN * HG_BK * 4;
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ alignas(8) uint64_t bars[2 * HC_STAGES];         // full[s], empty[s]
+    const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
+    const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * HC_STAGES;
+    const int tid = threadIdx.x, wg = tid >> 7;
+    if (tid == 0) {
+        for (int s = 0; s < HC_STAGES; ++s) {
+            mbar_init(full0 + 8 * s, 128);                 // the producer's 128 threads (+ the TMA bytes)
+            mbar_init(empty0 + 8 * s, HC_CONSUMERS / 32);  // one arrival per consumer warp
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    const typename Op::Cta cta = op.template cta<BN>();
+    const int nkb = op.kblocks(cta);
+    if (wg == 0) {
+        // ---- producer
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HC_PRODUCER_REGS));
+        constexpr int NB4 = BN * HG_BK / 4 / 128;                 // float4 of B per thread per stage
+        int boff[NB4];                                            // this thread's B elements, the same in every K block
+        uint32_t live = 0;
+#pragma unroll
+        for (int j = 0; j < NB4; ++j) {
+            const int idx = tid + 128 * j, o = op.template b_col<BN>(cta, idx >> 3, idx & 7);
+            boff[j] = o < 0 ? 0 : o;                              // a column past the end loads column 0 and stores zeros
+            live |= (o >= 0 ? 1u : 0u) << j;
+        }
+        // one loop per weight format, so that the loads of a tile are issued back to back; the pre-split format moves
+        // the tile in 2 parts (2 loads per float4)
+        auto produce = [&](auto fmt) -> bool {
+            constexpr int FMT = decltype(fmt)::value, PART = FMT == Op::B_SPLIT ? NB4 / 2 : NB4;
+            for (int kb = 0; kb < nkb; ++kb) {
+                const int s = kb % HC_STAGES, use = kb / HC_STAGES;
+                if (use > 0 && !mbar_wait(empty0 + 8 * s, (use - 1) & 1)) return false;
+                const uint32_t st = base_u32 + s * STAGE, full = full0 + 8 * s;
+                if (tid == 0) {
+                    const int3 c = op.a_box(cta, kb);
+                    mbar_expect_tx(full, HG_TILE_BYTES);
+                    tma_load_3d(st, &xmap, c.x, c.y, c.z, full);
+                }
+                uint8_t* bh = smem + s * STAGE + HG_TILE_BYTES;
+                const long long base = op.b_base(cta, kb);
+#pragma unroll
+                for (int p = 0; p < NB4; p += PART) {
+                    float4 v[PART];
+#pragma unroll
+                    for (int j = 0; j < PART; ++j) v[j] = op.template b4<FMT>(cta, base + boff[p + j]);
+#pragma unroll
+                    for (int j = 0; j < PART; ++j) {
+                        const int idx = tid + 128 * (p + j);
+                        if (!((live >> (p + j)) & 1)) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
+                        HgSlot<true, BN>::store(bh, bh + B_TILE, idx >> 3, idx & 7, v[j]);
+                    }
+                }
+                fence_proxy_async();                               // the generic-proxy stores, before the wgmmas read them
+                mbar_arrive(full);
+            }
+            return true;
+        };
+        const int f = op.b_format();
+        const bool ok = f == Op::B_RAW     ? produce(std::integral_constant<int, Op::B_RAW>())
+                        : f == Op::B_SPLIT ? produce(std::integral_constant<int, Op::B_SPLIT>())
+                                           : produce(std::integral_constant<int, Op::B_F16>());
+        if (!ok && op.err) atomicCAS(op.err, 0, HC_ERR_EMPTY);
+        return;
+    }
+    // ---- consumers
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HC_CONSUMER_REGS));
+    const int cg = wg - 1, lane = tid & 31, grp = lane >> 2, tq = lane & 3;
+    const int r0 = 64 * cg + 16 * ((tid >> 5) & 3) + grp;        // A rows r0 and r0 + 8 of the fragment; r0 & 7 = grp
+    float acc[NACC], part[NACC];
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb % HC_STAGES, use = kb / HC_STAGES;
+        if (!mbar_wait(full0 + 8 * s, use & 1)) {
+            if (op.err) atomicCAS(op.err, 0, HC_ERR_FULL);
+            return;
+        }
+        const float* at = reinterpret_cast<const float*>(smem + s * STAGE);
+        float hi[4][4], lo[4][4];                   // [k8][fragment element]
+#pragma unroll
+        for (int kk = 0; kk < HG_BK / 8; ++kk) {
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {           // element e: row r0 + 8 (e & 1), 16-byte chunk 2 kk + (e >> 1), word tq
+                const int r = r0 + 8 * (e & 1), q = 2 * kk + (e >> 1);
+                tf32_split(at[r * 32 + ((q ^ grp) << 2) + tq], hi[kk][e], lo[kk][e]);
+            }
+        }
+        const uint32_t b_hi = base_u32 + s * STAGE + HG_TILE_BYTES, b_lo = b_hi + B_TILE;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < HG_BK / 8; ++kk) {
+            const uint32_t off = kk * 32;
+            const uint64_t dbh = wgmma_desc_k_sw128(b_hi + off), dbl = wgmma_desc_k_sw128(b_lo + off);
+            wgmma_tf32_rs<BN>(part, lo[kk], dbh, kk != 0);
+            wgmma_tf32_rs<BN>(part, hi[kk], dbl, 1);
+            wgmma_tf32_rs<BN>(part, hi[kk], dbh, 1);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty0 + 8 * s);
+#pragma unroll
+        for (int i = 0; i < NACC; ++i) acc[i] += part[i];
+    }
+    op.template epilogue<BN>(cta, acc, 64 * cg);
+}
+
+// x [B][T][Cin] fp32 as a 3D tensor map with a [1][128][32] box, 128-byte swizzle, zero fill out of bounds
+inline int hc_x_map(CUtensorMap* m, const float* x, int B, int T, int Cin, const char* who) {
+    using Encode = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
+                                const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
+                                CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+    static Encode encode = []() -> Encode {          // the driver's encoder, without linking libcuda
+        void* fn = nullptr;
+        cudaDriverEntryPointQueryResult q;
+        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &q) != cudaSuccess ||
+            q != cudaDriverEntryPointSuccess)
+            return nullptr;
+        return reinterpret_cast<Encode>(fn);
+    }();
+    if (!encode) return set_error(3, "%s: cuTensorMapEncodeTiled is not available%s", who);
+    if (reinterpret_cast<uintptr_t>(x) & 15) return set_error(2, "%s: x must be 16-byte aligned%s", who);
+    const cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)T, (cuuint64_t)B};
+    const cuuint64_t strides[2] = {(cuuint64_t)Cin * 4, (cuuint64_t)T * Cin * 4};
+    const cuuint32_t box[3] = {HG_BK, HG_BM, 1}, elem[3] = {1, 1, 1};
+    const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, elem,
+                              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return set_error(2, "%s: cuTensorMapEncodeTiled failed%s", who);
+    return 0;
+}
+
+template <int BN, class Op>
+inline int hc_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) {
+    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hc_conv_kernel<Op, BN>), hc_smem_bytes<BN>())) return rc;
+    if (grid.x == 0 || grid.y == 0 || grid.z == 0) return 0;
+    if (grid.y > 65535 || grid.z > 65535) return set_error(2, "%s: grid too large%s", who);
+    CUtensorMap xmap;
+    if (int rc = hc_x_map(&xmap, op.x, op.B, op.T, op.Cin, who)) return rc;
+    hc_conv_kernel<Op, BN><<<grid, HC_THREADS, hc_smem_bytes<BN>(), st>>>(op, xmap);
+    ++g_launches;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", who, cudaGetErrorString(e));
+    return 0;
+}
+template <class Op>
+inline int hc_launch_bn(int bn, const Op& op, dim3 grid, cudaStream_t st, const char* who) {
+    return bn == 160 ? hc_launch<160>(op, grid, st, who) : hc_launch<128>(op, grid, st, who);
 }
 
 // the plain epilogue: D[z plane][row][col] = acc for rows < rows, cols < cols (row-major, leading dimension ld)

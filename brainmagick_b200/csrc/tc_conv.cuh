@@ -4,10 +4,12 @@
 //   y[b, t, n] = bias[n] + sum_{tap} sum_{k} x[b, t + shift(tap), k] * W[wset(b)][tap][n][k]      (channels-last x, y)
 //
 // shift(tap) = sign * (tap - taps/2) * dilation; a shifted time outside [0, T) reads zeros (the conv's zero padding, never
-// the neighbouring sample).  One CTA = 128 times of one sample x 128 output columns (GLU: 64 'a' columns and the 64 gate
-// columns they pair with, so that a * sigmoid(gate) is formed in registers).  The weights arrive either as fp32
-// [sets][taps][Ntot][Cin] or as the two fp16 pieces of a power-of-two-scaled copy (bm_tc_weight_split_f16), which are
-// summed back on load (~22 significant bits of the weight: the precision the pieces carry).  Fused epilogue: bias, addend (skip gradient / in-place accumulate),
+// the neighbouring sample: the activation tile is a TMA box of one sample).  Runs on hc_conv_kernel of tc_common.cuh.  One
+// CTA = 128 times of one sample x BN output columns, BN = hg_pick_bn(Ntot): 160 for the 320- and 640-wide layers, 128 for
+// 1024 (GLU: BN/2 'a' columns and the BN/2 gate columns they pair with, so that a * sigmoid(gate) is formed in registers).
+// The weights arrive as raw fp32 [sets][taps][Ntot][Cin], as its two tf32 pieces (bm_tc_weight_split) or as the two fp16
+// pieces of a power-of-two-scaled copy (bm_tc_weight_split_f16); the pieces are summed back on load (fp16: ~22 significant
+// bits of the weight, the precision the pieces carry).  Fused epilogue: bias, addend (skip gradient / in-place accumulate),
 // pre-activation copy, exact GELU, channel-major store, GLU, BatchNorm column statistics (fp64), max |output|.
 #pragma once
 #include <cuda_fp16.h>
@@ -40,7 +42,6 @@ __host__ __device__ __forceinline__ float f16_scale_of(float amax) {
 }
 
 struct ConvOp {
-    static constexpr bool A_KCONTIG = true, B_KCONTIG = true;
     const float* x;                       // [B, T, Cin]
     const float* w;                       // fp32 weights [sets][taps][Ntot][Cin], or null: fp16 pieces below
     const float* w_lo32;                  // nullable: second tf32 piece of w (bm_tc_weight_split), added back on load
@@ -58,10 +59,7 @@ struct ConvOp {
     int* err;
 
     struct Cta { int b, t0, n_tile, wbase; float w_inv; };
-    // 128 columns: with the engine's current main loop (every thread stages its operands through registers), 160-wide
-    // tiles run the 320-wide conv slower than 128-wide ones although they skip the 64 padding columns
     template <int BN> __device__ Cta cta() const {
-        static_assert(BN == HG_BN, "ConvOp tiles are 128 columns wide");
         Cta c;
         c.b = blockIdx.x / ttiles;
         c.t0 = (blockIdx.x - c.b * ttiles) * HG_BM;
@@ -76,29 +74,38 @@ struct ConvOp {
         return c;
     }
     __device__ int kblocks(const Cta&) const { return taps * (Cin / HG_BK); }
-    __device__ float4 a4(const Cta& c, int kb, int r, int q) const {
+    // TMA box (channel k0, time, sample) of the A tile of K block kb: the tile's times shifted by the tap.  Shifted times
+    // outside [0, T) arrive as zeros; tile rows t >= T may read live times, but their outputs are never stored.
+    __device__ int3 a_box(const Cta& c, int kb) const {
         const int kch = Cin / HG_BK, tap = kb / kch, k0 = (kb - tap * kch) * HG_BK;
-        const int t = c.t0 + r, ts = t + sign * (tap - taps / 2) * dilation;
-        if (t >= T || ts < 0 || ts >= T) return make_float4(0.f, 0.f, 0.f, 0.f);
-        return __ldg(reinterpret_cast<const float4*>(x + ((long long)c.b * T + ts) * Cin + k0) + q);
+        return make_int3(k0, c.t0 + sign * (tap - taps / 2) * dilation, c.b);
     }
-    // output column of tile column j (GLU: j < 64 'a' columns, j >= 64 their gates), -1 past the end
-    __device__ int col_of(const Cta& c, int j) const {
+    // output column of tile column j (GLU: j < BN/2 'a' columns, j >= BN/2 their gates), -1 past the end
+    template <int BN> __device__ int col_of(const Cta& c, int j) const {
         if (glu) {
-            const int H = Ntot / 2, cc = c.n_tile * 64 + (j & 63);
-            return cc < H ? cc + (j >= 64 ? H : 0) : -1;
+            const int H = Ntot / 2, cc = c.n_tile * (BN / 2) + (j % (BN / 2));
+            return cc < H ? cc + (j >= BN / 2 ? H : 0) : -1;
         }
-        const int n = c.n_tile * HG_BN + j;
+        const int n = c.n_tile * BN + j;
         return n < Ntot ? n : -1;
     }
-    __device__ float4 b4(const Cta& c, int kb, int j, int q) const {
-        const int n = col_of(c, j);
-        if (n < 0) return make_float4(0.f, 0.f, 0.f, 0.f);
+    // B operand, in three steps so that the producer can issue a whole tile's loads back to back:
+    //   b_col: element offset of (tile column j, k quad q) within a K block, -1 past the end (the same for every block);
+    //   b_base: element offset of K block kb;  b4<FMT>: the 4 fp32 weights at element offset `off`
+    enum { B_RAW, B_SPLIT, B_F16 };
+    __device__ int b_format() const { return w ? (w_lo32 ? B_SPLIT : B_RAW) : B_F16; }
+    template <int BN> __device__ int b_col(const Cta& c, int j, int q) const {
+        const int n = col_of<BN>(c, j);
+        return n < 0 ? -1 : n * Cin + 4 * q;
+    }
+    __device__ long long b_base(const Cta& c, int kb) const {
         const int kch = Cin / HG_BK, tap = kb / kch, k0 = (kb - tap * kch) * HG_BK;
-        const long long off = ((long long)(c.wbase + tap) * Ntot + n) * Cin + k0 + 4 * q;
-        if (w) {
+        return (long long)(c.wbase + tap) * Ntot * Cin + k0;
+    }
+    template <int FMT> __device__ float4 b4(const Cta& c, long long off) const {
+        if (FMT != B_F16) {
             float4 v = __ldg(reinterpret_cast<const float4*>(w + off));
-            if (w_lo32) {
+            if (FMT == B_SPLIT) {
                 const float4 l = __ldg(reinterpret_cast<const float4*>(w_lo32 + off));
                 v.x += l.x; v.y += l.y; v.z += l.z; v.w += l.w;
             }
@@ -110,17 +117,18 @@ struct ConvOp {
         return make_float4((h0.x + l0.x) * c.w_inv, (h0.y + l0.y) * c.w_inv, (h1.x + l1.x) * c.w_inv, (h1.y + l1.y) * c.w_inv);
     }
 
+    // run by the 256 consumer threads of hc_conv_kernel
     template <int BN> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
-        __shared__ double col_sums[2 * HG_BN];
+        __shared__ double col_sums[2 * BN];
         float am = 0.f;
         if (glu) {
             const int H = Ntot / 2;
 #pragma unroll
-            for (int i = 0; i < 32; ++i) {               // tile columns 0..63; the gate of column j is column j + 64
-                const int t = c.t0 + m0 + hg_row(i), cc = c.n_tile * 64 + hg_col(i);
+            for (int i = 0; i < BN / 4; ++i) {           // tile columns 0..BN/2-1; the gate of column j is column j + BN/2
+                const int t = c.t0 + m0 + hg_row(i), cc = c.n_tile * (BN / 2) + hg_col(i);
                 if (t >= T || cc >= H) continue;
                 const long long row = (long long)c.b * T + t;
-                float a = acc[i], g = acc[i + 32];
+                float a = acc[i], g = acc[i + BN / 4];
                 if (bias) { a += bias[cc]; g += bias[H + cc]; }
                 if (y) { y[row * Ntot + cc] = a; y[row * Ntot + H + cc] = g; }
                 const float o = a * sigmoid_f(g);
@@ -129,15 +137,15 @@ struct ConvOp {
             }
         } else {
             if (stats) {
-                for (int i = threadIdx.x; i < 2 * HG_BN; i += HG_THREADS) col_sums[i] = 0.0;
-                __syncthreads();
+                for (int i = hc_consumer_tid(); i < 2 * BN; i += HC_CONSUMERS) col_sums[i] = 0.0;
+                hc_consumer_sync();
             }
 #pragma unroll
-            for (int g = 0; g < 16; ++g) {
+            for (int g = 0; g < BN / 8; ++g) {
 #pragma unroll
                 for (int e = 0; e < 2; ++e) {
                     float s1 = 0.f, s2 = 0.f;
-                    const int j = 8 * g + 2 * (threadIdx.x & 3) + e, n = c.n_tile * HG_BN + j;
+                    const int j = 8 * g + 2 * (threadIdx.x & 3) + e, n = c.n_tile * BN + j;
 #pragma unroll
                     for (int h = 0; h < 2; ++h) {
                         const int i = 4 * g + 2 * h + e;
@@ -162,18 +170,18 @@ struct ConvOp {
                         }
                         if ((threadIdx.x & 31) < 4 && n < Ntot) {
                             atomicAdd(&col_sums[j], (double)s1);
-                            atomicAdd(&col_sums[HG_BN + j], (double)s2);
+                            atomicAdd(&col_sums[BN + j], (double)s2);
                         }
                     }
                 }
             }
             if (stats) {
-                __syncthreads();
-                for (int j = threadIdx.x; j < HG_BN; j += HG_THREADS) {
-                    const int n = c.n_tile * HG_BN + j;
+                hc_consumer_sync();
+                for (int j = hc_consumer_tid(); j < BN; j += HC_CONSUMERS) {
+                    const int n = c.n_tile * BN + j;
                     if (n < Ntot) {
                         atomicAdd(stats + n, col_sums[j]);
-                        atomicAdd(stats + Ntot + n, col_sums[HG_BN + j]);
+                        atomicAdd(stats + Ntot + n, col_sums[BN + j]);
                     }
                 }
             }
@@ -195,10 +203,10 @@ struct SensorMixBwdOp : ConvOp {
     const float* mask;
     template <int BN> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
 #pragma unroll
-        for (int g = 0; g < 16; ++g) {
+        for (int g = 0; g < BN / 8; ++g) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-                const int n = c.n_tile * HG_BN + 8 * g + 2 * (threadIdx.x & 3) + e;
+                const int n = c.n_tile * BN + 8 * g + 2 * (threadIdx.x & 3) + e;
                 if (n >= C) continue;
                 const float m = mask ? mask[n] : 1.f;
 #pragma unroll
@@ -224,12 +232,13 @@ inline int launch_conv_op(ConvOp o, cudaStream_t st, const char* who) {
     o.ttiles = (o.T + HG_BM - 1) / HG_BM;
     const long long ctas = (long long)o.B * o.ttiles;
     if (ctas >= (1ll << 31)) return set_error(2, "%s: too many rows%s", who);
-    const int ntiles = o.glu ? (o.Ntot / 2 + 63) / 64 : (o.Ntot + HG_BN - 1) / HG_BN;
+    const int bn = hg_pick_bn(o.Ntot);                   // GLU: BN/2 'a' columns and their gates per tile
+    const int ntiles = o.glu ? (o.Ntot / 2 + bn / 2 - 1) / (bn / 2) : (o.Ntot + bn - 1) / bn;
     if (o.stats) {
         cudaError_t em = cudaMemsetAsync(o.stats, 0, sizeof(double) * 2 * o.Ntot, st);
         if (em != cudaSuccess) return set_error(3, "%s: memset: %s", who, cudaGetErrorString(em));
     }
-    return hg_launch<HG_BN>(o, dim3((unsigned)ctas, (unsigned)ntiles, 1), st, who);
+    return hc_launch_bn(bn, o, dim3((unsigned)ctas, (unsigned)ntiles, 1), st, who);
 }
 
 // W[o][i][j] (nn.Conv1d layout) -> tf32-split K-major operands:
@@ -289,8 +298,8 @@ inline int launch_sensor_mix_bwd_tc(const float* du, const float* w_hi, const fl
     o.n_wsets = n_sets; o.wsel = wsel; o.y = dmeg; o.err = err; o.C = C; o.mask = mask;
     if ((long long)B * T >= (1ll << 31)) return set_error(2, "%s: too many rows%s", __func__);
     o.ttiles = (T + HG_BM - 1) / HG_BM;
-    return hg_launch<HG_BN>(o, dim3((unsigned)((long long)B * o.ttiles), (unsigned)((Cp + HG_BN - 1) / HG_BN), 1), st,
-                            __func__);
+    const int bn = hg_pick_bn(Cp);
+    return hc_launch_bn(bn, o, dim3((unsigned)((long long)B * o.ttiles), (unsigned)((Cp + bn - 1) / bn), 1), st, __func__);
 }
 
 }  // namespace tc

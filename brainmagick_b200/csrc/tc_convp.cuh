@@ -1,6 +1,6 @@
 // K3/K4/K5 (dilated Conv1d / Conv1d+GLU / head 1x1, forward and data gradient) with the RAW fp32 weights re-laid K-major
-// [Kw][Ntot][Cin] (bm_tc_weight_split with NULL lo pointers): the ConvOp GEMM of tc_conv.cuh, splitting both operands into
-// tf32 pieces on their way into shared memory.
+// [Kw][Ntot][Cin] (bm_tc_weight_split with NULL lo pointers): the ConvOp GEMM of tc_conv.cuh, whose producer warps split the
+// weights into tf32 pieces on their way into shared memory.
 //
 //   y[p, n] = bias[n] + sum_tap sum_k x[p + shift(tap), k] * W[tap][n][k]        p = b*T + t (channels-last rows)
 //
