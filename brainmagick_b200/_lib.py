@@ -82,7 +82,33 @@ SIGNATURES = {
     "bm_bn_act_skip_bwd": [P, P, P, P, P, P, I, L, I, I, F, P, P, P, P, P],
     "bm_clip_loss_bwd_cand": [P, P, P, P, P, P, I, I, L, I, P, P, P, P, P],
     "bm_clip_scores_bwd": [P, P, P, P, P, I, I, L, P, P, P, P, P, P],
+    # deterministic forms (deterministic() below) and their workspace size queries (which return long long floats)
+    "bm_col_stats_det_workspace": [L, I],
+    "bm_col_stats_det": [P, L, I, P, L, P, P],
+    "bm_col_sum_det_workspace": [L, I],
+    "bm_col_sum_det": [P, L, I, P, L, P, P],
+    "bm_bn_gelu_skip_bwd_det_workspace": [L, I],
+    "bm_bn_gelu_skip_bwd_det": [P, P, P, P, P, P, I, L, I, P, P, P, P, P, P, L, P],
+    "bm_bn_act_skip_bwd_det_workspace": [L, I],
+    "bm_bn_act_skip_bwd_det": [P, P, P, P, P, P, I, L, I, I, F, P, P, P, P, P, L, P],
+    "bm_glu_bwd_det_workspace": [L, I],
+    "bm_glu_bwd_det": [P, P, L, I, P, P, P, P, L, P],
+    "bm_conv1d_bwd_weight_det_workspace": [I, I, I, I, I],
+    "bm_conv1d_bwd_weight_det": [P, P, I, I, I, I, I, I, P, P, P, L, P],
+    "bm_initial_linear_bwd_det_workspace": [I, I, I, I],
+    "bm_initial_linear_bwd_det": [P, I, P, I, P, I, I, I, I, I, P, P, P, P, L, P],
+    "bm_sensor_chain_bwd_det_workspace": [I, I, I, I],
+    "bm_sensor_chain_bwd_det": [P, P, P, P, P, P, P, P, P, P, P, I, I, I, I, I, I, I, I, I, P, P, P, P, P, P, P, L, P],
+    "bm_attention_weights_bwd_det": [P, P, P, I, I, I, I, P, P, P],
+    "bm_head_bwd_params_det_workspace": [I, I, I, I],
+    "bm_head_bwd_params_det": [P, P, P, P, I, I, I, I, P, P, P, P, P, P, L, P],
+    "bm_head_bwd_det_workspace": [I, I, I, I],
+    "bm_head_bwd_det": [P, P, P, P, P, P, I, I, I, I, P, P, P, P, P, P, P, L, P],
+    "bm_candidate_inv_norms_det": [P, I, L, P, P, P],
+    "bm_clip_scores_det": [P, P, I, I, L, I, P, P, P, P, L, P, P],
+    "bm_clip_loss_fwd_det": [P, P, I, I, L, I, P, P, P, P, P, P, L, P, P],
 }
+
 
 _lib = None
 
@@ -115,7 +141,7 @@ def load():
     lib.bm_clip_workspace.argtypes = [I, I, L]
     for name, argtypes in SIGNATURES.items():
         fn = getattr(lib, name)          # AttributeError if the symbol is not exported
-        fn.restype = c_int
+        fn.restype = c_longlong if name.endswith("_det_workspace") else c_int
         fn.argtypes = argtypes
     _lib = lib
     return lib
@@ -134,6 +160,12 @@ def stream():
     """The current CUDA stream's handle (raw C accessors: torch.cuda.current_stream() builds a Stream object and resolves the
     device through several Python layers, 1.9 ms per step over the ~1 400 calls of one)."""
     return c_void_p(torch._C._cuda_getCurrentRawStream(torch._C._cuda_getDevice()))
+
+
+def deterministic() -> bool:
+    """True when every call should take its deterministic (`_det`) form: exactly when PyTorch's
+    torch.use_deterministic_algorithms(True) is in effect.  Read per call; the one place the host code asks."""
+    return torch.are_deterministic_algorithms_enabled()
 
 
 def launch_count() -> int:

@@ -17,7 +17,7 @@ import torch
 
 from . import _lib
 from ._lib import call, ptr, stream
-from .functional import _Conv, _empty, _round_up, tc_status_tensor
+from .functional import _Conv, _empty, _reducing_call, _round_up, tc_status_tensor
 
 ACT_GELU, ACT_LRELU, ACT_NONE = 0, 1, 2
 
@@ -162,7 +162,8 @@ class _ConvSequenceFn(torch.autograd.Function):
                 gconv: _Conv = rec["gconv"]
                 dh = _empty((B, T, gconv.cout), dout)
                 dgb = torch.empty((gconv.cout,), device=dout.device, dtype=torch.float32)
-                call("bm_glu_bwd", ptr(g), ptr(rec["h"]), rows, gconv.cout // 2, ptr(dh), ptr(dgb), None, st)
+                _reducing_call("bm_glu_bwd", dout, (rows, gconv.cout // 2), ptr(g), ptr(rec["h"]), rows, gconv.cout // 2,
+                               ptr(dh), ptr(dgb), None, st)
                 glu_grads[k] = gconv.backward_weight(dh, rec["x_new"], B, T, 1, dout, status, known_dbias=dgb)
                 g = _empty((B, T, gconv.cin), dout)
                 gconv.backward_data(dh, None, B, T, 1, g, status)
@@ -172,13 +173,14 @@ class _ConvSequenceFn(torch.autograd.Function):
                 dy = _empty((B, T, cout), dout)
                 dgamma, dbeta = _empty((cout,), dout), _empty((cout,), dout)
                 if rec["act"] == ACT_GELU:
-                    call("bm_bn_gelu_skip_bwd", ptr(g), ptr(rec["y"]), ptr(rec["mean"]), ptr(rec["invstd"]),
-                         ptr(gamma.contiguous()), ptr(beta.contiguous()), 1 if plan.training else 0, rows, cout, ptr(sums),
-                         ptr(dy), ptr(dgamma), ptr(dbeta), None, st)
+                    _reducing_call("bm_bn_gelu_skip_bwd", dout, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
+                                   ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()),
+                                   1 if plan.training else 0, rows, cout, ptr(sums), ptr(dy), ptr(dgamma), ptr(dbeta), None, st)
                 else:
-                    call("bm_bn_act_skip_bwd", ptr(g), ptr(rec["y"]), ptr(rec["mean"]), ptr(rec["invstd"]),
-                         ptr(gamma.contiguous()), ptr(beta.contiguous()), 1 if plan.training else 0, rows, cout,
-                         rec["act"], float(plan.act_slope), ptr(sums), ptr(dy), ptr(dgamma), ptr(dbeta), st)
+                    _reducing_call("bm_bn_act_skip_bwd", dout, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
+                                   ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()),
+                                   1 if plan.training else 0, rows, cout, rec["act"], float(plan.act_slope), ptr(sums), ptr(dy),
+                                   ptr(dgamma), ptr(dbeta), st)
             elif rec["act"] != ACT_NONE:
                 dy = _empty((B, T, cout), dout)
                 call("bm_bn_act_skip_bwd", ptr(g), ptr(rec["y"]), None, None, None, None, 0, rows, cout, rec["act"],

@@ -42,6 +42,69 @@ inline int pick_chunks(int Z, int tiles) {
 }
 inline int tiles_of(int M, int N) { return ((M + GBM - 1) / GBM) * ((N + GBN - 1) / GBN); }
 
+// ---- deterministic forms (the `_det` entry points) -------------------------------------------------------------------
+// Every floating-point reduction that the default entry points finish with atomics is split in two: each block stores its
+// partial row into a caller-owned [n_blocks][width] buffer, and reduce_rows_kernel sums the rows in index order.  The
+// split-batch FP32-FMA weight-gradient GEMMs store one partial plane per batch segment ([nseg][output], the segment count of
+// the atomic form, which follows the SM count) and sum the planes in segment order; the remaining split GEMMs (dheads over
+// the recordings, the FP32-FMA CLIP scores) run unsplit: one CTA per output tile adds onto the zeroed output exactly once.
+constexpr int COLSUM_RPB = 256, COLSTATS_RPB = 128;
+inline long long blocks_of(long long rows, int rpb) { return (rows + rpb - 1) / rpb; }
+inline long long colsum_ws_floats(long long rows, int C) { return blocks_of(rows, COLSUM_RPB) * C; }
+inline long long colstats_ws_floats(long long rows, int C) { return blocks_of(rows, COLSTATS_RPB) * 4ll * C; }  // fp64 [nb][2C]
+// BatchNorm backward reduce: the column-stationary kernel takes CS_ROWS_PER_BLOCK (96) rows per block, the generic one 128
+inline long long bn_bwd_ws_floats(long long rows, int C) { return blocks_of(rows, CS_ROWS_PER_BLOCK) * 4ll * C; }
+inline long long glu_bwd_ws_floats(long long rows, int H) { return blocks_of(rows, CS_ROWS_PER_BLOCK) * 2ll * H; }
+// batch segments of the split weight-gradient GEMMs (the atomic form's count); planes = segments x output elements
+inline int wgrad_segments(int B, int tiles) {
+    const int zchunk = (B + pick_chunks(B, tiles) - 1) / pick_chunks(B, tiles);
+    return (B + zchunk - 1) / zchunk;
+}
+inline long long planes_floats(int B, int M, int N, int taps = 1) {
+    return (long long)wgrad_segments(B, tiles_of(M, N) * taps) * M * N * taps;
+}
+inline long long head_ws_floats(int B, int T, int H, int F) {
+    return std::max({(long long)B * F, colsum_ws_floats((long long)B * T, 2 * H), planes_floats(B, 2 * H, F),
+                     planes_floats(B, 2 * H, H)});
+}
+
+template <class T>
+int reduce_rows(const T* part, long long n, int W, T* out, cudaStream_t st) {
+    reduce_rows_kernel<T><<<(W + 127) / 128, 128, 0, st>>>(part, n, W, out);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
+// out[c] = sum_r X[r*ld + c] over `rows` rows: atomically (part == NULL, out zeroed here) or through the partials `part`
+int colsum(const float* X, long long rows, int C, int ld, float* part, float* out, cudaStream_t st) {
+    dim3 grid((unsigned)blocks_of(rows, COLSUM_RPB), (C + 127) / 128);
+    if (!part) BM_CUDA(cudaMemsetAsync(out, 0, sizeof(float) * C, st));
+    if (ld == C) {
+        if (part) colsum_cl_kernel<true><<<grid, 128, 0, st>>>(X, part, rows, C, COLSUM_RPB);
+        else colsum_cl_kernel<<<grid, 128, 0, st>>>(X, out, rows, C, COLSUM_RPB);
+    } else {
+        if (part) colsum_strided_kernel<true><<<grid, 128, 0, st>>>(X, part, rows, C, ld, COLSUM_RPB);
+        else colsum_strided_kernel<<<grid, 128, 0, st>>>(X, out, rows, C, ld, COLSUM_RPB);
+    }
+    BM_CHECK_LAUNCH();
+    return part ? reduce_rows(part, (long long)grid.x, C, out, st) : 0;
+}
+
+// the split GEMM g (atomic form: g.D inside the output `out` of `elems` elements, g.atomic = 1) with one partial plane per
+// segment: segment s writes part[s * elems + (g.D - out) + ...]; sum_planes adds the planes in segment order
+cudaError_t launch_gemm_planes(GemmP g, const float* out, long long elems, float* part, cudaStream_t st) {
+    g.D = part + (g.D - out);
+    g.ldd_z = elems;
+    g.atomic = 0;
+    return launch_gemm(g, st);
+}
+int sum_planes(const float* part, int nseg, long long elems, float* out, cudaStream_t st) {
+    return reduce_rows(part, (long long)nseg, (int)elems, out, st);
+}
+
+#define BM_CHECK_WS(need)                                                                              \
+    BM_CHECK_ARG(workspace && workspace_floats >= (need) && (reinterpret_cast<uintptr_t>(workspace) & 7) == 0)
+
 }  // namespace
 
 // =================================================================================================
@@ -72,10 +135,9 @@ extern "C" int bm_attention_weights_fwd(const float* positions, const float* fre
     return 0;
 }
 
-extern "C" int bm_attention_weights_bwd(const float* dweights, const float* weights, const float* emb, int R,
-                                        int C, int O, int P, float* dscores, float* dheads, bm_stream_t stream) {
+static int attention_weights_bwd(const float* dweights, const float* weights, const float* emb, int R, int C, int O, int P,
+                                 float* dscores, float* dheads, bool det, cudaStream_t st) {
     BM_CHECK_ARG(dweights && weights && emb && dscores && dheads);
-    cudaStream_t st = ST(stream);
     int rows = R * O;
     softmax_bwd_kernel<<<(rows + 7) / 8, 256, 0, st>>>(weights, dweights, dscores, rows, C);
     BM_CHECK_LAUNCH();
@@ -83,12 +145,21 @@ extern "C" int bm_attention_weights_bwd(const float* dweights, const float* weig
     BM_CUDA(cudaMemsetAsync(dheads, 0, sizeof(float) * O * P, st));
     GemmP g = gemm_defaults();
     g.M = O; g.N = P; g.K = C; g.kchunk = C;
-    g.Z = R; g.zchunk = 1; g.nseg = R;
+    g.Z = R; g.zchunk = det ? R : 1; g.nseg = det ? 1 : R;
     g.A = dscores; g.lda_z = (long long)O * C; g.lda_m = C; g.lda_k = 1; g.a_mcontig = 0;
     g.B = emb; g.ldb_z = (long long)C * P; g.ldb_n = 1; g.ldb_k = P; g.b_ncontig = 1;
     g.D = dheads; g.ldd_z = 0; g.ldd_m = P; g.ldd_n = 1; g.atomic = 1;
     BM_CUDA(launch_gemm(g, st));
     return 0;
+}
+
+extern "C" int bm_attention_weights_bwd(const float* dweights, const float* weights, const float* emb, int R,
+                                        int C, int O, int P, float* dscores, float* dheads, bm_stream_t stream) {
+    return attention_weights_bwd(dweights, weights, emb, R, C, O, P, dscores, dheads, false, ST(stream));
+}
+extern "C" int bm_attention_weights_bwd_det(const float* dweights, const float* weights, const float* emb, int R,
+                                            int C, int O, int P, float* dscores, float* dheads, bm_stream_t stream) {
+    return attention_weights_bwd(dweights, weights, emb, R, C, O, P, dscores, dheads, true, ST(stream));
 }
 
 // =================================================================================================
@@ -176,11 +247,10 @@ extern "C" int bm_subject_layers_bwd(const float* dx0, int ld_x0, const float* v
     return 0;
 }
 
-extern "C" int bm_initial_linear_bwd(const float* dv, int ld_dv, const float* u, int ld_u, const float* il_w, int B, int T,
-                                     int O, int IL, int ld_du, float* du, float* d_il_w, float* d_il_b,
-                                     bm_stream_t stream) {
+// part: NULL (atomic reductions) or the colsum_ws_floats(B*T, IL) partials of the deterministic form
+static int initial_linear_bwd(const float* dv, int ld_dv, const float* u, int ld_u, const float* il_w, int B, int T, int O,
+                              int IL, int ld_du, float* du, float* d_il_w, float* d_il_b, float* part, cudaStream_t st) {
     BM_CHECK_ARG(dv && u && il_w && du && d_il_w && d_il_b && ld_dv >= IL && ld_u >= O && ld_du >= O);
-    cudaStream_t st = ST(stream);
     {   // d_il_w[p][o] = sum_{b,t} dv[b][t][p] u[b][t][o]
         BM_CUDA(cudaMemsetAsync(d_il_w, 0, sizeof(float) * IL * O, st));
         GemmP g = gemm_defaults();
@@ -190,9 +260,16 @@ extern "C" int bm_initial_linear_bwd(const float* dv, int ld_dv, const float* u,
         g.A = dv; g.lda_z = (long long)T * ld_dv; g.lda_m = 1; g.lda_k = ld_dv; g.a_mcontig = 1;
         g.B = u; g.ldb_z = (long long)T * ld_u; g.ldb_n = 1; g.ldb_k = ld_u; g.b_ncontig = 1;
         g.D = d_il_w; g.ldd_z = 0; g.ldd_m = O; g.ldd_n = 1; g.atomic = 1;
-        BM_CUDA(launch_gemm(g, st));
+        if (part) {
+            BM_CUDA(launch_gemm_planes(g, d_il_w, (long long)IL * O, part, st));
+            if (int rc = sum_planes(part, g.nseg, (long long)IL * O, d_il_w, st)) return rc;
+        } else {
+            BM_CUDA(launch_gemm(g, st));
+        }
     }
-    {   // d_il_b[p] = sum dv
+    if (part) {   // d_il_b[p] = sum dv, through the partials
+        if (int rc = colsum(dv, (long long)B * T, IL, ld_dv, part, d_il_b, st)) return rc;
+    } else {   // d_il_b[p] = sum dv
         BM_CUDA(cudaMemsetAsync(d_il_b, 0, sizeof(float) * IL, st));
         GemmP g = gemm_defaults();                      // column sums as a 1-row GEMM would waste a tile: dedicated kernel
         (void)g;
@@ -210,6 +287,23 @@ extern "C" int bm_initial_linear_bwd(const float* dv, int ld_dv, const float* u,
         BM_CUDA(launch_gemm(g, st));
     }
     return 0;
+}
+
+extern "C" int bm_initial_linear_bwd(const float* dv, int ld_dv, const float* u, int ld_u, const float* il_w, int B, int T,
+                                     int O, int IL, int ld_du, float* du, float* d_il_w, float* d_il_b,
+                                     bm_stream_t stream) {
+    return initial_linear_bwd(dv, ld_dv, u, ld_u, il_w, B, T, O, IL, ld_du, du, d_il_w, d_il_b, nullptr, ST(stream));
+}
+extern "C" long long bm_initial_linear_bwd_det_workspace(int B, int T, int O, int IL) {
+    if (B <= 0 || T <= 0 || O <= 0 || IL <= 0) return 0;
+    return std::max(colsum_ws_floats((long long)B * T, IL), planes_floats(B, IL, O));
+}
+extern "C" int bm_initial_linear_bwd_det(const float* dv, int ld_dv, const float* u, int ld_u, const float* il_w, int B, int T,
+                                         int O, int IL, int ld_du, float* du, float* d_il_w, float* d_il_b, float* workspace,
+                                         long long workspace_floats, bm_stream_t stream) {
+    BM_CHECK_ARG(B > 0 && T > 0 && O > 0 && IL > 0);
+    BM_CHECK_WS(bm_initial_linear_bwd_det_workspace(B, T, O, IL));
+    return initial_linear_bwd(dv, ld_dv, u, ld_u, il_w, B, T, O, IL, ld_du, du, d_il_w, d_il_b, workspace, ST(stream));
 }
 
 extern "C" int bm_sensor_mix_bwd(const float* du, int ld_du, const float* meg, const int* rec_order, const int* rec_off,
@@ -253,6 +347,27 @@ extern "C" int bm_sensor_chain_bwd(const float* dx0, const float* meg, const flo
     int rc = bm_subject_layers_bwd(dx0, ld_x0, v, IL, subj_w, subject, subj_order, subj_off, B, T, IL, D, S, IL, dv,
                                    d_subj_w, stream);
     if (!rc) rc = bm_initial_linear_bwd(dv, IL, u, O, il_w, B, T, O, IL, O, du, d_il_w, d_il_b, stream);
+    if (!rc) rc = bm_sensor_mix_bwd(du, O, meg, rec_order, rec_off, B, C, T, O, R, d_weights, stream);
+    return rc;
+}
+
+extern "C" long long bm_sensor_chain_bwd_det_workspace(int B, int T, int O, int IL) {
+    return bm_initial_linear_bwd_det_workspace(B, T, O, IL);
+}
+extern "C" int bm_sensor_chain_bwd_det(const float* dx0, const float* meg, const float* il_w, const float* subj_w,
+                                       const int* subject, const float* u, const float* v, const int* subj_order,
+                                       const int* subj_off, const int* rec_order, const int* rec_off, int B, int C,
+                                       int T, int O, int IL, int D, int ld_x0, int S, int R, float* dv, float* du,
+                                       float* d_subj_w, float* d_il_w, float* d_il_b, float* d_weights, float* workspace,
+                                       long long workspace_floats, bm_stream_t stream) {
+    BM_CHECK_ARG(dx0 && meg && il_w && subj_w && subject && u && v && subj_order && subj_off && rec_order && rec_off);
+    BM_CHECK_ARG(dv && du && d_subj_w && d_il_w && d_il_b && d_weights);
+    BM_CHECK_ARG(ld_x0 >= D);
+    // the subject and sensor-mix gradients reduce each segment inside one CTA: already fixed-order
+    int rc = bm_subject_layers_bwd(dx0, ld_x0, v, IL, subj_w, subject, subj_order, subj_off, B, T, IL, D, S, IL, dv,
+                                   d_subj_w, stream);
+    if (!rc) rc = bm_initial_linear_bwd_det(dv, IL, u, O, il_w, B, T, O, IL, O, du, d_il_w, d_il_b, workspace,
+                                            workspace_floats, stream);
     if (!rc) rc = bm_sensor_mix_bwd(du, O, meg, rec_order, rec_off, B, C, T, O, R, d_weights, stream);
     return rc;
 }
@@ -349,22 +464,28 @@ extern "C" int bm_bn_gelu_skip_fwd(const float* y, const float* mean, const floa
     return 0;
 }
 
-extern "C" int bm_bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd,
-                                   const float* gamma, const float* beta, int batch_stats, long long rows, int C,
-                                   double* sums, float* dy, float* dgamma, float* dbeta, float* amax_out,
-                                   bm_stream_t stream) {
+// part: NULL (fp64 atomics into sums) or the bn_bwd_ws_floats(rows, C) partials of the deterministic form
+static int bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                            const float* beta, int batch_stats, long long rows, int C, double* sums, float* dy, float* dgamma,
+                            float* dbeta, float* amax_out, double* part, cudaStream_t st) {
     BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && sums && dy && dgamma && dbeta && rows > 0 && C > 0);
-    cudaStream_t st = ST(stream);
-    BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
+    if (!part) BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
     if (int rc = amax_begin(amax_out, st)) return rc;
     const long long total = rows * C;
     const bool vec = (C % 4 == 0) && aligned16(g, y, dy) && aligned16(mean, invstd, gamma) && aligned16(beta);
     if (vec && C / 4 <= 256 && aligned16(dgamma, dbeta)) {
         const int cx = C / 4, ry = std::max(1, 320 / cx);
         const unsigned nblk = (unsigned)((rows + CS_ROWS_PER_BLOCK - 1) / CS_ROWS_PER_BLOCK);
-        bn_gelu_bwd_reduce_cs_kernel<<<nblk, dim3(cx, ry), sizeof(float) * 2 * C * ry, st>>>(g, y, mean, invstd, gamma, beta,
-                                                                                          sums, rows, C);
-        BM_CHECK_LAUNCH();
+        if (part) {
+            bn_gelu_bwd_reduce_cs_kernel<true><<<nblk, dim3(cx, ry), sizeof(float) * 2 * C * ry, st>>>(
+                g, y, mean, invstd, gamma, beta, part, rows, C);
+            BM_CHECK_LAUNCH();
+            if (int rc = reduce_rows(part, (long long)nblk, 2 * C, sums, st)) return rc;
+        } else {
+            bn_gelu_bwd_reduce_cs_kernel<<<nblk, dim3(cx, ry), sizeof(float) * 2 * C * ry, st>>>(g, y, mean, invstd, gamma,
+                                                                                              beta, sums, rows, C);
+            BM_CHECK_LAUNCH();
+        }
         bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
         BM_CHECK_LAUNCH();
         bn_gelu_bwd_apply_cs_kernel<<<nblk, dim3(cx, ry), 0, st>>>(g, y, mean, invstd, gamma, beta, dgamma, dbeta,
@@ -376,9 +497,15 @@ extern "C" int bm_bn_gelu_skip_bwd(const float* g, const float* y, const float* 
     {   // generic shapes: one thread per column, 128 rows per block
         const int rpb = 128;
         dim3 grid((unsigned)((rows + rpb - 1) / rpb), (C + 127) / 128);
-        bn_gelu_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C, rpb);
+        if (part) {
+            bn_gelu_bwd_reduce_kernel<true><<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, part, rows, C, rpb);
+            BM_CHECK_LAUNCH();
+            if (int rc = reduce_rows(part, (long long)grid.x, 2 * C, sums, st)) return rc;
+        } else {
+            bn_gelu_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C, rpb);
+            BM_CHECK_LAUNCH();
+        }
     }
-    BM_CHECK_LAUNCH();
     bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
     BM_CHECK_LAUNCH();
     if (vec)
@@ -395,6 +522,26 @@ extern "C" int bm_bn_gelu_skip_bwd(const float* g, const float* y, const float* 
     return 0;
 }
 
+extern "C" int bm_bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd,
+                                   const float* gamma, const float* beta, int batch_stats, long long rows, int C,
+                                   double* sums, float* dy, float* dgamma, float* dbeta, float* amax_out,
+                                   bm_stream_t stream) {
+    return bn_gelu_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, sums, dy, dgamma, dbeta, amax_out, nullptr,
+                            ST(stream));
+}
+extern "C" long long bm_bn_gelu_skip_bwd_det_workspace(long long rows, int C) {
+    return rows > 0 && C > 0 ? bn_bwd_ws_floats(rows, C) : 0;
+}
+extern "C" int bm_bn_gelu_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd,
+                                       const float* gamma, const float* beta, int batch_stats, long long rows, int C,
+                                       double* sums, float* dy, float* dgamma, float* dbeta, float* amax_out,
+                                       float* workspace, long long workspace_floats, bm_stream_t stream) {
+    BM_CHECK_ARG(rows > 0 && C > 0);
+    BM_CHECK_WS(bn_bwd_ws_floats(rows, C));
+    return bn_gelu_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, sums, dy, dgamma, dbeta, amax_out,
+                            reinterpret_cast<double*>(workspace), ST(stream));
+}
+
 extern "C" int bm_conv1d_bwd_data(const float* dy, const float* wb, const float* addend, int B, int T, int Cin,
                                   int Cout, int Kw, int dilation, float* dx, bm_stream_t stream) {
     BM_CHECK_ARG(dy && wb && dx && B > 0 && T > 0 && Cin > 0 && Cout > 0 && dilation >= 1);
@@ -402,11 +549,11 @@ extern "C" int bm_conv1d_bwd_data(const float* dy, const float* wb, const float*
                      ST(stream));
 }
 
-extern "C" int bm_conv1d_bwd_weight(const float* dy, const float* x, int B, int T, int Cin, int Cout, int Kw,
-                                    int dilation, float* dw, float* dbias, bm_stream_t stream) {
+// part: NULL (atomic reductions) or the colsum_ws_floats(B*T, Cout) partials of the deterministic form
+static int conv1d_bwd_weight(const float* dy, const float* x, int B, int T, int Cin, int Cout, int Kw, int dilation, float* dw,
+                             float* dbias, float* part, cudaStream_t st) {
     BM_CHECK_ARG(dy && x && dw && B > 0 && T > 0 && Cin > 0 && Cout > 0 && Kw >= 1 && Kw <= 3);
-    cudaStream_t st = ST(stream);
-    BM_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * (size_t)Cout * Cin * Kw, st));
+    if (!part) BM_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * (size_t)Cout * Cin * Kw, st));
     int nseg = pick_chunks(B, tiles_of(Cout, Cin) * Kw);
     int zchunk = (B + nseg - 1) / nseg;
     nseg = (B + zchunk - 1) / zchunk;
@@ -418,7 +565,12 @@ extern "C" int bm_conv1d_bwd_weight(const float* dy, const float* x, int B, int 
         g.B = x; g.ldb_z = (long long)T * Cin; g.ldb_n = 1; g.ldb_k = Cin; g.b_ncontig = 1;
         g.b_shift_k[0] = (j - Kw / 2) * dilation;
         g.D = dw + j; g.ldd_z = 0; g.ldd_m = (long long)Cin * Kw; g.ldd_n = Kw; g.atomic = 1;
-        BM_CUDA(launch_gemm(g, st));
+        if (part) BM_CUDA(launch_gemm_planes(g, dw, (long long)Cout * Cin * Kw, part, st));
+        else BM_CUDA(launch_gemm(g, st));
+    }
+    if (part) {                                     // every tap's planes are written: sum them, then the bias (reusing part)
+        if (int rc = sum_planes(part, nseg, (long long)Cout * Cin * Kw, dw, st)) return rc;
+        return dbias ? colsum(dy, (long long)B * T, Cout, Cout, part, dbias, st) : 0;
     }
     if (dbias) {
         BM_CUDA(cudaMemsetAsync(dbias, 0, sizeof(float) * Cout, st));
@@ -430,21 +582,43 @@ extern "C" int bm_conv1d_bwd_weight(const float* dy, const float* x, int B, int 
     return 0;
 }
 
+extern "C" int bm_conv1d_bwd_weight(const float* dy, const float* x, int B, int T, int Cin, int Cout, int Kw,
+                                    int dilation, float* dw, float* dbias, bm_stream_t stream) {
+    return conv1d_bwd_weight(dy, x, B, T, Cin, Cout, Kw, dilation, dw, dbias, nullptr, ST(stream));
+}
+extern "C" long long bm_conv1d_bwd_weight_det_workspace(int B, int T, int Cin, int Cout, int Kw) {
+    if (B <= 0 || T <= 0 || Cin <= 0 || Cout <= 0 || Kw <= 0) return 0;
+    return std::max(colsum_ws_floats((long long)B * T, Cout), planes_floats(B, Cout, Cin, Kw));
+}
+extern "C" int bm_conv1d_bwd_weight_det(const float* dy, const float* x, int B, int T, int Cin, int Cout, int Kw,
+                                        int dilation, float* dw, float* dbias, float* workspace, long long workspace_floats,
+                                        bm_stream_t stream) {
+    BM_CHECK_ARG(B > 0 && T > 0 && Cin > 0 && Cout > 0 && Kw >= 1 && Kw <= 3);
+    BM_CHECK_WS(bm_conv1d_bwd_weight_det_workspace(B, T, Cin, Cout, Kw));
+    return conv1d_bwd_weight(dy, x, B, T, Cin, Cout, Kw, dilation, dw, dbias, workspace, ST(stream));
+}
+
 extern "C" int bm_conv1d_glu_fwd(const float* x, const float* wf, const float* bias, int B, int T, int Cin, int H,
                                  int Kw, float* h, float* out, bm_stream_t stream) {
     BM_CHECK_ARG(x && wf && out && B > 0 && T > 0 && Cin > 0 && H > 0);
     return conv_gemm(x, wf, bias, nullptr, B, T, Cin, 2 * H, Kw, 1, +1, h, nullptr, 1, out, ST(stream));
 }
 
-extern "C" int bm_glu_bwd(const float* g, const float* h, long long rows, int H, float* dh, float* dbias,
-                          float* amax_out, bm_stream_t stream) {
+// part: NULL (atomic reductions) or the glu_bwd_ws_floats(rows, H) partials of the deterministic form
+static int glu_bwd(const float* g, const float* h, long long rows, int H, float* dh, float* dbias, float* amax_out, float* part,
+                   cudaStream_t st) {
     BM_CHECK_ARG(g && h && dh && rows > 0 && H > 0);
-    cudaStream_t st = ST(stream);
-    if (dbias) BM_CUDA(cudaMemsetAsync(dbias, 0, sizeof(float) * 2 * H, st));
+    if (dbias && !part) BM_CUDA(cudaMemsetAsync(dbias, 0, sizeof(float) * 2 * H, st));
     if (int rc = amax_begin(amax_out, st)) return rc;
     if (H % 4 == 0 && H / 4 <= 256 && aligned16(g, h, dh)) {
         const int cx = H / 4, ry = std::max(1, 320 / cx);
         const unsigned nblk = (unsigned)((rows + CS_ROWS_PER_BLOCK - 1) / CS_ROWS_PER_BLOCK);
+        if (dbias && part) {
+            glu_bwd_cs_kernel<true><<<nblk, dim3(cx, ry), sizeof(float) * 2 * H * ry, st>>>(
+                g, h, dh, part, rows, H, reinterpret_cast<unsigned int*>(amax_out));
+            BM_CHECK_LAUNCH();
+            return reduce_rows(part, (long long)nblk, 2 * H, dbias, st);
+        }
         glu_bwd_cs_kernel<<<nblk, dim3(cx, ry), dbias ? sizeof(float) * 2 * H * ry : 0, st>>>(
             g, h, dh, dbias, rows, H, reinterpret_cast<unsigned int*>(amax_out));
         BM_CHECK_LAUNCH();
@@ -456,13 +630,30 @@ extern "C" int bm_glu_bwd(const float* g, const float* h, long long rows, int H,
     else
         glu_bwd_kernel<<<ew_grid(rows * H), 256, 0, st>>>(g, h, dh, rows, H);
     BM_CHECK_LAUNCH();
-    if (dbias) {
+    if (dbias && part) {
+        if (int rc = colsum(dh, rows, 2 * H, 2 * H, part, dbias, st)) return rc;
+    } else if (dbias) {
         dim3 grid((unsigned)((rows + 255) / 256), (2 * H + 127) / 128);
         colsum_cl_kernel<<<grid, 128, 0, st>>>(dh, dbias, rows, 2 * H, 256);
         BM_CHECK_LAUNCH();
     }
     if (amax_out) return tc::launch_amax(dh, rows * 2 * H, amax_out, st);
     return 0;
+}
+
+extern "C" int bm_glu_bwd(const float* g, const float* h, long long rows, int H, float* dh, float* dbias,
+                          float* amax_out, bm_stream_t stream) {
+    return glu_bwd(g, h, rows, H, dh, dbias, amax_out, nullptr, ST(stream));
+}
+extern "C" long long bm_glu_bwd_det_workspace(long long rows, int H) {
+    // the column-stationary kernel's partial rows, or the colsum's for the generic kernels (fewer rows of 2H)
+    return rows > 0 && H > 0 ? glu_bwd_ws_floats(rows, H) : 0;
+}
+extern "C" int bm_glu_bwd_det(const float* g, const float* h, long long rows, int H, float* dh, float* dbias,
+                              float* amax_out, float* workspace, long long workspace_floats, bm_stream_t stream) {
+    BM_CHECK_ARG(rows > 0 && H > 0);
+    BM_CHECK_WS(glu_bwd_ws_floats(rows, H));
+    return glu_bwd(g, h, rows, H, dh, dbias, amax_out, workspace, ST(stream));
 }
 
 // =================================================================================================
@@ -496,15 +687,13 @@ extern "C" int bm_head_fwd(const float* x, const float* w0, const float* b0, con
 }
 
 // dW2, db2, dh1 = dq*GELU'(h1) (in place in dq), dW0, db0 -- the parameter-gradient half of the head backward
-extern "C" int bm_head_bwd_params(const float* dest, const float* x, const float* h1, const float* q, int B, int T,
-                                  int H, int F, float* dq, float* dw0, float* db0, float* dw2, float* db2,
-                                  bm_stream_t stream) {
+// part: NULL (atomic reductions) or the head_ws_floats(B, T, H, F) partials of the deterministic form
+static int head_bwd_params(const float* dest, const float* x, const float* h1, const float* q, int B, int T, int H, int F,
+                           float* dq, float* dw0, float* db0, float* dw2, float* db2, float* part, cudaStream_t st) {
     BM_CHECK_ARG(dest && x && h1 && q && dq && dw0 && db0 && dw2 && db2);
-    cudaStream_t st = ST(stream);
     const int H2 = 2 * H;
     const long long rows = (long long)B * T;
     {   // dw2[i][f] = sum_{b,t} q[b][t][i] dest[b][f][t]
-        BM_CUDA(cudaMemsetAsync(dw2, 0, sizeof(float) * (size_t)H2 * F, st));
         GemmP g = gemm_defaults();
         g.M = H2; g.N = F; g.K = T; g.kchunk = T;
         g.Z = B; g.nseg = pick_chunks(B, tiles_of(H2, F)); g.zchunk = (B + g.nseg - 1) / g.nseg;
@@ -512,18 +701,29 @@ extern "C" int bm_head_bwd_params(const float* dest, const float* x, const float
         g.A = q; g.lda_z = (long long)T * H2; g.lda_m = 1; g.lda_k = H2; g.a_mcontig = 1;
         g.B = dest; g.ldb_z = (long long)F * T; g.ldb_n = T; g.ldb_k = 1; g.b_ncontig = 0;
         g.D = dw2; g.ldd_m = F; g.ldd_n = 1; g.atomic = 1;
-        BM_CUDA(launch_gemm(g, st));
+        if (part) {
+            BM_CUDA(launch_gemm_planes(g, dw2, (long long)H2 * F, part, st));
+            if (int rc = sum_planes(part, g.nseg, (long long)H2 * F, dw2, st)) return rc;
+        } else {
+            BM_CUDA(cudaMemsetAsync(dw2, 0, sizeof(float) * (size_t)H2 * F, st));
+            BM_CUDA(launch_gemm(g, st));
+        }
     }
     {   // db2[f] = sum_{b,t} dest[b][f][t]
-        BM_CUDA(cudaMemsetAsync(db2, 0, sizeof(float) * F, st));
         long long nrows = (long long)B * F;
-        rowsum_cm_kernel<<<(unsigned)((nrows + 7) / 8), 256, 0, st>>>(dest, db2, B, F, T);
-        BM_CHECK_LAUNCH();
+        if (part) {
+            rowsum_cm_kernel<true><<<(unsigned)((nrows + 7) / 8), 256, 0, st>>>(dest, part, B, F, T);
+            BM_CHECK_LAUNCH();
+            if (int rc = reduce_rows(part, (long long)B, F, db2, st)) return rc;
+        } else {
+            BM_CUDA(cudaMemsetAsync(db2, 0, sizeof(float) * F, st));
+            rowsum_cm_kernel<<<(unsigned)((nrows + 7) / 8), 256, 0, st>>>(dest, db2, B, F, T);
+            BM_CHECK_LAUNCH();
+        }
     }
     gelu_bwd_kernel<<<ew_grid(rows * H2), 256, 0, st>>>(dq, h1, dq, rows * H2);   // dq <- dh1
     BM_CHECK_LAUNCH();
     {   // dw0[n][k] = sum_rows dh1[row][n] x[row][k]
-        BM_CUDA(cudaMemsetAsync(dw0, 0, sizeof(float) * (size_t)H2 * H, st));
         GemmP g = gemm_defaults();
         g.M = H2; g.N = H; g.K = T; g.kchunk = T;
         g.Z = B; g.nseg = pick_chunks(B, tiles_of(H2, H)); g.zchunk = (B + g.nseg - 1) / g.nseg;
@@ -531,8 +731,15 @@ extern "C" int bm_head_bwd_params(const float* dest, const float* x, const float
         g.A = dq; g.lda_z = (long long)T * H2; g.lda_m = 1; g.lda_k = H2; g.a_mcontig = 1;
         g.B = x; g.ldb_z = (long long)T * H; g.ldb_n = 1; g.ldb_k = H; g.b_ncontig = 1;
         g.D = dw0; g.ldd_m = H; g.ldd_n = 1; g.atomic = 1;
-        BM_CUDA(launch_gemm(g, st));
+        if (part) {
+            BM_CUDA(launch_gemm_planes(g, dw0, (long long)H2 * H, part, st));
+            if (int rc = sum_planes(part, g.nseg, (long long)H2 * H, dw0, st)) return rc;
+        } else {
+            BM_CUDA(cudaMemsetAsync(dw0, 0, sizeof(float) * (size_t)H2 * H, st));
+            BM_CUDA(launch_gemm(g, st));
+        }
     }
+    if (part) return colsum(dq, rows, H2, H2, part, db0, st);   // db0; the partials buffer is reused stage after stage
     {   // db0
         BM_CUDA(cudaMemsetAsync(db0, 0, sizeof(float) * H2, st));
         dim3 grid((unsigned)((rows + 255) / 256), (H2 + 127) / 128);
@@ -542,11 +749,26 @@ extern "C" int bm_head_bwd_params(const float* dest, const float* x, const float
     return 0;
 }
 
-extern "C" int bm_head_bwd(const float* dest, const float* x, const float* w0, const float* w2, const float* h1,
-                           const float* q, int B, int T, int H, int F, float* dq, float* dx, float* dw0,
-                           float* db0, float* dw2, float* db2, bm_stream_t stream) {
+extern "C" int bm_head_bwd_params(const float* dest, const float* x, const float* h1, const float* q, int B, int T,
+                                  int H, int F, float* dq, float* dw0, float* db0, float* dw2, float* db2,
+                                  bm_stream_t stream) {
+    return head_bwd_params(dest, x, h1, q, B, T, H, F, dq, dw0, db0, dw2, db2, nullptr, ST(stream));
+}
+extern "C" long long bm_head_bwd_params_det_workspace(int B, int T, int H, int F) {
+    return B > 0 && T > 0 && H > 0 && F > 0 ? head_ws_floats(B, T, H, F) : 0;
+}
+extern "C" int bm_head_bwd_params_det(const float* dest, const float* x, const float* h1, const float* q, int B, int T,
+                                      int H, int F, float* dq, float* dw0, float* db0, float* dw2, float* db2,
+                                      float* workspace, long long workspace_floats, bm_stream_t stream) {
+    BM_CHECK_ARG(B > 0 && T > 0 && H > 0 && F > 0);
+    BM_CHECK_WS(head_ws_floats(B, T, H, F));
+    return head_bwd_params(dest, x, h1, q, B, T, H, F, dq, dw0, db0, dw2, db2, workspace, ST(stream));
+}
+
+static int head_bwd(const float* dest, const float* x, const float* w0, const float* w2, const float* h1, const float* q, int B,
+                    int T, int H, int F, float* dq, float* dx, float* dw0, float* db0, float* dw2, float* db2, float* part,
+                    cudaStream_t st) {
     BM_CHECK_ARG(dest && x && w0 && w2 && h1 && q && dq && dx && dw0 && db0 && dw2 && db2);
-    cudaStream_t st = ST(stream);
     const int H2 = 2 * H;
     const long long rows = (long long)B * T;
     {   // dq[b][t][i] = sum_f dest[b][f][t] w2[i][f]
@@ -558,7 +780,7 @@ extern "C" int bm_head_bwd(const float* dest, const float* x, const float* w0, c
         g.D = dq; g.ldd_z = (long long)T * H2; g.ldd_m = H2; g.ldd_n = 1;
         BM_CUDA(launch_gemm(g, st));
     }
-    int rc = bm_head_bwd_params(dest, x, h1, q, B, T, H, F, dq, dw0, db0, dw2, db2, stream);
+    int rc = head_bwd_params(dest, x, h1, q, B, T, H, F, dq, dw0, db0, dw2, db2, part, st);
     if (rc) return rc;
     {   // dx[row][k] = sum_n dh1[row][n] w0[n][k]
         GemmP g = gemm_defaults();
@@ -569,6 +791,23 @@ extern "C" int bm_head_bwd(const float* dest, const float* x, const float* w0, c
         BM_CUDA(launch_gemm(g, st));
     }
     return 0;
+}
+
+extern "C" int bm_head_bwd(const float* dest, const float* x, const float* w0, const float* w2, const float* h1,
+                           const float* q, int B, int T, int H, int F, float* dq, float* dx, float* dw0,
+                           float* db0, float* dw2, float* db2, bm_stream_t stream) {
+    return head_bwd(dest, x, w0, w2, h1, q, B, T, H, F, dq, dx, dw0, db0, dw2, db2, nullptr, ST(stream));
+}
+extern "C" long long bm_head_bwd_det_workspace(int B, int T, int H, int F) {
+    return bm_head_bwd_params_det_workspace(B, T, H, F);
+}
+extern "C" int bm_head_bwd_det(const float* dest, const float* x, const float* w0, const float* w2, const float* h1,
+                               const float* q, int B, int T, int H, int F, float* dq, float* dx, float* dw0,
+                               float* db0, float* dw2, float* db2, float* workspace, long long workspace_floats,
+                               bm_stream_t stream) {
+    BM_CHECK_ARG(B > 0 && T > 0 && H > 0 && F > 0);
+    BM_CHECK_WS(head_ws_floats(B, T, H, F));
+    return head_bwd(dest, x, w0, w2, h1, q, B, T, H, F, dq, dx, dw0, db0, dw2, db2, workspace, ST(stream));
 }
 
 // =================================================================================================
@@ -582,13 +821,13 @@ extern "C" long long bm_clip_workspace(int Bn, int Bc, long long KT) {
     return 2ll * Bc + 2;
 }
 
-extern "C" int bm_candidate_inv_norms(const float* cand, int Bc, long long KT, double* ss, float* inv_norm,
-                                      bm_stream_t stream) {
+// det: one block per candidate (one add per slot), else up to 32 K splits per candidate
+static int candidate_inv_norms(const float* cand, int Bc, long long KT, double* ss, float* inv_norm, bool det, cudaStream_t st) {
     BM_CHECK_ARG(cand && ss && inv_norm && Bc > 0 && KT > 0);
-    cudaStream_t st = ST(stream);
     BM_CUDA(cudaMemsetAsync(ss, 0, sizeof(double) * Bc, st));
     int splits = (int)((KT + 65535) / 65536);
     if (splits > 32) splits = 32;
+    if (det) splits = 1;
     row_sumsq_kernel<<<dim3(Bc, splits), 256, 0, st>>>(cand, ss, KT);
     BM_CHECK_LAUNCH();
     inv_norm_kernel<<<(Bc + 127) / 128, 128, 0, st>>>(ss, inv_norm, Bc);
@@ -596,28 +835,38 @@ extern "C" int bm_candidate_inv_norms(const float* cand, int Bc, long long KT, d
     return 0;
 }
 
+extern "C" int bm_candidate_inv_norms(const float* cand, int Bc, long long KT, double* ss, float* inv_norm,
+                                      bm_stream_t stream) {
+    return candidate_inv_norms(cand, Bc, KT, ss, inv_norm, false, ST(stream));
+}
+extern "C" int bm_candidate_inv_norms_det(const float* cand, int Bc, long long KT, double* ss, float* inv_norm,
+                                          bm_stream_t stream) {
+    return candidate_inv_norms(cand, Bc, KT, ss, inv_norm, true, ST(stream));
+}
+
 namespace {
 // scores (+ probs / row_loss / loss) on whichever kernel the shape allows
+// det: the candidate sums of squares one block per candidate, the FP32-FMA score GEMM without a K split
 int clip_forward(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given, int target_offset,
                  float* inv_norm, float* scores, float* probs, float* row_loss, float* loss, float* ws,
-                 long long ws_floats, int* status, cudaStream_t st) {
+                 long long ws_floats, int* status, bool det, cudaStream_t st) {
     BM_CHECK_ARG(est && cand && inv_norm && scores && ws && Bn > 0 && Bc > 0 && KT > 0);
     BM_CHECK_ARG(KT < (1ll << 31));
     BM_CHECK_ARG(ws_floats >= bm_clip_workspace(Bn, Bc, KT));
     BM_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 7) == 0);
     if (tc::clip_tc_supported(Bn, Bc, KT))
         return tc::launch_clip_scores(est, cand, Bn, Bc, KT, norms_given, target_offset, inv_norm, scores, probs, row_loss,
-                                      loss, ws, status, st);
+                                      loss, ws, status, st, det);
     // FP32-FMA GEMM (feature sizes not a multiple of 4 floats: no TMA row pitch)
     if (!norms_given) {
-        int rc = bm_candidate_inv_norms(cand, Bc, KT, reinterpret_cast<double*>(ws), inv_norm, st);
+        int rc = candidate_inv_norms(cand, Bc, KT, reinterpret_cast<double*>(ws), inv_norm, det, st);
         if (rc) return rc;
     }
     BM_CUDA(cudaMemsetAsync(scores, 0, sizeof(float) * (size_t)Bn * Bc, st));
     GemmP g = gemm_defaults();
     g.M = Bn; g.N = Bc; g.K = (int)KT;
     int tiles = tiles_of(Bn, Bc);
-    int ks = (2 * num_sms() + tiles - 1) / tiles;
+    int ks = det ? 1 : (2 * num_sms() + tiles - 1) / tiles;
     long long kchunk = (KT + ks - 1) / ks;
     kchunk = ((kchunk + GBK - 1) / GBK) * GBK;
     ks = (int)((KT + kchunk - 1) / kchunk);
@@ -643,7 +892,13 @@ extern "C" int bm_clip_scores(const float* est, const float* cand, int Bn, int B
                               float* inv_norm, float* scores, float* probs, float* workspace,
                               long long workspace_floats, int* status, bm_stream_t stream) {
     return clip_forward(est, cand, Bn, Bc, KT, norms_given, 0, inv_norm, scores, probs, nullptr, nullptr, workspace,
-                        workspace_floats, status, ST(stream));
+                        workspace_floats, status, false, ST(stream));
+}
+extern "C" int bm_clip_scores_det(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
+                                  float* inv_norm, float* scores, float* probs, float* workspace,
+                                  long long workspace_floats, int* status, bm_stream_t stream) {
+    return clip_forward(est, cand, Bn, Bc, KT, norms_given, 0, inv_norm, scores, probs, nullptr, nullptr, workspace,
+                        workspace_floats, status, true, ST(stream));
 }
 
 extern "C" int bm_clip_loss_fwd(const float* est, const float* cand, int Bn, int Bc, long long KT,
@@ -653,7 +908,16 @@ extern "C" int bm_clip_loss_fwd(const float* est, const float* cand, int Bn, int
     BM_CHECK_ARG(probs && row_loss && loss);
     BM_CHECK_ARG(target_offset >= 0 && target_offset + Bn <= Bc);
     return clip_forward(est, cand, Bn, Bc, KT, 0, target_offset, inv_norm, scores, probs, row_loss, loss, workspace,
-                        workspace_floats, status, ST(stream));
+                        workspace_floats, status, false, ST(stream));
+}
+extern "C" int bm_clip_loss_fwd_det(const float* est, const float* cand, int Bn, int Bc, long long KT,
+                                    int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss,
+                                    float* loss, float* workspace, long long workspace_floats, int* status,
+                                    bm_stream_t stream) {
+    BM_CHECK_ARG(probs && row_loss && loss);
+    BM_CHECK_ARG(target_offset >= 0 && target_offset + Bn <= Bc);
+    return clip_forward(est, cand, Bn, Bc, KT, 0, target_offset, inv_norm, scores, probs, row_loss, loss, workspace,
+                        workspace_floats, status, true, ST(stream));
 }
 
 namespace {
@@ -741,19 +1005,25 @@ extern "C" int bm_bn_act_skip_fwd(const float* y, const float* mean, const float
     return 0;
 }
 
-extern "C" int bm_bn_act_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd,
-                                  const float* gamma, const float* beta, int batch_stats, long long rows, int C,
-                                  int act, float slope, double* sums, float* dy, float* dgamma, float* dbeta,
-                                  bm_stream_t stream) {
+// part: NULL (fp64 atomics into sums) or the bn_bwd_ws_floats(rows, C) partials of the deterministic form
+static int bn_act_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                           const float* beta, int batch_stats, long long rows, int C, int act, float slope, double* sums,
+                           float* dy, float* dgamma, float* dbeta, double* part, cudaStream_t st) {
     BM_CHECK_ARG(g && y && dy && rows > 0 && C > 0 && act >= 0 && act <= 2);
     BM_CHECK_ARG(!mean || (invstd && gamma && beta && sums && dgamma && dbeta));
-    cudaStream_t st = ST(stream);
     if (mean) {
-        BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
         const int rpb = 128;
         dim3 grid((unsigned)((rows + rpb - 1) / rpb), (C + 127) / 128);
-        bn_act_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C, rpb, act, slope);
-        BM_CHECK_LAUNCH();
+        if (part) {
+            bn_act_bwd_reduce_kernel<true><<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, part, rows, C, rpb, act,
+                                                                 slope);
+            BM_CHECK_LAUNCH();
+            if (int rc = reduce_rows(part, (long long)grid.x, 2 * C, sums, st)) return rc;
+        } else {
+            BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
+            bn_act_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C, rpb, act, slope);
+            BM_CHECK_LAUNCH();
+        }
         bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
         BM_CHECK_LAUNCH();
     }
@@ -761,6 +1031,29 @@ extern "C" int bm_bn_act_skip_bwd(const float* g, const float* y, const float* m
                                                                batch_stats, dy, rows * C, C, act, slope);
     BM_CHECK_LAUNCH();
     return 0;
+}
+
+extern "C" int bm_bn_act_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd,
+                                  const float* gamma, const float* beta, int batch_stats, long long rows, int C,
+                                  int act, float slope, double* sums, float* dy, float* dgamma, float* dbeta,
+                                  bm_stream_t stream) {
+    return bn_act_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, sums, dy, dgamma, dbeta, nullptr,
+                           ST(stream));
+}
+extern "C" long long bm_bn_act_skip_bwd_det_workspace(long long rows, int C) {
+    return rows > 0 && C > 0 ? bn_bwd_ws_floats(rows, C) : 0;
+}
+extern "C" int bm_bn_act_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd,
+                                      const float* gamma, const float* beta, int batch_stats, long long rows, int C,
+                                      int act, float slope, double* sums, float* dy, float* dgamma, float* dbeta,
+                                      float* workspace, long long workspace_floats, bm_stream_t stream) {
+    BM_CHECK_ARG(rows > 0 && C > 0);
+    if (!mean)                                   // no BatchNorm: nothing is reduced, the workspace is not used
+        return bn_act_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, sums, dy, dgamma, dbeta,
+                               nullptr, ST(stream));
+    BM_CHECK_WS(bn_bwd_ws_floats(rows, C));
+    return bn_act_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, sums, dy, dgamma, dbeta,
+                           reinterpret_cast<double*>(workspace), ST(stream));
 }
 
 extern "C" int bm_clip_loss_bwd_cand(const float* probs, const float* scores, const float* inv_norm, const float* est,
@@ -933,6 +1226,21 @@ extern "C" int bm_col_stats(const float* y, long long rows, int C, double* stats
     return 0;
 }
 
+extern "C" long long bm_col_stats_det_workspace(long long rows, int C) {
+    return rows > 0 && C > 0 ? colstats_ws_floats(rows, C) : 0;
+}
+extern "C" int bm_col_stats_det(const float* y, long long rows, int C, float* workspace, long long workspace_floats,
+                                double* stats, bm_stream_t stream) {
+    BM_CHECK_ARG(y && stats && rows > 0 && C > 0);
+    BM_CHECK_WS(colstats_ws_floats(rows, C));
+    cudaStream_t st = ST(stream);
+    double* part = reinterpret_cast<double*>(workspace);
+    dim3 grid((unsigned)blocks_of(rows, COLSTATS_RPB), (C + 127) / 128);
+    col_stats_kernel<true><<<grid, 128, 0, st>>>(y, part, rows, C, COLSTATS_RPB);
+    BM_CHECK_LAUNCH();
+    return reduce_rows(part, (long long)grid.x, 2 * C, stats, st);
+}
+
 // y = x * mask[c] over [B, C, T] (SimpleConv's subsample_meg_channels, simpleconv.py:97-102,200-203); y may alias x
 extern "C" int bm_channel_mask(const float* x, const float* mask, int B, int C, int T, float* y, bm_stream_t stream) {
     BM_CHECK_ARG(x && mask && y && B > 0 && C > 0 && T > 0);
@@ -1007,6 +1315,15 @@ extern "C" int bm_col_sum(const float* x, long long rows, int C, float* out, bm_
     }
     BM_CHECK_LAUNCH();
     return 0;
+}
+extern "C" long long bm_col_sum_det_workspace(long long rows, int C) {
+    return rows > 0 && C > 0 ? colsum_ws_floats(rows, C) : 0;
+}
+extern "C" int bm_col_sum_det(const float* x, long long rows, int C, float* workspace, long long workspace_floats, float* out,
+                              bm_stream_t stream) {
+    BM_CHECK_ARG(x && out && rows > 0 && C > 0);
+    BM_CHECK_WS(colsum_ws_floats(rows, C));
+    return colsum(x, rows, C, C, workspace, out, ST(stream));
 }
 
 // dh = dq * GELU'(h)  (elementwise; dh may alias dq)

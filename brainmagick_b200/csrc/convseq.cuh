@@ -41,6 +41,8 @@ __global__ void bn_act_skip_fwd_kernel(const float* __restrict__ y, const float*
 }
 
 // backward pass 1 (BatchNorm only): sums[c] += sum dz, sums[C+c] += sum dz*yhat  with dz = g * act'(z)
+// DET: sums is a [gridDim.x][2C] partials buffer, the block stores its row
+template <bool DET = false>
 __global__ void bn_act_bwd_reduce_kernel(const float* __restrict__ g, const float* __restrict__ y,
                                          const float* __restrict__ mean, const float* __restrict__ invstd,
                                          const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -58,6 +60,11 @@ __global__ void bn_act_bwd_reduce_kernel(const float* __restrict__ g, const floa
         float dz = g[r * C + c] * act_grad_f(act, yh * ga + be, slope);
         s1 += dz;
         s2 += dz * yh;
+    }
+    if (DET) {
+        sums[(long long)blockIdx.x * 2 * C + c] = (double)s1;
+        sums[(long long)blockIdx.x * 2 * C + C + c] = (double)s2;
+        return;
     }
     atomicAdd(sums + c, (double)s1);
     atomicAdd(sums + C + c, (double)s2);

@@ -145,6 +145,8 @@ __global__ void bn_gelu_skip_fwd_kernel(const float* __restrict__ y, const float
 }
 
 // backward pass 1: sums[c] += sum dz, sums[C+c] += sum dz*yhat  with dz = g * GELU'(z)
+// DET: sums is a [gridDim.x][2C] partials buffer; the block stores its own row (see reduce_rows_kernel)
+template <bool DET = false>
 __global__ void bn_gelu_bwd_reduce_kernel(const float* __restrict__ g, const float* __restrict__ y,
                                           const float* __restrict__ mean, const float* __restrict__ invstd,
                                           const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -162,6 +164,11 @@ __global__ void bn_gelu_bwd_reduce_kernel(const float* __restrict__ g, const flo
         float dz = g[r * C + c] * gelu_grad_f(z);
         s1 += dz;
         s2 += dz * yh;
+    }
+    if (DET) {
+        sums[(long long)blockIdx.x * 2 * C + c] = (double)s1;
+        sums[(long long)blockIdx.x * 2 * C + C + c] = (double)s2;
+        return;
     }
     atomicAdd(sums + c, (double)s1);
     atomicAdd(sums + C + c, (double)s2);
@@ -226,6 +233,8 @@ __global__ void gelu_bwd_kernel(const float* __restrict__ dq, const float* __res
 // bias gradients
 // ------------------------------------------------------------------------------------------------
 // out[c] += sum_r X[r][c]   (channels-last rows); out must be zeroed by the caller
+// DET (here and in the column reductions below): out is a [gridDim.x][C] partials buffer, the block stores its row
+template <bool DET = false>
 __global__ void colsum_cl_kernel(const float* __restrict__ X, float* __restrict__ out, long long rows, int C,
                                  int rows_per_block) {
     int c = blockIdx.y * blockDim.x + threadIdx.x;
@@ -235,10 +244,12 @@ __global__ void colsum_cl_kernel(const float* __restrict__ X, float* __restrict_
     float s = 0.f;
 #pragma unroll 4
     for (long long r = r0; r < r1; ++r) s += X[r * C + c];
-    atomicAdd(out + c, s);
+    if (DET) out[(long long)blockIdx.x * C + c] = s;
+    else atomicAdd(out + c, s);
 }
 
 // out[c] += sum_r X[r*ld + c]   (rows with a leading dimension ld >= C)
+template <bool DET = false>
 __global__ void colsum_strided_kernel(const float* __restrict__ X, float* __restrict__ out, long long rows, int C,
                                       int ld, int rows_per_block) {
     int c = blockIdx.y * blockDim.x + threadIdx.x;
@@ -248,10 +259,13 @@ __global__ void colsum_strided_kernel(const float* __restrict__ X, float* __rest
     float s = 0.f;
 #pragma unroll 4
     for (long long r = r0; r < r1; ++r) s += X[r * ld + c];
-    atomicAdd(out + c, s);
+    if (DET) out[(long long)blockIdx.x * C + c] = s;
+    else atomicAdd(out + c, s);
 }
 
 // stats[c] += sum_r X[r][c], stats[C+c] += sum_r X[r][c]^2   (fp64 atomics; BatchNorm batch statistics)
+// DET: stats is a [gridDim.x][2C] partials buffer
+template <bool DET = false>
 __global__ void col_stats_kernel(const float* __restrict__ X, double* __restrict__ stats, long long rows, int C,
                                  int rows_per_block) {
     int c = blockIdx.y * blockDim.x + threadIdx.x;
@@ -265,11 +279,18 @@ __global__ void col_stats_kernel(const float* __restrict__ X, double* __restrict
         s += v;
         q = fmaf(v, v, q);
     }
+    if (DET) {
+        stats[(long long)blockIdx.x * 2 * C + c] = (double)s;
+        stats[(long long)blockIdx.x * 2 * C + C + c] = (double)q;
+        return;
+    }
     atomicAdd(stats + c, (double)s);
     atomicAdd(stats + C + c, (double)q);
 }
 
 // out[n] += sum_{z,t} X[z][n][t]  (channel-major [Z,N,T]); one warp per (z, n) row
+// DET: out is a [Z][N] partials buffer that receives each row's sum
+template <bool DET = false>
 __global__ void rowsum_cm_kernel(const float* __restrict__ X, float* __restrict__ out, int Z, int N, int T) {
     long long row = blockIdx.x * (long long)(blockDim.x >> 5) + (threadIdx.x >> 5);
     int lane = threadIdx.x & 31;
@@ -278,7 +299,10 @@ __global__ void rowsum_cm_kernel(const float* __restrict__ X, float* __restrict_
     float s = 0.f;
     for (int t = lane; t < T; t += 32) s += x[t];
     s = warp_sum(s);
-    if (lane == 0) atomicAdd(out + (int)(row % N), s);
+    if (lane == 0) {
+        if (DET) out[row] = s;
+        else atomicAdd(out + (int)(row % N), s);
+    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -301,7 +325,8 @@ __global__ void weight_prep_kernel(const float* __restrict__ W, float* __restric
 // ------------------------------------------------------------------------------------------------
 // ClipLoss pieces (losses.py:91-114)
 // ------------------------------------------------------------------------------------------------
-// ss[o] += sum_k cand[o][k]^2 (fp64 atomics; grid = (rows, splits))
+// ss[o] += sum_k cand[o][k]^2 (fp64 atomics; grid = (rows, splits)).  With one split, every slot receives exactly one add
+// onto its zero: the deterministic form.
 __global__ void row_sumsq_kernel(const float* __restrict__ X, double* __restrict__ ss, long long K) {
     __shared__ double red[32];
     const float* x = X + (long long)blockIdx.x * K;
@@ -579,7 +604,9 @@ bn_gelu_skip_fwd_cs_kernel(const float* __restrict__ y, const float* __restrict_
 }
 
 // backward pass 1: sums[c] += sum dz, sums[C+c] += sum dz*yhat  with dz = g * GELU'(z); fp32 per thread, combined over the
-// block's RY row lanes in shared memory, ONE fp64 atomic pair per column per block
+// block's RY row lanes in shared memory, ONE fp64 atomic pair per column per block (DET: sums is a [gridDim.x][2C] partials
+// buffer, the block stores its row)
+template <bool DET = false>
 __global__ void __launch_bounds__(320, 2)
 bn_gelu_bwd_reduce_cs_kernel(const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ mean,
                              const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta,
@@ -617,7 +644,8 @@ bn_gelu_bwd_reduce_cs_kernel(const float* __restrict__ g, const float* __restric
     for (int i = tid; i < 2 * C; i += nthr) {
         double acc = 0.0;
         for (int ry = 0; ry < RY; ++ry) acc += (double)red[(size_t)ry * 2 * C + i];
-        atomicAdd(sums + i, acc);
+        if (DET) sums[(long long)blockIdx.x * 2 * C + i] = acc;
+        else atomicAdd(sums + i, acc);
     }
 }
 
@@ -668,6 +696,8 @@ bn_gelu_bwd_apply_cs_kernel(const float* __restrict__ g, const float* __restrict
 // GLU backward, column-stationary (H % 4 == 0, H/4 <= 256): thread (cx, ry) owns a-columns 4cx.. and the matching gate columns;
 // optionally accumulates the bias gradient of the GLU convolution, dbias[c] = sum_rows dh[row][c] (2H columns), from the values
 // it has just produced (shared-memory combine over the row lanes, one fp32 atomic per column per block; zeroed by the caller).
+// DET: dbias is a [gridDim.x][2H] partials buffer, the block stores its row.
+template <bool DET = false>
 __global__ void __launch_bounds__(320, 2)
 glu_bwd_cs_kernel(const float* __restrict__ g, const float* __restrict__ h, float* __restrict__ dh, float* __restrict__ dbias,
                   long long rows, int H, unsigned int* __restrict__ amax) {
@@ -713,8 +743,20 @@ glu_bwd_cs_kernel(const float* __restrict__ g, const float* __restrict__ h, floa
     for (int i = tid; i < 2 * H; i += nthr) {
         float acc = 0.f;
         for (int ry = 0; ry < RY; ++ry) acc += red[(size_t)ry * 2 * H + i];
-        atomicAdd(dbias + i, acc);
+        if (DET) dbias[(long long)blockIdx.x * 2 * H + i] = acc;
+        else atomicAdd(dbias + i, acc);
     }
+}
+
+// out[c] = sum_{r < n} part[r][c] in the order r = 0, 1, ..., n-1: the fixed-order second half of every deterministic column
+// reduction above (T = double where the atomic form accumulates in fp64, float where it accumulates in fp32)
+template <class T>
+__global__ void reduce_rows_kernel(const T* __restrict__ part, long long n, int W, T* __restrict__ out) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= W) return;
+    T s = 0;
+    for (long long r = 0; r < n; ++r) s += part[r * W + c];
+    out[c] = s;
 }
 
 inline bool aligned16(const void* a, const void* b = nullptr, const void* c = nullptr) {

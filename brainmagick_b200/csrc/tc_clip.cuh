@@ -8,7 +8,9 @@
 // engine adds every 32-wide K block into a round-to-nearest fp32 sum instead.  The candidate norms (the 1/||c|| of
 // losses.py:91) come from a fp64 row sum of squares beside the GEMM.
 //   grid: 128-estimate x 128-candidate tiles x K slices; outputs: partial scores [ks][Bn][Bc] and [ks][Bc] fp64 partial sums
-//   of squares (slice 0 holds the full sums); `clip_finalize_kernel` reduces both in a fixed order (deterministic).
+//   of squares (slice 0 holds the full sums); `clip_finalize_kernel` reduces both in a fixed order.  The sums of squares in
+//   slot 0 come from up to 32 K splits per candidate added with fp64 atomics, so their last bits depend on block order; the
+//   deterministic form (`det`) computes each candidate's sum in one block, which adds onto its zeroed slot exactly once.
 #pragma once
 #include "tc_common.cuh"
 #include "elementwise.cuh"
@@ -162,7 +164,7 @@ inline long long clip_ws_floats(int Bn, int Bc, long long KT) {
 // scores [Bn][Bc] (+ inv_norm when !norms_given, + probs / row_loss / loss when requested)
 inline int launch_clip_scores(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
                               int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss,
-                              float* loss, float* ws, int* err, cudaStream_t st) {
+                              float* loss, float* ws, int* err, cudaStream_t st, bool det = false) {
     (void)err;
     const ClipGeom g = clip_geometry(Bn, Bc, KT);
     long long nP = (long long)g.ks * Bn * Bc;
@@ -178,6 +180,7 @@ inline int launch_clip_scores(const float* est, const float* cand, int Bn, int B
         if (em != cudaSuccess) return set_error(3, "%s: memset: %s", __func__, cudaGetErrorString(em));
         int splits = (int)((KT + 65535) / 65536);
         if (splits > 32) splits = 32;
+        if (det) splits = 1;                                      // one add per slot: independent of block order
         row_sumsq_kernel<<<dim3(Bc, splits), 256, 0, st>>>(cand, ssp, KT);
         ++g_launches;
         cudaError_t e = cudaGetLastError();

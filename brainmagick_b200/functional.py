@@ -100,6 +100,44 @@ def _round_up(n, m):
     return (n + m - 1) // m * m
 
 
+# ---- deterministic forms ------------------------------------------------------------------------------------------
+# Under torch.use_deterministic_algorithms(True) (`_lib.deterministic()`) every entry point whose default form finishes a
+# floating-point reduction with atomics is replaced by its `_det` form (include/bm_b200.h), which reduces in a fixed order
+# through a workspace allocated here.  With the flag off the call stream is exactly the default one.
+def _det_workspace(name, like, *dims) -> torch.Tensor:
+    n = int(getattr(_lib.load(), name + "_workspace")(*dims))
+    return torch.empty((max(n, 2),), device=like.device, dtype=torch.float32)
+
+
+def _reducing_call(name, like, ws_dims, *args):
+    """call(name, *args) -- or, under the determinism flag, `name`_det with the workspace of `name`_det_workspace(*ws_dims)
+    inserted before the stream argument (ws_dims None: a _det form without workspace, same arguments)."""
+    if not _lib.deterministic():
+        return call(name, *args)
+    if ws_dims is None:
+        return call(name + "_det", *args)
+    ws = _det_workspace(name + "_det", like, *ws_dims)
+    return call(name + "_det", *args[:-1], ptr(ws), ws.numel(), args[-1])
+
+
+def col_sum(x, rows, C, out, st):
+    """out[c] = sum_r x[r, c] (bm_col_sum, or bm_col_sum_det under the determinism flag)."""
+    if _lib.deterministic():
+        ws = _det_workspace("bm_col_sum_det", x, rows, C)
+        call("bm_col_sum_det", ptr(x), rows, C, ptr(ws), ws.numel(), ptr(out), st)
+    else:
+        call("bm_col_sum", ptr(x), rows, C, ptr(out), st)
+
+
+def col_stats(y, rows, C, stats, st):
+    """BatchNorm batch statistics of channels-last y (bm_col_stats, or bm_col_stats_det under the determinism flag)."""
+    if _lib.deterministic():
+        ws = _det_workspace("bm_col_stats_det", y, rows, C)
+        call("bm_col_stats_det", ptr(y), rows, C, ptr(ws), ws.numel(), ptr(stats), st)
+    else:
+        call("bm_col_stats", ptr(y), rows, C, ptr(stats), st)
+
+
 # The fp16-piece entry points (bm_tc_conv1d_f16, bm_tc_wgrad_conv_f16: operands as fp16 hi/lo pieces of power-of-two-scaled
 # tensors, with their amax) compute on the same 3xTF32 engine as the fp32 ones, so on this GPU they would only add the amax
 # passes and the fp16 weight preparation to every step: off by default, kept switchable for the ABI's callers.
@@ -127,11 +165,14 @@ def tc_wgrad(dy, x, B, T, M, N, Ntrue, kw, dilation, status, dbias=None, dy_amax
         else:
             call("bm_tc_wgrad_conv", ptr(dy), ptr(x), B, T, M, N, Ntrue, kw, dilation, ptr(ws), ptr(dw), ptr(status), stream())
         if dbias is not None:
-            call("bm_col_sum", ptr(dy), B * T, M, ptr(dbias), stream())
+            col_sum(dy, B * T, M, dbias, stream())
         return dw
     ws = _empty((int(lib.bm_tc_wgrad_workspace(B, M, N, kw)),), dy)
-    call("bm_tc_wgrad", ptr(dy), ptr(x), B, T, M, N, Ntrue, kw, dilation, ptr(ws), ptr(dw), ptr(dbias), ptr(status),
-         stream())
+    det = _lib.deterministic()                # the kernel's own bias reduction is atomic: a fixed-order column sum instead
+    call("bm_tc_wgrad", ptr(dy), ptr(x), B, T, M, N, Ntrue, kw, dilation, ptr(ws), ptr(dw), None if det else ptr(dbias),
+         ptr(status), stream())
+    if det and dbias is not None:
+        col_sum(dy, B * T, M, dbias, stream())
     return dw
 
 
@@ -255,12 +296,17 @@ class _Conv:
         st = stream()
         if self.fwd_tc:
             fused = stats is not None and self.fwd_pp          # BatchNorm statistics out of the conv epilogue
-            if self.cout > 320:
-                fused = False                                   # the kernel keeps the statistics of ONE N tile in smem
+            if self.cout > 320 or _lib.deterministic():
+                fused = False                                   # the kernel keeps the statistics of ONE N tile in smem, and
+                                                                # commits them with atomics
             self.run_tc(True, x, bias, None, B, T, dilation, 0, 0, 0, y, None, None, stats if fused else None, status,
                         x_amax=x_amax)
             if stats is not None and not fused:
-                call("bm_col_stats", ptr(y), B * T, self.cout, ptr(stats), st)
+                col_stats(y, B * T, self.cout, stats, st)
+        elif stats is not None and _lib.deterministic():
+            call("bm_conv1d_fwd", ptr(x), ptr(self.wf), ptr(bias), B, T, self.cin, self.cout, self.kw, dilation,
+                 ptr(y), None, st)
+            col_stats(y, B * T, self.cout, stats, st)
         else:
             call("bm_conv1d_fwd", ptr(x), ptr(self.wf), ptr(bias), B, T, self.cin, self.cout, self.kw, dilation,
                  ptr(y), ptr(stats), st)
@@ -300,8 +346,8 @@ class _Conv:
             return dw, db
         db = _empty((self.cout,), like)
         dw = _empty((self.cout, self.cin, self.kw), like)
-        call("bm_conv1d_bwd_weight", ptr(dy), ptr(x), B, T, self.cin, self.cout, self.kw, dilation, ptr(dw), ptr(db),
-             stream())
+        _reducing_call("bm_conv1d_bwd_weight", like, (B, T, self.cin, self.cout, self.kw), ptr(dy), ptr(x), B, T, self.cin, self.cout, self.kw,
+                       dilation, ptr(dw), ptr(db), stream())
         if self.cin != self.cin_true:
             dw = dw[:, :self.cin_true].contiguous()
         return dw, db
@@ -379,8 +425,8 @@ def _staged_front_backward(plan: "EncoderPlan", saved, g, heads, il_w, subj_w, s
         d_il_w = _empty((w_v, w_u), meg)
         d_il_b = _empty((w_v,), meg)
         du = _empty((B, T, w_u), meg)
-        call("bm_initial_linear_bwd", ptr(g), w_v, ptr(saved["u"]), w_u, ptr(il_w.reshape(w_v, w_u).contiguous()), B, T, w_u,
-             w_v, w_u, ptr(du), ptr(d_il_w), ptr(d_il_b), st)
+        _reducing_call("bm_initial_linear_bwd", meg, (B, T, w_u, w_v), ptr(g), w_v, ptr(saved["u"]), w_u,
+                       ptr(il_w.reshape(w_v, w_u).contiguous()), B, T, w_u, w_v, w_u, ptr(du), ptr(d_il_w), ptr(d_il_b), st)
         d_il_w = d_il_w.reshape(il_w.shape)
         g = du
     dheads = None
@@ -390,8 +436,8 @@ def _staged_front_backward(plan: "EncoderPlan", saved, g, heads, il_w, subj_w, s
         call("bm_sensor_mix_bwd", ptr(g), w_u, ptr(meg), ptr(plan.rec_order), ptr(plan.rec_off), B, C, T, O, R, ptr(d_att), st)
         dscores = _empty((R, O, C), meg)
         dheads = _empty((O, P), meg)
-        call("bm_attention_weights_bwd", ptr(d_att), ptr(saved["att"]), ptr(saved["emb"]), R, C, O, P, ptr(dscores),
-             ptr(dheads), st)
+        _reducing_call("bm_attention_weights_bwd", meg, None, ptr(d_att), ptr(saved["att"]), ptr(saved["emb"]), R, C, O, P,
+                       ptr(dscores), ptr(dheads), st)
     dmeg = None
     if want_dmeg:
         # g is now the gradient at the first stage present: the mix output, or the raw sensors transposed (merger=False)
@@ -760,18 +806,18 @@ class _EncoderFn(torch.autograd.Function):
                 # dW2 / db2 only need dest_t and q: they overlap the dq contraction queued just before
                 dw2 = on_side(lambda: tc_wgrad(s["q"], dest_t, B, T, H2, F, F, 1, 1, status, dy_amax=s.get("q_amax"),
                                                x_amax=dest_amax), s["q"], dest_t, dest_amax).reshape(H2, F)
-                call("bm_col_sum", ptr(dest_t), rows, F, ptr(db2), st)
+                col_sum(dest_t, rows, F, db2, st)
                 call("bm_gelu_bwd", ptr(dq), ptr(s["h1"]), rows * H2, ptr(dq), st)           # dq <- dh1
                 dw0 = on_side(lambda: tc_wgrad(dq, s["x_last"], B, T, H2, H, H, 1, 1, status, dbias=db0), dq,
                               s["x_last"], db0).reshape(H2, H)
             else:
-                call("bm_head_bwd_params", ptr(dest), ptr(s["x_last"]), ptr(s["h1"]), ptr(s["q"]), B, T, H, F,
-                     ptr(dq), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st)   # dq <- dq*GELU'(h1); dW0, db0, dW2, db2
+                _reducing_call("bm_head_bwd_params", meg, (B, T, H, F), ptr(dest), ptr(s["x_last"]), ptr(s["h1"]), ptr(s["q"]),
+                               B, T, H, F, ptr(dq), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st)   # dq <- dq*GELU'(h1); dW0..db2
             head0.run_tc(False, dq, None, None, B, T, 1, 0, 0, 0, g, None, None, None, status)
             del dest_t
         else:
-            call("bm_head_bwd", ptr(dest), ptr(s["x_last"]), ptr(s["w0_2"]), ptr(s["w2_2"]), ptr(s["h1"]), ptr(s["q"]),
-                 B, T, H, F, ptr(dq), ptr(g), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st)
+            _reducing_call("bm_head_bwd", meg, (B, T, H, F), ptr(dest), ptr(s["x_last"]), ptr(s["w0_2"]), ptr(s["w2_2"]),
+                           ptr(s["h1"]), ptr(s["q"]), B, T, H, F, ptr(dq), ptr(g), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st)
         del dq
 
         sums = _empty((2 * H,), meg, torch.float64)
@@ -808,7 +854,8 @@ class _EncoderFn(torch.autograd.Function):
                 dh = _empty((B, T, gconv.cout), meg)
                 dgb = _empty((gconv.cout,), meg)          # the GLU conv's bias gradient, summed while dh is produced
                 dh_amax = amax_cell(meg)
-                call("bm_glu_bwd", ptr(g), ptr(rec["h"]), rows, gconv.cout // 2, ptr(dh), ptr(dgb), ptr(dh_amax), st)
+                _reducing_call("bm_glu_bwd", meg, (rows, gconv.cout // 2), ptr(g), ptr(rec["h"]), rows, gconv.cout // 2, ptr(dh),
+                               ptr(dgb), ptr(dh_amax), st)
                 glu_grads[k] = weight_grad(gconv, dh, rec["x_new"], 1, False, dgb, dy_amax=dh_amax, x_amax=rec.get("x_new_amax"))
                 g = _empty((B, T, gconv.cin), meg)
                 gconv.backward_data(dh, None, B, T, 1, g, status, dy_amax=dh_amax)
@@ -832,13 +879,14 @@ class _EncoderFn(torch.autograd.Function):
             dy_amax = None
             if plan.act_code == 0:
                 dy_amax = amax_cell(meg)
-                call("bm_bn_gelu_skip_bwd", ptr(g), ptr(rec["y"]), ptr(rec["mean"]), ptr(rec["invstd"]),
-                     ptr(gamma.contiguous()), ptr(beta.contiguous()), 1 if plan.training else 0, rows, cout, ptr(sums),
-                     ptr(dy), ptr(dgamma), ptr(dbeta), ptr(dy_amax), st)
+                _reducing_call("bm_bn_gelu_skip_bwd", meg, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
+                               ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()), 1 if plan.training else 0,
+                               rows, cout, ptr(sums), ptr(dy), ptr(dgamma), ptr(dbeta), ptr(dy_amax), st)
             else:
-                call("bm_bn_act_skip_bwd", ptr(g), ptr(rec["y"]), ptr(rec["mean"]), ptr(rec["invstd"]),
-                     ptr(gamma.contiguous()), ptr(beta.contiguous()), 1 if plan.training else 0, rows, cout,
-                     plan.act_code, float(plan.act_slope), ptr(sums), ptr(dy), ptr(dgamma), ptr(dbeta), st)
+                _reducing_call("bm_bn_act_skip_bwd", meg, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
+                               ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()), 1 if plan.training else 0,
+                               rows, cout, plan.act_code, float(plan.act_slope), ptr(sums), ptr(dy), ptr(dgamma), ptr(dbeta),
+                               st)
             dcw, dcb = weight_grad(conv, dy, rec["x_in"], plan.dilations[k], plan.training, dy_amax=dy_amax,
                                    x_amax=rec.get("x_in_amax"))
             if rec["skip"]:
@@ -903,9 +951,10 @@ class _EncoderFn(torch.autograd.Function):
                 du = _empty((B, T, O), meg)
                 d_il_w = _empty((IL, O), meg)
                 d_il_b = _empty((IL,), meg)
-                call("bm_sensor_chain_bwd", ptr(g), ptr(meg), ptr(s["il_w2"]), ptr(s["subj_w"]), ptr(plan.subject),
-                     ptr(s["u"]), ptr(s["v"]), ptr(subj_order), ptr(subj_off), ptr(plan.rec_order), ptr(plan.rec_off),
-                     B, C, T, O, IL, D, Dp, S, R, ptr(dv), ptr(du), ptr(d_subj), ptr(d_il_w), ptr(d_il_b), ptr(d_att), st)
+                _reducing_call("bm_sensor_chain_bwd", meg, (B, T, O, IL), ptr(g), ptr(meg), ptr(s["il_w2"]), ptr(s["subj_w"]),
+                               ptr(plan.subject), ptr(s["u"]), ptr(s["v"]), ptr(subj_order), ptr(subj_off), ptr(plan.rec_order),
+                               ptr(plan.rec_off), B, C, T, O, IL, D, Dp, S, R, ptr(dv), ptr(du), ptr(d_subj), ptr(d_il_w),
+                               ptr(d_il_b), ptr(d_att), st)
             dmeg = _sensor_mix_bwd_data(plan, s, du, ctx.dims, status) if ctx.needs_input_grad[1] else None
             dscores = _empty((R, O, C), meg)
             if s["heads_tc"]:
@@ -916,8 +965,8 @@ class _EncoderFn(torch.autograd.Function):
                 dheads = tc_wgrad(ds_t, s["emb"], R, C, Opad, P, P, 1, 1, status)[:O, :, 0].contiguous()
             else:
                 dheads = _empty((O, P), meg)
-                call("bm_attention_weights_bwd", ptr(d_att), ptr(s["att"]), ptr(s["emb"]), R, C, O, P, ptr(dscores),
-                     ptr(dheads), st)
+                _reducing_call("bm_attention_weights_bwd", meg, None, ptr(d_att), ptr(s["att"]), ptr(s["emb"]), R, C, O, P,
+                               ptr(dscores), ptr(dheads), st)
 
         if d_il_w is not None:
             d_il_w = d_il_w.reshape(s["il_shape"])
@@ -981,8 +1030,8 @@ def clip_scores(estimates: torch.Tensor, candidates: torch.Tensor, want_probs: b
     scores = _empty((Bn, Bc), est)
     probs = _empty((Bn, Bc), est) if want_probs else None
     ws = _clip_workspace(est, Bn, Bc, KT)
-    call("bm_clip_scores", ptr(est), ptr(cand), Bn, Bc, KT, 0, ptr(inv), ptr(scores), ptr(probs), ptr(ws), ws.numel(),
-         ptr(tc_status_tensor(est.device)), stream())
+    _reducing_call("bm_clip_scores", est, None, ptr(est), ptr(cand), Bn, Bc, KT, 0, ptr(inv), ptr(scores), ptr(probs), ptr(ws),
+                   ws.numel(), ptr(tc_status_tensor(est.device)), stream())
     return probs if want_probs else scores
 
 
@@ -1001,8 +1050,8 @@ class _ClipScoresFn(torch.autograd.Function):
         scores = _empty((Bn, Bc), est)
         probs = _empty((Bn, Bc), est) if want_probs else None
         ws = _clip_workspace(est, Bn, Bc, KT)
-        call("bm_clip_scores", ptr(est), ptr(cand), Bn, Bc, KT, 0, ptr(inv), ptr(scores), ptr(probs), ptr(ws), ws.numel(),
-             ptr(tc_status_tensor(est.device)), stream())
+        _reducing_call("bm_clip_scores", est, None, ptr(est), ptr(cand), Bn, Bc, KT, 0, ptr(inv), ptr(scores), ptr(probs),
+                       ptr(ws), ws.numel(), ptr(tc_status_tensor(est.device)), stream())
         ctx.save_for_backward(est, cand, inv, scores, probs)
         ctx.meta = (Bn, Bc, KT, estimate.shape, candidate.shape)
         return probs if want_probs else scores
@@ -1038,7 +1087,7 @@ def candidate_inv_norms(candidates: torch.Tensor) -> torch.Tensor:
     Bc, KT = cand.shape[0], cand[0].numel()
     ss = _empty((Bc,), cand, torch.float64)
     inv = _empty((Bc,), cand)
-    call("bm_candidate_inv_norms", ptr(cand), Bc, KT, ptr(ss), ptr(inv), stream())
+    _reducing_call("bm_candidate_inv_norms", cand, None, ptr(cand), Bc, KT, ptr(ss), ptr(inv), stream())
     return inv
 
 
@@ -1053,8 +1102,8 @@ def clip_scores_prenormed(estimates: torch.Tensor, candidates: torch.Tensor, inv
     assert cand[0].numel() == KT and inv_norms.numel() == Bc
     scores = _empty((Bn, Bc), est)
     ws = _clip_workspace(est, Bn, Bc, KT)
-    call("bm_clip_scores", ptr(est), ptr(cand), Bn, Bc, KT, 1, ptr(inv_norms), ptr(scores), None, ptr(ws), ws.numel(),
-         ptr(tc_status_tensor(est.device)), stream())
+    _reducing_call("bm_clip_scores", est, None, ptr(est), ptr(cand), Bn, Bc, KT, 1, ptr(inv_norms), ptr(scores), None,
+                   ptr(ws), ws.numel(), ptr(tc_status_tensor(est.device)), stream())
     return scores
 
 
@@ -1072,8 +1121,9 @@ class _ClipLossFn(torch.autograd.Function):
         row_loss = _empty((Bn,), est)
         loss = _empty((1,), est)
         ws = _clip_workspace(est, Bn, Bc, KT)
-        call("bm_clip_loss_fwd", ptr(est), ptr(cand), Bn, Bc, KT, int(target_offset), ptr(inv), ptr(scores), ptr(probs),
-             ptr(row_loss), ptr(loss), ptr(ws), ws.numel(), ptr(tc_status_tensor(est.device)), stream())
+        _reducing_call("bm_clip_loss_fwd", est, None, ptr(est), ptr(cand), Bn, Bc, KT, int(target_offset), ptr(inv),
+                       ptr(scores), ptr(probs), ptr(row_loss), ptr(loss), ptr(ws), ws.numel(),
+                       ptr(tc_status_tensor(est.device)), stream())
         if candidate.requires_grad:      # a trainable feature model produced the candidates (solver.py:304-320)
             ctx.save_for_backward(probs, inv, cand, scores, est)
         else:
@@ -1142,7 +1192,8 @@ class _MergerFn(torch.autograd.Function):
         call("bm_transpose_nt", ptr(gout.contiguous()), B, O, T, ptr(g), st)
         d_att, dscores, dheads = _empty((R, O, C), meg), _empty((R, O, C), meg), _empty((O, P), meg)
         call("bm_sensor_mix_bwd", ptr(g), O, ptr(meg), ptr(rec_order), ptr(rec_off), B, C, T, O, R, ptr(d_att), st)
-        call("bm_attention_weights_bwd", ptr(d_att), ptr(att), ptr(emb), R, C, O, P, ptr(dscores), ptr(dheads), st)
+        _reducing_call("bm_attention_weights_bwd", meg, None, ptr(d_att), ptr(att), ptr(emb), R, C, O, P, ptr(dscores),
+                       ptr(dheads), st)
         dmeg = None
         if ctx.needs_input_grad[0]:
             dmeg = _empty((B, C, T), meg)

@@ -345,6 +345,71 @@ int bm_transpose_nt(const float* in, int Z, int N, int T, float* out, bm_stream_
 /* same with an output row stride ld_out >= N (pad columns written as zeros): meg [B,C,T] -> channels-last, channel-padded. */
 int bm_transpose_nt_ld(const float* in, int Z, int N, int T, int ld_out, float* out, bm_stream_t stream);
 
+/* ---- Deterministic forms (torch.use_deterministic_algorithms(True) in the drop-in modules) -------------------------
+ * Every `_det` entry point computes what its default form computes, with the same arguments plus (where noted) a
+ * caller-owned workspace of bm_<op>_det_workspace(dims) floats, 8-byte aligned, checked against `workspace_floats`.  Its
+ * floating-point reductions run in a fixed order: each block stores its partial row into the workspace ([n_blocks][width],
+ * fp64 where the default form accumulates in fp64) and one more kernel sums the rows in index order; the FP32-FMA
+ * split-batch weight-gradient GEMMs store one partial plane per batch segment and sum the planes in segment order (the
+ * segment count follows the SM count, so these workspace sizes depend on the device), and the other split GEMMs (dheads,
+ * the FP32-FMA CLIP scores) run unsplit.  Repeated calls on the same inputs give bitwise-identical outputs on the same
+ * device model and library build; the bits may differ from the default form's.  The entry points of this header that are
+ * not listed here have no order-dependent floating-point reduction (or only atomicMax on amax cells, which is exact).
+ * With the default form, bm_tc_conv1d_persistent / bm_tc_conv1d_f16 / bm_conv1d_fwd fold the BatchNorm statistics into
+ * the conv with atomics; a deterministic caller passes stats = NULL and calls bm_col_stats_det on the output instead, and
+ * bm_tc_wgrad callers pass dbias = NULL and call bm_col_sum_det. */
+long long bm_col_stats_det_workspace(long long rows, int C);
+int bm_col_stats_det(const float* y, long long rows, int C, float* workspace, long long workspace_floats, double* stats,
+                     bm_stream_t stream);
+long long bm_col_sum_det_workspace(long long rows, int C);
+int bm_col_sum_det(const float* x, long long rows, int C, float* workspace, long long workspace_floats, float* out,
+                   bm_stream_t stream);
+long long bm_bn_gelu_skip_bwd_det_workspace(long long rows, int C);
+int bm_bn_gelu_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                            const float* beta, int batch_stats, long long rows, int C, double* sums, float* dy, float* dgamma,
+                            float* dbeta, float* amax_out, float* workspace, long long workspace_floats, bm_stream_t stream);
+/* workspace unused (may be NULL) when mean == NULL */
+long long bm_bn_act_skip_bwd_det_workspace(long long rows, int C);
+int bm_bn_act_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                           const float* beta, int batch_stats, long long rows, int C, int act, float slope, double* sums,
+                           float* dy, float* dgamma, float* dbeta, float* workspace, long long workspace_floats,
+                           bm_stream_t stream);
+long long bm_glu_bwd_det_workspace(long long rows, int H);
+int bm_glu_bwd_det(const float* g, const float* h, long long rows, int H, float* dh, float* dbias, float* amax_out,
+                   float* workspace, long long workspace_floats, bm_stream_t stream);
+long long bm_conv1d_bwd_weight_det_workspace(int B, int T, int Cin, int Cout, int Kw);
+int bm_conv1d_bwd_weight_det(const float* dy, const float* x, int B, int T, int Cin, int Cout, int Kw, int dilation,
+                             float* dw, float* dbias, float* workspace, long long workspace_floats, bm_stream_t stream);
+long long bm_initial_linear_bwd_det_workspace(int B, int T, int O, int IL);
+int bm_initial_linear_bwd_det(const float* dv, int ld_dv, const float* u, int ld_u, const float* il_w, int B, int T, int O,
+                              int IL, int ld_du, float* du, float* d_il_w, float* d_il_b, float* workspace,
+                              long long workspace_floats, bm_stream_t stream);
+long long bm_sensor_chain_bwd_det_workspace(int B, int T, int O, int IL);
+int bm_sensor_chain_bwd_det(const float* dx0, const float* meg, const float* il_w, const float* subj_w, const int* subject,
+                            const float* u, const float* v, const int* subj_order, const int* subj_off, const int* rec_order,
+                            const int* rec_off, int B, int C, int T, int O, int IL, int D, int ld_x0, int S, int R, float* dv,
+                            float* du, float* d_subj_w, float* d_il_w, float* d_il_b, float* d_weights, float* workspace,
+                            long long workspace_floats, bm_stream_t stream);
+/* no workspace */
+int bm_attention_weights_bwd_det(const float* dweights, const float* weights, const float* emb, int R, int C, int O, int P,
+                                 float* dscores, float* dheads, bm_stream_t stream);
+long long bm_head_bwd_params_det_workspace(int B, int T, int H, int F);
+int bm_head_bwd_params_det(const float* dest, const float* x, const float* h1, const float* q, int B, int T, int H, int F,
+                           float* dq, float* dw0, float* db0, float* dw2, float* db2, float* workspace,
+                           long long workspace_floats, bm_stream_t stream);
+long long bm_head_bwd_det_workspace(int B, int T, int H, int F);
+int bm_head_bwd_det(const float* dest, const float* x, const float* w0, const float* w2, const float* h1, const float* q,
+                    int B, int T, int H, int F, float* dq, float* dx, float* dw0, float* db0, float* dw2, float* db2,
+                    float* workspace, long long workspace_floats, bm_stream_t stream);
+/* CLIP: the candidate sums of squares one block per candidate; same scratch as the default forms (bm_clip_workspace) */
+int bm_candidate_inv_norms_det(const float* cand, int Bc, long long KT, double* ss, float* inv_norm, bm_stream_t stream);
+int bm_clip_scores_det(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given, float* inv_norm,
+                       float* scores, float* probs, float* workspace, long long workspace_floats, int* status,
+                       bm_stream_t stream);
+int bm_clip_loss_fwd_det(const float* est, const float* cand, int Bn, int Bc, long long KT, int target_offset,
+                         float* inv_norm, float* scores, float* probs, float* row_loss, float* loss, float* workspace,
+                         long long workspace_floats, int* status, bm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
