@@ -17,7 +17,7 @@ import torch
 
 from . import _lib
 from ._lib import call, ptr, stream
-from .functional import _Conv, _empty, _reducing_call, _round_up, tc_status_tensor
+from .functional import _Conv, _Needs, _empty, _reducing_call, _round_up, tc_status_tensor
 
 ACT_GELU, ACT_LRELU, ACT_NONE = 0, 1, 2
 
@@ -47,8 +47,30 @@ def _epilogue_fwd(plan: SequencePlan, y, mean, invstd, gamma, beta, x_old, x_new
              act, float(plan.act_slope), stream())
 
 
+def _sequence_needs(needs_input_grad, plan: SequencePlan) -> _Needs:
+    """`_Needs` of a ConvSequence call: front = (x,), layer k = (conv_w, conv_b, gamma, beta) (False where absent)."""
+    n = [bool(v) for v in needs_input_grad]
+    depth = len(plan.dilations)
+    layer, at = [], 2
+    for k in range(depth):
+        cnt = 4 if (plan.has_act[k] and plan.batch_norm) else 2
+        layer.append(tuple(n[at:at + cnt]) + (False,) * (4 - cnt))
+        at += cnt
+    glu = {}
+    for k in range(depth):
+        if plan.glu_after[k]:
+            glu[k] = tuple(n[at:at + 2])
+            at += 2
+    below = [n[1]]
+    for k in range(depth):
+        below.append(below[-1] or any(layer[k]) or any(glu.get(k, ())))
+    return _Needs(front=(n[1],), head=(), layer=layer, glu=glu, below=below)
+
+
 class _ConvSequenceFn(torch.autograd.Function):
-    """inputs: plan, x, then per layer (conv_w, conv_b[, gamma, beta]) and, appended in layer order, (glu_w, glu_b)."""
+    """inputs: plan, x, then per layer (conv_w, conv_b[, gamma, beta]) and, appended in layer order, (glu_w, glu_b).
+    Only what requires grad is backpropagated, as in `functional._EncoderFn`: frozen parameters get no gradient work, the
+    backward stops at the first layer that still needs a data gradient, and the forward saves only what it reads."""
 
     @staticmethod
     def forward(ctx, plan: SequencePlan, x_in, *params):
@@ -62,22 +84,23 @@ class _ConvSequenceFn(torch.autograd.Function):
                 gamma, beta = next(it), next(it)
             conv_p.append((w, b, gamma, beta))
         glu_p = {k: (next(it), next(it)) for k in range(depth) if plan.glu_after[k]}
+        nd = _sequence_needs(ctx.needs_input_grad, plan)
         st = stream()
         x_in = x_in.contiguous()
         B, C0, T = x_in.shape
         rows = B * T
         tc = plan.use_tensor_cores
-        save = plan.keep_for_backward
+        save = plan.keep_for_backward and any(ctx.needs_input_grad)
         status = tc_status_tensor(x_in.device)
 
         # channels-last input, zero-padded to a multiple of 64 channels when the first conv can use the tensor cores
         Cp = _round_up(C0, 64)
         if plan.skip and conv_p[0][0].shape[0] == C0:
             Cp = C0                                         # layer 0 has a residual: its input keeps the true width
-        conv0 = _Conv(conv_p[0][0], T, False, tc, pad_cin_to=Cp, want_bwd=save)
+        conv0 = _Conv(conv_p[0][0], T, False, tc, pad_cin_to=Cp, want_bwd=save and nd.below[0])
         if not conv0.fwd_tc and Cp != C0:
             Cp = C0
-            conv0 = _Conv(conv_p[0][0], T, False, False, want_bwd=save)
+            conv0 = _Conv(conv_p[0][0], T, False, False, want_bwd=save and nd.below[0])
         x = _empty((B, T, Cp), x_in)                               # the transpose writes the pad columns as zeros
         call("bm_transpose_nt_ld", ptr(x_in), B, C0, T, Cp, ptr(x), st)
 
@@ -86,7 +109,8 @@ class _ConvSequenceFn(torch.autograd.Function):
         layers = []
         for k in range(depth):
             w, b, gamma, beta = conv_p[k]
-            conv = conv0 if k == 0 else _Conv(w, T, False, tc, want_bwd=save)
+            conv = conv0 if k == 0 else _Conv(w, T, False, tc, want_bwd=save and nd.below[k])
+            keep = save and nd.below[k + 1]          # the backward reaches this layer
             cout = conv.cout
             y = _empty((B, T, cout), x_in)
             skip = plan.skip and conv.cin_true == cout
@@ -111,23 +135,26 @@ class _ConvSequenceFn(torch.autograd.Function):
                               None if beta is None else beta.contiguous(), x if skip else None, x_new, rows, cout, act)
             else:
                 x_new = y                                   # a bare convolution (DeepMel's last layer)
-            rec = dict(x_in=x, y=y, mean=mean, invstd=invstd, conv=conv, skip=skip, act=act, has_bn=has_bn, x_new=x_new)
+            # kept: the conv input for its weight gradient, y for the activation backward, x_new for the GLU weight gradient
+            rec = dict(x_in=x if nd.layer[k][0] else None, y=y if nd.layer_up(k) else None, mean=mean, invstd=invstd,
+                       conv=conv, skip=skip, act=act, has_bn=has_bn, x_new=x_new if nd.glu.get(k, (False,))[0] else None)
             x = x_new
             if plan.glu_after[k]:
                 gw, gb = glu_p[k]
-                gconv = _Conv(gw, T, True, tc, want_bwd=save)
-                h = _empty((B, T, gconv.cout), x_in) if save else None
+                gconv = _Conv(gw, T, True, tc, want_bwd=save and nd.layer_up(k))
+                h = _empty((B, T, gconv.cout), x_in) if keep else None
                 out = _empty((B, T, gconv.cout // 2), x_in)
                 gconv.forward_glu(x, gb.contiguous(), B, T, h, out, status)
                 rec.update(h=h, gconv=gconv)
                 x = out
-            layers.append(rec if save else None)
+            layers.append(rec if keep else None)
 
         C_last = x.shape[2]
         out_cm = _empty((B, C_last, T), x_in)
         call("bm_transpose_nt", ptr(x), B, T, C_last, ptr(out_cm), st)       # [B, T, C] -> [B, C, T]
         if save:
             ctx.plan = plan
+            ctx.needs = nd
             ctx.dims = (B, C0, Cp, T, C_last)
             ctx.saved = dict(layers=layers, conv_p=conv_p, glu_p=glu_p)
         return out_cm
@@ -148,39 +175,55 @@ class _ConvSequenceFn(torch.autograd.Function):
         status = tc_status_tensor(dout.device)
         g = _empty((B, T, C_last), dout)
         call("bm_transpose_nt", ptr(dout), B, C_last, T, ptr(g), st)          # [B, C, T] -> [B, T, C]
-        need_dx = ctx.needs_input_grad[1]
+        nd: _Needs = ctx.needs
+        need_dx = nd.front[0]
         max_c = max(w.shape[0] for w, _, _, _ in s["conv_p"])
         sums = _empty((2 * max_c,), dout, torch.float64)
         layer_grads: tp.List[tp.Any] = [None] * depth
-        glu_grads = {}
+        glu_grads = {k: (None, None) for k in nd.glu}
         for k in reversed(range(depth)):
-            rec = s["layers"][k]
             w, b, gamma, beta = s["conv_p"][k]
+            if not nd.below[k + 1]:
+                layer_grads[k] = (None,) * (4 if gamma is not None else 2)
+                continue                               # nothing at or below this layer requires grad
+            rec = s["layers"][k]
             conv: _Conv = rec["conv"]
             cout = conv.cout
+            n_cw, n_cb, n_gamma, n_beta = nd.layer[k]
             if plan.glu_after[k]:
                 gconv: _Conv = rec["gconv"]
+                n_gw, n_gb = nd.glu[k]
                 dh = _empty((B, T, gconv.cout), dout)
-                dgb = torch.empty((gconv.cout,), device=dout.device, dtype=torch.float32)
+                dgb = torch.empty((gconv.cout,), device=dout.device, dtype=torch.float32) if n_gb else None
                 _reducing_call("bm_glu_bwd", dout, (rows, gconv.cout // 2), ptr(g), ptr(rec["h"]), rows, gconv.cout // 2,
-                               ptr(dh), ptr(dgb), None, st)
-                glu_grads[k] = gconv.backward_weight(dh, rec["x_new"], B, T, 1, dout, status, known_dbias=dgb)
+                               ptr(dh), ptr(dgb), None, st, reduces=n_gb)
+                glu_grads[k] = gconv.backward_weight(dh, rec["x_new"], B, T, 1, dout, status, known_dbias=dgb, want_w=n_gw,
+                                                     want_b=n_gb)
+                if not nd.layer_up(k):
+                    layer_grads[k] = (None,) * (4 if gamma is not None else 2)
+                    del dh
+                    continue
                 g = _empty((B, T, gconv.cin), dout)
                 gconv.backward_data(dh, None, B, T, 1, g, status)
                 del dh
             dgamma = dbeta = None
             if rec["has_bn"]:
+                # reduces in training mode; in eval mode only for trainable gamma / beta (else one elementwise pass)
+                reduce = plan.training or n_gamma or n_beta
                 dy = _empty((B, T, cout), dout)
-                dgamma, dbeta = _empty((cout,), dout), _empty((cout,), dout)
+                dgamma, dbeta = (_empty((cout,), dout), _empty((cout,), dout)) if reduce else (None, None)
+                sums_k = sums if reduce else None
                 if rec["act"] == ACT_GELU:
                     _reducing_call("bm_bn_gelu_skip_bwd", dout, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
                                    ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()),
-                                   1 if plan.training else 0, rows, cout, ptr(sums), ptr(dy), ptr(dgamma), ptr(dbeta), None, st)
+                                   1 if plan.training else 0, rows, cout, ptr(sums_k), ptr(dy), ptr(dgamma), ptr(dbeta), None,
+                                   st, reduces=reduce)
                 else:
                     _reducing_call("bm_bn_act_skip_bwd", dout, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
                                    ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()),
-                                   1 if plan.training else 0, rows, cout, rec["act"], float(plan.act_slope), ptr(sums), ptr(dy),
-                                   ptr(dgamma), ptr(dbeta), st)
+                                   1 if plan.training else 0, rows, cout, rec["act"], float(plan.act_slope), ptr(sums_k),
+                                   ptr(dy), ptr(dgamma), ptr(dbeta), st, reduces=reduce)
+                dgamma, dbeta = (dgamma if n_gamma else None), (dbeta if n_beta else None)
             elif rec["act"] != ACT_NONE:
                 dy = _empty((B, T, cout), dout)
                 call("bm_bn_act_skip_bwd", ptr(g), ptr(rec["y"]), None, None, None, None, 0, rows, cout, rec["act"],
@@ -189,8 +232,8 @@ class _ConvSequenceFn(torch.autograd.Function):
                 dy = g                                       # bare convolution (+ skip): dL/dy = dL/dx_new
             # with a training-mode BatchNorm behind the conv, sum(dy) is exactly 0: skip the bias reduction
             dcw, dcb = conv.backward_weight(dy, rec["x_in"], B, T, plan.dilations[k], dout, status,
-                                            bias_grad_is_zero=bool(rec["has_bn"] and plan.training))
-            if k == 0 and not need_dx:
+                                            bias_grad_is_zero=bool(rec["has_bn"] and plan.training), want_w=n_cw, want_b=n_cb)
+            if not nd.below[k]:
                 g = None
             elif rec["skip"]:
                 if dy is g:                                  # the in-place reduce-add needs distinct dy and g

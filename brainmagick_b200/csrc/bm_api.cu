@@ -223,10 +223,11 @@ extern "C" int bm_sensor_chain_fwd(const float* meg, const float* weights, const
 extern "C" int bm_subject_layers_bwd(const float* dx0, int ld_x0, const float* v, int ld_v, const float* subj_w,
                                      const int* subject, const int* subj_order, const int* subj_off, int B, int T, int IL,
                                      int D, int S, int ld_dv, float* dv, float* d_subj_w, bm_stream_t stream) {
-    BM_CHECK_ARG(dx0 && v && subj_w && subject && subj_order && subj_off && dv && d_subj_w);
+    // dv NULL: no data gradient (nothing below needs it); d_subj_w NULL: frozen weights
+    BM_CHECK_ARG(dx0 && (!dv || (subj_w && subject)) && (!d_subj_w || (v && subj_order && subj_off)));
     BM_CHECK_ARG(ld_x0 >= D && ld_v >= IL && ld_dv >= IL);
     cudaStream_t st = ST(stream);
-    {   // dv[b][t][p] = sum_d g[b][t][d] M[s_b][p][d]
+    if (dv) {   // dv[b][t][p] = sum_d g[b][t][d] M[s_b][p][d]
         GemmP g = gemm_defaults();
         g.M = T; g.N = IL; g.K = D; g.kchunk = D;
         g.Z = B; g.nseg = B; g.zchunk = 1;
@@ -235,7 +236,7 @@ extern "C" int bm_subject_layers_bwd(const float* dx0, int ld_x0, const float* v
         g.D = dv; g.ldd_z = (long long)T * ld_dv; g.ldd_m = ld_dv; g.ldd_n = 1;
         BM_CUDA(launch_gemm(g, st));
     }
-    {   // dM[s][p][d] = sum_{b in s} sum_t v[b][t][p] g[b][t][d]
+    if (d_subj_w) {   // dM[s][p][d] = sum_{b in s} sum_t v[b][t][p] g[b][t][d]
         GemmP g = gemm_defaults();
         g.M = IL; g.N = D; g.K = T; g.kchunk = T;
         g.Z = B; g.nseg = S; g.seg_off = subj_off; g.zlist = subj_order;
@@ -247,11 +248,12 @@ extern "C" int bm_subject_layers_bwd(const float* dx0, int ld_x0, const float* v
     return 0;
 }
 
-// part: NULL (atomic reductions) or the colsum_ws_floats(B*T, IL) partials of the deterministic form
+// part: NULL (atomic reductions) or the colsum_ws_floats(B*T, IL) partials of the deterministic form.
+// du, d_il_w, d_il_b may each be NULL (no data gradient below / frozen parameter): its GEMM or reduction is skipped.
 static int initial_linear_bwd(const float* dv, int ld_dv, const float* u, int ld_u, const float* il_w, int B, int T, int O,
                               int IL, int ld_du, float* du, float* d_il_w, float* d_il_b, float* part, cudaStream_t st) {
-    BM_CHECK_ARG(dv && u && il_w && du && d_il_w && d_il_b && ld_dv >= IL && ld_u >= O && ld_du >= O);
-    {   // d_il_w[p][o] = sum_{b,t} dv[b][t][p] u[b][t][o]
+    BM_CHECK_ARG(dv && (!du || il_w) && (!d_il_w || u) && ld_dv >= IL && ld_u >= O && ld_du >= O);
+    if (d_il_w) {   // d_il_w[p][o] = sum_{b,t} dv[b][t][p] u[b][t][o]
         BM_CUDA(cudaMemsetAsync(d_il_w, 0, sizeof(float) * IL * O, st));
         GemmP g = gemm_defaults();
         g.M = IL; g.N = O; g.K = T; g.kchunk = T;
@@ -267,9 +269,9 @@ static int initial_linear_bwd(const float* dv, int ld_dv, const float* u, int ld
             BM_CUDA(launch_gemm(g, st));
         }
     }
-    if (part) {   // d_il_b[p] = sum dv, through the partials
+    if (d_il_b && part) {   // d_il_b[p] = sum dv, through the partials
         if (int rc = colsum(dv, (long long)B * T, IL, ld_dv, part, d_il_b, st)) return rc;
-    } else {   // d_il_b[p] = sum dv
+    } else if (d_il_b) {   // d_il_b[p] = sum dv
         BM_CUDA(cudaMemsetAsync(d_il_b, 0, sizeof(float) * IL, st));
         GemmP g = gemm_defaults();                      // column sums as a 1-row GEMM would waste a tile: dedicated kernel
         (void)g;
@@ -278,7 +280,7 @@ static int initial_linear_bwd(const float* dv, int ld_dv, const float* u, int ld
         colsum_strided_kernel<<<grid, 128, 0, st>>>(dv, d_il_b, rows, IL, ld_dv, 256);
         BM_CHECK_LAUNCH();
     }
-    {   // du[row][o] = sum_p dv[row][p] il_w[p][o]
+    if (du) {   // du[row][o] = sum_p dv[row][p] il_w[p][o]
         GemmP g = gemm_defaults();
         g.M = B * T; g.N = O; g.K = IL; g.kchunk = IL;
         g.A = dv; g.lda_m = ld_dv; g.lda_k = 1;
@@ -302,6 +304,8 @@ extern "C" int bm_initial_linear_bwd_det(const float* dv, int ld_dv, const float
                                          int O, int IL, int ld_du, float* du, float* d_il_w, float* d_il_b, float* workspace,
                                          long long workspace_floats, bm_stream_t stream) {
     BM_CHECK_ARG(B > 0 && T > 0 && O > 0 && IL > 0);
+    if (!d_il_w && !d_il_b)                      // the data gradient alone reduces nothing: no workspace
+        return initial_linear_bwd(dv, ld_dv, u, ld_u, il_w, B, T, O, IL, ld_du, du, nullptr, nullptr, nullptr, ST(stream));
     BM_CHECK_WS(bm_initial_linear_bwd_det_workspace(B, T, O, IL));
     return initial_linear_bwd(dv, ld_dv, u, ld_u, il_w, B, T, O, IL, ld_du, du, d_il_w, d_il_b, workspace, ST(stream));
 }
@@ -335,20 +339,38 @@ extern "C" int bm_sensor_mix_bwd_data(const float* du, int ld_du, const float* w
     return 0;
 }
 
+// det: the _det form (initial_linear's reductions through `workspace`).  Each stage runs only as far as its outputs are asked for:
+// d_subj_w, d_il_w, d_il_b, d_weights NULL = frozen parameter; du NULL = no mix gradient and no meg gradient below (then
+// d_weights must be NULL); dv NULL = nothing below the subject layer (then du, d_il_w, d_il_b must be NULL).
+static int sensor_chain_bwd(const float* dx0, const float* meg, const float* il_w, const float* subj_w, const int* subject,
+                            const float* u, const float* v, const int* subj_order, const int* subj_off, const int* rec_order,
+                            const int* rec_off, int B, int C, int T, int O, int IL, int D, int ld_x0, int S, int R, float* dv,
+                            float* du, float* d_subj_w, float* d_il_w, float* d_il_b, float* d_weights, float* workspace,
+                            long long workspace_floats, bool det, bm_stream_t stream) {
+    BM_CHECK_ARG(dx0 && ld_x0 >= D);
+    BM_CHECK_ARG((dv || !(du || d_il_w || d_il_b)) && (du || !d_weights));
+    BM_CHECK_ARG(!d_weights || (meg && rec_order && rec_off));
+    // the subject and sensor-mix gradients reduce each segment inside one CTA: already fixed-order
+    int rc = 0;
+    if (dv || d_subj_w)
+        rc = bm_subject_layers_bwd(dx0, ld_x0, v, IL, subj_w, subject, subj_order, subj_off, B, T, IL, D, S, IL, dv, d_subj_w,
+                                   stream);
+    if (!rc && (du || d_il_w || d_il_b))
+        rc = det ? bm_initial_linear_bwd_det(dv, IL, u, O, il_w, B, T, O, IL, O, du, d_il_w, d_il_b, workspace,
+                                             workspace_floats, stream)
+                 : bm_initial_linear_bwd(dv, IL, u, O, il_w, B, T, O, IL, O, du, d_il_w, d_il_b, stream);
+    if (!rc && d_weights) rc = bm_sensor_mix_bwd(du, O, meg, rec_order, rec_off, B, C, T, O, R, d_weights, stream);
+    return rc;
+}
+
 extern "C" int bm_sensor_chain_bwd(const float* dx0, const float* meg, const float* il_w, const float* subj_w,
                                    const int* subject, const float* u, const float* v, const int* subj_order,
                                    const int* subj_off, const int* rec_order, const int* rec_off, int B, int C,
                                    int T, int O, int IL, int D, int ld_x0, int S, int R, float* dv, float* du,
                                    float* d_subj_w, float* d_il_w, float* d_il_b, float* d_weights,
                                    bm_stream_t stream) {
-    BM_CHECK_ARG(dx0 && meg && il_w && subj_w && subject && u && v && subj_order && subj_off && rec_order && rec_off);
-    BM_CHECK_ARG(dv && du && d_subj_w && d_il_w && d_il_b && d_weights);
-    BM_CHECK_ARG(ld_x0 >= D);
-    int rc = bm_subject_layers_bwd(dx0, ld_x0, v, IL, subj_w, subject, subj_order, subj_off, B, T, IL, D, S, IL, dv,
-                                   d_subj_w, stream);
-    if (!rc) rc = bm_initial_linear_bwd(dv, IL, u, O, il_w, B, T, O, IL, O, du, d_il_w, d_il_b, stream);
-    if (!rc) rc = bm_sensor_mix_bwd(du, O, meg, rec_order, rec_off, B, C, T, O, R, d_weights, stream);
-    return rc;
+    return sensor_chain_bwd(dx0, meg, il_w, subj_w, subject, u, v, subj_order, subj_off, rec_order, rec_off, B, C, T, O, IL,
+                            D, ld_x0, S, R, dv, du, d_subj_w, d_il_w, d_il_b, d_weights, nullptr, 0, false, stream);
 }
 
 extern "C" long long bm_sensor_chain_bwd_det_workspace(int B, int T, int O, int IL) {
@@ -360,16 +382,9 @@ extern "C" int bm_sensor_chain_bwd_det(const float* dx0, const float* meg, const
                                        int T, int O, int IL, int D, int ld_x0, int S, int R, float* dv, float* du,
                                        float* d_subj_w, float* d_il_w, float* d_il_b, float* d_weights, float* workspace,
                                        long long workspace_floats, bm_stream_t stream) {
-    BM_CHECK_ARG(dx0 && meg && il_w && subj_w && subject && u && v && subj_order && subj_off && rec_order && rec_off);
-    BM_CHECK_ARG(dv && du && d_subj_w && d_il_w && d_il_b && d_weights);
-    BM_CHECK_ARG(ld_x0 >= D);
-    // the subject and sensor-mix gradients reduce each segment inside one CTA: already fixed-order
-    int rc = bm_subject_layers_bwd(dx0, ld_x0, v, IL, subj_w, subject, subj_order, subj_off, B, T, IL, D, S, IL, dv,
-                                   d_subj_w, stream);
-    if (!rc) rc = bm_initial_linear_bwd_det(dv, IL, u, O, il_w, B, T, O, IL, O, du, d_il_w, d_il_b, workspace,
-                                            workspace_floats, stream);
-    if (!rc) rc = bm_sensor_mix_bwd(du, O, meg, rec_order, rec_off, B, C, T, O, R, d_weights, stream);
-    return rc;
+    return sensor_chain_bwd(dx0, meg, il_w, subj_w, subject, u, v, subj_order, subj_off, rec_order, rec_off, B, C, T, O, IL,
+                            D, ld_x0, S, R, dv, du, d_subj_w, d_il_w, d_il_b, d_weights, workspace, workspace_floats, true,
+                            stream);
 }
 
 // =================================================================================================
@@ -464,18 +479,34 @@ extern "C" int bm_bn_gelu_skip_fwd(const float* y, const float* mean, const floa
     return 0;
 }
 
+// The column reduction (sums, dgamma, dbeta) runs unless batch_stats == 0 and dgamma == dbeta == NULL: the data gradient of an
+// eval-mode BatchNorm whose affine parameters are frozen is then one elementwise pass (the apply kernels read the sums / dgamma /
+// dbeta only when use_batch_stats is set, so its dy is bitwise the reducing form's).
+static bool bn_bwd_reduces(int batch_stats, const float* dgamma, const float* dbeta) {
+    return batch_stats || dgamma || dbeta;
+}
+
 // part: NULL (fp64 atomics into sums) or the bn_bwd_ws_floats(rows, C) partials of the deterministic form
 static int bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
                             const float* beta, int batch_stats, long long rows, int C, double* sums, float* dy, float* dgamma,
                             float* dbeta, float* amax_out, double* part, cudaStream_t st) {
-    BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && sums && dy && dgamma && dbeta && rows > 0 && C > 0);
-    if (!part) BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
+    BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && dy && rows > 0 && C > 0);
+    const bool reduce = bn_bwd_reduces(batch_stats, dgamma, dbeta);
+    BM_CHECK_ARG(!reduce || (sums && dgamma && dbeta));
+    if (reduce && !part) BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
     if (int rc = amax_begin(amax_out, st)) return rc;
     const long long total = rows * C;
     const bool vec = (C % 4 == 0) && aligned16(g, y, dy) && aligned16(mean, invstd, gamma) && aligned16(beta);
     if (vec && C / 4 <= 256 && aligned16(dgamma, dbeta)) {
         const int cx = C / 4, ry = std::max(1, 320 / cx);
         const unsigned nblk = (unsigned)((rows + CS_ROWS_PER_BLOCK - 1) / CS_ROWS_PER_BLOCK);
+        if (!reduce) {
+            bn_gelu_bwd_apply_cs_kernel<<<nblk, dim3(cx, ry), 0, st>>>(g, y, mean, invstd, gamma, beta, nullptr, nullptr,
+                                                                       (float)(1.0 / (double)rows), 0, dy, rows, C,
+                                                                       reinterpret_cast<unsigned int*>(amax_out));
+            BM_CHECK_LAUNCH();
+            return 0;
+        }
         if (part) {
             bn_gelu_bwd_reduce_cs_kernel<true><<<nblk, dim3(cx, ry), sizeof(float) * 2 * C * ry, st>>>(
                 g, y, mean, invstd, gamma, beta, part, rows, C);
@@ -494,7 +525,7 @@ static int bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, c
         BM_CHECK_LAUNCH();
         return 0;
     }
-    {   // generic shapes: one thread per column, 128 rows per block
+    if (reduce) {   // generic shapes: one thread per column, 128 rows per block
         const int rpb = 128;
         dim3 grid((unsigned)((rows + rpb - 1) / rpb), (C + 127) / 128);
         if (part) {
@@ -505,9 +536,9 @@ static int bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, c
             bn_gelu_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C, rpb);
             BM_CHECK_LAUNCH();
         }
+        bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
+        BM_CHECK_LAUNCH();
     }
-    bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
-    BM_CHECK_LAUNCH();
     if (vec)
         bn_gelu_bwd_apply_v4_kernel<<<ew_grid(total / 4), 256, 0, st>>>(
             reinterpret_cast<const float4*>(g), reinterpret_cast<const float4*>(y), reinterpret_cast<const float4*>(mean),
@@ -537,6 +568,9 @@ extern "C" int bm_bn_gelu_skip_bwd_det(const float* g, const float* y, const flo
                                        double* sums, float* dy, float* dgamma, float* dbeta, float* amax_out,
                                        float* workspace, long long workspace_floats, bm_stream_t stream) {
     BM_CHECK_ARG(rows > 0 && C > 0);
+    if (!bn_bwd_reduces(batch_stats, dgamma, dbeta))     // one elementwise pass: nothing is reduced, no workspace
+        return bn_gelu_skip_bwd(g, y, mean, invstd, gamma, beta, 0, rows, C, sums, dy, nullptr, nullptr, amax_out, nullptr,
+                                ST(stream));
     BM_CHECK_WS(bn_bwd_ws_floats(rows, C));
     return bn_gelu_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, sums, dy, dgamma, dbeta, amax_out,
                             reinterpret_cast<double*>(workspace), ST(stream));
@@ -652,6 +686,8 @@ extern "C" long long bm_glu_bwd_det_workspace(long long rows, int H) {
 extern "C" int bm_glu_bwd_det(const float* g, const float* h, long long rows, int H, float* dh, float* dbias,
                               float* amax_out, float* workspace, long long workspace_floats, bm_stream_t stream) {
     BM_CHECK_ARG(rows > 0 && H > 0);
+    if (!dbias)                                  // no bias gradient: nothing is reduced, the workspace is not used
+        return glu_bwd(g, h, rows, H, dh, nullptr, amax_out, nullptr, ST(stream));
     BM_CHECK_WS(glu_bwd_ws_floats(rows, H));
     return glu_bwd(g, h, rows, H, dh, dbias, amax_out, workspace, ST(stream));
 }
@@ -687,13 +723,17 @@ extern "C" int bm_head_fwd(const float* x, const float* w0, const float* b0, con
 }
 
 // dW2, db2, dh1 = dq*GELU'(h1) (in place in dq), dW0, db0 -- the parameter-gradient half of the head backward
-// part: NULL (atomic reductions) or the head_ws_floats(B, T, H, F) partials of the deterministic form
+// part: NULL (atomic reductions) or the head_ws_floats(B, T, H, F) partials of the deterministic form.  Each of dw0, db0, dw2,
+// db2 may be NULL (a frozen parameter): its GEMM / reduction is skipped.  want_dh1 = 0: dq is not turned into dh1 (nothing
+// reads it: the caller wants neither dx nor dw0 / db0).
 static int head_bwd_params(const float* dest, const float* x, const float* h1, const float* q, int B, int T, int H, int F,
-                           float* dq, float* dw0, float* db0, float* dw2, float* db2, float* part, cudaStream_t st) {
-    BM_CHECK_ARG(dest && x && h1 && q && dq && dw0 && db0 && dw2 && db2);
+                           float* dq, float* dw0, float* db0, float* dw2, float* db2, float* part, cudaStream_t st,
+                           bool want_dh1 = true) {
+    BM_CHECK_ARG(dest && (!want_dh1 || (h1 && dq)) && (!dw0 || x) && (!dw2 || q));
+    BM_CHECK_ARG(want_dh1 || (!dw0 && !db0));
     const int H2 = 2 * H;
     const long long rows = (long long)B * T;
-    {   // dw2[i][f] = sum_{b,t} q[b][t][i] dest[b][f][t]
+    if (dw2) {   // dw2[i][f] = sum_{b,t} q[b][t][i] dest[b][f][t]
         GemmP g = gemm_defaults();
         g.M = H2; g.N = F; g.K = T; g.kchunk = T;
         g.Z = B; g.nseg = pick_chunks(B, tiles_of(H2, F)); g.zchunk = (B + g.nseg - 1) / g.nseg;
@@ -709,7 +749,7 @@ static int head_bwd_params(const float* dest, const float* x, const float* h1, c
             BM_CUDA(launch_gemm(g, st));
         }
     }
-    {   // db2[f] = sum_{b,t} dest[b][f][t]
+    if (db2) {   // db2[f] = sum_{b,t} dest[b][f][t]
         long long nrows = (long long)B * F;
         if (part) {
             rowsum_cm_kernel<true><<<(unsigned)((nrows + 7) / 8), 256, 0, st>>>(dest, part, B, F, T);
@@ -721,9 +761,10 @@ static int head_bwd_params(const float* dest, const float* x, const float* h1, c
             BM_CHECK_LAUNCH();
         }
     }
+    if (!want_dh1) return 0;
     gelu_bwd_kernel<<<ew_grid(rows * H2), 256, 0, st>>>(dq, h1, dq, rows * H2);   // dq <- dh1
     BM_CHECK_LAUNCH();
-    {   // dw0[n][k] = sum_rows dh1[row][n] x[row][k]
+    if (dw0) {   // dw0[n][k] = sum_rows dh1[row][n] x[row][k]
         GemmP g = gemm_defaults();
         g.M = H2; g.N = H; g.K = T; g.kchunk = T;
         g.Z = B; g.nseg = pick_chunks(B, tiles_of(H2, H)); g.zchunk = (B + g.nseg - 1) / g.nseg;
@@ -739,6 +780,7 @@ static int head_bwd_params(const float* dest, const float* x, const float* h1, c
             BM_CUDA(launch_gemm(g, st));
         }
     }
+    if (!db0) return 0;
     if (part) return colsum(dq, rows, H2, H2, part, db0, st);   // db0; the partials buffer is reused stage after stage
     {   // db0
         BM_CUDA(cudaMemsetAsync(db0, 0, sizeof(float) * H2, st));
@@ -761,17 +803,18 @@ extern "C" int bm_head_bwd_params_det(const float* dest, const float* x, const f
                                       int H, int F, float* dq, float* dw0, float* db0, float* dw2, float* db2,
                                       float* workspace, long long workspace_floats, bm_stream_t stream) {
     BM_CHECK_ARG(B > 0 && T > 0 && H > 0 && F > 0);
-    BM_CHECK_WS(head_ws_floats(B, T, H, F));
+    if (dw0 || db0 || dw2 || db2) BM_CHECK_WS(head_ws_floats(B, T, H, F));
     return head_bwd_params(dest, x, h1, q, B, T, H, F, dq, dw0, db0, dw2, db2, workspace, ST(stream));
 }
 
 static int head_bwd(const float* dest, const float* x, const float* w0, const float* w2, const float* h1, const float* q, int B,
                     int T, int H, int F, float* dq, float* dx, float* dw0, float* db0, float* dw2, float* db2, float* part,
                     cudaStream_t st) {
-    BM_CHECK_ARG(dest && x && w0 && w2 && h1 && q && dq && dx && dw0 && db0 && dw2 && db2);
+    const bool want_dh1 = dx || dw0 || db0;       // else only dw2 / db2 (or nothing) is asked for: no dq, no GELU'
+    BM_CHECK_ARG(dest && (!want_dh1 || (w2 && h1 && dq)) && (!dx || w0));
     const int H2 = 2 * H;
     const long long rows = (long long)B * T;
-    {   // dq[b][t][i] = sum_f dest[b][f][t] w2[i][f]
+    if (want_dh1) {   // dq[b][t][i] = sum_f dest[b][f][t] w2[i][f]
         GemmP g = gemm_defaults();
         g.M = T; g.N = H2; g.K = F; g.kchunk = F;
         g.Z = B; g.nseg = B; g.zchunk = 1;
@@ -780,9 +823,9 @@ static int head_bwd(const float* dest, const float* x, const float* w0, const fl
         g.D = dq; g.ldd_z = (long long)T * H2; g.ldd_m = H2; g.ldd_n = 1;
         BM_CUDA(launch_gemm(g, st));
     }
-    int rc = head_bwd_params(dest, x, h1, q, B, T, H, F, dq, dw0, db0, dw2, db2, part, st);
+    int rc = head_bwd_params(dest, x, h1, q, B, T, H, F, dq, dw0, db0, dw2, db2, part, st, want_dh1);
     if (rc) return rc;
-    {   // dx[row][k] = sum_n dh1[row][n] w0[n][k]
+    if (dx) {   // dx[row][k] = sum_n dh1[row][n] w0[n][k]
         GemmP g = gemm_defaults();
         g.M = (int)rows; g.N = H; g.K = H2; g.kchunk = H2;
         g.A = dq; g.lda_m = H2; g.lda_k = 1;
@@ -806,7 +849,7 @@ extern "C" int bm_head_bwd_det(const float* dest, const float* x, const float* w
                                float* db0, float* dw2, float* db2, float* workspace, long long workspace_floats,
                                bm_stream_t stream) {
     BM_CHECK_ARG(B > 0 && T > 0 && H > 0 && F > 0);
-    BM_CHECK_WS(head_ws_floats(B, T, H, F));
+    if (dw0 || db0 || dw2 || db2) BM_CHECK_WS(head_ws_floats(B, T, H, F));
     return head_bwd(dest, x, w0, w2, h1, q, B, T, H, F, dq, dx, dw0, db0, dw2, db2, workspace, ST(stream));
 }
 
@@ -1010,8 +1053,10 @@ static int bn_act_skip_bwd(const float* g, const float* y, const float* mean, co
                            const float* beta, int batch_stats, long long rows, int C, int act, float slope, double* sums,
                            float* dy, float* dgamma, float* dbeta, double* part, cudaStream_t st) {
     BM_CHECK_ARG(g && y && dy && rows > 0 && C > 0 && act >= 0 && act <= 2);
-    BM_CHECK_ARG(!mean || (invstd && gamma && beta && sums && dgamma && dbeta));
-    if (mean) {
+    BM_CHECK_ARG(!mean || (invstd && gamma && beta));
+    const bool reduce = mean && bn_bwd_reduces(batch_stats, dgamma, dbeta);
+    BM_CHECK_ARG(!reduce || (sums && dgamma && dbeta));
+    if (reduce) {
         const int rpb = 128;
         dim3 grid((unsigned)((rows + rpb - 1) / rpb), (C + 127) / 128);
         if (part) {
@@ -1048,7 +1093,7 @@ extern "C" int bm_bn_act_skip_bwd_det(const float* g, const float* y, const floa
                                       int act, float slope, double* sums, float* dy, float* dgamma, float* dbeta,
                                       float* workspace, long long workspace_floats, bm_stream_t stream) {
     BM_CHECK_ARG(rows > 0 && C > 0);
-    if (!mean)                                   // no BatchNorm: nothing is reduced, the workspace is not used
+    if (!mean || !bn_bwd_reduces(batch_stats, dgamma, dbeta))   // nothing is reduced, the workspace is not used
         return bn_act_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, sums, dy, dgamma, dbeta,
                                nullptr, ST(stream));
     BM_CHECK_WS(bn_bwd_ws_floats(rows, C));

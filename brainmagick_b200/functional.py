@@ -109,11 +109,14 @@ def _det_workspace(name, like, *dims) -> torch.Tensor:
     return torch.empty((max(n, 2),), device=like.device, dtype=torch.float32)
 
 
-def _reducing_call(name, like, ws_dims, *args):
+def _reducing_call(name, like, ws_dims, *args, reduces=True):
     """call(name, *args) -- or, under the determinism flag, `name`_det with the workspace of `name`_det_workspace(*ws_dims)
-    inserted before the stream argument (ws_dims None: a _det form without workspace, same arguments)."""
+    inserted before the stream argument (ws_dims None: a _det form without workspace, same arguments).  `reduces=False`:
+    the NULL gradient pointers of this call leave nothing to reduce, so the _det form gets no workspace (NULL, 0)."""
     if not _lib.deterministic():
         return call(name, *args)
+    if ws_dims is not None and not reduces:
+        return call(name + "_det", *args[:-1], None, 0, args[-1])
     if ws_dims is None:
         return call(name + "_det", *args)
     ws = _det_workspace(name + "_det", like, *ws_dims)
@@ -330,10 +333,28 @@ class _Conv:
                  dilation, ptr(dx), st)
 
     def backward_weight(self, dy, x, B, T, dilation, like, status, bias_grad_is_zero=False, known_dbias=None, dy_amax=None,
-                        x_amax=None):
+                        x_amax=None, want_w=True, want_b=True):
         """`bias_grad_is_zero`: the conv feeds a training-mode BatchNorm, whose backward makes sum(dy) == 0 exactly
         (the reference's value there is rounding noise around 0); skip the reduction.  `known_dbias`: the producer of dy
-        already summed it over the rows.  `dy_amax` / `x_amax`: see tc_wgrad."""
+        already summed it over the rows.  `dy_amax` / `x_amax`: see tc_wgrad.  `want_w` / `want_b` False: that parameter is
+        frozen; its gradient is neither computed nor returned (None)."""
+        if not want_w:
+            if not want_b:
+                return None, None
+            if known_dbias is not None:
+                return None, known_dbias
+            db = torch.zeros((self.cout,), device=like.device) if bias_grad_is_zero else _empty((self.cout,), like)
+            if not bias_grad_is_zero:
+                col_sum(dy, B * T, self.cout, db, stream())
+            return None, db
+        if not want_b:
+            if self.wgrad_tc:
+                return tc_wgrad(dy, x, B, T, self.cout, self.cin, self.cin_true, self.kw, dilation, status, dy_amax=dy_amax,
+                                x_amax=x_amax), None
+            dw = _empty((self.cout, self.cin, self.kw), like)
+            _reducing_call("bm_conv1d_bwd_weight", like, (B, T, self.cin, self.cout, self.kw), ptr(dy), ptr(x), B, T,
+                           self.cin, self.cout, self.kw, dilation, ptr(dw), None, stream())
+            return (dw[:, :self.cin_true].contiguous() if self.cin != self.cin_true else dw), None
         if self.wgrad_tc:
             am = dict(dy_amax=dy_amax, x_amax=x_amax)
             if known_dbias is not None:
@@ -399,38 +420,45 @@ def _staged_front_forward(plan: "EncoderPlan", meg, heads, il_w, il_b, subj_w, s
     return x, saved
 
 
-def _staged_front_backward(plan: "EncoderPlan", saved, g, heads, il_w, subj_w, sub_emb, want_dmeg=False):
-    """g = dL/dx [B,T,D_total] -> (dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg); None where the stage is absent or
-    (dmeg) not wanted."""
+def _staged_front_backward(plan: "EncoderPlan", saved, g, heads, il_w, subj_w, sub_emb, need):
+    """g = dL/dx [B,T,D_total] -> (dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg); None where the stage is absent or its
+    gradient is not wanted.  need = requires-grad of (meg, heads, il_w, il_b, subj_w, sub_emb): each stage computes the
+    gradients asked of it, and its data gradient only while a stage below it still needs one."""
     st = stream()
     meg = saved["meg"]
     B, C, T = meg.shape
     R = plan.rec_positions.shape[0]
     _, w_u, w_v, w_x = saved["widths"]
+    n_meg, n_heads, n_il_w, n_il_b, n_subj, n_emb = need
     d_sub_emb = None
     if sub_emb is not None:
-        d_sub_emb = g[:, :, w_x:].sum(dim=1)                   # the embedding is constant over time
-        g = g[:, :, :w_x].contiguous()
+        if n_emb:
+            d_sub_emb = g[:, :, w_x:].sum(dim=1)               # the embedding is constant over time
+        g = g[:, :, :w_x].contiguous() if any(need[:5]) else None
     d_subj = None
-    if subj_w is not None:
+    if subj_w is not None and (n_subj or any(need[:4])):
         S = subj_w.shape[0]
-        subj_order, subj_off = group_layout(plan.subject, S)
-        d_subj = _empty((S, w_v, w_x), meg)
-        dv = _empty((B, T, w_v), meg)
+        subj_order, subj_off = group_layout(plan.subject, S) if n_subj else (None, None)
+        d_subj = _empty((S, w_v, w_x), meg) if n_subj else None
+        dv = _empty((B, T, w_v), meg) if any(need[:4]) else None
         call("bm_subject_layers_bwd", ptr(g), w_x, ptr(saved["v"]), w_v, ptr(subj_w.contiguous()), ptr(plan.subject),
              ptr(subj_order), ptr(subj_off), B, T, w_v, w_x, S, w_v, ptr(dv), ptr(d_subj), st)
         g = dv
     d_il_w = d_il_b = None
-    if il_w is not None:
-        d_il_w = _empty((w_v, w_u), meg)
-        d_il_b = _empty((w_v,), meg)
-        du = _empty((B, T, w_u), meg)
+    if il_w is not None and any(need[:4]):
+        d_il_w = _empty((w_v, w_u), meg) if n_il_w else None
+        d_il_b = _empty((w_v,), meg) if n_il_b else None
+        # du feeds the merger's and meg's gradients.  Without a merger it is kept whenever this stage runs: one GEMM onto the
+        # raw sensors, and a trainable step keeps the call stream it has always had
+        du = _empty((B, T, w_u), meg) if (n_meg or n_heads or heads is None) else None
         _reducing_call("bm_initial_linear_bwd", meg, (B, T, w_u, w_v), ptr(g), w_v, ptr(saved["u"]), w_u,
-                       ptr(il_w.reshape(w_v, w_u).contiguous()), B, T, w_u, w_v, w_u, ptr(du), ptr(d_il_w), ptr(d_il_b), st)
-        d_il_w = d_il_w.reshape(il_w.shape)
+                       ptr(il_w.reshape(w_v, w_u).contiguous()), B, T, w_u, w_v, w_u, ptr(du), ptr(d_il_w), ptr(d_il_b), st,
+                       reduces=bool(n_il_w or n_il_b))
+        if d_il_w is not None:
+            d_il_w = d_il_w.reshape(il_w.shape)
         g = du
     dheads = None
-    if heads is not None:
+    if heads is not None and n_heads:
         O, P = heads.shape
         d_att = _empty((R, O, C), meg)
         call("bm_sensor_mix_bwd", ptr(g), w_u, ptr(meg), ptr(plan.rec_order), ptr(plan.rec_off), B, C, T, O, R, ptr(d_att), st)
@@ -439,7 +467,7 @@ def _staged_front_backward(plan: "EncoderPlan", saved, g, heads, il_w, subj_w, s
         _reducing_call("bm_attention_weights_bwd", meg, None, ptr(d_att), ptr(saved["att"]), ptr(saved["emb"]), R, C, O, P,
                        ptr(dscores), ptr(dheads), st)
     dmeg = None
-    if want_dmeg:
+    if n_meg:
         # g is now the gradient at the first stage present: the mix output, or the raw sensors transposed (merger=False)
         dmeg = _empty((B, C, T), meg)
         if heads is not None:
@@ -474,9 +502,45 @@ def _sensor_mix_bwd_data(plan: "EncoderPlan", s, du, dims, status) -> torch.Tens
     return dmeg
 
 
+@dataclasses.dataclass
+class _Needs:
+    """Which gradients a backward is asked for (`ctx.needs_input_grad`, fixed at forward time), stage by stage from the input.
+    below[k]: the data gradient at the input of conv layer k is needed, i.e. `meg` or a parameter of an earlier stage
+    requires grad (below[depth]: at the input of the head)."""
+    front: tp.Tuple[bool, ...]                 # meg, heads, il_w, il_b, subj_w, sub_emb
+    head: tp.Tuple[bool, ...]                  # w0, b0, w2, b2
+    layer: tp.List[tp.Tuple[bool, ...]]        # conv_w, conv_b, gamma, beta
+    glu: tp.Dict[int, tp.Tuple[bool, ...]]     # glu_w, glu_b of the GLU block after layer k
+    below: tp.List[bool]
+
+    @staticmethod
+    def of(needs_input_grad, plan: "EncoderPlan") -> "_Needs":
+        n = [bool(v) for v in needs_input_grad]
+        depth = len(plan.dilations)
+        layer = [tuple(n[10 + 4 * k:14 + 4 * k]) for k in range(depth)]
+        glu, at = {}, 10 + 4 * depth
+        for k in range(depth):
+            if plan.glu_after[k]:
+                glu[k] = tuple(n[at:at + 2])
+                at += 2
+        front = tuple(n[1:6]) + ((n[-1],) if plan.has_sub_emb else (False,))
+        below = [any(front)]
+        for k in range(depth):
+            below.append(below[-1] or any(layer[k]) or any(glu.get(k, ())))
+        return _Needs(front=front, head=tuple(n[6:10]), layer=layer, glu=glu, below=below)
+
+    def layer_up(self, k: int) -> bool:
+        """the gradient at layer k's output (below its GLU block) is needed"""
+        return self.below[k] or any(self.layer[k])
+
+
 class _EncoderFn(torch.autograd.Function):
     """inputs: plan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, then per layer k: (conv_w, conv_b, gamma, beta)
-    and, appended in layer order, (glu_w, glu_b) for every layer followed by a GLU block."""
+    and, appended in layer order, (glu_w, glu_b) for every layer followed by a GLU block.
+
+    Only what requires grad is backpropagated: a frozen parameter's gradient is not computed, the backward stops at the
+    deepest stage that still needs a data gradient, and the forward saves only what those gradients read (nothing when no
+    tensor argument requires grad: it then issues the calls of a `torch.no_grad()` forward)."""
 
     @staticmethod
     def forward(ctx, plan: EncoderPlan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, *layer_params):
@@ -505,15 +569,21 @@ class _EncoderFn(torch.autograd.Function):
         H = conv_p[0][0].shape[0]
         F = conv_p[-1][0].shape[0] if plan.bare_last else w2.shape[1]
         rows = B * T
-        save = plan.keep_for_backward
+        nd = _Needs.of(ctx.needs_input_grad, plan)
+        save = plan.keep_for_backward and any(ctx.needs_input_grad)
+        n_meg, n_heads, n_il_w, n_il_b, n_subj, _ = nd.front
         tc = plan.use_tensor_cores
         status = tc_status_tensor(meg.device)
 
         if plan.staged:
             # sensor-side ablation rows: the chain as optional stages (see _staged_front_forward)
             x, front = _staged_front_forward(plan, meg, heads, il_w, il_b, subj_w, sub_emb, status)
+            if not n_il_w:
+                front["u"] = None                    # read by the initial_linear weight gradient only
+            if not n_subj:
+                front["v"] = None                    # read by the subject-layer weight gradient only
             D = Dp = x.shape[2]
-            conv0 = _Conv(conv_p[0][0], T, False, tc, want_bwd=save)
+            conv0 = _Conv(conv_p[0][0], T, False, tc, want_bwd=save and nd.below[0])
             emb = att = u = v = il_w2 = il_conv = subj_pad = megT = heads_conv = None
             Op = ILp = 0
         else:
@@ -542,10 +612,10 @@ class _EncoderFn(torch.autograd.Function):
                      ptr(plan.ban_centre), float(plan.ban_radius), R, C, O, P, ptr(emb), ptr(att), st)
             # K2 sensor chain; x0 is kept zero-padded to a multiple of 64 channels when the tensor-core conv follows
             Dp = _round_up(D, 64)
-            conv0 = _Conv(conv_p[0][0], T, False, tc, pad_cin_to=Dp, want_bwd=save)
+            conv0 = _Conv(conv_p[0][0], T, False, tc, pad_cin_to=Dp, want_bwd=save and nd.below[0])
             if not conv0.fwd_tc:
                 Dp = D
-                conv0 = _Conv(conv_p[0][0], T, False, False, want_bwd=save)
+                conv0 = _Conv(conv_p[0][0], T, False, False, want_bwd=save and nd.below[0])
             il_w2 = il_w.reshape(IL, O).contiguous()
             # `initial_linear` on the tensor cores when the (64-padded) widths fit: u and v are then kept zero-padded
             Op, ILp = _round_up(O, 64), _round_up(IL, 64)
@@ -553,7 +623,7 @@ class _EncoderFn(torch.autograd.Function):
             if tc:
                 wpad = torch.zeros((ILp, Op, 1), device=meg.device)
                 wpad[:IL, :O, 0] = il_w2
-                il_conv = _Conv(wpad, T, False, True, want_bwd=save)
+                il_conv = _Conv(wpad, T, False, True, want_bwd=save and (n_meg or n_heads))
                 if not (il_conv.fwd_tc and il_conv.bwd_tc and il_conv.wgrad_tc):
                     il_conv = None
             # u [B,T,Op] and x [B,T,Dp] carry zero pad columns.  The tensor-core contractions write every column (their padded
@@ -619,9 +689,10 @@ class _EncoderFn(torch.autograd.Function):
         x_amax = None                                   # device float with max |x| when x's producer reported it (F16 pipe)
         for k in range(depth):
             cw, cb, gamma, beta = conv_p[k]
-            conv = conv0 if k == 0 else _Conv(cw, T, False, tc, want_bwd=save)
+            conv = conv0 if k == 0 else _Conv(cw, T, False, tc, want_bwd=save and nd.below[k])
             cout = conv.cout
             y = _empty((B, T, cout), meg)
+            keep = save and nd.below[k + 1]          # the backward reaches this layer
             if plan.bare_last and k == depth - 1:
                 conv.forward(x, cb.contiguous(), B, T, plan.dilations[k], y, None, status, x_amax=x_amax)
                 x_amax = None
@@ -630,17 +701,18 @@ class _EncoderFn(torch.autograd.Function):
                 if skip:
                     x_new = _empty((B, T, cout), meg)
                     call("bm_bn_act_skip_fwd", ptr(y), None, None, None, None, ptr(x), ptr(x_new), rows, cout, 2, 0.0, st)
-                rec = dict(x_in=x, y=y, mean=None, invstd=None, conv=conv, skip=skip, x_new=x_new, bare=True)
+                rec = dict(x_in=x if nd.layer[k][0] else None, mean=None, invstd=None, conv=conv, skip=skip,
+                           x_new=x_new if nd.glu.get(k, (False,))[0] else None, bare=True)
                 x = x_new
                 if plan.glu_after[k]:
                     gw, gb = glu_p[k]
-                    gconv = _Conv(gw, T, True, tc, want_bwd=save)
-                    h = _empty((B, T, gconv.cout), meg) if save else None
+                    gconv = _Conv(gw, T, True, tc, want_bwd=save and nd.layer_up(k))
+                    h = _empty((B, T, gconv.cout), meg) if keep else None
                     out = _empty((B, T, gconv.cout // 2), meg)
                     x_amax = gconv.forward_glu(x, gb.contiguous(), B, T, h, out, status, x_amax=x_amax, out_amax=amax_cell(meg))
                     rec.update(h=h, gconv=gconv)
                     x = out
-                saved_layers.append(rec if save else None)
+                saved_layers.append(rec if keep else None)
                 continue
             mean = _empty((cout,), meg)
             invstd = _empty((cout,), meg)
@@ -663,18 +735,20 @@ class _EncoderFn(torch.autograd.Function):
                 call("bm_bn_act_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma.contiguous()),
                      ptr(beta.contiguous()), ptr(x) if skip else None, ptr(x_new), rows, cout, plan.act_code,
                      float(plan.act_slope), st)
-            rec = dict(x_in=x, y=y, mean=mean, invstd=invstd, conv=conv, skip=skip, x_new=x_new, x_in_amax=x_in_amax,
+            # kept: the conv input for its weight gradient, y for the BatchNorm backward, x_new for the GLU weight gradient
+            rec = dict(x_in=x if nd.layer[k][0] else None, y=y if nd.layer_up(k) else None, mean=mean, invstd=invstd,
+                       conv=conv, skip=skip, x_new=x_new if nd.glu.get(k, (False,))[0] else None, x_in_amax=x_in_amax,
                        x_new_amax=x_amax)
             x = x_new
             if plan.glu_after[k]:
                 gw, gb = glu_p[k]
-                gconv = _Conv(gw, T, True, tc, want_bwd=save)
-                h = _empty((B, T, gconv.cout), meg) if save else None
+                gconv = _Conv(gw, T, True, tc, want_bwd=save and nd.layer_up(k))
+                h = _empty((B, T, gconv.cout), meg) if keep else None
                 out = _empty((B, T, gconv.cout // 2), meg)
                 x_amax = gconv.forward_glu(x, gb.contiguous(), B, T, h, out, status, x_amax=x_amax, out_amax=amax_cell(meg))
                 rec.update(h=h, gconv=gconv)
                 x = out
-            saved_layers.append(rec if save else None)
+            saved_layers.append(rec if keep else None)
 
         if plan.bare_last:
             # no head: the sequence already ends on out_channels; hand it out channel-major
@@ -682,9 +756,11 @@ class _EncoderFn(torch.autograd.Function):
             call("bm_transpose_nt", ptr(x), B, T, F, ptr(est), st)
             if save:
                 ctx.plan = plan
+                ctx.needs = nd
                 ctx.dims = (B, C, T, R, O, P, IL, S, D, Dp, H, F)
                 ctx.pads = (Op, ILp)
-                ctx.saved = dict(meg=meg, emb=emb, att=att, u=u, v=v, il_w2=il_w2, subj_w=None if subj_w is None else subj_w.contiguous(),
+                ctx.saved = dict(meg=meg, emb=emb, att=att, u=u if n_il_w else None, v=v if n_subj else None, il_w2=il_w2,
+                                 subj_w=None if subj_w is None else subj_w.contiguous(),
                                  il_conv=il_conv, subj_pad=subj_pad, megT=megT, heads_tc=heads_conv is not None,
                                  layers=saved_layers, conv_p=conv_p, glu_p=glu_p,
                                  il_shape=None if il_w is None else il_w.shape, front=front,
@@ -693,9 +769,10 @@ class _EncoderFn(torch.autograd.Function):
 
         # K5 head
         H2 = 2 * H
-        head0 = _Conv(w0, T, False, tc, want_bwd=save)                       # [2H, H, 1]
+        want_dh1 = nd.below[depth] or nd.head[0] or nd.head[1]               # the gradient below the head's GELU
+        head0 = _Conv(w0, T, False, tc, want_bwd=save and nd.below[depth])   # [2H, H, 1]
         w2_as_conv = w2.permute(1, 0, 2).contiguous()                        # ConvTranspose1d [2H,F,1] -> [F,2H,1]
-        head2 = _Conv(w2_as_conv, T, False, tc, want_bwd=save)
+        head2 = _Conv(w2_as_conv, T, False, tc, want_bwd=save and want_dh1)
         head_tc = head0.fwd_tc and head2.fwd_tc and head0.bwd_tc and head2.bwd_tc
         h1 = _empty((B, T, H2), meg)
         q = _empty((B, T, H2), meg)
@@ -725,11 +802,14 @@ class _EncoderFn(torch.autograd.Function):
 
         if save:
             ctx.plan = plan
+            ctx.needs = nd
             ctx.dims = (B, C, T, R, O, P, IL, S, D, Dp, H, F)
             ctx.pads = (Op, ILp)
-            ctx.saved = dict(meg=meg, emb=emb, att=att, u=u, v=v, il_w2=il_w2, subj_w=None if subj_w is None else subj_w.contiguous(), il_conv=il_conv,
+            ctx.saved = dict(meg=meg, emb=emb, att=att, u=u if n_il_w else None, v=v if n_subj else None, il_w2=il_w2,
+                             subj_w=None if subj_w is None else subj_w.contiguous(), il_conv=il_conv,
                              subj_pad=subj_pad, megT=megT, heads_tc=heads_conv is not None,
-                             layers=saved_layers, x_last=x, w0_2=w0_2, w2_2=w2_2, h1=h1, q=q, q_amax=q_amax,
+                             layers=saved_layers, x_last=x if nd.head[0] else None, w0_2=w0_2, w2_2=w2_2,
+                             h1=h1, q=q if nd.head[2] else None, q_amax=q_amax,
                              head0=head0, head2=head2, head_tc=head_tc, head_generic=head_generic,
                              conv_p=conv_p, glu_p=glu_p, il_shape=None if il_w is None else il_w.shape,
                              w0_shape=w0.shape, w2_shape=w2.shape, front=front, params=(heads, il_w, subj_w, sub_emb))
@@ -752,6 +832,11 @@ class _EncoderFn(torch.autograd.Function):
         dest = dest.contiguous()
         status = tc_status_tensor(meg.device)
 
+        nd: _Needs = ctx.needs
+        n_w0, n_b0, n_w2, n_b2 = nd.head
+        want_g = nd.below[depth]                # the gradient at the head's input (the sequence's output)
+        want_dh1 = want_g or n_w0 or n_b0       # the gradient below the head's GELU
+
         ctx_keep: tp.List[tp.Any] = []          # operands of side-stream kernels, released after the streams join
         # ---- head ----
         if plan.bare_last:
@@ -759,36 +844,50 @@ class _EncoderFn(torch.autograd.Function):
             call("bm_transpose_nt", ptr(dest), B, F, T, ptr(g), st)
             dw0 = db0 = dw2 = db2 = dq = None
         else:
-            g = _empty((B, T, H), meg)
-            dw0 = _empty((H2, H), meg)
-            db0 = _empty((H2,), meg)
-            dw2 = _empty((H2, F), meg)
-            db2 = _empty((F,), meg)
-            dq = _empty((B, T, H2), meg)
+            g = _empty((B, T, H), meg) if want_g else None
+            dw0 = _empty((H2, H), meg) if n_w0 else None
+            db0 = _empty((H2,), meg) if n_b0 else None
+            dw2 = _empty((H2, F), meg) if n_w2 else None
+            db2 = _empty((F,), meg) if n_b2 else None
+            dq = _empty((B, T, H2), meg) if want_dh1 else None
         if plan.bare_last:
             pass
         elif s["head_generic"]:
             head0, head2 = s["head0"], s["head2"]
             dest_t = _empty((B, T, F), meg)
             call("bm_transpose_nt", ptr(dest), B, F, T, ptr(dest_t), st)
-            head2.backward_data(dest_t, None, B, T, 1, dq, status)                 # dq = dest_t @ w2^T
-            dw2c, db2 = head2.backward_weight(dest_t, s["q"], B, T, 1, meg, status)    # [F, 2H, 1]
-            dw2 = dw2c.permute(1, 0, 2).reshape(H2, F).contiguous()
-            dh1 = _empty((B, T, H2), meg)
-            call("bm_bn_act_skip_bwd", ptr(dq), ptr(s["h1"]), None, None, None, None, 0, rows, H2, plan.act_code,
-                 float(plan.act_slope), None, ptr(dh1), None, None, st)
-            dw0, db0 = head0.backward_weight(dh1, s["x_last"], B, T, 1, meg, status)   # [2H, H, 1]
-            head0.backward_data(dh1, None, B, T, 1, g, status)
-            del dest_t, dh1
+            if want_dh1:
+                head2.backward_data(dest_t, None, B, T, 1, dq, status)             # dq = dest_t @ w2^T
+            dw2c, db2 = head2.backward_weight(dest_t, s["q"], B, T, 1, meg, status, want_w=n_w2, want_b=n_b2)  # [F, 2H, 1]
+            dw2 = None if dw2c is None else dw2c.permute(1, 0, 2).reshape(H2, F).contiguous()
+            if want_dh1:
+                dh1 = _empty((B, T, H2), meg)
+                call("bm_bn_act_skip_bwd", ptr(dq), ptr(s["h1"]), None, None, None, None, 0, rows, H2, plan.act_code,
+                     float(plan.act_slope), None, ptr(dh1), None, None, st)
+                dw0, db0 = head0.backward_weight(dh1, s["x_last"], B, T, 1, meg, status, want_w=n_w0, want_b=n_b0)  # [2H,H,1]
+                if want_g:
+                    head0.backward_data(dh1, None, B, T, 1, g, status)
+                del dh1
+            del dest_t
         elif s["head_tc"]:
             head0, head2 = s["head0"], s["head2"]
             dest_t = _empty((B, T, F), meg)
             call("bm_transpose_nt", ptr(dest), B, F, T, ptr(dest_t), st)
             # dq = dest_t @ w2^T  (w2_as_conv [F,2H,1]: its data-gradient operand is [1][2H][F])
             dest_amax = tensor_amax(dest_t) if USE_CONV_F16 else None      # one pass serves the dgrad and the wgrad below
-            head2.run_tc(False, dest_t, None, None, B, T, 1, 0, 0, 0, dq, None, None, None, status, x_amax=dest_amax)
             lib = _lib.load()
-            if lib.bm_tc_wgrad_supported(H2, F) and lib.bm_tc_wgrad_supported(H2, H):
+            wgrad_tc = lib.bm_tc_wgrad_supported(H2, F) and lib.bm_tc_wgrad_supported(H2, H)
+            if dq is None and not wgrad_tc and (n_w2 or n_b2):
+                dq = _empty((B, T, H2), meg)                               # bm_head_bwd_params turns dq into dh1 in any case
+            if dq is not None:
+                head2.run_tc(False, dest_t, None, None, B, T, 1, 0, 0, 0, dq, None, None, None, status, x_amax=dest_amax)
+            if not wgrad_tc:
+                if dw0 is not None or db0 is not None or dw2 is not None or db2 is not None:
+                    _reducing_call("bm_head_bwd_params", meg, (B, T, H, F), ptr(dest), ptr(s["x_last"]), ptr(s["h1"]),
+                                   ptr(s["q"]), B, T, H, F, ptr(dq), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st)
+                elif want_g:
+                    call("bm_gelu_bwd", ptr(dq), ptr(s["h1"]), rows * H2, ptr(dq), st)       # dq <- dh1
+            else:
                 main0 = torch.cuda.current_stream()
                 side0 = _side_stream(meg.device) if OVERLAP_WGRAD else None
 
@@ -804,67 +903,87 @@ class _EncoderFn(torch.autograd.Function):
                     return out
 
                 # dW2 / db2 only need dest_t and q: they overlap the dq contraction queued just before
-                dw2 = on_side(lambda: tc_wgrad(s["q"], dest_t, B, T, H2, F, F, 1, 1, status, dy_amax=s.get("q_amax"),
-                                               x_amax=dest_amax), s["q"], dest_t, dest_amax).reshape(H2, F)
-                col_sum(dest_t, rows, F, db2, st)
-                call("bm_gelu_bwd", ptr(dq), ptr(s["h1"]), rows * H2, ptr(dq), st)           # dq <- dh1
-                dw0 = on_side(lambda: tc_wgrad(dq, s["x_last"], B, T, H2, H, H, 1, 1, status, dbias=db0), dq,
-                              s["x_last"], db0).reshape(H2, H)
-            else:
-                _reducing_call("bm_head_bwd_params", meg, (B, T, H, F), ptr(dest), ptr(s["x_last"]), ptr(s["h1"]), ptr(s["q"]),
-                               B, T, H, F, ptr(dq), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st)   # dq <- dq*GELU'(h1); dW0..db2
-            head0.run_tc(False, dq, None, None, B, T, 1, 0, 0, 0, g, None, None, None, status)
+                if n_w2:
+                    dw2 = on_side(lambda: tc_wgrad(s["q"], dest_t, B, T, H2, F, F, 1, 1, status, dy_amax=s.get("q_amax"),
+                                                   x_amax=dest_amax), s["q"], dest_t, dest_amax).reshape(H2, F)
+                if n_b2:
+                    col_sum(dest_t, rows, F, db2, st)
+                if want_dh1:
+                    call("bm_gelu_bwd", ptr(dq), ptr(s["h1"]), rows * H2, ptr(dq), st)       # dq <- dh1
+                if n_w0:
+                    dw0 = on_side(lambda: tc_wgrad(dq, s["x_last"], B, T, H2, H, H, 1, 1, status, dbias=db0), dq,
+                                  s["x_last"], db0).reshape(H2, H)
+                elif n_b0:
+                    col_sum(dq, rows, H2, db0, st)
+            if want_g:
+                head0.run_tc(False, dq, None, None, B, T, 1, 0, 0, 0, g, None, None, None, status)
             del dest_t
         else:
             _reducing_call("bm_head_bwd", meg, (B, T, H, F), ptr(dest), ptr(s["x_last"]), ptr(s["w0_2"]), ptr(s["w2_2"]),
-                           ptr(s["h1"]), ptr(s["q"]), B, T, H, F, ptr(dq), ptr(g), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st)
+                           ptr(s["h1"]), ptr(s["q"]), B, T, H, F, ptr(dq), ptr(g), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st,
+                           reduces=any(nd.head))
         del dq
 
         sums = _empty((2 * H,), meg, torch.float64)
-        layer_grads: tp.List[tp.Any] = [None] * depth
-        glu_grads = {}
+        layer_grads: tp.List[tp.Any] = [(None, None, None, None)] * depth
+        glu_grads = {k: (None, None) for k in nd.glu}
         # The weight gradient and the data gradient of a layer are independent given dy: the weight-gradient kernels go to
-        # a side stream so that their CTAs fill the SMs left idle by the partial last wave of the data-gradient kernel.
+        # a side stream so that their CTAs fill the SMs left idle by the partial last wave of the data-gradient kernel
+        # (when there is a weight gradient to overlap at all).
+        any_wgrad = any(any(n[:2]) for n in nd.layer) or any(any(n) for n in nd.glu.values())
         main = torch.cuda.current_stream()
-        side = _side_stream(meg.device) if (OVERLAP_WGRAD and plan.use_tensor_cores) else None
+        side = _side_stream(meg.device) if (OVERLAP_WGRAD and plan.use_tensor_cores and any_wgrad) else None
         keep_alive: tp.List[tp.Any] = ctx_keep
 
-        def weight_grad(conv_obj, dy_t, x_t, dil, bias_zero, known_dbias=None, dy_amax=None, x_amax=None):
+        def weight_grad(conv_obj, dy_t, x_t, dil, bias_zero, known_dbias=None, dy_amax=None, x_amax=None, want=(True, True)):
+            if not any(want):
+                return None, None
+            kw = dict(bias_grad_is_zero=bias_zero, known_dbias=known_dbias, dy_amax=dy_amax, x_amax=x_amax, want_w=want[0],
+                      want_b=want[1])
             if side is None:
-                return conv_obj.backward_weight(dy_t, x_t, B, T, dil, meg, status, bias_grad_is_zero=bias_zero,
-                                                known_dbias=known_dbias, dy_amax=dy_amax, x_amax=x_amax)
+                return conv_obj.backward_weight(dy_t, x_t, B, T, dil, meg, status, **kw)
             side.wait_stream(main)
             with torch.cuda.stream(side):
-                out = conv_obj.backward_weight(dy_t, x_t, B, T, dil, meg, status, bias_grad_is_zero=bias_zero,
-                                               known_dbias=known_dbias, dy_amax=dy_amax, x_amax=x_amax)
+                out = conv_obj.backward_weight(dy_t, x_t, B, T, dil, meg, status, **kw)
             # the big operands are kept alive until the streams join (no record_stream: with the host running steps ahead
             # it would block the allocator from reusing ~3 GB of blocks and force cudaMallocs in the timed loop)
             keep_alive.append((dy_t, x_t, dy_amax, x_amax))
             for o in out:
-                o.record_stream(main)
+                if o is not None:
+                    o.record_stream(main)
             return out
 
         for k in reversed(range(depth)):
+            if not nd.below[k + 1]:
+                break                                  # nothing at or below this layer requires grad
             rec = s["layers"][k]
             cw, cb, gamma, beta = s["conv_p"][k]
             conv: _Conv = rec["conv"]
             cout = conv.cout
+            n_cw, n_cb, n_gamma, n_beta = nd.layer[k]
             if plan.glu_after[k]:
                 gconv: _Conv = rec["gconv"]
+                n_gw, n_gb = nd.glu[k]
                 dh = _empty((B, T, gconv.cout), meg)
-                dgb = _empty((gconv.cout,), meg)          # the GLU conv's bias gradient, summed while dh is produced
+                dgb = _empty((gconv.cout,), meg) if n_gb else None    # the GLU conv's bias gradient, summed while dh is made
                 dh_amax = amax_cell(meg)
                 _reducing_call("bm_glu_bwd", meg, (rows, gconv.cout // 2), ptr(g), ptr(rec["h"]), rows, gconv.cout // 2, ptr(dh),
-                               ptr(dgb), ptr(dh_amax), st)
-                glu_grads[k] = weight_grad(gconv, dh, rec["x_new"], 1, False, dgb, dy_amax=dh_amax, x_amax=rec.get("x_new_amax"))
+                               ptr(dgb), ptr(dh_amax), st, reduces=n_gb)
+                glu_grads[k] = weight_grad(gconv, dh, rec["x_new"], 1, False, dgb, dy_amax=dh_amax, x_amax=rec.get("x_new_amax"),
+                                           want=(n_gw, n_gb))
+                if not nd.layer_up(k):
+                    del dh
+                    break
                 g = _empty((B, T, gconv.cin), meg)
                 gconv.backward_data(dh, None, B, T, 1, g, status, dy_amax=dh_amax)
                 del dh
             if rec.get("bare"):
                 # bare convolution (+ residual): dL/dy = dL/dx_new; no BatchNorm behind it, so the bias gradient is real
-                dy = g.clone() if rec["skip"] else g
-                dcw, dcb = weight_grad(conv, dy, rec["x_in"], plan.dilations[k], False)
-                if rec["skip"]:
+                dy = g.clone() if (rec["skip"] and nd.below[k]) else g
+                dcw, dcb = weight_grad(conv, dy, rec["x_in"], plan.dilations[k], False, want=(n_cw, n_cb))
+                if not nd.below[k]:
+                    pass
+                elif rec["skip"]:
                     conv.backward_data(dy, g, B, T, plan.dilations[k], g, status)
                 else:
                     g_in = _empty((B, T, conv.cin), meg)
@@ -873,70 +992,94 @@ class _EncoderFn(torch.autograd.Function):
                 layer_grads[k] = (dcw, dcb, None, None)
                 del dy
                 continue
+            # the batch statistics' backward reduces in training mode; in eval mode only for trainable gamma / beta (else the
+            # BatchNorm + activation backward is one elementwise pass)
+            reduce = plan.training or n_gamma or n_beta
             dy = _empty((B, T, cout), meg)
-            dgamma = _empty((cout,), meg)
-            dbeta = _empty((cout,), meg)
+            dgamma = _empty((cout,), meg) if reduce else None
+            dbeta = _empty((cout,), meg) if reduce else None
             dy_amax = None
             if plan.act_code == 0:
                 dy_amax = amax_cell(meg)
                 _reducing_call("bm_bn_gelu_skip_bwd", meg, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
                                ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()), 1 if plan.training else 0,
-                               rows, cout, ptr(sums), ptr(dy), ptr(dgamma), ptr(dbeta), ptr(dy_amax), st)
+                               rows, cout, ptr(sums if reduce else None), ptr(dy), ptr(dgamma), ptr(dbeta), ptr(dy_amax), st,
+                               reduces=reduce)
             else:
                 _reducing_call("bm_bn_act_skip_bwd", meg, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
                                ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()), 1 if plan.training else 0,
-                               rows, cout, plan.act_code, float(plan.act_slope), ptr(sums), ptr(dy), ptr(dgamma), ptr(dbeta),
-                               st)
+                               rows, cout, plan.act_code, float(plan.act_slope), ptr(sums if reduce else None), ptr(dy),
+                               ptr(dgamma), ptr(dbeta), st, reduces=reduce)
             dcw, dcb = weight_grad(conv, dy, rec["x_in"], plan.dilations[k], plan.training, dy_amax=dy_amax,
-                                   x_amax=rec.get("x_in_amax"))
-            if rec["skip"]:
+                                   x_amax=rec.get("x_in_amax"), want=(n_cw, n_cb))
+            if not nd.below[k]:
+                pass
+            elif rec["skip"]:
                 # in place: g += conv_transpose(dy) (addend == output: the pair kernel turns this into a TMA reduce-add)
                 conv.backward_data(dy, g, B, T, plan.dilations[k], g, status, dy_amax=dy_amax)
             else:
                 g_in = _empty((B, T, conv.cin), meg)
                 conv.backward_data(dy, None, B, T, plan.dilations[k], g_in, status, dy_amax=dy_amax)
                 g = g_in
-            layer_grads[k] = (dcw, dcb, dgamma, dbeta)
+            layer_grads[k] = (dcw, dcb, dgamma if n_gamma else None, dbeta if n_beta else None)
             del dy
 
         if side is not None:
             main.wait_stream(side)
         keep_alive.clear()
-        if plan.staged:
+        n_meg, n_heads, n_il_w, n_il_b, n_subj, _ = nd.front
+        dheads = d_il_w = d_il_b = d_subj = d_sub_emb = dmeg = None
+        if not nd.below[0]:
+            pass                                       # the sensor side is frozen and meg does not require grad
+        elif plan.staged:
             heads_p, il_w_p, subj_w_p, sub_emb_p = s["params"]
             dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg = _staged_front_backward(
-                plan, s["front"], g, heads_p, il_w_p, subj_w_p, sub_emb_p, want_dmeg=ctx.needs_input_grad[1])
+                plan, s["front"], g, heads_p, il_w_p, subj_w_p, sub_emb_p, nd.front)
         else:
-            d_sub_emb = None
-            # ---- sensor chain + attention ----
-            subj_order, subj_off = group_layout(plan.subject, S)
+            # ---- sensor chain + attention: each stage as far as a gradient below it is asked for ----
+            want_dv = n_meg or n_heads or n_il_w or n_il_b          # the gradient at the subject layer's input
+            want_du = n_meg or n_heads                              # ... and at initial_linear's input
+            subj_order, subj_off = group_layout(plan.subject, S) if n_subj else (None, None)
             Op, ILp = ctx.pads
-            d_subj = _empty((S, IL, D), meg)
-            d_att = _empty((R, O, C), meg)
+            d_att = _empty((R, O, C), meg) if n_heads else None
+            du = None
             il_conv = s["il_conv"]
             if il_conv is not None:
+                dv = None
                 if s["subj_pad"] is not None:
-                    subj_pad = s["subj_pad"]                                   # [S][ILp][Dp]: data-gradient operand as is
-                    sb_hi, sb_lo = _empty((S * ILp, Dp), meg), _empty((S * ILp, Dp), meg)
-                    call("bm_tc_weight_split", ptr(subj_pad), S * ILp, Dp, 1, ptr(sb_hi), ptr(sb_lo), None, None, st)
-                    dv = _empty((B, T, ILp), meg)
-                    call("bm_tc_pointwise_sel", ptr(g), ptr(sb_hi), ptr(sb_lo), ptr(plan.subject), S, B, T, Dp, ILp, ptr(dv),
-                         ptr(status), st)
-                    mpad = _round_up(ILp, 128)
-                    dm = _empty((S, mpad, Dp), meg)
-                    call("bm_tc_wgrad_grouped", ptr(s["v"]), ptr(g), ptr(subj_order), ptr(subj_off), S, B, T, ILp, Dp,
-                         ptr(dm), ptr(status), st)
-                    d_subj = dm[:, :IL, :D].contiguous()
+                    if want_dv:
+                        subj_pad = s["subj_pad"]                               # [S][ILp][Dp]: data-gradient operand as is
+                        sb_hi, sb_lo = _empty((S * ILp, Dp), meg), _empty((S * ILp, Dp), meg)
+                        call("bm_tc_weight_split", ptr(subj_pad), S * ILp, Dp, 1, ptr(sb_hi), ptr(sb_lo), None, None, st)
+                        dv = _empty((B, T, ILp), meg)
+                        call("bm_tc_pointwise_sel", ptr(g), ptr(sb_hi), ptr(sb_lo), ptr(plan.subject), S, B, T, Dp, ILp,
+                             ptr(dv), ptr(status), st)
+                    if n_subj:
+                        mpad = _round_up(ILp, 128)
+                        dm = _empty((S, mpad, Dp), meg)
+                        call("bm_tc_wgrad_grouped", ptr(s["v"]), ptr(g), ptr(subj_order), ptr(subj_off), S, B, T, ILp, Dp,
+                             ptr(dm), ptr(status), st)
+                        d_subj = dm[:, :IL, :D].contiguous()
                 else:
-                    dv = torch.zeros((B, T, ILp), device=meg.device) if ILp != IL else _empty((B, T, IL), meg)
+                    if want_dv:
+                        dv = torch.zeros((B, T, ILp), device=meg.device) if ILp != IL else _empty((B, T, IL), meg)
+                    d_subj = _empty((S, IL, D), meg) if n_subj else None
                     call("bm_subject_layers_bwd", ptr(g), Dp, ptr(s["v"]), ILp, ptr(s["subj_w"]), ptr(plan.subject),
                          ptr(subj_order), ptr(subj_off), B, T, IL, D, S, ILp, ptr(dv), ptr(d_subj), st)
-                du = _empty((B, T, Op), meg)
-                il_conv.backward_data(dv, None, B, T, 1, du, status)
-                dbp = _empty((ILp,), meg)
-                d_il_w = tc_wgrad(dv, s["u"], B, T, ILp, Op, O, 1, 1, status, dbias=dbp)[:IL, :, 0].contiguous()
-                d_il_b = dbp[:IL].contiguous()
-                if s["megT"] is not None:
+                if want_du:
+                    du = _empty((B, T, Op), meg)
+                    il_conv.backward_data(dv, None, B, T, 1, du, status)
+                if n_il_w:
+                    dbp = _empty((ILp,), meg) if n_il_b else None
+                    d_il_w = tc_wgrad(dv, s["u"], B, T, ILp, Op, O, 1, 1, status, dbias=dbp)[:IL, :, 0].contiguous()
+                    d_il_b = dbp[:IL].contiguous() if n_il_b else None
+                elif n_il_b:
+                    dbp = _empty((ILp,), meg)
+                    col_sum(dv, rows, ILp, dbp, st)
+                    d_il_b = dbp[:IL].contiguous()
+                if not n_heads:
+                    pass
+                elif s["megT"] is not None:
                     megT = s["megT"]
                     Cp = megT.shape[2]
                     dwp = _empty((R, _round_up(Op, 128), Cp), meg)
@@ -947,23 +1090,27 @@ class _EncoderFn(torch.autograd.Function):
                     call("bm_sensor_mix_bwd", ptr(du), Op, ptr(meg), ptr(plan.rec_order), ptr(plan.rec_off), B, C, T, O, R,
                          ptr(d_att), st)
             else:
-                dv = _empty((B, T, IL), meg)
-                du = _empty((B, T, O), meg)
-                d_il_w = _empty((IL, O), meg)
-                d_il_b = _empty((IL,), meg)
+                dv = _empty((B, T, IL), meg) if want_dv else None
+                du = _empty((B, T, O), meg) if want_du else None
+                d_subj = _empty((S, IL, D), meg) if n_subj else None
+                d_il_w = _empty((IL, O), meg) if n_il_w else None
+                d_il_b = _empty((IL,), meg) if n_il_b else None
                 _reducing_call("bm_sensor_chain_bwd", meg, (B, T, O, IL), ptr(g), ptr(meg), ptr(s["il_w2"]), ptr(s["subj_w"]),
                                ptr(plan.subject), ptr(s["u"]), ptr(s["v"]), ptr(subj_order), ptr(subj_off), ptr(plan.rec_order),
                                ptr(plan.rec_off), B, C, T, O, IL, D, Dp, S, R, ptr(dv), ptr(du), ptr(d_subj), ptr(d_il_w),
-                               ptr(d_il_b), ptr(d_att), st)
-            dmeg = _sensor_mix_bwd_data(plan, s, du, ctx.dims, status) if ctx.needs_input_grad[1] else None
-            dscores = _empty((R, O, C), meg)
-            if s["heads_tc"]:
+                               ptr(d_il_b), ptr(d_att), st, reduces=n_il_w or n_il_b)
+            dmeg = _sensor_mix_bwd_data(plan, s, du, ctx.dims, status) if n_meg else None
+            if not n_heads:
+                pass
+            elif s["heads_tc"]:
+                dscores = _empty((R, O, C), meg)
                 Opad = _round_up(O, 64)
                 call("bm_softmax_bwd", ptr(s["att"]), ptr(d_att), R * O, C, ptr(dscores), st)
                 ds_t = _empty((R, C, Opad), meg)                   # pad columns zeroed by the transpose
                 call("bm_transpose_nt_ld", ptr(dscores), R, O, C, Opad, ptr(ds_t), st)
                 dheads = tc_wgrad(ds_t, s["emb"], R, C, Opad, P, P, 1, 1, status)[:O, :, 0].contiguous()
             else:
+                dscores = _empty((R, O, C), meg)
                 dheads = _empty((O, P), meg)
                 _reducing_call("bm_attention_weights_bwd", meg, None, ptr(d_att), ptr(s["att"]), ptr(s["emb"]), R, C, O, P,
                                ptr(dscores), ptr(dheads), st)
@@ -973,8 +1120,8 @@ class _EncoderFn(torch.autograd.Function):
         if plan.bare_last:
             grads = [None, dmeg, dheads, d_il_w, d_il_b, d_subj, None, None, None, None]
         else:
-            grads = [None, dmeg, dheads, d_il_w, d_il_b, d_subj,
-                     dw0.reshape(s["w0_shape"]), db0, dw2.reshape(s["w2_shape"]), db2]
+            grads = [None, dmeg, dheads, d_il_w, d_il_b, d_subj, None if dw0 is None else dw0.reshape(s["w0_shape"]), db0,
+                     None if dw2 is None else dw2.reshape(s["w2_shape"]), db2]
         for k in range(depth):
             grads.extend(layer_grads[k])
         for k in range(depth):
@@ -1178,7 +1325,8 @@ class _MergerFn(torch.autograd.Function):
         call("bm_sensor_mix_fwd", ptr(meg), ptr(att), ptr(rec_of_sample), B, C, T, O, O, ptr(u), st)
         out = _empty((B, O, T), meg)
         call("bm_transpose_nt", ptr(u), B, T, O, ptr(out), st)
-        ctx.save_for_backward(meg, emb, att, rec_of_sample, rec_order, rec_off)
+        if any(ctx.needs_input_grad):                  # else nothing is kept: there will be no backward
+            ctx.save_for_backward(meg, emb, att, rec_of_sample, rec_order, rec_off)
         ctx.dims = (B, C, T, R, O, P)
         return out
 
@@ -1190,10 +1338,12 @@ class _MergerFn(torch.autograd.Function):
         st = stream()
         g = _empty((B, T, O), meg)
         call("bm_transpose_nt", ptr(gout.contiguous()), B, O, T, ptr(g), st)
-        d_att, dscores, dheads = _empty((R, O, C), meg), _empty((R, O, C), meg), _empty((O, P), meg)
-        call("bm_sensor_mix_bwd", ptr(g), O, ptr(meg), ptr(rec_order), ptr(rec_off), B, C, T, O, R, ptr(d_att), st)
-        _reducing_call("bm_attention_weights_bwd", meg, None, ptr(d_att), ptr(att), ptr(emb), R, C, O, P, ptr(dscores),
-                       ptr(dheads), st)
+        dheads = None
+        if ctx.needs_input_grad[1]:                    # frozen heads: no mix or attention gradient
+            d_att, dscores, dheads = _empty((R, O, C), meg), _empty((R, O, C), meg), _empty((O, P), meg)
+            call("bm_sensor_mix_bwd", ptr(g), O, ptr(meg), ptr(rec_order), ptr(rec_off), B, C, T, O, R, ptr(d_att), st)
+            _reducing_call("bm_attention_weights_bwd", meg, None, ptr(d_att), ptr(att), ptr(emb), R, C, O, P, ptr(dscores),
+                           ptr(dheads), st)
         dmeg = None
         if ctx.needs_input_grad[0]:
             dmeg = _empty((B, C, T), meg)
@@ -1219,7 +1369,9 @@ class _SubjectLayersFn(torch.autograd.Function):
         call("bm_subject_layers_fwd", ptr(xl), Cin, ptr(w), ptr(subject), B, T, Cin, D, D, ptr(yl), st)
         out = _empty((B, D, T), x)
         call("bm_transpose_nt", ptr(yl), B, T, D, ptr(out), st)
-        ctx.save_for_backward(xl, w, subject)
+        if any(ctx.needs_input_grad):                  # else nothing is kept: there will be no backward
+            # x for the weight gradient, the weights for the data gradient
+            ctx.save_for_backward(xl if ctx.needs_input_grad[1] else None, w if ctx.needs_input_grad[0] else None, subject)
         ctx.dims = (B, Cin, T, S, D)
         return out
 
@@ -1228,15 +1380,19 @@ class _SubjectLayersFn(torch.autograd.Function):
     def backward(ctx, gout):
         xl, w, subject = ctx.saved_tensors
         B, Cin, T, S, D = ctx.dims
+        want_dx, want_dw = ctx.needs_input_grad[:2]
         st = stream()
-        g = _empty((B, T, D), xl)
+        g = _empty((B, T, D), gout)
         call("bm_transpose_nt", ptr(gout.contiguous()), B, D, T, ptr(g), st)
-        order, off = group_layout(subject, S)
-        dxl, dw = _empty((B, T, Cin), xl), _empty((S, Cin, D), xl)
+        order, off = group_layout(subject, S) if want_dw else (None, None)
+        dxl = _empty((B, T, Cin), g) if want_dx else None
+        dw = _empty((S, Cin, D), g) if want_dw else None
         call("bm_subject_layers_bwd", ptr(g), D, ptr(xl), Cin, ptr(w), ptr(subject), ptr(order), ptr(off), B, T, Cin, D, S,
              Cin, ptr(dxl), ptr(dw), st)
-        dx = _empty((B, Cin, T), xl)
-        call("bm_transpose_nt", ptr(dxl), B, T, Cin, ptr(dx), st)
+        dx = None
+        if want_dx:
+            dx = _empty((B, Cin, T), g)
+            call("bm_transpose_nt", ptr(dxl), B, T, Cin, ptr(dx), st)
         return dx, dw, None
 
 

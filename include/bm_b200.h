@@ -66,7 +66,10 @@ int bm_sensor_chain_fwd(const float* meg, const float* weights, const int* rec_o
                         int IL, int D, int ld_x0, float* u, float* v, float* x0, bm_stream_t stream);
 /* dx0 [B,T,D] -> d_subj_w [S,IL,D], d_il_w [IL,O], d_il_b [IL], d_weights [R,O,C].
  * (subj_order, subj_off[S+1]) and (rec_order, rec_off[R+1]) are CSR groupings of the samples by subject and by
- * recording; dv [B,T,IL] and du [B,T,O] are scratch. */
+ * recording; dv [B,T,IL] and du [B,T,O] are scratch (du also out: the gradient at the mix output).
+ * Frozen parameters: d_subj_w, d_il_w, d_il_b, d_weights may each be NULL; its GEMM / reduction is skipped.  du may be
+ * NULL when d_weights is (nothing below needs it), dv when du, d_il_w and d_il_b are; a stage with no output left is not
+ * run.  With every pointer non-NULL the call is the full backward. */
 int bm_sensor_chain_bwd(const float* dx0, const float* meg, const float* il_w, const float* subj_w,
                         const int* subject, const float* u, const float* v, const int* subj_order,
                         const int* subj_off, const int* rec_order, const int* rec_off, int B, int C, int T, int O,
@@ -81,6 +84,10 @@ int bm_initial_linear_fwd(const float* u, int ld_u, const float* il_w, const flo
                           int ld_v, float* v, bm_stream_t stream);
 int bm_subject_layers_fwd(const float* v, int ld_v, const float* subj_w, const int* subject, int B, int T, int IL, int D,
                           int ld_x0, float* x0, bm_stream_t stream);
+/* bm_subject_layers_bwd: dv (the data gradient) and d_subj_w may each be NULL -- NULL dv: nothing below needs it (v, the
+ * CSR grouping are then read only for d_subj_w); NULL d_subj_w: frozen weights (v and the grouping may be NULL).
+ * bm_initial_linear_bwd (and its _det form): du, d_il_w and d_il_b may each be NULL and skip their GEMM / column sum; the
+ * _det form needs no workspace (NULL, 0) when d_il_w and d_il_b are both NULL. */
 int bm_subject_layers_bwd(const float* dx0, int ld_x0, const float* v, int ld_v, const float* subj_w, const int* subject,
                           const int* subj_order, const int* subj_off, int B, int T, int IL, int D, int S, int ld_dv,
                           float* dv, float* d_subj_w, bm_stream_t stream);
@@ -115,7 +122,11 @@ int bm_bn_gelu_skip_fwd(const float* y, const float* mean, const float* invstd, 
                         const float* beta, const float* x_old, float* x_new, long long rows, int C, float* amax_out,
                         bm_stream_t stream);
 /* g = dL/dx_new -> dy (through GELU and BN), dgamma, dbeta.  batch_stats=1: training-mode BN backward.
- * sums: fp64 [2*C] scratch. */
+ * sums: fp64 [2*C] scratch.
+ * batch_stats=0 with dgamma == dbeta == NULL (an eval-mode BatchNorm whose affine parameters are frozen): sums may be NULL
+ * too, and the call is one elementwise pass over g and y -- no column reduction, no fp64 scratch, and no workspace in the
+ * _det form (NULL, 0).  Its dy is bitwise the reducing form's.  With batch_stats=1, sums / dgamma / dbeta stay required:
+ * the data gradient needs the sums.  The same holds for bm_bn_act_skip_bwd(_det) with a BatchNorm (mean != NULL). */
 int bm_bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd,
                         const float* gamma, const float* beta, int batch_stats, long long rows, int C,
                         double* sums, float* dy, float* dgamma, float* dbeta, float* amax_out /* of dy */,
@@ -134,18 +145,23 @@ int bm_conv1d_glu_fwd(const float* x, const float* wf, const float* bias, int B,
 int bm_glu_bwd(const float* g, const float* h, long long rows, int H, float* dh,
                float* dbias /* nullable [2H]: sum over rows of dh = the GLU conv's bias gradient, from the same pass */,
                float* amax_out /* of dh */, bm_stream_t stream);
+/* (bm_glu_bwd_det with dbias == NULL reduces nothing and needs no workspace: NULL, 0.) */
 
 /* ---- K5: head Conv1d(H,2H,1) -> GELU -> ConvTranspose1d(2H,F,1) (simpleconv.py:185-189,246-249) --------
  * x [B,T,H]; w0 [2H,H]; w2 [2H,F] (ConvTranspose1d weight is input-major); out h1,q [B,T,2H], est [B,F,T]. */
 int bm_head_fwd(const float* x, const float* w0, const float* b0, const float* w2, const float* b2, int B, int T,
                 int H, int F, float* h1, float* q, float* est, bm_stream_t stream);
-/* dest [B,F,T] -> dx [B,T,H], dw0 [2H,H], db0 [2H], dw2 [2H,F], db2 [F]; dq [B,T,2H] scratch. */
+/* dest [B,F,T] -> dx [B,T,H], dw0 [2H,H], db0 [2H], dw2 [2H,F], db2 [F]; dq [B,T,2H] scratch.
+ * dw0, db0, dw2, db2 (frozen head parameters) and dx (nothing below needs it) may each be NULL and skip their GEMM /
+ * reduction; with dx, dw0 and db0 all NULL neither dq nor GELU'(h1) is computed (dq, h1, w2 may then be NULL).  The _det
+ * form needs no workspace (NULL, 0) when all four parameter gradients are NULL. */
 int bm_head_bwd(const float* dest, const float* x, const float* w0, const float* w2, const float* h1,
                 const float* q, int B, int T, int H, int F, float* dq, float* dx, float* dw0, float* db0,
                 float* dw2, float* db2, bm_stream_t stream);
 
 /* parameter-gradient half of bm_head_bwd, for callers that compute dq and dx themselves (tensor-core path):
- * in: dq = d(loss)/dq [B,T,2H]; out: dw2, db2, dq <- dq*GELU'(h1) (in place), dw0, db0. */
+ * in: dq = d(loss)/dq [B,T,2H]; out: dw2, db2, dq <- dq*GELU'(h1) (in place), dw0, db0.  dw0, db0, dw2, db2 may each be
+ * NULL (x is read only for dw0, q only for dw2); dq always becomes dh1. */
 int bm_head_bwd_params(const float* dest, const float* x, const float* h1, const float* q, int B, int T, int H, int F,
                        float* dq, float* dw0, float* db0, float* dw2, float* db2, bm_stream_t stream);
 
@@ -368,7 +384,7 @@ long long bm_bn_gelu_skip_bwd_det_workspace(long long rows, int C);
 int bm_bn_gelu_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
                             const float* beta, int batch_stats, long long rows, int C, double* sums, float* dy, float* dgamma,
                             float* dbeta, float* amax_out, float* workspace, long long workspace_floats, bm_stream_t stream);
-/* workspace unused (may be NULL) when mean == NULL */
+/* workspace unused (may be NULL) when mean == NULL, or batch_stats == 0 with dgamma == dbeta == NULL */
 long long bm_bn_act_skip_bwd_det_workspace(long long rows, int C);
 int bm_bn_act_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
                            const float* beta, int batch_stats, long long rows, int C, int act, float slope, double* sums,
