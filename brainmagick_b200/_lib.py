@@ -108,6 +108,11 @@ SIGNATURES = {
     "bm_clip_scores_det": [P, P, I, I, L, I, P, P, P, P, L, P, P],
     "bm_clip_loss_fwd_det": [P, P, I, I, L, I, P, P, P, P, P, P, L, P, P],
 }
+# single-pass TF32 forms (tf32() below): the default form's arguments
+TF32_FORMS = ("bm_tc_conv1d", "bm_tc_conv1d_persistent", "bm_tc_pointwise_sel", "bm_tc_sensor_mix_bwd_data", "bm_tc_wgrad",
+              "bm_tc_wgrad_conv", "bm_tc_wgrad_grouped", "bm_clip_scores", "bm_clip_scores_det", "bm_clip_loss_fwd",
+              "bm_clip_loss_fwd_det", "bm_clip_loss_bwd", "bm_clip_loss_bwd_cand", "bm_clip_scores_bwd")
+SIGNATURES.update({name + "_tf32": SIGNATURES[name] for name in TF32_FORMS})
 
 
 _lib = None
@@ -166,6 +171,15 @@ def deterministic() -> bool:
     """True when every call should take its deterministic (`_det`) form: exactly when PyTorch's
     torch.use_deterministic_algorithms(True) is in effect.  Read per call; the one place the host code asks."""
     return torch.are_deterministic_algorithms_enabled()
+
+
+def tf32() -> bool:
+    """True when every tensor-core contraction should take its single-pass TF32 (`_tf32`) form: exactly when PyTorch's float32
+    matmul precision allows TF32 (torch.backends.cuda.matmul.fp32_precision == "tf32", which torch sets whichever of
+    set_float32_matmul_precision("high" / "medium"), matmul.allow_tf32 = True or fp32_precision = "tf32" the caller used).
+    cuDNN's conv flag is deliberately not read: it defaults to TF32, and the library's default stays 3xTF32.  Read per call;
+    the one place the host code asks."""
+    return torch.backends.cuda.matmul.fp32_precision == "tf32"
 
 
 def launch_count() -> int:

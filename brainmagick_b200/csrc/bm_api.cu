@@ -25,6 +25,15 @@ using namespace bm;
 
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 
+// ---- TF32 forms (the `_tf32` entry points) -----------------------------------------------------------------------------
+// Every entry point that runs a tensor-core contraction is a static implementation whose first argument is the engine's
+// pass count (tc_common.cuh).  BM_TC_FORMS defines over it the default entry point (3xTF32) and its `_tf32` twin
+// (single-pass TF32: each fp32 operand element rounded once to tf32), with identical arguments.
+#define BM_ARGS(...) __VA_ARGS__
+#define BM_TC_FORMS(name, impl, params, args)                                                                            \
+    extern "C" int name params { return impl(3, BM_ARGS args); }                                                          \
+    extern "C" int name##_tf32 params { return impl(1, BM_ARGS args); }
+
 extern "C" const char* bm_last_error(void) { return bm::g_last_error; }
 extern "C" int bm_abi_version(void) { return 1; }
 extern "C" unsigned long long bm_launch_count(void) { return bm::g_launches; }
@@ -892,14 +901,14 @@ namespace {
 // det: the candidate sums of squares one block per candidate, the FP32-FMA score GEMM without a K split
 int clip_forward(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given, int target_offset,
                  float* inv_norm, float* scores, float* probs, float* row_loss, float* loss, float* ws,
-                 long long ws_floats, int* status, bool det, cudaStream_t st) {
+                 long long ws_floats, int* status, bool det, int passes, cudaStream_t st) {
     BM_CHECK_ARG(est && cand && inv_norm && scores && ws && Bn > 0 && Bc > 0 && KT > 0);
     BM_CHECK_ARG(KT < (1ll << 31));
     BM_CHECK_ARG(ws_floats >= bm_clip_workspace(Bn, Bc, KT));
     BM_CHECK_ARG((reinterpret_cast<uintptr_t>(ws) & 7) == 0);
     if (tc::clip_tc_supported(Bn, Bc, KT))
         return tc::launch_clip_scores(est, cand, Bn, Bc, KT, norms_given, target_offset, inv_norm, scores, probs, row_loss,
-                                      loss, ws, status, st, det);
+                                      loss, ws, passes, status, st, det);
     // FP32-FMA GEMM (feature sizes not a multiple of 4 floats: no TMA row pitch)
     if (!norms_given) {
         int rc = candidate_inv_norms(cand, Bc, KT, reinterpret_cast<double*>(ws), inv_norm, det, st);
@@ -929,55 +938,55 @@ int clip_forward(const float* est, const float* cand, int Bn, int Bc, long long 
     }
     return 0;
 }
+int clip_scores(int passes, bool det, const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
+                float* inv_norm, float* scores, float* probs, float* workspace, long long workspace_floats, int* status,
+                bm_stream_t stream) {
+    return clip_forward(est, cand, Bn, Bc, KT, norms_given, 0, inv_norm, scores, probs, nullptr, nullptr, workspace,
+                        workspace_floats, status, det, passes, ST(stream));
+}
+int clip_loss_fwd(int passes, bool det, const float* est, const float* cand, int Bn, int Bc, long long KT, int target_offset,
+                  float* inv_norm, float* scores, float* probs, float* row_loss, float* loss, float* workspace,
+                  long long workspace_floats, int* status, bm_stream_t stream) {
+    BM_CHECK_ARG(probs && row_loss && loss);
+    BM_CHECK_ARG(target_offset >= 0 && target_offset + Bn <= Bc);
+    return clip_forward(est, cand, Bn, Bc, KT, 0, target_offset, inv_norm, scores, probs, row_loss, loss, workspace,
+                        workspace_floats, status, det, passes, ST(stream));
+}
 }  // namespace
 
-extern "C" int bm_clip_scores(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
-                              float* inv_norm, float* scores, float* probs, float* workspace,
-                              long long workspace_floats, int* status, bm_stream_t stream) {
-    return clip_forward(est, cand, Bn, Bc, KT, norms_given, 0, inv_norm, scores, probs, nullptr, nullptr, workspace,
-                        workspace_floats, status, false, ST(stream));
-}
-extern "C" int bm_clip_scores_det(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
-                                  float* inv_norm, float* scores, float* probs, float* workspace,
-                                  long long workspace_floats, int* status, bm_stream_t stream) {
-    return clip_forward(est, cand, Bn, Bc, KT, norms_given, 0, inv_norm, scores, probs, nullptr, nullptr, workspace,
-                        workspace_floats, status, true, ST(stream));
-}
+#define BM_CLIP_SCORES_PARAMS                                                                                            \
+    (const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given, float* inv_norm, float* scores, \
+     float* probs, float* workspace, long long workspace_floats, int* status, bm_stream_t stream)
+#define BM_CLIP_SCORES_ARGS(det) \
+    (det, est, cand, Bn, Bc, KT, norms_given, inv_norm, scores, probs, workspace, workspace_floats, status, stream)
+BM_TC_FORMS(bm_clip_scores, clip_scores, BM_CLIP_SCORES_PARAMS, BM_CLIP_SCORES_ARGS(false))
+BM_TC_FORMS(bm_clip_scores_det, clip_scores, BM_CLIP_SCORES_PARAMS, BM_CLIP_SCORES_ARGS(true))
 
-extern "C" int bm_clip_loss_fwd(const float* est, const float* cand, int Bn, int Bc, long long KT,
-                                int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss,
-                                float* loss, float* workspace, long long workspace_floats, int* status,
-                                bm_stream_t stream) {
-    BM_CHECK_ARG(probs && row_loss && loss);
-    BM_CHECK_ARG(target_offset >= 0 && target_offset + Bn <= Bc);
-    return clip_forward(est, cand, Bn, Bc, KT, 0, target_offset, inv_norm, scores, probs, row_loss, loss, workspace,
-                        workspace_floats, status, false, ST(stream));
-}
-extern "C" int bm_clip_loss_fwd_det(const float* est, const float* cand, int Bn, int Bc, long long KT,
-                                    int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss,
-                                    float* loss, float* workspace, long long workspace_floats, int* status,
-                                    bm_stream_t stream) {
-    BM_CHECK_ARG(probs && row_loss && loss);
-    BM_CHECK_ARG(target_offset >= 0 && target_offset + Bn <= Bc);
-    return clip_forward(est, cand, Bn, Bc, KT, 0, target_offset, inv_norm, scores, probs, row_loss, loss, workspace,
-                        workspace_floats, status, true, ST(stream));
-}
+#define BM_CLIP_LOSS_FWD_PARAMS                                                                                          \
+    (const float* est, const float* cand, int Bn, int Bc, long long KT, int target_offset, float* inv_norm,              \
+     float* scores, float* probs, float* row_loss, float* loss, float* workspace, long long workspace_floats,            \
+     int* status, bm_stream_t stream)
+#define BM_CLIP_LOSS_FWD_ARGS(det)                                                                                       \
+    (det, est, cand, Bn, Bc, KT, target_offset, inv_norm, scores, probs, row_loss, loss, workspace, workspace_floats,    \
+     status, stream)
+BM_TC_FORMS(bm_clip_loss_fwd, clip_loss_fwd, BM_CLIP_LOSS_FWD_PARAMS, BM_CLIP_LOSS_FWD_ARGS(false))
+BM_TC_FORMS(bm_clip_loss_fwd_det, clip_loss_fwd, BM_CLIP_LOSS_FWD_PARAMS, BM_CLIP_LOSS_FWD_ARGS(true))
 
 namespace {
 // dest = G @ cand, the GEMM of the CLIP backward.  fill(transposed) writes G [Bn][Bc] (transposed: [Bc][Bn]) in the layout
 // the chosen GEMM reads.
 template <class Fill>
-int clip_dest_gemm(Fill fill, const float* cand, int Bn, int Bc, long long KT, float* G, float* dest, int* status,
-                   cudaStream_t st) {
+int clip_dest_gemm(Fill fill, const float* cand, int Bn, int Bc, long long KT, float* G, float* dest, int passes,
+                   int* status, cudaStream_t st) {
     if (tc::gemm_nt_pp_supported(Bn, (int)KT, Bc) && Bn >= 192) {
         // csrc/tc_gemm_nt.cuh: dE = G C with G [Bn][Bc], C [Bc][KT]; smaller batches take the weight-gradient form below
         if (int rc = fill(0)) return rc;
-        return tc::launch_gemm_nt_pp(G, cand, dest, Bn, (int)KT, Bc, status, st);
+        return tc::launch_gemm_nt_pp(G, cand, dest, Bn, (int)KT, Bc, passes, status, st);
     }
     if (tc::wgrad_tc_supported(Bn, (int)KT)) {
         // tensor cores: dE[b][k] = sum_o G^T[o][b] C[o][k]  == weight-gradient GEMM with "positions" = candidates
         if (int rc = fill(1)) return rc;
-        return tc::launch_wgrad_tc(G, cand, 1, Bc, Bn, (int)KT, (int)KT, 1, 1, dest, dest, status, st);   // direct mode: no workspace
+        return tc::launch_wgrad_tc(G, cand, 1, Bc, Bn, (int)KT, (int)KT, 1, 1, dest, dest, passes, status, st);   // direct mode
     }
     if (int rc = fill(0)) return rc;
     GemmP g = gemm_defaults();
@@ -992,7 +1001,7 @@ int clip_dest_gemm(Fill fill, const float* cand, int Bn, int Bc, long long KT, f
 // dcand[o] = sum_b G[b][o] est[b] - coef[o] cand[o] (see clip_cand_coef_kernel); fill as in clip_dest_gemm
 template <class Fill>
 int clip_dcand_gemm(Fill fill, const float* scores, const float* inv_norm, const float* est, const float* cand, int Bn, int Bc,
-                    long long KT, float* G, float* coef, float* dcand, int* status, cudaStream_t st) {
+                    long long KT, float* G, float* coef, float* dcand, int passes, int* status, cudaStream_t st) {
     if (int rc = fill(0)) return rc;
     clip_cand_coef_kernel<<<(Bc + 127) / 128, 128, 0, st>>>(G, scores, inv_norm, Bn, Bc, coef);     // needs G as [Bn][Bc]
     BM_CHECK_LAUNCH();
@@ -1000,10 +1009,10 @@ int clip_dcand_gemm(Fill fill, const float* scores, const float* inv_norm, const
     if (tc::gemm_nt_pp_supported(Bc, (int)KT, Bn)) {
         // csrc/tc_gemm_nt.cuh: A = G^T [Bc][Bn] (rewritten into the same scratch), B = est [Bn][KT]
         if (int rc = fill(1)) return rc;
-        int rc = tc::launch_gemm_nt_pp(G, est, dcand, Bc, (int)KT, Bn, status, st);
+        int rc = tc::launch_gemm_nt_pp(G, est, dcand, Bc, (int)KT, Bn, passes, status, st);
         if (rc) return rc;
     } else if (tc::wgrad_tc_supported(Bc, (int)KT)) {
-        int rc = tc::launch_wgrad_tc(G, est, 1, Bn, Bc, (int)KT, (int)KT, 1, 1, dcand, dcand, status, st);   // direct mode
+        int rc = tc::launch_wgrad_tc(G, est, 1, Bn, Bc, (int)KT, (int)KT, 1, 1, dcand, dcand, passes, status, st);   // direct
         if (rc) return rc;
     } else {
         GemmP g = gemm_defaults();
@@ -1017,11 +1026,9 @@ int clip_dcand_gemm(Fill fill, const float* scores, const float* inv_norm, const
     BM_CHECK_LAUNCH();
     return 0;
 }
-}  // namespace
 
-extern "C" int bm_clip_loss_bwd(const float* probs, const float* inv_norm, const float* cand, const float* gout,
-                                int Bn, int Bc, long long KT, int target_offset, float* G, float* dest,
-                                int* status, bm_stream_t stream) {
+int clip_loss_bwd(int passes, const float* probs, const float* inv_norm, const float* cand, const float* gout, int Bn, int Bc,
+                  long long KT, int target_offset, float* G, float* dest, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(probs && inv_norm && cand && gout && G && dest && Bn > 0 && Bc > 0 && KT > 0);
     BM_CHECK_ARG(KT < (1ll << 31));
     cudaStream_t st = ST(stream);
@@ -1031,8 +1038,14 @@ extern "C" int bm_clip_loss_bwd(const float* probs, const float* inv_norm, const
         BM_CHECK_LAUNCH();
         return 0;
     };
-    return clip_dest_gemm(fill, cand, Bn, Bc, KT, G, dest, status, st);
+    return clip_dest_gemm(fill, cand, Bn, Bc, KT, G, dest, passes, status, st);
 }
+}  // namespace
+
+BM_TC_FORMS(bm_clip_loss_bwd, clip_loss_bwd,
+            (const float* probs, const float* inv_norm, const float* cand, const float* gout, int Bn, int Bc, long long KT,
+             int target_offset, float* G, float* dest, int* status, bm_stream_t stream),
+            (probs, inv_norm, cand, gout, Bn, Bc, KT, target_offset, G, dest, status, stream))
 
 // =================================================================================================
 // Stand-alone ConvSequence epilogues + candidate-side ClipLoss gradient (SURVEY 8(f) row 3: DeepMel)
@@ -1101,10 +1114,9 @@ extern "C" int bm_bn_act_skip_bwd_det(const float* g, const float* y, const floa
                            reinterpret_cast<double*>(workspace), ST(stream));
 }
 
-extern "C" int bm_clip_loss_bwd_cand(const float* probs, const float* scores, const float* inv_norm, const float* est,
-                                     const float* cand, const float* gout, int Bn, int Bc, long long KT,
-                                     int target_offset, float* G, float* coef, float* dcand, int* status,
-                                     bm_stream_t stream) {
+static int clip_loss_bwd_cand(int passes, const float* probs, const float* scores, const float* inv_norm, const float* est,
+                              const float* cand, const float* gout, int Bn, int Bc, long long KT, int target_offset, float* G,
+                              float* coef, float* dcand, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(probs && scores && inv_norm && est && cand && gout && G && coef && dcand);
     BM_CHECK_ARG(Bn > 0 && Bc > 0 && KT > 0 && KT < (1ll << 31));
     cudaStream_t st = ST(stream);
@@ -1114,12 +1126,17 @@ extern "C" int bm_clip_loss_bwd_cand(const float* probs, const float* scores, co
         BM_CHECK_LAUNCH();
         return 0;
     };
-    return clip_dcand_gemm(fill, scores, inv_norm, est, cand, Bn, Bc, KT, G, coef, dcand, status, st);
+    return clip_dcand_gemm(fill, scores, inv_norm, est, cand, Bn, Bc, KT, G, coef, dcand, passes, status, st);
 }
+BM_TC_FORMS(bm_clip_loss_bwd_cand, clip_loss_bwd_cand,
+            (const float* probs, const float* scores, const float* inv_norm, const float* est, const float* cand,
+             const float* gout, int Bn, int Bc, long long KT, int target_offset, float* G, float* coef, float* dcand,
+             int* status, bm_stream_t stream),
+            (probs, scores, inv_norm, est, cand, gout, Bn, Bc, KT, target_offset, G, coef, dcand, status, stream))
 
-extern "C" int bm_clip_scores_bwd(const float* dscores, const float* scores, const float* inv_norm, const float* est,
-                                  const float* cand, int Bn, int Bc, long long KT, float* G, float* coef, float* dest,
-                                  float* dcand, int* status, bm_stream_t stream) {
+static int clip_scores_bwd(int passes, const float* dscores, const float* scores, const float* inv_norm, const float* est,
+                           const float* cand, int Bn, int Bc, long long KT, float* G, float* coef, float* dest, float* dcand,
+                           int* status, bm_stream_t stream) {
     BM_CHECK_ARG(dscores && inv_norm && cand && G && Bn > 0 && Bc > 0 && KT > 0 && KT < (1ll << 31));
     BM_CHECK_ARG(!dcand || (scores && est && coef));
     cudaStream_t st = ST(stream);
@@ -1129,11 +1146,16 @@ extern "C" int bm_clip_scores_bwd(const float* dscores, const float* scores, con
         return 0;
     };
     if (dest)
-        if (int rc = clip_dest_gemm(fill, cand, Bn, Bc, KT, G, dest, status, st)) return rc;
+        if (int rc = clip_dest_gemm(fill, cand, Bn, Bc, KT, G, dest, passes, status, st)) return rc;
     if (dcand)
-        if (int rc = clip_dcand_gemm(fill, scores, inv_norm, est, cand, Bn, Bc, KT, G, coef, dcand, status, st)) return rc;
+        if (int rc = clip_dcand_gemm(fill, scores, inv_norm, est, cand, Bn, Bc, KT, G, coef, dcand, passes, status, st))
+            return rc;
     return 0;
 }
+BM_TC_FORMS(bm_clip_scores_bwd, clip_scores_bwd,
+            (const float* dscores, const float* scores, const float* inv_norm, const float* est, const float* cand, int Bn,
+             int Bc, long long KT, float* G, float* coef, float* dest, float* dcand, int* status, bm_stream_t stream),
+            (dscores, scores, inv_norm, est, cand, Bn, Bc, KT, G, coef, dest, dcand, status, stream))
 
 // =================================================================================================
 // Retrieval evaluation (SURVEY 8(f) row 1)
@@ -1239,12 +1261,12 @@ extern "C" int bm_tc_weight_split(const float* w, int Cout, int Cin, int Kw, flo
     return 0;
 }
 
-extern "C" int bm_tc_conv1d(const float* x, const float* w_hi, const float* w_lo, const float* bias,
-                            const float* addend, int B, int T, int Cin, int Ntot, int Kw, int dilation, int sign,
-                            int glu, int act, int out_tmajor, float* y, float* aux, float* glu_out, double* stats,
-                            int* status, bm_stream_t stream) {
+// passes = 1 (the _tf32 form): w_hi alone is read, w_lo may be NULL
+static int tc_conv1d(int passes, const float* x, const float* w_hi, const float* w_lo, const float* bias, const float* addend,
+                     int B, int T, int Cin, int Ntot, int Kw, int dilation, int sign, int glu, int act, int out_tmajor,
+                     float* y, float* aux, float* glu_out, double* stats, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(stats == nullptr);      // BatchNorm statistics in the epilogue: bm_tc_conv1d_persistent / bm_tc_conv1d_f16
-    BM_CHECK_ARG(x && w_hi && w_lo && B > 0 && T > 0 && dilation >= 1 && (sign == 1 || sign == -1));
+    BM_CHECK_ARG(x && w_hi && (w_lo || passes == 1) && B > 0 && T > 0 && dilation >= 1 && (sign == 1 || sign == -1));
     BM_CHECK_ARG(glu ? (glu_out != nullptr) : (y != nullptr));
     BM_CHECK_ARG(B <= 65535);
     BM_CHECK_ARG(!(glu && (act || out_tmajor || aux)));
@@ -1252,10 +1274,16 @@ extern "C" int bm_tc_conv1d(const float* x, const float* w_hi, const float* w_lo
     tc::ConvTcP p;
     p.B = B; p.T = T; p.Cin = Cin; p.Ntot = Ntot; p.taps = Kw; p.dilation = dilation; p.sign = sign; p.glu = glu;
     p.bias = bias; p.addend = addend; p.y = y; p.glu_out = glu_out; p.err = status;
-    p.act = act; p.out_tmajor = out_tmajor; p.aux = aux; p.wsel = nullptr; p.n_wsets = 1;
+    p.act = act; p.out_tmajor = out_tmajor; p.aux = aux; p.wsel = nullptr; p.n_wsets = 1; p.passes = passes;
     BM_CHECK_ARG(!(glu && (act || out_tmajor || aux)));
-    return tc::launch_conv_tc(x, w_hi, w_lo, p, ST(stream));
+    return tc::launch_conv_tc(x, w_hi, passes == 1 ? nullptr : w_lo, p, ST(stream));
 }
+BM_TC_FORMS(bm_tc_conv1d, tc_conv1d,
+            (const float* x, const float* w_hi, const float* w_lo, const float* bias, const float* addend, int B, int T,
+             int Cin, int Ntot, int Kw, int dilation, int sign, int glu, int act, int out_tmajor, float* y, float* aux,
+             float* glu_out, double* stats, int* status, bm_stream_t stream),
+            (x, w_hi, w_lo, bias, addend, B, T, Cin, Ntot, Kw, dilation, sign, glu, act, out_tmajor, y, aux, glu_out, stats,
+             status, stream))
 
 // per-column sum / sum of squares of a channels-last matrix (BatchNorm batch statistics after bm_tc_conv1d)
 extern "C" int bm_col_stats(const float* y, long long rows, int C, double* stats, bm_stream_t stream) {
@@ -1318,12 +1346,16 @@ extern "C" int bm_tc_wgrad_supported(int M, int N) { return tc::wgrad_tc_support
 extern "C" long long bm_tc_wgrad_workspace(int B, int M, int N, int Kw) {
     return (long long)tc::wgrad_workspace_floats(B, M, N, Kw);
 }
-extern "C" int bm_tc_wgrad(const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw,
-                           int dilation, float* workspace, float* dw, float* dbias, int* status, bm_stream_t stream) {
+static int tc_wgrad(int passes, const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw, int dilation,
+                    float* workspace, float* dw, float* dbias, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(dy && x && workspace && dw && B > 0 && T > 0 && Kw >= 1 && Kw <= 3 && dilation >= 1);
     BM_CHECK_ARG(tc::wgrad_tc_supported(M, N) && Ntrue > 0 && Ntrue <= N);
-    return tc::launch_wgrad_tc(dy, x, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, status, ST(stream), dbias);
+    return tc::launch_wgrad_tc(dy, x, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, passes, status, ST(stream), dbias);
 }
+BM_TC_FORMS(bm_tc_wgrad, tc_wgrad,
+            (const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw, int dilation, float* workspace,
+             float* dw, float* dbias, int* status, bm_stream_t stream),
+            (dy, x, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, dbias, status, stream))
 
 // weight gradient of a k-tap conv (csrc/tc_wgradp.cuh): output rows = (tap, x channel), reduction over the
 // flattened rows; no bias gradient (use bm_col_sum on dy where the layer's bias gradient is not exactly zero)
@@ -1333,12 +1365,16 @@ extern "C" int bm_tc_wgrad_conv_supported(int T, int M, int N, int Kw) {
 extern "C" long long bm_tc_wgrad_conv_workspace(int B, int T, int M, int N, int Kw) {
     return (long long)tc::wgradp_workspace_floats(B, T, M, N, Kw);
 }
-extern "C" int bm_tc_wgrad_conv(const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw,
-                                int dilation, float* workspace, float* dw, int* status, bm_stream_t stream) {
+static int tc_wgrad_conv(int passes, const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw,
+                         int dilation, float* workspace, float* dw, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(dy && x && workspace && dw && B > 0 && T > 0 && dilation >= 1);
     BM_CHECK_ARG(tc::wgradp_supported(T, M, N, Kw) && Ntrue > 0 && Ntrue <= N);
-    return tc::launch_wgrad_pp(dy, x, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, status, ST(stream));
+    return tc::launch_wgrad_pp(dy, x, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, passes, status, ST(stream));
 }
+BM_TC_FORMS(bm_tc_wgrad_conv, tc_wgrad_conv,
+            (const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw, int dilation, float* workspace,
+             float* dw, int* status, bm_stream_t stream),
+            (dy, x, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, status, stream))
 
 // the same weight gradient for callers that hold the operands' amax (csrc/tc_wgradp.cuh): dy_amax / x_amax = device floats with max |dy|, max |x|
 // (bm_amax, or the amax_out of the kernels that produced the tensors); same shape gate and workspace as bm_tc_wgrad_conv
@@ -1388,19 +1424,24 @@ extern "C" int bm_tc_conv1d_persistent_supported(int T, int Cin, int Ntot, int K
 }
 // csrc/tc_convp.cuh: w_raw = the RAW fp32 weights re-laid K-major [Kw][Ntot][Cin]
 // (bm_tc_weight_split with f_lo / g_lo = NULL); accumulate=1: y += conv (in place, TMA reduce-add)
-extern "C" int bm_tc_conv1d_persistent(const float* x, const float* w_raw, const float* bias, int accumulate, int B, int T,
-                                       int Cin, int Ntot, int Kw, int dilation, int sign, int glu, int act,
-                                       int out_tmajor, float* y, float* aux, float* glu_out, double* stats, int* status,
-                                       bm_stream_t stream) {
+static int tc_conv1d_persistent(int passes, const float* x, const float* w_raw, const float* bias, int accumulate, int B,
+                                int T, int Cin, int Ntot, int Kw, int dilation, int sign, int glu, int act, int out_tmajor,
+                                float* y, float* aux, float* glu_out, double* stats, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(x && w_raw && B > 0 && T > 0 && dilation >= 1 && (sign == 1 || sign == -1));
     BM_CHECK_ARG(glu ? (glu_out != nullptr) : (y != nullptr));
     BM_CHECK_ARG(tc::conv_pp_supported(T, Cin, Ntot, Kw, glu));
     tc::ConvPPArgs a;
     a.x = x; a.w_raw = w_raw; a.bias = bias; a.B = B; a.T = T; a.Cin = Cin; a.Ntot = Ntot; a.taps = Kw;
     a.dilation = dilation; a.sign = sign; a.glu = glu; a.act = act; a.out_tmajor = out_tmajor; a.accumulate = accumulate;
-    a.y = y; a.aux = aux; a.glu_out = glu_out; a.stats = stats; a.err = status;
+    a.y = y; a.aux = aux; a.glu_out = glu_out; a.stats = stats; a.err = status; a.passes = passes;
     return tc::launch_conv_pp(a, ST(stream));
 }
+BM_TC_FORMS(bm_tc_conv1d_persistent, tc_conv1d_persistent,
+            (const float* x, const float* w_raw, const float* bias, int accumulate, int B, int T, int Cin, int Ntot, int Kw,
+             int dilation, int sign, int glu, int act, int out_tmajor, float* y, float* aux, float* glu_out, double* stats,
+             int* status, bm_stream_t stream),
+            (x, w_raw, bias, accumulate, B, T, Cin, Ntot, Kw, dilation, sign, glu, act, out_tmajor, y, aux, glu_out, stats,
+             status, stream))
 
 // ---- the same conv with fp16-piece weights (csrc/tc_convh.cuh): fp32 weights as two fp16 pieces of a power-of-two-scaled
 // tensor.  bm_amax writes the largest magnitude of a tensor into a device float; bm_f16_split prepares the weights
@@ -1434,7 +1475,7 @@ extern "C" int bm_tc_conv1d_f16(const float* x, const float* x_amax, const void*
     tc::ConvPPArgs& a = h.c;
     a.x = x; a.w_raw = nullptr; a.bias = bias; a.B = B; a.T = T; a.Cin = Cin; a.Ntot = Ntot; a.taps = Kw;
     a.dilation = dilation; a.sign = sign; a.glu = glu; a.act = act; a.out_tmajor = out_tmajor; a.accumulate = accumulate;
-    a.y = y; a.aux = aux; a.glu_out = glu_out; a.stats = stats; a.err = status;
+    a.y = y; a.aux = aux; a.glu_out = glu_out; a.stats = stats; a.err = status; a.passes = 3;
     h.x_amax = x_amax; h.w_hi = w_hi; h.w_lo = w_lo; h.w_amax = w_amax; h.out_amax = amax_out;
     BM_CHECK_ARG(!amax_out || ((glu || act) && !out_tmajor));      // the outputs another conv consumes: GLU out, GELU out
     if (int rc = amax_begin(amax_out, ST(stream))) return rc;
@@ -1443,35 +1484,48 @@ extern "C" int bm_tc_conv1d_f16(const float* x, const float* x_amax, const void*
 
 // pointwise (1x1) contraction with a per-sample weight set (SubjectLayers.forward / its data gradient, common.py:55-58):
 //   y[b,t,n] = sum_k x[b,t,k] W[wsel[b]][n][k];  w_hi/w_lo are the tf32-split K-major weight sets [S][Ntot][Cin]
-extern "C" int bm_tc_pointwise_sel(const float* x, const float* w_hi, const float* w_lo, const int* wsel, int n_sets,
-                                   int B, int T, int Cin, int Ntot, float* y, int* status, bm_stream_t stream) {
-    BM_CHECK_ARG(x && w_hi && w_lo && wsel && y && n_sets > 0 && B > 0 && B <= 65535 && T > 0);
+static int tc_pointwise_sel(int passes, const float* x, const float* w_hi, const float* w_lo, const int* wsel, int n_sets,
+                            int B, int T, int Cin, int Ntot, float* y, int* status, bm_stream_t stream) {
+    BM_CHECK_ARG(x && w_hi && (w_lo || passes == 1) && wsel && y && n_sets > 0 && B > 0 && B <= 65535 && T > 0);
     BM_CHECK_ARG(tc::conv_tc_supported(T, Cin, Ntot, 1, 0));
     tc::ConvTcP p;
     p.B = B; p.T = T; p.Cin = Cin; p.Ntot = Ntot; p.taps = 1; p.dilation = 1; p.sign = 1; p.glu = 0;
     p.bias = nullptr; p.addend = nullptr; p.y = y; p.glu_out = nullptr; p.err = status;
-    p.act = 0; p.out_tmajor = 0; p.aux = nullptr; p.wsel = wsel; p.n_wsets = n_sets;
-    return tc::launch_conv_tc(x, w_hi, w_lo, p, ST(stream));
+    p.act = 0; p.out_tmajor = 0; p.aux = nullptr; p.wsel = wsel; p.n_wsets = n_sets; p.passes = passes;
+    return tc::launch_conv_tc(x, w_hi, passes == 1 ? nullptr : w_lo, p, ST(stream));
 }
+BM_TC_FORMS(bm_tc_pointwise_sel, tc_pointwise_sel,
+            (const float* x, const float* w_hi, const float* w_lo, const int* wsel, int n_sets, int B, int T, int Cin,
+             int Ntot, float* y, int* status, bm_stream_t stream),
+            (x, w_hi, w_lo, wsel, n_sets, B, T, Cin, Ntot, y, status, stream))
 
 // data gradient of the sensor mix on the tensor cores (ChannelMerger, common.py:358):
 //   dmeg[b,c,t] = mask[c] sum_o du[b,t,o] W[wsel[b]][c][o], c < C;  w_hi / w_lo: tf32-split transposed weight sets [S][Cp][Op]
-extern "C" int bm_tc_sensor_mix_bwd_data(const float* du, const float* w_hi, const float* w_lo, const int* wsel, int n_sets,
-                                         const float* mask, int B, int T, int Op, int Cp, int C, float* dmeg, int* status,
-                                         bm_stream_t stream) {
-    BM_CHECK_ARG(du && w_hi && w_lo && wsel && dmeg && n_sets > 0 && B > 0 && T > 0 && C > 0 && C <= Cp);
+static int tc_sensor_mix_bwd_data(int passes, const float* du, const float* w_hi, const float* w_lo, const int* wsel,
+                                  int n_sets, const float* mask, int B, int T, int Op, int Cp, int C, float* dmeg, int* status,
+                                  bm_stream_t stream) {
+    BM_CHECK_ARG(du && w_hi && (w_lo || passes == 1) && wsel && dmeg && n_sets > 0 && B > 0 && T > 0 && C > 0 && C <= Cp);
     BM_CHECK_ARG(tc::conv_tc_supported(T, Op, Cp, 1, 0));
-    return tc::launch_sensor_mix_bwd_tc(du, w_hi, w_lo, wsel, n_sets, mask, B, T, Op, Cp, C, dmeg, status, ST(stream));
+    return tc::launch_sensor_mix_bwd_tc(du, w_hi, passes == 1 ? nullptr : w_lo, wsel, n_sets, mask, B, T, Op, Cp, C, dmeg,
+                                        passes, status, ST(stream));
 }
+BM_TC_FORMS(bm_tc_sensor_mix_bwd_data, tc_sensor_mix_bwd_data,
+            (const float* du, const float* w_hi, const float* w_lo, const int* wsel, int n_sets, const float* mask, int B,
+             int T, int Op, int Cp, int C, float* dmeg, int* status, bm_stream_t stream),
+            (du, w_hi, w_lo, wsel, n_sets, mask, B, T, Op, Cp, C, dmeg, status, stream))
 
 // per-group pointwise weight gradient (SubjectLayers: dM[s] = sum over the samples of subject s), tensor cores:
 //   out[g][m][n] = sum_{b in group g} sum_t dy[b,t,m] x[b,t,n];  out is [G][ceil(M/128)*128][N]
-extern "C" int bm_tc_wgrad_grouped(const float* dy, const float* x, const int* order, const int* seg_off, int G, int B,
-                                   int T, int M, int N, float* out, int* status, bm_stream_t stream) {
+static int tc_wgrad_grouped(int passes, const float* dy, const float* x, const int* order, const int* seg_off, int G, int B,
+                            int T, int M, int N, float* out, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(dy && x && order && seg_off && out && G > 0 && B > 0 && T > 0);
     BM_CHECK_ARG(tc::wgrad_tc_supported(M, N));
-    return tc::launch_wgrad_tc_grouped(dy, x, order, seg_off, G, B, T, M, N, out, status, ST(stream));
+    return tc::launch_wgrad_tc_grouped(dy, x, order, seg_off, G, B, T, M, N, out, passes, status, ST(stream));
 }
+BM_TC_FORMS(bm_tc_wgrad_grouped, tc_wgrad_grouped,
+            (const float* dy, const float* x, const int* order, const int* seg_off, int G, int B, int T, int M, int N,
+             float* out, int* status, bm_stream_t stream),
+            (dy, x, order, seg_off, G, B, T, M, N, out, status, stream))
 
 // ---- K1 pieces, for callers that run the two attention contractions on the tensor cores -------------------------
 extern "C" int bm_fourier_emb(const float* positions, const float* freq, int R, int C, int P, float* emb,

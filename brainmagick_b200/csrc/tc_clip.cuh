@@ -1,4 +1,5 @@
-// K6: ClipLoss.get_scores (bm/losses.py:91-94) as ONE split-K tensor-core GEMM (3xTF32 wgmma engine of tc_common.cuh)
+// K6: ClipLoss.get_scores (bm/losses.py:91-94) as ONE split-K tensor-core GEMM (3xTF32 wgmma engine of tc_common.cuh, or
+// its single-pass TF32 form: passes = 1; the candidate norms stay fp64 sums of squares of the fp32 values either way)
 // followed by ONE finalize kernel (split reduction + 1/norm scale + row softmax / cross-entropy + batch mean,
 // bm/losses.py:97-114).
 //
@@ -164,7 +165,7 @@ inline long long clip_ws_floats(int Bn, int Bc, long long KT) {
 // scores [Bn][Bc] (+ inv_norm when !norms_given, + probs / row_loss / loss when requested)
 inline int launch_clip_scores(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
                               int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss,
-                              float* loss, float* ws, int* err, cudaStream_t st, bool det = false) {
+                              float* loss, float* ws, int passes, int* err, cudaStream_t st, bool det = false) {
     (void)err;
     const ClipGeom g = clip_geometry(Bn, Bc, KT);
     long long nP = (long long)g.ks * Bn * Bc;
@@ -188,7 +189,8 @@ inline int launch_clip_scores(const float* est, const float* cand, int Bn, int B
     }
     ClipOp o;
     o.E = est; o.C = cand; o.Bn = Bn; o.Bc = Bc; o.chunks = g.chunks; o.per_split = g.per_split; o.KT = KT; o.P = ws;
-    if (int rc = hg_launch<HG_BN>(o, dim3((Bc + HG_BN - 1) / HG_BN, (Bn + HG_BM - 1) / HG_BM, g.ks), st, __func__)) return rc;
+    if (int rc = hg_launch<HG_BN>(o, dim3((Bc + HG_BN - 1) / HG_BN, (Bn + HG_BM - 1) / HG_BM, g.ks), passes, st, __func__))
+        return rc;
     clip_finalize_kernel<<<Bn, 256, 0, st>>>(ws, ssp, g.ks, Bn, Bc, target_offset, inv_norm, scores, probs, row_loss,
                                              loss, counter);
     ++g_launches;

@@ -1,4 +1,5 @@
 // Hopper (sm_90a) tensor-core engine shared by the conv / weight-gradient / CLIP kernels: one 3xTF32 wgmma GEMM
+// (or, with the compile-time pass count PASSES = 1, its single-pass TF32 form: see below)
 //
 //     D[m][n] = sum_k A[m][k] * B[n][k]        (fp32 operands, fp32-faithful result)
 //
@@ -20,6 +21,12 @@
 //   * the block's products are accumulated in a fresh register tile and then added into the running fp32 sum with
 //     ordinary round-to-nearest FADDs.  The tensor core's internal accumulation truncates; chaining at most 12 MMAs per
 //     block keeps that bias below 1e-7 relative however long K is, with no correction factor to calibrate per GPU.
+//
+// Both main loops take the pass count as a template argument: PASSES = 3 is the form above (the library's default, 1e-4
+// parity with fp32), PASSES = 1 the TF32 form of the `_tf32` entry points (PyTorch's TF32 matmul precision): every fp32
+// operand element is rounded once to tf32 (round to nearest, ties away from zero: the `hi` piece of the split), the stages
+// hold no lo tiles, and ONE wgmma per k8 replaces the three.  The per-block fresh register tile and its round-to-nearest
+// adds into the running sum are kept, so the accumulation bias bound and the fixed reduction order do not change.
 #pragma once
 #include <cuda.h>
 #include <type_traits>
@@ -30,7 +37,7 @@ namespace bm {
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device): the attribute is per device, so a
 // process-wide flag would leave a second device of the same process without it.
 inline int ensure_dyn_smem(const void* func, int bytes) {
-    constexpr int kMaxDev = 64, kMaxFn = 16;
+    constexpr int kMaxDev = 64, kMaxFn = 32;
     static const void* fns[kMaxFn];
     static bool done[kMaxFn][kMaxDev];
     static int nfn = 0;
@@ -240,9 +247,12 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
 // ---------------------------------------------------------------------------------------------------
 constexpr int HG_BM = 128, HG_BN = 128, HG_BK = 32, HG_THREADS = 256;
 constexpr int HG_TILE_BYTES = 128 * HG_BK * 4;                        // 16 KB: 128 rows x 32 fp32
-// one stage: A hi | A lo (128 rows each) | B hi | B lo (BN rows each); double-buffered, 1 KB alignment slack
-template <int BN> constexpr int hg_stage_bytes() { return 2 * HG_TILE_BYTES + 2 * BN * HG_BK * 4; }
-template <int BN> constexpr int hg_smem_bytes() { return 2 * hg_stage_bytes<BN>() + 1024; }
+// one stage: A hi | A lo (128 rows each) | B hi | B lo (BN rows each), the lo tiles only when PASSES = 3; double-buffered,
+// 1 KB alignment slack
+template <int BN, int PASSES> constexpr int hg_stage_bytes() {
+    return (PASSES == 3 ? 2 : 1) * (HG_TILE_BYTES + BN * HG_BK * 4);
+}
+template <int BN, int PASSES> constexpr int hg_smem_bytes() { return 2 * hg_stage_bytes<BN, PASSES>() + 1024; }
 
 // The tile width for an output of n columns: 160 where it pads no more columns than 128 (320 columns: 2 exact tiles instead
 // of 3 with 64 padding columns), else 128.
@@ -254,7 +264,8 @@ inline int hg_pick_bn(long long n) {
 // Operand fetch, per tile of ROWS rows (128 for A, BN for B) and K block (ops implement a4 / b4 with the signature below):
 //   K-contiguous operand (Op::A_KCONTIG / B_KCONTIG):  v4(cta, kb, row, q) = elements k = 4q .. 4q+3 of tile row `row`
 //   M/N-contiguous operand:                            v4(cta, kb, k, q)   = tile rows 4q .. 4q+3 at reduction index k
-// Out-of-range elements (padding, tails, other samples) are returned as zeros.
+// Out-of-range elements (padding, tails, other samples) are returned as zeros.  store<PASSES> writes the tf32 pieces of a
+// float4 into the hi and lo tiles (PASSES = 3) or its rounded value into the hi tile alone (PASSES = 1: `lo` is not touched).
 template <bool KCONTIG, int ROWS>
 struct HgSlot {
     static constexpr int N4 = ROWS / 32;       // float4 moved per thread per tile
@@ -268,13 +279,14 @@ struct HgSlot {
             q = (w >> 2) * 4 + (lane >> 3);
         }
     }
+    template <int PASSES>
     __device__ static void store(uint8_t* hi, uint8_t* lo, int i, int q, float4 v) {
         if (KCONTIG) {
             float4 h, l;
             tf32_split(v.x, h.x, l.x); tf32_split(v.y, h.y, l.y); tf32_split(v.z, h.z, l.z); tf32_split(v.w, h.w, l.w);
             const int off = i * 128 + ((q ^ (i & 7)) << 4);
             *reinterpret_cast<float4*>(hi + off) = h;
-            *reinterpret_cast<float4*>(lo + off) = l;
+            if (PASSES == 3) *reinterpret_cast<float4*>(lo + off) = l;
         } else {
             const float e[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
@@ -284,7 +296,7 @@ struct HgSlot {
                 float h, l;
                 tf32_split(e[c], h, l);
                 *reinterpret_cast<float*>(hi + off) = h;
-                *reinterpret_cast<float*>(lo + off) = l;
+                if (PASSES == 3) *reinterpret_cast<float*>(lo + off) = l;
             }
         }
     }
@@ -299,9 +311,11 @@ __device__ __forceinline__ int hg_row(int i) {
 }
 __device__ __forceinline__ int hg_col(int i) { return 8 * (i >> 2) + 2 * (threadIdx.x & 3) + (i & 1); }
 
-template <class Op, int BN>
+template <class Op, int BN, int PASSES>
 __global__ void __launch_bounds__(HG_THREADS, 1) hg_gemm_kernel(const __grid_constant__ Op op) {
-    constexpr int NACC = BN / 2, STAGE = hg_stage_bytes<BN>(), B_TILE = BN * HG_BK * 4;
+    static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or single-pass TF32");
+    constexpr int NACC = BN / 2, STAGE = hg_stage_bytes<BN, PASSES>(), B_TILE = BN * HG_BK * 4;
+    constexpr int A_LO = HG_TILE_BYTES, B_HI = (PASSES == 3 ? 2 : 1) * HG_TILE_BYTES;   // tile offsets in a stage
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
@@ -332,13 +346,13 @@ __global__ void __launch_bounds__(HG_THREADS, 1) hg_gemm_kernel(const __grid_con
         for (int j = 0; j < SA::N4; ++j) {
             int i, q;
             SA::coords(tid, j, i, q);
-            SA::store(st, st + HG_TILE_BYTES, i, q, ra[j]);
+            SA::template store<PASSES>(st, st + A_LO, i, q, ra[j]);
         }
 #pragma unroll
         for (int j = 0; j < SB::N4; ++j) {
             int i, q;
             SB::coords(tid, j, i, q);
-            SB::store(st + 2 * HG_TILE_BYTES, st + 2 * HG_TILE_BYTES + B_TILE, i, q, rb[j]);
+            SB::template store<PASSES>(st + B_HI, st + B_HI + B_TILE, i, q, rb[j]);
         }
     };
 
@@ -355,17 +369,21 @@ __global__ void __launch_bounds__(HG_THREADS, 1) hg_gemm_kernel(const __grid_con
         const int s = kb & 1;
         if (kb + 1 < nkb) fetch(kb + 1);
         const uint32_t st = base_u32 + s * STAGE;
-        const uint32_t a_hi = st + wg * (HG_TILE_BYTES / 2), a_lo = a_hi + HG_TILE_BYTES;
-        const uint32_t b_hi = st + 2 * HG_TILE_BYTES, b_lo = b_hi + B_TILE;
+        const uint32_t a_hi = st + wg * (HG_TILE_BYTES / 2), a_lo = a_hi + A_LO;
+        const uint32_t b_hi = st + B_HI, b_lo = b_hi + B_TILE;
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < HG_BK / 8; ++kk) {
             const uint32_t off = kk * 32;                  // 8 tf32 = 32 bytes along K inside the swizzle span
-            const uint64_t dah = wgmma_desc_k_sw128(a_hi + off), dal = wgmma_desc_k_sw128(a_lo + off);
-            const uint64_t dbh = wgmma_desc_k_sw128(b_hi + off), dbl = wgmma_desc_k_sw128(b_lo + off);
-            wgmma_tf32<BN>(part, dal, dbh, kk != 0);
-            wgmma_tf32<BN>(part, dah, dbl, 1);
-            wgmma_tf32<BN>(part, dah, dbh, 1);
+            const uint64_t dah = wgmma_desc_k_sw128(a_hi + off), dbh = wgmma_desc_k_sw128(b_hi + off);
+            if constexpr (PASSES == 3) {
+                const uint64_t dal = wgmma_desc_k_sw128(a_lo + off), dbl = wgmma_desc_k_sw128(b_lo + off);
+                wgmma_tf32<BN>(part, dal, dbh, kk != 0);
+                wgmma_tf32<BN>(part, dah, dbl, 1);
+                wgmma_tf32<BN>(part, dah, dbh, 1);
+            } else {
+                wgmma_tf32<BN>(part, dah, dbh, kk != 0);
+            }
         }
         wgmma_commit();
         if (kb + 1 < nkb) stash(s ^ 1);                    // the other stage's MMAs completed in the previous iteration
@@ -378,21 +396,27 @@ __global__ void __launch_bounds__(HG_THREADS, 1) hg_gemm_kernel(const __grid_con
     op.template epilogue<BN>(cta, acc, 64 * wg);
 }
 
-template <int BN, class Op>
-inline int hg_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) {
-    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hg_gemm_kernel<Op, BN>), hg_smem_bytes<BN>())) return rc;
+template <int BN, int PASSES, class Op>
+inline int hg_run(const Op& op, dim3 grid, cudaStream_t st, const char* who) {
+    constexpr int SMEM = hg_smem_bytes<BN, PASSES>();
+    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hg_gemm_kernel<Op, BN, PASSES>), SMEM)) return rc;
     if (grid.x == 0 || grid.y == 0 || grid.z == 0) return 0;
     if (grid.y > 65535 || grid.z > 65535) return set_error(2, "%s: grid too large%s", who);
-    hg_gemm_kernel<Op, BN><<<grid, HG_THREADS, hg_smem_bytes<BN>(), st>>>(op);
+    hg_gemm_kernel<Op, BN, PASSES><<<grid, HG_THREADS, SMEM, st>>>(op);
     ++g_launches;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", who, cudaGetErrorString(e));
     return 0;
 }
+// passes: 3 (3xTF32) or 1 (single-pass TF32)
+template <int BN, class Op>
+inline int hg_launch(const Op& op, dim3 grid, int passes, cudaStream_t st, const char* who) {
+    return passes == 1 ? hg_run<BN, 1>(op, grid, st, who) : hg_run<BN, 3>(op, grid, st, who);
+}
 // the same with the tile width of hg_pick_bn
 template <class Op>
-inline int hg_launch_bn(int bn, const Op& op, dim3 grid, cudaStream_t st, const char* who) {
-    return bn == 160 ? hg_launch<160>(op, grid, st, who) : hg_launch<128>(op, grid, st, who);
+inline int hg_launch_bn(int bn, const Op& op, dim3 grid, int passes, cudaStream_t st, const char* who) {
+    return bn == 160 ? hg_launch<160>(op, grid, passes, st, who) : hg_launch<128>(op, grid, passes, st, who);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -409,21 +433,25 @@ inline int hg_launch_bn(int bn, const Op& op, dim3 grid, cudaStream_t st, const 
 //     `acc` with round-to-nearest FADDs per K block -- the pieces, MMA order and per-block adds of hg_gemm_kernel.
 // Shared-memory traffic per K block at BN = 160: A 16 KB written by TMA + 16 KB read, B hi/lo 40 KB written + 120 KB
 // read by the wgmmas (the register-staged loop also wrote A hi/lo and read A twice per MMA).
+// PASSES = 1 (single-pass TF32): the producer stores B's rounded value alone (the pre-split format reads only its hi
+// piece), the consumers round A in registers with cvt.rna and issue one wgmma per k8; B traffic: 20 KB written + 40 KB read.
 constexpr int HC_THREADS = 384, HC_CONSUMERS = 256, HC_STAGES = 3;
 constexpr int HC_PRODUCER_REGS = 104, HC_CONSUMER_REGS = 200;    // 104 * 128 + 200 * 256 = 168 * 384 registers
 constexpr int HC_ERR_FULL = 901, HC_ERR_EMPTY = 902;           // status codes of a timed-out consumer / producer wait
-// one stage: A raw fp32 (128 rows) | B hi | B lo (BN rows each), every tile 1 KB-aligned for the 128-byte swizzle
-template <int BN> constexpr int hc_stage_bytes() { return HG_TILE_BYTES + 2 * BN * HG_BK * 4; }
-template <int BN> constexpr int hc_smem_bytes() { return HC_STAGES * hc_stage_bytes<BN>() + 1024; }
+// one stage: A raw fp32 (128 rows) | B hi | B lo (BN rows each; no lo tile when PASSES = 1), every tile 1 KB-aligned for
+// the 128-byte swizzle
+template <int BN, int PASSES> constexpr int hc_stage_bytes() { return HG_TILE_BYTES + (PASSES == 3 ? 2 : 1) * BN * HG_BK * 4; }
+template <int BN, int PASSES> constexpr int hc_smem_bytes() { return HC_STAGES * hc_stage_bytes<BN, PASSES>() + 1024; }
 
 // index of a consumer thread in [0, 256) and a barrier over the consumer warpgroups only (the producer has exited)
 __device__ __forceinline__ int hc_consumer_tid() { return threadIdx.x - (HC_THREADS - HC_CONSUMERS); }
 __device__ __forceinline__ void hc_consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(HC_CONSUMERS) : "memory"); }
 
-template <class Op, int BN>
+template <class Op, int BN, int PASSES>
 __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_constant__ Op op,
                                                                const __grid_constant__ CUtensorMap xmap) {
-    constexpr int NACC = BN / 2, STAGE = hc_stage_bytes<BN>(), B_TILE = BN * HG_BK * 4;
+    static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or single-pass TF32");
+    constexpr int NACC = BN / 2, STAGE = hc_stage_bytes<BN, PASSES>(), B_TILE = BN * HG_BK * 4;
     extern __shared__ uint8_t smem_raw[];
     __shared__ alignas(8) uint64_t bars[2 * HC_STAGES];         // full[s], empty[s]
     const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -477,7 +505,7 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_con
                     for (int j = 0; j < PART; ++j) {
                         const int idx = tid + 128 * (p + j);
                         if (!((live >> (p + j)) & 1)) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-                        HgSlot<true, BN>::store(bh, bh + B_TILE, idx >> 3, idx & 7, v[j]);
+                        HgSlot<true, BN>::template store<PASSES>(bh, bh + B_TILE, idx >> 3, idx & 7, v[j]);
                     }
                 }
                 fence_proxy_async();                               // the generic-proxy stores, before the wgmmas read them
@@ -486,9 +514,13 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_con
             return true;
         };
         const int f = op.b_format();
-        const bool ok = f == Op::B_RAW     ? produce(std::integral_constant<int, Op::B_RAW>())
-                        : f == Op::B_SPLIT ? produce(std::integral_constant<int, Op::B_SPLIT>())
-                                           : produce(std::integral_constant<int, Op::B_F16>());
+        bool ok;
+        if constexpr (PASSES == 1)                      // raw or the hi piece of the split (rounding it again changes nothing);
+            ok = produce(std::integral_constant<int, Op::B_RAW>());     // the launcher refuses the fp16 pieces
+        else
+            ok = f == Op::B_RAW     ? produce(std::integral_constant<int, Op::B_RAW>())
+                 : f == Op::B_SPLIT ? produce(std::integral_constant<int, Op::B_SPLIT>())
+                                    : produce(std::integral_constant<int, Op::B_F16>());
         if (!ok && op.err) atomicCAS(op.err, 0, HC_ERR_EMPTY);
         return;
     }
@@ -506,24 +538,40 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_con
             return;
         }
         const float* at = reinterpret_cast<const float*>(smem + s * STAGE);
-        float hi[4][4], lo[4][4];                   // [k8][fragment element]
+        if constexpr (PASSES == 3) {
+            float hi[4][4], lo[4][4];               // [k8][fragment element]
 #pragma unroll
-        for (int kk = 0; kk < HG_BK / 8; ++kk) {
+            for (int kk = 0; kk < HG_BK / 8; ++kk) {
 #pragma unroll
-            for (int e = 0; e < 4; ++e) {           // element e: row r0 + 8 (e & 1), 16-byte chunk 2 kk + (e >> 1), word tq
-                const int r = r0 + 8 * (e & 1), q = 2 * kk + (e >> 1);
-                tf32_split(at[r * 32 + ((q ^ grp) << 2) + tq], hi[kk][e], lo[kk][e]);
+                for (int e = 0; e < 4; ++e) {       // element e: row r0 + 8 (e & 1), 16-byte chunk 2 kk + (e >> 1), word tq
+                    const int r = r0 + 8 * (e & 1), q = 2 * kk + (e >> 1);
+                    tf32_split(at[r * 32 + ((q ^ grp) << 2) + tq], hi[kk][e], lo[kk][e]);
+                }
             }
-        }
-        const uint32_t b_hi = base_u32 + s * STAGE + HG_TILE_BYTES, b_lo = b_hi + B_TILE;
-        wgmma_fence();
+            const uint32_t b_hi = base_u32 + s * STAGE + HG_TILE_BYTES, b_lo = b_hi + B_TILE;
+            wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < HG_BK / 8; ++kk) {
-            const uint32_t off = kk * 32;
-            const uint64_t dbh = wgmma_desc_k_sw128(b_hi + off), dbl = wgmma_desc_k_sw128(b_lo + off);
-            wgmma_tf32_rs<BN>(part, lo[kk], dbh, kk != 0);
-            wgmma_tf32_rs<BN>(part, hi[kk], dbl, 1);
-            wgmma_tf32_rs<BN>(part, hi[kk], dbh, 1);
+            for (int kk = 0; kk < HG_BK / 8; ++kk) {
+                const uint32_t off = kk * 32;
+                const uint64_t dbh = wgmma_desc_k_sw128(b_hi + off), dbl = wgmma_desc_k_sw128(b_lo + off);
+                wgmma_tf32_rs<BN>(part, lo[kk], dbh, kk != 0);
+                wgmma_tf32_rs<BN>(part, hi[kk], dbl, 1);
+                wgmma_tf32_rs<BN>(part, hi[kk], dbh, 1);
+            }
+        } else {
+            float a[4][4];                          // the same fragment, rounded once
+#pragma unroll
+            for (int kk = 0; kk < HG_BK / 8; ++kk) {
+#pragma unroll
+                for (int e = 0; e < 4; ++e) {
+                    const int r = r0 + 8 * (e & 1), q = 2 * kk + (e >> 1);
+                    a[kk][e] = tf32_rna(at[r * 32 + ((q ^ grp) << 2) + tq]);
+                }
+            }
+            const uint32_t b_hi = base_u32 + s * STAGE + HG_TILE_BYTES;
+            wgmma_fence();
+#pragma unroll
+            for (int kk = 0; kk < HG_BK / 8; ++kk) wgmma_tf32_rs<BN>(part, a[kk], wgmma_desc_k_sw128(b_hi + kk * 32), kk != 0);
         }
         wgmma_commit();
         wgmma_wait_all();
@@ -532,7 +580,7 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_con
 #pragma unroll
         for (int i = 0; i < NACC; ++i) acc[i] += part[i];
     }
-    op.template epilogue<BN>(cta, acc, 64 * cg);
+    op.template epilogue<BN, PASSES>(cta, acc, 64 * cg);
 }
 
 // x [B][T][Cin] fp32 as a 3D tensor map with a [1][128][32] box, 128-byte swizzle, zero fill out of bounds
@@ -560,22 +608,28 @@ inline int hc_x_map(CUtensorMap* m, const float* x, int B, int T, int Cin, const
     return 0;
 }
 
-template <int BN, class Op>
+template <int BN, int PASSES, class Op>
 inline int hc_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) {
-    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hc_conv_kernel<Op, BN>), hc_smem_bytes<BN>())) return rc;
+    constexpr int SMEM = hc_smem_bytes<BN, PASSES>();
+    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hc_conv_kernel<Op, BN, PASSES>), SMEM)) return rc;
     if (grid.x == 0 || grid.y == 0 || grid.z == 0) return 0;
     if (grid.y > 65535 || grid.z > 65535) return set_error(2, "%s: grid too large%s", who);
     CUtensorMap xmap;
     if (int rc = hc_x_map(&xmap, op.x, op.B, op.T, op.Cin, who)) return rc;
-    hc_conv_kernel<Op, BN><<<grid, HC_THREADS, hc_smem_bytes<BN>(), st>>>(op, xmap);
+    hc_conv_kernel<Op, BN, PASSES><<<grid, HC_THREADS, SMEM, st>>>(op, xmap);
     ++g_launches;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", who, cudaGetErrorString(e));
     return 0;
 }
+// the tile width of hg_pick_bn and the pass count op.passes (3 or 1; the fp16-piece weights only with 3)
 template <class Op>
 inline int hc_launch_bn(int bn, const Op& op, dim3 grid, cudaStream_t st, const char* who) {
-    return bn == 160 ? hc_launch<160>(op, grid, st, who) : hc_launch<128>(op, grid, st, who);
+    if (op.passes == 1) {
+        if (!op.w) return set_error(2, "%s: the single-pass form takes fp32 weights%s", who);
+        return bn == 160 ? hc_launch<160, 1>(op, grid, st, who) : hc_launch<128, 1>(op, grid, st, who);
+    }
+    return bn == 160 ? hc_launch<160, 3>(op, grid, st, who) : hc_launch<128, 3>(op, grid, st, who);
 }
 
 // the plain epilogue: D[z plane][row][col] = acc for rows < rows, cols < cols (row-major, leading dimension ld)

@@ -1,5 +1,5 @@
 // K3/K4/K5 on the Hopper tensor cores: dilated Conv1d (and its data gradient, and the 1x1 head / subject layers) as an
-// implicit GEMM on the 3xTF32 wgmma engine of tc_common.cuh.
+// implicit GEMM on the 3xTF32 wgmma engine of tc_common.cuh (or its single-pass TF32 form: ConvOp::passes = 1).
 //
 //   y[b, t, n] = bias[n] + sum_{tap} sum_{k} x[b, t + shift(tap), k] * W[wset(b)][tap][n][k]      (channels-last x, y)
 //
@@ -57,6 +57,7 @@ struct ConvOp {
     unsigned int* out_amax;               // max |GELU / GLU output| (float bits) or null
     int act, out_tmajor;
     int* err;
+    int passes;                           // 3: 3xTF32, 1: single-pass TF32 (reads w alone; not with the fp16 pieces)
 
     struct Cta { int b, t0, n_tile, wbase; float w_inv; };
     template <int BN> __device__ Cta cta() const {
@@ -117,8 +118,9 @@ struct ConvOp {
         return make_float4((h0.x + l0.x) * c.w_inv, (h0.y + l0.y) * c.w_inv, (h1.x + l1.x) * c.w_inv, (h1.y + l1.y) * c.w_inv);
     }
 
-    // run by the 256 consumer threads of hc_conv_kernel
-    template <int BN> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+    // run by the 256 consumer threads of hc_conv_kernel; PASSES only gives each kernel instantiation its own col_sums (a
+    // static shared array shared by the 3- and 1-pass kernels would change the shared-memory layout of both)
+    template <int BN, int PASSES> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
         __shared__ double col_sums[2 * BN];
         float am = 0.f;
         if (glu) {
@@ -201,7 +203,7 @@ struct ConvOp {
 struct SensorMixBwdOp : ConvOp {
     int C;
     const float* mask;
-    template <int BN> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+    template <int BN, int PASSES> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
 #pragma unroll
         for (int g = 0; g < BN / 8; ++g) {
 #pragma unroll
@@ -224,6 +226,7 @@ inline ConvOp conv_op_defaults() {
     ConvOp o;
     memset(&o, 0, sizeof(o));
     o.n_wsets = 1;
+    o.passes = 3;
     return o;
 }
 
@@ -272,8 +275,9 @@ inline bool conv_tc_supported(int T, int Cin, int Ntot, int Kw, int glu) {
 }
 
 // x [B,T,Cin]; w_hi / w_lo [Kw][Ntot][Cin] (wsel: [n_wsets][Kw][Ntot][Cin]), the tf32 pieces of bm_tc_weight_split
+// (passes = 1: w_hi alone is read, w_lo may be null)
 struct ConvTcP {
-    int B, T, Cin, Ntot, taps, dilation, sign, glu, act, out_tmajor;
+    int B, T, Cin, Ntot, taps, dilation, sign, glu, act, out_tmajor, passes;
     const float* bias; const float* addend;
     float* y; float* aux; float* glu_out;
     int n_wsets; const int* wsel;
@@ -284,18 +288,19 @@ inline int launch_conv_tc(const float* x, const float* w_hi, const float* w_lo, 
     o.x = x; o.w = w_hi; o.w_lo32 = w_lo; o.B = p.B; o.T = p.T; o.Cin = p.Cin; o.Ntot = p.Ntot; o.taps = p.taps; o.dilation = p.dilation;
     o.sign = p.sign; o.glu = p.glu; o.n_wsets = p.wsel ? p.n_wsets : 1; o.wsel = p.wsel; o.bias = p.bias;
     o.addend = p.addend; o.y = p.y; o.aux = p.aux; o.glu_out = p.glu_out; o.act = p.act; o.out_tmajor = p.out_tmajor;
-    o.err = p.err;
+    o.err = p.err; o.passes = p.passes;
     return launch_conv_op(o, st, __func__);
 }
 
-// du [B,T,Op]; w_hi / w_lo [n_sets][Cp][Op] (tf32 pieces); dmeg [B,C,T] with C <= Cp; mask [C] or null
+// du [B,T,Op]; w_hi / w_lo [n_sets][Cp][Op] (tf32 pieces; passes = 1: w_hi alone); dmeg [B,C,T] with C <= Cp; mask [C]
+// or null
 inline int launch_sensor_mix_bwd_tc(const float* du, const float* w_hi, const float* w_lo, const int* wsel, int n_sets,
-                                    const float* mask, int B, int T, int Op, int Cp, int C, float* dmeg, int* err,
-                                    cudaStream_t st) {
+                                    const float* mask, int B, int T, int Op, int Cp, int C, float* dmeg, int passes,
+                                    int* err, cudaStream_t st) {
     SensorMixBwdOp o;
     memset(&o, 0, sizeof(o));
     o.x = du; o.w = w_hi; o.w_lo32 = w_lo; o.B = B; o.T = T; o.Cin = Op; o.Ntot = Cp; o.taps = 1; o.dilation = 1; o.sign = 1;
-    o.n_wsets = n_sets; o.wsel = wsel; o.y = dmeg; o.err = err; o.C = C; o.mask = mask;
+    o.n_wsets = n_sets; o.wsel = wsel; o.y = dmeg; o.err = err; o.C = C; o.mask = mask; o.passes = passes;
     if ((long long)B * T >= (1ll << 31)) return set_error(2, "%s: too many rows%s", __func__);
     o.ttiles = (T + HG_BM - 1) / HG_BM;
     const int bn = hg_pick_bn(Cp);

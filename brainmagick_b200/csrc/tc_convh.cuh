@@ -85,6 +85,7 @@ inline int launch_conv_hp(const ConvHPArgs& h, cudaStream_t st) {
     if (a.out_tmajor && (a.act || a.accumulate)) return set_error(2, "%s: channel-major output is a plain store%s", __func__);
     if (a.act && a.accumulate) return set_error(2, "%s: accumulate excludes the activation%s", __func__);
     ConvOp o = conv_pp_op(a);
+    o.passes = 3;                    // the fp16-piece entry points have no single-pass form
     o.w = nullptr;
     o.w_hi = reinterpret_cast<const __half*>(h.w_hi); o.w_lo = reinterpret_cast<const __half*>(h.w_lo); o.w_amax = h.w_amax;
     o.out_amax = reinterpret_cast<unsigned int*>(h.out_amax);

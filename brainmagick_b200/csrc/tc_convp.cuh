@@ -21,6 +21,7 @@ struct ConvPPArgs {
     const float* x; const float* w_raw; const float* bias;
     int B, T, Cin, Ntot, taps, dilation, sign;
     int glu, act, out_tmajor, accumulate;     // accumulate: y += conv (in place)
+    int passes;                               // 3: 3xTF32, 1: single-pass TF32
     float* y; float* aux; float* glu_out; double* stats; int* err;
 };
 
@@ -29,7 +30,7 @@ inline ConvOp conv_pp_op(const ConvPPArgs& a) {
     o.x = a.x; o.w = a.w_raw; o.bias = a.bias; o.B = a.B; o.T = a.T; o.Cin = a.Cin; o.Ntot = a.Ntot; o.taps = a.taps;
     o.dilation = a.dilation; o.sign = a.sign; o.glu = a.glu; o.act = a.act; o.out_tmajor = a.out_tmajor;
     o.addend = a.accumulate ? a.y : nullptr; o.y = a.y; o.aux = a.act ? a.aux : nullptr; o.glu_out = a.glu_out;
-    o.stats = a.stats; o.err = a.err;
+    o.stats = a.stats; o.err = a.err; o.passes = a.passes;
     return o;
 }
 

@@ -1,4 +1,5 @@
-// ClipLoss backward contractions (bm/losses.py:91-114 differentiated, SURVEY.md A.6) on the 3xTF32 wgmma engine:
+// ClipLoss backward contractions (bm/losses.py:91-114 differentiated, SURVEY.md A.6) on the 3xTF32 wgmma engine (or its
+// single-pass TF32 form: passes = 1):
 //
 //     D[m][n] = sum_k A[m][k] * B[k][n]        A [M][K] row-major (K contiguous), B [K][N] row-major (N contiguous)
 //
@@ -38,10 +39,11 @@ inline bool gemm_nt_pp_supported(int M, int N, int K) {
 }
 
 // D [M][N] = A [M][K] * B [K][N], all row-major fp32
-inline int launch_gemm_nt_pp(const float* A, const float* B, float* D, int M, int N, int K, int* err, cudaStream_t st) {
+inline int launch_gemm_nt_pp(const float* A, const float* B, float* D, int M, int N, int K, int passes, int* err,
+                             cudaStream_t st) {
     (void)err;
     GemmNTOp o{A, B, D, M, N, K};
-    return hg_launch<HG_BN>(o, dim3((N + HG_BN - 1) / HG_BN, (M + HG_BM - 1) / HG_BM, 1), st, __func__);
+    return hg_launch<HG_BN>(o, dim3((N + HG_BN - 1) / HG_BN, (M + HG_BM - 1) / HG_BM, 1), passes, st, __func__);
 }
 
 }  // namespace tc

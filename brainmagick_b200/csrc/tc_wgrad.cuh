@@ -1,4 +1,5 @@
-// Weight gradients on the tensor cores (3xTF32 wgmma engine of tc_common.cuh):  for one tap shift s
+// Weight gradients on the tensor cores (3xTF32 wgmma engine of tc_common.cuh, or its single-pass TF32 form: passes = 1):
+// for one tap shift s
 //
 //     P[ks][m][n] = sum_{b in split ks} sum_t  dY[b, t, m] * X[b, t + s, n]          (dY, X channels-last)
 //
@@ -105,7 +106,8 @@ struct WgradOp {
 
 // dY [B,T,M], X [B,T,N] -> dW [M][Ntrue][taps]; ws: wgrad_workspace_floats() floats
 inline int launch_wgrad_tc(const float* dY, const float* X, int B, int T, int M, int N, int Ntrue, int taps,
-                           int dilation, float* ws, float* dW, int* err, cudaStream_t st, float* dbias = nullptr) {
+                           int dilation, float* ws, float* dW, int passes, int* err, cudaStream_t st,
+                           float* dbias = nullptr) {
     (void)err;
     int nh, mblocks, ksplit, bchunk;
     wgrad_geometry(B, M, N, taps, &nh, &mblocks, &ksplit, &bchunk);
@@ -119,7 +121,7 @@ inline int launch_wgrad_tc(const float* dY, const float* X, int B, int T, int M,
     o.P = direct ? dW : ws;
     o.plane = (long long)(direct ? M : Mpad) * N;
     o.rows = direct ? M : Mpad;
-    if (int rc = hg_launch_bn(bn, o, dim3(o.ntiles * taps, mblocks, ksplit), st, __func__)) return rc;
+    if (int rc = hg_launch_bn(bn, o, dim3(o.ntiles * taps, mblocks, ksplit), passes, st, __func__)) return rc;
     if (dbias) {               // bias gradient sum_{b,t} dY[b,t,m]
         cudaError_t em = cudaMemsetAsync(dbias, 0, sizeof(float) * M, st);
         if (em != cudaSuccess) return set_error(3, "%s: memset: %s", __func__, cudaGetErrorString(em));
@@ -140,7 +142,7 @@ inline int launch_wgrad_tc(const float* dY, const float* X, int B, int T, int M,
 // grouped pointwise weight gradient: out[g][m][n] = sum_{b in group g} sum_t dY[b,t,m] X[b,t,n]; out is [G][Mpad][N] with
 // Mpad = ceil(M/128)*128 (rows >= M are zero); groups given as CSR (zlist, seg_off[G+1]) over the samples.
 inline int launch_wgrad_tc_grouped(const float* dY, const float* X, const int* zlist, const int* seg_off, int G, int B,
-                                   int T, int M, int N, float* out, int* err, cudaStream_t st) {
+                                   int T, int M, int N, float* out, int passes, int* err, cudaStream_t st) {
     (void)err;
     if (wgrad_pick_nh(N) == 0) return set_error(2, "%s: unsupported N%s", __func__);
     if (G > 65535) return set_error(2, "%s: too many groups%s", __func__);
@@ -151,7 +153,7 @@ inline int launch_wgrad_tc_grouped(const float* dY, const float* X, const int* z
     o.P = out; o.plane = (long long)mblocks * WG_BM * N; o.rows = mblocks * WG_BM;
     // 128 columns: one CTA per (tile, group) and no K-slice count to raise, so fewer, wider tiles fill the waves worse
     // (27 groups of 320 x 320: 162 CTAs at 160, a second wave of 30 on 132 SMs, ran slower than 243 at 128)
-    return hg_launch<HG_BN>(o, dim3(o.ntiles, mblocks, G), st, __func__);
+    return hg_launch<HG_BN>(o, dim3(o.ntiles, mblocks, G), passes, st, __func__);
 }
 
 }  // namespace tc

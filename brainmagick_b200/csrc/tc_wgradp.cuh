@@ -1,4 +1,4 @@
-// Weight gradient of a (dilated) k-tap conv (3xTF32 wgmma engine of tc_common.cuh):
+// Weight gradient of a (dilated) k-tap conv (3xTF32 wgmma engine of tc_common.cuh, or its single-pass TF32 form):
 //
 //     dW[m][n][tap] = sum_p dY[p, m] * X[p + shift(tap), n]          p = b*T + t flattened rows, channels-last operands
 //
@@ -108,7 +108,7 @@ inline size_t wgradp_workspace_floats(int B, int T, int Mdy, int Nx, int taps) {
 
 // dY [B,T,Mdy], X [B,T,Nx] channels-last -> dW [Mdy][Ntrue][taps]; ws: wgradp_workspace_floats() floats
 inline int launch_wgrad_pp(const float* dY, const float* X, int B, int T, int Mdy, int Nx, int Ntrue, int taps,
-                           int dilation, float* ws, float* dW, int* err, cudaStream_t st) {
+                           int dilation, float* ws, float* dW, int passes, int* err, cudaStream_t st) {
     (void)err;
     const WgradPPGeom g = wgradp_geometry(B, T, Mdy, Nx, taps);
     const long long R = (long long)B * T;
@@ -117,7 +117,7 @@ inline int launch_wgrad_pp(const float* dY, const float* X, int B, int T, int Md
     o.R = (int)R; o.T = T; o.Mdy = Mdy; o.Nx = Nx; o.taps = taps; o.dilation = dilation; o.rows = g.rows;
     o.per_split = g.per_split; o.chunks = g.chunks; o.dY = dY; o.X = X; o.P = ws; o.rows_pad = g.mtiles * 256;
     const dim3 grid((Mdy + g.bn - 1) / g.bn, o.rows_pad / HG_BM, g.ks);
-    if (int rc = hg_launch_bn(g.bn, o, grid, st, __func__)) return rc;
+    if (int rc = hg_launch_bn(g.bn, o, grid, passes, st, __func__)) return rc;
     wgradp_reduce_kernel<<<ew_grid((long long)Mdy * Ntrue * taps), 256, 0, st>>>(ws, dW, taps, g.ks, o.rows_pad, Mdy, Nx,
                                                                                 Ntrue);
     ++g_launches;
@@ -131,7 +131,7 @@ inline int launch_wgrad_pp(const float* dY, const float* X, int B, int T, int Md
 inline int launch_wgrad_hp(const float* dY, const float* dy_amax, const float* X, const float* x_amax, int B, int T, int Mdy,
                            int Nx, int Ntrue, int taps, int dilation, float* ws, float* dW, int* err, cudaStream_t st) {
     (void)dy_amax; (void)x_amax;
-    return launch_wgrad_pp(dY, X, B, T, Mdy, Nx, Ntrue, taps, dilation, ws, dW, err, st);
+    return launch_wgrad_pp(dY, X, B, T, Mdy, Nx, Ntrue, taps, dilation, ws, dW, 3, err, st);
 }
 
 }  // namespace tc

@@ -8,7 +8,8 @@ flashy.distrib.sync_model expect), and on `meg` when it requires grad (gradient-
 
 Kernel selection is by shape only: contractions whose channel counts fit the tensor-core tiling (K % 32 == 0 and an
 N tile of 64..160 dividing N -- every layer of the real clip_conv model) run on the tensor-core kernels
-(3xTF32, `bm_tc_*`); other shapes (the tiny unit-test models) run on the FP32-FMA kernels of the same library.
+(3xTF32, `bm_tc_*`; single-pass TF32 when PyTorch's float32 matmul precision allows TF32, see `_tc_call`); other shapes
+(the tiny unit-test models) run on the FP32-FMA kernels of the same library.
 """
 from __future__ import annotations
 
@@ -123,6 +124,23 @@ def _reducing_call(name, like, ws_dims, *args, reduces=True):
     return call(name + "_det", *args[:-1], ptr(ws), ws.numel(), args[-1])
 
 
+# ---- TF32 forms -----------------------------------------------------------------------------------------------------
+# Under TF32 matmul precision (`_lib.tf32()`: torch.set_float32_matmul_precision("high"), matmul.allow_tf32 = True, ...) every
+# tensor-core contraction takes its single-pass `_tf32` form (include/bm_b200.h), with the same arguments.  The FP32-FMA
+# kernels stay exact (TF32 is permitted, not required) and the fp16-piece entry points keep their one form.
+_DET_SAME_ARGS = ("bm_clip_scores", "bm_clip_loss_fwd")      # tensor-core entry points with a `_det` form of the same arguments
+
+
+def _tc_call(name, *args):
+    """call(name[_det][_tf32], *args) for a tensor-core entry point: its `_det` form under the determinism flag where it has
+    one, then the `_tf32` form under TF32 matmul precision."""
+    if name in _DET_SAME_ARGS and _lib.deterministic():
+        name += "_det"
+    if _lib.tf32():
+        name += "_tf32"
+    return call(name, *args)
+
+
 def col_sum(x, rows, C, out, st):
     """out[c] = sum_r x[r, c] (bm_col_sum, or bm_col_sum_det under the determinism flag)."""
     if _lib.deterministic():
@@ -166,14 +184,15 @@ def tc_wgrad(dy, x, B, T, M, N, Ntrue, kw, dilation, status, dbias=None, dy_amax
             call("bm_tc_wgrad_conv_f16", ptr(dy), ptr(dy_amax), ptr(x), ptr(x_amax), B, T, M, N, Ntrue, kw, dilation, ptr(ws),
                  ptr(dw), ptr(status), stream())
         else:
-            call("bm_tc_wgrad_conv", ptr(dy), ptr(x), B, T, M, N, Ntrue, kw, dilation, ptr(ws), ptr(dw), ptr(status), stream())
+            _tc_call("bm_tc_wgrad_conv", ptr(dy), ptr(x), B, T, M, N, Ntrue, kw, dilation, ptr(ws), ptr(dw), ptr(status),
+                     stream())
         if dbias is not None:
             col_sum(dy, B * T, M, dbias, stream())
         return dw
     ws = _empty((int(lib.bm_tc_wgrad_workspace(B, M, N, kw)),), dy)
     det = _lib.deterministic()                # the kernel's own bias reduction is atomic: a fixed-order column sum instead
-    call("bm_tc_wgrad", ptr(dy), ptr(x), B, T, M, N, Ntrue, kw, dilation, ptr(ws), ptr(dw), None if det else ptr(dbias),
-         ptr(status), stream())
+    _tc_call("bm_tc_wgrad", ptr(dy), ptr(x), B, T, M, N, Ntrue, kw, dilation, ptr(ws), ptr(dw), None if det else ptr(dbias),
+             ptr(status), stream())
     if det and dbias is not None:
         col_sum(dy, B * T, M, dbias, stream())
     return dw
@@ -286,12 +305,12 @@ class _Conv:
             return out_amax
         elif pp:
             assert addend is None or addend.data_ptr() == y.data_ptr(), "the persistent kernel accumulates in place only"
-            call("bm_tc_conv1d_persistent", ptr(x), ptr(hi), ptr(bias), 0 if addend is None else 1, B, T, cin, ntot,
-                 self.kw, dilation, sign, glu, act, tmajor, ptr(y), ptr(aux), ptr(glu_out), ptr(stats), ptr(status), st)
+            _tc_call("bm_tc_conv1d_persistent", ptr(x), ptr(hi), ptr(bias), 0 if addend is None else 1, B, T, cin, ntot,
+                     self.kw, dilation, sign, glu, act, tmajor, ptr(y), ptr(aux), ptr(glu_out), ptr(stats), ptr(status), st)
         else:
             assert stats is None
-            call("bm_tc_conv1d", ptr(x), ptr(hi), ptr(lo), ptr(bias), ptr(addend), B, T, cin, ntot, self.kw, dilation,
-                 sign, glu, act, tmajor, ptr(y), ptr(aux), ptr(glu_out), None, ptr(status), st)
+            _tc_call("bm_tc_conv1d", ptr(x), ptr(hi), ptr(lo), ptr(bias), ptr(addend), B, T, cin, ntot, self.kw, dilation,
+                     sign, glu, act, tmajor, ptr(y), ptr(aux), ptr(glu_out), None, ptr(status), st)
         return None                        # the tf32 kernels do not report max |output|
 
     # y = conv(x) (+bias); optionally BatchNorm statistics into `stats`
@@ -494,8 +513,8 @@ def _sensor_mix_bwd_data(plan: "EncoderPlan", s, du, dims, status) -> torch.Tens
         att_t[:, :C, :O] = att.transpose(1, 2)
         w_hi, w_lo = _empty((R * Cp, Op), meg), _empty((R * Cp, Op), meg)
         call("bm_tc_weight_split", ptr(att_t), R * Cp, Op, 1, ptr(w_hi), ptr(w_lo), None, None, st)
-        call("bm_tc_sensor_mix_bwd_data", ptr(du), ptr(w_hi), ptr(w_lo), ptr(plan.rec_of_sample), R, ptr(plan.channel_mask),
-             B, T, Op, Cp, C, ptr(dmeg), ptr(status), st)
+        _tc_call("bm_tc_sensor_mix_bwd_data", ptr(du), ptr(w_hi), ptr(w_lo), ptr(plan.rec_of_sample), R,
+                 ptr(plan.channel_mask), B, T, Op, Cp, C, ptr(dmeg), ptr(status), st)
     else:
         call("bm_sensor_mix_bwd_data", ptr(du), Op, ptr(att), ptr(plan.rec_of_sample), ptr(plan.channel_mask), B, C, T, O,
              ptr(dmeg), st)
@@ -655,8 +674,8 @@ class _EncoderFn(torch.autograd.Function):
                     att_pad[:, :O, :C] = att
                     aw_hi, aw_lo = _empty((R * Op, Cp), meg), _empty((R * Op, Cp), meg)
                     call("bm_tc_weight_split", ptr(att_pad), R * Op, Cp, 1, ptr(aw_hi), ptr(aw_lo), None, None, st)
-                    call("bm_tc_pointwise_sel", ptr(megT), ptr(aw_hi), ptr(aw_lo), ptr(plan.rec_of_sample), R, B, T, Cp, Op,
-                         ptr(u), ptr(status), st)
+                    _tc_call("bm_tc_pointwise_sel", ptr(megT), ptr(aw_hi), ptr(aw_lo), ptr(plan.rec_of_sample), R, B, T, Cp,
+                             Op, ptr(u), ptr(status), st)
                 else:
                     call("bm_sensor_mix_fwd", ptr(meg), ptr(att), ptr(plan.rec_of_sample), B, C, T, O, Op, ptr(u), st)
                 il_conv.forward(u, bpad, B, T, 1, v, None, status)
@@ -667,8 +686,8 @@ class _EncoderFn(torch.autograd.Function):
                     mt = subj_pad.transpose(1, 2).contiguous()
                     sf_hi, sf_lo = _empty((S * Dp, ILp), meg), _empty((S * Dp, ILp), meg)
                     call("bm_tc_weight_split", ptr(mt), S * Dp, ILp, 1, ptr(sf_hi), ptr(sf_lo), None, None, st)
-                    call("bm_tc_pointwise_sel", ptr(v), ptr(sf_hi), ptr(sf_lo), ptr(plan.subject), S, B, T, ILp, Dp, ptr(x),
-                         ptr(status), st)
+                    _tc_call("bm_tc_pointwise_sel", ptr(v), ptr(sf_hi), ptr(sf_lo), ptr(plan.subject), S, B, T, ILp, Dp,
+                             ptr(x), ptr(status), st)
                 else:
                     subj_pad = None
                     call("bm_subject_layers_fwd", ptr(v), ILp, ptr(subj_w.contiguous()), ptr(plan.subject), B, T, IL, D, Dp,
@@ -1052,13 +1071,13 @@ class _EncoderFn(torch.autograd.Function):
                         sb_hi, sb_lo = _empty((S * ILp, Dp), meg), _empty((S * ILp, Dp), meg)
                         call("bm_tc_weight_split", ptr(subj_pad), S * ILp, Dp, 1, ptr(sb_hi), ptr(sb_lo), None, None, st)
                         dv = _empty((B, T, ILp), meg)
-                        call("bm_tc_pointwise_sel", ptr(g), ptr(sb_hi), ptr(sb_lo), ptr(plan.subject), S, B, T, Dp, ILp,
-                             ptr(dv), ptr(status), st)
+                        _tc_call("bm_tc_pointwise_sel", ptr(g), ptr(sb_hi), ptr(sb_lo), ptr(plan.subject), S, B, T, Dp, ILp,
+                                 ptr(dv), ptr(status), st)
                     if n_subj:
                         mpad = _round_up(ILp, 128)
                         dm = _empty((S, mpad, Dp), meg)
-                        call("bm_tc_wgrad_grouped", ptr(s["v"]), ptr(g), ptr(subj_order), ptr(subj_off), S, B, T, ILp, Dp,
-                             ptr(dm), ptr(status), st)
+                        _tc_call("bm_tc_wgrad_grouped", ptr(s["v"]), ptr(g), ptr(subj_order), ptr(subj_off), S, B, T, ILp,
+                                 Dp, ptr(dm), ptr(status), st)
                         d_subj = dm[:, :IL, :D].contiguous()
                 else:
                     if want_dv:
@@ -1083,8 +1102,8 @@ class _EncoderFn(torch.autograd.Function):
                     megT = s["megT"]
                     Cp = megT.shape[2]
                     dwp = _empty((R, _round_up(Op, 128), Cp), meg)
-                    call("bm_tc_wgrad_grouped", ptr(du), ptr(megT), ptr(plan.rec_order), ptr(plan.rec_off), R, B, T, Op, Cp,
-                         ptr(dwp), ptr(status), st)
+                    _tc_call("bm_tc_wgrad_grouped", ptr(du), ptr(megT), ptr(plan.rec_order), ptr(plan.rec_off), R, B, T, Op,
+                             Cp, ptr(dwp), ptr(status), st)
                     d_att = dwp[:, :O, :C].contiguous()
                 else:
                     call("bm_sensor_mix_bwd", ptr(du), Op, ptr(meg), ptr(plan.rec_order), ptr(plan.rec_off), B, C, T, O, R,
@@ -1177,8 +1196,8 @@ def clip_scores(estimates: torch.Tensor, candidates: torch.Tensor, want_probs: b
     scores = _empty((Bn, Bc), est)
     probs = _empty((Bn, Bc), est) if want_probs else None
     ws = _clip_workspace(est, Bn, Bc, KT)
-    _reducing_call("bm_clip_scores", est, None, ptr(est), ptr(cand), Bn, Bc, KT, 0, ptr(inv), ptr(scores), ptr(probs), ptr(ws),
-                   ws.numel(), ptr(tc_status_tensor(est.device)), stream())
+    _tc_call("bm_clip_scores", ptr(est), ptr(cand), Bn, Bc, KT, 0, ptr(inv), ptr(scores), ptr(probs), ptr(ws), ws.numel(),
+             ptr(tc_status_tensor(est.device)), stream())
     return probs if want_probs else scores
 
 
@@ -1197,8 +1216,8 @@ class _ClipScoresFn(torch.autograd.Function):
         scores = _empty((Bn, Bc), est)
         probs = _empty((Bn, Bc), est) if want_probs else None
         ws = _clip_workspace(est, Bn, Bc, KT)
-        _reducing_call("bm_clip_scores", est, None, ptr(est), ptr(cand), Bn, Bc, KT, 0, ptr(inv), ptr(scores), ptr(probs),
-                       ptr(ws), ws.numel(), ptr(tc_status_tensor(est.device)), stream())
+        _tc_call("bm_clip_scores", ptr(est), ptr(cand), Bn, Bc, KT, 0, ptr(inv), ptr(scores), ptr(probs), ptr(ws),
+                 ws.numel(), ptr(tc_status_tensor(est.device)), stream())
         ctx.save_for_backward(est, cand, inv, scores, probs)
         ctx.meta = (Bn, Bc, KT, estimate.shape, candidate.shape)
         return probs if want_probs else scores
@@ -1218,8 +1237,8 @@ class _ClipScoresFn(torch.autograd.Function):
         dcand = _empty(cand_shape, est) if ctx.needs_input_grad[1] else None
         G = _empty((Bn, Bc), est)
         coef = _empty((Bc,), est) if dcand is not None else None
-        call("bm_clip_scores_bwd", ptr(dscores), ptr(scores), ptr(inv), ptr(est), ptr(cand), Bn, Bc, KT, ptr(G), ptr(coef),
-             ptr(dest), ptr(dcand), ptr(tc_status_tensor(est.device)), st)
+        _tc_call("bm_clip_scores_bwd", ptr(dscores), ptr(scores), ptr(inv), ptr(est), ptr(cand), Bn, Bc, KT, ptr(G),
+                 ptr(coef), ptr(dest), ptr(dcand), ptr(tc_status_tensor(est.device)), st)
         return dest, dcand, None
 
 
@@ -1249,8 +1268,8 @@ def clip_scores_prenormed(estimates: torch.Tensor, candidates: torch.Tensor, inv
     assert cand[0].numel() == KT and inv_norms.numel() == Bc
     scores = _empty((Bn, Bc), est)
     ws = _clip_workspace(est, Bn, Bc, KT)
-    _reducing_call("bm_clip_scores", est, None, ptr(est), ptr(cand), Bn, Bc, KT, 1, ptr(inv_norms), ptr(scores), None,
-                   ptr(ws), ws.numel(), ptr(tc_status_tensor(est.device)), stream())
+    _tc_call("bm_clip_scores", ptr(est), ptr(cand), Bn, Bc, KT, 1, ptr(inv_norms), ptr(scores), None, ptr(ws), ws.numel(),
+             ptr(tc_status_tensor(est.device)), stream())
     return scores
 
 
@@ -1268,9 +1287,8 @@ class _ClipLossFn(torch.autograd.Function):
         row_loss = _empty((Bn,), est)
         loss = _empty((1,), est)
         ws = _clip_workspace(est, Bn, Bc, KT)
-        _reducing_call("bm_clip_loss_fwd", est, None, ptr(est), ptr(cand), Bn, Bc, KT, int(target_offset), ptr(inv),
-                       ptr(scores), ptr(probs), ptr(row_loss), ptr(loss), ptr(ws), ws.numel(),
-                       ptr(tc_status_tensor(est.device)), stream())
+        _tc_call("bm_clip_loss_fwd", ptr(est), ptr(cand), Bn, Bc, KT, int(target_offset), ptr(inv), ptr(scores),
+                 ptr(probs), ptr(row_loss), ptr(loss), ptr(ws), ws.numel(), ptr(tc_status_tensor(est.device)), stream())
         if candidate.requires_grad:      # a trainable feature model produced the candidates (solver.py:304-320)
             ctx.save_for_backward(probs, inv, cand, scores, est)
         else:
@@ -1289,15 +1307,15 @@ class _ClipLossFn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             G = _empty((Bn, Bc), probs)
             dest = _empty(shape, probs)
-            call("bm_clip_loss_bwd", ptr(probs), ptr(inv), ptr(cand), ptr(gout), Bn, Bc, KT, off, ptr(G), ptr(dest),
-                 ptr(status), stream())
+            _tc_call("bm_clip_loss_bwd", ptr(probs), ptr(inv), ptr(cand), ptr(gout), Bn, Bc, KT, off, ptr(G), ptr(dest),
+                     ptr(status), stream())
         if ctx.needs_input_grad[1]:
             scores, est = ctx.saved_tensors[3:]
             G = _empty((Bn, Bc), probs)
             coef = _empty((Bc,), probs)
             dcand = _empty(cand_shape, probs)
-            call("bm_clip_loss_bwd_cand", ptr(probs), ptr(scores), ptr(inv), ptr(est), ptr(cand), ptr(gout), Bn, Bc, KT,
-                 off, ptr(G), ptr(coef), ptr(dcand), ptr(status), stream())
+            _tc_call("bm_clip_loss_bwd_cand", ptr(probs), ptr(scores), ptr(inv), ptr(est), ptr(cand), ptr(gout), Bn, Bc,
+                     KT, off, ptr(G), ptr(coef), ptr(dcand), ptr(status), stream())
         return dest, dcand, None
 
 

@@ -426,6 +426,56 @@ int bm_clip_loss_fwd_det(const float* est, const float* cand, int Bn, int Bc, lo
                          float* inv_norm, float* scores, float* probs, float* row_loss, float* loss, float* workspace,
                          long long workspace_floats, int* status, bm_stream_t stream);
 
+/* ---- TF32 forms (PyTorch's TF32 matmul precision in the drop-in modules) -------------------------------------------
+ * Every `_tf32` entry point takes its default form's arguments and computes its contraction in single-pass TF32 instead of
+ * 3xTF32: each fp32 operand element is rounded once to tf32 (round to nearest, ties away from zero: cvt.rna.tf32.f32, the
+ * hi piece of bm_tc_weight_split), the products are exact, and they are accumulated in fp32 exactly as in the default
+ * form (a fresh register tile per 32-wide K block, added into the running sum with round-to-nearest adds), so the result is
+ * within ~1e-5 relative of an fp64 contraction of the rounded operands however long K is.  Everything outside the
+ * contraction is unchanged: epilogues, the CLIP candidate norms (fp64 sums of squares of the fp32 values), softmax and the
+ * FP32-FMA kernels the default forms fall back to for shapes outside the tensor-core gates.  The forms that take
+ * w_hi / w_lo read only w_hi and accept w_lo == NULL; w_hi may then hold the raw fp32 weights (bm_tc_weight_split with NULL
+ * lo outputs), which they round.  bm_clip_scores_det_tf32 / bm_clip_loss_fwd_det_tf32 combine both forms: repeated calls
+ * are bitwise identical, as with the `_det` forms.  The fp16-piece entry points (`*_f16`) have no TF32 form. */
+int bm_tc_conv1d_tf32(const float* x, const float* w_hi, const float* w_lo, const float* bias, const float* addend,
+                      int B, int T, int Cin, int Ntot, int Kw, int dilation, int sign, int glu, int act, int out_tmajor,
+                      float* y, float* aux, float* glu_out, double* stats, int* status, bm_stream_t stream);
+int bm_tc_conv1d_persistent_tf32(const float* x, const float* w_raw, const float* bias, int accumulate, int B, int T,
+                                 int Cin, int Ntot, int Kw, int dilation, int sign, int glu, int act, int out_tmajor,
+                                 float* y, float* aux, float* glu_out, double* stats, int* status, bm_stream_t stream);
+int bm_tc_pointwise_sel_tf32(const float* x, const float* w_hi, const float* w_lo, const int* wsel, int n_sets, int B,
+                             int T, int Cin, int Ntot, float* y, int* status, bm_stream_t stream);
+int bm_tc_sensor_mix_bwd_data_tf32(const float* du, const float* w_hi, const float* w_lo, const int* wsel, int n_sets,
+                                   const float* mask, int B, int T, int Op, int Cp, int C, float* dmeg, int* status,
+                                   bm_stream_t stream);
+int bm_tc_wgrad_tf32(const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw, int dilation,
+                     float* workspace, float* dw, float* dbias, int* status, bm_stream_t stream);
+int bm_tc_wgrad_conv_tf32(const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw, int dilation,
+                          float* workspace, float* dw, int* status, bm_stream_t stream);
+int bm_tc_wgrad_grouped_tf32(const float* dy, const float* x, const int* order, const int* seg_off, int G, int B, int T,
+                             int M, int N, float* out, int* status, bm_stream_t stream);
+int bm_clip_scores_tf32(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
+                        float* inv_norm, float* scores, float* probs, float* workspace, long long workspace_floats,
+                        int* status, bm_stream_t stream);
+int bm_clip_scores_det_tf32(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
+                            float* inv_norm, float* scores, float* probs, float* workspace, long long workspace_floats,
+                            int* status, bm_stream_t stream);
+int bm_clip_loss_fwd_tf32(const float* est, const float* cand, int Bn, int Bc, long long KT, int target_offset,
+                          float* inv_norm, float* scores, float* probs, float* row_loss, float* loss, float* workspace,
+                          long long workspace_floats, int* status, bm_stream_t stream);
+int bm_clip_loss_fwd_det_tf32(const float* est, const float* cand, int Bn, int Bc, long long KT, int target_offset,
+                              float* inv_norm, float* scores, float* probs, float* row_loss, float* loss,
+                              float* workspace, long long workspace_floats, int* status, bm_stream_t stream);
+int bm_clip_loss_bwd_tf32(const float* probs, const float* inv_norm, const float* cand, const float* gout, int Bn,
+                          int Bc, long long KT, int target_offset, float* G, float* dest, int* status,
+                          bm_stream_t stream);
+int bm_clip_loss_bwd_cand_tf32(const float* probs, const float* scores, const float* inv_norm, const float* est,
+                               const float* cand, const float* gout, int Bn, int Bc, long long KT, int target_offset,
+                               float* G, float* coef, float* dcand, int* status, bm_stream_t stream);
+int bm_clip_scores_bwd_tf32(const float* dscores, const float* scores, const float* inv_norm, const float* est,
+                            const float* cand, int Bn, int Bc, long long KT, float* G, float* coef, float* dest,
+                            float* dcand, int* status, bm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
