@@ -7,9 +7,11 @@
 // addressing (tap shifts with per-sample zero padding, position-major weight-gradient operands, K slices) and its own fused
 // epilogue without a copy of the pipeline.
 //
-// Two main loops share the wgmma wrappers, the tile layout and the numerics below: hc_conv_kernel (further down: TMA-fed,
-// warp-specialised) for the conv ops, whose A operand is a K-contiguous activation tile, and hg_gemm_kernel (register-staged)
-// for the weight gradients and the CLIP GEMMs, whose M/N-contiguous operands are transposed on their way into shared memory.
+// Three main loops share the wgmma wrappers, the tile layout and the numerics below: hc_conv_kernel (further down: TMA-fed,
+// warp-specialised) for the conv ops, whose A operand is a K-contiguous activation tile; hw_wgrad_kernel (the same pipeline,
+// A transposed in registers, B transposed by the producer) for the conv weight gradient (WgradPOp); and hg_gemm_kernel
+// (register-staged) for the other weight gradients and the CLIP GEMMs, whose M/N-contiguous operands are transposed on their
+// way into shared memory.
 //
 // hg_gemm_kernel: one CTA = two warpgroups = one 128 x BN output tile (warpgroup g owns rows [64 g, 64 g + 64)); BN = 128,
 // or 160 where the output width asks for it (hg_pick_bn).  Per K block of 32:
@@ -241,6 +243,12 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
                  ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(c2), "r"(bar)
                  : "memory");
 }
+// the same for a 2D tensor map
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];"
+                 ::"r"(dst), "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
+                 : "memory");
+}
 
 // ---------------------------------------------------------------------------------------------------
 // the GEMM engine
@@ -447,6 +455,48 @@ template <int BN, int PASSES> constexpr int hc_smem_bytes() { return HC_STAGES *
 __device__ __forceinline__ int hc_consumer_tid() { return threadIdx.x - (HC_THREADS - HC_CONSUMERS); }
 __device__ __forceinline__ void hc_consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(HC_CONSUMERS) : "memory"); }
 
+// One K block of a consumer warpgroup (hc_conv_kernel, hw_wgrad_kernel), where the numerics live: the warpgroup's 64 x 32
+// A fragment, read raw through a(kk, e) (fp32 element e of k8 step kk in the register layout of wgmma_tf32_rs), is split
+// into tf32 hi/lo in registers (PASSES = 1: rounded once with cvt.rna) and multiplied with the stage's B tiles at b_hi
+// (hi) and b_hi + BN x 32 x 4 (lo): lo*hi + hi*lo + hi*hi per k8 into a fresh `part` tile (PASSES = 1: one wgmma per k8);
+// once the MMAs have drained, release() hands the stage back and `part` is added into `acc` with round-to-nearest FADDs.
+template <int BN, int PASSES, class LoadA, class Release>
+__device__ __forceinline__ void hc_consume_block(float* acc, float* part, uint32_t b_hi, const LoadA& a,
+                                                 const Release& release) {
+    constexpr int NACC = BN / 2, B_TILE = BN * HG_BK * 4;
+    if constexpr (PASSES == 3) {
+        float hi[4][4], lo[4][4];                   // [k8][fragment element]
+#pragma unroll
+        for (int kk = 0; kk < HG_BK / 8; ++kk)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) tf32_split(a(kk, e), hi[kk][e], lo[kk][e]);
+        const uint32_t b_lo = b_hi + B_TILE;
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < HG_BK / 8; ++kk) {
+            const uint32_t off = kk * 32;
+            const uint64_t dbh = wgmma_desc_k_sw128(b_hi + off), dbl = wgmma_desc_k_sw128(b_lo + off);
+            wgmma_tf32_rs<BN>(part, lo[kk], dbh, kk != 0);
+            wgmma_tf32_rs<BN>(part, hi[kk], dbl, 1);
+            wgmma_tf32_rs<BN>(part, hi[kk], dbh, 1);
+        }
+    } else {
+        float r[4][4];                              // the same fragment, rounded once
+#pragma unroll
+        for (int kk = 0; kk < HG_BK / 8; ++kk)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) r[kk][e] = tf32_rna(a(kk, e));
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < HG_BK / 8; ++kk) wgmma_tf32_rs<BN>(part, r[kk], wgmma_desc_k_sw128(b_hi + kk * 32), kk != 0);
+    }
+    wgmma_commit();
+    wgmma_wait_all();
+    release();
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) acc[i] += part[i];
+}
+
 template <class Op, int BN, int PASSES>
 __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_constant__ Op op,
                                                                const __grid_constant__ CUtensorMap xmap) {
@@ -538,53 +588,21 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_con
             return;
         }
         const float* at = reinterpret_cast<const float*>(smem + s * STAGE);
-        if constexpr (PASSES == 3) {
-            float hi[4][4], lo[4][4];               // [k8][fragment element]
-#pragma unroll
-            for (int kk = 0; kk < HG_BK / 8; ++kk) {
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {       // element e: row r0 + 8 (e & 1), 16-byte chunk 2 kk + (e >> 1), word tq
-                    const int r = r0 + 8 * (e & 1), q = 2 * kk + (e >> 1);
-                    tf32_split(at[r * 32 + ((q ^ grp) << 2) + tq], hi[kk][e], lo[kk][e]);
-                }
-            }
-            const uint32_t b_hi = base_u32 + s * STAGE + HG_TILE_BYTES, b_lo = b_hi + B_TILE;
-            wgmma_fence();
-#pragma unroll
-            for (int kk = 0; kk < HG_BK / 8; ++kk) {
-                const uint32_t off = kk * 32;
-                const uint64_t dbh = wgmma_desc_k_sw128(b_hi + off), dbl = wgmma_desc_k_sw128(b_lo + off);
-                wgmma_tf32_rs<BN>(part, lo[kk], dbh, kk != 0);
-                wgmma_tf32_rs<BN>(part, hi[kk], dbl, 1);
-                wgmma_tf32_rs<BN>(part, hi[kk], dbh, 1);
-            }
-        } else {
-            float a[4][4];                          // the same fragment, rounded once
-#pragma unroll
-            for (int kk = 0; kk < HG_BK / 8; ++kk) {
-#pragma unroll
-                for (int e = 0; e < 4; ++e) {
-                    const int r = r0 + 8 * (e & 1), q = 2 * kk + (e >> 1);
-                    a[kk][e] = tf32_rna(at[r * 32 + ((q ^ grp) << 2) + tq]);
-                }
-            }
-            const uint32_t b_hi = base_u32 + s * STAGE + HG_TILE_BYTES;
-            wgmma_fence();
-#pragma unroll
-            for (int kk = 0; kk < HG_BK / 8; ++kk) wgmma_tf32_rs<BN>(part, a[kk], wgmma_desc_k_sw128(b_hi + kk * 32), kk != 0);
-        }
-        wgmma_commit();
-        wgmma_wait_all();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty0 + 8 * s);
-#pragma unroll
-        for (int i = 0; i < NACC; ++i) acc[i] += part[i];
+        // element e: row r0 + 8 (e & 1), 16-byte chunk 2 kk + (e >> 1), word tq
+        hc_consume_block<BN, PASSES>(
+            acc, part, base_u32 + s * STAGE + HG_TILE_BYTES,
+            [&](int kk, int e) { return at[(r0 + 8 * (e & 1)) * 32 + (((2 * kk + (e >> 1)) ^ grp) << 2) + tq]; },
+            [&] {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty0 + 8 * s);
+            });
     }
     op.template epilogue<BN, PASSES>(cta, acc, 64 * cg);
 }
 
-// x [B][T][Cin] fp32 as a 3D tensor map with a [1][128][32] box, 128-byte swizzle, zero fill out of bounds
-inline int hc_x_map(CUtensorMap* m, const float* x, int B, int T, int Cin, const char* who) {
+// A dense fp32 tensor x of `rank` dimensions (dims[0] contiguous, no padding between rows) as a tensor map with the box
+// box[0 .. rank), 128-byte swizzle (box[0] = 32 fp32: one 128-byte row), zero fill out of bounds
+inline int hc_x_map(CUtensorMap* m, const float* x, int rank, const long long* dims, const int* box, const char* who) {
     using Encode = CUresult (*)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                 const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
                                 CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
@@ -598,10 +616,16 @@ inline int hc_x_map(CUtensorMap* m, const float* x, int B, int T, int Cin, const
     }();
     if (!encode) return set_error(3, "%s: cuTensorMapEncodeTiled is not available%s", who);
     if (reinterpret_cast<uintptr_t>(x) & 15) return set_error(2, "%s: x must be 16-byte aligned%s", who);
-    const cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)T, (cuuint64_t)B};
-    const cuuint64_t strides[2] = {(cuuint64_t)Cin * 4, (cuuint64_t)T * Cin * 4};
-    const cuuint32_t box[3] = {HG_BK, HG_BM, 1}, elem[3] = {1, 1, 1};
-    const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, elem,
+    if (rank < 1 || rank > 5) return set_error(2, "%s: tensor map rank out of range%s", who);
+    cuuint64_t d[5], strides[4];
+    cuuint32_t b[5], elem[5];
+    for (int i = 0; i < rank; ++i) {
+        d[i] = (cuuint64_t)dims[i];
+        b[i] = (cuuint32_t)box[i];
+        elem[i] = 1;
+        if (i > 0) strides[i - 1] = (i == 1 ? 4 : strides[i - 2]) * d[i - 1];
+    }
+    const CUresult r = encode(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, rank, const_cast<float*>(x), d, strides, b, elem,
                               CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                               CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return set_error(2, "%s: cuTensorMapEncodeTiled failed%s", who);
@@ -614,8 +638,10 @@ inline int hc_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) 
     if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hc_conv_kernel<Op, BN, PASSES>), SMEM)) return rc;
     if (grid.x == 0 || grid.y == 0 || grid.z == 0) return 0;
     if (grid.y > 65535 || grid.z > 65535) return set_error(2, "%s: grid too large%s", who);
-    CUtensorMap xmap;
-    if (int rc = hc_x_map(&xmap, op.x, op.B, op.T, op.Cin, who)) return rc;
+    CUtensorMap xmap;                                   // x [B][T][Cin], box [1][128][32]
+    const long long dims[3] = {op.Cin, op.T, op.B};
+    const int box[3] = {HG_BK, HG_BM, 1};
+    if (int rc = hc_x_map(&xmap, op.x, 3, dims, box, who)) return rc;
     hc_conv_kernel<Op, BN, PASSES><<<grid, HC_THREADS, SMEM, st>>>(op, xmap);
     ++g_launches;
     cudaError_t e = cudaGetLastError();
@@ -630,6 +656,164 @@ inline int hc_launch_bn(int bn, const Op& op, dim3 grid, cudaStream_t st, const 
         return bn == 160 ? hc_launch<160, 1>(op, grid, st, who) : hc_launch<128, 1>(op, grid, st, who);
     }
     return bn == 160 ? hc_launch<160, 3>(op, grid, st, who) : hc_launch<128, 3>(op, grid, st, who);
+}
+
+// ---------------------------------------------------------------------------------------------------
+// the weight-gradient engine: the same GEMM, warp-specialised, for operands that are contiguous along M and N
+// ---------------------------------------------------------------------------------------------------
+// For WgradPOp (tc_wgradp.cuh): G[(tap, n)][m] = sum_p X[p + shift(tap), n] * dY[p, m] over flattened rows p = b T + t, with
+// X [R][Nx] and dY [R][Mdy] channel-contiguous, while tf32 wgmma reads K-major shared-memory operands only.  The CTA shape,
+// the stage layout (A raw | B hi | B lo), the full/empty mbarriers and the consumer block are hc_conv_kernel's:
+//   * producer: thread 0 loads the A tile with TMA as 4 boxes [32 rows p][32 channels] of a 2D map over X (128-byte
+//     swizzle).  Box j holds tile rows 32 j .. 32 j + 31, which are channels of ONE tap (Nx % 32 == 0), and is loaded at
+//     row p0 + shift(tap); rows outside [0, R) arrive as zeros.  All 128 threads load the dY tile [32 p][BN m] as float4
+//     from global memory one K block ahead (rows p >= R and columns m >= Mdy as zeros) and store its tf32 pieces
+//     transposed into the K-major B tiles (HgSlot<false, BN>);
+//   * consumers read their A fragment transposed out of the boxes, zero the elements whose t + shift leaves [0, T) (sample
+//     edges inside the flattened rows, which TMA cannot see) or whose p >= R, and run hc_consume_block.
+// t = p mod T is carried from block to block (T >= 32: at most one sample edge per block), so the loop divides nothing.
+// Op provides: R, T, X, Nx, err; cta<BN>(), kblocks(c), row0(c) (first flattened row of the CTA's K slice),
+// a_box(c, j) = {first channel, tap shift} of box j (shift >= T for rows past the last tap), b4(c, kb, k, q) = dY
+// elements m = n0 + 4q .. +3 at row k of block kb, and epilogue<BN>(c, acc, m0).
+// Shared memory per K block at BN = 160: A 16 KB written by TMA + 16 KB read, B 40 KB written + 120 KB read by the
+// wgmmas; dY is read from L2 / HBM by the producer (20 KB), not staged.  HC_STAGES = 3 stages of 56 KB (169 KB per CTA):
+// a 4th stage fits in 227 KB but measured no faster.
+
+// bits a .. b-1 of a 32-bit mask (clamped to [0, 32))
+__device__ __forceinline__ uint32_t hw_bits(int a, int b) {
+    a = max(a, 0);
+    b = min(b, 32);
+    return a >= b ? 0u : (0xFFFFFFFFu >> (32 - (b - a))) << a;
+}
+
+template <class Op, int BN, int PASSES>
+__global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_constant__ Op op,
+                                                                const __grid_constant__ CUtensorMap xmap) {
+    static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or single-pass TF32");
+    constexpr int NACC = BN / 2, STAGE = hc_stage_bytes<BN, PASSES>(), B_TILE = BN * HG_BK * 4;
+    constexpr int BOX_BYTES = HG_BK * HG_BK * 4;                 // one [32 p][32 channels] box of A
+    extern __shared__ uint8_t smem_raw[];
+    __shared__ alignas(8) uint64_t bars[2 * HC_STAGES];         // full[s], empty[s]
+    const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
+    uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
+    const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * HC_STAGES;
+    const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
+    if (tid == 0) {
+        for (int s = 0; s < HC_STAGES; ++s) {
+            mbar_init(full0 + 8 * s, 128);                 // the producer's 128 threads (+ the TMA bytes)
+            mbar_init(empty0 + 8 * s, HC_CONSUMERS / 32);  // one arrival per consumer warp
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+
+    const typename Op::Cta cta = op.template cta<BN>();
+    const int nkb = op.kblocks(cta), p0 = op.row0(cta), T = op.T;
+    if (wg == 0) {
+        // ---- producer
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HC_PRODUCER_REGS));
+        constexpr int NB4 = BN / 16;                     // float4 of dY per thread per K block
+        const int k = 8 * (tid >> 5) + (lane & 7), q0 = lane >> 3;    // row k, column quads q0 + 4 j (HgSlot<false>'s lanes)
+        int bc[4], bs[4];                                // box j: channel and row shift (0 for a box of padding)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+            const int2 b = op.a_box(cta, j);
+            bc[j] = b.x;
+            bs[j] = (b.y >= T || b.y <= -T) ? 0 : b.y;
+        }
+        float4 v[NB4];
+        auto load = [&](int kb) {
+#pragma unroll
+            for (int j = 0; j < NB4; ++j) v[j] = op.b4(cta, kb, k, q0 + 4 * j);
+        };
+        if (nkb > 0) load(0);
+        for (int kb = 0; kb < nkb; ++kb) {
+            const int s = kb % HC_STAGES, use = kb / HC_STAGES;
+            if (use > 0 && !mbar_wait(empty0 + 8 * s, (use - 1) & 1)) {
+                if (op.err) atomicCAS(op.err, 0, HC_ERR_EMPTY);
+                return;
+            }
+            const uint32_t st = base_u32 + s * STAGE, full = full0 + 8 * s;
+            if (tid == 0) {
+                const int p = p0 + kb * HG_BK;
+                mbar_expect_tx(full, HG_TILE_BYTES);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) tma_load_2d(st + j * BOX_BYTES, &xmap, bc[j], p + bs[j], full);
+            }
+            uint8_t* bh = smem + s * STAGE + HG_TILE_BYTES;
+#pragma unroll
+            for (int j = 0; j < NB4; ++j) HgSlot<false, BN>::template store<PASSES>(bh, bh + B_TILE, k, q0 + 4 * j, v[j]);
+            if (kb + 1 < nkb) load(kb + 1);
+            fence_proxy_async();                               // the generic-proxy stores, before the wgmmas read them
+            mbar_arrive(full);
+        }
+        return;
+    }
+    // ---- consumers
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HC_CONSUMER_REGS));
+    const int cg = wg - 1, grp = lane >> 2, tq = lane & 3;
+    const int r0 = 64 * cg + 16 * ((tid >> 5) & 3) + grp;        // A rows r0 and r0 + 8: one box, one tap
+    const int sh = op.a_box(cta, r0 >> 5).y;
+    const int tlo = max(0, -sh), thi = min(T, T - sh);          // t + shift in [0, T)  <=>  t in [tlo, thi)
+    // word offset of fragment element e (row r0 + 8 (e & 1), k = tq + 4 (e >> 1)) at kk = 0; kk adds 8 rows of the box
+    int off[4];
+#pragma unroll
+    for (int e = 0; e < 4; ++e) {
+        const int c = (r0 & 31) + 8 * (e & 1), kq = tq + 4 * (e >> 1);
+        off[e] = (r0 >> 5) * (BOX_BYTES / 4) + kq * 32 + (((c >> 2) ^ kq) << 2) + (c & 3);
+    }
+    float acc[NACC], part[NACC];
+#pragma unroll
+    for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+    int t0 = p0 % T;                                            // t of the block's first row
+    for (int kb = 0; kb < nkb; ++kb) {
+        const int s = kb % HC_STAGES, use = kb / HC_STAGES;
+        // rows k of this block that contribute: t0 + k in [tlo, thi), or in [tlo + T, thi + T) past the sample's end,
+        // and p < R
+        const int p = p0 + kb * HG_BK;
+        const uint32_t live = ((hw_bits(tlo - t0, thi - t0) | hw_bits(tlo + T - t0, thi + T - t0)) & hw_bits(0, op.R - p)) >> tq;
+        t0 += HG_BK;
+        if (t0 >= T) t0 -= T;
+        if (!mbar_wait(full0 + 8 * s, use & 1)) {
+            if (op.err) atomicCAS(op.err, 0, HC_ERR_FULL);
+            return;
+        }
+        const float* at = reinterpret_cast<const float*>(smem + s * STAGE);
+        hc_consume_block<BN, PASSES>(
+            acc, part, base_u32 + s * STAGE + HG_TILE_BYTES,
+            [&](int kk, int e) {
+                const float v = at[off[e] + 8 * 32 * kk];
+                return (live >> (8 * kk + 4 * (e >> 1))) & 1 ? v : 0.f;
+            },
+            [&] {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty0 + 8 * s);
+            });
+    }
+    op.template epilogue<BN>(cta, acc, 64 * cg);
+}
+
+template <int BN, int PASSES, class Op>
+inline int hw_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) {
+    constexpr int SMEM = hc_smem_bytes<BN, PASSES>();
+    if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hw_wgrad_kernel<Op, BN, PASSES>), SMEM)) return rc;
+    if (grid.x == 0 || grid.y == 0 || grid.z == 0) return 0;
+    if (grid.y > 65535 || grid.z > 65535) return set_error(2, "%s: grid too large%s", who);
+    CUtensorMap xmap;                                   // X [R][Nx], box [32][32]
+    const long long dims[2] = {op.Nx, op.R};
+    const int box[2] = {HG_BK, HG_BK};
+    if (int rc = hc_x_map(&xmap, op.X, 2, dims, box, who)) return rc;
+    hw_wgrad_kernel<Op, BN, PASSES><<<grid, HC_THREADS, SMEM, st>>>(op, xmap);
+    ++g_launches;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", who, cudaGetErrorString(e));
+    return 0;
+}
+// tile width 160 or 128 (hg_pick_bn), passes 3 or 1
+template <class Op>
+inline int hw_launch_bn(int bn, const Op& op, dim3 grid, int passes, cudaStream_t st, const char* who) {
+    if (passes == 1) return bn == 160 ? hw_launch<160, 1>(op, grid, st, who) : hw_launch<128, 1>(op, grid, st, who);
+    return bn == 160 ? hw_launch<160, 3>(op, grid, st, who) : hw_launch<128, 3>(op, grid, st, who);
 }
 
 // the plain epilogue: D[z plane][row][col] = acc for rows < rows, cols < cols (row-major, leading dimension ld)

@@ -7,9 +7,10 @@
 //     G[(tap, n)][m] = sum_p Xs[p, (tap, n)] * dY[p, m],     Xs[p, (tap, n)] = X[p + shift(tap), n] (0 across a sample edge)
 //
 // so the taps share one tile grid (3 x 320 rows = 7.5 tiles of 128 instead of 3 x 3) and the reduction runs over the
-// flattened rows in exact blocks of 32.  One CTA = one (128-row tile, 128- or 160-column tile, K slice); partial tiles go to the
-// workspace and `wgradp_reduce_kernel` sums the K slices in a fixed order (deterministic) while scattering into the
-// nn.Conv1d layout [m][n][tap].
+// flattened rows in exact blocks of 32.  One CTA = one (128-row tile, 128- or 160-column tile, K slice) of hw_wgrad_kernel
+// (tc_common.cuh: X by TMA, transposed in registers; dY converted in the kernel); partial tiles go to the workspace and
+// `wgradp_reduce_kernel` sums the K slices in a fixed order (deterministic) while scattering into the nn.Conv1d layout
+// [m][n][tap].
 #pragma once
 #include "tc_wgrad.cuh"
 
@@ -17,11 +18,11 @@ namespace bm {
 namespace tc {
 
 struct WgradPOp {
-    static constexpr bool A_KCONTIG = false, B_KCONTIG = false;
     int R, T, Mdy, Nx, taps, dilation, rows, per_split, chunks;
     const float* dY; const float* X;
     float* P;                   // [ks][rows_pad][Mdy]
     int rows_pad;
+    int* err;                   // pipeline status (HC_ERR_FULL / HC_ERR_EMPTY), or null
 
     struct Cta { int m0, n0, c0, c1; };
     template <int BN> __device__ Cta cta() const {
@@ -33,13 +34,14 @@ struct WgradPOp {
         return c;
     }
     __device__ int kblocks(const Cta& c) const { return max(0, c.c1 - c.c0); }
-    __device__ float4 a4(const Cta& c, int kb, int k, int q) const {         // Xs^T: rows (tap, n), 4 never straddle a tap
-        const int r = c.m0 + 4 * q, p = (c.c0 + kb) * HG_BK + k;
-        if (r >= rows || p >= R) return make_float4(0.f, 0.f, 0.f, 0.f);
-        const int tap = r / Nx, n = r - tap * Nx;
-        const int b = p / T, t = p - b * T, ts = t + (tap - taps / 2) * dilation;
-        if (ts < 0 || ts >= T) return make_float4(0.f, 0.f, 0.f, 0.f);
-        return __ldg(reinterpret_cast<const float4*>(X + ((long long)b * T + ts) * Nx + n));
+    __device__ int row0(const Cta& c) const { return c.c0 * HG_BK; }
+    // box j of the A tile (tile rows 32 j .. 32 j + 31 = Xs rows (tap, n .. n + 31)): {n, shift(tap)}; rows past the last
+    // tap are padding: shift T (every element is zeroed)
+    __device__ int2 a_box(const Cta& c, int j) const {
+        const int r = c.m0 + 32 * j;
+        if (r >= rows) return make_int2(0, T);
+        const int tap = r / Nx;
+        return make_int2(r - tap * Nx, (tap - taps / 2) * dilation);
     }
     __device__ float4 b4(const Cta& c, int kb, int k, int q) const {         // dY^T
         const int m = c.n0 + 4 * q, p = (c.c0 + kb) * HG_BK + k;
@@ -109,15 +111,16 @@ inline size_t wgradp_workspace_floats(int B, int T, int Mdy, int Nx, int taps) {
 // dY [B,T,Mdy], X [B,T,Nx] channels-last -> dW [Mdy][Ntrue][taps]; ws: wgradp_workspace_floats() floats
 inline int launch_wgrad_pp(const float* dY, const float* X, int B, int T, int Mdy, int Nx, int Ntrue, int taps,
                            int dilation, float* ws, float* dW, int passes, int* err, cudaStream_t st) {
-    (void)err;
     const WgradPPGeom g = wgradp_geometry(B, T, Mdy, Nx, taps);
     const long long R = (long long)B * T;
     if (R >= (1ll << 31)) return set_error(2, "%s: too many rows%s", __func__);
+    if (reinterpret_cast<uintptr_t>(dY) & 15) return set_error(2, "%s: dy must be 16-byte aligned%s", __func__);
     WgradPOp o;
     o.R = (int)R; o.T = T; o.Mdy = Mdy; o.Nx = Nx; o.taps = taps; o.dilation = dilation; o.rows = g.rows;
     o.per_split = g.per_split; o.chunks = g.chunks; o.dY = dY; o.X = X; o.P = ws; o.rows_pad = g.mtiles * 256;
+    o.err = err;
     const dim3 grid((Mdy + g.bn - 1) / g.bn, o.rows_pad / HG_BM, g.ks);
-    if (int rc = hg_launch_bn(g.bn, o, grid, passes, st, __func__)) return rc;
+    if (int rc = hw_launch_bn(g.bn, o, grid, passes, st, __func__)) return rc;
     wgradp_reduce_kernel<<<ew_grid((long long)Mdy * Ntrue * taps), 256, 0, st>>>(ws, dW, taps, g.ks, o.rows_pad, Mdy, Nx,
                                                                                 Ntrue);
     ++g_launches;
