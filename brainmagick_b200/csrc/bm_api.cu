@@ -39,6 +39,19 @@ extern "C" int bm_abi_version(void) { return 1; }
 extern "C" unsigned long long bm_launch_count(void) { return bm::g_launches; }
 extern "C" int bm_set_debug_buffer(long long* buf) { bm::g_debug_buf = buf; return 0; }
 extern "C" int bm_set_debug_flags(int flags) { int old = bm::g_debug_flags; bm::g_debug_flags = flags; return old; }
+#ifdef BM_HC_PHASES
+// the per-phase probe's counters (tc_common.cuh HcPhase): out[kernel * HP_N + phase] after the device is idle; reset: zero
+// them.  Only in the probe build of profiles/conv_phase_probe.py, not part of the ABI.
+extern "C" int bm_hc_phases(unsigned long long* out, int reset) {
+    BM_CUDA(cudaDeviceSynchronize());
+    BM_CUDA(cudaMemcpyFromSymbol(out, tc::g_hc_phases, sizeof(tc::g_hc_phases)));
+    if (reset) {
+        static const unsigned long long zeros[2 * tc::HP_N] = {};
+        BM_CUDA(cudaMemcpyToSymbol(tc::g_hc_phases, zeros, sizeof(zeros)));
+    }
+    return 0;
+}
+#endif
 
 namespace {
 

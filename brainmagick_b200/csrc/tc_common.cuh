@@ -8,7 +8,8 @@
 // epilogue without a copy of the pipeline.
 //
 // Three main loops share the wgmma wrappers, the tile layout and the numerics below: hc_conv_kernel (further down: TMA-fed,
-// warp-specialised) for the conv ops, whose A operand is a K-contiguous activation tile; hw_wgrad_kernel (the same pipeline,
+// warp-specialised, persistent CTAs that walk the tiles) for the conv ops, whose A operand is a K-contiguous activation
+// tile; hw_wgrad_kernel (the same pipeline,
 // A transposed in registers, B transposed by the producer) for the conv weight gradient (WgradPOp); and hg_gemm_kernel
 // (register-staged) for the other weight gradients and the CLIP GEMMs, whose M/N-contiguous operands are transposed on their
 // way into shared memory.
@@ -31,6 +32,7 @@
 // adds into the running sum are kept, so the accumulation bias bound and the fixed reduction order do not change.
 #pragma once
 #include <cuda.h>
+#include <algorithm>
 #include <type_traits>
 #include "common.cuh"
 
@@ -251,6 +253,68 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 }
 
 // ---------------------------------------------------------------------------------------------------
+// per-phase probe of the warp-specialised loops (profiles/conv_phase_probe.py)
+// ---------------------------------------------------------------------------------------------------
+// Compiled only with -DBM_HC_PHASES (the shipped library never is: every method below is then empty).  Thread 0 of each
+// warpgroup sums the SM clocks (%clock) spent in each phase over its CTA and adds them to g_hc_phases[kernel][phase]
+// (kernel 0: hc_conv_kernel, 1: hw_wgrad_kernel), which bm_hc_phases() reads back.  Consumer phases are summed over both
+// consumer warpgroups.
+enum HcPhase {
+    HP_FULL_WAIT,      // consumer: waiting on the full barrier
+    HP_SPLIT_ADD,      // consumer: A fragment split + stage release + acc += part
+    HP_MMA,            // consumer: wgmma issue to drain (wait_group 0)
+    HP_EPILOGUE,       // consumer: the tile's epilogue
+    HP_C_BLOCKS,       // consumer: K blocks (count)
+    HP_TILES,          // consumer: tiles (count)
+    HP_EMPTY_WAIT,     // producer: waiting on the empty barrier
+    HP_B_LOAD,         // producer: B loads issued (or, loaded ahead, needed) until they are in registers
+    HP_STORE,          // producer: TMA issue, B split / stores, fence, arrive
+    HP_FIRST_FULL,     // producer: CTA start to its first full-barrier arrival
+    HP_P_BLOCKS,       // producer: K blocks (count)
+    HP_CTAS,           // CTAs (count, by the producer)
+    HP_N
+};
+// one float4 of a B operand as loaded (tc_conv.cuh ConvOp::b_load): raw fp32 in h, or two pieces in h and l
+struct HcB { float4 h, l; };
+#ifdef BM_HC_PHASES
+__device__ unsigned long long g_hc_phases[2][HP_N];
+struct HcProbe {
+    uint32_t start, t, acc[HP_N];
+    __device__ static uint32_t now() {
+        uint32_t c;
+        asm volatile("mov.u32 %0, %%clock;" : "=r"(c));
+        return c;
+    }
+    __device__ explicit HcProbe(uint32_t t0) : start(t0), t(now()) {
+#pragma unroll
+        for (int i = 0; i < HP_N; ++i) acc[i] = 0;
+    }
+    __device__ void mark(int p) { const uint32_t n = now(); acc[p] += n - t; t = n; }    // clocks since the last mark
+    __device__ void count(int p) { acc[p] += 1; }
+    __device__ void first_full() { if (acc[HP_FIRST_FULL] == 0) acc[HP_FIRST_FULL] = now() - start; }
+    __device__ void ready(const float4& v) { asm volatile("" ::"f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)); }
+    __device__ void ready(const HcB& v) { ready(v.h); ready(v.l); }
+    __device__ void flush(int kernel) const {
+        if (threadIdx.x % 128 != 0) return;
+#pragma unroll
+        for (int i = 0; i < HP_N; ++i)
+            if (acc[i]) atomicAdd(&g_hc_phases[kernel][i], (unsigned long long)acc[i]);
+    }
+};
+#else
+struct HcProbe {
+    __device__ static uint32_t now() { return 0; }
+    __device__ explicit HcProbe(uint32_t) {}
+    __device__ void mark(int) {}
+    __device__ void count(int) {}
+    __device__ void first_full() {}
+    __device__ void ready(const float4&) {}
+    __device__ void ready(const HcB&) {}
+    __device__ void flush(int) const {}
+};
+#endif
+
+// ---------------------------------------------------------------------------------------------------
 // the GEMM engine
 // ---------------------------------------------------------------------------------------------------
 constexpr int HG_BM = 128, HG_BN = 128, HG_BK = 32, HG_THREADS = 256;
@@ -432,10 +496,16 @@ inline int hg_launch_bn(int bn, const Op& op, dim3 grid, int passes, cudaStream_
 // ---------------------------------------------------------------------------------------------------
 // For ops whose A operand is a K-contiguous activation tile [1 sample][128 times][32 channels] of x [B][T][Cin] (ConvOp
 // and its variants).  One CTA = one producer warpgroup + two consumer warpgroups, HC_STAGES stages, each with a full and
-// an empty mbarrier:
+// an empty mbarrier.  The kernel is persistent: min(tiles, SMs) CTAs, CTA i computing tiles i, i + gridDim.x, ... of the
+// op's tile list (Op::cta(tile): column tile fastest, so that the CTAs running together read the same weights from L2).
+// The stage index and the barrier phases run on across tiles (one ring position per CTA), so the producer fills the next
+// tile's stages while the consumers run the current tile's epilogue, and a tile pays no barrier set-up or pipeline fill.
 //   * producer: thread 0 loads the A tile with TMA (op.a_box: the tap shift is in the t coordinate, and TMA's zero fill
-//     outside [0, T) is the conv's zero padding); all 128 threads fetch B through op.b4 into registers, split it into tf32
-//     hi/lo and store both into the stage (128-byte-swizzled K-major, as in hg_gemm_kernel);
+//     outside [0, T) is the conv's zero padding); all 128 threads fetch B through op.b_load into registers, split it into
+//     tf32 hi/lo and store both into the stage (128-byte-swizzled K-major, as in hg_gemm_kernel).  B is loaded one K block
+//     ahead: block g+1's loads are issued as soon as block g is stored, so their L2 latency overlaps the wait for the next
+//     free stage (the pre-split format, two loads per float4, loads the first half of the tile ahead and the second half
+//     in turn, within the producer's register budget);
 //   * consumers: warpgroup g reads its 64 raw fp32 A rows from the stage, splits them in registers with tf32_split and
 //     issues 4 x 3 wgmma with A from registers: lo*hi + hi*lo + hi*hi per k8 into a fresh `part` tile, which is added into
 //     `acc` with round-to-nearest FADDs per K block -- the pieces, MMA order and per-block adds of hg_gemm_kernel.
@@ -451,18 +521,34 @@ constexpr int HC_ERR_FULL = 901, HC_ERR_EMPTY = 902;           // status codes o
 template <int BN, int PASSES> constexpr int hc_stage_bytes() { return HG_TILE_BYTES + (PASSES == 3 ? 2 : 1) * BN * HG_BK * 4; }
 template <int BN, int PASSES> constexpr int hc_smem_bytes() { return HC_STAGES * hc_stage_bytes<BN, PASSES>() + 1024; }
 
-// index of a consumer thread in [0, 256) and a barrier over the consumer warpgroups only (the producer has exited)
+// index of a consumer thread in [0, 256) and a barrier over the consumer warpgroups only (the producer does not take part)
 __device__ __forceinline__ int hc_consumer_tid() { return threadIdx.x - (HC_THREADS - HC_CONSUMERS); }
 __device__ __forceinline__ void hc_consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(HC_CONSUMERS) : "memory"); }
+
+// The stage ring's barriers (full[s], empty[s]), initialised by thread 0 before a __syncthreads
+struct HcBars {
+    uint64_t b[2 * HC_STAGES];
+    __device__ void init() {
+        for (int s = 0; s < HC_STAGES; ++s) {
+            mbar_init(smem_u32(&b[s]), 128);                             // the producer's 128 threads (+ the TMA bytes)
+            mbar_init(smem_u32(&b[HC_STAGES + s]), HC_CONSUMERS / 32);   // one arrival per consumer warp
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __device__ uint32_t full(int s) const { return smem_u32(&b[s]); }
+    __device__ uint32_t empty(int s) const { return smem_u32(&b[HC_STAGES + s]); }
+};
 
 // One K block of a consumer warpgroup (hc_conv_kernel, hw_wgrad_kernel), where the numerics live: the warpgroup's 64 x 32
 // A fragment, read raw through a(kk, e) (fp32 element e of k8 step kk in the register layout of wgmma_tf32_rs), is split
 // into tf32 hi/lo in registers (PASSES = 1: rounded once with cvt.rna) and multiplied with the stage's B tiles at b_hi
 // (hi) and b_hi + BN x 32 x 4 (lo): lo*hi + hi*lo + hi*hi per k8 into a fresh `part` tile (PASSES = 1: one wgmma per k8);
 // once the MMAs have drained, release() hands the stage back and `part` is added into `acc` with round-to-nearest FADDs.
+// The two warpgroups issue their blocks concurrently: their 2 x 12 MMAs then take ~1900 clocks per block at BN = 160, the
+// tensor floor; issuing them one warpgroup after the other measured slower (DESIGN §4.2).
 template <int BN, int PASSES, class LoadA, class Release>
 __device__ __forceinline__ void hc_consume_block(float* acc, float* part, uint32_t b_hi, const LoadA& a,
-                                                 const Release& release) {
+                                                 const Release& release, HcProbe& pr) {
     constexpr int NACC = BN / 2, B_TILE = BN * HG_BK * 4;
     if constexpr (PASSES == 3) {
         float hi[4][4], lo[4][4];                   // [k8][fragment element]
@@ -470,6 +556,7 @@ __device__ __forceinline__ void hc_consume_block(float* acc, float* part, uint32
         for (int kk = 0; kk < HG_BK / 8; ++kk)
 #pragma unroll
             for (int e = 0; e < 4; ++e) tf32_split(a(kk, e), hi[kk][e], lo[kk][e]);
+        pr.mark(HP_SPLIT_ADD);
         const uint32_t b_lo = b_hi + B_TILE;
         wgmma_fence();
 #pragma unroll
@@ -486,59 +573,71 @@ __device__ __forceinline__ void hc_consume_block(float* acc, float* part, uint32
         for (int kk = 0; kk < HG_BK / 8; ++kk)
 #pragma unroll
             for (int e = 0; e < 4; ++e) r[kk][e] = tf32_rna(a(kk, e));
+        pr.mark(HP_SPLIT_ADD);
         wgmma_fence();
 #pragma unroll
         for (int kk = 0; kk < HG_BK / 8; ++kk) wgmma_tf32_rs<BN>(part, r[kk], wgmma_desc_k_sw128(b_hi + kk * 32), kk != 0);
     }
     wgmma_commit();
     wgmma_wait_all();
+    pr.mark(HP_MMA);
     release();
 #pragma unroll
     for (int i = 0; i < NACC; ++i) acc[i] += part[i];
+    pr.mark(HP_SPLIT_ADD);
 }
 
 template <class Op, int BN, int PASSES>
 __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_constant__ Op op,
-                                                               const __grid_constant__ CUtensorMap xmap) {
+                                                               const __grid_constant__ CUtensorMap xmap, int tiles) {
     static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or single-pass TF32");
+    const uint32_t t_start = HcProbe::now();        // the probe's CTA start (BM_HC_PHASES)
     constexpr int NACC = BN / 2, STAGE = hc_stage_bytes<BN, PASSES>(), B_TILE = BN * HG_BK * 4;
     extern __shared__ uint8_t smem_raw[];
-    __shared__ alignas(8) uint64_t bars[2 * HC_STAGES];         // full[s], empty[s]
+    __shared__ HcBars bars;
     const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
-    const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * HC_STAGES;
     const int tid = threadIdx.x, wg = tid >> 7;
-    if (tid == 0) {
-        for (int s = 0; s < HC_STAGES; ++s) {
-            mbar_init(full0 + 8 * s, 128);                 // the producer's 128 threads (+ the TMA bytes)
-            mbar_init(empty0 + 8 * s, HC_CONSUMERS / 32);  // one arrival per consumer warp
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    if (tid == 0) bars.init();
     __syncthreads();
 
-    const typename Op::Cta cta = op.template cta<BN>();
-    const int nkb = op.kblocks(cta);
     if (wg == 0) {
         // ---- producer
         asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HC_PRODUCER_REGS));
+        HcProbe pr(t_start);
         constexpr int NB4 = BN * HG_BK / 4 / 128;                 // float4 of B per thread per stage
-        int boff[NB4];                                            // this thread's B elements, the same in every K block
-        uint32_t live = 0;
-#pragma unroll
-        for (int j = 0; j < NB4; ++j) {
-            const int idx = tid + 128 * j, o = op.template b_col<BN>(cta, idx >> 3, idx & 7);
-            boff[j] = o < 0 ? 0 : o;                              // a column past the end loads column 0 and stores zeros
-            live |= (o >= 0 ? 1u : 0u) << j;
-        }
-        // one loop per weight format, so that the loads of a tile are issued back to back; the pre-split format moves
-        // the tile in 2 parts (2 loads per float4)
+        // one loop per weight format, so that the loads of a tile are issued back to back; PART float4 per thread are
+        // loaded one block ahead (the pre-split format, 2 loads per float4: half of them)
         auto produce = [&](auto fmt) -> bool {
             constexpr int FMT = decltype(fmt)::value, PART = FMT == Op::B_SPLIT ? NB4 / 2 : NB4;
-            for (int kb = 0; kb < nkb; ++kb) {
-                const int s = kb % HC_STAGES, use = kb / HC_STAGES;
-                if (use > 0 && !mbar_wait(empty0 + 8 * s, (use - 1) & 1)) return false;
-                const uint32_t st = base_u32 + s * STAGE, full = full0 + 8 * s;
+            int tile = blockIdx.x, kb = 0;
+            typename Op::Cta cta = op.template cta<BN>(tile);
+            // this thread's B elements j of a K block, the same in every block of the tile: tile column row + 16 j, k quad q
+            const int row = (tid & 127) >> 3, q = tid & 7;        // tid < 128
+            int boff[NB4];
+            uint32_t live;
+            auto columns = [&] {
+                live = 0;
+#pragma unroll
+                for (int j = 0; j < NB4; ++j) {
+                    const int o = op.template b_col<BN>(cta, row + 16 * j, q);
+                    boff[j] = o < 0 ? 0 : o;                      // a column past the end loads column 0 and stores zeros
+                    live |= (o >= 0 ? 1u : 0u) << j;
+                }
+            };
+            HcB r[PART];
+            auto load = [&](int p, long long base) {
+#pragma unroll
+                for (int j = 0; j < PART; ++j) r[j] = op.template b_load<FMT>(base + boff[p + j]);
+            };
+            columns();
+            load(0, op.b_base(cta, 0));
+            // the ring position: the stage (bits 0-1), the round through the ring mod 2 (bit 2), past the first round (bit 3)
+            for (uint32_t sp = 0;; sp = (sp & 3) == HC_STAGES - 1 ? ((sp & 4) ^ 4) | 8 : sp + 1) {
+                const int s = sp & 3;
+                if ((sp & 8) && !mbar_wait(bars.empty(s), ((sp >> 2) & 1) ^ 1)) return false;
+                pr.mark(HP_EMPTY_WAIT);
+                const uint32_t st = base_u32 + s * STAGE, full = bars.full(s);
                 if (tid == 0) {
                     const int3 c = op.a_box(cta, kb);
                     mbar_expect_tx(full, HG_TILE_BYTES);
@@ -548,19 +647,33 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_con
                 const long long base = op.b_base(cta, kb);
 #pragma unroll
                 for (int p = 0; p < NB4; p += PART) {
-                    float4 v[PART];
+                    if (p > 0) load(p, base);
 #pragma unroll
-                    for (int j = 0; j < PART; ++j) v[j] = op.template b4<FMT>(cta, base + boff[p + j]);
+                    for (int j = 0; j < PART; ++j) pr.ready(r[j]);
+                    pr.mark(HP_B_LOAD);
 #pragma unroll
                     for (int j = 0; j < PART; ++j) {
-                        const int idx = tid + 128 * (p + j);
-                        if (!((live >> (p + j)) & 1)) v[j] = make_float4(0.f, 0.f, 0.f, 0.f);
-                        HgSlot<true, BN>::template store<PASSES>(bh, bh + B_TILE, idx >> 3, idx & 7, v[j]);
+                        const float4 v = (live >> (p + j)) & 1 ? op.template b_value<FMT>(cta, r[j])
+                                                                : make_float4(0.f, 0.f, 0.f, 0.f);
+                        HgSlot<true, BN>::template store<PASSES>(bh, bh + B_TILE, row + 16 * (p + j), q, v);
                     }
+                    pr.mark(HP_STORE);
                 }
                 fence_proxy_async();                               // the generic-proxy stores, before the wgmmas read them
                 mbar_arrive(full);
+                pr.first_full();
+                pr.count(HP_P_BLOCKS);
+                if (++kb == op.kblocks(cta)) {                     // the CTA's next tile
+                    tile += gridDim.x;
+                    if (tile >= tiles) break;
+                    cta = op.template cta<BN>(tile);
+                    kb = 0;
+                    columns();
+                }
+                load(0, op.b_base(cta, kb));                       // the next block's loads, in flight during the wait
+                pr.mark(HP_STORE);
             }
+            pr.mark(HP_STORE);
             return true;
         };
         const int f = op.b_format();
@@ -572,32 +685,51 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_con
                  : f == Op::B_SPLIT ? produce(std::integral_constant<int, Op::B_SPLIT>())
                                     : produce(std::integral_constant<int, Op::B_F16>());
         if (!ok && op.err) atomicCAS(op.err, 0, HC_ERR_EMPTY);
+        pr.count(HP_CTAS);
+        pr.flush(0);
         return;
     }
     // ---- consumers
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HC_CONSUMER_REGS));
+    HcProbe pr(t_start);
     const int cg = wg - 1, lane = tid & 31, grp = lane >> 2, tq = lane & 3;
     const int r0 = 64 * cg + 16 * ((tid >> 5) & 3) + grp;        // A rows r0 and r0 + 8 of the fragment; r0 & 7 = grp
+    // Fragment element e of k8 step kk is row r0 + 8 (e & 1), 16-byte chunk c = 2 kk + (e >> 1), word tq: word
+    // 32 row + 4 (c ^ grp) + tq of the swizzled tile, i.e. (w0 ^ 4 c) + 256 (e & 1) with w0 = 32 r0 + 4 grp + tq (bits 2-4
+    // of w0 hold grp alone), one register for all 16 addresses.
+    const int w0 = 32 * r0 + 4 * grp + tq;
     float acc[NACC], part[NACC];
+    // The ring position, packed into one register (the consumers' registers are taken by acc, part and the A fragment):
+    // the stage (bits 0-1), the round through the ring mod 2 = the parity of the stage's full-barrier phase (bit 2) and the
+    // tile's K blocks left (bits 3-)
+    uint32_t pos = 0;
+    for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
 #pragma unroll
-    for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
-    for (int kb = 0; kb < nkb; ++kb) {
-        const int s = kb % HC_STAGES, use = kb / HC_STAGES;
-        if (!mbar_wait(full0 + 8 * s, use & 1)) {
-            if (op.err) atomicCAS(op.err, 0, HC_ERR_FULL);
-            return;
+        for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
+        for (pos |= (uint32_t)op.kblocks(op.template cta<BN>(tile)) << 3; pos >> 3; pos -= 8) {
+            const int s = pos & 3;
+            if (!mbar_wait(bars.full(s), (pos >> 2) & 1)) {
+                if (op.err) atomicCAS(op.err, 0, HC_ERR_FULL);
+                return;
+            }
+            pr.mark(HP_FULL_WAIT);
+            pr.count(HP_C_BLOCKS);
+            const float* at = reinterpret_cast<const float*>(smem + s * STAGE);
+            hc_consume_block<BN, PASSES>(
+                acc, part, base_u32 + s * STAGE + HG_TILE_BYTES,
+                [&](int kk, int e) { return at[(w0 ^ (4 * (2 * kk + (e >> 1)))) + 256 * (e & 1)]; },
+                [&] {
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(bars.empty(s));
+                },
+                pr);
+            pos = s == HC_STAGES - 1 ? (pos & ~7u) | ((pos & 4) ^ 4) : pos + 1;
         }
-        const float* at = reinterpret_cast<const float*>(smem + s * STAGE);
-        // element e: row r0 + 8 (e & 1), 16-byte chunk 2 kk + (e >> 1), word tq
-        hc_consume_block<BN, PASSES>(
-            acc, part, base_u32 + s * STAGE + HG_TILE_BYTES,
-            [&](int kk, int e) { return at[(r0 + 8 * (e & 1)) * 32 + (((2 * kk + (e >> 1)) ^ grp) << 2) + tq]; },
-            [&] {
-                __syncwarp();
-                if (lane == 0) mbar_arrive(empty0 + 8 * s);
-            });
+        op.template epilogue<BN, PASSES>(op.template cta<BN>(tile), acc, 64 * cg);
+        pr.mark(HP_EPILOGUE);
+        pr.count(HP_TILES);
     }
-    op.template epilogue<BN, PASSES>(cta, acc, 64 * cg);
+    pr.flush(0);
 }
 
 // A dense fp32 tensor x of `rank` dimensions (dims[0] contiguous, no padding between rows) as a tensor map with the box
@@ -632,17 +764,19 @@ inline int hc_x_map(CUtensorMap* m, const float* x, int rank, const long long* d
     return 0;
 }
 
+// `tiles` output tiles (Op::cta(tile), tile in [0, tiles)) on min(tiles, SMs) persistent CTAs
 template <int BN, int PASSES, class Op>
-inline int hc_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) {
+inline int hc_launch(const Op& op, long long tiles, cudaStream_t st, const char* who) {
     constexpr int SMEM = hc_smem_bytes<BN, PASSES>();
     if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hc_conv_kernel<Op, BN, PASSES>), SMEM)) return rc;
-    if (grid.x == 0 || grid.y == 0 || grid.z == 0) return 0;
-    if (grid.y > 65535 || grid.z > 65535) return set_error(2, "%s: grid too large%s", who);
+    if (tiles <= 0) return 0;
+    if (tiles >= (1ll << 31)) return set_error(2, "%s: too many tiles%s", who);
     CUtensorMap xmap;                                   // x [B][T][Cin], box [1][128][32]
     const long long dims[3] = {op.Cin, op.T, op.B};
     const int box[3] = {HG_BK, HG_BM, 1};
     if (int rc = hc_x_map(&xmap, op.x, 3, dims, box, who)) return rc;
-    hc_conv_kernel<Op, BN, PASSES><<<grid, HC_THREADS, SMEM, st>>>(op, xmap);
+    const int grid = (int)std::min<long long>(tiles, num_sms());
+    hc_conv_kernel<Op, BN, PASSES><<<grid, HC_THREADS, SMEM, st>>>(op, xmap, (int)tiles);
     ++g_launches;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", who, cudaGetErrorString(e));
@@ -650,12 +784,12 @@ inline int hc_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) 
 }
 // the tile width of hg_pick_bn and the pass count op.passes (3 or 1; the fp16-piece weights only with 3)
 template <class Op>
-inline int hc_launch_bn(int bn, const Op& op, dim3 grid, cudaStream_t st, const char* who) {
+inline int hc_launch_bn(int bn, const Op& op, long long tiles, cudaStream_t st, const char* who) {
     if (op.passes == 1) {
         if (!op.w) return set_error(2, "%s: the single-pass form takes fp32 weights%s", who);
-        return bn == 160 ? hc_launch<160, 1>(op, grid, st, who) : hc_launch<128, 1>(op, grid, st, who);
+        return bn == 160 ? hc_launch<160, 1>(op, tiles, st, who) : hc_launch<128, 1>(op, tiles, st, who);
     }
-    return bn == 160 ? hc_launch<160, 3>(op, grid, st, who) : hc_launch<128, 3>(op, grid, st, who);
+    return bn == 160 ? hc_launch<160, 3>(op, tiles, st, who) : hc_launch<128, 3>(op, tiles, st, who);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -691,20 +825,14 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
                                                                 const __grid_constant__ CUtensorMap xmap) {
     static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or single-pass TF32");
     constexpr int NACC = BN / 2, STAGE = hc_stage_bytes<BN, PASSES>(), B_TILE = BN * HG_BK * 4;
+    const uint32_t t_start = HcProbe::now();        // the probe's CTA start (BM_HC_PHASES)
     constexpr int BOX_BYTES = HG_BK * HG_BK * 4;                 // one [32 p][32 channels] box of A
     extern __shared__ uint8_t smem_raw[];
-    __shared__ alignas(8) uint64_t bars[2 * HC_STAGES];         // full[s], empty[s]
+    __shared__ HcBars bars;
     const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
-    const uint32_t full0 = smem_u32(bars), empty0 = full0 + 8 * HC_STAGES;
     const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
-    if (tid == 0) {
-        for (int s = 0; s < HC_STAGES; ++s) {
-            mbar_init(full0 + 8 * s, 128);                 // the producer's 128 threads (+ the TMA bytes)
-            mbar_init(empty0 + 8 * s, HC_CONSUMERS / 32);  // one arrival per consumer warp
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    if (tid == 0) bars.init();
     __syncthreads();
 
     const typename Op::Cta cta = op.template cta<BN>();
@@ -712,6 +840,7 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
     if (wg == 0) {
         // ---- producer
         asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HC_PRODUCER_REGS));
+        HcProbe pr(t_start);
         constexpr int NB4 = BN / 16;                     // float4 of dY per thread per K block
         const int k = 8 * (tid >> 5) + (lane & 7), q0 = lane >> 3;    // row k, column quads q0 + 4 j (HgSlot<false>'s lanes)
         int bc[4], bs[4];                                // box j: channel and row shift (0 for a box of padding)
@@ -729,11 +858,12 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
         if (nkb > 0) load(0);
         for (int kb = 0; kb < nkb; ++kb) {
             const int s = kb % HC_STAGES, use = kb / HC_STAGES;
-            if (use > 0 && !mbar_wait(empty0 + 8 * s, (use - 1) & 1)) {
+            if (use > 0 && !mbar_wait(bars.empty(s), (use - 1) & 1)) {
                 if (op.err) atomicCAS(op.err, 0, HC_ERR_EMPTY);
                 return;
             }
-            const uint32_t st = base_u32 + s * STAGE, full = full0 + 8 * s;
+            pr.mark(HP_EMPTY_WAIT);
+            const uint32_t st = base_u32 + s * STAGE, full = bars.full(s);
             if (tid == 0) {
                 const int p = p0 + kb * HG_BK;
                 mbar_expect_tx(full, HG_TILE_BYTES);
@@ -741,16 +871,26 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
                 for (int j = 0; j < 4; ++j) tma_load_2d(st + j * BOX_BYTES, &xmap, bc[j], p + bs[j], full);
             }
             uint8_t* bh = smem + s * STAGE + HG_TILE_BYTES;
+            pr.mark(HP_STORE);
+#pragma unroll
+            for (int j = 0; j < NB4; ++j) pr.ready(v[j]);
+            pr.mark(HP_B_LOAD);
 #pragma unroll
             for (int j = 0; j < NB4; ++j) HgSlot<false, BN>::template store<PASSES>(bh, bh + B_TILE, k, q0 + 4 * j, v[j]);
             if (kb + 1 < nkb) load(kb + 1);
             fence_proxy_async();                               // the generic-proxy stores, before the wgmmas read them
             mbar_arrive(full);
+            pr.mark(HP_STORE);
+            pr.first_full();
+            pr.count(HP_P_BLOCKS);
         }
+        pr.count(HP_CTAS);
+        pr.flush(1);
         return;
     }
     // ---- consumers
     asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(HC_CONSUMER_REGS));
+    HcProbe pr(t_start);
     const int cg = wg - 1, grp = lane >> 2, tq = lane & 3;
     const int r0 = 64 * cg + 16 * ((tid >> 5) & 3) + grp;        // A rows r0 and r0 + 8: one box, one tap
     const int sh = op.a_box(cta, r0 >> 5).y;
@@ -774,10 +914,12 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
         const uint32_t live = ((hw_bits(tlo - t0, thi - t0) | hw_bits(tlo + T - t0, thi + T - t0)) & hw_bits(0, op.R - p)) >> tq;
         t0 += HG_BK;
         if (t0 >= T) t0 -= T;
-        if (!mbar_wait(full0 + 8 * s, use & 1)) {
+        if (!mbar_wait(bars.full(s), use & 1)) {
             if (op.err) atomicCAS(op.err, 0, HC_ERR_FULL);
             return;
         }
+        pr.mark(HP_FULL_WAIT);
+        pr.count(HP_C_BLOCKS);
         const float* at = reinterpret_cast<const float*>(smem + s * STAGE);
         hc_consume_block<BN, PASSES>(
             acc, part, base_u32 + s * STAGE + HG_TILE_BYTES,
@@ -787,10 +929,14 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
             },
             [&] {
                 __syncwarp();
-                if (lane == 0) mbar_arrive(empty0 + 8 * s);
-            });
+                if (lane == 0) mbar_arrive(bars.empty(s));
+            },
+            pr);
     }
     op.template epilogue<BN>(cta, acc, 64 * cg);
+    pr.mark(HP_EPILOGUE);
+    pr.count(HP_TILES);
+    pr.flush(1);
 }
 
 template <int BN, int PASSES, class Op>

@@ -4,9 +4,10 @@
 //   y[b, t, n] = bias[n] + sum_{tap} sum_{k} x[b, t + shift(tap), k] * W[wset(b)][tap][n][k]      (channels-last x, y)
 //
 // shift(tap) = sign * (tap - taps/2) * dilation; a shifted time outside [0, T) reads zeros (the conv's zero padding, never
-// the neighbouring sample: the activation tile is a TMA box of one sample).  Runs on hc_conv_kernel of tc_common.cuh.  One
-// CTA = 128 times of one sample x BN output columns, BN = hg_pick_bn(Ntot): 160 for the 320- and 640-wide layers, 128 for
-// 1024 (GLU: BN/2 'a' columns and the BN/2 gate columns they pair with, so that a * sigmoid(gate) is formed in registers).
+// the neighbouring sample: the activation tile is a TMA box of one sample).  Runs on hc_conv_kernel of tc_common.cuh, whose
+// persistent CTAs walk the tiles: one tile = 128 times of one sample x BN output columns, BN = hg_pick_bn(Ntot): 160 for the
+// 320- and 640-wide layers, 128 for 1024 (GLU: BN/2 'a' columns and the BN/2 gate columns they pair with, so that
+// a * sigmoid(gate) is formed in registers).  Tiles are numbered column tile fastest, then time tile, then sample.
 // The weights arrive as raw fp32 [sets][taps][Ntot][Cin], as its two tf32 pieces (bm_tc_weight_split) or as the two fp16
 // pieces of a power-of-two-scaled copy (bm_tc_weight_split_f16); the pieces are summed back on load (fp16: ~22 significant
 // bits of the weight, the precision the pieces carry).  Fused epilogue: bias, addend (skip gradient / in-place accumulate),
@@ -46,7 +47,7 @@ struct ConvOp {
     const float* w;                       // fp32 weights [sets][taps][Ntot][Cin], or null: fp16 pieces below
     const float* w_lo32;                  // nullable: second tf32 piece of w (bm_tc_weight_split), added back on load
     const __half* w_hi; const __half* w_lo; const float* w_amax;
-    int B, T, Cin, Ntot, taps, dilation, sign, glu, ttiles;
+    int B, T, Cin, Ntot, taps, dilation, sign, glu, ttiles, ncols;     // ttiles / ncols: time / column tiles
     int n_wsets; const int* wsel;         // per-sample weight set (SubjectLayers) or null
     const float* bias;                    // [Ntot] or null
     const float* addend;                  // [B,T,Ntot] or null (may alias y: in-place accumulate)
@@ -60,14 +61,16 @@ struct ConvOp {
     int passes;                           // 3: 3xTF32, 1: single-pass TF32 (reads w alone; not with the fp16 pieces)
 
     struct Cta { int b, t0, n_tile, wbase; float w_inv; };
-    template <int BN> __device__ Cta cta() const {
+    template <int BN> __device__ Cta cta(int tile) const {
         Cta c;
-        c.b = blockIdx.x / ttiles;
-        c.t0 = (blockIdx.x - c.b * ttiles) * HG_BM;
-        c.n_tile = blockIdx.y;
+        const int bt = tile / ncols;
+        c.n_tile = tile - bt * ncols;
+        c.b = bt / ttiles;
+        c.t0 = (bt - c.b * ttiles) * HG_BM;
         int s = wsel ? wsel[c.b] : 0;
         if (s < 0 || s >= n_wsets) {                 // a subject / recording index outside the weight sets: report it like
-            if (err && threadIdx.x == 0) atomicCAS(err, 0, 900);     // the reference's gather would raise
+            if (err && threadIdx.x == 0) atomicCAS(err, 0, 900);     // the reference's gather would raise (thread 0: the
+                                                                     // producer, which evaluates every tile)
             s = 0;
         }
         c.wbase = s * taps;
@@ -84,15 +87,16 @@ struct ConvOp {
     // output column of tile column j (GLU: j < BN/2 'a' columns, j >= BN/2 their gates), -1 past the end
     template <int BN> __device__ int col_of(const Cta& c, int j) const {
         if (glu) {
-            const int H = Ntot / 2, cc = c.n_tile * (BN / 2) + (j % (BN / 2));
+            const int H = Ntot / 2, cc = c.n_tile * (BN / 2) + (int)((unsigned)j % (BN / 2));
             return cc < H ? cc + (j >= BN / 2 ? H : 0) : -1;
         }
         const int n = c.n_tile * BN + j;
         return n < Ntot ? n : -1;
     }
-    // B operand, in three steps so that the producer can issue a whole tile's loads back to back:
+    // B operand, in steps so that the producer can issue a whole tile's loads back to back and ahead of their use:
     //   b_col: element offset of (tile column j, k quad q) within a K block, -1 past the end (the same for every block);
-    //   b_base: element offset of K block kb;  b4<FMT>: the 4 fp32 weights at element offset `off`
+    //   b_base: element offset of K block kb;  b_load<FMT>: the loads of the 4 fp32 weights at element offset `off`, as
+    //   they arrive;  b_value<FMT>: the 4 weights from them
     enum { B_RAW, B_SPLIT, B_F16 };
     __device__ int b_format() const { return w ? (w_lo32 ? B_SPLIT : B_RAW) : B_F16; }
     template <int BN> __device__ int b_col(const Cta& c, int j, int q) const {
@@ -103,23 +107,33 @@ struct ConvOp {
         const int kch = Cin / HG_BK, tap = kb / kch, k0 = (kb - tap * kch) * HG_BK;
         return (long long)(c.wbase + tap) * Ntot * Cin + k0;
     }
-    template <int FMT> __device__ float4 b4(const Cta& c, long long off) const {
+    template <int FMT> __device__ HcB b_load(long long off) const {
+        HcB r;
+        if (FMT == B_F16) {                          // h = the fp16 hi and lo pieces' bits
+            const uint2 h = __ldg(reinterpret_cast<const uint2*>(w_hi + off));
+            const uint2 l = __ldg(reinterpret_cast<const uint2*>(w_lo + off));
+            r.h = make_float4(__uint_as_float(h.x), __uint_as_float(h.y), __uint_as_float(l.x), __uint_as_float(l.y));
+            return r;
+        }
+        r.h = __ldg(reinterpret_cast<const float4*>(w + off));
+        if (FMT == B_SPLIT) r.l = __ldg(reinterpret_cast<const float4*>(w_lo32 + off));
+        return r;
+    }
+    template <int FMT> __device__ float4 b_value(const Cta& c, const HcB& r) const {
         if (FMT != B_F16) {
-            float4 v = __ldg(reinterpret_cast<const float4*>(w + off));
-            if (FMT == B_SPLIT) {
-                const float4 l = __ldg(reinterpret_cast<const float4*>(w_lo32 + off));
-                v.x += l.x; v.y += l.y; v.z += l.z; v.w += l.w;
-            }
+            float4 v = r.h;
+            if (FMT == B_SPLIT) { v.x += r.l.x; v.y += r.l.y; v.z += r.l.z; v.w += r.l.w; }
             return v;
         }
-        const uint2 h = __ldg(reinterpret_cast<const uint2*>(w_hi + off)), l = __ldg(reinterpret_cast<const uint2*>(w_lo + off));
-        const float2 h0 = __half22float2(*reinterpret_cast<const __half2*>(&h.x)), h1 = __half22float2(*reinterpret_cast<const __half2*>(&h.y));
-        const float2 l0 = __half22float2(*reinterpret_cast<const __half2*>(&l.x)), l1 = __half22float2(*reinterpret_cast<const __half2*>(&l.y));
+        const uint32_t hx = __float_as_uint(r.h.x), hy = __float_as_uint(r.h.y);
+        const uint32_t lx = __float_as_uint(r.h.z), ly = __float_as_uint(r.h.w);
+        const float2 h0 = __half22float2(*reinterpret_cast<const __half2*>(&hx)), h1 = __half22float2(*reinterpret_cast<const __half2*>(&hy));
+        const float2 l0 = __half22float2(*reinterpret_cast<const __half2*>(&lx)), l1 = __half22float2(*reinterpret_cast<const __half2*>(&ly));
         return make_float4((h0.x + l0.x) * c.w_inv, (h0.y + l0.y) * c.w_inv, (h1.x + l1.x) * c.w_inv, (h1.y + l1.y) * c.w_inv);
     }
 
-    // run by the 256 consumer threads of hc_conv_kernel; PASSES only gives each kernel instantiation its own col_sums (a
-    // static shared array shared by the 3- and 1-pass kernels would change the shared-memory layout of both)
+    // run by the 256 consumer threads of hc_conv_kernel, once per tile; PASSES only gives each kernel instantiation its own
+    // col_sums (a static shared array shared by the 3- and 1-pass kernels would change the shared-memory layout of both)
     template <int BN, int PASSES> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
         __shared__ double col_sums[2 * BN];
         float am = 0.f;
@@ -139,6 +153,7 @@ struct ConvOp {
             }
         } else {
             if (stats) {
+                hc_consumer_sync();                      // the previous tile's reads of col_sums, before they are cleared
                 for (int i = hc_consumer_tid(); i < 2 * BN; i += HC_CONSUMERS) col_sums[i] = 0.0;
                 hc_consumer_sync();
             }
@@ -233,15 +248,13 @@ inline ConvOp conv_op_defaults() {
 inline int launch_conv_op(ConvOp o, cudaStream_t st, const char* who) {
     if ((long long)o.B * o.T >= (1ll << 31)) return set_error(2, "%s: too many rows%s", who);
     o.ttiles = (o.T + HG_BM - 1) / HG_BM;
-    const long long ctas = (long long)o.B * o.ttiles;
-    if (ctas >= (1ll << 31)) return set_error(2, "%s: too many rows%s", who);
     const int bn = hg_pick_bn(o.Ntot);                   // GLU: BN/2 'a' columns and their gates per tile
-    const int ntiles = o.glu ? (o.Ntot / 2 + bn / 2 - 1) / (bn / 2) : (o.Ntot + bn - 1) / bn;
+    o.ncols = o.glu ? (o.Ntot / 2 + bn / 2 - 1) / (bn / 2) : (o.Ntot + bn - 1) / bn;
     if (o.stats) {
         cudaError_t em = cudaMemsetAsync(o.stats, 0, sizeof(double) * 2 * o.Ntot, st);
         if (em != cudaSuccess) return set_error(3, "%s: memset: %s", who, cudaGetErrorString(em));
     }
-    return hc_launch_bn(bn, o, dim3((unsigned)ctas, (unsigned)ntiles, 1), st, who);
+    return hc_launch_bn(bn, o, (long long)o.B * o.ttiles * o.ncols, st, who);
 }
 
 // W[o][i][j] (nn.Conv1d layout) -> tf32-split K-major operands:
@@ -304,7 +317,8 @@ inline int launch_sensor_mix_bwd_tc(const float* du, const float* w_hi, const fl
     if ((long long)B * T >= (1ll << 31)) return set_error(2, "%s: too many rows%s", __func__);
     o.ttiles = (T + HG_BM - 1) / HG_BM;
     const int bn = hg_pick_bn(Cp);
-    return hc_launch_bn(bn, o, dim3((unsigned)((long long)B * o.ttiles), (unsigned)((Cp + bn - 1) / bn), 1), st, __func__);
+    o.ncols = (Cp + bn - 1) / bn;
+    return hc_launch_bn(bn, o, (long long)B * o.ttiles * o.ncols, st, __func__);
 }
 
 }  // namespace tc
