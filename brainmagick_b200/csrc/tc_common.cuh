@@ -263,7 +263,9 @@ enum HcPhase {
     HP_FULL_WAIT,      // consumer: waiting on the full barrier
     HP_SPLIT_ADD,      // consumer: A fragment split + stage release + acc += part
     HP_MMA,            // consumer: wgmma issue to drain (wait_group 0)
-    HP_EPILOGUE,       // consumer: the tile's epilogue
+    HP_EPI_LOAD,       // consumer epilogue: its loads (bias, addend, mask) until they are issued
+    HP_EPI_STORE,      // consumer epilogue: the math and the stores (hw_wgrad_kernel: its whole epilogue)
+    HP_EPI_STATS,      // consumer epilogue: BatchNorm statistics and max |output| after the last store
     HP_C_BLOCKS,       // consumer: K blocks (count)
     HP_TILES,          // consumer: tiles (count)
     HP_EMPTY_WAIT,     // producer: waiting on the empty barrier
@@ -725,8 +727,8 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_con
                 pr);
             pos = s == HC_STAGES - 1 ? (pos & ~7u) | ((pos & 4) ^ 4) : pos + 1;
         }
-        op.template epilogue<BN, PASSES>(op.template cta<BN>(tile), acc, 64 * cg);
-        pr.mark(HP_EPILOGUE);
+        op.template epilogue<BN, PASSES>(op.template cta<BN>(tile), acc, 64 * cg, pr);
+        pr.mark(HP_EPI_STATS);
         pr.count(HP_TILES);
     }
     pr.flush(0);
@@ -934,7 +936,7 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
             pr);
     }
     op.template epilogue<BN>(cta, acc, 64 * cg);
-    pr.mark(HP_EPILOGUE);
+    pr.mark(HP_EPI_STORE);
     pr.count(HP_TILES);
     pr.flush(1);
 }

@@ -132,75 +132,142 @@ struct ConvOp {
         return make_float4((h0.x + l0.x) * c.w_inv, (h0.y + l0.y) * c.w_inv, (h1.x + l1.x) * c.w_inv, (h1.y + l1.y) * c.w_inv);
     }
 
-    // run by the 256 consumer threads of hc_conv_kernel, once per tile; PASSES only gives each kernel instantiation its own
-    // col_sums (a static shared array shared by the 3- and 1-pass kernels would change the shared-memory layout of both)
-    template <int BN, int PASSES> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
-        __shared__ double col_sums[2 * BN];
+    // Run by the 256 consumer threads of hc_conv_kernel, once per tile.  Element i of the thread's fragment is row
+    // t0 + m0 + hg_row(i) (two rows per thread: r and r + 8) and tile column hg_col(i); elements i and i + 1 (i even) are
+    // two adjacent columns, so the row-major outputs are stored as float2 (Ntot, H and every column offset are even; the
+    // launcher checks the pointers' 8-byte alignment).  A column group's loads (bias, addend) are all issued before its
+    // first store: `addend` may alias `y`, so a load behind a store would wait for it, one L2 round trip per element.
+    // Hoisting the addend above the y stores is legal: each element is read and then written by this thread alone.
+    // BatchNorm statistics: each warp's per-column fp32 sums over its 16 rows (shuffle tree over the 8 row lanes) go to
+    // `partial` with plain stores; after a consumer barrier one thread per column adds the 8 warps' partials in fixed order
+    // in fp64 and issues the global fp64 atomics.  PASSES only gives each kernel instantiation its own `partial` (a static
+    // shared array shared by the 3- and 1-pass kernels would change the shared-memory layout of both).
+    template <int BN, int PASSES> __device__ void epilogue(const Cta& c, const float* acc, int m0, HcProbe& pr) const {
+        constexpr int NW = HC_CONSUMERS / 32, NG = BN / 8;    // consumer warps; 8-column groups of the fragment
+        constexpr int GS = NG / 2;                           // column groups per load batch (registers: acc + 60)
+        __shared__ __align__(8) float partial[NW][2][BN];
+        const int tq = threadIdx.x & 3, t = c.t0 + m0 + hg_row(0);
+        const bool r_ok[2] = {t < T, t + 8 < T};
+        const long long row = (long long)c.b * T + t;          // the thread's rows: row and row + 8
         float am = 0.f;
         if (glu) {
-            const int H = Ntot / 2;
+            const int H = Ntot / 2, c0 = c.n_tile * (BN / 2) + 2 * tq;   // 'a' columns c0 + 8 g (+1); gates at + H
+            float2 ba[NG / 2], bg[NG / 2];
 #pragma unroll
-            for (int i = 0; i < BN / 4; ++i) {           // tile columns 0..BN/2-1; the gate of column j is column j + BN/2
-                const int t = c.t0 + m0 + hg_row(i), cc = c.n_tile * (BN / 2) + hg_col(i);
-                if (t >= T || cc >= H) continue;
-                const long long row = (long long)c.b * T + t;
-                float a = acc[i], g = acc[i + BN / 4];
-                if (bias) { a += bias[cc]; g += bias[H + cc]; }
-                if (y) { y[row * Ntot + cc] = a; y[row * Ntot + H + cc] = g; }
-                const float o = a * sigmoid_f(g);
-                glu_out[row * H + cc] = o;
-                am = fmaxf(am, fabsf(o));
+            for (int g = 0; g < NG / 2; ++g) {
+                const int cc = c0 + 8 * g;
+                ba[g] = bg[g] = make_float2(0.f, 0.f);
+                if (bias && cc < H) {
+                    ba[g] = __ldg(reinterpret_cast<const float2*>(bias + cc));
+                    bg[g] = __ldg(reinterpret_cast<const float2*>(bias + H + cc));
+                }
             }
+            pr.mark(HP_EPI_LOAD);
+#pragma unroll
+            for (int g = 0; g < NG / 2; ++g) {             // tile columns 0..BN/2-1; the gate of column j is column j + BN/2
+                const int cc = c0 + 8 * g;
+                if (cc >= H) continue;
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    if (!r_ok[h]) continue;
+                    const int i = 4 * g + 2 * h;
+                    const long long r = row + 8 * h;
+                    float2 a = make_float2(acc[i], acc[i + 1]), gt = make_float2(acc[i + BN / 4], acc[i + 1 + BN / 4]);
+                    if (bias) { a.x += ba[g].x; a.y += ba[g].y; gt.x += bg[g].x; gt.y += bg[g].y; }
+                    if (y) {
+                        *reinterpret_cast<float2*>(y + r * Ntot + cc) = a;
+                        *reinterpret_cast<float2*>(y + r * Ntot + H + cc) = gt;
+                    }
+                    const float2 o = make_float2(a.x * sigmoid_f(gt.x), a.y * sigmoid_f(gt.y));
+                    *reinterpret_cast<float2*>(glu_out + r * H + cc) = o;
+                    am = fmaxf(am, fmaxf(fabsf(o.x), fabsf(o.y)));
+                }
+            }
+            pr.mark(HP_EPI_STORE);
         } else {
-            if (stats) {
-                hc_consumer_sync();                      // the previous tile's reads of col_sums, before they are cleared
-                for (int i = hc_consumer_tid(); i < 2 * BN; i += HC_CONSUMERS) col_sums[i] = 0.0;
-                hc_consumer_sync();
-            }
+            const int n0 = c.n_tile * BN + 2 * tq;            // the thread's columns: n0 + 8 g (+1)
+            const int warp = hc_consumer_tid() >> 5;
 #pragma unroll
-            for (int g = 0; g < BN / 8; ++g) {
+            for (int g0 = 0; g0 < NG; g0 += GS) {
+                float2 bv[GS], av[GS][2];
 #pragma unroll
-                for (int e = 0; e < 2; ++e) {
-                    float s1 = 0.f, s2 = 0.f;
-                    const int j = 8 * g + 2 * (threadIdx.x & 3) + e, n = c.n_tile * BN + j;
+                for (int k = 0; k < GS; ++k) {
+                    const int n = n0 + 8 * (g0 + k);
+                    bv[k] = av[k][0] = av[k][1] = make_float2(0.f, 0.f);
+                    if (n >= Ntot) continue;
+                    if (bias) bv[k] = __ldg(reinterpret_cast<const float2*>(bias + n));
+                    if (addend) {
 #pragma unroll
-                    for (int h = 0; h < 2; ++h) {
-                        const int i = 4 * g + 2 * h + e;
-                        const int t = c.t0 + m0 + hg_row(i);
-                        if (t >= T || n >= Ntot) continue;
-                        const long long row = (long long)c.b * T + t;
-                        float v = acc[i];
-                        if (bias) v += bias[n];
-                        if (addend) v += addend[row * Ntot + n];
-                        if (aux) aux[row * Ntot + n] = v;
-                        if (act) { v = gelu_f(v); am = fmaxf(am, fabsf(v)); }
-                        if (out_tmajor) y[((long long)c.b * Ntot + n) * T + t] = v;
-                        else y[row * Ntot + n] = v;
-                        s1 += v;
-                        s2 = fmaf(v, v, s2);
+                        for (int h = 0; h < 2; ++h)
+                            if (r_ok[h]) av[k][h] = *reinterpret_cast<const float2*>(addend + (row + 8 * h) * Ntot + n);
+                    }
+                }
+                pr.mark(HP_EPI_LOAD);
+#pragma unroll
+                for (int k = 0; k < GS; ++k) {
+                    const int g = g0 + k, n = n0 + 8 * g;
+                    float s1[2] = {0.f, 0.f}, s2[2] = {0.f, 0.f};     // columns n and n + 1, summed over rows r, r + 8
+                    if (n < Ntot) {
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            if (!r_ok[h]) continue;
+                            const long long r = row + 8 * h;
+                            float v[2] = {acc[4 * g + 2 * h], acc[4 * g + 2 * h + 1]};
+                            if (bias) { v[0] += bv[k].x; v[1] += bv[k].y; }
+                            if (addend) { v[0] += av[k][h].x; v[1] += av[k][h].y; }
+                            if (aux) *reinterpret_cast<float2*>(aux + r * Ntot + n) = make_float2(v[0], v[1]);
+                            if (act) {
+                                v[0] = gelu_f(v[0]);
+                                v[1] = gelu_f(v[1]);
+                                am = fmaxf(am, fmaxf(fabsf(v[0]), fabsf(v[1])));
+                            }
+                            if (out_tmajor) {
+                                y[((long long)c.b * Ntot + n) * T + t + 8 * h] = v[0];
+                                y[((long long)c.b * Ntot + n + 1) * T + t + 8 * h] = v[1];
+                            } else {
+                                *reinterpret_cast<float2*>(y + r * Ntot + n) = make_float2(v[0], v[1]);
+                            }
+                            if (stats) {
+#pragma unroll
+                                for (int e = 0; e < 2; ++e) {
+                                    s1[e] += v[e];
+                                    s2[e] = fmaf(v[e], v[e], s2[e]);
+                                }
+                            }
+                        }
                     }
                     if (stats) {
 #pragma unroll
-                        for (int o = 4; o < 32; o <<= 1) {
-                            s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-                            s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+                        for (int e = 0; e < 2; ++e) {
+#pragma unroll
+                            for (int o = 4; o < 32; o <<= 1) {
+                                s1[e] += __shfl_xor_sync(0xffffffffu, s1[e], o);
+                                s2[e] += __shfl_xor_sync(0xffffffffu, s2[e], o);
+                            }
                         }
-                        if ((threadIdx.x & 31) < 4 && n < Ntot) {
-                            atomicAdd(&col_sums[j], (double)s1);
-                            atomicAdd(&col_sums[BN + j], (double)s2);
+                        if ((threadIdx.x & 31) < 4) {
+                            const int j = 8 * g + 2 * tq;
+                            *reinterpret_cast<float2*>(&partial[warp][0][j]) = make_float2(s1[0], s1[1]);
+                            *reinterpret_cast<float2*>(&partial[warp][1][j]) = make_float2(s2[0], s2[1]);
                         }
                     }
                 }
+                pr.mark(HP_EPI_STORE);
             }
             if (stats) {
-                hc_consumer_sync();
-                for (int j = hc_consumer_tid(); j < BN; j += HC_CONSUMERS) {
-                    const int n = c.n_tile * BN + j;
-                    if (n < Ntot) {
-                        atomicAdd(stats + n, col_sums[j]);
-                        atomicAdd(stats + Ntot + n, col_sums[BN + j]);
+                hc_consumer_sync();                      // every warp's partials of this tile are in `partial`
+                const int j = hc_consumer_tid(), n = c.n_tile * BN + j;
+                if (j < BN && n < Ntot) {
+                    double d1 = 0.0, d2 = 0.0;
+#pragma unroll
+                    for (int w = 0; w < NW; ++w) {
+                        d1 += (double)partial[w][0][j];
+                        d2 += (double)partial[w][1][j];
                     }
+                    atomicAdd(stats + n, d1);
+                    atomicAdd(stats + Ntot + n, d2);
                 }
+                hc_consumer_sync();                      // the reads, before the next tile's partials overwrite them
             }
         }
         if (out_amax) {
@@ -214,26 +281,34 @@ struct ConvOp {
 // Data gradient of the sensor mix (ChannelMerger, common.py:358) as a pointwise ConvOp with one weight set per recording:
 //   dmeg[b, c, t] = mask[c] * sum_o du[b, t, o] * W[wsel[b]][c][o]
 // x = du [B,T,Cin=Op], w = the transposed attention weights [R][Ntot=Cp][Op].  Its own epilogue stores only the C live sensor
-// rows, channel-major [B,C,T], times the channel mask (nullable); the ConvOp epilogue itself is untouched.
+// rows, channel-major [B,C,T], times the channel mask (nullable; its columns are loaded before the first store); the
+// ConvOp epilogue itself is untouched.
 struct SensorMixBwdOp : ConvOp {
     int C;
     const float* mask;
-    template <int BN, int PASSES> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
+    template <int BN, int PASSES> __device__ void epilogue(const Cta& c, const float* acc, int m0, HcProbe& pr) const {
+        const int n0 = c.n_tile * BN + 2 * (threadIdx.x & 3), t = c.t0 + m0 + hg_row(0);   // columns n0 + 8 g + e
+        float m[BN / 8][2];
+#pragma unroll
+        for (int g = 0; g < BN / 8; ++g)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+                const int n = n0 + 8 * g + e;
+                m[g][e] = mask && n < C ? __ldg(mask + n) : 1.f;
+            }
+        pr.mark(HP_EPI_LOAD);
 #pragma unroll
         for (int g = 0; g < BN / 8; ++g) {
 #pragma unroll
             for (int e = 0; e < 2; ++e) {
-                const int n = c.n_tile * BN + 8 * g + 2 * (threadIdx.x & 3) + e;
+                const int n = n0 + 8 * g + e;
                 if (n >= C) continue;
-                const float m = mask ? mask[n] : 1.f;
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int i = 4 * g + 2 * h + e;
-                    const int t = c.t0 + m0 + hg_row(i);
-                    if (t < T) y[((long long)c.b * C + n) * T + t] = acc[i] * m;
-                }
+                for (int h = 0; h < 2; ++h)
+                    if (t + 8 * h < T) y[((long long)c.b * C + n) * T + t + 8 * h] = acc[4 * g + 2 * h + e] * m[g][e];
             }
         }
+        pr.mark(HP_EPI_STORE);
     }
 };
 
@@ -247,6 +322,9 @@ inline ConvOp conv_op_defaults() {
 
 inline int launch_conv_op(ConvOp o, cudaStream_t st, const char* who) {
     if ((long long)o.B * o.T >= (1ll << 31)) return set_error(2, "%s: too many rows%s", who);
+    auto a8 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; };     // the epilogue's float2 accesses
+    if (!a8(o.bias) || !a8(o.addend) || !a8(o.aux) || !a8(o.glu_out) || (!o.out_tmajor && !a8(o.y)))
+        return set_error(2, "%s: bias, addend and the row-major outputs must be 8-byte aligned%s", who);
     o.ttiles = (o.T + HG_BM - 1) / HG_BM;
     const int bn = hg_pick_bn(o.Ntot);                   // GLU: BN/2 'a' columns and their gates per tile
     o.ncols = o.glu ? (o.Ntot / 2 + bn / 2 - 1) / (bn / 2) : (o.Ntot + bn - 1) / bn;

@@ -12,7 +12,9 @@ shapes of the cfg2 training step (B = 256, T = 360) and the three conv weight gr
   subj        subject layers 288 -> 320 with 4 per-sample weight sets    (bm_tc_pointwise_sel)
   wg_k3, wg_k4, wg_head   bm_tc_wgrad_conv at 320 x 320 x 3, 640 x 320 x 3, 640 x 1024 x 1
 
-Per shape and pass count it prints, in SM clocks: the consumer warpgroup's full-barrier wait, A split + release + adds and MMA issue-to-drain per K block, and its epilogue per tile; the producer's empty-barrier wait,
+Per shape and pass count it prints, in SM clocks: the consumer warpgroup's full-barrier wait, A split + release + adds and MMA issue-to-drain per K block, and its epilogue per tile in three phases (load: the bias / addend / mask loads until issued; store: the math and the
+stores; stats: BatchNorm statistics and max |output| after the last store; the weight gradient's whole epilogue is
+`store`); the producer's empty-barrier wait,
 B load latency (issue, or the point of use when loaded ahead, to registers) and TMA / store / fence / arrive per K block,
 and its start-to-first-full per CTA; and the launch's wall time (CUDA events, probe build: the clock reads cost a little).
 
@@ -38,7 +40,7 @@ import torch  # noqa: E402
 
 from brainmagick_b200 import _lib, build  # noqa: E402
 
-PHASES = ["full_wait", "split_add", "mma", "epilogue", "c_blocks", "tiles",
+PHASES = ["full_wait", "split_add", "mma", "epi_load", "epi_store", "epi_stats", "c_blocks", "tiles",
           "empty_wait", "b_load", "store", "first_full", "p_blocks", "ctas"]          # tc_common.cuh HcPhase
 B, T = 256, 360
 # name: (entry, Cin, Ntot, Kw, dilation, sign, mode)
@@ -113,7 +115,9 @@ def breakdown(c, kernel, launches):
              ctas=v["ctas"] // launches)
     r["consumer_per_kblock"] = {k: round(v[k] / cb, 1) for k in ("full_wait", "split_add", "mma")}
     r["consumer_per_kblock"]["total"] = round(sum(r["consumer_per_kblock"].values()), 1)
-    r["consumer_epilogue_per_tile"] = round(v["epilogue"] / max(v["tiles"], 1), 1)
+    r["consumer_epilogue_per_tile"] = {k[4:]: round(v[k] / max(v["tiles"], 1), 1) for k in ("epi_load", "epi_store",
+                                                                                             "epi_stats")}
+    r["consumer_epilogue_per_tile"]["total"] = round(sum(r["consumer_epilogue_per_tile"].values()), 1)
     r["producer_per_kblock"] = {k: round(v[k] / pb, 1) for k in ("empty_wait", "b_load", "store")}
     r["producer_first_full_per_cta"] = round(v["first_full"] / max(v["ctas"], 1), 1)
     return r
