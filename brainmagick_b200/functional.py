@@ -22,16 +22,35 @@ from . import _lib
 from ._lib import call, ptr, stream
 
 
+ACT_GELU, ACT_LRELU, ACT_NONE = 0, 1, 2      # activation codes of the epilogue kernels
+
+
 @dataclasses.dataclass
-class EncoderPlan:
-    """Everything `encoder_forward` needs that is not a differentiable tensor."""
+class SequencePlan:
+    """The layers of a ConvSequence (bm/models/common.py:79-151) as `conv_stack_forward` / `conv_stack_backward` run them:
+    layer k is conv (+ BatchNorm if `batch_norm` and has_act[k]) (+ activation if has_act[k]) (+ the layer input if `skip`
+    and the conv keeps the width), then a GLU block if glu_after[k]."""
     dilations: tp.List[int]
     glu_after: tp.List[bool]
-    kernel_size: int
-    glu_kernel: int
+    has_act: tp.List[bool]            # layer k ends with (BatchNorm +) activation (activation_on_last, common.py:112)
+    batch_norm: bool
+    act_code: int                     # ACT_GELU, or ACT_LRELU with slope act_slope (ReLU: slope 0)
+    act_slope: float
+    skip: bool
     training: bool
     bn_eps: float
     bn_momentum: float
+    bn_buffers: tp.List[tp.Optional[tp.Tuple[torch.Tensor, torch.Tensor]]]   # (running_mean, running_var) per layer
+    use_tensor_cores: bool
+    keep_for_backward: bool
+
+
+@dataclasses.dataclass
+class EncoderPlan(SequencePlan):
+    """Everything `encoder_forward` needs that is not a differentiable tensor.  SimpleConv's ConvSequence has BatchNorm and
+    an activation on every layer, except a bare last layer when complex_out=False (simpleconv.py:190-193)."""
+    kernel_size: int
+    glu_kernel: int
     rec_positions: torch.Tensor            # [R,C,2] fp32, rows = recordings present in the batch
     rec_of_sample: torch.Tensor            # [B] int32 -> row of rec_positions
     rec_order: torch.Tensor                # [B] int32 samples sorted by recording
@@ -40,19 +59,16 @@ class EncoderPlan:
     freq: torch.Tensor                     # [sqrt(P/2)] fp32 Fourier frequencies
     ban_centre: tp.Optional[torch.Tensor]  # [2] fp32 or None
     ban_radius: float
-    bn_buffers: tp.List[tp.Tuple[torch.Tensor, torch.Tensor]]   # (running_mean, running_var) per layer
-    keep_for_backward: bool = True
-    use_tensor_cores: bool = True
-    skip: bool = True                      # ConvSequence(skip=...): residual where a layer keeps its width (common.py:146-147)
-    act_code: int = 0                      # 0 = GELU (clip_conv); 1 = LeakyReLU(act_slope), i.e. simpleconv.gelu=False
-    act_slope: float = 0.0
-    bare_last: bool = False                # simpleconv.complex_out=False: no head, the last conv maps to out_channels and
-                                           # has neither BatchNorm nor activation (simpleconv.py:190-193)
     staged: bool = False                   # a sensor-chain stage is missing (merger / initial_linear / subject_layers
                                            # ablations) or a subject embedding is appended: run the chain stage by stage
     has_sub_emb: bool = False              # the last tensor argument is the [B, E] subject-embedding rows
     channel_mask: tp.Optional[torch.Tensor] = None   # [C] subsample_meg_channels mask (simpleconv.py:200-203), or None
     masked_meg: tp.Optional[torch.Tensor] = None     # [B,C,T] buffer that receives meg * channel_mask
+
+    @property
+    def bare_last(self) -> bool:
+        """no head: the last conv maps to out_channels and has neither BatchNorm nor activation"""
+        return not self.has_act[-1]
 
 
 def _empty(shape, like, dtype=torch.float32):
@@ -84,7 +100,6 @@ def check_tc_status(device=None) -> None:
 
 
 OVERLAP_WGRAD = True   # weight-gradient kernels on a side stream, concurrent with the data-gradient kernels of the layer
-USE_CONV_PP = True     # raw-weight conv entry point (tc_convp.cuh) where its shape gate fits
 
 
 _side_streams: tp.Dict[torch.device, torch.cuda.Stream] = {}
@@ -159,33 +174,18 @@ def col_stats(y, rows, C, stats, st):
         call("bm_col_stats", ptr(y), rows, C, ptr(stats), st)
 
 
-# The fp16-piece entry points (bm_tc_conv1d_f16, bm_tc_wgrad_conv_f16: operands as fp16 hi/lo pieces of power-of-two-scaled
-# tensors, with their amax) compute on the same 3xTF32 engine as the fp32 ones, so on this GPU they would only add the amax
-# passes and the fp16 weight preparation to every step: off by default, kept switchable for the ABI's callers.
-USE_CONV_F16 = False
-USE_WGRAD_F16 = False
-USE_WGRAD_PP = True    # all-taps weight-gradient GEMM (tc_wgradp.cuh) where its 256-row padding wastes < 10 %
-
-
-def tc_wgrad(dy, x, B, T, M, N, Ntrue, kw, dilation, status, dbias=None, dy_amax=None, x_amax=None):
+def tc_wgrad(dy, x, B, T, M, N, Ntrue, kw, dilation, status, dbias=None):
     """dw[m][n][tap] = sum_{b,t} dy[b,t,m] x[b,t+(tap-kw//2)*dilation,n] on the tensor cores -> [M, Ntrue, kw];
-    `dbias` [M] (optional) receives sum_{b,t} dy[b,t,m].  `dy_amax` / `x_amax` (USE_WGRAD_F16 only): device floats with
-    max |dy| / max |x| when their producers reported them, else a bm_amax pass here."""
+    `dbias` [M] (optional) receives sum_{b,t} dy[b,t,m]."""
     lib = _lib.load()
     dw = _empty((M, Ntrue, kw), dy)
     rows = kw * N                                       # output rows of the pair kernel, tiled in blocks of 256
-    pair_ok = USE_WGRAD_PP and bool(lib.bm_tc_wgrad_conv_supported(T, M, N, kw)) and \
+    pair_ok = bool(lib.bm_tc_wgrad_conv_supported(T, M, N, kw)) and \
         rows / (-(-rows // 256) * 256) >= 0.9            # else the single-CTA kernel wastes less on padding rows
     if pair_ok:
         ws = _empty((int(lib.bm_tc_wgrad_conv_workspace(B, T, M, N, kw)),), dy)
-        if USE_WGRAD_F16:
-            dy_amax = tensor_amax(dy) if dy_amax is None else dy_amax
-            x_amax = tensor_amax(x) if x_amax is None else x_amax
-            call("bm_tc_wgrad_conv_f16", ptr(dy), ptr(dy_amax), ptr(x), ptr(x_amax), B, T, M, N, Ntrue, kw, dilation, ptr(ws),
-                 ptr(dw), ptr(status), stream())
-        else:
-            _tc_call("bm_tc_wgrad_conv", ptr(dy), ptr(x), B, T, M, N, Ntrue, kw, dilation, ptr(ws), ptr(dw), ptr(status),
-                     stream())
+        _tc_call("bm_tc_wgrad_conv", ptr(dy), ptr(x), B, T, M, N, Ntrue, kw, dilation, ptr(ws), ptr(dw), ptr(status),
+                 stream())
         if dbias is not None:
             col_sum(dy, B * T, M, dbias, stream())
         return dw
@@ -210,20 +210,6 @@ def group_layout(index: torch.Tensor, n_groups: int):
     return order, off
 
 
-def tensor_amax(x: torch.Tensor) -> torch.Tensor:
-    """max |x| as a device float [1] (bm_amax: one pass over x): the F16 pipe's per-tensor scale comes from it."""
-    cell = _empty((1,), x)
-    if x.data_ptr() % 16:                       # the kernel reads float4: a view at an odd offset goes through an aligned copy
-        x = x.clone()
-    call("bm_amax", ptr(x), x.numel(), ptr(cell), stream())
-    return cell
-
-
-def amax_cell(like: torch.Tensor) -> tp.Optional[torch.Tensor]:
-    """A device float for a producer kernel to leave max |output| in (its `amax_out`), when the F16 pipe is in use."""
-    return _empty((1,), like) if USE_CONV_F16 else None
-
-
 class _Conv:
     """One conv layer's prepared operands + the kernel choice (tensor-core or FP32-FMA)."""
 
@@ -241,32 +227,15 @@ class _Conv:
         g = 1 if glu else 0
         # raw-weight entry point (csrc/tc_convp.cuh) where its shape gate fits, else the pre-split one (tc_conv.cuh),
         # else FP32 FMA
-        self.fwd_pp = allow_tc and USE_CONV_PP and bool(lib.bm_tc_conv1d_persistent_supported(T, self.cin, self.cout, self.kw, g))
-        self.bwd_pp = allow_tc and USE_CONV_PP and bool(lib.bm_tc_conv1d_persistent_supported(T, self.cout, self.cin, self.kw, 0))
+        self.fwd_pp = allow_tc and bool(lib.bm_tc_conv1d_persistent_supported(T, self.cin, self.cout, self.kw, g))
+        self.bwd_pp = allow_tc and bool(lib.bm_tc_conv1d_persistent_supported(T, self.cout, self.cin, self.kw, 0))
         fwd_tc = self.fwd_pp or (allow_tc and bool(lib.bm_tc_conv_supported(T, self.cin, self.cout, self.kw, g)))
         bwd_tc = self.bwd_pp or (allow_tc and bool(lib.bm_tc_conv_supported(T, self.cout, self.cin, self.kw, 0)))
         self.fwd_tc, self.bwd_tc = fwd_tc, bwd_tc
         self.wgrad_tc = allow_tc and bool(lib.bm_tc_wgrad_supported(self.cout, self.cin))
         self.f_hi = self.f_lo = self.g_hi = self.g_lo = self.wf = self.wb = None
-        self.f_h16 = self.g_h16 = self.w_amax = None
-        f16_f = USE_CONV_F16 and self.fwd_pp                      # operands of the F16-pipe kernel (tc_convh.cuh)
-        f16_g = USE_CONV_F16 and self.bwd_pp and want_bwd
-        if f16_f or f16_g:
-            # fp16 hi/lo pieces of w * 2^k (k from the weights' largest magnitude), straight into the K-major layouts:
-            # bm_amax + ONE re-layout-and-split launch per layer and step
-            self.w_amax = _empty((1,), w)
-            call("bm_amax", ptr(w), w.numel(), ptr(self.w_amax), st)
-            half = dict(device=w.device, dtype=torch.float16)
-            if f16_f:
-                self.f_h16 = (torch.empty((self.kw, self.cout, self.cin), **half), torch.empty((self.kw, self.cout, self.cin), **half))
-            if f16_g:
-                self.g_h16 = (torch.empty((self.kw, self.cin, self.cout), **half), torch.empty((self.kw, self.cin, self.cout), **half))
-            fh, fl = self.f_h16 if f16_f else (None, None)
-            gh, gl = self.g_h16 if f16_g else (None, None)
-            call("bm_tc_weight_split_f16", ptr(w), ptr(self.w_amax), self.cout, self.cin, self.kw, ptr(fh), ptr(fl), ptr(gh),
-                 ptr(gl), st)
-        need_f = fwd_tc and not f16_f                              # fp32 K-major operands for the TF32-pipe kernels
-        need_g = bwd_tc and want_bwd and not f16_g
+        need_f = fwd_tc                                            # fp32 K-major operands for the tensor-core kernels
+        need_g = bwd_tc and want_bwd
         if need_f or need_g:
             # RAW fp32 for the persistent kernel (it derives the tf32 lo part itself), a pre-split tf32 hi/lo pair for the
             # single-CTA kernel
@@ -283,27 +252,15 @@ class _Conv:
             self.wb = _empty((self.kw, self.cout, self.cin), w) if (want_bwd and not bwd_tc) else None
             call("bm_conv_weight_prep", ptr(w), self.cout, self.cin, self.kw, ptr(self.wf), ptr(self.wb), st)
 
-    def run_tc(self, fwd: bool, x, bias, addend, B, T, dilation, glu, act, tmajor, y, aux, glu_out, stats, status,
-               x_amax=None, out_amax=None):
+    def run_tc(self, fwd: bool, x, bias, addend, B, T, dilation, glu, act, tmajor, y, aux, glu_out, stats, status):
         """One tensor-core conv launch: forward taps (fwd) or the data gradient; `addend` must be None or `y` itself
-        (in-place accumulation) on the persistent kernel.  `x_amax` (F16 pipe): the device float holding max |x| when the
-        producer of x already knows it, else one bm_amax pass here; `out_amax`: a device float that receives max |output| of a
-        GLU / GELU epilogue for the conv that consumes it next (`amax_cell`)."""
+        (in-place accumulation) on the persistent kernel."""
         st = stream()
         if fwd:
             pp, hi, lo, cin, ntot, sign = self.fwd_pp, self.f_hi, self.f_lo, self.cin, self.cout, 1
         else:
             pp, hi, lo, cin, ntot, sign = self.bwd_pp, self.g_hi, self.g_lo, self.cout, self.cin, -1
-        h16 = self.f_h16 if fwd else self.g_h16
-        if pp and h16 is not None:
-            assert addend is None or addend.data_ptr() == y.data_ptr(), "the persistent kernel accumulates in place only"
-            if x_amax is None:
-                x_amax = tensor_amax(x)
-            call("bm_tc_conv1d_f16", ptr(x), ptr(x_amax), ptr(h16[0]), ptr(h16[1]), ptr(self.w_amax), ptr(bias),
-                 0 if addend is None else 1, B, T, cin, ntot, self.kw, dilation, sign, glu, act, tmajor, ptr(y), ptr(aux),
-                 ptr(glu_out), ptr(stats), ptr(out_amax), ptr(status), st)
-            return out_amax
-        elif pp:
+        if pp:
             assert addend is None or addend.data_ptr() == y.data_ptr(), "the persistent kernel accumulates in place only"
             _tc_call("bm_tc_conv1d_persistent", ptr(x), ptr(hi), ptr(bias), 0 if addend is None else 1, B, T, cin, ntot,
                      self.kw, dilation, sign, glu, act, tmajor, ptr(y), ptr(aux), ptr(glu_out), ptr(stats), ptr(status), st)
@@ -311,18 +268,16 @@ class _Conv:
             assert stats is None
             _tc_call("bm_tc_conv1d", ptr(x), ptr(hi), ptr(lo), ptr(bias), ptr(addend), B, T, cin, ntot, self.kw, dilation,
                      sign, glu, act, tmajor, ptr(y), ptr(aux), ptr(glu_out), None, ptr(status), st)
-        return None                        # the tf32 kernels do not report max |output|
 
     # y = conv(x) (+bias); optionally BatchNorm statistics into `stats`
-    def forward(self, x, bias, B, T, dilation, y, stats, status, x_amax=None):
+    def forward(self, x, bias, B, T, dilation, y, stats, status):
         st = stream()
         if self.fwd_tc:
             fused = stats is not None and self.fwd_pp          # BatchNorm statistics out of the conv epilogue
             if self.cout > 320 or _lib.deterministic():
                 fused = False                                   # the kernel keeps the statistics of ONE N tile in smem, and
                                                                 # commits them with atomics
-            self.run_tc(True, x, bias, None, B, T, dilation, 0, 0, 0, y, None, None, stats if fused else None, status,
-                        x_amax=x_amax)
+            self.run_tc(True, x, bias, None, B, T, dilation, 0, 0, 0, y, None, None, stats if fused else None, status)
             if stats is not None and not fused:
                 col_stats(y, B * T, self.cout, stats, st)
         elif stats is not None and _lib.deterministic():
@@ -333,30 +288,28 @@ class _Conv:
             call("bm_conv1d_fwd", ptr(x), ptr(self.wf), ptr(bias), B, T, self.cin, self.cout, self.kw, dilation,
                  ptr(y), ptr(stats), st)
 
-    def forward_glu(self, x, bias, B, T, h, out, status, x_amax=None, out_amax=None):
-        """-> the device float holding max |out| when the kernel produced it (F16 pipe), else None."""
+    def forward_glu(self, x, bias, B, T, h, out, status):
         st = stream()
         if self.fwd_tc:
-            return self.run_tc(True, x, bias, None, B, T, 1, 1, 0, 0, h, None, out, None, status, x_amax=x_amax,
-                               out_amax=out_amax)
+            self.run_tc(True, x, bias, None, B, T, 1, 1, 0, 0, h, None, out, None, status)
         else:
             call("bm_conv1d_glu_fwd", ptr(x), ptr(self.wf), ptr(bias), B, T, self.cin, self.cout // 2, self.kw,
                  ptr(h), ptr(out), st)
 
-    def backward_data(self, dy, addend, B, T, dilation, dx, status, dy_amax=None):
+    def backward_data(self, dy, addend, B, T, dilation, dx, status):
         st = stream()
         if self.bwd_tc:
-            self.run_tc(False, dy, None, addend, B, T, dilation, 0, 0, 0, dx, None, None, None, status, x_amax=dy_amax)
+            self.run_tc(False, dy, None, addend, B, T, dilation, 0, 0, 0, dx, None, None, None, status)
         else:
             call("bm_conv1d_bwd_data", ptr(dy), ptr(self.wb), ptr(addend), B, T, self.cin, self.cout, self.kw,
                  dilation, ptr(dx), st)
 
-    def backward_weight(self, dy, x, B, T, dilation, like, status, bias_grad_is_zero=False, known_dbias=None, dy_amax=None,
-                        x_amax=None, want_w=True, want_b=True):
+    def backward_weight(self, dy, x, B, T, dilation, like, status, bias_grad_is_zero=False, known_dbias=None, want_w=True,
+                        want_b=True):
         """`bias_grad_is_zero`: the conv feeds a training-mode BatchNorm, whose backward makes sum(dy) == 0 exactly
         (the reference's value there is rounding noise around 0); skip the reduction.  `known_dbias`: the producer of dy
-        already summed it over the rows.  `dy_amax` / `x_amax`: see tc_wgrad.  `want_w` / `want_b` False: that parameter is
-        frozen; its gradient is neither computed nor returned (None)."""
+        already summed it over the rows.  `want_w` / `want_b` False: that parameter is frozen; its gradient is neither
+        computed nor returned (None)."""
         if not want_w:
             if not want_b:
                 return None, None
@@ -368,21 +321,19 @@ class _Conv:
             return None, db
         if not want_b:
             if self.wgrad_tc:
-                return tc_wgrad(dy, x, B, T, self.cout, self.cin, self.cin_true, self.kw, dilation, status, dy_amax=dy_amax,
-                                x_amax=x_amax), None
+                return tc_wgrad(dy, x, B, T, self.cout, self.cin, self.cin_true, self.kw, dilation, status), None
             dw = _empty((self.cout, self.cin, self.kw), like)
             _reducing_call("bm_conv1d_bwd_weight", like, (B, T, self.cin, self.cout, self.kw), ptr(dy), ptr(x), B, T,
                            self.cin, self.cout, self.kw, dilation, ptr(dw), None, stream())
             return (dw[:, :self.cin_true].contiguous() if self.cin != self.cin_true else dw), None
         if self.wgrad_tc:
-            am = dict(dy_amax=dy_amax, x_amax=x_amax)
             if known_dbias is not None:
-                return tc_wgrad(dy, x, B, T, self.cout, self.cin, self.cin_true, self.kw, dilation, status, **am), known_dbias
+                return tc_wgrad(dy, x, B, T, self.cout, self.cin, self.cin_true, self.kw, dilation, status), known_dbias
             if bias_grad_is_zero:
-                dw = tc_wgrad(dy, x, B, T, self.cout, self.cin, self.cin_true, self.kw, dilation, status, **am)
+                dw = tc_wgrad(dy, x, B, T, self.cout, self.cin, self.cin_true, self.kw, dilation, status)
                 return dw, torch.zeros((self.cout,), device=like.device)
             db = _empty((self.cout,), like)
-            dw = tc_wgrad(dy, x, B, T, self.cout, self.cin, self.cin_true, self.kw, dilation, status, dbias=db, **am)
+            dw = tc_wgrad(dy, x, B, T, self.cout, self.cin, self.cin_true, self.kw, dilation, status, dbias=db)
             return dw, db
         db = _empty((self.cout,), like)
         dw = _empty((self.cout, self.cin, self.kw), like)
@@ -391,6 +342,163 @@ class _Conv:
         if self.cin != self.cin_true:
             dw = dw[:, :self.cin_true].contiguous()
         return dw, db
+
+
+# ----------------------------------------------------------------------------------------------------
+# The ConvSequence layers (bm/models/common.py:142-151) on channels-last activations: SimpleConv's encoder and the
+# stand-alone ConvSequence / DeepMel both run them through these two functions.
+# ----------------------------------------------------------------------------------------------------
+def conv_stack_forward(plan: SequencePlan, x, conv0: _Conv, conv_p, glu_p, nd: "_Needs", save: bool, B, T, status,
+                       bare_slope: float):
+    """x [B,T,C] -> (output [B,T,C_last], per-layer records for `conv_stack_backward`, None where the backward does not
+    reach).  conv_p[k] = (conv_w, conv_b, gamma, beta), gamma / beta None without BatchNorm; glu_p[k] = (glu_w, glu_b).
+    `conv0`: layer 0's prepared `_Conv`, its input padding chosen by the caller.  `save`: a backward will run.
+    `bare_slope`: the slope handed to the epilogue kernel of a bare conv with a residual (act = none: the kernel ignores it)."""
+    st = stream()
+    rows = B * T
+    tc = plan.use_tensor_cores
+    stats = _empty((2 * max(p[0].shape[0] for p in conv_p),), x, torch.float64)
+    layers = []
+    for k, (w, b, gamma, beta) in enumerate(conv_p):
+        conv = conv0 if k == 0 else _Conv(w, T, False, tc, want_bwd=save and nd.below[k])
+        cout = conv.cout
+        y = _empty((B, T, cout), x)
+        keep = save and nd.below[k + 1]          # the backward reaches this layer
+        has_bn = plan.has_act[k] and plan.batch_norm
+        act = plan.act_code if plan.has_act[k] else ACT_NONE
+        mean = invstd = None
+        if has_bn:
+            mean, invstd = _empty((cout,), x), _empty((cout,), x)
+            rm, rv = plan.bn_buffers[k]
+            if plan.training:
+                conv.forward(x, b.contiguous(), B, T, plan.dilations[k], y, stats, status)
+                call("bm_bn_stats_finalize", ptr(stats), rows, float(plan.bn_eps), float(plan.bn_momentum),
+                     ptr(rm), ptr(rv), ptr(mean), ptr(invstd), cout, st)
+            else:
+                conv.forward(x, b.contiguous(), B, T, plan.dilations[k], y, None, status)
+                call("bm_bn_eval_stats", ptr(rm), ptr(rv), float(plan.bn_eps), ptr(mean), ptr(invstd), cout, st)
+        else:
+            conv.forward(x, b.contiguous(), B, T, plan.dilations[k], y, None, status)
+        skip = plan.skip and conv.cin_true == cout
+        x_new = y                                   # a bare convolution
+        if has_bn or act != ACT_NONE or skip:
+            x_new = _empty((B, T, cout), x)
+            gamma, beta = (gamma.contiguous(), beta.contiguous()) if has_bn else (None, None)
+            if has_bn and act == ACT_GELU:
+                call("bm_bn_gelu_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), ptr(x) if skip else None,
+                     ptr(x_new), rows, cout, None, st)
+            else:
+                call("bm_bn_act_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), ptr(x) if skip else None,
+                     ptr(x_new), rows, cout, act, float(plan.act_slope if plan.has_act[k] else bare_slope), st)
+        # kept: the conv input for its weight gradient, y for the activation backward, x_new for the GLU weight gradient
+        rec = dict(x_in=x if nd.layer[k][0] else None, y=y if plan.has_act[k] and nd.layer_up(k) else None, mean=mean,
+                   invstd=invstd, conv=conv, skip=skip, act=act, has_bn=has_bn,
+                   x_new=x_new if nd.glu.get(k, (False,))[0] else None)
+        x = x_new
+        if plan.glu_after[k]:
+            gw, gb = glu_p[k]
+            gconv = _Conv(gw, T, True, tc, want_bwd=save and nd.layer_up(k))
+            h = _empty((B, T, gconv.cout), x) if keep else None
+            out = _empty((B, T, gconv.cout // 2), x)
+            gconv.forward_glu(x, gb.contiguous(), B, T, h, out, status)
+            rec.update(h=h, gconv=gconv)
+            x = out
+        layers.append(rec if keep else None)
+    return x, layers
+
+
+def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, T, status, side=None, keep_alive=None):
+    """g = dL/d(output of conv_stack_forward) [B,T,C_last] -> (per layer (d conv_w, d conv_b, d gamma, d beta),
+    {k: (d glu_w, d glu_b)}, dL/dx); None for every gradient not asked for, and dL/dx only if nd.below[0].  The backward
+    stops at the deepest layer that needs a gradient.  `side`: a stream for the weight-gradient kernels, concurrent with the
+    data-gradient kernels (None: inline); their operands go to `keep_alive`, which the caller keeps until it has joined the
+    streams (no record_stream: with the host running steps ahead it would block the allocator from reusing ~3 GB of blocks
+    and force cudaMallocs in the timed loop)."""
+    st = stream()
+    rows = B * T
+    like = status                                   # allocations only read the device off it
+    sums = _empty((2 * max(p[0].shape[0] for p in conv_p),), like, torch.float64)
+    layer_grads: tp.List[tp.Any] = [(None, None, None, None)] * len(conv_p)
+    glu_grads = {k: (None, None) for k in nd.glu}
+    main = torch.cuda.current_stream() if side is not None else None
+
+    def weight_grad(conv: _Conv, dy, x, dilation, bias_zero, known_dbias=None, want=(True, True)):
+        if not any(want):
+            return None, None
+        kw = dict(bias_grad_is_zero=bias_zero, known_dbias=known_dbias, want_w=want[0], want_b=want[1])
+        if side is None:
+            return conv.backward_weight(dy, x, B, T, dilation, like, status, **kw)
+        side.wait_stream(main)
+        with torch.cuda.stream(side):
+            out = conv.backward_weight(dy, x, B, T, dilation, like, status, **kw)
+        keep_alive.append((dy, x))
+        for o in out:
+            if o is not None:
+                o.record_stream(main)
+        return out
+
+    for k in reversed(range(len(conv_p))):
+        if not nd.below[k + 1]:
+            break                                  # nothing at or below this layer requires grad
+        rec = layers[k]
+        _, _, gamma, beta = conv_p[k]
+        conv: _Conv = rec["conv"]
+        cout = conv.cout
+        n_cw, n_cb, n_gamma, n_beta = nd.layer[k]
+        if plan.glu_after[k]:
+            gconv: _Conv = rec["gconv"]
+            n_gw, n_gb = nd.glu[k]
+            dh = _empty((B, T, gconv.cout), like)
+            dgb = _empty((gconv.cout,), like) if n_gb else None    # the GLU conv's bias gradient, summed while dh is made
+            _reducing_call("bm_glu_bwd", like, (rows, gconv.cout // 2), ptr(g), ptr(rec["h"]), rows, gconv.cout // 2,
+                           ptr(dh), ptr(dgb), None, st, reduces=n_gb)
+            glu_grads[k] = weight_grad(gconv, dh, rec["x_new"], 1, False, dgb, want=(n_gw, n_gb))
+            if not nd.layer_up(k):
+                del dh
+                break
+            g = _empty((B, T, gconv.cin), like)
+            gconv.backward_data(dh, None, B, T, 1, g, status)
+            del dh
+        dgamma = dbeta = None
+        if rec["has_bn"]:
+            # the batch statistics' backward reduces in training mode; in eval mode only for trainable gamma / beta (else
+            # the BatchNorm + activation backward is one elementwise pass)
+            reduce = plan.training or n_gamma or n_beta
+            dy = _empty((B, T, cout), like)
+            dgamma, dbeta = (_empty((cout,), like), _empty((cout,), like)) if reduce else (None, None)
+            if rec["act"] == ACT_GELU:
+                _reducing_call("bm_bn_gelu_skip_bwd", like, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
+                               ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()),
+                               1 if plan.training else 0, rows, cout, ptr(sums if reduce else None), ptr(dy), ptr(dgamma),
+                               ptr(dbeta), None, st, reduces=reduce)
+            else:
+                _reducing_call("bm_bn_act_skip_bwd", like, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
+                               ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()),
+                               1 if plan.training else 0, rows, cout, rec["act"], float(plan.act_slope),
+                               ptr(sums if reduce else None), ptr(dy), ptr(dgamma), ptr(dbeta), st, reduces=reduce)
+        elif rec["act"] != ACT_NONE:
+            dy = _empty((B, T, cout), like)
+            call("bm_bn_act_skip_bwd", ptr(g), ptr(rec["y"]), None, None, None, None, 0, rows, cout, rec["act"],
+                 float(plan.act_slope), None, ptr(dy), None, None, st)
+        else:
+            # bare convolution: dL/dy = dL/dx_new.  With a residual, g is accumulated in place below while the weight
+            # gradient may still read dy: dy is then a copy
+            dy = g.clone() if (rec["skip"] and nd.below[k]) else g
+        # with a training-mode BatchNorm behind the conv, sum(dy) is exactly 0: no bias reduction
+        dcw, dcb = weight_grad(conv, dy, rec["x_in"], plan.dilations[k], rec["has_bn"] and plan.training,
+                               want=(n_cw, n_cb))
+        if not nd.below[k]:
+            pass
+        elif rec["skip"]:
+            # in place: g += conv_transpose(dy) (addend == output: the pair kernel turns this into a TMA reduce-add)
+            conv.backward_data(dy, g, B, T, plan.dilations[k], g, status)
+        else:
+            g_in = _empty((B, T, conv.cin), like)
+            conv.backward_data(dy, None, B, T, plan.dilations[k], g_in, status)
+            g = g_in
+        layer_grads[k] = (dcw, dcb, dgamma if n_gamma else None, dbeta if n_beta else None)
+        del dy
+    return layer_grads, glu_grads, g
 
 
 # ----------------------------------------------------------------------------------------------------
@@ -703,71 +811,7 @@ class _EncoderFn(torch.autograd.Function):
                      ptr(v), ptr(x), st)
 
         # K3/K4 ConvSequence
-        stats = _empty((2 * H,), meg, torch.float64)
-        saved_layers = []
-        x_amax = None                                   # device float with max |x| when x's producer reported it (F16 pipe)
-        for k in range(depth):
-            cw, cb, gamma, beta = conv_p[k]
-            conv = conv0 if k == 0 else _Conv(cw, T, False, tc, want_bwd=save and nd.below[k])
-            cout = conv.cout
-            y = _empty((B, T, cout), meg)
-            keep = save and nd.below[k + 1]          # the backward reaches this layer
-            if plan.bare_last and k == depth - 1:
-                conv.forward(x, cb.contiguous(), B, T, plan.dilations[k], y, None, status, x_amax=x_amax)
-                x_amax = None
-                skip = plan.skip and conv.cin_true == cout
-                x_new = y
-                if skip:
-                    x_new = _empty((B, T, cout), meg)
-                    call("bm_bn_act_skip_fwd", ptr(y), None, None, None, None, ptr(x), ptr(x_new), rows, cout, 2, 0.0, st)
-                rec = dict(x_in=x if nd.layer[k][0] else None, mean=None, invstd=None, conv=conv, skip=skip,
-                           x_new=x_new if nd.glu.get(k, (False,))[0] else None, bare=True)
-                x = x_new
-                if plan.glu_after[k]:
-                    gw, gb = glu_p[k]
-                    gconv = _Conv(gw, T, True, tc, want_bwd=save and nd.layer_up(k))
-                    h = _empty((B, T, gconv.cout), meg) if keep else None
-                    out = _empty((B, T, gconv.cout // 2), meg)
-                    x_amax = gconv.forward_glu(x, gb.contiguous(), B, T, h, out, status, x_amax=x_amax, out_amax=amax_cell(meg))
-                    rec.update(h=h, gconv=gconv)
-                    x = out
-                saved_layers.append(rec if keep else None)
-                continue
-            mean = _empty((cout,), meg)
-            invstd = _empty((cout,), meg)
-            rm, rv = plan.bn_buffers[k]
-            if plan.training:
-                conv.forward(x, cb.contiguous(), B, T, plan.dilations[k], y, stats, status, x_amax=x_amax)
-                call("bm_bn_stats_finalize", ptr(stats), rows, float(plan.bn_eps), float(plan.bn_momentum),
-                     ptr(rm), ptr(rv), ptr(mean), ptr(invstd), cout, st)
-            else:
-                conv.forward(x, cb.contiguous(), B, T, plan.dilations[k], y, None, status, x_amax=x_amax)
-                call("bm_bn_eval_stats", ptr(rm), ptr(rv), float(plan.bn_eps), ptr(mean), ptr(invstd), cout, st)
-            skip = plan.skip and conv.cin_true == cout
-            x_new = _empty((B, T, cout), meg)
-            x_in_amax, x_amax = x_amax, None
-            if plan.act_code == 0:
-                x_amax = amax_cell(meg)
-                call("bm_bn_gelu_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma.contiguous()),
-                     ptr(beta.contiguous()), ptr(x) if skip else None, ptr(x_new), rows, cout, ptr(x_amax), st)
-            else:
-                call("bm_bn_act_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma.contiguous()),
-                     ptr(beta.contiguous()), ptr(x) if skip else None, ptr(x_new), rows, cout, plan.act_code,
-                     float(plan.act_slope), st)
-            # kept: the conv input for its weight gradient, y for the BatchNorm backward, x_new for the GLU weight gradient
-            rec = dict(x_in=x if nd.layer[k][0] else None, y=y if nd.layer_up(k) else None, mean=mean, invstd=invstd,
-                       conv=conv, skip=skip, x_new=x_new if nd.glu.get(k, (False,))[0] else None, x_in_amax=x_in_amax,
-                       x_new_amax=x_amax)
-            x = x_new
-            if plan.glu_after[k]:
-                gw, gb = glu_p[k]
-                gconv = _Conv(gw, T, True, tc, want_bwd=save and nd.layer_up(k))
-                h = _empty((B, T, gconv.cout), meg) if keep else None
-                out = _empty((B, T, gconv.cout // 2), meg)
-                x_amax = gconv.forward_glu(x, gb.contiguous(), B, T, h, out, status, x_amax=x_amax, out_amax=amax_cell(meg))
-                rec.update(h=h, gconv=gconv)
-                x = out
-            saved_layers.append(rec if keep else None)
+        x, saved_layers = conv_stack_forward(plan, x, conv0, conv_p, glu_p, nd, save, B, T, status, bare_slope=0.0)
 
         if plan.bare_last:
             # no head: the sequence already ends on out_channels; hand it out channel-major
@@ -798,8 +842,7 @@ class _EncoderFn(torch.autograd.Function):
         est = _empty((B, F, T), meg)
         w0_2 = w0.reshape(H2, H).contiguous()
         w2_2 = w2.reshape(H2, F).contiguous()
-        head_generic = plan.act_code != 0
-        q_amax = None
+        head_generic = plan.act_code != ACT_GELU
         if head_generic:
             # simpleconv.gelu=False (simpleconv.py:85-90,187): conv -> activation kernel -> conv, channels-last, then one
             # transpose to the channel-major estimate (the fused GELU epilogues below do not apply)
@@ -812,9 +855,8 @@ class _EncoderFn(torch.autograd.Function):
             call("bm_transpose_nt", ptr(est_cl), B, T, F, ptr(est), st)
             del est_cl
         elif head_tc:
-            q_amax = head0.run_tc(True, x, b0.contiguous(), None, B, T, 1, 0, 1, 0, q, h1 if save else None, None, None, status,
-                                  x_amax=x_amax, out_amax=amax_cell(meg))
-            head2.run_tc(True, q, b2.contiguous(), None, B, T, 1, 0, 0, 1, est, None, None, None, status, x_amax=q_amax)
+            head0.run_tc(True, x, b0.contiguous(), None, B, T, 1, 0, 1, 0, q, h1 if save else None, None, None, status)
+            head2.run_tc(True, q, b2.contiguous(), None, B, T, 1, 0, 0, 1, est, None, None, None, status)
         else:
             call("bm_head_fwd", ptr(x), ptr(w0_2), ptr(b0.contiguous()), ptr(w2_2), ptr(b2.contiguous()), B, T, H, F,
                  ptr(h1), ptr(q), ptr(est), st)
@@ -828,7 +870,7 @@ class _EncoderFn(torch.autograd.Function):
                              subj_w=None if subj_w is None else subj_w.contiguous(), il_conv=il_conv,
                              subj_pad=subj_pad, megT=megT, heads_tc=heads_conv is not None,
                              layers=saved_layers, x_last=x if nd.head[0] else None, w0_2=w0_2, w2_2=w2_2,
-                             h1=h1, q=q if nd.head[2] else None, q_amax=q_amax,
+                             h1=h1, q=q if nd.head[2] else None,
                              head0=head0, head2=head2, head_tc=head_tc, head_generic=head_generic,
                              conv_p=conv_p, glu_p=glu_p, il_shape=None if il_w is None else il_w.shape,
                              w0_shape=w0.shape, w2_shape=w2.shape, front=front, params=(heads, il_w, subj_w, sub_emb))
@@ -893,13 +935,12 @@ class _EncoderFn(torch.autograd.Function):
             dest_t = _empty((B, T, F), meg)
             call("bm_transpose_nt", ptr(dest), B, F, T, ptr(dest_t), st)
             # dq = dest_t @ w2^T  (w2_as_conv [F,2H,1]: its data-gradient operand is [1][2H][F])
-            dest_amax = tensor_amax(dest_t) if USE_CONV_F16 else None      # one pass serves the dgrad and the wgrad below
             lib = _lib.load()
             wgrad_tc = lib.bm_tc_wgrad_supported(H2, F) and lib.bm_tc_wgrad_supported(H2, H)
             if dq is None and not wgrad_tc and (n_w2 or n_b2):
                 dq = _empty((B, T, H2), meg)                               # bm_head_bwd_params turns dq into dh1 in any case
             if dq is not None:
-                head2.run_tc(False, dest_t, None, None, B, T, 1, 0, 0, 0, dq, None, None, None, status, x_amax=dest_amax)
+                head2.run_tc(False, dest_t, None, None, B, T, 1, 0, 0, 0, dq, None, None, None, status)
             if not wgrad_tc:
                 if dw0 is not None or db0 is not None or dw2 is not None or db2 is not None:
                     _reducing_call("bm_head_bwd_params", meg, (B, T, H, F), ptr(dest), ptr(s["x_last"]), ptr(s["h1"]),
@@ -923,8 +964,8 @@ class _EncoderFn(torch.autograd.Function):
 
                 # dW2 / db2 only need dest_t and q: they overlap the dq contraction queued just before
                 if n_w2:
-                    dw2 = on_side(lambda: tc_wgrad(s["q"], dest_t, B, T, H2, F, F, 1, 1, status, dy_amax=s.get("q_amax"),
-                                                   x_amax=dest_amax), s["q"], dest_t, dest_amax).reshape(H2, F)
+                    dw2 = on_side(lambda: tc_wgrad(s["q"], dest_t, B, T, H2, F, F, 1, 1, status), s["q"],
+                                  dest_t).reshape(H2, F)
                 if n_b2:
                     col_sum(dest_t, rows, F, db2, st)
                 if want_dh1:
@@ -943,109 +984,17 @@ class _EncoderFn(torch.autograd.Function):
                            reduces=any(nd.head))
         del dq
 
-        sums = _empty((2 * H,), meg, torch.float64)
-        layer_grads: tp.List[tp.Any] = [(None, None, None, None)] * depth
-        glu_grads = {k: (None, None) for k in nd.glu}
         # The weight gradient and the data gradient of a layer are independent given dy: the weight-gradient kernels go to
         # a side stream so that their CTAs fill the SMs left idle by the partial last wave of the data-gradient kernel
         # (when there is a weight gradient to overlap at all).
         any_wgrad = any(any(n[:2]) for n in nd.layer) or any(any(n) for n in nd.glu.values())
         main = torch.cuda.current_stream()
         side = _side_stream(meg.device) if (OVERLAP_WGRAD and plan.use_tensor_cores and any_wgrad) else None
-        keep_alive: tp.List[tp.Any] = ctx_keep
-
-        def weight_grad(conv_obj, dy_t, x_t, dil, bias_zero, known_dbias=None, dy_amax=None, x_amax=None, want=(True, True)):
-            if not any(want):
-                return None, None
-            kw = dict(bias_grad_is_zero=bias_zero, known_dbias=known_dbias, dy_amax=dy_amax, x_amax=x_amax, want_w=want[0],
-                      want_b=want[1])
-            if side is None:
-                return conv_obj.backward_weight(dy_t, x_t, B, T, dil, meg, status, **kw)
-            side.wait_stream(main)
-            with torch.cuda.stream(side):
-                out = conv_obj.backward_weight(dy_t, x_t, B, T, dil, meg, status, **kw)
-            # the big operands are kept alive until the streams join (no record_stream: with the host running steps ahead
-            # it would block the allocator from reusing ~3 GB of blocks and force cudaMallocs in the timed loop)
-            keep_alive.append((dy_t, x_t, dy_amax, x_amax))
-            for o in out:
-                if o is not None:
-                    o.record_stream(main)
-            return out
-
-        for k in reversed(range(depth)):
-            if not nd.below[k + 1]:
-                break                                  # nothing at or below this layer requires grad
-            rec = s["layers"][k]
-            cw, cb, gamma, beta = s["conv_p"][k]
-            conv: _Conv = rec["conv"]
-            cout = conv.cout
-            n_cw, n_cb, n_gamma, n_beta = nd.layer[k]
-            if plan.glu_after[k]:
-                gconv: _Conv = rec["gconv"]
-                n_gw, n_gb = nd.glu[k]
-                dh = _empty((B, T, gconv.cout), meg)
-                dgb = _empty((gconv.cout,), meg) if n_gb else None    # the GLU conv's bias gradient, summed while dh is made
-                dh_amax = amax_cell(meg)
-                _reducing_call("bm_glu_bwd", meg, (rows, gconv.cout // 2), ptr(g), ptr(rec["h"]), rows, gconv.cout // 2, ptr(dh),
-                               ptr(dgb), ptr(dh_amax), st, reduces=n_gb)
-                glu_grads[k] = weight_grad(gconv, dh, rec["x_new"], 1, False, dgb, dy_amax=dh_amax, x_amax=rec.get("x_new_amax"),
-                                           want=(n_gw, n_gb))
-                if not nd.layer_up(k):
-                    del dh
-                    break
-                g = _empty((B, T, gconv.cin), meg)
-                gconv.backward_data(dh, None, B, T, 1, g, status, dy_amax=dh_amax)
-                del dh
-            if rec.get("bare"):
-                # bare convolution (+ residual): dL/dy = dL/dx_new; no BatchNorm behind it, so the bias gradient is real
-                dy = g.clone() if (rec["skip"] and nd.below[k]) else g
-                dcw, dcb = weight_grad(conv, dy, rec["x_in"], plan.dilations[k], False, want=(n_cw, n_cb))
-                if not nd.below[k]:
-                    pass
-                elif rec["skip"]:
-                    conv.backward_data(dy, g, B, T, plan.dilations[k], g, status)
-                else:
-                    g_in = _empty((B, T, conv.cin), meg)
-                    conv.backward_data(dy, None, B, T, plan.dilations[k], g_in, status)
-                    g = g_in
-                layer_grads[k] = (dcw, dcb, None, None)
-                del dy
-                continue
-            # the batch statistics' backward reduces in training mode; in eval mode only for trainable gamma / beta (else the
-            # BatchNorm + activation backward is one elementwise pass)
-            reduce = plan.training or n_gamma or n_beta
-            dy = _empty((B, T, cout), meg)
-            dgamma = _empty((cout,), meg) if reduce else None
-            dbeta = _empty((cout,), meg) if reduce else None
-            dy_amax = None
-            if plan.act_code == 0:
-                dy_amax = amax_cell(meg)
-                _reducing_call("bm_bn_gelu_skip_bwd", meg, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
-                               ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()), 1 if plan.training else 0,
-                               rows, cout, ptr(sums if reduce else None), ptr(dy), ptr(dgamma), ptr(dbeta), ptr(dy_amax), st,
-                               reduces=reduce)
-            else:
-                _reducing_call("bm_bn_act_skip_bwd", meg, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
-                               ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()), 1 if plan.training else 0,
-                               rows, cout, plan.act_code, float(plan.act_slope), ptr(sums if reduce else None), ptr(dy),
-                               ptr(dgamma), ptr(dbeta), st, reduces=reduce)
-            dcw, dcb = weight_grad(conv, dy, rec["x_in"], plan.dilations[k], plan.training, dy_amax=dy_amax,
-                                   x_amax=rec.get("x_in_amax"), want=(n_cw, n_cb))
-            if not nd.below[k]:
-                pass
-            elif rec["skip"]:
-                # in place: g += conv_transpose(dy) (addend == output: the pair kernel turns this into a TMA reduce-add)
-                conv.backward_data(dy, g, B, T, plan.dilations[k], g, status, dy_amax=dy_amax)
-            else:
-                g_in = _empty((B, T, conv.cin), meg)
-                conv.backward_data(dy, None, B, T, plan.dilations[k], g_in, status, dy_amax=dy_amax)
-                g = g_in
-            layer_grads[k] = (dcw, dcb, dgamma if n_gamma else None, dbeta if n_beta else None)
-            del dy
-
+        layer_grads, glu_grads, g = conv_stack_backward(plan, s["conv_p"], s["layers"], g, nd, B, T, status, side=side,
+                                                        keep_alive=ctx_keep)
         if side is not None:
             main.wait_stream(side)
-        keep_alive.clear()
+        ctx_keep.clear()
         n_meg, n_heads, n_il_w, n_il_b, n_subj, _ = nd.front
         dheads = d_il_w = d_il_b = d_subj = d_sub_emb = dmeg = None
         if not nd.below[0]:

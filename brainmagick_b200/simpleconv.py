@@ -211,7 +211,7 @@ class SimpleConv(nn.Module):
             ban_radius=0.0 if self.merger is None else float(self.merger.dropout),
             bn_buffers=bn_buffers, keep_for_backward=torch.is_grad_enabled(),
             use_tensor_cores=self.use_tensor_cores, skip=seq.skip, act_code=seq.act_code, act_slope=seq.act_slope,
-            bare_last=not seq.has_act[-1], staged=self._staged, has_sub_emb=self.subject_embedding is not None)
+            has_act=list(seq.has_act), batch_norm=True, staged=self._staged, has_sub_emb=self.subject_embedding is not None)
 
     def forward(self, inputs, batch):
         meg = inputs["meg"]

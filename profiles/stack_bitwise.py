@@ -1,0 +1,118 @@
+"""Bitwise fingerprint of deterministic training steps, for comparing two builds of the library's host code.
+
+Under torch.use_deterministic_algorithms(True), from fixed seeds: 3 SimpleConv training steps at bench.py's cfg2 (forward,
+ClipLoss, backward, Adam) and 3 DeepMel training steps at conf/feature_model/deep_mel.yaml's widths (ClipLoss against a
+trainable estimate, Adam on both).  Every loss, estimate, gradient, parameter and BatchNorm running statistic after each step
+is hashed (sha256 of its bytes), so two host-code versions that issue the same kernels must give identical fingerprints.
+
+    python profiles/stack_bitwise.py --dump a.json [--root TREE]    # TREE: the checkout whose brainmagick_b200 is imported
+    python profiles/stack_bitwise.py --compare a.json b.json
+
+Needs cuda:0 for --dump.
+"""
+from __future__ import annotations
+
+import argparse
+import hashlib
+import json
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+def _digest(t) -> str:
+    return hashlib.sha256(t.detach().contiguous().cpu().numpy().tobytes()).hexdigest()
+
+
+def _record(out, tag, loss, est, modules):
+    out[f"{tag}.loss"] = _digest(loss)
+    out[f"{tag}.estimate"] = _digest(est)
+    for m_name, m in modules.items():
+        for name, p in m.named_parameters():
+            out[f"{tag}.{m_name}.grad.{name}"] = None if p.grad is None else _digest(p.grad)
+        for name, v in m.state_dict().items():
+            out[f"{tag}.{m_name}.state.{name}"] = _digest(v)
+
+
+def dump(steps, batch, deepmel_batch):
+    import torch
+    import brainmagick_b200 as bb                  # first: from --root, before bench.py puts this tree on the path
+    from brainmagick_b200 import functional as BF, synthetic
+    sys.path.append(ROOT)
+    import bench
+
+    torch.use_deterministic_algorithms(True)
+    dev = torch.device("cuda:0")
+    torch.cuda.set_device(dev)
+    out = {"library": os.path.abspath(bb.__file__)}
+
+    cfg = bench.CONFIGS["cfg2"]
+    C, T, F, S = cfg["C"], cfg["T"], cfg["F"], cfg["S"]
+    torch.manual_seed(2036)
+    model = bb.SimpleConv(in_channels=dict(meg=C), out_channels=F, n_subjects=S,
+                          **{k: (dict(v) if isinstance(v, dict) else v) for k, v in bench.CLIP_CONV.items()}).to(dev).train()
+    clip = bb.ClipLoss().to(dev).train()
+    opt = torch.optim.Adam(model.parameters(), lr=3e-4)
+    positions = synthetic.normalised_positions(S, C, seed=7)
+    recs = [synthetic.SyntheticRecording(s, positions[s]) for s in range(S)]
+    meg, feats, subj = (t.to(dev) for t in bench.make_host_batch(cfg, batch, 2036))
+    sbatch = synthetic.SyntheticBatch(meg, subj, [recs[s] for s in subj.tolist()])
+    mask = torch.ones(batch, 1, T, dtype=torch.bool, device=dev)
+    for step in range(steps):
+        opt.zero_grad(set_to_none=True)
+        est = model(dict(meg=meg), sbatch)
+        loss = clip(est, feats, mask)
+        loss.backward()
+        _record(out, f"simpleconv.{step}", loss, est, {"model": model})
+        opt.step()
+    BF.check_tc_status()
+
+    torch.manual_seed(2037)
+    dm = bb.DeepMel(n_in_channels=120, n_hidden_channels=320, n_hidden_layers=10, n_out_channels=768, kernel=3, stride=1,
+                    dilation_growth=2, dilation_period=5, batch_norm=True, activation_on_last=False, skip=True,
+                    glu_context=1, glu=2).to(dev).train()
+    mel = torch.randn(deepmel_batch, 120, T, device=dev)
+    brain = torch.randn(deepmel_batch, 768, T, device=dev).requires_grad_(True)
+    opt = torch.optim.Adam(list(dm.parameters()) + [brain], lr=3e-4)
+    mask = torch.ones(deepmel_batch, 1, T, dtype=torch.bool, device=dev)
+    for step in range(steps):
+        opt.zero_grad(set_to_none=True)
+        cand = dm(mel)
+        loss = clip(brain, cand, mask)
+        loss.backward()
+        _record(out, f"deepmel.{step}", loss, cand, {"deepmel": dm})
+        out[f"deepmel.{step}.grad.brain"] = _digest(brain.grad)
+        opt.step()
+    BF.check_tc_status()
+    return out
+
+
+def compare(a, b):
+    keys = sorted((set(a) | set(b)) - {"library"})
+    diff = [k for k in keys if a.get(k) != b.get(k)]
+    print(json.dumps(dict(compared=len(keys), differ=len(diff), first=diff[:20])))
+    return not diff
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--dump", default="")
+    ap.add_argument("--root", default=ROOT, help="tree whose brainmagick_b200 package is imported")
+    ap.add_argument("--compare", nargs=2, default=None)
+    ap.add_argument("--steps", type=int, default=3)
+    ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--deepmel-batch", type=int, default=64)
+    args = ap.parse_args()
+    if args.compare:
+        a, b = (json.load(open(p)) for p in args.compare)
+        sys.exit(0 if compare(a, b) else 1)
+    sys.path.insert(0, os.path.abspath(args.root))
+    res = dump(args.steps, args.batch, args.deepmel_batch)
+    with open(args.dump, "w") as f:
+        json.dump(res, f, indent=0)
+    print(f"{len(res)} fingerprints from {res['library']} -> {args.dump}")
+
+
+if __name__ == "__main__":
+    main()

@@ -5,14 +5,6 @@ import pytest
 import abi_trace
 
 
-@pytest.fixture
-def f16_pieces(monkeypatch):
-    """The fp16-piece host path (functional.USE_CONV_F16 / USE_WGRAD_F16, off by default) switched on."""
-    from brainmagick_b200 import functional
-    monkeypatch.setattr(functional, "USE_CONV_F16", True)
-    monkeypatch.setattr(functional, "USE_WGRAD_F16", True)
-
-
 def test_default_step_prepares_no_fp16_pieces():
     """By default the step runs the fp32 entry points: no amax pass, no fp16 operand preparation, one weight re-layout
     launch per prepared weight set (the forward and data-gradient operands of a layer in the same launch)."""
@@ -25,19 +17,12 @@ def test_default_step_prepares_no_fp16_pieces():
     assert producers and all(c[-2] is False for c in producers)          # amax_out == NULL: no max |output| reductions
 
 
-def test_full_size_step_runs_on_tensor_cores_only(f16_pieces):
+def test_default_full_size_step_runs_on_tensor_cores_only():
     """At the BASELINE widths no FP32-FMA contraction is left in the step."""
     names = {c[0] for c in abi_trace.simpleconv_step(abi_trace.CONFIGS["full"], True)}
     assert not names & {"bm_conv1d_fwd", "bm_conv1d_bwd_data", "bm_conv1d_bwd_weight", "bm_conv1d_glu_fwd", "bm_head_fwd",
                         "bm_head_bwd", "bm_sensor_chain_fwd", "bm_sensor_chain_bwd", "bm_attention_weights_fwd"}
-    assert {"bm_tc_conv1d_f16", "bm_tc_wgrad_conv_f16", "bm_tc_pointwise_sel", "bm_tc_wgrad_grouped"} <= names
-    # F16 pipe: the tensors between two kernels of the conv stack carry their max |.| from the producer; bm_amax passes are
-    # left only in front of the convs whose input comes from elsewhere (sensor chain, head gradient, ...)
-    calls = abi_trace.simpleconv_step(abi_trace.CONFIGS["full"], True)
-    n_conv = sum(c[0] == "bm_tc_conv1d_f16" for c in calls)
-    rows = abi_trace.CONFIGS["full"][0] * abi_trace.CONFIGS["full"][2]                    # B*T: passes over ACTIVATIONS
-    n_pass = sum(c[0] == "bm_amax" and c[2] % rows == 0 for c in calls)
-    assert n_conv >= 30 and n_pass <= 8, (n_conv, n_pass)
+    assert {"bm_tc_conv1d_persistent", "bm_tc_wgrad_conv", "bm_tc_pointwise_sel", "bm_tc_wgrad_grouped"} <= names
 
 
 @pytest.mark.parametrize("override", [dict(glu=0), dict(skip=False), dict(gelu=False), dict(complex_out=False),
@@ -84,14 +69,3 @@ def test_group_layout_matches_bincount_without_a_sync():
         assert torch.equal(order.long(), torch.argsort(idx.long(), stable=True))
         for s in range(n_groups):
             assert (idx[order.long()[off[s]:off[s + 1]]] == s).all()
-
-
-def test_weight_preparation_is_two_launches_per_layer(f16_pieces):
-    """F16 pipe: per conv layer and step, one bm_amax over the nn.Conv1d weight and ONE re-layout-and-split launch."""
-    calls = abi_trace.simpleconv_step(abi_trace.CONFIGS["full"], True)
-    names = [c[0] for c in calls]
-    n_f16_layers = names.count("bm_tc_weight_split_f16")
-    assert n_f16_layers >= 17                                   # 10 conv + 5 GLU + 2 head (+ the sensor-chain 1x1 convs)
-    assert names.count("bm_f16_split") == 0                      # the two-step preparation is not used by the training step
-    # one bm_amax per prepared weight set + the few activation tensors whose producer does not report its maximum
-    assert n_f16_layers <= names.count("bm_amax") <= n_f16_layers + 10
