@@ -264,6 +264,8 @@ __global__ void colsum_strided_kernel(const float* __restrict__ X, float* __rest
 }
 
 // stats[c] += sum_r X[r][c], stats[C+c] += sum_r X[r][c]^2   (fp64 atomics; BatchNorm batch statistics)
+// The per-thread sums are fp64 too: bn_finalize_kernel takes the variance as E[y^2] - E[y]^2, and fp32 partial sums of
+// squares would lose it to rounding once a channel's mean is ~100x its standard deviation.
 // DET: stats is a [gridDim.x][2C] partials buffer
 template <bool DET = false>
 __global__ void col_stats_kernel(const float* __restrict__ X, double* __restrict__ stats, long long rows, int C,
@@ -272,20 +274,20 @@ __global__ void col_stats_kernel(const float* __restrict__ X, double* __restrict
     if (c >= C) return;
     long long r0 = (long long)blockIdx.x * rows_per_block;
     long long r1 = min(rows, r0 + rows_per_block);
-    float s = 0.f, q = 0.f;
+    double s = 0.0, q = 0.0;
 #pragma unroll 4
     for (long long r = r0; r < r1; ++r) {
-        float v = X[r * C + c];
+        const double v = X[r * C + c];
         s += v;
-        q = fmaf(v, v, q);
+        q = fma(v, v, q);
     }
     if (DET) {
-        stats[(long long)blockIdx.x * 2 * C + c] = (double)s;
-        stats[(long long)blockIdx.x * 2 * C + C + c] = (double)q;
+        stats[(long long)blockIdx.x * 2 * C + c] = s;
+        stats[(long long)blockIdx.x * 2 * C + C + c] = q;
         return;
     }
-    atomicAdd(stats + c, (double)s);
-    atomicAdd(stats + C + c, (double)q);
+    atomicAdd(stats + c, s);
+    atomicAdd(stats + C + c, q);
 }
 
 // out[n] += sum_{z,t} X[z][n][t]  (channel-major [Z,N,T]); one warp per (z, n) row

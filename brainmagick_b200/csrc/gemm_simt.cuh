@@ -190,15 +190,18 @@ __global__ void __launch_bounds__(GNT, 2) gemm_simt_kernel(const GemmP p) {
         }
     }
     if (p.stats) {
-        // per-column sum / sumsq over this tile's valid rows -> fp64 atomics (BatchNorm batch statistics)
-        float* red_s = &As[0][0][0];   // [16][128]
-        float* red_q = &Bs[0][0][0];
+        // per-column sum / sumsq over this tile's valid rows -> fp64 atomics (BatchNorm batch statistics).  fp64 from the
+        // first add: bn_finalize_kernel takes the variance as E[y^2] - E[y]^2, and fp32 sums of squares would lose it to
+        // rounding once a channel's mean is ~100x its standard deviation.  The two [16][128] fp64 tables fit in As / Bs.
+        double* red_s = reinterpret_cast<double*>(&As[0][0][0]);
+        double* red_q = reinterpret_cast<double*>(&Bs[0][0][0]);
+        static_assert(sizeof(As) >= 16 * GBN * sizeof(double) && sizeof(Bs) >= 16 * GBN * sizeof(double), "");
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
-            float s = 0.f, q = 0.f;
+            double s = 0.0, q = 0.0;
 #pragma unroll
             for (int i = 0; i < 8; ++i)
-                if (rows[i] >= 0 && cols[j] >= 0) { s += acc[i][j]; q += acc[i][j] * acc[i][j]; }
+                if (rows[i] >= 0 && cols[j] >= 0) { const double v = acc[i][j]; s += v; q = fma(v, v, q); }
             int nn = j < 4 ? tx * 4 + j : 64 + tx * 4 + (j - 4);
             red_s[ty * GBN + nn] = s;
             red_q[ty * GBN + nn] = q;
@@ -209,7 +212,7 @@ __global__ void __launch_bounds__(GNT, 2) gemm_simt_kernel(const GemmP p) {
             if (n >= 0) {
                 double s = 0.0, q = 0.0;
 #pragma unroll
-                for (int r = 0; r < 16; ++r) { s += (double)red_s[r * GBN + tid]; q += (double)red_q[r * GBN + tid]; }
+                for (int r = 0; r < 16; ++r) { s += red_s[r * GBN + tid]; q += red_q[r * GBN + tid]; }
                 atomicAdd(p.stats + n, s);
                 atomicAdd(p.stats + p.N + n, q);
             }

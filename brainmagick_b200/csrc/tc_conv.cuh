@@ -138,9 +138,11 @@ struct ConvOp {
     // launcher checks the pointers' 8-byte alignment).  A column group's loads (bias, addend) are all issued before its
     // first store: `addend` may alias `y`, so a load behind a store would wait for it, one L2 round trip per element.
     // Hoisting the addend above the y stores is legal: each element is read and then written by this thread alone.
-    // BatchNorm statistics: each warp's per-column fp32 sums over its 16 rows (shuffle tree over the 8 row lanes) go to
-    // `partial` with plain stores; after a consumer barrier one thread per column adds the 8 warps' partials in fixed order
-    // in fp64 and issues the global fp64 atomics.  PASSES only gives each kernel instantiation its own `partial` (a static
+    // BatchNorm statistics: each warp's per-column fp32 sums of d = y - bias and d^2 over its 16 rows (shuffle tree over the
+    // 8 row lanes) go to `partial` with plain stores; after a consumer barrier one thread per column adds the 8 warps'
+    // partials in fixed order in fp64, adds the bias back in fp64 and issues the global fp64 atomics.  Unshifted fp32 sums
+    // of y^2 would cancel the variance away in bn_finalize_kernel's E[y^2] - E[y]^2 once the bias puts a channel's mean
+    // ~100x above its standard deviation.  PASSES only gives each kernel instantiation its own `partial` (a static
     // shared array shared by the 3- and 1-pass kernels would change the shared-memory layout of both).
     template <int BN, int PASSES> __device__ void epilogue(const Cta& c, const float* acc, int m0, HcProbe& pr) const {
         constexpr int NW = HC_CONSUMERS / 32, NG = BN / 8;    // consumer warps; 8-column groups of the fragment
@@ -228,10 +230,12 @@ struct ConvOp {
                                 *reinterpret_cast<float2*>(y + r * Ntot + n) = make_float2(v[0], v[1]);
                             }
                             if (stats) {
+                                // about the bias: exact (Sterbenz) while the bias dominates, and what is left is centred
+                                const float d[2] = {v[0] - bv[k].x, v[1] - bv[k].y};
 #pragma unroll
                                 for (int e = 0; e < 2; ++e) {
-                                    s1[e] += v[e];
-                                    s2[e] = fmaf(v[e], v[e], s2[e]);
+                                    s1[e] += d[e];
+                                    s2[e] = fmaf(d[e], d[e], s2[e]);
                                 }
                             }
                         }
@@ -264,8 +268,10 @@ struct ConvOp {
                         d1 += (double)partial[w][0][j];
                         d2 += (double)partial[w][1][j];
                     }
-                    atomicAdd(stats + n, d1);
-                    atomicAdd(stats + Ntot + n, d2);
+                    // back from the bias-shifted sums over the tile's rows: sum (d + b) and sum (d + b)^2
+                    const double b = bias ? (double)__ldg(bias + n) : 0.0, rows = (double)min(HG_BM, T - c.t0);
+                    atomicAdd(stats + n, fma(rows, b, d1));
+                    atomicAdd(stats + Ntot + n, d2 + b * fma(rows, b, 2.0 * d1));
                 }
                 hc_consumer_sync();                      // the reads, before the next tile's partials overwrite them
             }

@@ -56,10 +56,24 @@ def deep_mel_spec(n_in_channels, n_hidden_channels, n_hidden_layers, n_out_chann
     return SequenceSpec(channels=channels, **kw)
 
 
+def convseq_spec(channels, activation: tp.Optional[str] = None, kernel: int = 4, dilation_growth: int = 1,
+                 dilation_period: tp.Optional[int] = None, batch_norm: bool = False, skip: bool = False,
+                 activation_on_last: bool = True, glu: int = 0, glu_context: int = 0, leakiness: float = 0.0,
+                 stride: int = 1) -> SequenceSpec:
+    """SequenceSpec of `ConvSequence(channels, ...)` with the reference constructor's defaults (common.py:81-87).
+    `activation`: None (LeakyReLU(leakiness)), "relu" (nn.ReLU), "leaky_relu" (nn.LeakyReLU: slope 0.01) or "gelu"."""
+    assert stride == 1
+    slope = {None: leakiness, "relu": 0.0, "leaky_relu": 0.01, "gelu": 0.0}[activation]
+    return SequenceSpec(channels=tuple(channels), kernel=kernel, dilation_growth=dilation_growth,
+                        dilation_period=dilation_period, batch_norm=batch_norm, skip=skip,
+                        activation_on_last=activation_on_last, glu=glu, glu_context=glu_context,
+                        activation="gelu" if activation == "gelu" else "lrelu", leakiness=slope)
+
+
 def conv_sequence(x: torch.Tensor, p: tp.Dict[str, torch.Tensor], spec: SequenceSpec, training: bool,
-                  new_stats: tp.Optional[dict] = None) -> torch.Tensor:
+                  new_stats: tp.Optional[dict] = None, pre_act: tp.Optional[list] = None) -> torch.Tensor:
     """x [B, C0, T] -> [B, C_last, T].  `new_stats` (optional dict) receives the BatchNorm running statistics a
-    training forward would leave behind."""
+    training forward would leave behind; `pre_act` (optional list) the input of every activation, detached."""
     for k, dil in enumerate(spec.dilations()):
         old = x
         pre = f"sequence.{k}."
@@ -79,6 +93,8 @@ def conv_sequence(x: torch.Tensor, p: tp.Dict[str, torch.Tensor], spec: Sequence
                     mean, var = p[pre + "1.running_mean"], p[pre + "1.running_var"]
                 x = (x - mean[None, :, None]) / torch.sqrt(var[None, :, None] + spec.bn_eps)
                 x = x * p[pre + "1.weight"][None, :, None] + p[pre + "1.bias"][None, :, None]
+            if pre_act is not None:
+                pre_act.append(x.detach())
             x = F.gelu(x) if spec.activation == "gelu" else F.leaky_relu(x, spec.leakiness)
         if spec.skip and x.shape == old.shape:
             x = x + old

@@ -263,6 +263,77 @@ def run_deepmel(name, c):
           f"|d_cand|={float(cand.grad.norm()):.4e} size={os.path.getsize(os.path.join(OUT, name + '.npz')) / 1024:.0f} KiB")
 
 
+# Stand-alone ConvSequence options that DeepMel's settings leave out (bm/models/common.py:79-151), FMA-sized.  `kw` are the
+# reference constructor's keyword arguments, `activation` a name: None (LeakyReLU(leakiness), the default), "relu",
+# "leaky_relu" (nn.LeakyReLU, slope 0.01) or "gelu".
+CONVSEQ_CASES = {
+    "convseq_kernel1": dict(channels=(6, 8, 8, 5), kw=dict(kernel=1, batch_norm=True, skip=True, activation_on_last=False,
+                                                           leakiness=0.1), activation=None, B=3, T=11, seed=51),
+    "convseq_relu_act_last": dict(channels=(7, 9, 9, 9), kw=dict(kernel=3, dilation_growth=2, batch_norm=True, skip=True,
+                                                                 activation_on_last=True, glu=2, glu_context=1),
+                                  activation="relu", B=4, T=13, seed=52),
+    "convseq_leaky_noskip": dict(channels=(5, 8, 8, 6), kw=dict(kernel=3, dilation_growth=2, batch_norm=True, skip=False,
+                                                                activation_on_last=False, glu=1, glu_context=0),
+                                 activation="leaky_relu", B=3, T=16, seed=53),
+    "convseq_gelu_widths": dict(channels=(8, 8, 12, 12, 6), kw=dict(kernel=3, dilation_growth=2, batch_norm=True, skip=True,
+                                                                    activation_on_last=False, glu=3, glu_context=1),
+                                activation="gelu", B=3, T=12, seed=54),
+    "convseq_dilation_ge_T": dict(channels=(6, 6, 6, 6, 6), kw=dict(kernel=3, dilation_growth=3, dilation_period=None,
+                                                                    batch_norm=True, skip=True, activation_on_last=True,
+                                                                    leakiness=0.2),
+                                  activation=None, B=2, T=8, seed=55),
+    "convseq_nobn_gelu": dict(channels=(5, 7, 7, 7), kw=dict(kernel=3, dilation_growth=2, batch_norm=False, skip=True,
+                                                             activation_on_last=True, glu=2, glu_context=0),
+                              activation="gelu", B=3, T=10, seed=56),
+}
+CONVSEQ_ACTIVATIONS = {None: None, "relu": torch.nn.ReLU, "leaky_relu": torch.nn.LeakyReLU, "gelu": torch.nn.GELU}
+
+
+def run_convseq(name, c):
+    """Verbatim ConvSequence (stride 1): a training forward/backward against a random upstream gradient (input and every
+    parameter gradient, BatchNorm running statistics after the step), then an eval-mode forward AND backward with those
+    running statistics."""
+    common, _, _ = ref_loader.load_reference()
+    torch.manual_seed(c["seed"])
+    model = common.ConvSequence(c["channels"], stride=1, activation=CONVSEQ_ACTIVATIONS[c["activation"]], **c["kw"])
+    with torch.no_grad():
+        for m in model.modules():
+            if isinstance(m, torch.nn.BatchNorm1d):
+                m.weight.add_(0.1 * torch.randn_like(m.weight))
+                m.bias.add_(0.1 * torch.randn_like(m.bias))
+                m.running_mean.add_(0.1 * torch.randn_like(m.running_mean))
+                m.running_var.mul_(1 + 0.2 * torch.rand_like(m.running_var))
+    state = {k: v.detach().clone() for k, v in model.state_dict().items()}
+    B, T, C0, CL = c["B"], c["T"], c["channels"][0], c["channels"][-1]
+    x = torch.randn(B, C0, T, requires_grad=True)
+    gout, gout_eval = torch.randn(B, CL, T), torch.randn(B, CL, T)
+    out = dict(x=x.detach().numpy().copy(), gout=gout.numpy(), gout_eval=gout_eval.numpy())
+    for k, v in state.items():
+        out["p." + k] = v.numpy()
+    model.train()
+    y = model(x)
+    y.backward(gout)
+    out["out"] = y.detach().numpy()
+    out["g.x"] = x.grad.numpy().copy()
+    for k, v in model.named_parameters():
+        out["g." + k] = v.grad.numpy().copy()
+    for k, v in model.state_dict().items():
+        if "running" in k or "num_batches" in k:
+            out["bn." + k] = v.numpy().copy()
+    model.eval()
+    model.zero_grad()
+    x.grad = None
+    y = model(x)
+    y.backward(gout_eval)
+    out["out_eval"] = y.detach().numpy()
+    out["ge.x"] = x.grad.numpy()
+    for k, v in model.named_parameters():
+        out["ge." + k] = v.grad.numpy()
+    np.savez_compressed(os.path.join(OUT, name + ".npz"), **out)
+    print(f"{name}: out.std={out['out'].std():.4f} |g.x|={np.linalg.norm(out['g.x']):.4e} "
+          f"|ge.x|={np.linalg.norm(out['ge.x']):.4e}")
+
+
 # The ablation table of the paper (grids/nmi/ablation_final.py:42-52), each as a change to the small clip_conv case
 ABLATION_BASE = dict(B=6, C=10, T=24, F=8, S=3, hidden=16, depth=4, MC=12, IL=12, P=32, seed=41)
 ABLATIONS = {
@@ -357,6 +428,9 @@ def generate(wanted):
     for name, c in DEEPMEL_CASES.items():
         if not wanted or name in wanted:
             run_deepmel(name, c)
+    for name, c in CONVSEQ_CASES.items():
+        if not wanted or name in wanted:
+            run_convseq(name, c)
     for name, change in ABLATIONS.items():
         if not wanted or name in wanted:
             run_ablation(name, change)

@@ -124,41 +124,51 @@ def _persistent(passes, x, wop, bias, acc, T, Ntot, Kw, dil, sign, y, stats):
     assert int(status.item()) == 0, f"status {int(status.item())}"
 
 
-def _kernel_order_stats(y):
-    """column sum and sum of squares of y [B,T,N] in the kernel's order: per thread (0 + v_r) + v_r+8 and
-    fma(v_r+8, v_r+8, fma(v_r, v_r, 0)) in fp32, a fp32 tree over the 8 row lanes of a warp (lane groups 1, 2, 4
-    apart), then fp64 over the warps; rows past T are zeros, which change no sum"""
+def _kernel_order_stats(y, bias):
+    """column sum and sum of squares of y [B,T,N] in the kernel's order: d = y - bias in fp32, per thread (0 + d_r) + d_r+8
+    and fma(d_r+8, d_r+8, fma(d_r, d_r, 0)) in fp32, a fp32 tree over the 8 row lanes of a warp (lane groups 1, 2, 4
+    apart), fp64 over the warps; then per time tile of n rows, sum = n b + d1 and sum of squares = d2 + b (n b + 2 d1) in
+    fp64; rows past T are zeros of d, which change no sum"""
     B, T, N = y.shape
     tt = (T + 127) // 128
     yp = torch.zeros(B, tt * 128, N, device=DEV)
-    yp[:, :T] = y
+    yp[:, :T] = y - bias
     v = yp.view(B, tt, 8, 2, 8, N)                             # [b][time tile][warp][row half h][row lane][n]
     v0, v1 = v[:, :, :, 0], v[:, :, :, 1]
     s1 = v0 + v1
     sq0 = (v0.double() * v0.double()).float()                  # fma(v, v, 0): the exact square, rounded once
     s2 = (v1.double() * v1.double() + sq0.double()).float()    # fma(v, v, s): exact in fp64 but for rare ties
-    out = []
+    d = []
     for s in (s1, s2):
         s = s[:, :, :, 0::2] + s[:, :, :, 1::2]                # lanes 4 apart: row lanes k, k ^ 1
         s = s[:, :, :, 0::2] + s[:, :, :, 1::2]
         s = s[:, :, :, 0] + s[:, :, :, 1]                      # [b][tile][warp][n]
-        out.append(s.double().sum(dim=(0, 1, 2)))
-    return torch.cat(out), torch.cat([yp.double().abs().sum(dim=(0, 1)), (yp.double() ** 2).sum(dim=(0, 1))])
+        d.append(s.double().sum(dim=2))                        # [b][tile][n]
+    rows = torch.tensor([min(128, T - 128 * i) for i in range(tt)], device=DEV, dtype=torch.float64)[None, :, None]
+    b = bias.double()
+    tile_sum = rows * b + d[0]
+    tile_sq = d[1] + b * (rows * b + 2 * d[0])
+    want = torch.cat([tile_sum.sum(dim=(0, 1)), tile_sq.sum(dim=(0, 1))])
+    yd = y.double()
+    return want, torch.cat([yd.abs().sum(dim=(0, 1)), (yd ** 2).sum(dim=(0, 1))])
 
 
 @pytest.mark.parametrize("passes", [3, 1])
 @pytest.mark.parametrize("Ntot", [320, 256])
-def test_batchnorm_statistics_match_own_output(passes, Ntot):
+@pytest.mark.parametrize("bias_scale", [1.0, 1e3, None])
+def test_batchnorm_statistics_bias_shifted_match_own_output(passes, Ntot, bias_scale):
+    """the fused statistics are the bias-shifted sums of the kernel's own y, in its order, to fp64 rounding; with no bias,
+    with a unit one and with one 1e3 times the conv's spread (where unshifted fp32 sums of y^2 would lose the variance)"""
     torch.manual_seed(43)
     B, T, Cin, Kw = 23, 343, 320, 3
     x = torch.randn(B, T, Cin, device=DEV)
     wop = torch.randn(Kw, Ntot, Cin, device=DEV) * 0.05
-    bias = torch.randn(Ntot, device=DEV)
+    bias = None if bias_scale is None else torch.randn(Ntot, device=DEV) * bias_scale
     y = torch.full((B, T, Ntot), float("nan"), device=DEV)
     stats = torch.full((2 * Ntot,), float("nan"), device=DEV, dtype=torch.float64)
     _persistent(passes, x, wop, bias, 0, T, Ntot, Kw, 2, 1, y, stats)
     assert torch.isfinite(y).all()
-    want, scale = _kernel_order_stats(y)
+    want, scale = _kernel_order_stats(y, torch.zeros(Ntot, device=DEV) if bias is None else bias)
     bad = (stats - want).abs() > 1e-10 * scale
     assert not bad.any(), f"columns {bad.nonzero().flatten().tolist()[:8]} off by {(stats - want).abs().max().item()}"
 
