@@ -59,8 +59,6 @@ class EncoderPlan(SequencePlan):
     freq: torch.Tensor                     # [sqrt(P/2)] fp32 Fourier frequencies
     ban_centre: tp.Optional[torch.Tensor]  # [2] fp32 or None
     ban_radius: float
-    staged: bool = False                   # a sensor-chain stage is missing (merger / initial_linear / subject_layers
-                                           # ablations) or a subject embedding is appended: run the chain stage by stage
     has_sub_emb: bool = False              # the last tensor argument is the [B, E] subject-embedding rows
     channel_mask: tp.Optional[torch.Tensor] = None   # [C] subsample_meg_channels mask (simpleconv.py:200-203), or None
     masked_meg: tp.Optional[torch.Tensor] = None     # [B,C,T] buffer that receives meg * channel_mask
@@ -502,131 +500,344 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
 
 
 # ----------------------------------------------------------------------------------------------------
-# Sensor chain in optional stages: the ablation rows merger=False / initial_linear=0 / subject_layers=False / subject_dim
-# (grids/nmi/ablation_final.py:44,46,50,51; simpleconv.py:104-151, 207-233).  Each stage is the FP32-FMA stage kernel that
-# the fused `bm_sensor_chain_fwd/bwd` is made of (csrc/bm_api.cu), called on its own; activations are channels-last.
+# The sensor-side front (simpleconv.py:104-151, 207-233): ChannelMerger attention -> sensor mix -> initial_linear ->
+# SubjectLayers -> subject embedding, on channels-last activations.  A stage whose parameters are None is absent (the
+# ablation rows merger=False / initial_linear=0 / subject_layers=False / subject_dim, grids/nmi/ablation_final.py:44,46,50,51).
+# SimpleConv's encoder runs it through `front_forward` / `front_backward`; the stand-alone ChannelMerger and SubjectLayers
+# call its FP32-FMA stage helpers.
 # ----------------------------------------------------------------------------------------------------
-def _staged_front_forward(plan: "EncoderPlan", meg, heads, il_w, il_b, subj_w, sub_emb, status):
-    """-> (x [B,T,D_total] channels-last, saved dict).  meg [B,C,T]; missing stages have None parameters."""
+def _attention_fwd(heads, positions, freq, ban_centre, radius, C):
+    """ChannelMerger attention weights of every recording on the FP32-FMA kernel -> (emb [R,C,P], att [R,O,C])."""
+    R, (O, P) = positions.shape[0], heads.shape
+    emb, att = _empty((R, C, P), heads), _empty((R, O, C), heads)
+    call("bm_attention_weights_fwd", ptr(positions), ptr(freq), ptr(heads.contiguous()), ptr(ban_centre), float(radius), R,
+         C, O, P, ptr(emb), ptr(att), stream())
+    return emb, att
+
+
+def _attention_bwd(d_att, att, emb):
+    """dheads [O,P] from the attention weights' gradient d_att [R,O,C], on the FP32-FMA kernel."""
+    R, O, C = att.shape
+    P = emb.shape[2]
+    dscores, dheads = _empty((R, O, C), att), _empty((O, P), att)
+    _reducing_call("bm_attention_weights_bwd", att, None, ptr(d_att), ptr(att), ptr(emb), R, C, O, P, ptr(dscores),
+                   ptr(dheads), stream())
+    return dheads
+
+
+def _mix_fwd(meg, att, rec_of_sample, u):
+    """u[b,t,o] = sum_c att[rec_b][o][c] meg[b,c,t] on the FP32-FMA kernel, into the first O columns of u [B,T,ld]."""
+    B, C, T = meg.shape
+    call("bm_sensor_mix_fwd", ptr(meg), ptr(att), ptr(rec_of_sample), B, C, T, att.shape[1], u.shape[2], ptr(u), stream())
+
+
+def _mix_bwd(du, meg, att, rec_order, rec_off):
+    """The mix's weight gradient d_att [R,O,C] from du [B,T,ld], samples grouped by recording, on the FP32-FMA kernel."""
+    B, C, T = meg.shape
+    R, O, _ = att.shape
+    d_att = _empty((R, O, C), meg)
+    call("bm_sensor_mix_bwd", ptr(du), du.shape[2], ptr(meg), ptr(rec_order), ptr(rec_off), B, C, T, O, R, ptr(d_att),
+         stream())
+    return d_att
+
+
+def _mix_bwd_data(du, att, rec_of_sample, mask):
+    """dmeg [B,C,T] = mask[c] * sum_o att[rec_b][o][c] du[b,t,o] (mask None: no mask) on the FP32-FMA kernel."""
+    B, T = du.shape[:2]
+    _, O, C = att.shape
+    dmeg = _empty((B, C, T), du)
+    call("bm_sensor_mix_bwd_data", ptr(du), du.shape[2], ptr(att), ptr(rec_of_sample), ptr(mask), B, C, T, O, ptr(dmeg),
+         stream())
+    return dmeg
+
+
+def _subject_fwd(x, subj_w, subject, out):
+    """out[b,t,:D] = x[b,t,:IL] @ subj_w[subject_b] on the FP32-FMA kernel; x [B,T,ld_x], out [B,T,ld_out]."""
+    B, T = x.shape[:2]
+    _, IL, D = subj_w.shape
+    call("bm_subject_layers_fwd", ptr(x), x.shape[2], ptr(subj_w.contiguous()), ptr(subject), B, T, IL, D, out.shape[2],
+         ptr(out), stream())
+
+
+def _subject_bwd(g, x, subj_w, subject, shape, ld, want_dx, want_dw):
+    """g [B,T,ld_g] (first D columns) -> (dx [B,T,ld], d_subj_w [S,IL,D]) on the FP32-FMA kernel, None where not wanted.
+    shape = (S, IL, D); x [B,T,ld], the forward input, is read for d_subj_w only, subj_w for dx only.  The pad columns of dx
+    are zero: a tensor-core contraction reads them."""
+    S, IL, D = shape
+    B, T = g.shape[:2]
+    order, off = group_layout(subject, S) if want_dw else (None, None)
+    dx = None
+    if want_dx:
+        dx = torch.zeros((B, T, ld), device=g.device) if ld != IL else _empty((B, T, ld), g)
+    dw = _empty((S, IL, D), g) if want_dw else None
+    call("bm_subject_layers_bwd", ptr(g), g.shape[2], ptr(x), ld, ptr(subj_w), ptr(subject), ptr(order), ptr(off), B, T, IL,
+         D, S, ld, ptr(dx), ptr(dw), stream())
+    return dx, dw
+
+
+def front_forward(plan: "EncoderPlan", meg, heads, il_w, il_b, subj_w, sub_emb, w0, nd: "_Needs", save: bool, status):
+    """meg [B,C,T] -> (x [B,T,Dp] channels-last input of conv layer 0, conv0 = layer 0's prepared `_Conv` of weight w0 with
+    its input padded to Dp, the record `front_backward` reads).  heads, (il_w, il_b), subj_w, sub_emb [B,E]: the stages'
+    parameters, None where a stage is absent.  `save`: a backward will run.
+
+    Kernel choice: the tensor-core stages run only in the complete chain (merger, initial_linear and subject layers, no
+    subject embedding), each where its padded widths pass the shape gates; a complete chain whose initial_linear is not on
+    the tensor cores is the fused FP32-FMA `bm_sensor_chain_fwd`; everything else runs the FP32-FMA stage kernels one by one,
+    with layer 0 unpadded."""
     st = stream()
+    lib = _lib.load()
     B, C, T = meg.shape
     R = plan.rec_positions.shape[0]
-    saved = dict(meg=meg, att=None, emb=None, u=None, v=None)
-    width = C
-    if heads is not None:                                     # ChannelMerger (common.py:334-362)
-        O, P = heads.shape
-        emb = _empty((R, C, P), meg)
-        att = _empty((R, O, C), meg)
-        call("bm_attention_weights_fwd", ptr(plan.rec_positions), ptr(plan.freq), ptr(heads.contiguous()),
-             ptr(plan.ban_centre), float(plan.ban_radius), R, C, O, P, ptr(emb), ptr(att), st)
-        u = _empty((B, T, O), meg)
-        call("bm_sensor_mix_fwd", ptr(meg), ptr(att), ptr(plan.rec_of_sample), B, C, T, O, O, ptr(u), st)
-        saved.update(att=att, emb=emb)
-        width = O
-    else:                                                      # raw sensors, channels-last
-        u = _empty((B, T, C), meg)
-        call("bm_transpose_nt", ptr(meg), B, C, T, ptr(u), st)
-    saved["u"] = u
-    x = u
-    if il_w is not None:                                       # initial_linear (simpleconv.py:112-120)
-        IL = il_w.shape[0]
-        v = _empty((B, T, IL), meg)
-        call("bm_initial_linear_fwd", ptr(x), width, ptr(il_w.reshape(IL, width).contiguous()), ptr(il_b.contiguous()), B, T,
-             width, IL, IL, ptr(v), st)
-        x, width = v, IL
-    saved["v"] = x                                             # input of the subject stage
-    if subj_w is not None:                                     # SubjectLayers (common.py:45-62)
-        D = subj_w.shape[2]
-        x0 = _empty((B, T, D), meg)
-        call("bm_subject_layers_fwd", ptr(x), width, ptr(subj_w.contiguous()), ptr(plan.subject), B, T, width, D, D,
-             ptr(x0), st)
-        x, width = x0, D
+    n_meg, n_heads, n_il_w, _, n_subj, _ = nd.front
+    want_bwd0 = save and nd.below[0]
+    chain = heads is not None and il_w is not None and subj_w is not None and sub_emb is None
+    tc = chain and plan.use_tensor_cores
+    O = heads.shape[0] if heads is not None else C          # the mix, initial_linear and subject-layer output widths
+    IL = il_w.shape[0] if il_w is not None else O
+    D = subj_w.shape[2] if subj_w is not None else IL
+    Op, ILp, Dp = O, IL, D                                  # ... and their widths in the buffers, zero-padded
+    rec = dict(meg=meg, chain=chain, emb=None, att=None, heads_tc=False, megT=None, subj_pad=None)
+
+    def _padded(width_pad, width, written_in_full):
+        """[B,T,width_pad]; the pad columns need a fill only where an FP32-FMA kernel (valid columns only) writes it"""
+        if width_pad == width or written_in_full:
+            return _empty((B, T, width_pad), meg)
+        return torch.zeros((B, T, width_pad), device=meg.device)
+
+    if heads is not None:
+        # K1 attention weights per recording (the score contraction on the tensor cores when the widths fit)
+        P = heads.shape[1]
+        Opad = _round_up(O, 64)
+        if tc and bool(lib.bm_tc_conv1d_persistent_supported(C, P, Opad, 1, 0)) and bool(lib.bm_tc_wgrad_supported(Opad, P)):
+            hpad = torch.zeros((Opad, P, 1), device=meg.device)
+            hpad[:O, :, 0] = heads
+            heads_conv = _Conv(hpad, C, False, True, want_bwd=False)
+            emb = _empty((R, C, P), meg)
+            call("bm_fourier_emb", ptr(plan.rec_positions), ptr(plan.freq), R, C, P, ptr(emb), st)
+            att_full = _empty((R, Opad, C), meg)          # scores[r][o][c] = <emb[r][c], heads[o]> written channel-major
+            heads_conv.run_tc(True, emb, None, None, R, C, 1, 0, 0, 1, att_full, None, None, None, status)
+            call("bm_masked_softmax", ptr(att_full), ptr(plan.rec_positions), ptr(plan.ban_centre), float(plan.ban_radius),
+                 R, Opad, C, st)
+            att = att_full[:, :O].contiguous()
+            rec["heads_tc"] = True
+        else:
+            emb, att = _attention_fwd(heads, plan.rec_positions, plan.freq, plan.ban_centre, plan.ban_radius, C)
+        rec.update(emb=emb, att=att)
+
+    conv0 = il_conv = None
+    if chain:
+        # x0 kept zero-padded to a multiple of 64 channels when the tensor-core conv follows
+        Dp = _round_up(D, 64)
+        conv0 = _Conv(w0, T, False, plan.use_tensor_cores, pad_cin_to=Dp, want_bwd=want_bwd0)
+        if not conv0.fwd_tc:
+            Dp = D
+            conv0 = _Conv(w0, T, False, False, want_bwd=want_bwd0)
+    if tc:
+        # `initial_linear` on the tensor cores when the (64-padded) widths fit: u and v are then kept zero-padded
+        Op, ILp = _round_up(O, 64), _round_up(IL, 64)
+        wpad = torch.zeros((ILp, Op, 1), device=meg.device)
+        wpad[:IL, :O, 0] = il_w.reshape(IL, O)
+        il_conv = _Conv(wpad, T, False, True, want_bwd=save and (n_meg or n_heads))
+        if not (il_conv.fwd_tc and il_conv.bwd_tc and il_conv.wgrad_tc):
+            il_conv = None
+            Op, ILp = O, IL
+    Cp = _round_up(C, 128)
+    mix_tc = il_conv is not None and bool(lib.bm_tc_conv_supported(T, Cp, Op, 1, 0)) and \
+        bool(lib.bm_tc_wgrad_supported(Op, Cp))
+    subj_tc = il_conv is not None and (Dp != D or D % 64 == 0) and bool(lib.bm_tc_conv_supported(T, ILp, Dp, 1, 0)) and \
+        bool(lib.bm_tc_conv_supported(T, Dp, ILp, 1, 0)) and bool(lib.bm_tc_wgrad_supported(ILp, Dp))
+
+    if chain and il_conv is None:
+        # One call: the library's own composition of the three FP32-FMA stage kernels, which the pinned call streams hold.
+        u, v, x = _empty((B, T, O), meg), _empty((B, T, IL), meg), _padded(Dp, D, False)
+        call("bm_sensor_chain_fwd", ptr(meg), ptr(att), ptr(plan.rec_of_sample), ptr(il_w.reshape(IL, O).contiguous()),
+             ptr(il_b.contiguous()), ptr(subj_w.contiguous()), ptr(plan.subject), B, C, T, O, IL, D, Dp, ptr(u), ptr(v),
+             ptr(x), st)
+    else:
+        # K2 sensor mix (without a merger: the raw sensors, channels-last)
+        if heads is None:
+            u = _empty((B, T, C), meg)
+            call("bm_transpose_nt", ptr(meg), B, C, T, ptr(u), st)
+        elif mix_tc:
+            # meg transposed once to channels-last (sensor count padded to 128), then u = megT @ att[rec]^T is a pointwise
+            # contraction with a per-sample weight set (one per recording)
+            u = _padded(Op, O, True)
+            megT = _empty((B, T, Cp), meg)                 # the transpose writes the pad columns as zeros
+            call("bm_transpose_nt_ld", ptr(meg), B, C, T, Cp, ptr(megT), st)
+            att_pad = torch.zeros((R, Op, Cp), device=meg.device)
+            att_pad[:, :O, :C] = att
+            aw_hi, aw_lo = _empty((R * Op, Cp), meg), _empty((R * Op, Cp), meg)
+            call("bm_tc_weight_split", ptr(att_pad), R * Op, Cp, 1, ptr(aw_hi), ptr(aw_lo), None, None, st)
+            _tc_call("bm_tc_pointwise_sel", ptr(megT), ptr(aw_hi), ptr(aw_lo), ptr(plan.rec_of_sample), R, B, T, Cp, Op,
+                     ptr(u), ptr(status), st)
+            rec["megT"] = megT
+        else:
+            u = _padded(Op, O, False)
+            _mix_fwd(meg, att, plan.rec_of_sample, u)
+        # initial_linear (simpleconv.py:112-120)
+        v = u
+        if il_conv is not None:
+            v = _empty((B, T, ILp), meg)
+            bpad = torch.zeros((ILp,), device=meg.device)
+            bpad[:IL] = il_b
+            il_conv.forward(u, bpad, B, T, 1, v, None, status)
+        elif il_w is not None:
+            v = _empty((B, T, IL), meg)
+            call("bm_initial_linear_fwd", ptr(u), O, ptr(il_w.reshape(IL, O).contiguous()), ptr(il_b.contiguous()), B, T, O,
+                 IL, IL, ptr(v), st)
+        # SubjectLayers (common.py:45-62)
+        x = v
+        if subj_tc:
+            # per-subject weights, zero-padded; forward operand [s][d][p] (K-major in p), tf32-split
+            S = subj_w.shape[0]
+            x = _padded(Dp, D, True)
+            subj_pad = torch.zeros((S, ILp, Dp), device=meg.device)
+            subj_pad[:, :IL, :D] = subj_w
+            mt = subj_pad.transpose(1, 2).contiguous()
+            sf_hi, sf_lo = _empty((S * Dp, ILp), meg), _empty((S * Dp, ILp), meg)
+            call("bm_tc_weight_split", ptr(mt), S * Dp, ILp, 1, ptr(sf_hi), ptr(sf_lo), None, None, st)
+            _tc_call("bm_tc_pointwise_sel", ptr(v), ptr(sf_hi), ptr(sf_lo), ptr(plan.subject), S, B, T, ILp, Dp, ptr(x),
+                     ptr(status), st)
+            rec["subj_pad"] = subj_pad
+        elif subj_w is not None:
+            x = _padded(Dp, D, False)
+            _subject_fwd(v, subj_w, plan.subject, x)
     if sub_emb is not None:                                    # ScaledEmbedding appended as channels (simpleconv.py:231-233)
         x = torch.cat([x, sub_emb[:, None, :].expand(B, T, sub_emb.shape[1])], dim=2).contiguous()
-    saved["widths"] = (C, saved["u"].shape[2], saved["v"].shape[2], width)
-    return x, saved
+    if conv0 is None:
+        conv0 = _Conv(w0, T, False, plan.use_tensor_cores, want_bwd=want_bwd0)
+    # u and v (the initial_linear and subject-layer inputs) are read by those stages' weight gradients only
+    rec.update(u=u if n_il_w else None, v=v if n_subj else None, il_conv=il_conv, widths=(O, IL, D), pads=(Op, ILp, Dp))
+    return x, conv0, rec
 
 
-def _staged_front_backward(plan: "EncoderPlan", saved, g, heads, il_w, subj_w, sub_emb, need):
-    """g = dL/dx [B,T,D_total] -> (dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg); None where the stage is absent or its
-    gradient is not wanted.  need = requires-grad of (meg, heads, il_w, il_b, subj_w, sub_emb): each stage computes the
-    gradients asked of it, and its data gradient only while a stage below it still needs one."""
+def front_backward(plan: "EncoderPlan", rec, g, heads, il_w, subj_w, sub_emb, need, status):
+    """g = dL/dx [B,T,Dp] (x of `front_forward`) -> (dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg); None where a stage is
+    absent or its gradient is not asked for.  need = requires-grad of (meg, heads, il_w, il_b, subj_w, sub_emb): each stage
+    computes the gradients asked of it, and its data gradient only while a stage below it still needs one."""
     st = stream()
-    meg = saved["meg"]
+    meg, att, il_conv, megT = rec["meg"], rec["att"], rec["il_conv"], rec["megT"]
     B, C, T = meg.shape
     R = plan.rec_positions.shape[0]
-    _, w_u, w_v, w_x = saved["widths"]
+    O, IL, D = rec["widths"]
+    Op, ILp, Dp = rec["pads"]
     n_meg, n_heads, n_il_w, n_il_b, n_subj, n_emb = need
-    d_sub_emb = None
+    want_dv = n_meg or n_heads or n_il_w or n_il_b          # the gradient at the subject layers' input
+    want_du = n_meg or n_heads                              # ... and at initial_linear's input
+    dheads = d_il_w = d_il_b = d_subj = d_sub_emb = dmeg = d_att = None
     if sub_emb is not None:
         if n_emb:
-            d_sub_emb = g[:, :, w_x:].sum(dim=1)               # the embedding is constant over time
-        g = g[:, :, :w_x].contiguous() if any(need[:5]) else None
-    d_subj = None
-    if subj_w is not None and (n_subj or any(need[:4])):
+            d_sub_emb = g[:, :, D:].sum(dim=1)               # the embedding is constant over time
+        g = g[:, :, :D].contiguous() if any(need[:5]) else None
+
+    if rec["chain"] and il_conv is None:
         S = subj_w.shape[0]
         subj_order, subj_off = group_layout(plan.subject, S) if n_subj else (None, None)
-        d_subj = _empty((S, w_v, w_x), meg) if n_subj else None
-        dv = _empty((B, T, w_v), meg) if any(need[:4]) else None
-        call("bm_subject_layers_bwd", ptr(g), w_x, ptr(saved["v"]), w_v, ptr(subj_w.contiguous()), ptr(plan.subject),
-             ptr(subj_order), ptr(subj_off), B, T, w_v, w_x, S, w_v, ptr(dv), ptr(d_subj), st)
-        g = dv
-    d_il_w = d_il_b = None
-    if il_w is not None and any(need[:4]):
-        d_il_w = _empty((w_v, w_u), meg) if n_il_w else None
-        d_il_b = _empty((w_v,), meg) if n_il_b else None
-        # du feeds the merger's and meg's gradients.  Without a merger it is kept whenever this stage runs: one GEMM onto the
-        # raw sensors, and a trainable step keeps the call stream it has always had
-        du = _empty((B, T, w_u), meg) if (n_meg or n_heads or heads is None) else None
-        _reducing_call("bm_initial_linear_bwd", meg, (B, T, w_u, w_v), ptr(g), w_v, ptr(saved["u"]), w_u,
-                       ptr(il_w.reshape(w_v, w_u).contiguous()), B, T, w_u, w_v, w_u, ptr(du), ptr(d_il_w), ptr(d_il_b), st,
-                       reduces=bool(n_il_w or n_il_b))
-        if d_il_w is not None:
-            d_il_w = d_il_w.reshape(il_w.shape)
-        g = du
-    dheads = None
-    if heads is not None and n_heads:
-        O, P = heads.shape
-        d_att = _empty((R, O, C), meg)
-        call("bm_sensor_mix_bwd", ptr(g), w_u, ptr(meg), ptr(plan.rec_order), ptr(plan.rec_off), B, C, T, O, R, ptr(d_att), st)
-        dscores = _empty((R, O, C), meg)
-        dheads = _empty((O, P), meg)
-        _reducing_call("bm_attention_weights_bwd", meg, None, ptr(d_att), ptr(saved["att"]), ptr(saved["emb"]), R, C, O, P,
-                       ptr(dscores), ptr(dheads), st)
-    dmeg = None
-    if n_meg:
-        # g is now the gradient at the first stage present: the mix output, or the raw sensors transposed (merger=False)
-        dmeg = _empty((B, C, T), meg)
-        if heads is not None:
-            call("bm_sensor_mix_bwd_data", ptr(g), g.shape[2], ptr(saved["att"]), ptr(plan.rec_of_sample),
-                 ptr(plan.channel_mask), B, C, T, heads.shape[0], ptr(dmeg), st)
+        dv = _empty((B, T, IL), meg) if want_dv else None
+        du = _empty((B, T, O), meg) if want_du else None
+        d_subj = _empty((S, IL, D), meg) if n_subj else None
+        d_il_w = _empty((IL, O), meg) if n_il_w else None
+        d_il_b = _empty((IL,), meg) if n_il_b else None
+        d_att = _empty((R, O, C), meg) if n_heads else None
+        _reducing_call("bm_sensor_chain_bwd", meg, (B, T, O, IL), ptr(g), ptr(meg), ptr(il_w.reshape(IL, O).contiguous()),
+                       ptr(subj_w.contiguous()), ptr(plan.subject), ptr(rec["u"]), ptr(rec["v"]), ptr(subj_order),
+                       ptr(subj_off), ptr(plan.rec_order), ptr(plan.rec_off), B, C, T, O, IL, D, Dp, S, R, ptr(dv), ptr(du),
+                       ptr(d_subj), ptr(d_il_w), ptr(d_il_b), ptr(d_att), st, reduces=n_il_w or n_il_b)
+    else:
+        # SubjectLayers
+        dv = g
+        if rec["subj_pad"] is not None:
+            S = subj_w.shape[0]
+            dv = None
+            if want_dv:
+                subj_pad = rec["subj_pad"]                               # [S][ILp][Dp]: data-gradient operand as is
+                sb_hi, sb_lo = _empty((S * ILp, Dp), meg), _empty((S * ILp, Dp), meg)
+                call("bm_tc_weight_split", ptr(subj_pad), S * ILp, Dp, 1, ptr(sb_hi), ptr(sb_lo), None, None, st)
+                dv = _empty((B, T, ILp), meg)
+                _tc_call("bm_tc_pointwise_sel", ptr(g), ptr(sb_hi), ptr(sb_lo), ptr(plan.subject), S, B, T, Dp, ILp,
+                         ptr(dv), ptr(status), st)
+            if n_subj:
+                subj_order, subj_off = group_layout(plan.subject, S)
+                dm = _empty((S, _round_up(ILp, 128), Dp), meg)
+                _tc_call("bm_tc_wgrad_grouped", ptr(rec["v"]), ptr(g), ptr(subj_order), ptr(subj_off), S, B, T, ILp, Dp,
+                         ptr(dm), ptr(status), st)
+                d_subj = dm[:, :IL, :D].contiguous()
+        elif subj_w is not None and (want_dv or n_subj):
+            dv, d_subj = _subject_bwd(g, rec["v"], subj_w.contiguous(), plan.subject, subj_w.shape, ILp, want_dv, n_subj)
+        # initial_linear
+        du = dv if il_w is None else None
+        if il_conv is not None:
+            if want_du:
+                du = _empty((B, T, Op), meg)
+                il_conv.backward_data(dv, None, B, T, 1, du, status)
+            if n_il_w:
+                dbp = _empty((ILp,), meg) if n_il_b else None
+                d_il_w = tc_wgrad(dv, rec["u"], B, T, ILp, Op, O, 1, 1, status, dbias=dbp)[:IL, :, 0].contiguous()
+                d_il_b = dbp[:IL].contiguous() if n_il_b else None
+            elif n_il_b:
+                dbp = _empty((ILp,), meg)
+                col_sum(dv, B * T, ILp, dbp, st)
+                d_il_b = dbp[:IL].contiguous()
+        elif il_w is not None and want_dv:
+            # du feeds the merger's and meg's gradients.  Without a merger it is kept whenever this stage runs: one GEMM
+            # onto the raw sensors, and a trainable step keeps the call stream it has always had
+            du = _empty((B, T, O), meg) if (want_du or heads is None) else None
+            d_il_w = _empty((IL, O), meg) if n_il_w else None
+            d_il_b = _empty((IL,), meg) if n_il_b else None
+            _reducing_call("bm_initial_linear_bwd", meg, (B, T, O, IL), ptr(dv), IL, ptr(rec["u"]), O,
+                           ptr(il_w.reshape(IL, O).contiguous()), B, T, O, IL, O, ptr(du), ptr(d_il_w), ptr(d_il_b), st,
+                           reduces=bool(n_il_w or n_il_b))
+        # the sensor mix's weight gradient
+        if not n_heads:
+            pass
+        elif megT is not None:
+            Cp = megT.shape[2]
+            dwp = _empty((R, _round_up(Op, 128), Cp), meg)
+            _tc_call("bm_tc_wgrad_grouped", ptr(du), ptr(megT), ptr(plan.rec_order), ptr(plan.rec_off), R, B, T, Op, Cp,
+                     ptr(dwp), ptr(status), st)
+            d_att = dwp[:, :O, :C].contiguous()
         else:
-            call("bm_transpose_nt", ptr(g), B, T, C, ptr(dmeg), st)
+            d_att = _mix_bwd(du, meg, att, plan.rec_order, plan.rec_off)
+
+    def meg_grad():
+        """dmeg [B,C,T] from du, the gradient at the mix output (without a merger: at the raw sensors, channels-last)"""
+        if heads is None:
+            dmeg = _empty((B, C, T), meg)
+            call("bm_transpose_nt", ptr(du), B, T, C, ptr(dmeg), st)
             if plan.channel_mask is not None:
                 call("bm_channel_mask", ptr(dmeg), ptr(plan.channel_mask), B, C, T, ptr(dmeg), st)
-    return dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg
-
-
-def _sensor_mix_bwd_data(plan: "EncoderPlan", s, du, dims, status) -> torch.Tensor:
-    """dmeg [B,C,T] = mask[c] * sum_o att[rec_b][o][c] du[b,t,o] for the fused sensor chain; du [B,T,O or Op].  On the tensor
-    cores when the mix ran there and the transposed contraction fits their shape gate, else the FP32-FMA stage kernel."""
-    B, C, T, R, O = dims[:5]
-    st = stream()
-    meg, att = s["meg"], s["att"]
-    dmeg = _empty((B, C, T), meg)
-    Op = du.shape[2]
-    Cp = s["megT"].shape[2] if s["megT"] is not None else 0
-    if Cp and bool(_lib.load().bm_tc_conv_supported(T, Op, Cp, 1, 0)):
+            return dmeg
+        if megT is None or not bool(_lib.load().bm_tc_conv_supported(T, Op, megT.shape[2], 1, 0)):
+            return _mix_bwd_data(du, att, plan.rec_of_sample, plan.channel_mask)
+        # on the tensor cores when the mix ran there and the transposed contraction fits their shape gate
+        Cp = megT.shape[2]
+        dmeg = _empty((B, C, T), meg)
         att_t = torch.zeros((R, Cp, Op), device=meg.device)           # weight set r: [c][o], zero-padded
         att_t[:, :C, :O] = att.transpose(1, 2)
         w_hi, w_lo = _empty((R * Cp, Op), meg), _empty((R * Cp, Op), meg)
         call("bm_tc_weight_split", ptr(att_t), R * Cp, Op, 1, ptr(w_hi), ptr(w_lo), None, None, st)
         _tc_call("bm_tc_sensor_mix_bwd_data", ptr(du), ptr(w_hi), ptr(w_lo), ptr(plan.rec_of_sample), R,
                  ptr(plan.channel_mask), B, T, Op, Cp, C, ptr(dmeg), ptr(status), st)
-    else:
-        call("bm_sensor_mix_bwd_data", ptr(du), Op, ptr(att), ptr(plan.rec_of_sample), ptr(plan.channel_mask), B, C, T, O,
-             ptr(dmeg), st)
-    return dmeg
+        return dmeg
+
+    # the complete chain forms dmeg before the attention backward, the stage-by-stage front after it (the pinned call order)
+    if n_meg and rec["chain"]:
+        dmeg = meg_grad()
+    if n_heads and rec["heads_tc"]:
+        emb, P = rec["emb"], heads.shape[1]
+        Opad = _round_up(O, 64)
+        dscores = _empty((R, O, C), meg)
+        call("bm_softmax_bwd", ptr(att), ptr(d_att), R * O, C, ptr(dscores), st)
+        ds_t = _empty((R, C, Opad), meg)                   # pad columns zeroed by the transpose
+        call("bm_transpose_nt_ld", ptr(dscores), R, O, C, Opad, ptr(ds_t), st)
+        dheads = tc_wgrad(ds_t, emb, R, C, Opad, P, P, 1, 1, status)[:O, :, 0].contiguous()
+    elif n_heads:
+        dheads = _attention_bwd(d_att, att, rec["emb"])
+    if n_meg and not rec["chain"]:
+        dmeg = meg_grad()
+    if d_il_w is not None:
+        d_il_w = d_il_w.reshape(il_w.shape)
+    return dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg
 
 
 @dataclasses.dataclass
@@ -689,145 +900,26 @@ class _EncoderFn(torch.autograd.Function):
             # inside the node, so that the gradient reaches the caller's unmasked tensor (the backward applies the mask)
             call("bm_channel_mask", ptr(meg), ptr(plan.channel_mask), B, C, T, ptr(plan.masked_meg), st)
             meg = plan.masked_meg
-        R = plan.rec_positions.shape[0]
-        O, P = heads.shape if heads is not None else (0, 0)
-        IL = il_w.shape[0] if il_w is not None else 0
-        S, _, D = subj_w.shape if subj_w is not None else (0, 0, 0)
         H = conv_p[0][0].shape[0]
         F = conv_p[-1][0].shape[0] if plan.bare_last else w2.shape[1]
         rows = B * T
         nd = _Needs.of(ctx.needs_input_grad, plan)
         save = plan.keep_for_backward and any(ctx.needs_input_grad)
-        n_meg, n_heads, n_il_w, n_il_b, n_subj, _ = nd.front
         tc = plan.use_tensor_cores
         status = tc_status_tensor(meg.device)
 
-        if plan.staged:
-            # sensor-side ablation rows: the chain as optional stages (see _staged_front_forward)
-            x, front = _staged_front_forward(plan, meg, heads, il_w, il_b, subj_w, sub_emb, status)
-            if not n_il_w:
-                front["u"] = None                    # read by the initial_linear weight gradient only
-            if not n_subj:
-                front["v"] = None                    # read by the subject-layer weight gradient only
-            D = Dp = x.shape[2]
-            conv0 = _Conv(conv_p[0][0], T, False, tc, want_bwd=save and nd.below[0])
-            emb = att = u = v = il_w2 = il_conv = subj_pad = megT = heads_conv = None
-            Op = ILp = 0
-        else:
-            front = None
-            # K1 attention weights per recording (the score contraction on the tensor cores when the widths fit)
-            emb = _empty((R, C, P), meg)
-            lib = _lib.load()
-            Opad = _round_up(O, 64)
-            heads_conv = None
-            if tc and bool(lib.bm_tc_conv1d_persistent_supported(C, P, Opad, 1, 0)) and bool(lib.bm_tc_wgrad_supported(Opad, P)):
-                hpad = torch.zeros((Opad, P, 1), device=meg.device)
-                hpad[:O, :, 0] = heads
-                heads_conv = _Conv(hpad, C, False, True, want_bwd=False)
-                if not heads_conv.fwd_pp:
-                    heads_conv = None
-            if heads_conv is not None:
-                call("bm_fourier_emb", ptr(plan.rec_positions), ptr(plan.freq), R, C, P, ptr(emb), st)
-                att_full = _empty((R, Opad, C), meg)          # scores[r][o][c] = <emb[r][c], heads[o]> written channel-major
-                heads_conv.run_tc(True, emb, None, None, R, C, 1, 0, 0, 1, att_full, None, None, None, status)
-                call("bm_masked_softmax", ptr(att_full), ptr(plan.rec_positions), ptr(plan.ban_centre), float(plan.ban_radius),
-                     R, Opad, C, st)
-                att = att_full[:, :O].contiguous()
-            else:
-                att = _empty((R, O, C), meg)
-                call("bm_attention_weights_fwd", ptr(plan.rec_positions), ptr(plan.freq), ptr(heads.contiguous()),
-                     ptr(plan.ban_centre), float(plan.ban_radius), R, C, O, P, ptr(emb), ptr(att), st)
-            # K2 sensor chain; x0 is kept zero-padded to a multiple of 64 channels when the tensor-core conv follows
-            Dp = _round_up(D, 64)
-            conv0 = _Conv(conv_p[0][0], T, False, tc, pad_cin_to=Dp, want_bwd=save and nd.below[0])
-            if not conv0.fwd_tc:
-                Dp = D
-                conv0 = _Conv(conv_p[0][0], T, False, False, want_bwd=save and nd.below[0])
-            il_w2 = il_w.reshape(IL, O).contiguous()
-            # `initial_linear` on the tensor cores when the (64-padded) widths fit: u and v are then kept zero-padded
-            Op, ILp = _round_up(O, 64), _round_up(IL, 64)
-            il_conv = None
-            if tc:
-                wpad = torch.zeros((ILp, Op, 1), device=meg.device)
-                wpad[:IL, :O, 0] = il_w2
-                il_conv = _Conv(wpad, T, False, True, want_bwd=save and (n_meg or n_heads))
-                if not (il_conv.fwd_tc and il_conv.bwd_tc and il_conv.wgrad_tc):
-                    il_conv = None
-            # u [B,T,Op] and x [B,T,Dp] carry zero pad columns.  The tensor-core contractions write every column (their padded
-            # weight rows are zero), so the buffers only need a fill when an FP32-FMA stage kernel (valid columns only) runs.
-            def _padded(width_pad, width, written_in_full):
-                if width_pad == width or written_in_full:
-                    return _empty((B, T, width_pad), meg)
-                return torch.zeros((B, T, width_pad), device=meg.device)
-
-            lib = _lib.load()
-            Cp = _round_up(C, 128)
-            mix_tc = il_conv is not None and bool(lib.bm_tc_conv_supported(T, Cp, Op, 1, 0)) and \
-                bool(lib.bm_tc_wgrad_supported(Op, Cp))
-            subj_tc = il_conv is not None and (Dp != D or D % 64 == 0) and bool(lib.bm_tc_conv_supported(T, ILp, Dp, 1, 0)) and \
-                bool(lib.bm_tc_conv_supported(T, Dp, ILp, 1, 0)) and bool(lib.bm_tc_wgrad_supported(ILp, Dp))
-            x = _padded(Dp, D, subj_tc)
-            if il_conv is not None:
-                u = _padded(Op, O, mix_tc)
-                v = _empty((B, T, ILp), meg)
-                bpad = torch.zeros((ILp,), device=meg.device)
-                bpad[:IL] = il_b
-                # sensor mix on the tensor cores: meg transposed once to channels-last (sensor count padded to 128), then
-                # u = megT @ w[rec]^T is a pointwise contraction with a per-sample weight set (one per recording)
-                megT = None
-                if mix_tc:
-                    megT = _empty((B, T, Cp), meg)                 # the transpose writes the pad columns as zeros
-                    call("bm_transpose_nt_ld", ptr(meg), B, C, T, Cp, ptr(megT), st)
-                    att_pad = torch.zeros((R, Op, Cp), device=meg.device)
-                    att_pad[:, :O, :C] = att
-                    aw_hi, aw_lo = _empty((R * Op, Cp), meg), _empty((R * Op, Cp), meg)
-                    call("bm_tc_weight_split", ptr(att_pad), R * Op, Cp, 1, ptr(aw_hi), ptr(aw_lo), None, None, st)
-                    _tc_call("bm_tc_pointwise_sel", ptr(megT), ptr(aw_hi), ptr(aw_lo), ptr(plan.rec_of_sample), R, B, T, Cp,
-                             Op, ptr(u), ptr(status), st)
-                else:
-                    call("bm_sensor_mix_fwd", ptr(meg), ptr(att), ptr(plan.rec_of_sample), B, C, T, O, Op, ptr(u), st)
-                il_conv.forward(u, bpad, B, T, 1, v, None, status)
-                if subj_tc:
-                    # per-subject weights, zero-padded; forward operand [s][d][p] (K-major in p), tf32-split
-                    subj_pad = torch.zeros((S, ILp, Dp), device=meg.device)
-                    subj_pad[:, :IL, :D] = subj_w
-                    mt = subj_pad.transpose(1, 2).contiguous()
-                    sf_hi, sf_lo = _empty((S * Dp, ILp), meg), _empty((S * Dp, ILp), meg)
-                    call("bm_tc_weight_split", ptr(mt), S * Dp, ILp, 1, ptr(sf_hi), ptr(sf_lo), None, None, st)
-                    _tc_call("bm_tc_pointwise_sel", ptr(v), ptr(sf_hi), ptr(sf_lo), ptr(plan.subject), S, B, T, ILp, Dp,
-                             ptr(x), ptr(status), st)
-                else:
-                    subj_pad = None
-                    call("bm_subject_layers_fwd", ptr(v), ILp, ptr(subj_w.contiguous()), ptr(plan.subject), B, T, IL, D, Dp,
-                         ptr(x), st)
-            else:
-                subj_pad = None
-                megT = None
-                Op, ILp = O, IL
-                u = _empty((B, T, O), meg)
-                v = _empty((B, T, IL), meg)
-                call("bm_sensor_chain_fwd", ptr(meg), ptr(att), ptr(plan.rec_of_sample), ptr(il_w2),
-                     ptr(il_b.contiguous()), ptr(subj_w.contiguous()), ptr(plan.subject), B, C, T, O, IL, D, Dp, ptr(u),
-                     ptr(v), ptr(x), st)
-
+        x, conv0, front = front_forward(plan, meg, heads, il_w, il_b, subj_w, sub_emb, conv_p[0][0], nd, save, status)
         # K3/K4 ConvSequence
         x, saved_layers = conv_stack_forward(plan, x, conv0, conv_p, glu_p, nd, save, B, T, status, bare_slope=0.0)
+
+        if save:
+            ctx.plan, ctx.needs, ctx.dims = plan, nd, (B, T, H, F)
+            ctx.saved = dict(front=front, layers=saved_layers, conv_p=conv_p, params=(heads, il_w, subj_w, sub_emb))
 
         if plan.bare_last:
             # no head: the sequence already ends on out_channels; hand it out channel-major
             est = _empty((B, F, T), meg)
             call("bm_transpose_nt", ptr(x), B, T, F, ptr(est), st)
-            if save:
-                ctx.plan = plan
-                ctx.needs = nd
-                ctx.dims = (B, C, T, R, O, P, IL, S, D, Dp, H, F)
-                ctx.pads = (Op, ILp)
-                ctx.saved = dict(meg=meg, emb=emb, att=att, u=u if n_il_w else None, v=v if n_subj else None, il_w2=il_w2,
-                                 subj_w=None if subj_w is None else subj_w.contiguous(),
-                                 il_conv=il_conv, subj_pad=subj_pad, megT=megT, heads_tc=heads_conv is not None,
-                                 layers=saved_layers, conv_p=conv_p, glu_p=glu_p,
-                                 il_shape=None if il_w is None else il_w.shape, front=front,
-                                 params=(heads, il_w, subj_w, sub_emb))
             return est
 
         # K5 head
@@ -862,18 +954,9 @@ class _EncoderFn(torch.autograd.Function):
                  ptr(h1), ptr(q), ptr(est), st)
 
         if save:
-            ctx.plan = plan
-            ctx.needs = nd
-            ctx.dims = (B, C, T, R, O, P, IL, S, D, Dp, H, F)
-            ctx.pads = (Op, ILp)
-            ctx.saved = dict(meg=meg, emb=emb, att=att, u=u if n_il_w else None, v=v if n_subj else None, il_w2=il_w2,
-                             subj_w=None if subj_w is None else subj_w.contiguous(), il_conv=il_conv,
-                             subj_pad=subj_pad, megT=megT, heads_tc=heads_conv is not None,
-                             layers=saved_layers, x_last=x if nd.head[0] else None, w0_2=w0_2, w2_2=w2_2,
-                             h1=h1, q=q if nd.head[2] else None,
-                             head0=head0, head2=head2, head_tc=head_tc, head_generic=head_generic,
-                             conv_p=conv_p, glu_p=glu_p, il_shape=None if il_w is None else il_w.shape,
-                             w0_shape=w0.shape, w2_shape=w2.shape, front=front, params=(heads, il_w, subj_w, sub_emb))
+            ctx.saved.update(x_last=x if nd.head[0] else None, w0_2=w0_2, w2_2=w2_2, h1=h1, q=q if nd.head[2] else None,
+                             head0=head0, head2=head2, head_tc=head_tc, head_generic=head_generic, w0_shape=w0.shape,
+                             w2_shape=w2.shape)
         return est
 
     @staticmethod
@@ -884,10 +967,10 @@ class _EncoderFn(torch.autograd.Function):
         if s is None:
             raise RuntimeError("brainmagick_b200.SimpleConv: backward through the graph a second time -- the saved activations "
                                "(~5 GB at B=256) are released by the first backward; retain_graph is not supported")
-        B, C, T, R, O, P, IL, S, D, Dp, H, F = ctx.dims
+        B, T, H, F = ctx.dims
         depth = len(plan.dilations)
         st = stream()
-        meg = s["meg"]
+        meg = s["front"]["meg"]
         rows = B * T
         H2 = 2 * H
         dest = dest.contiguous()
@@ -995,96 +1078,10 @@ class _EncoderFn(torch.autograd.Function):
         if side is not None:
             main.wait_stream(side)
         ctx_keep.clear()
-        n_meg, n_heads, n_il_w, n_il_b, n_subj, _ = nd.front
         dheads = d_il_w = d_il_b = d_subj = d_sub_emb = dmeg = None
-        if not nd.below[0]:
-            pass                                       # the sensor side is frozen and meg does not require grad
-        elif plan.staged:
-            heads_p, il_w_p, subj_w_p, sub_emb_p = s["params"]
-            dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg = _staged_front_backward(
-                plan, s["front"], g, heads_p, il_w_p, subj_w_p, sub_emb_p, nd.front)
-        else:
-            # ---- sensor chain + attention: each stage as far as a gradient below it is asked for ----
-            want_dv = n_meg or n_heads or n_il_w or n_il_b          # the gradient at the subject layer's input
-            want_du = n_meg or n_heads                              # ... and at initial_linear's input
-            subj_order, subj_off = group_layout(plan.subject, S) if n_subj else (None, None)
-            Op, ILp = ctx.pads
-            d_att = _empty((R, O, C), meg) if n_heads else None
-            du = None
-            il_conv = s["il_conv"]
-            if il_conv is not None:
-                dv = None
-                if s["subj_pad"] is not None:
-                    if want_dv:
-                        subj_pad = s["subj_pad"]                               # [S][ILp][Dp]: data-gradient operand as is
-                        sb_hi, sb_lo = _empty((S * ILp, Dp), meg), _empty((S * ILp, Dp), meg)
-                        call("bm_tc_weight_split", ptr(subj_pad), S * ILp, Dp, 1, ptr(sb_hi), ptr(sb_lo), None, None, st)
-                        dv = _empty((B, T, ILp), meg)
-                        _tc_call("bm_tc_pointwise_sel", ptr(g), ptr(sb_hi), ptr(sb_lo), ptr(plan.subject), S, B, T, Dp, ILp,
-                                 ptr(dv), ptr(status), st)
-                    if n_subj:
-                        mpad = _round_up(ILp, 128)
-                        dm = _empty((S, mpad, Dp), meg)
-                        _tc_call("bm_tc_wgrad_grouped", ptr(s["v"]), ptr(g), ptr(subj_order), ptr(subj_off), S, B, T, ILp,
-                                 Dp, ptr(dm), ptr(status), st)
-                        d_subj = dm[:, :IL, :D].contiguous()
-                else:
-                    if want_dv:
-                        dv = torch.zeros((B, T, ILp), device=meg.device) if ILp != IL else _empty((B, T, IL), meg)
-                    d_subj = _empty((S, IL, D), meg) if n_subj else None
-                    call("bm_subject_layers_bwd", ptr(g), Dp, ptr(s["v"]), ILp, ptr(s["subj_w"]), ptr(plan.subject),
-                         ptr(subj_order), ptr(subj_off), B, T, IL, D, S, ILp, ptr(dv), ptr(d_subj), st)
-                if want_du:
-                    du = _empty((B, T, Op), meg)
-                    il_conv.backward_data(dv, None, B, T, 1, du, status)
-                if n_il_w:
-                    dbp = _empty((ILp,), meg) if n_il_b else None
-                    d_il_w = tc_wgrad(dv, s["u"], B, T, ILp, Op, O, 1, 1, status, dbias=dbp)[:IL, :, 0].contiguous()
-                    d_il_b = dbp[:IL].contiguous() if n_il_b else None
-                elif n_il_b:
-                    dbp = _empty((ILp,), meg)
-                    col_sum(dv, rows, ILp, dbp, st)
-                    d_il_b = dbp[:IL].contiguous()
-                if not n_heads:
-                    pass
-                elif s["megT"] is not None:
-                    megT = s["megT"]
-                    Cp = megT.shape[2]
-                    dwp = _empty((R, _round_up(Op, 128), Cp), meg)
-                    _tc_call("bm_tc_wgrad_grouped", ptr(du), ptr(megT), ptr(plan.rec_order), ptr(plan.rec_off), R, B, T, Op,
-                             Cp, ptr(dwp), ptr(status), st)
-                    d_att = dwp[:, :O, :C].contiguous()
-                else:
-                    call("bm_sensor_mix_bwd", ptr(du), Op, ptr(meg), ptr(plan.rec_order), ptr(plan.rec_off), B, C, T, O, R,
-                         ptr(d_att), st)
-            else:
-                dv = _empty((B, T, IL), meg) if want_dv else None
-                du = _empty((B, T, O), meg) if want_du else None
-                d_subj = _empty((S, IL, D), meg) if n_subj else None
-                d_il_w = _empty((IL, O), meg) if n_il_w else None
-                d_il_b = _empty((IL,), meg) if n_il_b else None
-                _reducing_call("bm_sensor_chain_bwd", meg, (B, T, O, IL), ptr(g), ptr(meg), ptr(s["il_w2"]), ptr(s["subj_w"]),
-                               ptr(plan.subject), ptr(s["u"]), ptr(s["v"]), ptr(subj_order), ptr(subj_off), ptr(plan.rec_order),
-                               ptr(plan.rec_off), B, C, T, O, IL, D, Dp, S, R, ptr(dv), ptr(du), ptr(d_subj), ptr(d_il_w),
-                               ptr(d_il_b), ptr(d_att), st, reduces=n_il_w or n_il_b)
-            dmeg = _sensor_mix_bwd_data(plan, s, du, ctx.dims, status) if n_meg else None
-            if not n_heads:
-                pass
-            elif s["heads_tc"]:
-                dscores = _empty((R, O, C), meg)
-                Opad = _round_up(O, 64)
-                call("bm_softmax_bwd", ptr(s["att"]), ptr(d_att), R * O, C, ptr(dscores), st)
-                ds_t = _empty((R, C, Opad), meg)                   # pad columns zeroed by the transpose
-                call("bm_transpose_nt_ld", ptr(dscores), R, O, C, Opad, ptr(ds_t), st)
-                dheads = tc_wgrad(ds_t, s["emb"], R, C, Opad, P, P, 1, 1, status)[:O, :, 0].contiguous()
-            else:
-                dscores = _empty((R, O, C), meg)
-                dheads = _empty((O, P), meg)
-                _reducing_call("bm_attention_weights_bwd", meg, None, ptr(d_att), ptr(s["att"]), ptr(s["emb"]), R, C, O, P,
-                               ptr(dscores), ptr(dheads), st)
-
-        if d_il_w is not None:
-            d_il_w = d_il_w.reshape(s["il_shape"])
+        if nd.below[0]:                                # else the sensor side is frozen and meg does not require grad
+            dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg = front_backward(plan, s["front"], g, *s["params"], nd.front,
+                                                                             status)
         if plan.bare_last:
             grads = [None, dmeg, dheads, d_il_w, d_il_b, d_subj, None, None, None, None]
         else:
@@ -1285,11 +1282,9 @@ class _MergerFn(torch.autograd.Function):
         R = positions.shape[0]
         O, P = heads.shape
         st = stream()
-        emb, att = _empty((R, C, P), meg), _empty((R, O, C), meg)
-        call("bm_attention_weights_fwd", ptr(positions), ptr(freq), ptr(heads.contiguous()), ptr(ban_centre), float(radius),
-             R, C, O, P, ptr(emb), ptr(att), st)
+        emb, att = _attention_fwd(heads, positions, freq, ban_centre, radius, C)
         u = _empty((B, T, O), meg)
-        call("bm_sensor_mix_fwd", ptr(meg), ptr(att), ptr(rec_of_sample), B, C, T, O, O, ptr(u), st)
+        _mix_fwd(meg, att, rec_of_sample, u)
         out = _empty((B, O, T), meg)
         call("bm_transpose_nt", ptr(u), B, T, O, ptr(out), st)
         if any(ctx.needs_input_grad):                  # else nothing is kept: there will be no backward
@@ -1307,14 +1302,10 @@ class _MergerFn(torch.autograd.Function):
         call("bm_transpose_nt", ptr(gout.contiguous()), B, O, T, ptr(g), st)
         dheads = None
         if ctx.needs_input_grad[1]:                    # frozen heads: no mix or attention gradient
-            d_att, dscores, dheads = _empty((R, O, C), meg), _empty((R, O, C), meg), _empty((O, P), meg)
-            call("bm_sensor_mix_bwd", ptr(g), O, ptr(meg), ptr(rec_order), ptr(rec_off), B, C, T, O, R, ptr(d_att), st)
-            _reducing_call("bm_attention_weights_bwd", meg, None, ptr(d_att), ptr(att), ptr(emb), R, C, O, P, ptr(dscores),
-                           ptr(dheads), st)
+            dheads = _attention_bwd(_mix_bwd(g, meg, att, rec_order, rec_off), att, emb)
         dmeg = None
         if ctx.needs_input_grad[0]:
-            dmeg = _empty((B, C, T), meg)
-            call("bm_sensor_mix_bwd_data", ptr(g), O, ptr(att), ptr(rec_of_sample), None, B, C, T, O, ptr(dmeg), st)
+            dmeg = _mix_bwd_data(g, att, rec_of_sample, None)
         return dmeg, dheads, None, None, None, None, None, None, None
 
 
@@ -1333,7 +1324,7 @@ class _SubjectLayersFn(torch.autograd.Function):
         call("bm_transpose_nt", ptr(x), B, Cin, T, ptr(xl), st)
         yl = _empty((B, T, D), x)
         w = weights.contiguous()
-        call("bm_subject_layers_fwd", ptr(xl), Cin, ptr(w), ptr(subject), B, T, Cin, D, D, ptr(yl), st)
+        _subject_fwd(xl, w, subject, yl)
         out = _empty((B, D, T), x)
         call("bm_transpose_nt", ptr(yl), B, T, D, ptr(out), st)
         if any(ctx.needs_input_grad):                  # else nothing is kept: there will be no backward
@@ -1351,11 +1342,7 @@ class _SubjectLayersFn(torch.autograd.Function):
         st = stream()
         g = _empty((B, T, D), gout)
         call("bm_transpose_nt", ptr(gout.contiguous()), B, D, T, ptr(g), st)
-        order, off = group_layout(subject, S) if want_dw else (None, None)
-        dxl = _empty((B, T, Cin), g) if want_dx else None
-        dw = _empty((S, Cin, D), g) if want_dw else None
-        call("bm_subject_layers_bwd", ptr(g), D, ptr(xl), Cin, ptr(w), ptr(subject), ptr(order), ptr(off), B, T, Cin, D, S,
-             Cin, ptr(dxl), ptr(dw), st)
+        dxl, dw = _subject_bwd(g, xl, w, subject, (S, Cin, D), Cin, want_dx, want_dw)
         dx = None
         if want_dx:
             dx = _empty((B, Cin, T), g)

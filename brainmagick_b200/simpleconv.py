@@ -137,7 +137,6 @@ class SimpleConv(nn.Module):
         if subject_dim:
             self.subject_embedding = ScaledEmbedding(n_subjects, subject_dim, embedding_scale)
             in_channels["meg"] += subject_dim
-        self._staged = not (merger and initial_linear and subject_layers) or bool(subject_dim)
 
         # simpleconv.py:85-90: GELU, else LeakyReLU(relu_leakiness), else ReLU -- in the ConvSequence and in the head
         if gelu:
@@ -211,7 +210,7 @@ class SimpleConv(nn.Module):
             ban_radius=0.0 if self.merger is None else float(self.merger.dropout),
             bn_buffers=bn_buffers, keep_for_backward=torch.is_grad_enabled(),
             use_tensor_cores=self.use_tensor_cores, skip=seq.skip, act_code=seq.act_code, act_slope=seq.act_slope,
-            has_act=list(seq.has_act), batch_norm=True, staged=self._staged, has_sub_emb=self.subject_embedding is not None)
+            has_act=list(seq.has_act), batch_norm=True, has_sub_emb=self.subject_embedding is not None)
 
     def forward(self, inputs, batch):
         meg = inputs["meg"]

@@ -1,9 +1,15 @@
 """Bitwise fingerprint of deterministic training steps, for comparing two builds of the library's host code.
 
-Under torch.use_deterministic_algorithms(True), from fixed seeds: 3 SimpleConv training steps at bench.py's cfg2 (forward,
-ClipLoss, backward, Adam) and 3 DeepMel training steps at conf/feature_model/deep_mel.yaml's widths (ClipLoss against a
-trainable estimate, Adam on both).  Every loss, estimate, gradient, parameter and BatchNorm running statistic after each step
-is hashed (sha256 of its bytes), so two host-code versions that issue the same kernels must give identical fingerprints.
+Under torch.use_deterministic_algorithms(True), from fixed seeds:
+  * 3 SimpleConv training steps at bench.py's cfg2 (forward, ClipLoss, backward, Adam), and the same for the front's ablation
+    rows merger=False, initial_linear=0 and subject_layers=False with subject_dim=64;
+  * a cfg2 attribution step: eval mode, every parameter frozen, meg requiring grad;
+  * 3 stand-alone ChannelMerger -> SubjectLayers steps at clip_conv's widths (270 merger channels, pos_dim 2048), with the
+    gradient reaching meg;
+  * 3 DeepMel training steps at conf/feature_model/deep_mel.yaml's widths (ClipLoss against a trainable estimate, Adam on
+    both).
+Every loss, output, gradient, parameter and BatchNorm running statistic after each step is hashed (sha256 of its bytes), so
+two host-code versions that issue the same kernels must give identical fingerprints.
 
     python profiles/stack_bitwise.py --dump a.json [--root TREE]    # TREE: the checkout whose brainmagick_b200 is imported
     python profiles/stack_bitwise.py --compare a.json b.json
@@ -19,6 +25,10 @@ import os
 import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+
+
+ROWS = {"simpleconv": {}, "no_merger": dict(merger=False), "no_initial_linear": dict(initial_linear=0),
+        "no_subject_layers": dict(subject_layers=False, subject_dim=64)}     # SimpleConv training steps: tag -> overrides
 
 
 def _digest(t) -> str:
@@ -49,22 +59,52 @@ def dump(steps, batch, deepmel_batch):
 
     cfg = bench.CONFIGS["cfg2"]
     C, T, F, S = cfg["C"], cfg["T"], cfg["F"], cfg["S"]
-    torch.manual_seed(2036)
-    model = bb.SimpleConv(in_channels=dict(meg=C), out_channels=F, n_subjects=S,
-                          **{k: (dict(v) if isinstance(v, dict) else v) for k, v in bench.CLIP_CONV.items()}).to(dev).train()
-    clip = bb.ClipLoss().to(dev).train()
-    opt = torch.optim.Adam(model.parameters(), lr=3e-4)
     positions = synthetic.normalised_positions(S, C, seed=7)
     recs = [synthetic.SyntheticRecording(s, positions[s]) for s in range(S)]
     meg, feats, subj = (t.to(dev) for t in bench.make_host_batch(cfg, batch, 2036))
     sbatch = synthetic.SyntheticBatch(meg, subj, [recs[s] for s in subj.tolist()])
     mask = torch.ones(batch, 1, T, dtype=torch.bool, device=dev)
+    clip = bb.ClipLoss().to(dev).train()
+
+    def simpleconv(**overrides):
+        kw = {k: (dict(v) if isinstance(v, dict) else v) for k, v in bench.CLIP_CONV.items()}
+        kw.update(overrides)
+        torch.manual_seed(2036)
+        return bb.SimpleConv(in_channels=dict(meg=C), out_channels=F, n_subjects=S, **kw).to(dev).train()
+
+    for tag, overrides in ROWS.items():
+        model = simpleconv(**overrides)
+        opt = torch.optim.Adam(model.parameters(), lr=3e-4)
+        for step in range(steps):
+            opt.zero_grad(set_to_none=True)
+            est = model(dict(meg=meg), sbatch)
+            loss = clip(est, feats, mask)
+            loss.backward()
+            _record(out, f"{tag}.{step}", loss, est, {"model": model})
+            opt.step()
+    BF.check_tc_status()
+
+    model = simpleconv().eval().requires_grad_(False)
+    meg_in = meg.clone().requires_grad_(True)
+    est = model(dict(meg=meg_in), sbatch)
+    loss = clip(est, feats, mask)
+    loss.backward()
+    _record(out, "attribution", loss, est, {"model": model})
+    out["attribution.grad.meg"] = _digest(meg_in.grad)
+    BF.check_tc_status()
+
+    torch.manual_seed(2038)
+    merger = bb.ChannelMerger(270, pos_dim=2048, dropout=0.2, n_subjects=S).to(dev).train()
+    layer = bb.SubjectLayers(270, 270, S).to(dev)
+    gout = torch.randn(batch, 270, T, device=dev)
+    opt = torch.optim.Adam(list(merger.parameters()) + list(layer.parameters()), lr=3e-4)
     for step in range(steps):
         opt.zero_grad(set_to_none=True)
-        est = model(dict(meg=meg), sbatch)
-        loss = clip(est, feats, mask)
-        loss.backward()
-        _record(out, f"simpleconv.{step}", loss, est, {"model": model})
+        meg_in = meg.clone().requires_grad_(True)
+        y = layer(merger(meg_in, sbatch), subj)
+        y.backward(gout)
+        _record(out, f"merger_subject_layers.{step}", (y * gout).sum(), y, {"merger": merger, "subject_layers": layer})
+        out[f"merger_subject_layers.{step}.grad.meg"] = _digest(meg_in.grad)
         opt.step()
     BF.check_tc_status()
 
