@@ -63,11 +63,6 @@ class EncoderPlan(SequencePlan):
     channel_mask: tp.Optional[torch.Tensor] = None   # [C] subsample_meg_channels mask (simpleconv.py:200-203), or None
     masked_meg: tp.Optional[torch.Tensor] = None     # [B,C,T] buffer that receives meg * channel_mask
 
-    @property
-    def bare_last(self) -> bool:
-        """no head: the last conv maps to out_channels and has neither BatchNorm nor activation"""
-        return not self.has_act[-1]
-
 
 def _empty(shape, like, dtype=torch.float32):
     return torch.empty(shape, device=like.device, dtype=dtype)
@@ -108,6 +103,24 @@ def _side_stream(device) -> torch.cuda.Stream:
     if device not in _side_streams:
         _side_streams[device] = torch.cuda.Stream(device=device)
     return _side_streams[device]
+
+
+def _on_side(side, keep_alive, fn, *operands):
+    """fn() on the weight-gradient stream `side`, after everything queued so far on the current (main) stream; side None:
+    inline.  The operands the side kernels read go to `keep_alive`, which the caller keeps until the main stream has waited
+    on `side` (no record_stream on them: with the host running steps ahead it would block the allocator from reusing ~3 GB
+    of blocks and force cudaMallocs in the timed loop); fn's output tensors are recorded on the main stream."""
+    if side is None:
+        return fn()
+    main = torch.cuda.current_stream()
+    side.wait_stream(main)
+    with torch.cuda.stream(side):
+        out = fn()
+    keep_alive.append(operands)
+    for o in out if isinstance(out, tuple) else (out,):
+        if o is not None:
+            o.record_stream(main)
+    return out
 
 
 def _round_up(n, m):
@@ -408,32 +421,21 @@ def conv_stack_forward(plan: SequencePlan, x, conv0: _Conv, conv_p, glu_p, nd: "
 def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, T, status, side=None, keep_alive=None):
     """g = dL/d(output of conv_stack_forward) [B,T,C_last] -> (per layer (d conv_w, d conv_b, d gamma, d beta),
     {k: (d glu_w, d glu_b)}, dL/dx); None for every gradient not asked for, and dL/dx only if nd.below[0].  The backward
-    stops at the deepest layer that needs a gradient.  `side`: a stream for the weight-gradient kernels, concurrent with the
-    data-gradient kernels (None: inline); their operands go to `keep_alive`, which the caller keeps until it has joined the
-    streams (no record_stream: with the host running steps ahead it would block the allocator from reusing ~3 GB of blocks
-    and force cudaMallocs in the timed loop)."""
+    stops at the deepest layer that needs a gradient.  `side`, `keep_alive`: the weight-gradient kernels run through
+    `_on_side`, concurrent with the data-gradient kernels (side None: inline)."""
     st = stream()
     rows = B * T
     like = status                                   # allocations only read the device off it
     sums = _empty((2 * max(p[0].shape[0] for p in conv_p),), like, torch.float64)
     layer_grads: tp.List[tp.Any] = [(None, None, None, None)] * len(conv_p)
     glu_grads = {k: (None, None) for k in nd.glu}
-    main = torch.cuda.current_stream() if side is not None else None
 
     def weight_grad(conv: _Conv, dy, x, dilation, bias_zero, known_dbias=None, want=(True, True)):
         if not any(want):
             return None, None
-        kw = dict(bias_grad_is_zero=bias_zero, known_dbias=known_dbias, want_w=want[0], want_b=want[1])
-        if side is None:
-            return conv.backward_weight(dy, x, B, T, dilation, like, status, **kw)
-        side.wait_stream(main)
-        with torch.cuda.stream(side):
-            out = conv.backward_weight(dy, x, B, T, dilation, like, status, **kw)
-        keep_alive.append((dy, x))
-        for o in out:
-            if o is not None:
-                o.record_stream(main)
-        return out
+        return _on_side(side, keep_alive, lambda: conv.backward_weight(
+            dy, x, B, T, dilation, like, status, bias_grad_is_zero=bias_zero, known_dbias=known_dbias, want_w=want[0],
+            want_b=want[1]), dy, x)
 
     for k in reversed(range(len(conv_p))):
         if not nd.below[k + 1]:
@@ -840,6 +842,129 @@ def front_backward(plan: "EncoderPlan", rec, g, heads, il_w, subj_w, sub_emb, ne
     return dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg
 
 
+# ----------------------------------------------------------------------------------------------------
+# The output head (simpleconv.py:185-193, 245): `final` = 1x1 Conv1d [2H,H] -> activation -> 1x1 ConvTranspose1d [2H,F] on
+# the channels-last output of the conv stack, handed out channel-major; with complex_out=False only the transpose.
+# ----------------------------------------------------------------------------------------------------
+def head_forward(plan: "EncoderPlan", x, w0, b0, w2, b2, nd: "_Needs", save: bool, B, T, status):
+    """x [B,T,H] (the conv stack's output) -> (estimate [B,F,T], the record `head_backward` reads).  w0, b0, w2, b2: the
+    Conv1d and ConvTranspose1d parameters, all None without a head.  `save`: a backward will run.  The form is chosen here:
+      bare       no head: the stack already ends on out_channels, the estimate is its transpose;
+      generic    an activation other than GELU: the two convs as `_Conv`s with the activation kernel between them, then a
+                 transpose to channel-major;
+      tc         GELU, and both convs pass the tensor-core gates both ways: the GELU and the channel-major store fused into
+                 the conv epilogues, and the weight gradients on the tensor cores (on the side stream);
+      tc_params  the same where the weight gradients' shapes do not fit the tensor cores: they come from
+                 `bm_head_bwd_params`;
+      fma        GELU, a conv gate fails: the FP32-FMA `bm_head_fwd` / `bm_head_bwd`."""
+    st = stream()
+    if w0 is None:
+        F = x.shape[2]
+        est = _empty((B, F, T), x)
+        call("bm_transpose_nt", ptr(x), B, T, F, ptr(est), st)
+        return est, dict(form="bare", F=F)
+    H, F = w0.shape[1], w2.shape[1]
+    H2 = 2 * H
+    n_w0, n_b0, n_w2, _ = nd.head
+    want_g = nd.below[-1]                            # the gradient at the head's input (the stack's output)
+    want_dh1 = want_g or n_w0 or n_b0                # ... and below the head's activation
+    tc = plan.use_tensor_cores
+    head0 = _Conv(w0, T, False, tc, want_bwd=save and want_g)                                    # [2H, H, 1]
+    head2 = _Conv(w2.permute(1, 0, 2).contiguous(), T, False, tc, want_bwd=save and want_dh1)    # as a conv: [F, 2H, 1]
+    h1, q, est = _empty((B, T, H2), x), _empty((B, T, H2), x), _empty((B, F, T), x)
+    if plan.act_code != ACT_GELU:
+        form = "generic"
+    elif head0.fwd_tc and head2.fwd_tc and head0.bwd_tc and head2.bwd_tc:
+        form = "tc" if head0.wgrad_tc and bool(_lib.load().bm_tc_wgrad_supported(H2, F)) else "tc_params"
+    else:
+        form = "fma"
+    w0_2, w2_2 = w0.reshape(H2, H).contiguous(), w2.reshape(H2, F).contiguous()
+    if form == "fma":
+        call("bm_head_fwd", ptr(x), ptr(w0_2), ptr(b0.contiguous()), ptr(w2_2), ptr(b2.contiguous()), B, T, H, F, ptr(h1),
+             ptr(q), ptr(est), st)
+    elif form == "generic":
+        head0.forward(x, b0.contiguous(), B, T, 1, h1, None, status)
+        call("bm_bn_act_skip_fwd", ptr(h1), None, None, None, None, None, ptr(q), B * T, H2, plan.act_code,
+             float(plan.act_slope), st)
+        est_cl = _empty((B, T, F), x)
+        head2.forward(q, b2.contiguous(), B, T, 1, est_cl, None, status)
+        call("bm_transpose_nt", ptr(est_cl), B, T, F, ptr(est), st)
+    else:
+        head0.run_tc(True, x, b0.contiguous(), None, B, T, 1, 0, 1, 0, q, h1 if save else None, None, None, status)
+        head2.run_tc(True, q, b2.contiguous(), None, B, T, 1, 0, 0, 1, est, None, None, None, status)
+    return est, dict(form=form, H=H, F=F, want_g=want_g, want_dh1=want_dh1, head0=head0, head2=head2, w0_2=w0_2, w2_2=w2_2,
+                     h1=h1, x_last=x if n_w0 else None, q=q if n_w2 else None)
+
+
+def head_backward(plan: "EncoderPlan", rec, dest, need, B, T, status, side, keep_alive):
+    """dest = dL/d(estimate) [B,F,T] -> (g = dL/dx [B,T,H] of `head_forward`'s x, d w0, d b0, d w2, d b2); None for every
+    gradient not asked for, and g only if the forward's `nd.below` asked for it.  need = requires-grad of (w0, b0, w2, b2).
+    `side`, `keep_alive`: the tensor-core weight gradients run through `_on_side`."""
+    st = stream()
+    dest = dest.contiguous()
+    form = rec["form"]
+    if form == "bare":
+        g = _empty((B, T, rec["F"]), dest)   # the gradient of the estimate IS the stack's output gradient
+        call("bm_transpose_nt", ptr(dest), B, rec["F"], T, ptr(g), st)
+        return g, None, None, None, None
+    H, F = rec["H"], rec["F"]
+    H2, rows = 2 * H, B * T
+    n_w0, n_b0, n_w2, n_b2 = need
+    want_g, want_dh1 = rec["want_g"], rec["want_dh1"]
+    x_last, h1, q = rec["x_last"], rec["h1"], rec["q"]
+    g = _empty((B, T, H), dest) if want_g else None
+    dw0 = dw2 = db0 = db2 = None
+    if form in ("tc_params", "fma"):                   # the fused kernels write the gradients asked of them
+        dw0 = _empty((H2, H, 1), dest) if n_w0 else None
+        db0 = _empty((H2,), dest) if n_b0 else None
+        dw2 = _empty((H2, F, 1), dest) if n_w2 else None
+        db2 = _empty((F,), dest) if n_b2 else None
+    if form == "fma":
+        dq = _empty((B, T, H2), dest) if want_dh1 else None
+        _reducing_call("bm_head_bwd", dest, (B, T, H, F), ptr(dest), ptr(x_last), ptr(rec["w0_2"]), ptr(rec["w2_2"]),
+                       ptr(h1), ptr(q), B, T, H, F, ptr(dq), ptr(g), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st,
+                       reduces=any(need))
+        return g, dw0, db0, dw2, db2
+
+    head0: _Conv = rec["head0"]
+    head2: _Conv = rec["head2"]
+    dest_t = _empty((B, T, F), dest)
+    call("bm_transpose_nt", ptr(dest), B, F, T, ptr(dest_t), st)
+    dq = None                                         # dL/dq, q = act(h1) the ConvTranspose's input
+    if want_dh1 or (form == "tc_params" and (n_w2 or n_b2)):     # bm_head_bwd_params reads dq in any case
+        dq = _empty((B, T, H2), dest)
+        head2.backward_data(dest_t, None, B, T, 1, dq, status)
+    # dW2 / db2, and dh1 = dL/dh1 (in place of dq where the activation backward allows it)
+    dh1 = dq
+    if form == "generic":
+        dw2c, db2 = head2.backward_weight(dest_t, q, B, T, 1, dest, status, want_w=n_w2, want_b=n_b2)   # [F, 2H, 1]
+        dw2 = None if dw2c is None else dw2c.permute(1, 0, 2).contiguous()
+        if want_dh1:
+            dh1 = _empty((B, T, H2), dest)
+            call("bm_bn_act_skip_bwd", ptr(dq), ptr(h1), None, None, None, None, 0, rows, H2, plan.act_code,
+                 float(plan.act_slope), None, ptr(dh1), None, None, st)
+    elif form == "tc":
+        if n_w2:    # in the ConvTranspose layout [2H, F, 1]; overlaps the dq contraction queued just before
+            dw2 = _on_side(side, keep_alive, lambda: tc_wgrad(q, dest_t, B, T, H2, F, F, 1, 1, status), q, dest_t)
+        if n_b2:
+            db2 = _empty((F,), dest)
+            col_sum(dest_t, rows, F, db2, st)
+        if want_dh1:
+            call("bm_gelu_bwd", ptr(dq), ptr(h1), rows * H2, ptr(dq), st)
+    elif any(need):
+        _reducing_call("bm_head_bwd_params", dest, (B, T, H, F), ptr(dest), ptr(x_last), ptr(h1), ptr(q), B, T, H, F,
+                       ptr(dq), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st)
+    elif want_g:
+        call("bm_gelu_bwd", ptr(dq), ptr(h1), rows * H2, ptr(dq), st)
+    if form != "tc_params" and (n_w0 or n_b0):
+        # on the side stream only the weight contraction (a lone bias sum stays on the main stream)
+        dw0, db0 = _on_side(side if form == "tc" and n_w0 else None, keep_alive, lambda: head0.backward_weight(
+            dh1, x_last, B, T, 1, dest, status, want_w=n_w0, want_b=n_b0), dh1, x_last)
+    if want_g:
+        head0.backward_data(dh1, None, B, T, 1, g, status)
+    return g, dw0, db0, dw2, db2
+
+
 @dataclasses.dataclass
 class _Needs:
     """Which gradients a backward is asked for (`ctx.needs_input_grad`, fixed at forward time), stage by stage from the input.
@@ -900,63 +1025,16 @@ class _EncoderFn(torch.autograd.Function):
             # inside the node, so that the gradient reaches the caller's unmasked tensor (the backward applies the mask)
             call("bm_channel_mask", ptr(meg), ptr(plan.channel_mask), B, C, T, ptr(plan.masked_meg), st)
             meg = plan.masked_meg
-        H = conv_p[0][0].shape[0]
-        F = conv_p[-1][0].shape[0] if plan.bare_last else w2.shape[1]
-        rows = B * T
         nd = _Needs.of(ctx.needs_input_grad, plan)
         save = plan.keep_for_backward and any(ctx.needs_input_grad)
-        tc = plan.use_tensor_cores
         status = tc_status_tensor(meg.device)
 
         x, conv0, front = front_forward(plan, meg, heads, il_w, il_b, subj_w, sub_emb, conv_p[0][0], nd, save, status)
-        # K3/K4 ConvSequence
-        x, saved_layers = conv_stack_forward(plan, x, conv0, conv_p, glu_p, nd, save, B, T, status, bare_slope=0.0)
-
+        x, layers = conv_stack_forward(plan, x, conv0, conv_p, glu_p, nd, save, B, T, status, bare_slope=0.0)
+        est, head = head_forward(plan, x, w0, b0, w2, b2, nd, save, B, T, status)
         if save:
-            ctx.plan, ctx.needs, ctx.dims = plan, nd, (B, T, H, F)
-            ctx.saved = dict(front=front, layers=saved_layers, conv_p=conv_p, params=(heads, il_w, subj_w, sub_emb))
-
-        if plan.bare_last:
-            # no head: the sequence already ends on out_channels; hand it out channel-major
-            est = _empty((B, F, T), meg)
-            call("bm_transpose_nt", ptr(x), B, T, F, ptr(est), st)
-            return est
-
-        # K5 head
-        H2 = 2 * H
-        want_dh1 = nd.below[depth] or nd.head[0] or nd.head[1]               # the gradient below the head's GELU
-        head0 = _Conv(w0, T, False, tc, want_bwd=save and nd.below[depth])   # [2H, H, 1]
-        w2_as_conv = w2.permute(1, 0, 2).contiguous()                        # ConvTranspose1d [2H,F,1] -> [F,2H,1]
-        head2 = _Conv(w2_as_conv, T, False, tc, want_bwd=save and want_dh1)
-        head_tc = head0.fwd_tc and head2.fwd_tc and head0.bwd_tc and head2.bwd_tc
-        h1 = _empty((B, T, H2), meg)
-        q = _empty((B, T, H2), meg)
-        est = _empty((B, F, T), meg)
-        w0_2 = w0.reshape(H2, H).contiguous()
-        w2_2 = w2.reshape(H2, F).contiguous()
-        head_generic = plan.act_code != ACT_GELU
-        if head_generic:
-            # simpleconv.gelu=False (simpleconv.py:85-90,187): conv -> activation kernel -> conv, channels-last, then one
-            # transpose to the channel-major estimate (the fused GELU epilogues below do not apply)
-            head_tc = False
-            head0.forward(x, b0.contiguous(), B, T, 1, h1, None, status)
-            call("bm_bn_act_skip_fwd", ptr(h1), None, None, None, None, None, ptr(q), rows, H2, plan.act_code,
-                 float(plan.act_slope), st)
-            est_cl = _empty((B, T, F), meg)
-            head2.forward(q, b2.contiguous(), B, T, 1, est_cl, None, status)
-            call("bm_transpose_nt", ptr(est_cl), B, T, F, ptr(est), st)
-            del est_cl
-        elif head_tc:
-            head0.run_tc(True, x, b0.contiguous(), None, B, T, 1, 0, 1, 0, q, h1 if save else None, None, None, status)
-            head2.run_tc(True, q, b2.contiguous(), None, B, T, 1, 0, 0, 1, est, None, None, None, status)
-        else:
-            call("bm_head_fwd", ptr(x), ptr(w0_2), ptr(b0.contiguous()), ptr(w2_2), ptr(b2.contiguous()), B, T, H, F,
-                 ptr(h1), ptr(q), ptr(est), st)
-
-        if save:
-            ctx.saved.update(x_last=x if nd.head[0] else None, w0_2=w0_2, w2_2=w2_2, h1=h1, q=q if nd.head[2] else None,
-                             head0=head0, head2=head2, head_tc=head_tc, head_generic=head_generic, w0_shape=w0.shape,
-                             w2_shape=w2.shape)
+            ctx.plan, ctx.needs, ctx.dims = plan, nd, (B, T)
+            ctx.saved = dict(front=front, layers=layers, conv_p=conv_p, head=head, params=(heads, il_w, subj_w, sub_emb))
         return est
 
     @staticmethod
@@ -967,126 +1045,26 @@ class _EncoderFn(torch.autograd.Function):
         if s is None:
             raise RuntimeError("brainmagick_b200.SimpleConv: backward through the graph a second time -- the saved activations "
                                "(~5 GB at B=256) are released by the first backward; retain_graph is not supported")
-        B, T, H, F = ctx.dims
+        B, T = ctx.dims
         depth = len(plan.dilations)
-        st = stream()
-        meg = s["front"]["meg"]
-        rows = B * T
-        H2 = 2 * H
-        dest = dest.contiguous()
-        status = tc_status_tensor(meg.device)
-
         nd: _Needs = ctx.needs
-        n_w0, n_b0, n_w2, n_b2 = nd.head
-        want_g = nd.below[depth]                # the gradient at the head's input (the sequence's output)
-        want_dh1 = want_g or n_w0 or n_b0       # the gradient below the head's GELU
-
-        ctx_keep: tp.List[tp.Any] = []          # operands of side-stream kernels, released after the streams join
-        # ---- head ----
-        if plan.bare_last:
-            g = _empty((B, T, F), meg)           # no head: the gradient of the estimate IS the sequence's output gradient
-            call("bm_transpose_nt", ptr(dest), B, F, T, ptr(g), st)
-            dw0 = db0 = dw2 = db2 = dq = None
-        else:
-            g = _empty((B, T, H), meg) if want_g else None
-            dw0 = _empty((H2, H), meg) if n_w0 else None
-            db0 = _empty((H2,), meg) if n_b0 else None
-            dw2 = _empty((H2, F), meg) if n_w2 else None
-            db2 = _empty((F,), meg) if n_b2 else None
-            dq = _empty((B, T, H2), meg) if want_dh1 else None
-        if plan.bare_last:
-            pass
-        elif s["head_generic"]:
-            head0, head2 = s["head0"], s["head2"]
-            dest_t = _empty((B, T, F), meg)
-            call("bm_transpose_nt", ptr(dest), B, F, T, ptr(dest_t), st)
-            if want_dh1:
-                head2.backward_data(dest_t, None, B, T, 1, dq, status)             # dq = dest_t @ w2^T
-            dw2c, db2 = head2.backward_weight(dest_t, s["q"], B, T, 1, meg, status, want_w=n_w2, want_b=n_b2)  # [F, 2H, 1]
-            dw2 = None if dw2c is None else dw2c.permute(1, 0, 2).reshape(H2, F).contiguous()
-            if want_dh1:
-                dh1 = _empty((B, T, H2), meg)
-                call("bm_bn_act_skip_bwd", ptr(dq), ptr(s["h1"]), None, None, None, None, 0, rows, H2, plan.act_code,
-                     float(plan.act_slope), None, ptr(dh1), None, None, st)
-                dw0, db0 = head0.backward_weight(dh1, s["x_last"], B, T, 1, meg, status, want_w=n_w0, want_b=n_b0)  # [2H,H,1]
-                if want_g:
-                    head0.backward_data(dh1, None, B, T, 1, g, status)
-                del dh1
-            del dest_t
-        elif s["head_tc"]:
-            head0, head2 = s["head0"], s["head2"]
-            dest_t = _empty((B, T, F), meg)
-            call("bm_transpose_nt", ptr(dest), B, F, T, ptr(dest_t), st)
-            # dq = dest_t @ w2^T  (w2_as_conv [F,2H,1]: its data-gradient operand is [1][2H][F])
-            lib = _lib.load()
-            wgrad_tc = lib.bm_tc_wgrad_supported(H2, F) and lib.bm_tc_wgrad_supported(H2, H)
-            if dq is None and not wgrad_tc and (n_w2 or n_b2):
-                dq = _empty((B, T, H2), meg)                               # bm_head_bwd_params turns dq into dh1 in any case
-            if dq is not None:
-                head2.run_tc(False, dest_t, None, None, B, T, 1, 0, 0, 0, dq, None, None, None, status)
-            if not wgrad_tc:
-                if dw0 is not None or db0 is not None or dw2 is not None or db2 is not None:
-                    _reducing_call("bm_head_bwd_params", meg, (B, T, H, F), ptr(dest), ptr(s["x_last"]), ptr(s["h1"]),
-                                   ptr(s["q"]), B, T, H, F, ptr(dq), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st)
-                elif want_g:
-                    call("bm_gelu_bwd", ptr(dq), ptr(s["h1"]), rows * H2, ptr(dq), st)       # dq <- dh1
-            else:
-                main0 = torch.cuda.current_stream()
-                side0 = _side_stream(meg.device) if OVERLAP_WGRAD else None
-
-                def on_side(fn, *tensors):
-                    """runs fn() on the side stream after everything queued so far on the main stream"""
-                    if side0 is None:
-                        return fn()
-                    side0.wait_stream(main0)
-                    with torch.cuda.stream(side0):
-                        out = fn()
-                    ctx_keep.append(tensors)
-                    out.record_stream(main0)
-                    return out
-
-                # dW2 / db2 only need dest_t and q: they overlap the dq contraction queued just before
-                if n_w2:
-                    dw2 = on_side(lambda: tc_wgrad(s["q"], dest_t, B, T, H2, F, F, 1, 1, status), s["q"],
-                                  dest_t).reshape(H2, F)
-                if n_b2:
-                    col_sum(dest_t, rows, F, db2, st)
-                if want_dh1:
-                    call("bm_gelu_bwd", ptr(dq), ptr(s["h1"]), rows * H2, ptr(dq), st)       # dq <- dh1
-                if n_w0:
-                    dw0 = on_side(lambda: tc_wgrad(dq, s["x_last"], B, T, H2, H, H, 1, 1, status, dbias=db0), dq,
-                                  s["x_last"], db0).reshape(H2, H)
-                elif n_b0:
-                    col_sum(dq, rows, H2, db0, st)
-            if want_g:
-                head0.run_tc(False, dq, None, None, B, T, 1, 0, 0, 0, g, None, None, None, status)
-            del dest_t
-        else:
-            _reducing_call("bm_head_bwd", meg, (B, T, H, F), ptr(dest), ptr(s["x_last"]), ptr(s["w0_2"]), ptr(s["w2_2"]),
-                           ptr(s["h1"]), ptr(s["q"]), B, T, H, F, ptr(dq), ptr(g), ptr(dw0), ptr(db0), ptr(dw2), ptr(db2), st,
-                           reduces=any(nd.head))
-        del dq
-
-        # The weight gradient and the data gradient of a layer are independent given dy: the weight-gradient kernels go to
-        # a side stream so that their CTAs fill the SMs left idle by the partial last wave of the data-gradient kernel
-        # (when there is a weight gradient to overlap at all).
-        any_wgrad = any(any(n[:2]) for n in nd.layer) or any(any(n) for n in nd.glu.values())
-        main = torch.cuda.current_stream()
-        side = _side_stream(meg.device) if (OVERLAP_WGRAD and plan.use_tensor_cores and any_wgrad) else None
+        status = tc_status_tensor(dest.device)
+        # The weight gradient and the data gradient of a layer are independent given dy: the tensor-core weight-gradient
+        # kernels go to a side stream so that their CTAs fill the SMs left idle by the partial last wave of the
+        # data-gradient kernel.  What they read stays in ctx_keep until the main stream has waited on them.
+        side = _side_stream(dest.device) if (OVERLAP_WGRAD and plan.use_tensor_cores) else None
+        ctx_keep: tp.List[tp.Any] = []
+        g, *head_grads = head_backward(plan, s["head"], dest, nd.head, B, T, status, side, ctx_keep)
         layer_grads, glu_grads, g = conv_stack_backward(plan, s["conv_p"], s["layers"], g, nd, B, T, status, side=side,
                                                         keep_alive=ctx_keep)
-        if side is not None:
-            main.wait_stream(side)
+        if ctx_keep:                                   # something ran on the side stream
+            torch.cuda.current_stream().wait_stream(side)
         ctx_keep.clear()
         dheads = d_il_w = d_il_b = d_subj = d_sub_emb = dmeg = None
         if nd.below[0]:                                # else the sensor side is frozen and meg does not require grad
             dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg = front_backward(plan, s["front"], g, *s["params"], nd.front,
                                                                              status)
-        if plan.bare_last:
-            grads = [None, dmeg, dheads, d_il_w, d_il_b, d_subj, None, None, None, None]
-        else:
-            grads = [None, dmeg, dheads, d_il_w, d_il_b, d_subj, None if dw0 is None else dw0.reshape(s["w0_shape"]), db0,
-                     None if dw2 is None else dw2.reshape(s["w2_shape"]), db2]
+        grads = [None, dmeg, dheads, d_il_w, d_il_b, d_subj, *head_grads]
         for k in range(depth):
             grads.extend(layer_grads[k])
         for k in range(depth):

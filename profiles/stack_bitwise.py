@@ -2,7 +2,10 @@
 
 Under torch.use_deterministic_algorithms(True), from fixed seeds:
   * 3 SimpleConv training steps at bench.py's cfg2 (forward, ClipLoss, backward, Adam), and the same for the front's ablation
-    rows merger=False, initial_linear=0 and subject_layers=False with subject_dim=64;
+    rows merger=False, initial_linear=0 and subject_layers=False with subject_dim=64, and for the head's rows gelu=False
+    and complex_out=False;
+  * 3 cfg4 training steps (120 output channels: the FP32-FMA head behind tensor-core layers);
+  * 3 cfg2 head-only steps: every parameter but `final.*` frozen, Adam on `final.*`;
   * a cfg2 attribution step: eval mode, every parameter frozen, meg requiring grad;
   * 3 stand-alone ChannelMerger -> SubjectLayers steps at clip_conv's widths (270 merger channels, pos_dim 2048), with the
     gradient reaching meg;
@@ -28,7 +31,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
 ROWS = {"simpleconv": {}, "no_merger": dict(merger=False), "no_initial_linear": dict(initial_linear=0),
-        "no_subject_layers": dict(subject_layers=False, subject_dim=64)}     # SimpleConv training steps: tag -> overrides
+        "no_subject_layers": dict(subject_layers=False, subject_dim=64), "no_gelu": dict(gelu=False),
+        "no_complex_out": dict(complex_out=False)}                       # SimpleConv training steps: tag -> overrides
 
 
 def _digest(t) -> str:
@@ -57,24 +61,28 @@ def dump(steps, batch, deepmel_batch):
     torch.cuda.set_device(dev)
     out = {"library": os.path.abspath(bb.__file__)}
 
-    cfg = bench.CONFIGS["cfg2"]
-    C, T, F, S = cfg["C"], cfg["T"], cfg["F"], cfg["S"]
-    positions = synthetic.normalised_positions(S, C, seed=7)
-    recs = [synthetic.SyntheticRecording(s, positions[s]) for s in range(S)]
-    meg, feats, subj = (t.to(dev) for t in bench.make_host_batch(cfg, batch, 2036))
-    sbatch = synthetic.SyntheticBatch(meg, subj, [recs[s] for s in subj.tolist()])
+    def data(name):
+        cfg = bench.CONFIGS[name]
+        C, T, S = cfg["C"], cfg["T"], cfg["S"]
+        positions = synthetic.normalised_positions(S, C, seed=7)
+        recs = [synthetic.SyntheticRecording(s, positions[s]) for s in range(S)]
+        meg, feats, subj = (t.to(dev) for t in bench.make_host_batch(cfg, batch, 2036))
+        return cfg, meg, feats, subj, synthetic.SyntheticBatch(meg, subj, [recs[s] for s in subj.tolist()])
+
+    cfg, meg, feats, subj, sbatch = data("cfg2")
+    T, S = cfg["T"], cfg["S"]
     mask = torch.ones(batch, 1, T, dtype=torch.bool, device=dev)
     clip = bb.ClipLoss().to(dev).train()
 
-    def simpleconv(**overrides):
+    def simpleconv(cfg=cfg, **overrides):
         kw = {k: (dict(v) if isinstance(v, dict) else v) for k, v in bench.CLIP_CONV.items()}
         kw.update(overrides)
         torch.manual_seed(2036)
-        return bb.SimpleConv(in_channels=dict(meg=C), out_channels=F, n_subjects=S, **kw).to(dev).train()
+        model = bb.SimpleConv(in_channels=dict(meg=cfg["C"]), out_channels=cfg["F"], n_subjects=cfg["S"], **kw)
+        return model.to(dev).train()
 
-    for tag, overrides in ROWS.items():
-        model = simpleconv(**overrides)
-        opt = torch.optim.Adam(model.parameters(), lr=3e-4)
+    def train(tag, model, params, meg, feats, sbatch):
+        opt = torch.optim.Adam(params, lr=3e-4)
         for step in range(steps):
             opt.zero_grad(set_to_none=True)
             est = model(dict(meg=meg), sbatch)
@@ -82,7 +90,18 @@ def dump(steps, batch, deepmel_batch):
             loss.backward()
             _record(out, f"{tag}.{step}", loss, est, {"model": model})
             opt.step()
-    BF.check_tc_status()
+        BF.check_tc_status()
+
+    for tag, overrides in ROWS.items():
+        model = simpleconv(**overrides)
+        train(tag, model, model.parameters(), meg, feats, sbatch)
+    model = simpleconv()
+    model.requires_grad_(False)
+    model.final.requires_grad_(True)
+    train("head_only", model, model.final.parameters(), meg, feats, sbatch)
+    cfg4, meg4, feats4, _, sbatch4 = data("cfg4")
+    model = simpleconv(cfg4)
+    train("cfg4", model, model.parameters(), meg4, feats4, sbatch4)
 
     model = simpleconv().eval().requires_grad_(False)
     meg_in = meg.clone().requires_grad_(True)
