@@ -80,6 +80,8 @@ SIGNATURES = {
     "bm_gather_rows": [P, P, I, L, P, P],
     "bm_bn_act_skip_fwd": [P, P, P, P, P, P, P, L, I, I, F, P],
     "bm_bn_act_skip_bwd": [P, P, P, P, P, P, I, L, I, I, F, P, P, P, P, P],
+    "bm_bn_act_gain_skip_fwd": [P, P, P, P, P, P, P, L, I, I, F, P, F, P, P],
+    "bm_bn_act_gain_skip_bwd": [P, P, P, P, P, P, I, L, I, I, F, P, F, P, P, P, P, P, P, P, P],
     "bm_clip_loss_bwd_cand": [P, P, P, P, P, P, I, I, L, I, P, P, P, P, P],
     "bm_clip_scores_bwd": [P, P, P, P, P, I, I, L, P, P, P, P, P, P],
     # deterministic forms (deterministic() below) and their workspace size queries (which return long long floats)
@@ -91,6 +93,8 @@ SIGNATURES = {
     "bm_bn_gelu_skip_bwd_det": [P, P, P, P, P, P, I, L, I, P, P, P, P, P, P, L, P],
     "bm_bn_act_skip_bwd_det_workspace": [L, I],
     "bm_bn_act_skip_bwd_det": [P, P, P, P, P, P, I, L, I, I, F, P, P, P, P, P, L, P],
+    "bm_bn_act_gain_skip_bwd_det_workspace": [L, I],
+    "bm_bn_act_gain_skip_bwd_det": [P, P, P, P, P, P, I, L, I, I, F, P, F, P, P, P, P, P, P, P, P, L, P],
     "bm_glu_bwd_det_workspace": [L, I],
     "bm_glu_bwd_det": [P, P, L, I, P, P, P, P, L, P],
     "bm_conv1d_bwd_weight_det_workspace": [I, I, I, I, I],

@@ -216,15 +216,35 @@ class SubjectLayers(nn.Module):
         return f"SubjectLayers({C}, {D}, {S})"
 
 
+class LayerScale(nn.Module):
+    """Learnt per-channel gain on a residual branch, `(boost * scale)[:, None] * x` with `scale` initialised to
+    init / boost (reference: bm/models/common.py:65-76).  Inside a ConvSequence the gain is applied by the layer's
+    CUDA epilogue; `forward` is kept for callers that use the module on its own."""
+
+    def __init__(self, channels: int, init: float = 0.1, boost: float = 5.):
+        super().__init__()
+        self.scale = nn.Parameter(torch.zeros(channels, requires_grad=True))
+        self.scale.data[:] = init / boost
+        self.boost = boost
+
+    def forward(self, x):
+        return (self.boost * self.scale[:, None]) * x
+
+
 class ConvSequence(nn.Module):
     """Dilated Conv1d (+ BatchNorm) + activation stack with residual skips and GLU blocks (reference:
-    bm/models/common.py:79-151).  Submodule names (`sequence.{k}.0/1`, `glus.{k}.0`) and construction order match the
+    bm/models/common.py:79-151).  Submodule names (`sequence.{k}.{i}`, `glus.{k}.0`) and construction order match the
     reference, so `state_dict()` keys and seeded initialisation are interchangeable.
 
     Two users: `SimpleConv` fuses the `clip_conv` family (batch_norm, skip, GELU, GLU) into its own forward/backward;
     a stand-alone sequence (the `DeepMel` feature model) runs through `forward(x)` -> `convseq.conv_sequence`.
     Accelerated: stride 1, odd kernel <= 3, GELU / LeakyReLU / ReLU, with or without BatchNorm, skip,
-    activation_on_last, GLU every `glu` layers with context <= 1.  Everything else raises NotImplementedError."""
+    activation_on_last, GLU every `glu` layers with context <= 1, and the residual-branch options: `rewrite` (a 1x1 conv +
+    LeakyReLU(leakiness) after the activation), `scale` (LayerScale) and `post_skip` (a depthwise 1x1 gain), the last two on
+    layers that keep their width when `skip` is set.  Everything else raises NotImplementedError.
+
+    Per layer k: `has_act[k]`, `has_rewrite[k]`, `has_scale[k]`, `has_post_skip[k]`, and `index[k]`, the position of each
+    submodule in `sequence[k]` ('conv', 'bn', 'rewrite', 'scale', 'post_skip'; absent keys: no such module)."""
 
     def __init__(self, channels: tp.Sequence[int], kernel: int = 4, dilation_growth: int = 1,
                  dilation_period: tp.Optional[int] = None, stride: int = 2, dropout: float = 0.0,
@@ -234,8 +254,7 @@ class ConvSequence(nn.Module):
                  glu_context: int = 0, glu_glu: bool = True, activation: tp.Any = None) -> None:
         super().__init__()
         unsupported = dict(stride=stride != 1, dropout=bool(dropout), groups=groups != 1, decode=decode,
-                           dropout_input=bool(dropout_input), scale=scale is not None, rewrite=rewrite,
-                           post_skip=post_skip, glu_glu=not glu_glu, kernel=kernel % 2 != 1 or kernel > 3,
+                           dropout_input=bool(dropout_input), glu_glu=not glu_glu, kernel=kernel % 2 != 1 or kernel > 3,
                            activation=activation not in (None, nn.GELU, nn.ReLU, nn.LeakyReLU),
                            glu_context=bool(glu) and glu_context > 1)
         bad = [k for k, v in unsupported.items() if v]
@@ -255,21 +274,43 @@ class ConvSequence(nn.Module):
         self.clip_conv_family = bool(batch_norm)
         self.sequence = nn.ModuleList()
         self.glus = nn.ModuleList()
+        # the LeakyReLU after a rewrite conv is LeakyReLU(leakiness) whatever the stack's activation (common.py:124)
+        self.rewrite_slope = float(leakiness)
         self.dilations: tp.List[int] = []
         self.has_act: tp.List[bool] = []
+        self.has_rewrite: tp.List[bool] = []
+        self.has_scale: tp.List[bool] = []
+        self.has_post_skip: tp.List[bool] = []
+        self.index: tp.List[tp.Dict[str, int]] = []
         dilation = 1
         for k, (chin, chout) in enumerate(zip(channels[:-1], channels[1:])):
             if dilation_period and (k % dilation_period) == 0:
                 dilation = 1
             self.dilations.append(dilation)
             layers: tp.List[nn.Module] = [nn.Conv1d(chin, chout, kernel, 1, (kernel // 2) * dilation, dilation=dilation)]
+            index = dict(conv=0)
             dilation *= dilation_growth
             is_last = k == len(channels) - 2
             self.has_act.append(activation_on_last or not is_last)
             if self.has_act[-1]:
                 if batch_norm:
+                    index["bn"] = len(layers)
                     layers.append(nn.BatchNorm1d(num_features=chout))
                 layers.append(make_act())
+                if rewrite:
+                    index["rewrite"] = len(layers)
+                    layers += [nn.Conv1d(chout, chout, 1), nn.LeakyReLU(leakiness)]
+            self.has_rewrite.append(self.has_act[-1] and rewrite)
+            gains = chin == chout and skip
+            if gains and scale is not None:
+                index["scale"] = len(layers)
+                layers.append(LayerScale(chout, scale))
+            if gains and post_skip:
+                index["post_skip"] = len(layers)
+                layers.append(nn.Conv1d(chout, chout, 1, groups=chout, bias=False))
+            self.has_scale.append(gains and scale is not None)
+            self.has_post_skip.append(gains and post_skip)
+            self.index.append(index)
             self.sequence.append(nn.Sequential(*layers))
             if glu and (k + 1) % glu == 0:
                 self.glus.append(nn.Sequential(
@@ -279,6 +320,22 @@ class ConvSequence(nn.Module):
 
     def glu_after(self) -> tp.List[bool]:
         return [g is not None for g in self.glus]
+
+    def residual(self) -> tp.Optional[tp.List[tp.Tuple[bool, bool, bool]]]:
+        """Per layer (rewrite, scale, post_skip) for `functional.SequencePlan.residual`; None when no layer has one."""
+        flags = list(zip(self.has_rewrite, self.has_scale, self.has_post_skip))
+        return flags if any(any(f) for f in flags) else None
+
+    def scale_boost(self) -> float:
+        return next((m.boost for m in self.modules() if isinstance(m, LayerScale)), 5.0)
+
+    def residual_params(self, k: int) -> tp.List[tp.Optional[torch.Tensor]]:
+        """[rewrite_w, rewrite_b, layer_scale, post_skip_w] of layer k, None where absent."""
+        block, at = self.sequence[k], self.index[k]
+        rw = block[at["rewrite"]] if "rewrite" in at else None
+        return [None if rw is None else rw.weight, None if rw is None else rw.bias,
+                block[at["scale"]].scale if "scale" in at else None,
+                block[at["post_skip"]].weight if "post_skip" in at else None]
 
     def forward(self, x):
         from . import convseq

@@ -6,6 +6,8 @@ weight gradients, FP32-FMA kernels for shapes outside the tensor-core tiling) --
 x [B, C0, T] (channel-major, like every tensor the reference hands to a model) is transposed once to channels-last, the
 first layer's input channels zero-padded to the tensor-core granularity; every layer is
     y = conv_k(x);  x = act(bn(y)) [if the layer has an activation]  (+ x_prev if skip and the shapes agree);  GLU block
+with, where the module has them, a rewrite conv (1x1 + LeakyReLU) after the activation and the LayerScale / post_skip gains
+in front of the residual add;
 and the result is transposed back to [B, C_last, T].  The layers run on the conv stack SimpleConv's encoder uses
 (`functional.conv_stack_forward` / `conv_stack_backward`); backward is hand-written (no autograd through the layers).
 There is no CPU path: CUDA tensors only.
@@ -19,18 +21,32 @@ import torch
 from . import _lib
 from ._lib import call, ptr, stream
 from .functional import (SequencePlan, _Conv, _Needs, _empty, _round_up, conv_stack_backward, conv_stack_forward,
-                         tc_status_tensor)
+                         layer_width, tc_status_tensor)
+
+
+def _present(plan: SequencePlan, k: int) -> tp.List[bool]:
+    """Which entries of layer k's parameter tuple (`functional.layer_width`) the call passes: conv_w, conv_b, then gamma,
+    beta with a BatchNorm, then on a layer with a residual-branch option rewrite_w, rewrite_b, layer_scale, post_skip_w."""
+    bn = plan.has_act[k] and plan.batch_norm
+    out = [True, True, bn, bn]
+    if layer_width(plan, k) > 4:
+        rewrite, scale, post = plan.residual[k]
+        out += [rewrite, rewrite, scale, post]
+    return out
 
 
 def _sequence_needs(needs_input_grad, plan: SequencePlan) -> _Needs:
-    """`_Needs` of a ConvSequence call: front = (x,), layer k = (conv_w, conv_b, gamma, beta) (False where absent)."""
+    """`_Needs` of a ConvSequence call: front = (x,), layer k = (conv_w, conv_b, gamma, beta[, rewrite_w, rewrite_b,
+    layer_scale, post_skip_w]) (False where absent)."""
     n = [bool(v) for v in needs_input_grad]
     depth = len(plan.dilations)
     layer, at = [], 2
     for k in range(depth):
-        cnt = 4 if (plan.has_act[k] and plan.batch_norm) else 2
-        layer.append(tuple(n[at:at + cnt]) + (False,) * (4 - cnt))
-        at += cnt
+        flags = []
+        for present in _present(plan, k):
+            flags.append(present and n[at])
+            at += int(present)
+        layer.append(tuple(flags))
     glu = {}
     for k in range(depth):
         if plan.glu_after[k]:
@@ -43,7 +59,8 @@ def _sequence_needs(needs_input_grad, plan: SequencePlan) -> _Needs:
 
 
 class _ConvSequenceFn(torch.autograd.Function):
-    """inputs: plan, x, then per layer (conv_w, conv_b[, gamma, beta]) and, appended in layer order, (glu_w, glu_b).
+    """inputs: plan, x, then per layer (conv_w, conv_b[, gamma, beta][, rewrite_w, rewrite_b][, layer_scale][, post_skip_w])
+    and, appended in layer order, (glu_w, glu_b).
     Only what requires grad is backpropagated, as in `functional._EncoderFn`: frozen parameters get no gradient work, the
     backward stops at the first layer that still needs a data gradient, and the forward saves only what it reads."""
 
@@ -53,11 +70,7 @@ class _ConvSequenceFn(torch.autograd.Function):
         it = iter(params)
         conv_p = []
         for k in range(depth):
-            w, b = next(it), next(it)
-            gamma = beta = None
-            if plan.has_act[k] and plan.batch_norm:
-                gamma, beta = next(it), next(it)
-            conv_p.append((w, b, gamma, beta))
+            conv_p.append(tuple(next(it) if present else None for present in _present(plan, k)))
         glu_p = {k: (next(it), next(it)) for k in range(depth) if plan.glu_after[k]}
         nd = _sequence_needs(ctx.needs_input_grad, plan)
         st = stream()
@@ -113,7 +126,7 @@ class _ConvSequenceFn(torch.autograd.Function):
             dx = dx_full[:, :C0].contiguous() if Cp != C0 else dx_full
         grads: tp.List[tp.Any] = [None, dx]
         for k in range(depth):
-            grads.extend(layer_grads[k] if plan.has_act[k] and plan.batch_norm else layer_grads[k][:2])
+            grads.extend(gk for gk, present in zip(layer_grads[k], _present(plan, k)) if present)
         for k in range(depth):
             if plan.glu_after[k]:
                 grads.extend(glu_grads[k])
@@ -146,6 +159,7 @@ def conv_sequence(module, x: torch.Tensor) -> torch.Tensor:
             bn_buffers.append((bn.running_mean, bn.running_var))
         else:
             bn_buffers.append(None)
+        params += [t for t in module.residual_params(k) if t is not None]
     for glu in module.glus:
         if glu is not None:
             params += [glu[0].weight, glu[0].bias]
@@ -156,7 +170,8 @@ def conv_sequence(module, x: torch.Tensor) -> torch.Tensor:
         batch_norm=module.batch_norm, act_code=module.act_code, act_slope=module.act_slope, skip=module.skip,
         training=module.training, bn_eps=bn0.eps if bn0 is not None else 0.0,
         bn_momentum=bn0.momentum if bn0 is not None else 0.0, bn_buffers=bn_buffers,
-        use_tensor_cores=getattr(module, "use_tensor_cores", True), keep_for_backward=torch.is_grad_enabled())
+        use_tensor_cores=getattr(module, "use_tensor_cores", True), keep_for_backward=torch.is_grad_enabled(),
+        residual=module.residual(), rewrite_slope=module.rewrite_slope, scale_boost=module.scale_boost())
     out = _ConvSequenceFn.apply(plan, x, *params)
     if module.training and module.batch_norm:
         for k, block in enumerate(module.sequence):       # nn.BatchNorm1d bookkeeping (running stats updated on device)

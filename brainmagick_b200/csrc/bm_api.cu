@@ -1127,6 +1127,81 @@ extern "C" int bm_bn_act_skip_bwd_det(const float* g, const float* y, const floa
                            reinterpret_cast<double*>(workspace), ST(stream));
 }
 
+// ---- residual gain (LayerScale / post_skip) on a ConvSequence layer's branch ----------------------------------------------
+extern "C" int bm_bn_act_gain_skip_fwd(const float* y, const float* mean, const float* invstd, const float* gamma,
+                                       const float* beta, const float* x_old, float* x_new, long long rows, int C, int act,
+                                       float slope, const float* scale, float boost, const float* post, bm_stream_t stream) {
+    BM_CHECK_ARG(y && x_new && rows > 0 && C > 0 && act >= 0 && act <= 2);
+    BM_CHECK_ARG(!mean || (invstd && gamma && beta));
+    act_gain_skip_fwd_kernel<<<ew_grid(rows * C), 256, 0, ST(stream)>>>(y, mean, invstd, gamma, beta, x_old, x_new, rows * C,
+                                                                        C, act, slope, scale, boost, post);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
+constexpr int GAIN_ROWS_PER_BLOCK = 128;
+inline long long gain_bwd_ws_floats(long long rows, int C) { return blocks_of(rows, GAIN_ROWS_PER_BLOCK) * 6ll * C; }
+
+// part: NULL (fp64 atomics into sums [3C]) or the gain_bwd_ws_floats(rows, C) partials of the deterministic form
+static int act_gain_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                             const float* beta, int batch_stats, long long rows, int C, int act, float slope,
+                             const float* scale, float boost, const float* post, double* sums, float* dy, float* dgamma,
+                             float* dbeta, float* dscale, float* dpost, double* part, cudaStream_t st) {
+    BM_CHECK_ARG(g && y && dy && rows > 0 && C > 0 && act >= 0 && act <= 2);
+    BM_CHECK_ARG(!mean || (invstd && gamma && beta));
+    const bool bn_reduce = mean && bn_bwd_reduces(batch_stats, dgamma, dbeta);
+    BM_CHECK_ARG(!bn_reduce || (dgamma && dbeta));
+    const bool reduce = bn_reduce || dscale || dpost;
+    BM_CHECK_ARG(!reduce || sums);
+    if (reduce) {
+        dim3 grid((unsigned)blocks_of(rows, GAIN_ROWS_PER_BLOCK), (C + 127) / 128);
+        if (part) {
+            act_gain_bwd_reduce_kernel<true><<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, part, rows, C,
+                                                                   GAIN_ROWS_PER_BLOCK, act, slope, scale, boost, post);
+            BM_CHECK_LAUNCH();
+            if (int rc = reduce_rows(part, (long long)grid.x, 3 * C, sums, st)) return rc;
+        } else {
+            BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 3 * C, st));
+            act_gain_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C,
+                                                             GAIN_ROWS_PER_BLOCK, act, slope, scale, boost, post);
+            BM_CHECK_LAUNCH();
+        }
+        act_gain_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, C, scale, boost, post, bn_reduce ? dgamma : nullptr,
+                                                                    bn_reduce ? dbeta : nullptr, dscale, dpost);
+        BM_CHECK_LAUNCH();
+    }
+    act_gain_bwd_apply_kernel<<<ew_grid(rows * C), 256, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, (double)rows,
+                                                                 bn_reduce && batch_stats, dy, rows * C, C, act, slope, scale,
+                                                                 boost, post);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
+extern "C" int bm_bn_act_gain_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd,
+                                       const float* gamma, const float* beta, int batch_stats, long long rows, int C, int act,
+                                       float slope, const float* scale, float boost, const float* post, double* sums,
+                                       float* dy, float* dgamma, float* dbeta, float* dscale, float* dpost,
+                                       bm_stream_t stream) {
+    return act_gain_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, scale, boost, post, sums, dy,
+                             dgamma, dbeta, dscale, dpost, nullptr, ST(stream));
+}
+extern "C" long long bm_bn_act_gain_skip_bwd_det_workspace(long long rows, int C) {
+    return rows > 0 && C > 0 ? gain_bwd_ws_floats(rows, C) : 0;
+}
+extern "C" int bm_bn_act_gain_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd,
+                                           const float* gamma, const float* beta, int batch_stats, long long rows, int C,
+                                           int act, float slope, const float* scale, float boost, const float* post,
+                                           double* sums, float* dy, float* dgamma, float* dbeta, float* dscale, float* dpost,
+                                           float* workspace, long long workspace_floats, bm_stream_t stream) {
+    BM_CHECK_ARG(rows > 0 && C > 0);
+    if (!(mean && bn_bwd_reduces(batch_stats, dgamma, dbeta)) && !dscale && !dpost)   // nothing is reduced
+        return act_gain_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, scale, boost, post, sums,
+                                 dy, dgamma, dbeta, dscale, dpost, nullptr, ST(stream));
+    BM_CHECK_WS(gain_bwd_ws_floats(rows, C));
+    return act_gain_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, scale, boost, post, sums, dy,
+                             dgamma, dbeta, dscale, dpost, reinterpret_cast<double*>(workspace), ST(stream));
+}
+
 static int clip_loss_bwd_cand(int passes, const float* probs, const float* scores, const float* inv_norm, const float* est,
                               const float* cand, const float* gout, int Bn, int Bc, long long KT, int target_offset, float* G,
                               float* coef, float* dcand, int* status, bm_stream_t stream) {

@@ -94,6 +94,113 @@ __global__ void bn_act_bwd_apply_kernel(const float* __restrict__ g, const float
     }
 }
 
+// ---- Residual gain: LayerScale and post_skip (common.py:65-76,126-130) ------------------------------------------------
+// branch = act(bn(y)) (act(y) without BatchNorm), x_new = post[c] * ((boost * scale[c]) * branch) (+ x_old), in the
+// reference's operation order; a NULL gain is 1.
+__device__ __forceinline__ float gain_f(const float* __restrict__ scale, float boost, const float* __restrict__ post, int c,
+                                        float v) {
+    if (scale) v = (boost * scale[c]) * v;
+    if (post) v = post[c] * v;
+    return v;
+}
+
+__global__ void act_gain_skip_fwd_kernel(const float* __restrict__ y, const float* __restrict__ mean,
+                                         const float* __restrict__ invstd, const float* __restrict__ gamma,
+                                         const float* __restrict__ beta, const float* __restrict__ x_old,
+                                         float* __restrict__ x_new, long long total, int C, int act, float slope,
+                                         const float* __restrict__ scale, float boost, const float* __restrict__ post) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(i % C);
+        float z = y[i];
+        if (mean) z = (z - mean[c]) * invstd[c] * gamma[c] + beta[c];
+        const float a = gain_f(scale, boost, post, c, act_f(act, z, slope));
+        x_new[i] = x_old ? a + x_old[i] : a;
+    }
+}
+
+// backward pass 1: per column, fp64 per thread, sums[c] += sum dz, sums[C+c] += sum dz*yhat (BatchNorm only; dz = gain(g) *
+// act'(z)) and sums[2C+c] += sum g*branch (the gains' common reduction; branch recomputed from y).
+// DET: sums is a [gridDim.x][3C] partials buffer, the block stores its row
+template <bool DET = false>
+__global__ void act_gain_bwd_reduce_kernel(const float* __restrict__ g, const float* __restrict__ y,
+                                           const float* __restrict__ mean, const float* __restrict__ invstd,
+                                           const float* __restrict__ gamma, const float* __restrict__ beta,
+                                           double* __restrict__ sums, long long rows, int C, int rows_per_block, int act,
+                                           float slope, const float* __restrict__ scale, float boost,
+                                           const float* __restrict__ post) {
+    const int c = blockIdx.y * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    const long long r0 = (long long)blockIdx.x * rows_per_block;
+    const long long r1 = min(rows, r0 + rows_per_block);
+    float mu = 0.f, is = 1.f, ga = 1.f, be = 0.f;
+    if (mean) { mu = mean[c]; is = invstd[c]; ga = gamma[c]; be = beta[c]; }
+    double s1 = 0.0, s2 = 0.0, s3 = 0.0;
+#pragma unroll 4
+    for (long long r = r0; r < r1; ++r) {
+        const float gv = g[r * C + c], yv = y[r * C + c];
+        const float yh = mean ? (yv - mu) * is : yv;
+        const float z = mean ? yh * ga + be : yv;
+        s3 = fma((double)gv, (double)act_f(act, z, slope), s3);
+        if (mean) {
+            const double dz = gain_f(scale, boost, post, c, gv) * act_grad_f(act, z, slope);
+            s1 += dz;
+            s2 = fma(dz, (double)yh, s2);
+        }
+    }
+    if (DET) {
+        double* row = sums + (long long)blockIdx.x * 3 * C;
+        row[c] = s1;
+        row[C + c] = s2;
+        row[2 * C + c] = s3;
+        return;
+    }
+    if (mean) {
+        atomicAdd(sums + c, s1);
+        atomicAdd(sums + C + c, s2);
+    }
+    atomicAdd(sums + 2 * C + c, s3);
+}
+
+// dbeta = sums[c], dgamma = sums[C+c]; with S = sums[2C+c] = sum g*branch: dscale = boost*post*S, dpost = (boost*scale)*S.
+// Every output is nullable.
+__global__ void act_gain_param_grad_kernel(const double* __restrict__ sums, int C, const float* __restrict__ scale, float boost,
+                                           const float* __restrict__ post, float* __restrict__ dgamma,
+                                           float* __restrict__ dbeta, float* __restrict__ dscale, float* __restrict__ dpost) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    if (dbeta) dbeta[c] = (float)sums[c];
+    if (dgamma) dgamma[c] = (float)sums[C + c];
+    const double S = sums[2 * C + c];
+    if (dscale) dscale[c] = (float)((double)boost * (post ? (double)post[c] : 1.0) * S);
+    if (dpost) dpost[c] = (float)((scale ? (double)(boost * scale[c]) : 1.0) * S);
+}
+
+// backward pass 2 with gb = gain(g): dy = gamma*invstd*(dz - mean(dz) - yhat*mean(dz*yhat)), dz = gb*act'(z) (training
+// BatchNorm); dy = gamma*invstd*dz (eval: use_batch_stats = 0); dy = gb*act'(y) (no BatchNorm: mean == NULL)
+__global__ void act_gain_bwd_apply_kernel(const float* __restrict__ g, const float* __restrict__ y,
+                                          const float* __restrict__ mean, const float* __restrict__ invstd,
+                                          const float* __restrict__ gamma, const float* __restrict__ beta,
+                                          const double* __restrict__ sums, double n, int use_batch_stats,
+                                          float* __restrict__ dy, long long total, int C, int act, float slope,
+                                          const float* __restrict__ scale, float boost, const float* __restrict__ post) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)(i % C);
+        const float gb = gain_f(scale, boost, post, c, g[i]);
+        if (!mean) {
+            dy[i] = gb * act_grad_f(act, y[i], slope);
+            continue;
+        }
+        const float is = invstd[c], ga = gamma[c];
+        const float yh = (y[i] - mean[c]) * is;
+        const float dz = gb * act_grad_f(act, yh * ga + beta[c], slope);
+        float v = dz;
+        if (use_batch_stats) v = dz - (float)(sums[c] / n) - yh * (float)(sums[C + c] / n);
+        dy[i] = ga * is * v;
+    }
+}
+
 // ---- ClipLoss, gradient w.r.t. the candidates -----------------------------------------------------------------
 // scores[b][o] = inv_o <e_b, c_o>, inv_o = 1/(1e-8 + ||c_o||)   (losses.py:91-94).  With G = dL/d<e_b, c_o> (the matrix
 // clip_ce_bwd_kernel builds), dL/dc_o = sum_b G[b][o] e_b  -  coef_o c_o,

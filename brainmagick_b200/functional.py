@@ -29,7 +29,11 @@ ACT_GELU, ACT_LRELU, ACT_NONE = 0, 1, 2      # activation codes of the epilogue 
 class SequencePlan:
     """The layers of a ConvSequence (bm/models/common.py:79-151) as `conv_stack_forward` / `conv_stack_backward` run them:
     layer k is conv (+ BatchNorm if `batch_norm` and has_act[k]) (+ activation if has_act[k]) (+ the layer input if `skip`
-    and the conv keeps the width), then a GLU block if glu_after[k]."""
+    and the conv keeps the width), then a GLU block if glu_after[k].
+
+    `residual[k]` = (rewrite, scale, post_skip) of layer k (None: no layer has one): a 1x1 conv + LeakyReLU(rewrite_slope)
+    after the activation, then the LayerScale gain (its factor `scale_boost`) and the depthwise post_skip gain, in front of
+    the residual add (common.py:123-130).  A layer with any of them takes `layer_width(plan, k)` = 8 parameters."""
     dilations: tp.List[int]
     glu_after: tp.List[bool]
     has_act: tp.List[bool]            # layer k ends with (BatchNorm +) activation (activation_on_last, common.py:112)
@@ -43,6 +47,15 @@ class SequencePlan:
     bn_buffers: tp.List[tp.Optional[tp.Tuple[torch.Tensor, torch.Tensor]]]   # (running_mean, running_var) per layer
     use_tensor_cores: bool
     keep_for_backward: bool
+    residual: tp.Optional[tp.List[tp.Tuple[bool, bool, bool]]] = dataclasses.field(default=None, kw_only=True)
+    rewrite_slope: float = dataclasses.field(default=0.0, kw_only=True)
+    scale_boost: float = dataclasses.field(default=5.0, kw_only=True)
+
+
+def layer_width(plan: SequencePlan, k: int) -> int:
+    """Entries of layer k's parameter tuple: (conv_w, conv_b, gamma, beta), then on a layer with a residual-branch option
+    (rewrite_w, rewrite_b, layer_scale, post_skip_w); None where a parameter is absent."""
+    return 8 if plan.residual is not None and any(plan.residual[k]) else 4
 
 
 @dataclasses.dataclass
@@ -359,6 +372,98 @@ class _Conv:
 # The ConvSequence layers (bm/models/common.py:142-151) on channels-last activations: SimpleConv's encoder and the
 # stand-alone ConvSequence / DeepMel both run them through these two functions.
 # ----------------------------------------------------------------------------------------------------
+def _residual_branch_forward(plan: SequencePlan, k, p, x, y, mean, invstd, skip, act, save, nd: "_Needs", B, T, status,
+                             bare_slope):
+    """Epilogue of layer k with its residual-branch options (common.py:117-130): a = act(bn(y)); with `rewrite`
+    r = LeakyReLU(conv1x1(a)) (else r = a); x_new = post * ((boost * scale) * r) (+ x).  The gains and the residual add run
+    in `bm_bn_act_gain_skip_fwd` (without a gain, the rewrite's LeakyReLU and the add in `bm_bn_act_skip_fwd`).
+    -> (x_new, the record entries `_residual_branch_backward` reads)"""
+    st = stream()
+    rows, cout = B * T, y.shape[2]
+    _, _, gamma, beta, rw, rb, ls, ps = p
+    if mean is not None:
+        gamma, beta = gamma.contiguous(), beta.contiguous()
+    ls = None if ls is None else ls.contiguous()
+    ps = None if ps is None else ps.contiguous()            # [C, 1, 1]: one weight per channel
+    gain = ls is not None or ps is not None
+    slope = float(plan.act_slope if plan.has_act[k] else bare_slope)
+    x_old = x if skip else None
+    x_new = _empty((B, T, cout), x)
+    rec = dict(gain=gain, ls=ls, ps=ps, rconv=None, a=None, y2=None)
+    src = y
+    if rw is not None:
+        a = _empty((B, T, cout), x)
+        if mean is not None and act == ACT_GELU:
+            call("bm_bn_gelu_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), None, ptr(a), rows, cout, None,
+                 st)
+        else:
+            call("bm_bn_act_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), None, ptr(a), rows, cout, act,
+                 slope, st)
+        need_dy = nd.below[k] or any(nd.layer[k][:4])
+        rconv = _Conv(rw, T, False, plan.use_tensor_cores, want_bwd=save and need_dy)
+        y2 = _empty((B, T, cout), x)
+        rconv.forward(a, rb.contiguous(), B, T, 1, y2, None, status)
+        rec.update(rconv=rconv, a=a if nd.layer[k][4] else None, y2=y2 if nd.layer_up(k) else None)
+        src, mean, invstd, gamma, beta, act, slope = y2, None, None, None, None, ACT_LRELU, plan.rewrite_slope
+    if gain:
+        call("bm_bn_act_gain_skip_fwd", ptr(src), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), ptr(x_old), ptr(x_new),
+             rows, cout, act, float(slope), ptr(ls), float(plan.scale_boost), ptr(ps), st)
+    else:
+        call("bm_bn_act_skip_fwd", ptr(src), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), ptr(x_old), ptr(x_new), rows,
+             cout, act, float(slope), st)
+    return x_new, rec
+
+
+def _residual_branch_backward(plan: SequencePlan, k, p, rec, g, nd: "_Needs", B, T, status, sums3, weight_grad):
+    """Backward of `_residual_branch_forward` given g = dL/dx_new -> (dy, g_act, (d rewrite_w, d rewrite_b, d scale,
+    d post_skip_w), dgamma, dbeta).  Without a rewrite conv the gain kernel also runs the BatchNorm / activation backward:
+    dy = dL/dy and g_act None.  With one, dy is None and g_act = dL/da, the gradient the caller hands to the BatchNorm /
+    activation backward.  Frozen gains are not reduced, a frozen rewrite conv gets no weight gradient, and nothing below
+    the options is computed when no layer parameter or earlier stage needs it (dy and g_act None)."""
+    st = stream()
+    rows = B * T
+    like = status
+    cout = rec["conv"].cout
+    _, _, gamma, beta, rw, rb, _, _ = p
+    n_rw, n_rb, n_ls, n_ps = nd.layer[k][4:8]
+    _, _, n_gamma, n_beta = nd.layer[k][:4]
+    need_dy = nd.below[k] or any(nd.layer[k][:4])
+    ls, ps = rec["ls"], rec["ps"]
+    if rw is not None:
+        src, mean, invstd, gm, bt = rec["y2"], None, None, None, None
+        act, slope = ACT_LRELU, plan.rewrite_slope
+        want_dsrc = need_dy or n_rw or n_rb
+    else:
+        src, mean, invstd = rec["y"], rec["mean"], rec["invstd"]
+        gm, bt = (gamma.contiguous(), beta.contiguous()) if mean is not None else (None, None)
+        act, slope = rec["act"], (plan.act_slope if plan.has_act[k] else 0.0)
+        want_dsrc = need_dy
+    dsrc = dgamma = dbeta = dls = dps = None
+    if rec["gain"] and (want_dsrc or n_ls or n_ps):
+        bn_reduce = mean is not None and (plan.training or n_gamma or n_beta)
+        if bn_reduce:
+            dgamma, dbeta = _empty((cout,), like), _empty((cout,), like)
+        dls = _empty((cout,), like) if n_ls else None
+        dps = _empty((cout, 1, 1), like) if n_ps else None
+        dsrc = _empty((B, T, cout), like)
+        reduce = bool(bn_reduce or n_ls or n_ps)
+        _reducing_call("bm_bn_act_gain_skip_bwd", like, (rows, cout), ptr(g), ptr(src), ptr(mean), ptr(invstd), ptr(gm),
+                       ptr(bt), 1 if plan.training else 0, rows, cout, act, float(slope), ptr(ls), float(plan.scale_boost),
+                       ptr(ps), ptr(sums3 if reduce else None), ptr(dsrc), ptr(dgamma), ptr(dbeta), ptr(dls), ptr(dps), st,
+                       reduces=reduce)
+    elif not rec["gain"] and want_dsrc:                     # a rewrite without gain: the LeakyReLU backward alone
+        dsrc = _empty((B, T, cout), like)
+        call("bm_bn_act_skip_bwd", ptr(g), ptr(src), None, None, None, None, 0, rows, cout, ACT_LRELU, float(slope), None,
+             ptr(dsrc), None, None, st)
+    if rw is None:
+        return (dsrc if need_dy else None), None, (None, None, dls, dps), dgamma, dbeta
+    drw, drb = weight_grad(rec["rconv"], dsrc, rec["a"], 1, False, want=(n_rw, n_rb))
+    g_act = None
+    if need_dy:
+        g_act = _empty((B, T, cout), like)
+        rec["rconv"].backward_data(dsrc, None, B, T, 1, g_act, status)
+    return None, g_act, (drw, drb, dls, dps), None, None
+
 def conv_stack_forward(plan: SequencePlan, x, conv0: _Conv, conv_p, glu_p, nd: "_Needs", save: bool, B, T, status,
                        bare_slope: float):
     """x [B,T,C] -> (output [B,T,C_last], per-layer records for `conv_stack_backward`, None where the backward does not
@@ -370,7 +475,8 @@ def conv_stack_forward(plan: SequencePlan, x, conv0: _Conv, conv_p, glu_p, nd: "
     tc = plan.use_tensor_cores
     stats = _empty((2 * max(p[0].shape[0] for p in conv_p),), x, torch.float64)
     layers = []
-    for k, (w, b, gamma, beta) in enumerate(conv_p):
+    for k, p in enumerate(conv_p):
+        w, b, gamma, beta = p[:4]
         conv = conv0 if k == 0 else _Conv(w, T, False, tc, want_bwd=save and nd.below[k])
         cout = conv.cout
         y = _empty((B, T, cout), x)
@@ -392,7 +498,14 @@ def conv_stack_forward(plan: SequencePlan, x, conv0: _Conv, conv_p, glu_p, nd: "
             conv.forward(x, b.contiguous(), B, T, plan.dilations[k], y, None, status)
         skip = plan.skip and conv.cin_true == cout
         x_new = y                                   # a bare convolution
-        if has_bn or act != ACT_NONE or skip:
+        if len(p) > 4:
+            x_new, extra = _residual_branch_forward(plan, k, p, x, y, mean, invstd, skip, act, save, nd, B, T, status,
+                                                    bare_slope)
+            rec = dict(x_in=x if nd.layer[k][0] else None,
+                       y=y if (plan.has_act[k] or extra["gain"]) and nd.layer_up(k) else None, mean=mean, invstd=invstd,
+                       conv=conv, skip=skip, act=act, has_bn=has_bn, x_new=x_new if nd.glu.get(k, (False,))[0] else None,
+                       **extra)
+        elif has_bn or act != ACT_NONE or skip:
             x_new = _empty((B, T, cout), x)
             gamma, beta = (gamma.contiguous(), beta.contiguous()) if has_bn else (None, None)
             if has_bn and act == ACT_GELU:
@@ -401,10 +514,11 @@ def conv_stack_forward(plan: SequencePlan, x, conv0: _Conv, conv_p, glu_p, nd: "
             else:
                 call("bm_bn_act_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), ptr(x) if skip else None,
                      ptr(x_new), rows, cout, act, float(plan.act_slope if plan.has_act[k] else bare_slope), st)
-        # kept: the conv input for its weight gradient, y for the activation backward, x_new for the GLU weight gradient
-        rec = dict(x_in=x if nd.layer[k][0] else None, y=y if plan.has_act[k] and nd.layer_up(k) else None, mean=mean,
-                   invstd=invstd, conv=conv, skip=skip, act=act, has_bn=has_bn,
-                   x_new=x_new if nd.glu.get(k, (False,))[0] else None)
+        if len(p) == 4:
+            # kept: the conv input for its weight gradient, y for the activation backward, x_new for the GLU weight gradient
+            rec = dict(x_in=x if nd.layer[k][0] else None, y=y if plan.has_act[k] and nd.layer_up(k) else None, mean=mean,
+                       invstd=invstd, conv=conv, skip=skip, act=act, has_bn=has_bn,
+                       x_new=x_new if nd.glu.get(k, (False,))[0] else None)
         x = x_new
         if plan.glu_after[k]:
             gw, gb = glu_p[k]
@@ -427,7 +541,8 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
     rows = B * T
     like = status                                   # allocations only read the device off it
     sums = _empty((2 * max(p[0].shape[0] for p in conv_p),), like, torch.float64)
-    layer_grads: tp.List[tp.Any] = [(None, None, None, None)] * len(conv_p)
+    sums3 = _empty((3 * max(p[0].shape[0] for p in conv_p),), like, torch.float64) if plan.residual else None
+    layer_grads: tp.List[tp.Any] = [(None,) * len(p) for p in conv_p]
     glu_grads = {k: (None, None) for k in nd.glu}
 
     def weight_grad(conv: _Conv, dy, x, dilation, bias_zero, known_dbias=None, want=(True, True)):
@@ -441,10 +556,10 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
         if not nd.below[k + 1]:
             break                                  # nothing at or below this layer requires grad
         rec = layers[k]
-        _, _, gamma, beta = conv_p[k]
+        _, _, gamma, beta = conv_p[k][:4]
         conv: _Conv = rec["conv"]
         cout = conv.cout
-        n_cw, n_cb, n_gamma, n_beta = nd.layer[k]
+        n_cw, n_cb, n_gamma, n_beta = nd.layer[k][:4]
         if plan.glu_after[k]:
             gconv: _Conv = rec["gconv"]
             n_gw, n_gb = nd.glu[k]
@@ -459,26 +574,35 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
             g = _empty((B, T, gconv.cin), like)
             gconv.backward_data(dh, None, B, T, 1, g, status)
             del dh
-        dgamma = dbeta = None
-        if rec["has_bn"]:
+        dgamma = dbeta = dy = None
+        g_act, opt_grads = g, ()                    # the gradient at the activation's output; the options' gradients
+        if len(conv_p[k]) > 4:
+            dy, g_act, opt_grads, dgamma, dbeta = _residual_branch_backward(plan, k, conv_p[k], rec, g, nd, B, T, status,
+                                                                            sums3, weight_grad)
+            if dy is None and g_act is None:        # nothing below the residual-branch options needs a gradient
+                layer_grads[k] = (None, None, None, None) + opt_grads
+                continue
+        if dy is not None:
+            pass                                    # the gain kernel ran the BatchNorm / activation backward
+        elif rec["has_bn"]:
             # the batch statistics' backward reduces in training mode; in eval mode only for trainable gamma / beta (else
             # the BatchNorm + activation backward is one elementwise pass)
             reduce = plan.training or n_gamma or n_beta
             dy = _empty((B, T, cout), like)
             dgamma, dbeta = (_empty((cout,), like), _empty((cout,), like)) if reduce else (None, None)
             if rec["act"] == ACT_GELU:
-                _reducing_call("bm_bn_gelu_skip_bwd", like, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
+                _reducing_call("bm_bn_gelu_skip_bwd", like, (rows, cout), ptr(g_act), ptr(rec["y"]), ptr(rec["mean"]),
                                ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()),
                                1 if plan.training else 0, rows, cout, ptr(sums if reduce else None), ptr(dy), ptr(dgamma),
                                ptr(dbeta), None, st, reduces=reduce)
             else:
-                _reducing_call("bm_bn_act_skip_bwd", like, (rows, cout), ptr(g), ptr(rec["y"]), ptr(rec["mean"]),
+                _reducing_call("bm_bn_act_skip_bwd", like, (rows, cout), ptr(g_act), ptr(rec["y"]), ptr(rec["mean"]),
                                ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()),
                                1 if plan.training else 0, rows, cout, rec["act"], float(plan.act_slope),
                                ptr(sums if reduce else None), ptr(dy), ptr(dgamma), ptr(dbeta), st, reduces=reduce)
         elif rec["act"] != ACT_NONE:
             dy = _empty((B, T, cout), like)
-            call("bm_bn_act_skip_bwd", ptr(g), ptr(rec["y"]), None, None, None, None, 0, rows, cout, rec["act"],
+            call("bm_bn_act_skip_bwd", ptr(g_act), ptr(rec["y"]), None, None, None, None, 0, rows, cout, rec["act"],
                  float(plan.act_slope), None, ptr(dy), None, None, st)
         else:
             # bare convolution: dL/dy = dL/dx_new.  With a residual, g is accumulated in place below while the weight
@@ -496,8 +620,8 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
             g_in = _empty((B, T, conv.cin), like)
             conv.backward_data(dy, None, B, T, plan.dilations[k], g_in, status)
             g = g_in
-        layer_grads[k] = (dcw, dcb, dgamma if n_gamma else None, dbeta if n_beta else None)
-        del dy
+        layer_grads[k] = (dcw, dcb, dgamma if n_gamma else None, dbeta if n_beta else None) + opt_grads
+        del dy, g_act
     return layer_grads, glu_grads, g
 
 
@@ -972,7 +1096,7 @@ class _Needs:
     requires grad (below[depth]: at the input of the head)."""
     front: tp.Tuple[bool, ...]                 # meg, heads, il_w, il_b, subj_w, sub_emb
     head: tp.Tuple[bool, ...]                  # w0, b0, w2, b2
-    layer: tp.List[tp.Tuple[bool, ...]]        # conv_w, conv_b, gamma, beta
+    layer: tp.List[tp.Tuple[bool, ...]]        # conv_w, conv_b, gamma, beta (+ rewrite_w, rewrite_b, scale, post_skip_w)
     glu: tp.Dict[int, tp.Tuple[bool, ...]]     # glu_w, glu_b of the GLU block after layer k
     below: tp.List[bool]
 
@@ -980,8 +1104,11 @@ class _Needs:
     def of(needs_input_grad, plan: "EncoderPlan") -> "_Needs":
         n = [bool(v) for v in needs_input_grad]
         depth = len(plan.dilations)
-        layer = [tuple(n[10 + 4 * k:14 + 4 * k]) for k in range(depth)]
-        glu, at = {}, 10 + 4 * depth
+        layer, at = [], 10
+        for k in range(depth):
+            layer.append(tuple(n[at:at + layer_width(plan, k)]))
+            at += layer_width(plan, k)
+        glu = {}
         for k in range(depth):
             if plan.glu_after[k]:
                 glu[k] = tuple(n[at:at + 2])
@@ -999,7 +1126,8 @@ class _Needs:
 
 class _EncoderFn(torch.autograd.Function):
     """inputs: plan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, then per layer k: (conv_w, conv_b, gamma, beta)
-    and, appended in layer order, (glu_w, glu_b) for every layer followed by a GLU block.
+    (+ (rewrite_w, rewrite_b, layer_scale, post_skip_w) on a layer with a residual-branch option, see `layer_width`) and,
+    appended in layer order, (glu_w, glu_b) for every layer followed by a GLU block.
 
     Only what requires grad is backpropagated: a frozen parameter's gradient is not computed, the backward stops at the
     deepest stage that still needs a data gradient, and the forward saves only what those gradients read (nothing when no
@@ -1011,8 +1139,11 @@ class _EncoderFn(torch.autograd.Function):
         sub_emb = None
         if plan.has_sub_emb:                     # [B, E] rows of the (scaled) subject embedding, appended by the caller
             sub_emb, layer_params = layer_params[-1], layer_params[:-1]
-        conv_p = [layer_params[4 * k:4 * k + 4] for k in range(depth)]
-        glu_flat = layer_params[4 * depth:]
+        conv_p, at = [], 0
+        for k in range(depth):
+            conv_p.append(layer_params[at:at + layer_width(plan, k)])
+            at += layer_width(plan, k)
+        glu_flat = layer_params[at:]
         glu_p, gi = {}, 0
         for k in range(depth):
             if plan.glu_after[k]:

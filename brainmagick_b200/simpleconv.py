@@ -179,6 +179,8 @@ class SimpleConv(nn.Module):
                 out += [conv.weight, conv.bias, block[1].weight, block[1].bias]
             else:
                 out += [conv.weight, conv.bias, None, None]          # the bare last layer of complex_out=False
+            if any((seq.has_rewrite[k], seq.has_scale[k], seq.has_post_skip[k])):
+                out += seq.residual_params(k)                        # rewrite_w, rewrite_b, layer_scale, post_skip_w
         for glu in seq.glus:
             if glu is not None:
                 out += [glu[0].weight, glu[0].bias]
@@ -210,7 +212,8 @@ class SimpleConv(nn.Module):
             ban_radius=0.0 if self.merger is None else float(self.merger.dropout),
             bn_buffers=bn_buffers, keep_for_backward=torch.is_grad_enabled(),
             use_tensor_cores=self.use_tensor_cores, skip=seq.skip, act_code=seq.act_code, act_slope=seq.act_slope,
-            has_act=list(seq.has_act), batch_norm=True, has_sub_emb=self.subject_embedding is not None)
+            has_act=list(seq.has_act), batch_norm=True, has_sub_emb=self.subject_embedding is not None,
+            residual=seq.residual(), rewrite_slope=seq.rewrite_slope, scale_boost=seq.scale_boost())
 
     def forward(self, inputs, batch):
         meg = inputs["meg"]

@@ -202,6 +202,20 @@ int bm_bn_act_skip_fwd(const float* y, const float* mean, const float* invstd, c
 int bm_bn_act_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
                        const float* beta, int batch_stats, long long rows, int C, int act, float slope, double* sums,
                        float* dy, float* dgamma, float* dbeta, bm_stream_t stream);
+/* Residual gain of a ConvSequence layer (LayerScale and post_skip, common.py:65-76,126-130):
+ * x_new = post[c] * ((boost * scale[c]) * branch) (+ x_old), branch = act(bn(y)) as in bm_bn_act_skip_fwd; scale [C]
+ * (LayerScale's parameter, boost its factor 5) and post [C] (the depthwise 1x1 conv's weight) are each nullable (gain 1).
+ * bm_bn_act_gain_skip_bwd: dy = d/dy of the branch given gain(g), g = dL/dx_new, with the BatchNorm cases of
+ * bm_bn_act_skip_bwd, and in the same reduction pass S[c] = sum_rows g*branch (branch recomputed from y, fp64 per thread):
+ * dscale = boost*post*S, dpost = (boost*scale)*S, each nullable (frozen: not reduced).  sums: fp64 scratch [3C], needed
+ * when anything is reduced (a BatchNorm in training mode, dgamma / dbeta, dscale or dpost). */
+int bm_bn_act_gain_skip_fwd(const float* y, const float* mean, const float* invstd, const float* gamma, const float* beta,
+                            const float* x_old, float* x_new, long long rows, int C, int act, float slope,
+                            const float* scale, float boost, const float* post, bm_stream_t stream);
+int bm_bn_act_gain_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                            const float* beta, int batch_stats, long long rows, int C, int act, float slope,
+                            const float* scale, float boost, const float* post, double* sums, float* dy, float* dgamma,
+                            float* dbeta, float* dscale, float* dpost, bm_stream_t stream);
 /* Gradient of ClipLoss.forward w.r.t. the CANDIDATES (a trainable feature model, solver.py:304-320): with G as in
  * bm_clip_loss_bwd, dcand[o] = sum_b G[b,o] est[b] - coef[o] cand[o], coef[o] = (sum_b G[b,o] scores[b,o]) / ||cand_o||
  * (the derivative of the 1/(1e-8+||.||) normalisation, losses.py:91).  G [Bn,Bc], coef [Bc]: scratch. */
@@ -390,6 +404,13 @@ int bm_bn_act_skip_bwd_det(const float* g, const float* y, const float* mean, co
                            const float* beta, int batch_stats, long long rows, int C, int act, float slope, double* sums,
                            float* dy, float* dgamma, float* dbeta, float* workspace, long long workspace_floats,
                            bm_stream_t stream);
+/* workspace unused (may be NULL) when nothing is reduced (see bm_bn_act_gain_skip_bwd) */
+long long bm_bn_act_gain_skip_bwd_det_workspace(long long rows, int C);
+int bm_bn_act_gain_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                                const float* beta, int batch_stats, long long rows, int C, int act, float slope,
+                                const float* scale, float boost, const float* post, double* sums, float* dy, float* dgamma,
+                                float* dbeta, float* dscale, float* dpost, float* workspace, long long workspace_floats,
+                                bm_stream_t stream);
 long long bm_glu_bwd_det_workspace(long long rows, int H);
 int bm_glu_bwd_det(const float* g, const float* h, long long rows, int H, float* dh, float* dbias, float* amax_out,
                    float* workspace, long long workspace_floats, bm_stream_t stream);
