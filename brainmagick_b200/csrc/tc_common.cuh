@@ -270,7 +270,8 @@ enum HcPhase {
     HP_TILES,          // consumer: tiles (count)
     HP_EMPTY_WAIT,     // producer: waiting on the empty barrier
     HP_B_LOAD,         // producer: B loads issued (or, loaded ahead, needed) until they are in registers
-    HP_STORE,          // producer: TMA issue, B split / stores, fence, arrive
+                       // (hw_wgrad_kernel: the wait for the block's staged dY slot)
+    HP_STORE,          // producer: TMA issue, B split / stores, fence, arrive (hw_wgrad_kernel: + the producer barrier)
     HP_FIRST_FULL,     // producer: CTA start to its first full-barrier arrival
     HP_P_BLOCKS,       // producer: K blocks (count)
     HP_CTAS,           // CTAs (count, by the producer)
@@ -802,18 +803,76 @@ inline int hc_launch_bn(int bn, const Op& op, long long tiles, cudaStream_t st, 
 // the stage layout (A raw | B hi | B lo), the full/empty mbarriers and the consumer block are hc_conv_kernel's:
 //   * producer: thread 0 loads the A tile with TMA as 4 boxes [32 rows p][32 channels] of a 2D map over X (128-byte
 //     swizzle).  Box j holds tile rows 32 j .. 32 j + 31, which are channels of ONE tap (Nx % 32 == 0), and is loaded at
-//     row p0 + shift(tap); rows outside [0, R) arrive as zeros.  All 128 threads load the dY tile [32 p][BN m] as float4
-//     from global memory one K block ahead (rows p >= R and columns m >= Mdy as zeros) and store its tf32 pieces
-//     transposed into the K-major B tiles (HgSlot<false, BN>);
+//     row p0 + shift(tap); rows outside [0, R) arrive as zeros.  Thread 0 also loads block g+1's dY tile [32 p][BN m], as
+//     BN / 32 boxes [32 p][32 m] of a 2D map over dY (128-byte swizzle; rows p >= R and columns m >= Mdy as zeros), into
+//     a raw staging ring of 2 slots, apart from the stages, each slot with its own mbarrier.  All 128 threads then
+//     transpose block g's slot into the K-major B tiles with 128-bit accesses (hw_transpose_dy) and store its tf32
+//     pieces; a named barrier over the producer closes the block, so that every read of a slot precedes the TMA that
+//     refills it;
 //   * consumers read their A fragment transposed out of the boxes, zero the elements whose t + shift leaves [0, T) (sample
 //     edges inside the flattened rows, which TMA cannot see) or whose p >= R, and run hc_consume_block.
 // t = p mod T is carried from block to block (T >= 32: at most one sample edge per block), so the loop divides nothing.
-// Op provides: R, T, X, Nx, err; cta<BN>(), kblocks(c), row0(c) (first flattened row of the CTA's K slice),
-// a_box(c, j) = {first channel, tap shift} of box j (shift >= T for rows past the last tap), b4(c, kb, k, q) = dY
-// elements m = n0 + 4q .. +3 at row k of block kb, and epilogue<BN>(c, acc, m0).
-// Shared memory per K block at BN = 160: A 16 KB written by TMA + 16 KB read, B 40 KB written + 120 KB read by the
-// wgmmas; dY is read from L2 / HBM by the producer (20 KB), not staged.  HC_STAGES = 3 stages of 56 KB (169 KB per CTA):
-// a 4th stage fits in 227 KB but measured no faster.
+// Op provides: R, T, X, Nx, dY, Mdy, err; cta<BN>(), kblocks(c), row0(c) (first flattened row of the CTA's K slice),
+// a_box(c, j) = {first channel, tap shift} of box j (shift >= T for rows past the last tap), b_box(c, kb, j) = {first
+// channel, first row} of dY box j of block kb, and epilogue<BN>(c, acc, m0).
+// Shared memory per K block at BN = 160: A 16 KB written by TMA + 16 KB read; dY 20 KB written by TMA + 20 KB read by the
+// producer; B 40 KB written + 120 KB read by the wgmmas.  HC_STAGES = 3 stages of 56 KB + 2 staging slots of 20 KB
+// (209 KB per CTA at BN = 160, 3xTF32: a 4th stage no longer fits in 227 KB; the producer finishes a block in fewer
+// clocks than the consumers and waits for free stages, so a deeper ring would not feed them faster).
+
+// The producer's dY transpose, one K block: raw slot [BN / 32 boxes][32 p][32 m] (TMA's 128-byte swizzle: element (p, m)
+// of a box at byte 128 p + 16 ((m / 4) ^ (p & 7)) + 4 (m & 3)) -> B tile [BN rows m][32 k = p] (K-major, the same swizzle:
+// byte 128 m + 16 ((p / 4) ^ (m & 7)) + 4 (p & 3)).  The unit is a sub-block of 4 p x 4 m (p quad a, m quad c of a box):
+// 4 LDS.128 of 4 m each, a register transpose, and per m one STS.128 of 4 p into B hi (and one into B lo), so every element
+// keeps the position and the tf32 pieces of the scalar path.  A box has 64 sub-blocks, indexed by 6 bits s0 .. s5, with
+//     c = s0 + 2 s2 + 4 s4,   a = s1 + 2 (s2 ^ s3) + 4 s5,
+// and thread t takes sub-blocks t + 128 j.  A 128-bit access is served per quarter warp (8 lanes), which is conflict-free
+// when its 8 lanes hit 8 distinct 16-byte bank groups: with 128-byte rows, the chunk index inside the row.  The 8 lanes of
+// a quarter warp differ in s0, s1, s2 alone (s3, s4, s5 are lane bits 3, 4 and bit 5 of t):
+//   * LDS of row p = 4 a + i (i = 0 .. 3): chunk c ^ (p & 7) = c ^ 4 s1 ^ i, bits (s0 ^ i0, s2 ^ i1, s4 ^ s1): 8 distinct;
+//   * STS of row m = 4 c + e (e = 0 .. 3): chunk a ^ (m & 7) = a ^ 4 s0 ^ e, bits (s1 ^ e0, s2 ^ s3 ^ e1, s5 ^ s0): 8
+//     distinct.
+// (Plain c = s0 + 2 s1 + 4 s2 would leave the stores 4-way conflicted, since m & 7 sees only c's low bit; s2 feeding both
+// c and a is what spreads both sides.)
+template <int BN, int PASSES>
+struct HwTranspose {
+    static constexpr int NSUB = 2 * BN, NJ = (NSUB + 127) / 128;     // sub-blocks per block, per thread (the last partly)
+    int ro[NJ], bo[NJ];                                                // byte offsets in the raw slot and the B tile
+    __device__ explicit HwTranspose(int t) {
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+            const int idx = t + 128 * j, box = idx >> 6, s = idx & 63;
+            const int c = (s & 1) | ((s >> 1) & 2) | ((s >> 2) & 4);
+            const int a = ((s >> 1) & 1) | (((s >> 1) ^ (s >> 2)) & 2) | ((s >> 3) & 4);
+            ro[j] = box * (32 * 128) + a * 512 + ((c ^ 4 * (a & 1)) << 4);     // row 4 a, chunk c ^ (4 a & 7)
+            bo[j] = (32 * box + 4 * c) * 128 + ((a ^ 4 * (c & 1)) << 4);      // row 4 c, chunk a ^ (4 c & 7)
+        }
+    }
+    __device__ void run(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int t) const {
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+            if (NSUB % 128 != 0 && t + 128 * j >= NSUB) break;          // warp-uniform: the tail covers warps 0-1
+            float v[4][4];                                             // [p][m] of the sub-block
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+                const float4 r = *reinterpret_cast<const float4*>(raw + ((ro[j] + 128 * i) ^ (i << 4)));
+                v[i][0] = r.x; v[i][1] = r.y; v[i][2] = r.z; v[i][3] = r.w;
+            }
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                float4 h, l;
+                tf32_split(v[0][e], h.x, l.x); tf32_split(v[1][e], h.y, l.y);
+                tf32_split(v[2][e], h.z, l.z); tf32_split(v[3][e], h.w, l.w);
+                const int off = (bo[j] + 128 * e) ^ (e << 4);
+                *reinterpret_cast<float4*>(hi + off) = h;
+                if (PASSES == 3) *reinterpret_cast<float4*>(lo + off) = l;
+            }
+        }
+    }
+};
+// a barrier over the producer warpgroup's 128 threads only (id 2: hc_consumer_sync uses 1)
+__device__ __forceinline__ void hw_producer_sync() { asm volatile("bar.sync 2, 128;" ::: "memory"); }
+template <int BN, int PASSES> constexpr int hw_smem_bytes() { return hc_smem_bytes<BN, PASSES>() + 2 * BN * HG_BK * 4; }
 
 // bits a .. b-1 of a 32-bit mask (clamped to [0, 32))
 __device__ __forceinline__ uint32_t hw_bits(int a, int b) {
@@ -824,17 +883,24 @@ __device__ __forceinline__ uint32_t hw_bits(int a, int b) {
 
 template <class Op, int BN, int PASSES>
 __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_constant__ Op op,
-                                                                const __grid_constant__ CUtensorMap xmap) {
+                                                                const __grid_constant__ CUtensorMap xmap,
+                                                                const __grid_constant__ CUtensorMap ymap) {
     static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or single-pass TF32");
     constexpr int NACC = BN / 2, STAGE = hc_stage_bytes<BN, PASSES>(), B_TILE = BN * HG_BK * 4;
     const uint32_t t_start = HcProbe::now();        // the probe's CTA start (BM_HC_PHASES)
-    constexpr int BOX_BYTES = HG_BK * HG_BK * 4;                 // one [32 p][32 channels] box of A
+    constexpr int BOX_BYTES = HG_BK * HG_BK * 4;                 // one [32 p][32 channels] box of A or dY
+    constexpr int RAW = HC_STAGES * STAGE;                       // the dY staging ring: 2 slots of B_TILE bytes
     extern __shared__ uint8_t smem_raw[];
     __shared__ HcBars bars;
+    __shared__ uint64_t dy_bars[2];                              // one per staging slot: thread 0's arrival + the TMA bytes
     const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
     const int tid = threadIdx.x, wg = tid >> 7, lane = tid & 31;
-    if (tid == 0) bars.init();
+    if (tid == 0) {
+        mbar_init(smem_u32(&dy_bars[0]), 1);
+        mbar_init(smem_u32(&dy_bars[1]), 1);
+        bars.init();                                             // (its fence covers the two above)
+    }
     __syncthreads();
 
     const typename Op::Cta cta = op.template cta<BN>();
@@ -843,8 +909,6 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
         // ---- producer
         asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(HC_PRODUCER_REGS));
         HcProbe pr(t_start);
-        constexpr int NB4 = BN / 16;                     // float4 of dY per thread per K block
-        const int k = 8 * (tid >> 5) + (lane & 7), q0 = lane >> 3;    // row k, column quads q0 + 4 j (HgSlot<false>'s lanes)
         int bc[4], bs[4];                                // box j: channel and row shift (0 for a box of padding)
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
@@ -852,14 +916,23 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
             bc[j] = b.x;
             bs[j] = (b.y >= T || b.y <= -T) ? 0 : b.y;
         }
-        float4 v[NB4];
-        auto load = [&](int kb) {
+        const HwTranspose<BN, PASSES> tr(tid);
+        auto stage_dy = [&](int kb) {                    // thread 0: block kb's dY boxes into staging slot kb & 1
+            const uint32_t bar = smem_u32(&dy_bars[kb & 1]), slot = base_u32 + RAW + (kb & 1) * B_TILE;
+            mbar_expect_tx(bar, B_TILE);
 #pragma unroll
-            for (int j = 0; j < NB4; ++j) v[j] = op.b4(cta, kb, k, q0 + 4 * j);
+            for (int j = 0; j < BN / 32; ++j) {
+                const int2 c = op.b_box(cta, kb, j);
+                tma_load_2d(slot + j * BOX_BYTES, &ymap, c.x, c.y, bar);
+            }
+            mbar_arrive(bar);
         };
-        if (nkb > 0) load(0);
+        if (tid == 0 && nkb > 0) stage_dy(0);
         for (int kb = 0; kb < nkb; ++kb) {
             const int s = kb % HC_STAGES, use = kb / HC_STAGES;
+            // the next block's dY, in flight during this block's waits and transpose: its slot was last read by block
+            // kb - 1, which the producer barrier closed
+            if (tid == 0 && kb + 1 < nkb) stage_dy(kb + 1);
             if (use > 0 && !mbar_wait(bars.empty(s), (use - 1) & 1)) {
                 if (op.err) atomicCAS(op.err, 0, HC_ERR_EMPTY);
                 return;
@@ -872,16 +945,17 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
 #pragma unroll
                 for (int j = 0; j < 4; ++j) tma_load_2d(st + j * BOX_BYTES, &xmap, bc[j], p + bs[j], full);
             }
-            uint8_t* bh = smem + s * STAGE + HG_TILE_BYTES;
             pr.mark(HP_STORE);
-#pragma unroll
-            for (int j = 0; j < NB4; ++j) pr.ready(v[j]);
+            if (!mbar_wait(smem_u32(&dy_bars[kb & 1]), (kb >> 1) & 1)) {
+                if (op.err) atomicCAS(op.err, 0, HC_ERR_EMPTY);
+                return;
+            }
             pr.mark(HP_B_LOAD);
-#pragma unroll
-            for (int j = 0; j < NB4; ++j) HgSlot<false, BN>::template store<PASSES>(bh, bh + B_TILE, k, q0 + 4 * j, v[j]);
-            if (kb + 1 < nkb) load(kb + 1);
+            uint8_t* bh = smem + s * STAGE + HG_TILE_BYTES;
+            tr.run(smem + RAW + (kb & 1) * B_TILE, bh, bh + B_TILE, tid);
             fence_proxy_async();                               // the generic-proxy stores, before the wgmmas read them
             mbar_arrive(full);
+            hw_producer_sync();                                // every read of this staging slot, before its next TMA
             pr.mark(HP_STORE);
             pr.first_full();
             pr.count(HP_P_BLOCKS);
@@ -943,15 +1017,17 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
 
 template <int BN, int PASSES, class Op>
 inline int hw_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) {
-    constexpr int SMEM = hc_smem_bytes<BN, PASSES>();
+    constexpr int SMEM = hw_smem_bytes<BN, PASSES>();
     if (int rc = ensure_dyn_smem(reinterpret_cast<const void*>(hw_wgrad_kernel<Op, BN, PASSES>), SMEM)) return rc;
     if (grid.x == 0 || grid.y == 0 || grid.z == 0) return 0;
     if (grid.y > 65535 || grid.z > 65535) return set_error(2, "%s: grid too large%s", who);
-    CUtensorMap xmap;                                   // X [R][Nx], box [32][32]
-    const long long dims[2] = {op.Nx, op.R};
+    CUtensorMap xmap, ymap;                             // X [R][Nx] and dY [R][Mdy], boxes [32][32]
+    const long long xdims[2] = {op.Nx, op.R}, ydims[2] = {op.Mdy, op.R};
     const int box[2] = {HG_BK, HG_BK};
-    if (int rc = hc_x_map(&xmap, op.X, 2, dims, box, who)) return rc;
-    hw_wgrad_kernel<Op, BN, PASSES><<<grid, HC_THREADS, SMEM, st>>>(op, xmap);
+    if (int rc = hc_x_map(&xmap, op.X, 2, xdims, box, who)) return rc;
+    if (op.Mdy % 4 != 0) return set_error(2, "%s: dy rows must be a multiple of 16 bytes%s", who);
+    if (int rc = hc_x_map(&ymap, op.dY, 2, ydims, box, who)) return rc;
+    hw_wgrad_kernel<Op, BN, PASSES><<<grid, HC_THREADS, SMEM, st>>>(op, xmap, ymap);
     ++g_launches;
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", who, cudaGetErrorString(e));

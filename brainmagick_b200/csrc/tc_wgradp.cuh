@@ -8,7 +8,7 @@
 //
 // so the taps share one tile grid (3 x 320 rows = 7.5 tiles of 128 instead of 3 x 3) and the reduction runs over the
 // flattened rows in exact blocks of 32.  One CTA = one (128-row tile, 128- or 160-column tile, K slice) of hw_wgrad_kernel
-// (tc_common.cuh: X by TMA, transposed in registers; dY converted in the kernel); partial tiles go to the workspace and
+// (tc_common.cuh: X and dY by TMA, X transposed in registers, dY in shared memory); partial tiles go to the workspace and
 // `wgradp_reduce_kernel` sums the K slices in a fixed order (deterministic) while scattering into the nn.Conv1d layout
 // [m][n][tap].
 #pragma once
@@ -43,10 +43,10 @@ struct WgradPOp {
         const int tap = r / Nx;
         return make_int2(r - tap * Nx, (tap - taps / 2) * dilation);
     }
-    __device__ float4 b4(const Cta& c, int kb, int k, int q) const {         // dY^T
-        const int m = c.n0 + 4 * q, p = (c.c0 + kb) * HG_BK + k;
-        if (m >= Mdy || p >= R) return make_float4(0.f, 0.f, 0.f, 0.f);
-        return __ldg(reinterpret_cast<const float4*>(dY + (long long)p * Mdy + m));
+    // box j of block kb's dY tile (tile columns 32 j .. 32 j + 31): {first channel m, first row p} in the dY map; channels
+    // m >= Mdy and rows p >= R arrive as zeros
+    __device__ int2 b_box(const Cta& c, int kb, int j) const {
+        return make_int2(c.n0 + 32 * j, (c.c0 + kb) * HG_BK);
     }
     template <int BN> __device__ void epilogue(const Cta& c, const float* acc, int m0) const {
         HgStore s{P + (long long)blockIdx.z * rows_pad * Mdy, Mdy, rows_pad, Mdy};

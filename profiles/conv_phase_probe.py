@@ -15,7 +15,8 @@ shapes of the cfg2 training step (B = 256, T = 360) and the three conv weight gr
 Per shape and pass count it prints, in SM clocks: the consumer warpgroup's full-barrier wait, A split + release + adds and MMA issue-to-drain per K block, and its epilogue per tile in three phases (load: the bias / addend / mask loads until issued; store: the math and the
 stores; stats: BatchNorm statistics and max |output| after the last store; the weight gradient's whole epilogue is
 `store`); the producer's empty-barrier wait,
-B load latency (issue, or the point of use when loaded ahead, to registers) and TMA / store / fence / arrive per K block,
+B load latency (issue, or the point of use when loaded ahead, to registers; the weight gradient: the wait for its staged
+dY slot) and TMA / store / fence / arrive per K block (the weight gradient: dY transpose and producer barrier included),
 and its start-to-first-full per CTA; and the launch's wall time (CUDA events, probe build: the clock reads cost a little).
 
     python profiles/conv_phase_probe.py [--csrc DIR] [--outdir DIR] [--lib PATH] [--out result.json]
