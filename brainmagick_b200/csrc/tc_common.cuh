@@ -518,6 +518,11 @@ inline int hg_launch_bn(int bn, const Op& op, dim3 grid, int passes, cudaStream_
 // piece), the consumers round A in registers with cvt.rna and issue one wgmma per k8; B traffic: 20 KB written + 40 KB read.
 constexpr int HC_THREADS = 384, HC_CONSUMERS = 256, HC_STAGES = 3;
 constexpr int HC_PRODUCER_REGS = 104, HC_CONSUMER_REGS = 200;    // 104 * 128 + 200 * 256 = 168 * 384 registers
+// __launch_bounds__(HC_THREADS, 1) compiles the kernels for 168 registers per thread (65 536 / 384, rounded down to a
+// multiple of 8), so the CTA holds 168 * 384 registers, not 65 536.  setmaxnreg.inc waits until the pool can grant its
+// count: a split above that total would never start the consumers.
+static_assert(HC_PRODUCER_REGS * 128 + HC_CONSUMER_REGS * HC_CONSUMERS <= (65536 / HC_THREADS) / 8 * 8 * HC_THREADS,
+              "the producer / consumer register split must fit in the registers the CTA is launched with");
 constexpr int HC_ERR_FULL = 901, HC_ERR_EMPTY = 902;           // status codes of a timed-out consumer / producer wait
 // one stage: A raw fp32 (128 rows) | B hi | B lo (BN rows each; no lo tile when PASSES = 1), every tile 1 KB-aligned for
 // the 128-byte swizzle

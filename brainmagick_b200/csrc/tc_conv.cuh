@@ -146,7 +146,6 @@ struct ConvOp {
     // shared array shared by the 3- and 1-pass kernels would change the shared-memory layout of both).
     template <int BN, int PASSES> __device__ void epilogue(const Cta& c, const float* acc, int m0, HcProbe& pr) const {
         constexpr int NW = HC_CONSUMERS / 32, NG = BN / 8;    // consumer warps; 8-column groups of the fragment
-        constexpr int GS = NG / 2;                           // column groups per load batch (registers: acc + 60)
         __shared__ __align__(8) float partial[NW][2][BN];
         const int tq = threadIdx.x & 3, t = c.t0 + m0 + hg_row(0);
         const bool r_ok[2] = {t < T, t + 8 < T};
@@ -187,6 +186,41 @@ struct ConvOp {
             }
             pr.mark(HP_EPI_STORE);
         } else {
+            // One copy of the row loop per combination of fused outputs the launchers use, each compiled with only the
+            // code its outputs need, and the general loop for any other combination.  Every copy computes each output
+            // element with the same expression, so the outputs are bitwise those of the general loop.  The general loop
+            // is fully unrolled with every output behind a runtime branch: at BN = 160 the kernel's consumer code was
+            // ~140 KB of SASS, most of it branched over by any one combination, and the specialised copies ran the
+            // epilogues of the step's convs 5-37 % faster (DESIGN §4.2).
+            using F = std::false_type;
+            using Tr = std::true_type;
+            const bool plain = !addend && !aux && !act && !out_tmajor;
+            if (stats && plain) epilogue_rows<BN>(c, acc, m0, partial, pr, am, Tr(), F(), F(), F());
+            else if (stats) epilogue_rows<BN>(c, acc, m0, partial, pr, am, Tr(), Tr(), Tr(), Tr());
+            else if (plain) epilogue_rows<BN>(c, acc, m0, partial, pr, am, F(), F(), F(), F());
+            else if (out_tmajor && !addend && !aux && !act) epilogue_rows<BN>(c, acc, m0, partial, pr, am, F(), F(), F(), Tr());
+            else if ((aux || act) && !addend && !out_tmajor) epilogue_rows<BN>(c, acc, m0, partial, pr, am, F(), F(), Tr(), F());
+            else if (addend && !aux && !act && !out_tmajor) epilogue_rows<BN>(c, acc, m0, partial, pr, am, F(), Tr(), F(), F());
+            else epilogue_rows<BN>(c, acc, m0, partial, pr, am, F(), Tr(), Tr(), Tr());
+        }
+        if (out_amax) {
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, o));
+            if ((threadIdx.x & 31) == 0 && am > 0.f) atomicMax(out_amax, __float_as_uint(am));
+        }
+    }
+    // The non-GLU epilogue of `epilogue`: STATS / ADD / ACT / TMAJ compile in the BatchNorm statistics, the addend, the
+    // pre-activation copy with GELU, and the channel-major store (each still taken only where its pointer or flag is set).
+    template <int BN, class STATS, class ADD, class ACT, class TMAJ>
+    __device__ __forceinline__ void epilogue_rows(const Cta& c, const float* acc, int m0, float (*partial)[2][BN],
+                                                  HcProbe& pr, float& am, STATS, ADD, ACT, TMAJ) const {
+        constexpr int NW = HC_CONSUMERS / 32, NG = BN / 8;    // consumer warps; 8-column groups of the fragment
+        constexpr int GS = NG / 2;                           // column groups per load batch (registers: acc + 60)
+        constexpr bool S_ = STATS::value, A_ = ADD::value, G_ = ACT::value, M_ = TMAJ::value;
+        const int tq = threadIdx.x & 3, t = c.t0 + m0 + hg_row(0);
+        const bool r_ok[2] = {t < T, t + 8 < T};
+        const long long row = (long long)c.b * T + t;          // the thread's rows: row and row + 8
+        {
             const int n0 = c.n_tile * BN + 2 * tq;            // the thread's columns: n0 + 8 g (+1)
             const int warp = hc_consumer_tid() >> 5;
 #pragma unroll
@@ -198,7 +232,7 @@ struct ConvOp {
                     bv[k] = av[k][0] = av[k][1] = make_float2(0.f, 0.f);
                     if (n >= Ntot) continue;
                     if (bias) bv[k] = __ldg(reinterpret_cast<const float2*>(bias + n));
-                    if (addend) {
+                    if (A_ && addend) {
 #pragma unroll
                         for (int h = 0; h < 2; ++h)
                             if (r_ok[h]) av[k][h] = *reinterpret_cast<const float2*>(addend + (row + 8 * h) * Ntot + n);
@@ -216,20 +250,20 @@ struct ConvOp {
                             const long long r = row + 8 * h;
                             float v[2] = {acc[4 * g + 2 * h], acc[4 * g + 2 * h + 1]};
                             if (bias) { v[0] += bv[k].x; v[1] += bv[k].y; }
-                            if (addend) { v[0] += av[k][h].x; v[1] += av[k][h].y; }
-                            if (aux) *reinterpret_cast<float2*>(aux + r * Ntot + n) = make_float2(v[0], v[1]);
-                            if (act) {
+                            if (A_ && addend) { v[0] += av[k][h].x; v[1] += av[k][h].y; }
+                            if (G_ && aux) *reinterpret_cast<float2*>(aux + r * Ntot + n) = make_float2(v[0], v[1]);
+                            if (G_ && act) {
                                 v[0] = gelu_f(v[0]);
                                 v[1] = gelu_f(v[1]);
                                 am = fmaxf(am, fmaxf(fabsf(v[0]), fabsf(v[1])));
                             }
-                            if (out_tmajor) {
+                            if (M_ && out_tmajor) {
                                 y[((long long)c.b * Ntot + n) * T + t + 8 * h] = v[0];
                                 y[((long long)c.b * Ntot + n + 1) * T + t + 8 * h] = v[1];
                             } else {
                                 *reinterpret_cast<float2*>(y + r * Ntot + n) = make_float2(v[0], v[1]);
                             }
-                            if (stats) {
+                            if (S_ && stats) {
                                 // about the bias: exact (Sterbenz) while the bias dominates, and what is left is centred
                                 const float d[2] = {v[0] - bv[k].x, v[1] - bv[k].y};
 #pragma unroll
@@ -240,7 +274,7 @@ struct ConvOp {
                             }
                         }
                     }
-                    if (stats) {
+                    if (S_ && stats) {
 #pragma unroll
                         for (int e = 0; e < 2; ++e) {
 #pragma unroll
@@ -258,7 +292,7 @@ struct ConvOp {
                 }
                 pr.mark(HP_EPI_STORE);
             }
-            if (stats) {
+            if (S_ && stats) {
                 hc_consumer_sync();                      // every warp's partials of this tile are in `partial`
                 const int j = hc_consumer_tid(), n = c.n_tile * BN + j;
                 if (j < BN && n < Ntot) {
@@ -275,11 +309,6 @@ struct ConvOp {
                 }
                 hc_consumer_sync();                      // the reads, before the next tile's partials overwrite them
             }
-        }
-        if (out_amax) {
-#pragma unroll
-            for (int o = 16; o > 0; o >>= 1) am = fmaxf(am, __shfl_xor_sync(0xffffffffu, am, o));
-            if ((threadIdx.x & 31) == 0 && am > 0.f) atomicMax(out_amax, __float_as_uint(am));
         }
     }
 };
