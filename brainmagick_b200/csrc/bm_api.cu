@@ -7,8 +7,6 @@
 #include "tc_conv.cuh"
 #include "tc_wgrad.cuh"
 #include "tc_clip.cuh"
-#include "tc_convp.cuh"
-#include "tc_convh.cuh"
 #include "tc_wgradp.cuh"
 #include "tc_gemm_nt.cuh"
 #include "retrieval.cuh"
@@ -999,7 +997,7 @@ int clip_dest_gemm(Fill fill, const float* cand, int Bn, int Bc, long long KT, f
     if (tc::wgrad_tc_supported(Bn, (int)KT)) {
         // tensor cores: dE[b][k] = sum_o G^T[o][b] C[o][k]  == weight-gradient GEMM with "positions" = candidates
         if (int rc = fill(1)) return rc;
-        return tc::launch_wgrad_tc(G, cand, 1, Bc, Bn, (int)KT, (int)KT, 1, 1, dest, dest, passes, status, st);   // direct mode
+        return tc::launch_wgrad_tc(G, cand, 1, Bc, Bn, (int)KT, (int)KT, 1, 1, dest, dest, passes, st);   // direct mode
     }
     if (int rc = fill(0)) return rc;
     GemmP g = gemm_defaults();
@@ -1025,7 +1023,7 @@ int clip_dcand_gemm(Fill fill, const float* scores, const float* inv_norm, const
         int rc = tc::launch_gemm_nt_pp(G, est, dcand, Bc, (int)KT, Bn, passes, status, st);
         if (rc) return rc;
     } else if (tc::wgrad_tc_supported(Bc, (int)KT)) {
-        int rc = tc::launch_wgrad_tc(G, est, 1, Bn, Bc, (int)KT, (int)KT, 1, 1, dcand, dcand, passes, status, st);   // direct
+        int rc = tc::launch_wgrad_tc(G, est, 1, Bn, Bc, (int)KT, (int)KT, 1, 1, dcand, dcand, passes, st);   // direct
         if (rc) return rc;
     } else {
         GemmP g = gemm_defaults();
@@ -1359,12 +1357,12 @@ static int tc_conv1d(int passes, const float* x, const float* w_hi, const float*
     BM_CHECK_ARG(B <= 65535);
     BM_CHECK_ARG(!(glu && (act || out_tmajor || aux)));
     BM_CHECK_ARG(tc::conv_tc_supported(T, Cin, Ntot, Kw, glu));
-    tc::ConvTcP p;
-    p.B = B; p.T = T; p.Cin = Cin; p.Ntot = Ntot; p.taps = Kw; p.dilation = dilation; p.sign = sign; p.glu = glu;
-    p.bias = bias; p.addend = addend; p.y = y; p.glu_out = glu_out; p.err = status;
-    p.act = act; p.out_tmajor = out_tmajor; p.aux = aux; p.wsel = nullptr; p.n_wsets = 1; p.passes = passes;
-    BM_CHECK_ARG(!(glu && (act || out_tmajor || aux)));
-    return tc::launch_conv_tc(x, w_hi, passes == 1 ? nullptr : w_lo, p, ST(stream));
+    tc::ConvOp o = tc::conv_op_defaults();
+    o.x = x; o.w = w_hi; o.w_lo32 = passes == 1 ? nullptr : w_lo; o.passes = passes;
+    o.B = B; o.T = T; o.Cin = Cin; o.Ntot = Ntot; o.taps = Kw; o.dilation = dilation; o.sign = sign; o.glu = glu;
+    o.bias = bias; o.addend = addend; o.y = y; o.aux = aux; o.glu_out = glu_out; o.act = act; o.out_tmajor = out_tmajor;
+    o.err = status;
+    return tc::launch_conv(o, ST(stream), __func__);
 }
 BM_TC_FORMS(bm_tc_conv1d, tc_conv1d,
             (const float* x, const float* w_hi, const float* w_lo, const float* bias, const float* addend, int B, int T,
@@ -1438,7 +1436,7 @@ static int tc_wgrad(int passes, const float* dy, const float* x, int B, int T, i
                     float* workspace, float* dw, float* dbias, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(dy && x && workspace && dw && B > 0 && T > 0 && Kw >= 1 && Kw <= 3 && dilation >= 1);
     BM_CHECK_ARG(tc::wgrad_tc_supported(M, N) && Ntrue > 0 && Ntrue <= N);
-    return tc::launch_wgrad_tc(dy, x, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, passes, status, ST(stream), dbias);
+    return tc::launch_wgrad_tc(dy, x, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, passes, ST(stream), dbias);
 }
 BM_TC_FORMS(bm_tc_wgrad, tc_wgrad,
             (const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw, int dilation, float* workspace,
@@ -1471,7 +1469,7 @@ extern "C" int bm_tc_wgrad_conv_f16(const float* dy, const float* dy_amax, const
                                     bm_stream_t stream) {
     BM_CHECK_ARG(dy && dy_amax && x && x_amax && workspace && dw && B > 0 && T > 0 && dilation >= 1);
     BM_CHECK_ARG(tc::wgradp_supported(T, M, N, Kw) && Ntrue > 0 && Ntrue <= N);
-    return tc::launch_wgrad_hp(dy, dy_amax, x, x_amax, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, status, ST(stream));
+    return tc::launch_wgrad_pp(dy, x, B, T, M, N, Ntrue, Kw, dilation, workspace, dw, 3, status, ST(stream));
 }
 
 extern "C" int bm_col_sum(const float* x, long long rows, int C, float* out, bm_stream_t stream) {
@@ -1508,21 +1506,23 @@ extern "C" int bm_gelu_bwd(const float* dq, const float* h, long long n, float* 
 }
 
 extern "C" int bm_tc_conv1d_persistent_supported(int T, int Cin, int Ntot, int Kw, int glu) {
-    return tc::conv_pp_supported(T, Cin, Ntot, Kw, glu) ? 1 : 0;
+    return tc::conv_halves_supported(T, Cin, Ntot, Kw, glu) ? 1 : 0;
 }
-// csrc/tc_convp.cuh: w_raw = the RAW fp32 weights re-laid K-major [Kw][Ntot][Cin]
-// (bm_tc_weight_split with f_lo / g_lo = NULL); accumulate=1: y += conv (in place, TMA reduce-add)
+// w_raw = the RAW fp32 weights re-laid K-major [Kw][Ntot][Cin] (bm_tc_weight_split with f_lo / g_lo = NULL);
+// accumulate=1: y += conv (in place)
 static int tc_conv1d_persistent(int passes, const float* x, const float* w_raw, const float* bias, int accumulate, int B,
                                 int T, int Cin, int Ntot, int Kw, int dilation, int sign, int glu, int act, int out_tmajor,
                                 float* y, float* aux, float* glu_out, double* stats, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(x && w_raw && B > 0 && T > 0 && dilation >= 1 && (sign == 1 || sign == -1));
     BM_CHECK_ARG(glu ? (glu_out != nullptr) : (y != nullptr));
-    BM_CHECK_ARG(tc::conv_pp_supported(T, Cin, Ntot, Kw, glu));
-    tc::ConvPPArgs a;
-    a.x = x; a.w_raw = w_raw; a.bias = bias; a.B = B; a.T = T; a.Cin = Cin; a.Ntot = Ntot; a.taps = Kw;
-    a.dilation = dilation; a.sign = sign; a.glu = glu; a.act = act; a.out_tmajor = out_tmajor; a.accumulate = accumulate;
-    a.y = y; a.aux = aux; a.glu_out = glu_out; a.stats = stats; a.err = status; a.passes = passes;
-    return tc::launch_conv_pp(a, ST(stream));
+    BM_CHECK_ARG(tc::conv_halves_supported(T, Cin, Ntot, Kw, glu));
+    if (int rc = tc::conv_halves_epilogue_check(Ntot, glu, act, out_tmajor, accumulate, aux, stats, __func__)) return rc;
+    tc::ConvOp o = tc::conv_op_defaults();
+    o.x = x; o.w = w_raw; o.passes = passes;
+    o.B = B; o.T = T; o.Cin = Cin; o.Ntot = Ntot; o.taps = Kw; o.dilation = dilation; o.sign = sign; o.glu = glu;
+    o.bias = bias; o.addend = accumulate ? y : nullptr; o.y = y; o.aux = act ? aux : nullptr; o.glu_out = glu_out;
+    o.act = act; o.out_tmajor = out_tmajor; o.stats = stats; o.err = status;
+    return tc::launch_conv(o, ST(stream), __func__);
 }
 BM_TC_FORMS(bm_tc_conv1d_persistent, tc_conv1d_persistent,
             (const float* x, const float* w_raw, const float* bias, int accumulate, int B, int T, int Cin, int Ntot, int Kw,
@@ -1531,9 +1531,9 @@ BM_TC_FORMS(bm_tc_conv1d_persistent, tc_conv1d_persistent,
             (x, w_raw, bias, accumulate, B, T, Cin, Ntot, Kw, dilation, sign, glu, act, out_tmajor, y, aux, glu_out, stats,
              status, stream))
 
-// ---- the same conv with fp16-piece weights (csrc/tc_convh.cuh): fp32 weights as two fp16 pieces of a power-of-two-scaled
-// tensor.  bm_amax writes the largest magnitude of a tensor into a device float; bm_f16_split prepares the weights
-// (w_raw [Kw][Ntot][Cin] -> fp16 hi / lo copies of w_raw * scale(amax)); the kernel scales x itself.
+// ---- the same conv with fp16-piece weights: fp32 weights as two fp16 pieces of a power-of-two-scaled tensor.  bm_amax
+// writes the largest magnitude of a tensor into a device float; bm_f16_split prepares the weights (w_raw [Kw][Ntot][Cin] ->
+// fp16 hi / lo copies of w_raw * scale(amax)); the kernel scales x itself.
 extern "C" int bm_amax(const float* x, long long n, float* amax, bm_stream_t stream) {
     BM_CHECK_ARG(x && amax && n > 0);
     return tc::launch_amax(x, n, amax, ST(stream));
@@ -1558,16 +1558,17 @@ extern "C" int bm_tc_conv1d_f16(const float* x, const float* x_amax, const void*
                                 double* stats, float* amax_out, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(x && x_amax && w_hi && w_lo && w_amax && B > 0 && T > 0 && dilation >= 1 && (sign == 1 || sign == -1));
     BM_CHECK_ARG(glu ? (glu_out != nullptr) : (y != nullptr));
-    BM_CHECK_ARG(tc::conv_pp_supported(T, Cin, Ntot, Kw, glu));
-    tc::ConvHPArgs h;
-    tc::ConvPPArgs& a = h.c;
-    a.x = x; a.w_raw = nullptr; a.bias = bias; a.B = B; a.T = T; a.Cin = Cin; a.Ntot = Ntot; a.taps = Kw;
-    a.dilation = dilation; a.sign = sign; a.glu = glu; a.act = act; a.out_tmajor = out_tmajor; a.accumulate = accumulate;
-    a.y = y; a.aux = aux; a.glu_out = glu_out; a.stats = stats; a.err = status; a.passes = 3;
-    h.x_amax = x_amax; h.w_hi = w_hi; h.w_lo = w_lo; h.w_amax = w_amax; h.out_amax = amax_out;
+    BM_CHECK_ARG(tc::conv_halves_supported(T, Cin, Ntot, Kw, glu));
     BM_CHECK_ARG(!amax_out || ((glu || act) && !out_tmajor));      // the outputs another conv consumes: GLU out, GELU out
     if (int rc = amax_begin(amax_out, ST(stream))) return rc;
-    return tc::launch_conv_hp(h, ST(stream));
+    if (int rc = tc::conv_halves_epilogue_check(Ntot, glu, act, out_tmajor, accumulate, aux, stats, __func__)) return rc;
+    tc::ConvOp o = tc::conv_op_defaults();          // passes = 3: the fp16 pieces have no single-pass form
+    o.x = x; o.w_hi = reinterpret_cast<const __half*>(w_hi); o.w_lo = reinterpret_cast<const __half*>(w_lo); o.w_amax = w_amax;
+    o.B = B; o.T = T; o.Cin = Cin; o.Ntot = Ntot; o.taps = Kw; o.dilation = dilation; o.sign = sign; o.glu = glu;
+    o.bias = bias; o.addend = accumulate ? y : nullptr; o.y = y; o.aux = act ? aux : nullptr; o.glu_out = glu_out;
+    o.act = act; o.out_tmajor = out_tmajor; o.stats = stats; o.out_amax = reinterpret_cast<unsigned int*>(amax_out);
+    o.err = status;
+    return tc::launch_conv(o, ST(stream), __func__);
 }
 
 // pointwise (1x1) contraction with a per-sample weight set (SubjectLayers.forward / its data gradient, common.py:55-58):
@@ -1576,11 +1577,11 @@ static int tc_pointwise_sel(int passes, const float* x, const float* w_hi, const
                             int B, int T, int Cin, int Ntot, float* y, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(x && w_hi && (w_lo || passes == 1) && wsel && y && n_sets > 0 && B > 0 && B <= 65535 && T > 0);
     BM_CHECK_ARG(tc::conv_tc_supported(T, Cin, Ntot, 1, 0));
-    tc::ConvTcP p;
-    p.B = B; p.T = T; p.Cin = Cin; p.Ntot = Ntot; p.taps = 1; p.dilation = 1; p.sign = 1; p.glu = 0;
-    p.bias = nullptr; p.addend = nullptr; p.y = y; p.glu_out = nullptr; p.err = status;
-    p.act = 0; p.out_tmajor = 0; p.aux = nullptr; p.wsel = wsel; p.n_wsets = n_sets; p.passes = passes;
-    return tc::launch_conv_tc(x, w_hi, passes == 1 ? nullptr : w_lo, p, ST(stream));
+    tc::ConvOp o = tc::conv_op_defaults();
+    o.x = x; o.w = w_hi; o.w_lo32 = passes == 1 ? nullptr : w_lo; o.passes = passes;
+    o.B = B; o.T = T; o.Cin = Cin; o.Ntot = Ntot; o.taps = 1; o.dilation = 1; o.sign = 1;
+    o.n_wsets = n_sets; o.wsel = wsel; o.y = y; o.err = status;
+    return tc::launch_conv(o, ST(stream), __func__);
 }
 BM_TC_FORMS(bm_tc_pointwise_sel, tc_pointwise_sel,
             (const float* x, const float* w_hi, const float* w_lo, const int* wsel, int n_sets, int B, int T, int Cin,
@@ -1594,8 +1595,12 @@ static int tc_sensor_mix_bwd_data(int passes, const float* du, const float* w_hi
                                   bm_stream_t stream) {
     BM_CHECK_ARG(du && w_hi && (w_lo || passes == 1) && wsel && dmeg && n_sets > 0 && B > 0 && T > 0 && C > 0 && C <= Cp);
     BM_CHECK_ARG(tc::conv_tc_supported(T, Op, Cp, 1, 0));
-    return tc::launch_sensor_mix_bwd_tc(du, w_hi, passes == 1 ? nullptr : w_lo, wsel, n_sets, mask, B, T, Op, Cp, C, dmeg,
-                                        passes, status, ST(stream));
+    tc::SensorMixBwdOp o;
+    memset(&o, 0, sizeof(o));
+    o.x = du; o.w = w_hi; o.w_lo32 = passes == 1 ? nullptr : w_lo; o.passes = passes;
+    o.B = B; o.T = T; o.Cin = Op; o.Ntot = Cp; o.taps = 1; o.dilation = 1; o.sign = 1;
+    o.n_wsets = n_sets; o.wsel = wsel; o.y = dmeg; o.err = status; o.C = C; o.mask = mask;
+    return tc::launch_conv(o, ST(stream), __func__);
 }
 BM_TC_FORMS(bm_tc_sensor_mix_bwd_data, tc_sensor_mix_bwd_data,
             (const float* du, const float* w_hi, const float* w_lo, const int* wsel, int n_sets, const float* mask, int B,
@@ -1608,7 +1613,7 @@ static int tc_wgrad_grouped(int passes, const float* dy, const float* x, const i
                             int T, int M, int N, float* out, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(dy && x && order && seg_off && out && G > 0 && B > 0 && T > 0);
     BM_CHECK_ARG(tc::wgrad_tc_supported(M, N));
-    return tc::launch_wgrad_tc_grouped(dy, x, order, seg_off, G, B, T, M, N, out, passes, status, ST(stream));
+    return tc::launch_wgrad_tc_grouped(dy, x, order, seg_off, G, B, T, M, N, out, passes, ST(stream));
 }
 BM_TC_FORMS(bm_tc_wgrad_grouped, tc_wgrad_grouped,
             (const float* dy, const float* x, const int* order, const int* seg_off, int G, int B, int T, int M, int N,

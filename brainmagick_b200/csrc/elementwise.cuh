@@ -548,7 +548,7 @@ __device__ __forceinline__ float4 ld4(const float* p) { return *reinterpret_cast
 __device__ __forceinline__ float4 ld4s(const float* p) { return __ldcs(reinterpret_cast<const float4*>(p)); }   // streamed once
 
 // max |.| of what a block has just written -> ONE atomicMax per block on `cell` (the bits of a non-negative float order like
-// unsigned integers).  The consumer is the F16-pipe conv (tc_convh.cuh), which scales its operand by a power of two from it:
+// unsigned integers).  The consumer is the F16-pipe conv (bm_tc_conv1d_f16), which scales its operand by a power of two from it:
 // fusing the reduction here saves bm_amax's extra pass over the tensor.  Every thread of the block must call.
 __device__ __forceinline__ float amax4(float m, const float4& o) {
     return fmaxf(fmaxf(m, fmaxf(fabsf(o.x), fabsf(o.y))), fmaxf(fabsf(o.z), fabsf(o.w)));

@@ -12,10 +12,12 @@
 // pieces of a power-of-two-scaled copy (bm_tc_weight_split_f16); the pieces are summed back on load (fp16: ~22 significant
 // bits of the weight, the precision the pieces carry).  Fused epilogue: bias, addend (skip gradient / in-place accumulate),
 // pre-activation copy, exact GELU, channel-major store, GLU, BatchNorm column statistics (fp64), max |output|.
+// Every conv entry point of bm_api.cu fills its op and launches it through launch_conv.
 #pragma once
 #include <cuda_fp16.h>
 #include <cstring>
 #include "tc_common.cuh"
+#include "elementwise.cuh"
 
 namespace bm {
 namespace tc {
@@ -355,11 +357,15 @@ inline ConvOp conv_op_defaults() {
     return o;
 }
 
-inline int launch_conv_op(ConvOp o, cudaStream_t st, const char* who) {
+// The launch every conv entry point ends in, once it has filled its ConvOp (or SensorMixBwdOp): the time and column
+// tiling, the zeroed BatchNorm statistics and the kernel.  `who` is the entry point, for the error messages.
+template <class Op> inline int launch_conv(Op o, cudaStream_t st, const char* who) {
     if ((long long)o.B * o.T >= (1ll << 31)) return set_error(2, "%s: too many rows%s", who);
-    auto a8 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; };     // the epilogue's float2 accesses
-    if (!a8(o.bias) || !a8(o.addend) || !a8(o.aux) || !a8(o.glu_out) || (!o.out_tmajor && !a8(o.y)))
-        return set_error(2, "%s: bias, addend and the row-major outputs must be 8-byte aligned%s", who);
+    if (std::is_same<Op, ConvOp>::value) {    // ConvOp's epilogue accesses float2; SensorMixBwdOp's stores scalars
+        auto a8 = [](const void* p) { return (reinterpret_cast<uintptr_t>(p) & 7) == 0; };
+        if (!a8(o.bias) || !a8(o.addend) || !a8(o.aux) || !a8(o.glu_out) || (!o.out_tmajor && !a8(o.y)))
+            return set_error(2, "%s: bias, addend and the row-major outputs must be 8-byte aligned%s", who);
+    }
     o.ttiles = (o.T + HG_BM - 1) / HG_BM;
     const int bn = hg_pick_bn(o.Ntot);                   // GLU: BN/2 'a' columns and their gates per tile
     o.ncols = o.glu ? (o.Ntot / 2 + bn / 2 - 1) / (bn / 2) : (o.Ntot + bn - 1) / bn;
@@ -370,6 +376,47 @@ inline int launch_conv_op(ConvOp o, cudaStream_t st, const char* who) {
     return hc_launch_bn(bn, o, (long long)o.B * o.ttiles * o.ncols, st, who);
 }
 
+// ---- the published shape gates and epilogue rules ---------------------------------------------------------------------
+// The kernel itself handles any N; the gates are the library's contract.
+// bm_tc_conv1d / bm_tc_pointwise_sel: Ntot a multiple of 16 with a divisor in [64, 160] (GLU: H a multiple of 80), K chunks
+// of 32 input channels.
+inline bool conv_tc_supported(int T, int Cin, int Ntot, int Kw, int glu) {
+    if (Kw < 1 || Kw > 3 || (Kw & 1) == 0) return false;
+    if (Cin % HG_BK != 0) return false;
+    if (glu) return Ntot % 2 == 0 && (Ntot / 2) % 80 == 0;
+    for (int bn = 160; bn >= 64; bn -= 16)
+        if (Ntot % bn == 0) return true;
+    return false;
+}
+
+// bm_tc_conv1d_persistent / bm_tc_conv1d_f16: the output columns split into pairs of column halves of nh = 160 or 128
+// (Ntot a multiple of 2 nh; GLU: H a multiple of nh), K chunks of 32 input channels.  conv_half_width: nh, 0 if none.
+inline int conv_half_width(int Ntot, int glu) {
+    if (glu && (Ntot % 2)) return 0;
+    const int n = glu ? Ntot / 2 : Ntot;
+    for (int nh = 160; nh >= 128; nh -= 32)
+        if (n % (glu ? nh : 2 * nh) == 0) return nh;
+    return 0;
+}
+inline bool conv_halves_supported(int T, int Cin, int Ntot, int Kw, int glu) {
+    if (Kw < 1 || Kw > 3 || (Kw & 1) == 0) return false;
+    if (Cin % HG_BK != 0) return false;
+    return conv_half_width(Ntot, glu) != 0;
+}
+// The epilogue combinations bm_tc_conv1d_persistent* and bm_tc_conv1d_f16 accept (accumulate: y += conv in place), for a
+// shape that passed conv_halves_supported: 0, or 2 with the reason.  BatchNorm statistics need a plain conv of one pair of
+// column halves (Ntot = 2 nh).
+inline int conv_halves_epilogue_check(int Ntot, int glu, int act, int out_tmajor, int accumulate, const float* aux,
+                                      const double* stats, const char* who) {
+    if (stats && (glu || out_tmajor || act || accumulate || Ntot != 2 * conv_half_width(Ntot, 0)))
+        return set_error(2, "%s: statistics need a plain single-N-tile conv%s", who);
+    if (glu && (act || out_tmajor || aux || accumulate)) return set_error(2, "%s: GLU excludes the other epilogues%s", who);
+    if (out_tmajor && (act || accumulate)) return set_error(2, "%s: channel-major output is a plain store%s", who);
+    if (act && accumulate) return set_error(2, "%s: accumulate excludes the activation%s", who);
+    return 0;
+}
+
+// ---- weight preparation -------------------------------------------------------------------------------------------------
 // W[o][i][j] (nn.Conv1d layout) -> tf32-split K-major operands:
 //   fwd  operand: F[j][o][i]   (n = o, k = i)        data-gradient operand: G[j][i][o]   (n = i, k = o)
 __global__ void weight_split_kernel(const float* __restrict__ W, float* __restrict__ f_hi, float* __restrict__ f_lo,
@@ -383,55 +430,91 @@ __global__ void weight_split_kernel(const float* __restrict__ W, float* __restri
         float v = W[idx];
         float h = tf32_rna(v), l = tf32_rna(v - h);
         long long fi = ((long long)j * O + o) * I + i, gi = ((long long)j * I + i) * O + o;
-        // a NULL lo pointer asks for the RAW fp32 value in the re-laid array (the v2 kernel splits in shared memory)
+        // a NULL lo pointer asks for the RAW fp32 value in the re-laid array (bm_tc_conv1d_persistent's weights: the
+        // kernel splits them on load)
         if (f_hi) { if (f_lo) { f_hi[fi] = h; f_lo[fi] = l; } else f_hi[fi] = v; }
         if (g_hi) { if (g_lo) { g_hi[gi] = h; g_lo[gi] = l; } else g_hi[gi] = v; }
     }
 }
 
-// Shape gate of bm_tc_conv1d / bm_tc_pointwise_sel: Ntot a multiple of 16 with a divisor in [64, 160] (GLU: H a multiple
-// of 80), K chunks of 32 input channels.  The kernel itself handles any N; the gate is the library's published contract.
-inline bool conv_tc_supported(int T, int Cin, int Ntot, int Kw, int glu) {
-    if (Kw < 1 || Kw > 3 || (Kw & 1) == 0) return false;
-    if (Cin % HG_BK != 0) return false;
-    if (glu) return Ntot % 2 == 0 && (Ntot / 2) % 80 == 0;
-    for (int bn = 160; bn >= 64; bn -= 16)
-        if (Ntot % bn == 0) return true;
-    return false;
+// The fp16 pieces of bm_tc_conv1d_f16's weights: w*s = hi + lo (11 + 11 significant bits) with s = f16_scale_of(amax).
+// largest |x| of a tensor into `cell` (a float whose bits compare like an unsigned integer because it is non-negative);
+// NaNs are ignored by fmaxf, +-inf gives inf (=> scale 1: the conv then propagates the non-finite values like fp32 would)
+__global__ void __launch_bounds__(256) amax_kernel(const float* __restrict__ x, long long n, unsigned int* __restrict__ cell) {
+    float m = 0.f;
+    const long long n4 = n >> 2;
+    const float4* x4 = reinterpret_cast<const float4*>(x);
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
+        const float4 v = __ldg(x4 + i);
+        m = fmaxf(fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
+    }
+    if (blockIdx.x == 0)
+        for (long long i = (n4 << 2) + threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(x[i]));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    __shared__ float wm[8];
+    if ((threadIdx.x & 31) == 0) wm[threadIdx.x >> 5] = m;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < 8; ++w) m = fmaxf(m, wm[w]);
+        if (m > 0.f) atomicMax(cell, __float_as_uint(m));
+    }
+}
+// src * scale(amax) -> fp16 hi and lo copies (same element order)
+__global__ void __launch_bounds__(256) f16_split_kernel(const float* __restrict__ src, long long n,
+                                                        const float* __restrict__ amax, __half* __restrict__ hi,
+                                                        __half* __restrict__ lo) {
+    const float s = f16_scale_of(__ldg(amax));
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+        const float v = src[i] * s;
+        const __half h = __float2half_rn(v);
+        hi[i] = h;
+        lo[i] = __float2half_rn(v - __half2float(h));
+    }
 }
 
-// x [B,T,Cin]; w_hi / w_lo [Kw][Ntot][Cin] (wsel: [n_wsets][Kw][Ntot][Cin]), the tf32 pieces of bm_tc_weight_split
-// (passes = 1: w_hi alone is read, w_lo may be null)
-struct ConvTcP {
-    int B, T, Cin, Ntot, taps, dilation, sign, glu, act, out_tmajor, passes;
-    const float* bias; const float* addend;
-    float* y; float* aux; float* glu_out;
-    int n_wsets; const int* wsel;
-    int* err;
-};
-inline int launch_conv_tc(const float* x, const float* w_hi, const float* w_lo, const ConvTcP& p, cudaStream_t st) {
-    ConvOp o = conv_op_defaults();
-    o.x = x; o.w = w_hi; o.w_lo32 = w_lo; o.B = p.B; o.T = p.T; o.Cin = p.Cin; o.Ntot = p.Ntot; o.taps = p.taps; o.dilation = p.dilation;
-    o.sign = p.sign; o.glu = p.glu; o.n_wsets = p.wsel ? p.n_wsets : 1; o.wsel = p.wsel; o.bias = p.bias;
-    o.addend = p.addend; o.y = p.y; o.aux = p.aux; o.glu_out = p.glu_out; o.act = p.act; o.out_tmajor = p.out_tmajor;
-    o.err = p.err; o.passes = p.passes;
-    return launch_conv_op(o, st, __func__);
+// W[o][i][j] (nn.Conv1d layout) * scale(amax) -> fp16 hi / lo pieces in the K-major layouts of bm_tc_weight_split:
+//   forward operand F[j][o][i], data-gradient operand G[j][i][o]; either pair may be NULL.  One launch per layer and step
+//   instead of re-layout + two splits.
+__global__ void __launch_bounds__(256) weight_split_f16_kernel(const float* __restrict__ W, const float* __restrict__ amax,
+                                                               __half* __restrict__ f_hi, __half* __restrict__ f_lo,
+                                                               __half* __restrict__ g_hi, __half* __restrict__ g_lo, int O, int I,
+                                                               int Kw) {
+    const float s = f16_scale_of(__ldg(amax));
+    const long long total = (long long)O * I * Kw;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+        const int j = (int)(idx % Kw);
+        const long long oi = idx / Kw;
+        const int i = (int)(oi % I), o = (int)(oi / I);
+        const float v = W[idx] * s;
+        const __half h = __float2half_rn(v);
+        const __half l = __float2half_rn(v - __half2float(h));
+        const long long fi = ((long long)j * O + o) * I + i, gi = ((long long)j * I + i) * O + o;
+        if (f_hi) { f_hi[fi] = h; f_lo[fi] = l; }
+        if (g_hi) { g_hi[gi] = h; g_lo[gi] = l; }
+    }
 }
 
-// du [B,T,Op]; w_hi / w_lo [n_sets][Cp][Op] (tf32 pieces; passes = 1: w_hi alone); dmeg [B,C,T] with C <= Cp; mask [C]
-// or null
-inline int launch_sensor_mix_bwd_tc(const float* du, const float* w_hi, const float* w_lo, const int* wsel, int n_sets,
-                                    const float* mask, int B, int T, int Op, int Cp, int C, float* dmeg, int passes,
-                                    int* err, cudaStream_t st) {
-    SensorMixBwdOp o;
-    memset(&o, 0, sizeof(o));
-    o.x = du; o.w = w_hi; o.w_lo32 = w_lo; o.B = B; o.T = T; o.Cin = Op; o.Ntot = Cp; o.taps = 1; o.dilation = 1; o.sign = 1;
-    o.n_wsets = n_sets; o.wsel = wsel; o.y = dmeg; o.err = err; o.C = C; o.mask = mask; o.passes = passes;
-    if ((long long)B * T >= (1ll << 31)) return set_error(2, "%s: too many rows%s", __func__);
-    o.ttiles = (T + HG_BM - 1) / HG_BM;
-    const int bn = hg_pick_bn(Cp);
-    o.ncols = (Cp + bn - 1) / bn;
-    return hc_launch_bn(bn, o, (long long)B * o.ttiles * o.ncols, st, __func__);
+inline int launch_amax(const float* x, long long n, float* cell, cudaStream_t st) {
+    cudaError_t e = cudaMemsetAsync(cell, 0, 4, st);
+    if (e != cudaSuccess) return set_error(3, "%s: memset: %s", __func__, cudaGetErrorString(e));
+    long long blocks = (n / 4 + 255) / 256;
+    const long long cap = (long long)num_sms() * 8;
+    if (blocks > cap) blocks = cap;
+    if (blocks < 1) blocks = 1;
+    amax_kernel<<<(int)blocks, 256, 0, st>>>(x, n, reinterpret_cast<unsigned int*>(cell));
+    ++g_launches;
+    e = cudaGetLastError();
+    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", __func__, cudaGetErrorString(e));
+    return 0;
+}
+inline int launch_f16_split(const float* src, long long n, const float* amax, void* hi, void* lo, cudaStream_t st) {
+    f16_split_kernel<<<ew_grid(n), 256, 0, st>>>(src, n, amax, reinterpret_cast<__half*>(hi), reinterpret_cast<__half*>(lo));
+    ++g_launches;
+    cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", __func__, cudaGetErrorString(e));
+    return 0;
 }
 
 }  // namespace tc

@@ -106,9 +106,7 @@ struct WgradOp {
 
 // dY [B,T,M], X [B,T,N] -> dW [M][Ntrue][taps]; ws: wgrad_workspace_floats() floats
 inline int launch_wgrad_tc(const float* dY, const float* X, int B, int T, int M, int N, int Ntrue, int taps,
-                           int dilation, float* ws, float* dW, int passes, int* err, cudaStream_t st,
-                           float* dbias = nullptr) {
-    (void)err;
+                           int dilation, float* ws, float* dW, int passes, cudaStream_t st, float* dbias = nullptr) {
     int nh, mblocks, ksplit, bchunk;
     wgrad_geometry(B, M, N, taps, &nh, &mblocks, &ksplit, &bchunk);
     if (nh == 0) return set_error(2, "%s: unsupported N%s", __func__);
@@ -142,8 +140,7 @@ inline int launch_wgrad_tc(const float* dY, const float* X, int B, int T, int M,
 // grouped pointwise weight gradient: out[g][m][n] = sum_{b in group g} sum_t dY[b,t,m] X[b,t,n]; out is [G][Mpad][N] with
 // Mpad = ceil(M/128)*128 (rows >= M are zero); groups given as CSR (zlist, seg_off[G+1]) over the samples.
 inline int launch_wgrad_tc_grouped(const float* dY, const float* X, const int* zlist, const int* seg_off, int G, int B,
-                                   int T, int M, int N, float* out, int passes, int* err, cudaStream_t st) {
-    (void)err;
+                                   int T, int M, int N, float* out, int passes, cudaStream_t st) {
     if (wgrad_pick_nh(N) == 0) return set_error(2, "%s: unsupported N%s", __func__);
     if (G > 65535) return set_error(2, "%s: too many groups%s", __func__);
     const int mblocks = (M + WG_BM - 1) / WG_BM;

@@ -72,26 +72,15 @@ __global__ void wgradp_reduce_kernel(const float* __restrict__ P, float* __restr
     }
 }
 
-struct WgradPPGeom { int nt, h0, h1, mtiles, ntiles, ks, chunks, per_split, rows, bn; };
+struct WgradPPGeom { int mtiles, ks, chunks, per_split, rows, bn; };
 
-inline bool wgradp_pick_nt(int Mdy, int* nt, int* h0, int* h1) {
-    if (Mdy % 320 == 0) { *nt = 320; *h0 = 192; *h1 = 128; return true; }
-    if (Mdy % 256 == 0) { *nt = 256; *h0 = 128; *h1 = 128; return true; }
-    if (Mdy % 192 == 0) { *nt = 192; *h0 = 192; *h1 = 0; return true; }
-    if (Mdy % 128 == 0) { *nt = 128; *h0 = 128; *h1 = 0; return true; }
-    if (Mdy % 64 == 0) { *nt = 64; *h0 = 64; *h1 = 0; return true; }
-    return false;
-}
 inline bool wgradp_supported(int T, int Mdy, int Nx, int taps) {
-    int nt, h0, h1;
-    return T >= HG_BK && Nx % 32 == 0 && Nx >= 32 && taps >= 1 && taps <= 3 && wgradp_pick_nt(Mdy, &nt, &h0, &h1);
+    return T >= HG_BK && Nx % 32 == 0 && Nx >= 32 && taps >= 1 && taps <= 3 && Mdy % 64 == 0;
 }
 inline WgradPPGeom wgradp_geometry(int B, int T, int Mdy, int Nx, int taps) {
     WgradPPGeom g;
-    wgradp_pick_nt(Mdy, &g.nt, &g.h0, &g.h1);
     g.rows = taps * Nx;
     g.mtiles = (g.rows + 255) / 256;
-    g.ntiles = Mdy / g.nt;
     const long long R = (long long)B * T;
     g.chunks = (int)((R + HG_BK - 1) / HG_BK);
     g.bn = hg_pick_bn(Mdy);
@@ -127,14 +116,6 @@ inline int launch_wgrad_pp(const float* dY, const float* X, int B, int T, int Md
     cudaError_t e = cudaGetLastError();
     if (e != cudaSuccess) return set_error(3, "%s: reduce launch failed: %s", __func__, cudaGetErrorString(e));
     return 0;
-}
-
-// the entry point that takes max |dy| and max |x| (bm_tc_wgrad_conv_f16): the operands are read as fp32 and split on the
-// engine's 3xTF32 path, so the scales are not needed
-inline int launch_wgrad_hp(const float* dY, const float* dy_amax, const float* X, const float* x_amax, int B, int T, int Mdy,
-                           int Nx, int Ntrue, int taps, int dilation, float* ws, float* dW, int* err, cudaStream_t st) {
-    (void)dy_amax; (void)x_amax;
-    return launch_wgrad_pp(dY, X, B, T, Mdy, Nx, Ntrue, taps, dilation, ws, dW, 3, err, st);
 }
 
 }  // namespace tc

@@ -203,7 +203,7 @@ def tc_wgrad(dy, x, B, T, M, N, Ntrue, kw, dilation, status, dbias=None):
     `dbias` [M] (optional) receives sum_{b,t} dy[b,t,m]."""
     lib = _lib.load()
     dw = _empty((M, Ntrue, kw), dy)
-    rows = kw * N                                       # output rows of the pair kernel, tiled in blocks of 256
+    rows = kw * N                                       # output rows of bm_tc_wgrad_conv's GEMM, tiled in blocks of 256
     pair_ok = bool(lib.bm_tc_wgrad_conv_supported(T, M, N, kw)) and \
         rows / (-(-rows // 256) * 256) >= 0.9            # else the single-CTA kernel wastes less on padding rows
     if pair_ok:
@@ -249,8 +249,8 @@ class _Conv:
         st = stream()
         lib = _lib.load()
         g = 1 if glu else 0
-        # raw-weight entry point (csrc/tc_convp.cuh) where its shape gate fits, else the pre-split one (tc_conv.cuh),
-        # else FP32 FMA
+        # raw-weight entry point (bm_tc_conv1d_persistent) where its shape gate fits, else the pre-split one
+        # (bm_tc_conv1d), else FP32 FMA
         self.fwd_pp = allow_tc and bool(lib.bm_tc_conv1d_persistent_supported(T, self.cin, self.cout, self.kw, g))
         self.bwd_pp = allow_tc and bool(lib.bm_tc_conv1d_persistent_supported(T, self.cout, self.cin, self.kw, 0))
         fwd_tc = self.fwd_pp or (allow_tc and bool(lib.bm_tc_conv_supported(T, self.cin, self.cout, self.kw, g)))
@@ -614,7 +614,7 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
         if not nd.below[k]:
             pass
         elif rec["skip"]:
-            # in place: g += conv_transpose(dy) (addend == output: the pair kernel turns this into a TMA reduce-add)
+            # in place: g += conv_transpose(dy) (addend == output: the conv epilogue adds g and stores the sum over it)
             conv.backward_data(dy, g, B, T, plan.dilations[k], g, status)
         else:
             g_in = _empty((B, T, conv.cin), like)

@@ -294,7 +294,7 @@ int bm_tc_conv1d(const float* x, const float* w_hi, const float* w_lo, const flo
  * channel-major `estimate`).  With Kw=1 this is the pointwise (1x1) contraction of the head (K5).
  * bm_col_stats: stats[0:C] = sum_r y[r,c], stats[C:2C] = sum_r y[r,c]^2 (fp64), the BatchNorm batch statistics. */
 int bm_col_stats(const float* y, long long rows, int C, double* stats, bm_stream_t stream);
-/* csrc/tc_convp.cuh: the same conv from the RAW fp32 weights re-laid K-major [Kw][Ntot][Cin] (bm_tc_weight_split with
+/* bm_tc_conv1d_persistent: the same conv from the RAW fp32 weights re-laid K-major [Kw][Ntot][Cin] (bm_tc_weight_split with
  * f_lo / g_lo = NULL); the kernel splits them into tf32 pieces itself (taps that would cross a sample edge read zeros =
  * the conv padding).  accumulate=1: y += conv(x) in place (the skip-path gradient).  glu / act / out_tmajor / aux / glu_out as
  * bm_tc_conv1d.  stats (nullable; plain forward only): BatchNorm batch statistics stats[0:Ntot] = sum(y), stats[Ntot:2Ntot]
@@ -305,7 +305,7 @@ int bm_tc_conv1d_persistent(const float* x, const float* w_raw, const float* bia
                             int Ntot, int Kw, int dilation, int sign, int glu, int act, int out_tmajor, float* y,
                             float* aux, float* glu_out, double* stats, int* status, bm_stream_t stream);
 
-/* The same conv with the weights as fp16 pieces (csrc/tc_convh.cuh; replaces the same reference lines as
+/* The same conv with the weights as fp16 pieces (bm_tc_conv1d_f16; replaces the same reference lines as
  * bm_tc_conv1d_persistent: nn.Conv1d / GLU in bm/models/common.py:107-151, the head's 1x1 convs simpleconv.py:153-168).
  * The weights are carried as two fp16 pieces (11 + 11 significant bits) of the tensor times a power of two that puts its
  * largest magnitude in [2^14, 2^15); the kernel sums the pieces back (hi + lo: ~22 significant bits of the weight, the

@@ -393,7 +393,7 @@ class Emulator:
         self.bm_tc_conv1d(x, w_raw, None, bias, y if accumulate else None, B, T, Cin, Ntot, Kw, dilation, sign, glu, act,
                           out_tmajor, y, aux, glu_out, stats, status, stream)
 
-    # ---- F16 pipe (csrc/tc_convh.cuh): power-of-two scale from the tensor's amax, operands as fp16 hi + lo pieces ----
+    # ---- F16 pipe (bm_tc_conv1d_f16, csrc/tc_conv.cuh): power-of-two scale from the tensor's amax, operands as fp16 hi + lo pieces ----
     @staticmethod
     def _f16_scale(amax: float) -> float:
         import math

@@ -1,5 +1,5 @@
-"""GPU: the conv entry points -- fp32 weights (csrc/tc_convp.cuh, bm_tc_conv1d_persistent) and fp16-piece weights
-(csrc/tc_convh.cuh, bm_tc_conv1d_f16), both on the 3xTF32 wgmma engine -- in every epilogue mode against torch's fp64 conv (test-only
+"""GPU: the conv entry points -- fp32 weights (bm_tc_conv1d_persistent) and fp16-piece weights (bm_tc_conv1d_f16), both
+on the 3xTF32 wgmma engine of csrc/tc_conv.cuh -- in every epilogue mode against torch's fp64 conv (test-only
 reference), at the real layer shapes, incl. the flattened-row tiling across sample edges (odd batch sizes, T not a multiple
 of anything) and the BatchNorm statistics out of the epilogue."""
 import pytest

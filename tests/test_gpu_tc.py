@@ -105,7 +105,7 @@ def test_tc_conv_glu_and_data_gradient(gen):
     e = rel_err(dx.cpu(), ref_dx.cpu())
     print(f'[tc dgrad K=1920] rel_err vs fp64 = {e:.2e}')
     assert e < TOL
-    # in-place skip-gradient accumulation (addend == output): the pair kernel uses a TMA reduce-add
+    # in-place skip-gradient accumulation (addend == output): the epilogue reads each element before it overwrites it
     acc = addend.clone()
     call(_FN[gen], ptr(dy), ptr(gh), ptr(gl), None, ptr(acc), B, T, 2 * H, H, Kw, 1, -1, 0, 0, 0, ptr(acc), None, None,
          None, ptr(status), stream())
@@ -281,12 +281,12 @@ def test_tc_wgrad_pair_speed_report(capsys):
         amax = torch.empty(2, device=dev)
         call("bm_amax", ptr(dy), dy.numel(), ptr(amax[0:1]), stream())
         call("bm_amax", ptr(x), x.numel(), ptr(amax[1:2]), stream())
-        for name, fn in (("pair kernel, F16 pipe", lambda: call("bm_tc_wgrad_conv_f16", ptr(dy), ptr(amax[0:1]), ptr(x),
-                                                                 ptr(amax[1:2]), B, T, M, N, N, Kw, 4, ptr(ws_new), ptr(dw),
-                                                                 ptr(status), stream())),
-                         ("pair kernel", lambda: call("bm_tc_wgrad_conv", ptr(dy), ptr(x), B, T, M, N, N, Kw, 4, ptr(ws_new),
-                                                       ptr(dw), ptr(status), stream())),
-                         ("round-1 kernel", lambda: call("bm_tc_wgrad", ptr(dy), ptr(x), B, T, M, N, N, Kw, 4, ptr(ws_old),
+        for name, fn in (("fp16-piece entry", lambda: call("bm_tc_wgrad_conv_f16", ptr(dy), ptr(amax[0:1]), ptr(x),
+                                                            ptr(amax[1:2]), B, T, M, N, N, Kw, 4, ptr(ws_new), ptr(dw),
+                                                            ptr(status), stream())),
+                         ("fp32 entry", lambda: call("bm_tc_wgrad_conv", ptr(dy), ptr(x), B, T, M, N, N, Kw, 4, ptr(ws_new),
+                                                      ptr(dw), ptr(status), stream())),
+                         ("per-tap kernel", lambda: call("bm_tc_wgrad", ptr(dy), ptr(x), B, T, M, N, N, Kw, 4, ptr(ws_old),
                                                           ptr(dw), None, ptr(status), stream()))):
             times = []
             for i in range(13):
@@ -301,27 +301,6 @@ def test_tc_wgrad_pair_speed_report(capsys):
             ms = sum(times) / len(times)
             tf = 2.0 * M * N * Kw * T * B / (ms * 1e-3) / 1e12
             lines.append(f"[wgrad {M}x{N} k3 B=256 T=360, {name}] {ms:.4f} ms/launch = {tf:.1f} algorithmic TFLOP/s")
-    # where the pair kernel's warp roles wait (cycle counters of the debug buffer, averaged over the leader CTAs)
-    M, N = 320, 320
-    dy = torch.randn(B, T, M, device=dev)
-    x = torch.randn(B, T, N, device=dev)
-    dw = torch.empty(M, N, Kw, device=dev)
-    ws_new = torch.empty(int(_lib.load().bm_tc_wgrad_conv_workspace(B, T, M, N, Kw)), device=dev)
-    dbg = torch.zeros(8 * 148, device=dev, dtype=torch.int64)
-    call("bm_set_debug_buffer", ptr(dbg))
-    try:
-        flush.zero_()
-        call("bm_tc_wgrad_conv", ptr(dy), ptr(x), B, T, M, N, N, Kw, 4, ptr(ws_new), ptr(dw), ptr(status), stream())
-        torch.cuda.synchronize()
-    finally:
-        call("bm_set_debug_buffer", None)
-    d = dbg.reshape(148, 8).double()
-    lead, foll = d[0::2], d[1::2]
-    lines.append("[wgrad pair kernel cycles, mean over CTAs] MMA thread: waiting for converters %.0f of %.0f total; "
-                 "A converter: split+issue loads %.0f, wait slot free %.0f, tmem store+arrive %.0f; B converter: wait TMA %.0f "
-                 "(follower CTA: A %.0f / %.0f / %.0f, B %.0f)" % (
-                     lead[:, 0].mean(), lead[:, 1].mean(), lead[:, 2].mean(), lead[:, 3].mean(), lead[:, 4].mean(),
-                     lead[:, 5].mean(), foll[:, 2].mean(), foll[:, 3].mean(), foll[:, 4].mean(), foll[:, 5].mean()))
     assert int(status.item()) == 0
     with capsys.disabled():
         print("\n" + "\n".join(lines))
