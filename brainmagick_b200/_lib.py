@@ -32,9 +32,12 @@ SIGNATURES = {
     "bm_conv_weight_prep": [P, I, I, I, P, P, P],
     "bm_conv1d_fwd": [P, P, P, I, I, I, I, I, I, P, P, P],
     "bm_bn_stats_finalize": [P, L, F, F, P, P, P, P, I, P],
+    "bm_bn_stats_finalize_counted": [P, F, F, P, P, P, P, I, P],
     "bm_bn_eval_stats": [P, P, F, P, P, I, P],
     "bm_bn_gelu_skip_fwd": [P, P, P, P, P, P, P, L, I, P, P],
     "bm_bn_gelu_skip_bwd": [P, P, P, P, P, P, I, L, I, P, P, P, P, P, P],
+    "bm_bn_gelu_skip_bwd_reduce": [P, P, P, P, P, P, L, I, P, P, P, P],
+    "bm_bn_gelu_skip_bwd_apply": [P, P, P, P, P, P, L, I, P, P, P],
     "bm_conv1d_bwd_data": [P, P, P, I, I, I, I, I, I, P, P],
     "bm_conv1d_bwd_weight": [P, P, I, I, I, I, I, I, P, P, P],
     "bm_conv1d_glu_fwd": [P, P, P, I, I, I, I, I, P, P, P],
@@ -80,6 +83,8 @@ SIGNATURES = {
     "bm_gather_rows": [P, P, I, L, P, P],
     "bm_bn_act_skip_fwd": [P, P, P, P, P, P, P, L, I, I, F, P],
     "bm_bn_act_skip_bwd": [P, P, P, P, P, P, I, L, I, I, F, P, P, P, P, P],
+    "bm_bn_act_skip_bwd_reduce": [P, P, P, P, P, P, L, I, I, F, P, P, P, P],
+    "bm_bn_act_skip_bwd_apply": [P, P, P, P, P, P, L, I, I, F, P, P, P],
     "bm_bn_act_gain_skip_fwd": [P, P, P, P, P, P, P, L, I, I, F, P, F, P, P],
     "bm_bn_act_gain_skip_bwd": [P, P, P, P, P, P, I, L, I, I, F, P, F, P, P, P, P, P, P, P, P],
     "bm_clip_loss_bwd_cand": [P, P, P, P, P, P, I, I, L, I, P, P, P, P, P],
@@ -93,6 +98,10 @@ SIGNATURES = {
     "bm_bn_gelu_skip_bwd_det": [P, P, P, P, P, P, I, L, I, P, P, P, P, P, P, L, P],
     "bm_bn_act_skip_bwd_det_workspace": [L, I],
     "bm_bn_act_skip_bwd_det": [P, P, P, P, P, P, I, L, I, I, F, P, P, P, P, P, L, P],
+    "bm_bn_gelu_skip_bwd_reduce_det_workspace": [L, I],
+    "bm_bn_gelu_skip_bwd_reduce_det": [P, P, P, P, P, P, L, I, P, P, P, P, L, P],
+    "bm_bn_act_skip_bwd_reduce_det_workspace": [L, I],
+    "bm_bn_act_skip_bwd_reduce_det": [P, P, P, P, P, P, L, I, I, F, P, P, P, P, L, P],
     "bm_bn_act_gain_skip_bwd_det_workspace": [L, I],
     "bm_bn_act_gain_skip_bwd_det": [P, P, P, P, P, P, I, L, I, I, F, P, F, P, P, P, P, P, P, P, P, L, P],
     "bm_glu_bwd_det_workspace": [L, I],

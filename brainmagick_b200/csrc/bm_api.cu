@@ -457,6 +457,16 @@ extern "C" int bm_bn_stats_finalize(const double* stats, long long n, float eps,
     return 0;
 }
 
+extern "C" int bm_bn_stats_finalize_counted(const double* stats, float eps, float momentum, float* running_mean,
+                                            float* running_var, float* mean, float* invstd, int C, bm_stream_t stream) {
+    BM_CHECK_ARG(stats && mean && invstd && C > 0);
+    BM_CHECK_ARG((running_mean == nullptr) == (running_var == nullptr));
+    bn_finalize_kernel<true><<<(C + 127) / 128, 128, 0, ST(stream)>>>(stats, 0.0, eps, momentum, running_mean, running_var,
+                                                                     mean, invstd, C);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
 extern "C" int bm_bn_eval_stats(const float* running_mean, const float* running_var, float eps, float* mean,
                                 float* invstd, int C, bm_stream_t stream) {
     BM_CHECK_ARG(running_mean && running_var && mean && invstd && C > 0);
@@ -499,6 +509,86 @@ extern "C" int bm_bn_gelu_skip_fwd(const float* y, const float* mean, const floa
     return 0;
 }
 
+// The BatchNorm + GELU backward in its two halves, which a SyncBatchNorm caller runs as two calls with the all-reduce of the
+// sums between them (bm_bn_gelu_skip_bwd_reduce / _apply); bm_bn_gelu_skip_bwd runs them back to back.
+// cs: the column-stationary kernels (C % 4 == 0, C / 4 <= 256, 16-byte aligned operands), else the generic / float4 ones.
+static bool bn_gelu_vec(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                        const float* beta, int C) {
+    return (C % 4 == 0) && aligned16(g, y, mean) && aligned16(invstd, gamma, beta);
+}
+
+// reduce half: sums [2C] = (sum dz, sum dz*yhat) over the call's rows, then dbeta / dgamma = their float roundings.
+// part: NULL (fp64 atomics into sums, zeroed by the caller) or the bn_bwd_ws_floats(rows, C) partials of the deterministic form
+static int bn_gelu_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                              const float* beta, long long rows, int C, bool cs, double* sums, float* dgamma, float* dbeta,
+                              double* part, cudaStream_t st) {
+    if (cs) {
+        const int cx = C / 4, ry = std::max(1, 320 / cx);
+        const unsigned nblk = (unsigned)((rows + CS_ROWS_PER_BLOCK - 1) / CS_ROWS_PER_BLOCK);
+        if (part) {
+            bn_gelu_bwd_reduce_cs_kernel<true><<<nblk, dim3(cx, ry), sizeof(float) * 2 * C * ry, st>>>(
+                g, y, mean, invstd, gamma, beta, part, rows, C);
+            BM_CHECK_LAUNCH();
+            if (int rc = reduce_rows(part, (long long)nblk, 2 * C, sums, st)) return rc;
+        } else {
+            bn_gelu_bwd_reduce_cs_kernel<<<nblk, dim3(cx, ry), sizeof(float) * 2 * C * ry, st>>>(g, y, mean, invstd, gamma,
+                                                                                              beta, sums, rows, C);
+            BM_CHECK_LAUNCH();
+        }
+    } else {   // generic shapes: one thread per column, 128 rows per block
+        const int rpb = 128;
+        dim3 grid((unsigned)((rows + rpb - 1) / rpb), (C + 127) / 128);
+        if (part) {
+            bn_gelu_bwd_reduce_kernel<true><<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, part, rows, C, rpb);
+            BM_CHECK_LAUNCH();
+            if (int rc = reduce_rows(part, (long long)grid.x, 2 * C, sums, st)) return rc;
+        } else {
+            bn_gelu_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C, rpb);
+            BM_CHECK_LAUNCH();
+        }
+    }
+    bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
+// apply half: dy.  counted: the sums and the row count n come from `sums` [2C + 1] (n in sums[2C], read on the device);
+// else n = rows and the column-stationary kernel takes the sums as dgamma / dbeta.  Both give the same bits for the same n.
+static int bn_gelu_bwd_apply(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                             const float* beta, int batch_stats, long long rows, int C, bool cs, const double* sums,
+                             const float* dgamma, const float* dbeta, bool counted, float* dy, float* amax_out,
+                             cudaStream_t st) {
+    const long long total = rows * C;
+    if (cs) {
+        const int cx = C / 4, ry = std::max(1, 320 / cx);
+        const unsigned nblk = (unsigned)((rows + CS_ROWS_PER_BLOCK - 1) / CS_ROWS_PER_BLOCK);
+        unsigned int* amax = reinterpret_cast<unsigned int*>(amax_out);
+        if (counted)
+            bn_gelu_bwd_apply_cs_kernel<true><<<nblk, dim3(cx, ry), 0, st>>>(g, y, mean, invstd, gamma, beta, nullptr, nullptr,
+                                                                            sums, 0.f, 1, dy, rows, C, amax);
+        else
+            bn_gelu_bwd_apply_cs_kernel<<<nblk, dim3(cx, ry), 0, st>>>(g, y, mean, invstd, gamma, beta, dgamma, dbeta, nullptr,
+                                                                       (float)(1.0 / (double)rows), batch_stats, dy, rows, C,
+                                                                       amax);
+        BM_CHECK_LAUNCH();
+        return 0;
+    }
+    if (bn_gelu_vec(g, y, mean, invstd, gamma, beta, C) && aligned16(dy)) {
+        auto* kernel = counted ? bn_gelu_bwd_apply_v4_kernel<true> : bn_gelu_bwd_apply_v4_kernel<false>;
+        kernel<<<ew_grid(total / 4), 256, 0, st>>>(
+            reinterpret_cast<const float4*>(g), reinterpret_cast<const float4*>(y), reinterpret_cast<const float4*>(mean),
+            reinterpret_cast<const float4*>(invstd), reinterpret_cast<const float4*>(gamma),
+            reinterpret_cast<const float4*>(beta), sums, (double)rows, batch_stats, reinterpret_cast<float4*>(dy),
+            total / 4, C);
+    } else {
+        auto* kernel = counted ? bn_gelu_bwd_apply_kernel<true> : bn_gelu_bwd_apply_kernel<false>;
+        kernel<<<ew_grid(total), 256, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, (double)rows, batch_stats, dy, total, C);
+    }
+    BM_CHECK_LAUNCH();
+    if (amax_out) return tc::launch_amax(dy, total, amax_out, st);
+    return 0;
+}
+
 // The column reduction (sums, dgamma, dbeta) runs unless batch_stats == 0 and dgamma == dbeta == NULL: the data gradient of an
 // eval-mode BatchNorm whose affine parameters are frozen is then one elementwise pass (the apply kernels read the sums / dgamma /
 // dbeta only when use_batch_stats is set, so its dy is bitwise the reducing form's).
@@ -515,62 +605,12 @@ static int bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, c
     BM_CHECK_ARG(!reduce || (sums && dgamma && dbeta));
     if (reduce && !part) BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
     if (int rc = amax_begin(amax_out, st)) return rc;
-    const long long total = rows * C;
-    const bool vec = (C % 4 == 0) && aligned16(g, y, dy) && aligned16(mean, invstd, gamma) && aligned16(beta);
-    if (vec && C / 4 <= 256 && aligned16(dgamma, dbeta)) {
-        const int cx = C / 4, ry = std::max(1, 320 / cx);
-        const unsigned nblk = (unsigned)((rows + CS_ROWS_PER_BLOCK - 1) / CS_ROWS_PER_BLOCK);
-        if (!reduce) {
-            bn_gelu_bwd_apply_cs_kernel<<<nblk, dim3(cx, ry), 0, st>>>(g, y, mean, invstd, gamma, beta, nullptr, nullptr,
-                                                                       (float)(1.0 / (double)rows), 0, dy, rows, C,
-                                                                       reinterpret_cast<unsigned int*>(amax_out));
-            BM_CHECK_LAUNCH();
-            return 0;
-        }
-        if (part) {
-            bn_gelu_bwd_reduce_cs_kernel<true><<<nblk, dim3(cx, ry), sizeof(float) * 2 * C * ry, st>>>(
-                g, y, mean, invstd, gamma, beta, part, rows, C);
-            BM_CHECK_LAUNCH();
-            if (int rc = reduce_rows(part, (long long)nblk, 2 * C, sums, st)) return rc;
-        } else {
-            bn_gelu_bwd_reduce_cs_kernel<<<nblk, dim3(cx, ry), sizeof(float) * 2 * C * ry, st>>>(g, y, mean, invstd, gamma,
-                                                                                              beta, sums, rows, C);
-            BM_CHECK_LAUNCH();
-        }
-        bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
-        BM_CHECK_LAUNCH();
-        bn_gelu_bwd_apply_cs_kernel<<<nblk, dim3(cx, ry), 0, st>>>(g, y, mean, invstd, gamma, beta, dgamma, dbeta,
-                                                                   (float)(1.0 / (double)rows), batch_stats, dy, rows, C,
-                                                                   reinterpret_cast<unsigned int*>(amax_out));
-        BM_CHECK_LAUNCH();
-        return 0;
-    }
-    if (reduce) {   // generic shapes: one thread per column, 128 rows per block
-        const int rpb = 128;
-        dim3 grid((unsigned)((rows + rpb - 1) / rpb), (C + 127) / 128);
-        if (part) {
-            bn_gelu_bwd_reduce_kernel<true><<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, part, rows, C, rpb);
-            BM_CHECK_LAUNCH();
-            if (int rc = reduce_rows(part, (long long)grid.x, 2 * C, sums, st)) return rc;
-        } else {
-            bn_gelu_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C, rpb);
-            BM_CHECK_LAUNCH();
-        }
-        bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
-        BM_CHECK_LAUNCH();
-    }
-    if (vec)
-        bn_gelu_bwd_apply_v4_kernel<<<ew_grid(total / 4), 256, 0, st>>>(
-            reinterpret_cast<const float4*>(g), reinterpret_cast<const float4*>(y), reinterpret_cast<const float4*>(mean),
-            reinterpret_cast<const float4*>(invstd), reinterpret_cast<const float4*>(gamma),
-            reinterpret_cast<const float4*>(beta), sums, (double)rows, batch_stats, reinterpret_cast<float4*>(dy),
-            total / 4, C);
-    else
-        bn_gelu_bwd_apply_kernel<<<ew_grid(total), 256, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, (double)rows,
-                                                               batch_stats, dy, total, C);
-    BM_CHECK_LAUNCH();
-    if (amax_out) return tc::launch_amax(dy, total, amax_out, st);
-    return 0;
+    const bool cs = bn_gelu_vec(g, y, mean, invstd, gamma, beta, C) && aligned16(dy) && C / 4 <= 256 &&
+                    aligned16(dgamma, dbeta);
+    if (reduce)
+        if (int rc = bn_gelu_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, cs, sums, dgamma, dbeta, part, st)) return rc;
+    return bn_gelu_bwd_apply(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, cs, sums, dgamma, dbeta, false, dy,
+                             amax_out, st);
 }
 
 extern "C" int bm_bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd,
@@ -594,6 +634,41 @@ extern "C" int bm_bn_gelu_skip_bwd_det(const float* g, const float* y, const flo
     BM_CHECK_WS(bn_bwd_ws_floats(rows, C));
     return bn_gelu_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, sums, dy, dgamma, dbeta, amax_out,
                             reinterpret_cast<double*>(workspace), ST(stream));
+}
+
+// SyncBatchNorm halves (the kernel choice is bm_bn_gelu_skip_bwd's, so the pair gives its bits for the same sums and n)
+static int bn_gelu_skip_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                                   const float* beta, long long rows, int C, double* sums, float* dgamma, float* dbeta,
+                                   double* part, cudaStream_t st) {
+    BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && sums && dgamma && dbeta && rows > 0 && C > 0);
+    if (!part) BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
+    const bool cs = bn_gelu_vec(g, y, mean, invstd, gamma, beta, C) && C / 4 <= 256 && aligned16(dgamma, dbeta);
+    return bn_gelu_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, cs, sums, dgamma, dbeta, part, st);
+}
+extern "C" int bm_bn_gelu_skip_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd,
+                                          const float* gamma, const float* beta, long long rows, int C, double* sums,
+                                          float* dgamma, float* dbeta, bm_stream_t stream) {
+    return bn_gelu_skip_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, sums, dgamma, dbeta, nullptr, ST(stream));
+}
+extern "C" long long bm_bn_gelu_skip_bwd_reduce_det_workspace(long long rows, int C) {
+    return rows > 0 && C > 0 ? bn_bwd_ws_floats(rows, C) : 0;
+}
+extern "C" int bm_bn_gelu_skip_bwd_reduce_det(const float* g, const float* y, const float* mean, const float* invstd,
+                                              const float* gamma, const float* beta, long long rows, int C, double* sums,
+                                              float* dgamma, float* dbeta, float* workspace, long long workspace_floats,
+                                              bm_stream_t stream) {
+    BM_CHECK_ARG(rows > 0 && C > 0);
+    BM_CHECK_WS(bn_bwd_ws_floats(rows, C));
+    return bn_gelu_skip_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, sums, dgamma, dbeta,
+                                   reinterpret_cast<double*>(workspace), ST(stream));
+}
+extern "C" int bm_bn_gelu_skip_bwd_apply(const float* g, const float* y, const float* mean, const float* invstd,
+                                         const float* gamma, const float* beta, long long rows, int C, const double* sums,
+                                         float* dy, bm_stream_t stream) {
+    BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && sums && dy && rows > 0 && C > 0);
+    const bool cs = bn_gelu_vec(g, y, mean, invstd, gamma, beta, C) && aligned16(dy) && C / 4 <= 256;
+    return bn_gelu_bwd_apply(g, y, mean, invstd, gamma, beta, 1, rows, C, cs, sums, nullptr, nullptr, true, dy, nullptr,
+                             ST(stream));
 }
 
 extern "C" int bm_conv1d_bwd_data(const float* dy, const float* wb, const float* addend, int B, int T, int Cin,
@@ -1072,7 +1147,39 @@ extern "C" int bm_bn_act_skip_fwd(const float* y, const float* mean, const float
     return 0;
 }
 
-// part: NULL (fp64 atomics into sums) or the bn_bwd_ws_floats(rows, C) partials of the deterministic form
+// The BatchNorm + activation backward in its two halves, as bn_gelu_bwd_reduce / bn_gelu_bwd_apply.
+// reduce half: sums [2C], dgamma, dbeta.  part: NULL (fp64 atomics into sums) or the bn_bwd_ws_floats(rows, C) partials of
+// the deterministic form
+static int bn_act_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                             const float* beta, long long rows, int C, int act, float slope, double* sums, float* dgamma,
+                             float* dbeta, double* part, cudaStream_t st) {
+    const int rpb = 128;
+    dim3 grid((unsigned)((rows + rpb - 1) / rpb), (C + 127) / 128);
+    if (part) {
+        bn_act_bwd_reduce_kernel<true><<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, part, rows, C, rpb, act, slope);
+        BM_CHECK_LAUNCH();
+        if (int rc = reduce_rows(part, (long long)grid.x, 2 * C, sums, st)) return rc;
+    } else {
+        BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
+        bn_act_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C, rpb, act, slope);
+        BM_CHECK_LAUNCH();
+    }
+    bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
+// apply half: dy.  counted: n is read from sums[2C] on the device, else n = rows.
+static int bn_act_bwd_apply(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                            const float* beta, int batch_stats, long long rows, int C, int act, float slope,
+                            const double* sums, bool counted, float* dy, cudaStream_t st) {
+    auto* kernel = counted ? bn_act_bwd_apply_kernel<true> : bn_act_bwd_apply_kernel<false>;
+    kernel<<<ew_grid(rows * C), 256, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, (double)rows, batch_stats, dy, rows * C,
+                                              C, act, slope);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
 static int bn_act_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
                            const float* beta, int batch_stats, long long rows, int C, int act, float slope, double* sums,
                            float* dy, float* dgamma, float* dbeta, double* part, cudaStream_t st) {
@@ -1080,26 +1187,10 @@ static int bn_act_skip_bwd(const float* g, const float* y, const float* mean, co
     BM_CHECK_ARG(!mean || (invstd && gamma && beta));
     const bool reduce = mean && bn_bwd_reduces(batch_stats, dgamma, dbeta);
     BM_CHECK_ARG(!reduce || (sums && dgamma && dbeta));
-    if (reduce) {
-        const int rpb = 128;
-        dim3 grid((unsigned)((rows + rpb - 1) / rpb), (C + 127) / 128);
-        if (part) {
-            bn_act_bwd_reduce_kernel<true><<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, part, rows, C, rpb, act,
-                                                                 slope);
-            BM_CHECK_LAUNCH();
-            if (int rc = reduce_rows(part, (long long)grid.x, 2 * C, sums, st)) return rc;
-        } else {
-            BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
-            bn_act_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C, rpb, act, slope);
-            BM_CHECK_LAUNCH();
-        }
-        bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
-        BM_CHECK_LAUNCH();
-    }
-    bn_act_bwd_apply_kernel<<<ew_grid(rows * C), 256, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, (double)rows,
-                                                               batch_stats, dy, rows * C, C, act, slope);
-    BM_CHECK_LAUNCH();
-    return 0;
+    if (reduce)
+        if (int rc = bn_act_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, act, slope, sums, dgamma, dbeta, part, st))
+            return rc;
+    return bn_act_bwd_apply(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, sums, false, dy, st);
 }
 
 extern "C" int bm_bn_act_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd,
@@ -1123,6 +1214,39 @@ extern "C" int bm_bn_act_skip_bwd_det(const float* g, const float* y, const floa
     BM_CHECK_WS(bn_bwd_ws_floats(rows, C));
     return bn_act_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, sums, dy, dgamma, dbeta,
                            reinterpret_cast<double*>(workspace), ST(stream));
+}
+
+// SyncBatchNorm halves of bm_bn_act_skip_bwd with a training-mode BatchNorm
+static int bn_act_skip_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                                  const float* beta, long long rows, int C, int act, float slope, double* sums, float* dgamma,
+                                  float* dbeta, double* part, cudaStream_t st) {
+    BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && sums && dgamma && dbeta && rows > 0 && C > 0 && act >= 0 &&
+                 act <= 2);
+    return bn_act_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, act, slope, sums, dgamma, dbeta, part, st);
+}
+extern "C" int bm_bn_act_skip_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd,
+                                         const float* gamma, const float* beta, long long rows, int C, int act, float slope,
+                                         double* sums, float* dgamma, float* dbeta, bm_stream_t stream) {
+    return bn_act_skip_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, act, slope, sums, dgamma, dbeta, nullptr,
+                                  ST(stream));
+}
+extern "C" long long bm_bn_act_skip_bwd_reduce_det_workspace(long long rows, int C) {
+    return rows > 0 && C > 0 ? bn_bwd_ws_floats(rows, C) : 0;
+}
+extern "C" int bm_bn_act_skip_bwd_reduce_det(const float* g, const float* y, const float* mean, const float* invstd,
+                                             const float* gamma, const float* beta, long long rows, int C, int act,
+                                             float slope, double* sums, float* dgamma, float* dbeta, float* workspace,
+                                             long long workspace_floats, bm_stream_t stream) {
+    BM_CHECK_ARG(rows > 0 && C > 0);
+    BM_CHECK_WS(bn_bwd_ws_floats(rows, C));
+    return bn_act_skip_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, act, slope, sums, dgamma, dbeta,
+                                  reinterpret_cast<double*>(workspace), ST(stream));
+}
+extern "C" int bm_bn_act_skip_bwd_apply(const float* g, const float* y, const float* mean, const float* invstd,
+                                        const float* gamma, const float* beta, long long rows, int C, int act, float slope,
+                                        const double* sums, float* dy, bm_stream_t stream) {
+    BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && sums && dy && rows > 0 && C > 0 && act >= 0 && act <= 2);
+    return bn_act_bwd_apply(g, y, mean, invstd, gamma, beta, 1, rows, C, act, slope, sums, true, dy, ST(stream));
 }
 
 // ---- residual gain (LayerScale / post_skip) on a ConvSequence layer's branch ----------------------------------------------

@@ -73,11 +73,14 @@ __global__ void bn_act_bwd_reduce_kernel(const float* __restrict__ g, const floa
 // backward pass 2: dy = gamma*invstd*(dz - mean(dz) - yhat*mean(dz*yhat))   (training BatchNorm)
 //                  dy = gamma*invstd*dz                                      (eval BatchNorm: use_batch_stats = 0)
 //                  dy = g * act'(y)                                          (no BatchNorm: mean == NULL)
+// COUNTED: n is read from sums[2C] on the device (a SyncBatchNorm group's row count, all-reduced with the sums)
+template <bool COUNTED = false>
 __global__ void bn_act_bwd_apply_kernel(const float* __restrict__ g, const float* __restrict__ y,
                                         const float* __restrict__ mean, const float* __restrict__ invstd,
                                         const float* __restrict__ gamma, const float* __restrict__ beta,
                                         const double* __restrict__ sums, double n, int use_batch_stats,
                                         float* __restrict__ dy, long long total, int C, int act, float slope) {
+    if (COUNTED) n = sums[2 * C];
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
          i += (long long)gridDim.x * blockDim.x) {
         if (!mean) {

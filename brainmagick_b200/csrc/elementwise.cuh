@@ -86,11 +86,14 @@ __global__ void softmax_bwd_kernel(const float* __restrict__ w, const float* __r
 // ------------------------------------------------------------------------------------------------
 // stats[0:C] = sum y, stats[C:2C] = sum y^2 (fp64) over n = B*T rows  ->  mean, invstd (biased var),
 // running stats update with the unbiased variance (momentum), as nn.BatchNorm1d in training mode.
+// COUNTED: n is read from stats[2C] on the device (a SyncBatchNorm group's row count, all-reduced with the sums).
+template <bool COUNTED = false>
 __global__ void bn_finalize_kernel(const double* __restrict__ stats, double n, float eps, float momentum,
                                    float* running_mean, float* running_var, float* __restrict__ mean,
                                    float* __restrict__ invstd, int C) {
     int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
+    if (COUNTED) n = stats[2 * C];
     double m = stats[c] / n;
     double var = stats[C + c] / n - m * m;
     if (var < 0) var = 0;
@@ -185,11 +188,14 @@ __global__ void bn_param_grad_kernel(const double* __restrict__ sums, float* __r
 
 // backward pass 2: dy = gamma*invstd*(dz - mean(dz) - yhat*mean(dz*yhat))
 // eval mode (use_batch_stats = 0): dy = gamma*invstd*dz
+// COUNTED: n is read from sums[2C] on the device (as in bn_finalize_kernel), here and in the other apply kernels
+template <bool COUNTED = false>
 __global__ void bn_gelu_bwd_apply_kernel(const float* __restrict__ g, const float* __restrict__ y,
                                          const float* __restrict__ mean, const float* __restrict__ invstd,
                                          const float* __restrict__ gamma, const float* __restrict__ beta,
                                          const double* __restrict__ sums, double n, int use_batch_stats,
                                          float* __restrict__ dy, long long total, int C) {
+    if (COUNTED) n = sums[2 * C];
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
          i += (long long)gridDim.x * blockDim.x) {
         int c = (int)(i % C);
@@ -479,11 +485,13 @@ __global__ void transpose_nt_kernel(const float* __restrict__ in, float* __restr
 // ------------------------------------------------------------------------------------------------
 // float4 versions (C % 4 == 0, 16-byte aligned rows): one thread owns 4 consecutive channels
 // ------------------------------------------------------------------------------------------------
+template <bool COUNTED = false>
 __global__ void bn_gelu_bwd_apply_v4_kernel(const float4* __restrict__ g, const float4* __restrict__ y,
                                             const float4* __restrict__ mean, const float4* __restrict__ invstd,
                                             const float4* __restrict__ gamma, const float4* __restrict__ beta,
                                             const double* __restrict__ sums, double n, int use_batch_stats,
                                             float4* __restrict__ dy, long long total4, int C) {
+    if (COUNTED) n = sums[2 * C];
     const int C4 = C >> 2;
     const float rn = (float)(1.0 / n);
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total4;
@@ -652,18 +660,30 @@ bn_gelu_bwd_reduce_cs_kernel(const float* __restrict__ g, const float* __restric
 }
 
 // backward pass 2: dy = gamma*invstd*(dz - mean(dz) - yhat*mean(dz*yhat)); the two means come as dbeta/n and dgamma/n
-// (written by bn_param_grad_kernel from the fp64 sums); eval mode (use_batch_stats = 0): dy = gamma*invstd*dz
+// (written by bn_param_grad_kernel from the fp64 sums); eval mode (use_batch_stats = 0): dy = gamma*invstd*dz.
+// COUNTED: the two sums are rounded from `sums` [2C + 1] here and rn = (float)(1 / sums[2C]) -- the same bits as the
+// float sums of bn_param_grad_kernel and the host's (float)(1.0 / (double)rows) for the same row count.
+template <bool COUNTED = false>
 __global__ void __launch_bounds__(320, 2)
 bn_gelu_bwd_apply_cs_kernel(const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ mean,
                             const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta,
-                            const float* __restrict__ dgamma, const float* __restrict__ dbeta, float rn, int use_batch_stats,
-                            float* __restrict__ dy, long long rows, int C, unsigned int* __restrict__ amax) {
+                            const float* __restrict__ dgamma, const float* __restrict__ dbeta, const double* __restrict__ sums,
+                            float rn, int use_batch_stats, float* __restrict__ dy, long long rows, int C,
+                            unsigned int* __restrict__ amax) {
     const int c = threadIdx.x * 4, RY = blockDim.y;
     const float4 mu = ld4(mean + c), is = ld4(invstd + c), ga = ld4(gamma + c), be = ld4(beta + c);
     float am = 0.f;
     float4 m1 = make_float4(0.f, 0.f, 0.f, 0.f), m2 = m1;
     if (use_batch_stats) {
-        const float4 db = ld4(dbeta + c), dg = ld4(dgamma + c);
+        float4 db, dg;
+        if (COUNTED) {
+            rn = (float)(1.0 / sums[2 * C]);
+            db = make_float4((float)sums[c], (float)sums[c + 1], (float)sums[c + 2], (float)sums[c + 3]);
+            dg = make_float4((float)sums[C + c], (float)sums[C + c + 1], (float)sums[C + c + 2], (float)sums[C + c + 3]);
+        } else {
+            db = ld4(dbeta + c);
+            dg = ld4(dgamma + c);
+        }
         m1 = make_float4(db.x * rn, db.y * rn, db.z * rn, db.w * rn);
         m2 = make_float4(dg.x * rn, dg.y * rn, dg.z * rn, dg.w * rn);
     }

@@ -1,7 +1,7 @@
 """Multi-GPU plumbing (one process per GPU, torch.distributed/NCCL over NVLink).
 
-The path shards by batch row (SURVEY.md 8(e)): each rank encodes its rows (BatchNorm statistics stay per-rank,
-like the reference which never converts to SyncBatchNorm), then
+The path shards by batch row (SURVEY.md 8(e)): each rank encodes its rows (BatchNorm statistics per rank, or over the
+process group for layers converted with torch.nn.SyncBatchNorm.convert_sync_batchnorm, see functional.bn_sync_groups), then
   * `all_gather_candidates`: the ONE forward exchange -- NCCL all-gather of the candidate block so every rank
     scores its rows against the global batch (new semantic; the reference keeps negatives local, README.md:139-143);
   * `all_gather_candidates_with_grad`: the same exchange when a trainable feature model produced the candidates --

@@ -17,6 +17,7 @@ import dataclasses
 import typing as tp
 
 import torch
+import torch.distributed as dist
 
 from . import _lib
 from ._lib import call, ptr, stream
@@ -33,7 +34,10 @@ class SequencePlan:
 
     `residual[k]` = (rewrite, scale, post_skip) of layer k (None: no layer has one): a 1x1 conv + LeakyReLU(rewrite_slope)
     after the activation, then the LayerScale gain (its factor `scale_boost`) and the depthwise post_skip gain, in front of
-    the residual add (common.py:123-130).  A layer with any of them takes `layer_width(plan, k)` = 8 parameters."""
+    the residual add (common.py:123-130).  A layer with any of them takes `layer_width(plan, k)` = 8 parameters.
+
+    `bn_groups[k]`: the process group layer k's BatchNorm takes its statistics over (an nn.SyncBatchNorm, see
+    `bn_sync_groups`), None where the layer uses its own rows (None: no layer syncs)."""
     dilations: tp.List[int]
     glu_after: tp.List[bool]
     has_act: tp.List[bool]            # layer k ends with (BatchNorm +) activation (activation_on_last, common.py:112)
@@ -50,6 +54,37 @@ class SequencePlan:
     residual: tp.Optional[tp.List[tp.Tuple[bool, bool, bool]]] = dataclasses.field(default=None, kw_only=True)
     rewrite_slope: float = dataclasses.field(default=0.0, kw_only=True)
     scale_boost: float = dataclasses.field(default=5.0, kw_only=True)
+    bn_groups: tp.Optional[tp.List[tp.Any]] = dataclasses.field(default=None, kw_only=True)
+
+
+def bn_sync_groups(bns, residual=None):
+    """The plan's `bn_groups` from layer k's BatchNorm module bns[k] (None: the layer has none): torch's SyncBatchNorm rule
+    (`need_sync` in torch/nn/modules/batchnorm.py) -- an nn.SyncBatchNorm in training mode, torch.distributed initialised
+    and more than one rank in its process_group (None: WORLD) takes the group's statistics; every other layer its own.
+    -> the per-layer groups, or None when no layer syncs.  `residual`: the plan's residual-branch flags; a syncing layer
+    with a LayerScale or post_skip gain raises (its BatchNorm backward runs inside bm_bn_act_gain_skip_bwd)."""
+    if not (dist.is_available() and dist.is_initialized()):
+        return None
+    groups = []
+    for k, bn in enumerate(bns):
+        group = None
+        if isinstance(bn, torch.nn.SyncBatchNorm) and bn.training:
+            pg = bn.process_group if bn.process_group else dist.group.WORLD
+            if dist.get_world_size(pg) > 1:
+                group = pg
+        if group is not None and residual is not None and (residual[k][1] or residual[k][2]):
+            raise NotImplementedError("SyncBatchNorm on a ConvSequence layer with a LayerScale (scale) or post_skip gain")
+        groups.append(group)
+    return groups if any(g is not None for g in groups) else None
+
+
+def _sync_bn_sums(buf, C, rows, group):
+    """All-reduce (sum) over `group` of a SyncBatchNorm layer's fp64 column sums buf[:2C], with this rank's row count in
+    buf[2C]: the group's count (per-rank batches may be ragged) travels in the same collective, and the `_counted` /
+    `_apply` kernels read it on the device, so the host never waits for it."""
+    head = buf[:2 * C + 1]
+    head[2 * C].fill_(float(rows))
+    dist.all_reduce(head, group=group)
 
 
 def layer_width(plan: SequencePlan, k: int) -> int:
@@ -473,7 +508,8 @@ def conv_stack_forward(plan: SequencePlan, x, conv0: _Conv, conv_p, glu_p, nd: "
     st = stream()
     rows = B * T
     tc = plan.use_tensor_cores
-    stats = _empty((2 * max(p[0].shape[0] for p in conv_p),), x, torch.float64)
+    # a syncing layer's count goes into slot 2C of its sums (`_sync_bn_sums`)
+    stats = _empty((2 * max(p[0].shape[0] for p in conv_p) + (1 if plan.bn_groups else 0),), x, torch.float64)
     layers = []
     for k, p in enumerate(conv_p):
         w, b, gamma, beta = p[:4]
@@ -487,7 +523,14 @@ def conv_stack_forward(plan: SequencePlan, x, conv0: _Conv, conv_p, glu_p, nd: "
         if has_bn:
             mean, invstd = _empty((cout,), x), _empty((cout,), x)
             rm, rv = plan.bn_buffers[k]
-            if plan.training:
+            group = plan.bn_groups[k] if plan.bn_groups else None
+            if plan.training and group is not None:
+                # SyncBatchNorm: one all-reduce per layer, issued whatever the data, so every rank issues the same ones
+                conv.forward(x, b.contiguous(), B, T, plan.dilations[k], y, stats, status)
+                _sync_bn_sums(stats, cout, rows, group)
+                call("bm_bn_stats_finalize_counted", ptr(stats), float(plan.bn_eps), float(plan.bn_momentum), ptr(rm),
+                     ptr(rv), ptr(mean), ptr(invstd), cout, st)
+            elif plan.training:
                 conv.forward(x, b.contiguous(), B, T, plan.dilations[k], y, stats, status)
                 call("bm_bn_stats_finalize", ptr(stats), rows, float(plan.bn_eps), float(plan.bn_momentum),
                      ptr(rm), ptr(rv), ptr(mean), ptr(invstd), cout, st)
@@ -540,7 +583,7 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
     st = stream()
     rows = B * T
     like = status                                   # allocations only read the device off it
-    sums = _empty((2 * max(p[0].shape[0] for p in conv_p),), like, torch.float64)
+    sums = _empty((2 * max(p[0].shape[0] for p in conv_p) + (1 if plan.bn_groups else 0),), like, torch.float64)
     sums3 = _empty((3 * max(p[0].shape[0] for p in conv_p),), like, torch.float64) if plan.residual else None
     layer_grads: tp.List[tp.Any] = [(None,) * len(p) for p in conv_p]
     glu_grads = {k: (None, None) for k in nd.glu}
@@ -582,8 +625,25 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
             if dy is None and g_act is None:        # nothing below the residual-branch options needs a gradient
                 layer_grads[k] = (None, None, None, None) + opt_grads
                 continue
+        group = plan.bn_groups[k] if plan.bn_groups else None
         if dy is not None:
             pass                                    # the gain kernel ran the BatchNorm / activation backward
+        elif rec["has_bn"] and group is not None:
+            # SyncBatchNorm (torch's SyncBatchNorm backward): dgamma / dbeta from the local sums; the data gradient, when
+            # the layer's input needs one (torch's needs_input_grad[0]), from the group's sums after their all-reduce.
+            # Whether that all-reduce is issued depends on requires_grad flags only, never on data, so every rank issues
+            # the same collectives in the same order (DESIGN 4.1).
+            dgamma, dbeta = _empty((cout,), like), _empty((cout,), like)
+            gelu = rec["act"] == ACT_GELU
+            name = "bm_bn_gelu_skip_bwd" if gelu else "bm_bn_act_skip_bwd"
+            gm, bt = gamma.contiguous(), beta.contiguous()
+            args = (ptr(g_act), ptr(rec["y"]), ptr(rec["mean"]), ptr(rec["invstd"]), ptr(gm), ptr(bt), rows, cout) + \
+                (() if gelu else (rec["act"], float(plan.act_slope)))
+            _reducing_call(name + "_reduce", like, (rows, cout), *args, ptr(sums), ptr(dgamma), ptr(dbeta), st)
+            if n_cw or n_cb or nd.below[k]:
+                _sync_bn_sums(sums, cout, rows, group)
+                dy = _empty((B, T, cout), like)
+                call(name + "_apply", *args, ptr(sums), ptr(dy), st)
         elif rec["has_bn"]:
             # the batch statistics' backward reduces in training mode; in eval mode only for trainable gamma / beta (else
             # the BatchNorm + activation backward is one elementwise pass)
@@ -608,8 +668,9 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
             # bare convolution: dL/dy = dL/dx_new.  With a residual, g is accumulated in place below while the weight
             # gradient may still read dy: dy is then a copy
             dy = g.clone() if (rec["skip"] and nd.below[k]) else g
-        # with a training-mode BatchNorm behind the conv, sum(dy) is exactly 0: no bias reduction
-        dcw, dcb = weight_grad(conv, dy, rec["x_in"], plan.dilations[k], rec["has_bn"] and plan.training,
+        # with a training-mode BatchNorm behind the conv, sum(dy) is exactly 0: no bias reduction (a SyncBatchNorm's is 0
+        # summed over the group only)
+        dcw, dcb = weight_grad(conv, dy, rec["x_in"], plan.dilations[k], rec["has_bn"] and plan.training and group is None,
                                want=(n_cw, n_cb))
         if not nd.below[k]:
             pass

@@ -203,6 +203,8 @@ class SimpleConv(nn.Module):
         bn0 = seq.sequence[0][1]
         if bn0.momentum is None:
             raise NotImplementedError("BatchNorm cumulative-average mode (momentum=None)")
+        residual = seq.residual()
+        bn_groups = BF.bn_sync_groups([blk[1] if seq.has_act[k] else None for k, blk in enumerate(seq.sequence)], residual)
         return BF.EncoderPlan(
             dilations=list(seq.dilations), glu_after=seq.glu_after(), kernel_size=seq.kernel,
             glu_kernel=seq.glu_kernel, training=self.training, bn_eps=bn0.eps, bn_momentum=bn0.momentum,
@@ -213,7 +215,7 @@ class SimpleConv(nn.Module):
             bn_buffers=bn_buffers, keep_for_backward=torch.is_grad_enabled(),
             use_tensor_cores=self.use_tensor_cores, skip=seq.skip, act_code=seq.act_code, act_slope=seq.act_slope,
             has_act=list(seq.has_act), batch_norm=True, has_sub_emb=self.subject_embedding is not None,
-            residual=seq.residual(), rewrite_slope=seq.rewrite_slope, scale_boost=seq.scale_boost())
+            residual=residual, rewrite_slope=seq.rewrite_slope, scale_boost=seq.scale_boost(), bn_groups=bn_groups)
 
     def forward(self, inputs, batch):
         meg = inputs["meg"]

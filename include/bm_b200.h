@@ -112,6 +112,10 @@ int bm_conv1d_fwd(const float* x, const float* wf, const float* bias, int B, int
 /* batch statistics -> mean, invstd; updates running stats (nullable) like nn.BatchNorm1d(momentum). */
 int bm_bn_stats_finalize(const double* stats, long long n, float eps, float momentum, float* running_mean,
                          float* running_var, float* mean, float* invstd, int C, bm_stream_t stream);
+/* bm_bn_stats_finalize with n read on the device from stats[2C] (stats fp64 [2C + 1]): the SyncBatchNorm form, whose sums
+ * and row count are all-reduced over the group in one buffer without a host read of the count. */
+int bm_bn_stats_finalize_counted(const double* stats, float eps, float momentum, float* running_mean, float* running_var,
+                                 float* mean, float* invstd, int C, bm_stream_t stream);
 int bm_bn_eval_stats(const float* running_mean, const float* running_var, float eps, float* mean, float* invstd,
                      int C, bm_stream_t stream);
 /* x_new = GELU(gamma*(y-mean)*invstd + beta) (+ x_old if not NULL); rows = B*T.
@@ -131,6 +135,15 @@ int bm_bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, const
                         const float* gamma, const float* beta, int batch_stats, long long rows, int C,
                         double* sums, float* dy, float* dgamma, float* dbeta, float* amax_out /* of dy */,
                         bm_stream_t stream);
+/* bm_bn_gelu_skip_bwd with batch_stats=1 in two calls, so that a SyncBatchNorm caller can all-reduce the sums between them:
+ * _reduce writes sums [2C] = (sum dz, sum dz*yhat) over its rows and the local dbeta / dgamma (their float roundings);
+ * _apply writes dy from sums fp64 [2C + 1], the group's sums with the group's row count n in sums[2C] (read on the device).
+ * With the local sums and n = rows the pair gives bm_bn_gelu_skip_bwd's bits. */
+int bm_bn_gelu_skip_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                               const float* beta, long long rows, int C, double* sums, float* dgamma, float* dbeta,
+                               bm_stream_t stream);
+int bm_bn_gelu_skip_bwd_apply(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                              const float* beta, long long rows, int C, const double* sums, float* dy, bm_stream_t stream);
 /* dx = conv_transpose(dy) (+ addend, the skip-path gradient, if not NULL). */
 int bm_conv1d_bwd_data(const float* dy, const float* wb, const float* addend, int B, int T, int Cin, int Cout,
                        int Kw, int dilation, float* dx, bm_stream_t stream);
@@ -202,6 +215,13 @@ int bm_bn_act_skip_fwd(const float* y, const float* mean, const float* invstd, c
 int bm_bn_act_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
                        const float* beta, int batch_stats, long long rows, int C, int act, float slope, double* sums,
                        float* dy, float* dgamma, float* dbeta, bm_stream_t stream);
+/* bm_bn_act_skip_bwd with a training-mode BatchNorm in two calls, as bm_bn_gelu_skip_bwd_reduce / _apply. */
+int bm_bn_act_skip_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                              const float* beta, long long rows, int C, int act, float slope, double* sums, float* dgamma,
+                              float* dbeta, bm_stream_t stream);
+int bm_bn_act_skip_bwd_apply(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                             const float* beta, long long rows, int C, int act, float slope, const double* sums, float* dy,
+                             bm_stream_t stream);
 /* Residual gain of a ConvSequence layer (LayerScale and post_skip, common.py:65-76,126-130):
  * x_new = post[c] * ((boost * scale[c]) * branch) (+ x_old), branch = act(bn(y)) as in bm_bn_act_skip_fwd; scale [C]
  * (LayerScale's parameter, boost its factor 5) and post [C] (the depthwise 1x1 conv's weight) are each nullable (gain 1).
@@ -404,6 +424,14 @@ int bm_bn_act_skip_bwd_det(const float* g, const float* y, const float* mean, co
                            const float* beta, int batch_stats, long long rows, int C, int act, float slope, double* sums,
                            float* dy, float* dgamma, float* dbeta, float* workspace, long long workspace_floats,
                            bm_stream_t stream);
+long long bm_bn_gelu_skip_bwd_reduce_det_workspace(long long rows, int C);
+int bm_bn_gelu_skip_bwd_reduce_det(const float* g, const float* y, const float* mean, const float* invstd,
+                                   const float* gamma, const float* beta, long long rows, int C, double* sums, float* dgamma,
+                                   float* dbeta, float* workspace, long long workspace_floats, bm_stream_t stream);
+long long bm_bn_act_skip_bwd_reduce_det_workspace(long long rows, int C);
+int bm_bn_act_skip_bwd_reduce_det(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
+                                  const float* beta, long long rows, int C, int act, float slope, double* sums, float* dgamma,
+                                  float* dbeta, float* workspace, long long workspace_floats, bm_stream_t stream);
 /* workspace unused (may be NULL) when nothing is reduced (see bm_bn_act_gain_skip_bwd) */
 long long bm_bn_act_gain_skip_bwd_det_workspace(long long rows, int C);
 int bm_bn_act_gain_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
