@@ -72,8 +72,6 @@ constexpr int COLSUM_RPB = 256, COLSTATS_RPB = 128;
 inline long long blocks_of(long long rows, int rpb) { return (rows + rpb - 1) / rpb; }
 inline long long colsum_ws_floats(long long rows, int C) { return blocks_of(rows, COLSUM_RPB) * C; }
 inline long long colstats_ws_floats(long long rows, int C) { return blocks_of(rows, COLSTATS_RPB) * 4ll * C; }  // fp64 [nb][2C]
-// BatchNorm backward reduce: the column-stationary kernel takes CS_ROWS_PER_BLOCK (96) rows per block, the generic one 128
-inline long long bn_bwd_ws_floats(long long rows, int C) { return blocks_of(rows, CS_ROWS_PER_BLOCK) * 4ll * C; }
 inline long long glu_bwd_ws_floats(long long rows, int H) { return blocks_of(rows, CS_ROWS_PER_BLOCK) * 2ll * H; }
 // batch segments of the split weight-gradient GEMMs (the atomic form's count); planes = segments x output elements
 inline int wgrad_segments(int B, int tiles) {
@@ -482,193 +480,258 @@ static int amax_begin(float* amax_out, cudaStream_t st) {
     return 0;
 }
 
-extern "C" int bm_bn_gelu_skip_fwd(const float* y, const float* mean, const float* invstd, const float* gamma,
-                                   const float* beta, const float* x_old, float* x_new, long long rows, int C,
-                                   float* amax_out, bm_stream_t stream) {
-    BM_CHECK_ARG(y && mean && invstd && gamma && beta && x_new && rows > 0 && C > 0);
-    long long total = rows * C;
-    if (int rc = amax_begin(amax_out, ST(stream))) return rc;
-    bool vec = (C % 4 == 0) && ((reinterpret_cast<uintptr_t>(y) | reinterpret_cast<uintptr_t>(x_new) |
-                                 reinterpret_cast<uintptr_t>(x_old)) % 16 == 0);
-    if (vec && C / 4 <= 256 && aligned16(mean, invstd, gamma) && aligned16(beta)) {
-        const int cx = C / 4, ry = std::max(1, 320 / cx);
-        const unsigned nblk = (unsigned)((rows + CS_ROWS_PER_BLOCK - 1) / CS_ROWS_PER_BLOCK);
-        bn_gelu_skip_fwd_cs_kernel<<<nblk, dim3(cx, ry), 0, ST(stream)>>>(y, mean, invstd, gamma, beta, x_old, x_new, rows, C,
-                                                                          reinterpret_cast<unsigned int*>(amax_out));
-        BM_CHECK_LAUNCH();
-        return 0;
-    }
-    if (vec)
-        bn_gelu_skip_fwd_kernel<4><<<ew_grid(total, 256, 4), 256, 0, ST(stream)>>>(y, mean, invstd, gamma, beta,
-                                                                                 x_old, x_new, total, C);
-    else
-        bn_gelu_skip_fwd_kernel<1><<<ew_grid(total), 256, 0, ST(stream)>>>(y, mean, invstd, gamma, beta, x_old,
-                                                                          x_new, total, C);
+// ---- ConvSequence layer epilogue (convseq.cuh): one implementation behind every bm_bn_gelu_skip_*, bm_bn_act_skip_* and
+// bm_bn_act_gain_skip_* entry point; the column-stationary or the generic kernels by shape and alignment alone ----------------
+struct Epi {
+    const float *mean, *invstd, *gamma, *beta;      // mean == NULL: no BatchNorm
+    int act;
+    float slope;
+    const float *scale = nullptr, *post = nullptr;  // residual gains, NULL = 1
+    float boost = 0.f;
+    bool gain_grads = false;                        // dscale / dpost asked for: S is summed even when both gains are NULL
+    bool bn() const { return mean != nullptr; }
+    bool gain() const { return scale || post || gain_grads; }
+    int width(int C) const { return (gain() ? 3 : 2) * C; }   // fp64 sums: (sum dz, sum dz*yhat[, S = sum g*branch])
+};
+
+// C % 4 == 0 and every operand the call touches 16-byte aligned: the column-stationary kernels up to C / 4 <= 256, above it
+// the float4 form (VEC = 4) of the generic ones
+static bool epi_vec(const Epi& e, int C, std::initializer_list<const void*> ops) {
+    uintptr_t bits = reinterpret_cast<uintptr_t>(e.mean) | reinterpret_cast<uintptr_t>(e.invstd) |
+                     reinterpret_cast<uintptr_t>(e.gamma) | reinterpret_cast<uintptr_t>(e.beta) |
+                     reinterpret_cast<uintptr_t>(e.scale) | reinterpret_cast<uintptr_t>(e.post);
+    for (const void* p : ops) bits |= reinterpret_cast<uintptr_t>(p);
+    return C % 4 == 0 && (bits & 15) == 0;
+}
+static bool epi_cs(const Epi& e, int C, std::initializer_list<const void*> ops) { return epi_vec(e, C, ops) && C / 4 <= 256; }
+static dim3 epi_cs_block(int C) { return dim3(C / 4, std::max(1, 320 / (C / 4))); }
+
+// f(ACT, BN, GAIN) with the epilogue's form as std::integral_constant arguments: the kernels' instantiation
+template <class F>
+static void epi_form(const Epi& e, F&& f) {
+    auto with = [&](auto act) {
+        using T = std::true_type;
+        using N = std::false_type;
+        if (e.bn()) e.gain() ? f(act, T{}, T{}) : f(act, T{}, N{});
+        else e.gain() ? f(act, N{}, T{}) : f(act, N{}, N{});
+    };
+    if (e.act == ACT_GELU) with(std::integral_constant<int, ACT_GELU>{});
+    else if (e.act == ACT_LRELU) with(std::integral_constant<int, ACT_LRELU>{});
+    else with(std::integral_constant<int, ACT_NONE>{});
+}
+#define EPI_T(A, B, G) decltype(A)::value, decltype(B)::value, decltype(G)::value
+
+static int epi_fwd(const float* y, const Epi& e, const float* x_old, float* x_new, long long rows, int C, float* amax_out,
+                   cudaStream_t st) {
+    BM_CHECK_ARG(y && x_new && rows > 0 && C > 0 && e.act >= 0 && e.act <= 2);
+    BM_CHECK_ARG(!e.mean || (e.invstd && e.gamma && e.beta));
+    if (int rc = amax_begin(amax_out, st)) return rc;
+    const bool vec = epi_vec(e, C, {y, x_old, x_new}), cs = vec && C / 4 <= 256;
+    epi_form(e, [&](auto A, auto B, auto G) {
+        if (cs)
+            epi_fwd_cs_kernel<EPI_T(A, B, G)><<<(unsigned)blocks_of(rows, CS_ROWS_PER_BLOCK), epi_cs_block(C), 0, st>>>(
+                y, e.mean, e.invstd, e.gamma, e.beta, x_old, x_new, rows, C, reinterpret_cast<unsigned int*>(amax_out), e.slope,
+                e.scale, e.boost, e.post);
+        else if (vec)
+            epi_fwd_kernel<EPI_T(A, B, G), 4><<<ew_grid(rows * C, 256, 4), 256, 0, st>>>(
+                y, e.mean, e.invstd, e.gamma, e.beta, x_old, x_new, rows * C, C, e.slope, e.scale, e.boost, e.post);
+        else
+            epi_fwd_kernel<EPI_T(A, B, G), 1><<<ew_grid(rows * C), 256, 0, st>>>(
+                y, e.mean, e.invstd, e.gamma, e.beta, x_old, x_new, rows * C, C, e.slope, e.scale, e.boost, e.post);
+    });
     BM_CHECK_LAUNCH();
-    if (amax_out) return tc::launch_amax(x_new, total, amax_out, ST(stream));
+    if (amax_out && !cs) return tc::launch_amax(x_new, rows * C, amax_out, st);
     return 0;
 }
 
-// The BatchNorm + GELU backward in its two halves, which a SyncBatchNorm caller runs as two calls with the all-reduce of the
-// sums between them (bm_bn_gelu_skip_bwd_reduce / _apply); bm_bn_gelu_skip_bwd runs them back to back.
-// cs: the column-stationary kernels (C % 4 == 0, C / 4 <= 256, 16-byte aligned operands), else the generic / float4 ones.
-static bool bn_gelu_vec(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
-                        const float* beta, int C) {
-    return (C % 4 == 0) && aligned16(g, y, mean) && aligned16(invstd, gamma, beta);
-}
-
-// reduce half: sums [2C] = (sum dz, sum dz*yhat) over the call's rows, then dbeta / dgamma = their float roundings.
-// part: NULL (fp64 atomics into sums, zeroed by the caller) or the bn_bwd_ws_floats(rows, C) partials of the deterministic form
-static int bn_gelu_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
-                              const float* beta, long long rows, int C, bool cs, double* sums, float* dgamma, float* dbeta,
-                              double* part, cudaStream_t st) {
-    if (cs) {
-        const int cx = C / 4, ry = std::max(1, 320 / cx);
-        const unsigned nblk = (unsigned)((rows + CS_ROWS_PER_BLOCK - 1) / CS_ROWS_PER_BLOCK);
-        if (part) {
-            bn_gelu_bwd_reduce_cs_kernel<true><<<nblk, dim3(cx, ry), sizeof(float) * 2 * C * ry, st>>>(
-                g, y, mean, invstd, gamma, beta, part, rows, C);
-            BM_CHECK_LAUNCH();
-            if (int rc = reduce_rows(part, (long long)nblk, 2 * C, sums, st)) return rc;
-        } else {
-            bn_gelu_bwd_reduce_cs_kernel<<<nblk, dim3(cx, ry), sizeof(float) * 2 * C * ry, st>>>(g, y, mean, invstd, gamma,
-                                                                                              beta, sums, rows, C);
-            BM_CHECK_LAUNCH();
+// The backward in its two halves, which a SyncBatchNorm caller runs as two calls with the all-reduce of the sums between them
+// (the _reduce / _apply entry points); epi_bwd runs them back to back.
+// reduce half: sums [e.width(C)] over the call's rows, then the parameter gradients (each nullable) from them.
+// part: NULL (fp64 atomics into sums, zeroed here) or the epi_ws_floats partials of the deterministic form: fp64 [nb][W], nb
+// the block count of the column-stationary kernel (CS_ROWS_PER_BLOCK = 96 rows per block; the generic one takes 128)
+inline long long epi_ws_floats(long long rows, int W) { return blocks_of(rows, CS_ROWS_PER_BLOCK) * 2ll * W; }
+static int epi_bwd_reduce(const float* g, const float* y, const Epi& e, long long rows, int C, bool cs, double* sums,
+                          float* dgamma, float* dbeta, float* dscale, float* dpost, double* part, cudaStream_t st) {
+    const int W = e.width(C);
+    if (!part) BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * W, st));
+    double* out = part ? part : sums;
+    const int rpb = cs ? CS_ROWS_PER_BLOCK : 128;   // the generic kernel: one thread per column, 128 rows per block
+    const long long nblk = blocks_of(rows, rpb);
+    epi_form(e, [&](auto A, auto B, auto G) {
+        if constexpr (decltype(B)::value || decltype(G)::value) {   // without either there is nothing to reduce
+            if (cs) {
+                const dim3 block = epi_cs_block(C);
+                auto* kernel = part ? epi_bwd_reduce_cs_kernel<EPI_T(A, B, G), true> : epi_bwd_reduce_cs_kernel<EPI_T(A, B, G)>;
+                kernel<<<(unsigned)nblk, block, sizeof(float) * W * block.y, st>>>(g, y, e.mean, e.invstd, e.gamma, e.beta, out,
+                                                                                 rows, C, e.slope, e.scale, e.boost, e.post);
+            } else {
+                auto* kernel = part ? epi_bwd_reduce_kernel<EPI_T(A, B, G), true> : epi_bwd_reduce_kernel<EPI_T(A, B, G)>;
+                kernel<<<dim3((unsigned)nblk, (C + 127) / 128), 128, 0, st>>>(g, y, e.mean, e.invstd, e.gamma, e.beta, out,
+                                                                             rows, C, rpb, e.slope, e.scale, e.boost, e.post);
+            }
         }
-    } else {   // generic shapes: one thread per column, 128 rows per block
-        const int rpb = 128;
-        dim3 grid((unsigned)((rows + rpb - 1) / rpb), (C + 127) / 128);
-        if (part) {
-            bn_gelu_bwd_reduce_kernel<true><<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, part, rows, C, rpb);
-            BM_CHECK_LAUNCH();
-            if (int rc = reduce_rows(part, (long long)grid.x, 2 * C, sums, st)) return rc;
-        } else {
-            bn_gelu_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C, rpb);
-            BM_CHECK_LAUNCH();
-        }
-    }
-    bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
+    });
+    BM_CHECK_LAUNCH();
+    if (part)
+        if (int rc = reduce_rows(part, nblk, W, sums, st)) return rc;
+    epi_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, C, e.scale, e.boost, e.post, dgamma, dbeta, dscale, dpost);
     BM_CHECK_LAUNCH();
     return 0;
 }
 
 // apply half: dy.  counted: the sums and the row count n come from `sums` [2C + 1] (n in sums[2C], read on the device);
 // else n = rows and the column-stationary kernel takes the sums as dgamma / dbeta.  Both give the same bits for the same n.
-static int bn_gelu_bwd_apply(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
-                             const float* beta, int batch_stats, long long rows, int C, bool cs, const double* sums,
-                             const float* dgamma, const float* dbeta, bool counted, float* dy, float* amax_out,
-                             cudaStream_t st) {
+static int epi_bwd_apply(const float* g, const float* y, const Epi& e, int batch_stats, long long rows, int C, bool cs,
+                         bool vec, const double* sums, const float* dgamma, const float* dbeta, bool counted, float* dy, float* amax_out,
+                         cudaStream_t st) {
     const long long total = rows * C;
-    if (cs) {
-        const int cx = C / 4, ry = std::max(1, 320 / cx);
-        const unsigned nblk = (unsigned)((rows + CS_ROWS_PER_BLOCK - 1) / CS_ROWS_PER_BLOCK);
-        unsigned int* amax = reinterpret_cast<unsigned int*>(amax_out);
-        if (counted)
-            bn_gelu_bwd_apply_cs_kernel<true><<<nblk, dim3(cx, ry), 0, st>>>(g, y, mean, invstd, gamma, beta, nullptr, nullptr,
-                                                                            sums, 0.f, 1, dy, rows, C, amax);
-        else
-            bn_gelu_bwd_apply_cs_kernel<<<nblk, dim3(cx, ry), 0, st>>>(g, y, mean, invstd, gamma, beta, dgamma, dbeta, nullptr,
-                                                                       (float)(1.0 / (double)rows), batch_stats, dy, rows, C,
-                                                                       amax);
-        BM_CHECK_LAUNCH();
-        return 0;
-    }
-    if (bn_gelu_vec(g, y, mean, invstd, gamma, beta, C) && aligned16(dy)) {
-        auto* kernel = counted ? bn_gelu_bwd_apply_v4_kernel<true> : bn_gelu_bwd_apply_v4_kernel<false>;
-        kernel<<<ew_grid(total / 4), 256, 0, st>>>(
-            reinterpret_cast<const float4*>(g), reinterpret_cast<const float4*>(y), reinterpret_cast<const float4*>(mean),
-            reinterpret_cast<const float4*>(invstd), reinterpret_cast<const float4*>(gamma),
-            reinterpret_cast<const float4*>(beta), sums, (double)rows, batch_stats, reinterpret_cast<float4*>(dy),
-            total / 4, C);
-    } else {
-        auto* kernel = counted ? bn_gelu_bwd_apply_kernel<true> : bn_gelu_bwd_apply_kernel<false>;
-        kernel<<<ew_grid(total), 256, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, (double)rows, batch_stats, dy, total, C);
-    }
+    const float rn = (float)(1.0 / (double)rows);
+    unsigned int* amax = reinterpret_cast<unsigned int*>(amax_out);
+    epi_form(e, [&](auto A, auto B, auto G) {
+        const unsigned nblk = (unsigned)blocks_of(rows, CS_ROWS_PER_BLOCK);
+        if (counted) {   // the SyncBatchNorm apply half: a BatchNorm and no gain (epi_bwd_apply_half)
+            if constexpr (decltype(B)::value && !decltype(G)::value) {
+                if (cs)
+                    epi_bwd_apply_cs_kernel<EPI_T(A, B, G), true><<<nblk, epi_cs_block(C), 0, st>>>(
+                        g, y, e.mean, e.invstd, e.gamma, e.beta, nullptr, nullptr, sums, 0.f, 1, dy, rows, C, amax, e.slope,
+                        e.scale, e.boost, e.post);
+                else if (vec)
+                    epi_bwd_apply_kernel<EPI_T(A, B, G), 4, true><<<ew_grid(total, 256, 4), 256, 0, st>>>(
+                        g, y, e.mean, e.invstd, e.gamma, e.beta, sums, 0.0, 1, dy, total, C, e.slope, e.scale, e.boost, e.post);
+                else
+                    epi_bwd_apply_kernel<EPI_T(A, B, G), 1, true><<<ew_grid(total), 256, 0, st>>>(
+                        g, y, e.mean, e.invstd, e.gamma, e.beta, sums, 0.0, 1, dy, total, C, e.slope, e.scale, e.boost, e.post);
+            }
+        } else if (cs) {
+            epi_bwd_apply_cs_kernel<EPI_T(A, B, G)><<<nblk, epi_cs_block(C), 0, st>>>(
+                g, y, e.mean, e.invstd, e.gamma, e.beta, dgamma, dbeta, nullptr, rn, batch_stats, dy, rows, C, amax, e.slope,
+                e.scale, e.boost, e.post);
+        } else if (vec) {
+            epi_bwd_apply_kernel<EPI_T(A, B, G), 4><<<ew_grid(total, 256, 4), 256, 0, st>>>(
+                g, y, e.mean, e.invstd, e.gamma, e.beta, sums, (double)rows, batch_stats, dy, total, C, e.slope, e.scale, e.boost,
+                e.post);
+        } else {
+            epi_bwd_apply_kernel<EPI_T(A, B, G), 1><<<ew_grid(total), 256, 0, st>>>(
+                g, y, e.mean, e.invstd, e.gamma, e.beta, sums, (double)rows, batch_stats, dy, total, C, e.slope, e.scale, e.boost,
+                e.post);
+        }
+    });
     BM_CHECK_LAUNCH();
-    if (amax_out) return tc::launch_amax(dy, total, amax_out, st);
+    if (amax_out && !cs) return tc::launch_amax(dy, total, amax_out, st);
     return 0;
 }
 
-// The column reduction (sums, dgamma, dbeta) runs unless batch_stats == 0 and dgamma == dbeta == NULL: the data gradient of an
-// eval-mode BatchNorm whose affine parameters are frozen is then one elementwise pass (the apply kernels read the sums / dgamma /
-// dbeta only when use_batch_stats is set, so its dy is bitwise the reducing form's).
-static bool bn_bwd_reduces(int batch_stats, const float* dgamma, const float* dbeta) {
-    return batch_stats || dgamma || dbeta;
+// The BatchNorm sums are reduced unless batch_stats == 0 and dgamma == dbeta == NULL: the data gradient of an eval-mode
+// BatchNorm whose affine parameters are frozen is then one elementwise pass (the apply kernels read the sums / dgamma / dbeta
+// only when use_batch_stats is set, so its dy is bitwise the reducing form's).  The gains' S is reduced for dscale / dpost.
+static bool epi_bn_reduces(const Epi& e, int batch_stats, const float* dgamma, const float* dbeta) {
+    return e.bn() && (batch_stats || dgamma || dbeta);
 }
 
-// part: NULL (fp64 atomics into sums) or the bn_bwd_ws_floats(rows, C) partials of the deterministic form
-static int bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
-                            const float* beta, int batch_stats, long long rows, int C, double* sums, float* dy, float* dgamma,
-                            float* dbeta, float* amax_out, double* part, cudaStream_t st) {
-    BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && dy && rows > 0 && C > 0);
-    const bool reduce = bn_bwd_reduces(batch_stats, dgamma, dbeta);
-    BM_CHECK_ARG(!reduce || (sums && dgamma && dbeta));
-    if (reduce && !part) BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
+// part: NULL (fp64 atomics into sums) or the epi_ws_floats partials of the deterministic form
+static int epi_bwd(const float* g, const float* y, const Epi& e, int batch_stats, long long rows, int C, double* sums,
+                   float* dy, float* dgamma, float* dbeta, float* dscale, float* dpost, float* amax_out, double* part,
+                   cudaStream_t st) {
+    BM_CHECK_ARG(g && y && dy && rows > 0 && C > 0 && e.act >= 0 && e.act <= 2);
+    BM_CHECK_ARG(!e.mean || (e.invstd && e.gamma && e.beta));
+    const bool bn_reduce = epi_bn_reduces(e, batch_stats, dgamma, dbeta);
+    BM_CHECK_ARG(!bn_reduce || (dgamma && dbeta));
+    const bool reduce = bn_reduce || dscale || dpost;
+    BM_CHECK_ARG(!reduce || sums);
     if (int rc = amax_begin(amax_out, st)) return rc;
-    const bool cs = bn_gelu_vec(g, y, mean, invstd, gamma, beta, C) && aligned16(dy) && C / 4 <= 256 &&
-                    aligned16(dgamma, dbeta);
+    const bool vec = epi_vec(e, C, {g, y, dy, dgamma, dbeta}), cs = vec && C / 4 <= 256;
     if (reduce)
-        if (int rc = bn_gelu_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, cs, sums, dgamma, dbeta, part, st)) return rc;
-    return bn_gelu_bwd_apply(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, cs, sums, dgamma, dbeta, false, dy,
-                             amax_out, st);
+        if (int rc = epi_bwd_reduce(g, y, e, rows, C, cs, sums, bn_reduce ? dgamma : nullptr, bn_reduce ? dbeta : nullptr,
+                                    dscale, dpost, part, st))
+            return rc;
+    return epi_bwd_apply(g, y, e, bn_reduce && batch_stats, rows, C, cs, vec, sums, dgamma, dbeta, false, dy, amax_out, st);
 }
 
+// the deterministic form: the workspace is used (and checked) only when something is reduced
+static int epi_bwd_det(const float* g, const float* y, const Epi& e, int batch_stats, long long rows, int C, double* sums,
+                       float* dy, float* dgamma, float* dbeta, float* dscale, float* dpost, float* amax_out, float* workspace,
+                       long long workspace_floats, cudaStream_t st) {
+    BM_CHECK_ARG(rows > 0 && C > 0);
+    double* part = nullptr;
+    if (epi_bn_reduces(e, batch_stats, dgamma, dbeta) || dscale || dpost) {
+        BM_CHECK_WS(epi_ws_floats(rows, e.width(C)));
+        part = reinterpret_cast<double*>(workspace);
+    }
+    return epi_bwd(g, y, e, batch_stats, rows, C, sums, dy, dgamma, dbeta, dscale, dpost, amax_out, part, st);
+}
+
+// SyncBatchNorm halves of epi_bwd with a training-mode BatchNorm and no gain (the kernel choice is epi_bwd's, so the pair
+// gives its bits for the same sums and n)
+static int epi_bwd_reduce_half(const float* g, const float* y, const Epi& e, long long rows, int C, double* sums, float* dgamma,
+                               float* dbeta, double* part, cudaStream_t st) {
+    BM_CHECK_ARG(g && y && e.mean && e.invstd && e.gamma && e.beta && sums && dgamma && dbeta && rows > 0 && C > 0 &&
+                 e.act >= 0 && e.act <= 2);
+    return epi_bwd_reduce(g, y, e, rows, C, epi_cs(e, C, {g, y, dgamma, dbeta}), sums, dgamma, dbeta, nullptr, nullptr, part,
+                          st);
+}
+static int epi_bwd_reduce_half_det(const float* g, const float* y, const Epi& e, long long rows, int C, double* sums,
+                                   float* dgamma, float* dbeta, float* workspace, long long workspace_floats, cudaStream_t st) {
+    BM_CHECK_ARG(rows > 0 && C > 0);
+    BM_CHECK_WS(epi_ws_floats(rows, 2 * C));
+    return epi_bwd_reduce_half(g, y, e, rows, C, sums, dgamma, dbeta, reinterpret_cast<double*>(workspace), st);
+}
+static int epi_bwd_apply_half(const float* g, const float* y, const Epi& e, long long rows, int C, const double* sums,
+                              float* dy, cudaStream_t st) {
+    BM_CHECK_ARG(g && y && e.mean && e.invstd && e.gamma && e.beta && sums && dy && rows > 0 && C > 0 && e.act >= 0 &&
+                 e.act <= 2);
+    const bool vec = epi_vec(e, C, {g, y, dy});
+    return epi_bwd_apply(g, y, e, 1, rows, C, vec && C / 4 <= 256, vec, sums, nullptr, nullptr, true, dy, nullptr, st);
+}
+
+// BatchNorm + GELU (SimpleConv's layers): the BatchNorm is required
+extern "C" int bm_bn_gelu_skip_fwd(const float* y, const float* mean, const float* invstd, const float* gamma,
+                                   const float* beta, const float* x_old, float* x_new, long long rows, int C,
+                                   float* amax_out, bm_stream_t stream) {
+    BM_CHECK_ARG(mean);
+    const Epi e{mean, invstd, gamma, beta, ACT_GELU, 0.f};
+    return epi_fwd(y, e, x_old, x_new, rows, C, amax_out, ST(stream));
+}
 extern "C" int bm_bn_gelu_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd,
                                    const float* gamma, const float* beta, int batch_stats, long long rows, int C,
                                    double* sums, float* dy, float* dgamma, float* dbeta, float* amax_out,
                                    bm_stream_t stream) {
-    return bn_gelu_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, sums, dy, dgamma, dbeta, amax_out, nullptr,
-                            ST(stream));
+    BM_CHECK_ARG(mean);
+    const Epi e{mean, invstd, gamma, beta, ACT_GELU, 0.f};
+    return epi_bwd(g, y, e, batch_stats, rows, C, sums, dy, dgamma, dbeta, nullptr, nullptr, amax_out, nullptr, ST(stream));
 }
 extern "C" long long bm_bn_gelu_skip_bwd_det_workspace(long long rows, int C) {
-    return rows > 0 && C > 0 ? bn_bwd_ws_floats(rows, C) : 0;
+    return rows > 0 && C > 0 ? epi_ws_floats(rows, 2 * C) : 0;
 }
 extern "C" int bm_bn_gelu_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd,
                                        const float* gamma, const float* beta, int batch_stats, long long rows, int C,
                                        double* sums, float* dy, float* dgamma, float* dbeta, float* amax_out,
                                        float* workspace, long long workspace_floats, bm_stream_t stream) {
-    BM_CHECK_ARG(rows > 0 && C > 0);
-    if (!bn_bwd_reduces(batch_stats, dgamma, dbeta))     // one elementwise pass: nothing is reduced, no workspace
-        return bn_gelu_skip_bwd(g, y, mean, invstd, gamma, beta, 0, rows, C, sums, dy, nullptr, nullptr, amax_out, nullptr,
-                                ST(stream));
-    BM_CHECK_WS(bn_bwd_ws_floats(rows, C));
-    return bn_gelu_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, sums, dy, dgamma, dbeta, amax_out,
-                            reinterpret_cast<double*>(workspace), ST(stream));
-}
-
-// SyncBatchNorm halves (the kernel choice is bm_bn_gelu_skip_bwd's, so the pair gives its bits for the same sums and n)
-static int bn_gelu_skip_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
-                                   const float* beta, long long rows, int C, double* sums, float* dgamma, float* dbeta,
-                                   double* part, cudaStream_t st) {
-    BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && sums && dgamma && dbeta && rows > 0 && C > 0);
-    if (!part) BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
-    const bool cs = bn_gelu_vec(g, y, mean, invstd, gamma, beta, C) && C / 4 <= 256 && aligned16(dgamma, dbeta);
-    return bn_gelu_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, cs, sums, dgamma, dbeta, part, st);
+    BM_CHECK_ARG(mean);
+    const Epi e{mean, invstd, gamma, beta, ACT_GELU, 0.f};
+    return epi_bwd_det(g, y, e, batch_stats, rows, C, sums, dy, dgamma, dbeta, nullptr, nullptr, amax_out, workspace,
+                       workspace_floats, ST(stream));
 }
 extern "C" int bm_bn_gelu_skip_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd,
                                           const float* gamma, const float* beta, long long rows, int C, double* sums,
                                           float* dgamma, float* dbeta, bm_stream_t stream) {
-    return bn_gelu_skip_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, sums, dgamma, dbeta, nullptr, ST(stream));
+    const Epi e{mean, invstd, gamma, beta, ACT_GELU, 0.f};
+    return epi_bwd_reduce_half(g, y, e, rows, C, sums, dgamma, dbeta, nullptr, ST(stream));
 }
 extern "C" long long bm_bn_gelu_skip_bwd_reduce_det_workspace(long long rows, int C) {
-    return rows > 0 && C > 0 ? bn_bwd_ws_floats(rows, C) : 0;
+    return rows > 0 && C > 0 ? epi_ws_floats(rows, 2 * C) : 0;
 }
 extern "C" int bm_bn_gelu_skip_bwd_reduce_det(const float* g, const float* y, const float* mean, const float* invstd,
                                               const float* gamma, const float* beta, long long rows, int C, double* sums,
                                               float* dgamma, float* dbeta, float* workspace, long long workspace_floats,
                                               bm_stream_t stream) {
-    BM_CHECK_ARG(rows > 0 && C > 0);
-    BM_CHECK_WS(bn_bwd_ws_floats(rows, C));
-    return bn_gelu_skip_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, sums, dgamma, dbeta,
-                                   reinterpret_cast<double*>(workspace), ST(stream));
+    const Epi e{mean, invstd, gamma, beta, ACT_GELU, 0.f};
+    return epi_bwd_reduce_half_det(g, y, e, rows, C, sums, dgamma, dbeta, workspace, workspace_floats, ST(stream));
 }
 extern "C" int bm_bn_gelu_skip_bwd_apply(const float* g, const float* y, const float* mean, const float* invstd,
                                          const float* gamma, const float* beta, long long rows, int C, const double* sums,
                                          float* dy, bm_stream_t stream) {
-    BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && sums && dy && rows > 0 && C > 0);
-    const bool cs = bn_gelu_vec(g, y, mean, invstd, gamma, beta, C) && aligned16(dy) && C / 4 <= 256;
-    return bn_gelu_bwd_apply(g, y, mean, invstd, gamma, beta, 1, rows, C, cs, sums, nullptr, nullptr, true, dy, nullptr,
-                             ST(stream));
+    const Epi e{mean, invstd, gamma, beta, ACT_GELU, 0.f};
+    return epi_bwd_apply_half(g, y, e, rows, C, sums, dy, ST(stream));
 }
 
 extern "C" int bm_conv1d_bwd_data(const float* dy, const float* wb, const float* addend, int B, int T, int Cin,
@@ -1134,194 +1197,81 @@ BM_TC_FORMS(bm_clip_loss_bwd, clip_loss_bwd,
             (probs, inv_norm, cand, gout, Bn, Bc, KT, target_offset, G, dest, status, stream))
 
 // =================================================================================================
-// Stand-alone ConvSequence epilogues + candidate-side ClipLoss gradient (SURVEY 8(f) row 3: DeepMel)
+// Stand-alone ConvSequence epilogues (the forms of epi_fwd / epi_bwd above) + candidate-side ClipLoss gradient (SURVEY 8(f)
+// row 3: DeepMel)
 // =================================================================================================
+// any activation, BatchNorm optional (mean == NULL), with or without the residual gains
 extern "C" int bm_bn_act_skip_fwd(const float* y, const float* mean, const float* invstd, const float* gamma,
                                   const float* beta, const float* x_old, float* x_new, long long rows, int C, int act,
                                   float slope, bm_stream_t stream) {
-    BM_CHECK_ARG(y && x_new && rows > 0 && C > 0 && act >= 0 && act <= 2);
-    BM_CHECK_ARG(!mean || (invstd && gamma && beta));
-    bn_act_skip_fwd_kernel<<<ew_grid(rows * C), 256, 0, ST(stream)>>>(y, mean, invstd, gamma, beta, x_old, x_new,
-                                                                      rows * C, C, act, slope);
-    BM_CHECK_LAUNCH();
-    return 0;
+    const Epi e{mean, invstd, gamma, beta, act, slope};
+    return epi_fwd(y, e, x_old, x_new, rows, C, nullptr, ST(stream));
 }
-
-// The BatchNorm + activation backward in its two halves, as bn_gelu_bwd_reduce / bn_gelu_bwd_apply.
-// reduce half: sums [2C], dgamma, dbeta.  part: NULL (fp64 atomics into sums) or the bn_bwd_ws_floats(rows, C) partials of
-// the deterministic form
-static int bn_act_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
-                             const float* beta, long long rows, int C, int act, float slope, double* sums, float* dgamma,
-                             float* dbeta, double* part, cudaStream_t st) {
-    const int rpb = 128;
-    dim3 grid((unsigned)((rows + rpb - 1) / rpb), (C + 127) / 128);
-    if (part) {
-        bn_act_bwd_reduce_kernel<true><<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, part, rows, C, rpb, act, slope);
-        BM_CHECK_LAUNCH();
-        if (int rc = reduce_rows(part, (long long)grid.x, 2 * C, sums, st)) return rc;
-    } else {
-        BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * C, st));
-        bn_act_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C, rpb, act, slope);
-        BM_CHECK_LAUNCH();
-    }
-    bn_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, dgamma, dbeta, C);
-    BM_CHECK_LAUNCH();
-    return 0;
-}
-
-// apply half: dy.  counted: n is read from sums[2C] on the device, else n = rows.
-static int bn_act_bwd_apply(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
-                            const float* beta, int batch_stats, long long rows, int C, int act, float slope,
-                            const double* sums, bool counted, float* dy, cudaStream_t st) {
-    auto* kernel = counted ? bn_act_bwd_apply_kernel<true> : bn_act_bwd_apply_kernel<false>;
-    kernel<<<ew_grid(rows * C), 256, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, (double)rows, batch_stats, dy, rows * C,
-                                              C, act, slope);
-    BM_CHECK_LAUNCH();
-    return 0;
-}
-
-static int bn_act_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
-                           const float* beta, int batch_stats, long long rows, int C, int act, float slope, double* sums,
-                           float* dy, float* dgamma, float* dbeta, double* part, cudaStream_t st) {
-    BM_CHECK_ARG(g && y && dy && rows > 0 && C > 0 && act >= 0 && act <= 2);
-    BM_CHECK_ARG(!mean || (invstd && gamma && beta));
-    const bool reduce = mean && bn_bwd_reduces(batch_stats, dgamma, dbeta);
-    BM_CHECK_ARG(!reduce || (sums && dgamma && dbeta));
-    if (reduce)
-        if (int rc = bn_act_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, act, slope, sums, dgamma, dbeta, part, st))
-            return rc;
-    return bn_act_bwd_apply(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, sums, false, dy, st);
-}
-
 extern "C" int bm_bn_act_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd,
                                   const float* gamma, const float* beta, int batch_stats, long long rows, int C,
                                   int act, float slope, double* sums, float* dy, float* dgamma, float* dbeta,
                                   bm_stream_t stream) {
-    return bn_act_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, sums, dy, dgamma, dbeta, nullptr,
-                           ST(stream));
+    const Epi e{mean, invstd, gamma, beta, act, slope};
+    return epi_bwd(g, y, e, batch_stats, rows, C, sums, dy, dgamma, dbeta, nullptr, nullptr, nullptr, nullptr, ST(stream));
 }
 extern "C" long long bm_bn_act_skip_bwd_det_workspace(long long rows, int C) {
-    return rows > 0 && C > 0 ? bn_bwd_ws_floats(rows, C) : 0;
+    return rows > 0 && C > 0 ? epi_ws_floats(rows, 2 * C) : 0;
 }
 extern "C" int bm_bn_act_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd,
                                       const float* gamma, const float* beta, int batch_stats, long long rows, int C,
                                       int act, float slope, double* sums, float* dy, float* dgamma, float* dbeta,
                                       float* workspace, long long workspace_floats, bm_stream_t stream) {
-    BM_CHECK_ARG(rows > 0 && C > 0);
-    if (!mean || !bn_bwd_reduces(batch_stats, dgamma, dbeta))   // nothing is reduced, the workspace is not used
-        return bn_act_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, sums, dy, dgamma, dbeta,
-                               nullptr, ST(stream));
-    BM_CHECK_WS(bn_bwd_ws_floats(rows, C));
-    return bn_act_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, sums, dy, dgamma, dbeta,
-                           reinterpret_cast<double*>(workspace), ST(stream));
-}
-
-// SyncBatchNorm halves of bm_bn_act_skip_bwd with a training-mode BatchNorm
-static int bn_act_skip_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
-                                  const float* beta, long long rows, int C, int act, float slope, double* sums, float* dgamma,
-                                  float* dbeta, double* part, cudaStream_t st) {
-    BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && sums && dgamma && dbeta && rows > 0 && C > 0 && act >= 0 &&
-                 act <= 2);
-    return bn_act_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, act, slope, sums, dgamma, dbeta, part, st);
+    const Epi e{mean, invstd, gamma, beta, act, slope};
+    return epi_bwd_det(g, y, e, batch_stats, rows, C, sums, dy, dgamma, dbeta, nullptr, nullptr, nullptr, workspace,
+                       workspace_floats, ST(stream));
 }
 extern "C" int bm_bn_act_skip_bwd_reduce(const float* g, const float* y, const float* mean, const float* invstd,
                                          const float* gamma, const float* beta, long long rows, int C, int act, float slope,
                                          double* sums, float* dgamma, float* dbeta, bm_stream_t stream) {
-    return bn_act_skip_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, act, slope, sums, dgamma, dbeta, nullptr,
-                                  ST(stream));
+    const Epi e{mean, invstd, gamma, beta, act, slope};
+    return epi_bwd_reduce_half(g, y, e, rows, C, sums, dgamma, dbeta, nullptr, ST(stream));
 }
 extern "C" long long bm_bn_act_skip_bwd_reduce_det_workspace(long long rows, int C) {
-    return rows > 0 && C > 0 ? bn_bwd_ws_floats(rows, C) : 0;
+    return rows > 0 && C > 0 ? epi_ws_floats(rows, 2 * C) : 0;
 }
 extern "C" int bm_bn_act_skip_bwd_reduce_det(const float* g, const float* y, const float* mean, const float* invstd,
                                              const float* gamma, const float* beta, long long rows, int C, int act,
                                              float slope, double* sums, float* dgamma, float* dbeta, float* workspace,
                                              long long workspace_floats, bm_stream_t stream) {
-    BM_CHECK_ARG(rows > 0 && C > 0);
-    BM_CHECK_WS(bn_bwd_ws_floats(rows, C));
-    return bn_act_skip_bwd_reduce(g, y, mean, invstd, gamma, beta, rows, C, act, slope, sums, dgamma, dbeta,
-                                  reinterpret_cast<double*>(workspace), ST(stream));
+    const Epi e{mean, invstd, gamma, beta, act, slope};
+    return epi_bwd_reduce_half_det(g, y, e, rows, C, sums, dgamma, dbeta, workspace, workspace_floats, ST(stream));
 }
 extern "C" int bm_bn_act_skip_bwd_apply(const float* g, const float* y, const float* mean, const float* invstd,
                                         const float* gamma, const float* beta, long long rows, int C, int act, float slope,
                                         const double* sums, float* dy, bm_stream_t stream) {
-    BM_CHECK_ARG(g && y && mean && invstd && gamma && beta && sums && dy && rows > 0 && C > 0 && act >= 0 && act <= 2);
-    return bn_act_bwd_apply(g, y, mean, invstd, gamma, beta, 1, rows, C, act, slope, sums, true, dy, ST(stream));
+    const Epi e{mean, invstd, gamma, beta, act, slope};
+    return epi_bwd_apply_half(g, y, e, rows, C, sums, dy, ST(stream));
 }
-
-// ---- residual gain (LayerScale / post_skip) on a ConvSequence layer's branch ----------------------------------------------
 extern "C" int bm_bn_act_gain_skip_fwd(const float* y, const float* mean, const float* invstd, const float* gamma,
                                        const float* beta, const float* x_old, float* x_new, long long rows, int C, int act,
                                        float slope, const float* scale, float boost, const float* post, bm_stream_t stream) {
-    BM_CHECK_ARG(y && x_new && rows > 0 && C > 0 && act >= 0 && act <= 2);
-    BM_CHECK_ARG(!mean || (invstd && gamma && beta));
-    act_gain_skip_fwd_kernel<<<ew_grid(rows * C), 256, 0, ST(stream)>>>(y, mean, invstd, gamma, beta, x_old, x_new, rows * C,
-                                                                        C, act, slope, scale, boost, post);
-    BM_CHECK_LAUNCH();
-    return 0;
+    const Epi e{mean, invstd, gamma, beta, act, slope, scale, post, boost};
+    return epi_fwd(y, e, x_old, x_new, rows, C, nullptr, ST(stream));
 }
-
-constexpr int GAIN_ROWS_PER_BLOCK = 128;
-inline long long gain_bwd_ws_floats(long long rows, int C) { return blocks_of(rows, GAIN_ROWS_PER_BLOCK) * 6ll * C; }
-
-// part: NULL (fp64 atomics into sums [3C]) or the gain_bwd_ws_floats(rows, C) partials of the deterministic form
-static int act_gain_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd, const float* gamma,
-                             const float* beta, int batch_stats, long long rows, int C, int act, float slope,
-                             const float* scale, float boost, const float* post, double* sums, float* dy, float* dgamma,
-                             float* dbeta, float* dscale, float* dpost, double* part, cudaStream_t st) {
-    BM_CHECK_ARG(g && y && dy && rows > 0 && C > 0 && act >= 0 && act <= 2);
-    BM_CHECK_ARG(!mean || (invstd && gamma && beta));
-    const bool bn_reduce = mean && bn_bwd_reduces(batch_stats, dgamma, dbeta);
-    BM_CHECK_ARG(!bn_reduce || (dgamma && dbeta));
-    const bool reduce = bn_reduce || dscale || dpost;
-    BM_CHECK_ARG(!reduce || sums);
-    if (reduce) {
-        dim3 grid((unsigned)blocks_of(rows, GAIN_ROWS_PER_BLOCK), (C + 127) / 128);
-        if (part) {
-            act_gain_bwd_reduce_kernel<true><<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, part, rows, C,
-                                                                   GAIN_ROWS_PER_BLOCK, act, slope, scale, boost, post);
-            BM_CHECK_LAUNCH();
-            if (int rc = reduce_rows(part, (long long)grid.x, 3 * C, sums, st)) return rc;
-        } else {
-            BM_CUDA(cudaMemsetAsync(sums, 0, sizeof(double) * 3 * C, st));
-            act_gain_bwd_reduce_kernel<<<grid, 128, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, rows, C,
-                                                             GAIN_ROWS_PER_BLOCK, act, slope, scale, boost, post);
-            BM_CHECK_LAUNCH();
-        }
-        act_gain_param_grad_kernel<<<(C + 127) / 128, 128, 0, st>>>(sums, C, scale, boost, post, bn_reduce ? dgamma : nullptr,
-                                                                    bn_reduce ? dbeta : nullptr, dscale, dpost);
-        BM_CHECK_LAUNCH();
-    }
-    act_gain_bwd_apply_kernel<<<ew_grid(rows * C), 256, 0, st>>>(g, y, mean, invstd, gamma, beta, sums, (double)rows,
-                                                                 bn_reduce && batch_stats, dy, rows * C, C, act, slope, scale,
-                                                                 boost, post);
-    BM_CHECK_LAUNCH();
-    return 0;
-}
-
 extern "C" int bm_bn_act_gain_skip_bwd(const float* g, const float* y, const float* mean, const float* invstd,
                                        const float* gamma, const float* beta, int batch_stats, long long rows, int C, int act,
                                        float slope, const float* scale, float boost, const float* post, double* sums,
                                        float* dy, float* dgamma, float* dbeta, float* dscale, float* dpost,
                                        bm_stream_t stream) {
-    return act_gain_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, scale, boost, post, sums, dy,
-                             dgamma, dbeta, dscale, dpost, nullptr, ST(stream));
+    const Epi e{mean, invstd, gamma, beta, act, slope, scale, post, boost, dscale || dpost};
+    return epi_bwd(g, y, e, batch_stats, rows, C, sums, dy, dgamma, dbeta, dscale, dpost, nullptr, nullptr, ST(stream));
 }
 extern "C" long long bm_bn_act_gain_skip_bwd_det_workspace(long long rows, int C) {
-    return rows > 0 && C > 0 ? gain_bwd_ws_floats(rows, C) : 0;
+    return rows > 0 && C > 0 ? epi_ws_floats(rows, 3 * C) : 0;
 }
 extern "C" int bm_bn_act_gain_skip_bwd_det(const float* g, const float* y, const float* mean, const float* invstd,
                                            const float* gamma, const float* beta, int batch_stats, long long rows, int C,
                                            int act, float slope, const float* scale, float boost, const float* post,
                                            double* sums, float* dy, float* dgamma, float* dbeta, float* dscale, float* dpost,
                                            float* workspace, long long workspace_floats, bm_stream_t stream) {
-    BM_CHECK_ARG(rows > 0 && C > 0);
-    if (!(mean && bn_bwd_reduces(batch_stats, dgamma, dbeta)) && !dscale && !dpost)   // nothing is reduced
-        return act_gain_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, scale, boost, post, sums,
-                                 dy, dgamma, dbeta, dscale, dpost, nullptr, ST(stream));
-    BM_CHECK_WS(gain_bwd_ws_floats(rows, C));
-    return act_gain_skip_bwd(g, y, mean, invstd, gamma, beta, batch_stats, rows, C, act, slope, scale, boost, post, sums, dy,
-                             dgamma, dbeta, dscale, dpost, reinterpret_cast<double*>(workspace), ST(stream));
+    const Epi e{mean, invstd, gamma, beta, act, slope, scale, post, boost, dscale || dpost};
+    return epi_bwd_det(g, y, e, batch_stats, rows, C, sums, dy, dgamma, dbeta, dscale, dpost, nullptr, workspace,
+                       workspace_floats, ST(stream));
 }
 
 static int clip_loss_bwd_cand(int passes, const float* probs, const float* scores, const float* inv_norm, const float* est,

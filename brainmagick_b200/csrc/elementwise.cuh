@@ -82,7 +82,7 @@ __global__ void softmax_bwd_kernel(const float* __restrict__ w, const float* __r
 }
 
 // ------------------------------------------------------------------------------------------------
-// BatchNorm1d + GELU + skip  (common.py:118-120,146-147)
+// BatchNorm1d statistics (common.py:118-120); the layer epilogue that applies them is in convseq.cuh
 // ------------------------------------------------------------------------------------------------
 // stats[0:C] = sum y, stats[C:2C] = sum y^2 (fp64) over n = B*T rows  ->  mean, invstd (biased var),
 // running stats update with the unbiased variance (momentum), as nn.BatchNorm1d in training mode.
@@ -113,100 +113,6 @@ __global__ void bn_eval_stats_kernel(const float* __restrict__ rm, const float* 
     if (c >= C) return;
     mean[c] = rm[c];
     invstd[c] = 1.f / sqrtf(rv[c] + eps);
-}
-
-// x_new = GELU((y - mean) * invstd * gamma + beta) (+ x_old)
-template <int VEC>
-__global__ void bn_gelu_skip_fwd_kernel(const float* __restrict__ y, const float* __restrict__ mean,
-                                        const float* __restrict__ invstd, const float* __restrict__ gamma,
-                                        const float* __restrict__ beta, const float* __restrict__ x_old,
-                                        float* __restrict__ x_new, long long total, int C) {
-    for (long long i = (blockIdx.x * (long long)blockDim.x + threadIdx.x) * VEC; i < total;
-         i += (long long)gridDim.x * blockDim.x * VEC) {
-        int c = (int)(i % C);
-        float v[VEC], o[VEC];
-        if (VEC == 4) {
-            float4 t = *reinterpret_cast<const float4*>(y + i);
-            v[0] = t.x; v[1 % VEC] = t.y; v[2 % VEC] = t.z; v[3 % VEC] = t.w;
-            if (x_old) {
-                float4 u = *reinterpret_cast<const float4*>(x_old + i);
-                o[0] = u.x; o[1 % VEC] = u.y; o[2 % VEC] = u.z; o[3 % VEC] = u.w;
-            }
-        } else {
-            v[0] = y[i];
-            if (x_old) o[0] = x_old[i];
-        }
-#pragma unroll
-        for (int j = 0; j < VEC; ++j) {
-            float z = (v[j] - mean[c + j]) * invstd[c + j] * gamma[c + j] + beta[c + j];
-            float a = gelu_f(z);
-            v[j] = x_old ? a + o[j] : a;
-        }
-        if (VEC == 4) *reinterpret_cast<float4*>(x_new + i) = make_float4(v[0], v[1 % VEC], v[2 % VEC], v[3 % VEC]);
-        else x_new[i] = v[0];
-    }
-}
-
-// backward pass 1: sums[c] += sum dz, sums[C+c] += sum dz*yhat  with dz = g * GELU'(z)
-// DET: sums is a [gridDim.x][2C] partials buffer; the block stores its own row (see reduce_rows_kernel)
-template <bool DET = false>
-__global__ void bn_gelu_bwd_reduce_kernel(const float* __restrict__ g, const float* __restrict__ y,
-                                          const float* __restrict__ mean, const float* __restrict__ invstd,
-                                          const float* __restrict__ gamma, const float* __restrict__ beta,
-                                          double* __restrict__ sums, long long rows, int C, int rows_per_block) {
-    int c = blockIdx.y * blockDim.x + threadIdx.x;
-    if (c >= C) return;
-    long long r0 = (long long)blockIdx.x * rows_per_block;
-    long long r1 = min(rows, r0 + rows_per_block);
-    float mu = mean[c], is = invstd[c], ga = gamma[c], be = beta[c];
-    float s1 = 0.f, s2 = 0.f;
-#pragma unroll 4
-    for (long long r = r0; r < r1; ++r) {
-        float yh = (y[r * C + c] - mu) * is;
-        float z = yh * ga + be;
-        float dz = g[r * C + c] * gelu_grad_f(z);
-        s1 += dz;
-        s2 += dz * yh;
-    }
-    if (DET) {
-        sums[(long long)blockIdx.x * 2 * C + c] = (double)s1;
-        sums[(long long)blockIdx.x * 2 * C + C + c] = (double)s2;
-        return;
-    }
-    atomicAdd(sums + c, (double)s1);
-    atomicAdd(sums + C + c, (double)s2);
-}
-
-// dgamma = sum dz*yhat, dbeta = sum dz  (float outputs from the fp64 sums)
-__global__ void bn_param_grad_kernel(const double* __restrict__ sums, float* __restrict__ dgamma,
-                                     float* __restrict__ dbeta, int C) {
-    int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= C) return;
-    dbeta[c] = (float)sums[c];
-    dgamma[c] = (float)sums[C + c];
-}
-
-// backward pass 2: dy = gamma*invstd*(dz - mean(dz) - yhat*mean(dz*yhat))
-// eval mode (use_batch_stats = 0): dy = gamma*invstd*dz
-// COUNTED: n is read from sums[2C] on the device (as in bn_finalize_kernel), here and in the other apply kernels
-template <bool COUNTED = false>
-__global__ void bn_gelu_bwd_apply_kernel(const float* __restrict__ g, const float* __restrict__ y,
-                                         const float* __restrict__ mean, const float* __restrict__ invstd,
-                                         const float* __restrict__ gamma, const float* __restrict__ beta,
-                                         const double* __restrict__ sums, double n, int use_batch_stats,
-                                         float* __restrict__ dy, long long total, int C) {
-    if (COUNTED) n = sums[2 * C];
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-         i += (long long)gridDim.x * blockDim.x) {
-        int c = (int)(i % C);
-        float is = invstd[c], ga = gamma[c];
-        float yh = (y[i] - mean[c]) * is;
-        float z = yh * ga + beta[c];
-        float dz = g[i] * gelu_grad_f(z);
-        float v = dz;
-        if (use_batch_stats) v = dz - (float)(sums[c] / n) - yh * (float)(sums[C + c] / n);
-        dy[i] = ga * is * v;
-    }
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -485,36 +391,6 @@ __global__ void transpose_nt_kernel(const float* __restrict__ in, float* __restr
 // ------------------------------------------------------------------------------------------------
 // float4 versions (C % 4 == 0, 16-byte aligned rows): one thread owns 4 consecutive channels
 // ------------------------------------------------------------------------------------------------
-template <bool COUNTED = false>
-__global__ void bn_gelu_bwd_apply_v4_kernel(const float4* __restrict__ g, const float4* __restrict__ y,
-                                            const float4* __restrict__ mean, const float4* __restrict__ invstd,
-                                            const float4* __restrict__ gamma, const float4* __restrict__ beta,
-                                            const double* __restrict__ sums, double n, int use_batch_stats,
-                                            float4* __restrict__ dy, long long total4, int C) {
-    if (COUNTED) n = sums[2 * C];
-    const int C4 = C >> 2;
-    const float rn = (float)(1.0 / n);
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total4;
-         i += (long long)gridDim.x * blockDim.x) {
-        const int c4 = (int)(i % C4), c = c4 * 4;
-        const float4 mu = mean[c4], is = invstd[c4], ga = gamma[c4], be = beta[c4];
-        const float4 yv = y[i], gv = g[i];
-        float m1[4] = {0.f, 0.f, 0.f, 0.f}, m2[4] = {0.f, 0.f, 0.f, 0.f};
-        if (use_batch_stats) {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) { m1[j] = (float)(sums[c + j] / n); m2[j] = (float)(sums[C + c + j] / n); }
-        }
-        (void)rn;
-        float4 o;
-        float yh, dz;
-        yh = (yv.x - mu.x) * is.x; dz = gv.x * gelu_grad_f(yh * ga.x + be.x); o.x = ga.x * is.x * (dz - m1[0] - yh * m2[0]);
-        yh = (yv.y - mu.y) * is.y; dz = gv.y * gelu_grad_f(yh * ga.y + be.y); o.y = ga.y * is.y * (dz - m1[1] - yh * m2[1]);
-        yh = (yv.z - mu.z) * is.z; dz = gv.z * gelu_grad_f(yh * ga.z + be.z); o.z = ga.z * is.z * (dz - m1[2] - yh * m2[2]);
-        yh = (yv.w - mu.w) * is.w; dz = gv.w * gelu_grad_f(yh * ga.w + be.w); o.w = ga.w * is.w * (dz - m1[3] - yh * m2[3]);
-        dy[i] = o;
-    }
-}
-
 __global__ void glu_bwd_v4_kernel(const float4* __restrict__ g, const float4* __restrict__ h, float4* __restrict__ dh,
                                   long long rows, int H) {
     const int H4 = H >> 2;
@@ -545,7 +421,7 @@ __global__ void gelu_bwd_v4_kernel(const float4* __restrict__ dq, const float4* 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Column-stationary versions of the three BatchNorm + GELU kernels (channels-last rows, C % 4 == 0, C/4 <= 256):
+// Column-stationary kernels (channels-last rows, C % 4 == 0, C/4 <= 256: GLU backward here, the layer epilogue in convseq.cuh):
 // block = (C/4, RY) threads; thread (cx, ry) owns columns 4cx..4cx+3 for the rows ry, ry+RY, ... of the block's row range, so
 // the per-column parameters live in registers (no i % C, no parameter reloads, no fp64 divisions per element) and every
 // warp-level access is a contiguous row piece.  Rows are unrolled by 4 for memory-level parallelism.
@@ -572,147 +448,6 @@ __device__ __forceinline__ void block_amax_commit(float m, unsigned int* cell) {
         for (int w = 1; w < (nthr + 31) / 32; ++w) m = fmaxf(m, warp_max[w]);
         if (m > 0.f) atomicMax(cell, __float_as_uint(m));
     }
-}
-
-// x_new = GELU((y - mean) * invstd * gamma + beta) (+ x_old)
-__global__ void __launch_bounds__(320, 2)
-bn_gelu_skip_fwd_cs_kernel(const float* __restrict__ y, const float* __restrict__ mean, const float* __restrict__ invstd,
-                           const float* __restrict__ gamma, const float* __restrict__ beta, const float* __restrict__ x_old,
-                           float* __restrict__ x_new, long long rows, int C, unsigned int* __restrict__ amax) {
-    const int c = threadIdx.x * 4, RY = blockDim.y;
-    const float4 mu = ld4(mean + c), is = ld4(invstd + c), ga = ld4(gamma + c), be = ld4(beta + c);
-    const long long r0 = (long long)blockIdx.x * CS_ROWS_PER_BLOCK;
-    const long long r1 = min(rows, r0 + CS_ROWS_PER_BLOCK);
-    float am = 0.f;
-    for (long long r = r0 + threadIdx.y; r < r1; r += (long long)CS_U * RY) {
-        float4 v[CS_U], u[CS_U];
-#pragma unroll
-        for (int k = 0; k < CS_U; ++k) {
-            const long long rr = r + (long long)k * RY;
-            if (rr < r1) {
-                v[k] = ld4s(y + rr * C + c);
-                if (x_old) u[k] = ld4(x_old + rr * C + c);
-            }
-        }
-#pragma unroll
-        for (int k = 0; k < CS_U; ++k) {
-            const long long rr = r + (long long)k * RY;
-            if (rr < r1) {
-                float4 o;
-                // same operation order as the reference BatchNorm: ((y - mean) * invstd) * gamma + beta
-                o.x = gelu_f(fmaf((v[k].x - mu.x) * is.x, ga.x, be.x));
-                o.y = gelu_f(fmaf((v[k].y - mu.y) * is.y, ga.y, be.y));
-                o.z = gelu_f(fmaf((v[k].z - mu.z) * is.z, ga.z, be.z));
-                o.w = gelu_f(fmaf((v[k].w - mu.w) * is.w, ga.w, be.w));
-                if (x_old) { o.x += u[k].x; o.y += u[k].y; o.z += u[k].z; o.w += u[k].w; }
-                *reinterpret_cast<float4*>(x_new + rr * C + c) = o;
-                am = amax4(am, o);
-            }
-        }
-    }
-    if (amax) block_amax_commit(am, amax);
-}
-
-// backward pass 1: sums[c] += sum dz, sums[C+c] += sum dz*yhat  with dz = g * GELU'(z); fp32 per thread, combined over the
-// block's RY row lanes in shared memory, ONE fp64 atomic pair per column per block (DET: sums is a [gridDim.x][2C] partials
-// buffer, the block stores its row)
-template <bool DET = false>
-__global__ void __launch_bounds__(320, 2)
-bn_gelu_bwd_reduce_cs_kernel(const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ mean,
-                             const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta,
-                             double* __restrict__ sums, long long rows, int C) {
-    extern __shared__ float red[];                       // [RY][2][C]
-    const int c = threadIdx.x * 4, RY = blockDim.y;
-    const float4 mu = ld4(mean + c), is = ld4(invstd + c), ga = ld4(gamma + c), be = ld4(beta + c);
-    const long long r0 = (long long)blockIdx.x * CS_ROWS_PER_BLOCK;
-    const long long r1 = min(rows, r0 + CS_ROWS_PER_BLOCK);
-    float4 s1 = make_float4(0.f, 0.f, 0.f, 0.f), s2 = s1;
-    for (long long r = r0 + threadIdx.y; r < r1; r += (long long)CS_U * RY) {
-        float4 yv[CS_U], gv[CS_U];
-#pragma unroll
-        for (int k = 0; k < CS_U; ++k) {
-            const long long rr = r + (long long)k * RY;
-            if (rr < r1) { yv[k] = ld4(y + rr * C + c); gv[k] = ld4(g + rr * C + c); }
-        }
-#pragma unroll
-        for (int k = 0; k < CS_U; ++k) {
-            const long long rr = r + (long long)k * RY;
-            if (rr < r1) {
-                float yh, dz;
-                yh = (yv[k].x - mu.x) * is.x; dz = gv[k].x * gelu_grad_f(fmaf(yh, ga.x, be.x)); s1.x += dz; s2.x = fmaf(dz, yh, s2.x);
-                yh = (yv[k].y - mu.y) * is.y; dz = gv[k].y * gelu_grad_f(fmaf(yh, ga.y, be.y)); s1.y += dz; s2.y = fmaf(dz, yh, s2.y);
-                yh = (yv[k].z - mu.z) * is.z; dz = gv[k].z * gelu_grad_f(fmaf(yh, ga.z, be.z)); s1.z += dz; s2.z = fmaf(dz, yh, s2.z);
-                yh = (yv[k].w - mu.w) * is.w; dz = gv[k].w * gelu_grad_f(fmaf(yh, ga.w, be.w)); s1.w += dz; s2.w = fmaf(dz, yh, s2.w);
-            }
-        }
-    }
-    float* mine = red + (size_t)threadIdx.y * 2 * C;
-    *reinterpret_cast<float4*>(mine + c) = s1;
-    *reinterpret_cast<float4*>(mine + C + c) = s2;
-    __syncthreads();
-    const int tid = threadIdx.y * blockDim.x + threadIdx.x, nthr = blockDim.x * blockDim.y;
-    for (int i = tid; i < 2 * C; i += nthr) {
-        double acc = 0.0;
-        for (int ry = 0; ry < RY; ++ry) acc += (double)red[(size_t)ry * 2 * C + i];
-        if (DET) sums[(long long)blockIdx.x * 2 * C + i] = acc;
-        else atomicAdd(sums + i, acc);
-    }
-}
-
-// backward pass 2: dy = gamma*invstd*(dz - mean(dz) - yhat*mean(dz*yhat)); the two means come as dbeta/n and dgamma/n
-// (written by bn_param_grad_kernel from the fp64 sums); eval mode (use_batch_stats = 0): dy = gamma*invstd*dz.
-// COUNTED: the two sums are rounded from `sums` [2C + 1] here and rn = (float)(1 / sums[2C]) -- the same bits as the
-// float sums of bn_param_grad_kernel and the host's (float)(1.0 / (double)rows) for the same row count.
-template <bool COUNTED = false>
-__global__ void __launch_bounds__(320, 2)
-bn_gelu_bwd_apply_cs_kernel(const float* __restrict__ g, const float* __restrict__ y, const float* __restrict__ mean,
-                            const float* __restrict__ invstd, const float* __restrict__ gamma, const float* __restrict__ beta,
-                            const float* __restrict__ dgamma, const float* __restrict__ dbeta, const double* __restrict__ sums,
-                            float rn, int use_batch_stats, float* __restrict__ dy, long long rows, int C,
-                            unsigned int* __restrict__ amax) {
-    const int c = threadIdx.x * 4, RY = blockDim.y;
-    const float4 mu = ld4(mean + c), is = ld4(invstd + c), ga = ld4(gamma + c), be = ld4(beta + c);
-    float am = 0.f;
-    float4 m1 = make_float4(0.f, 0.f, 0.f, 0.f), m2 = m1;
-    if (use_batch_stats) {
-        float4 db, dg;
-        if (COUNTED) {
-            rn = (float)(1.0 / sums[2 * C]);
-            db = make_float4((float)sums[c], (float)sums[c + 1], (float)sums[c + 2], (float)sums[c + 3]);
-            dg = make_float4((float)sums[C + c], (float)sums[C + c + 1], (float)sums[C + c + 2], (float)sums[C + c + 3]);
-        } else {
-            db = ld4(dbeta + c);
-            dg = ld4(dgamma + c);
-        }
-        m1 = make_float4(db.x * rn, db.y * rn, db.z * rn, db.w * rn);
-        m2 = make_float4(dg.x * rn, dg.y * rn, dg.z * rn, dg.w * rn);
-    }
-    const float4 kk = make_float4(ga.x * is.x, ga.y * is.y, ga.z * is.z, ga.w * is.w);
-    const long long r0 = (long long)blockIdx.x * CS_ROWS_PER_BLOCK;
-    const long long r1 = min(rows, r0 + CS_ROWS_PER_BLOCK);
-    for (long long r = r0 + threadIdx.y; r < r1; r += (long long)CS_U * RY) {
-        float4 yv[CS_U], gv[CS_U];
-#pragma unroll
-        for (int k = 0; k < CS_U; ++k) {
-            const long long rr = r + (long long)k * RY;
-            if (rr < r1) { yv[k] = ld4s(y + rr * C + c); gv[k] = ld4s(g + rr * C + c); }
-        }
-#pragma unroll
-        for (int k = 0; k < CS_U; ++k) {
-            const long long rr = r + (long long)k * RY;
-            if (rr < r1) {
-                float4 o;
-                float yh, dz;
-                yh = (yv[k].x - mu.x) * is.x; dz = gv[k].x * gelu_grad_f(fmaf(yh, ga.x, be.x)); o.x = kk.x * (dz - m1.x - yh * m2.x);
-                yh = (yv[k].y - mu.y) * is.y; dz = gv[k].y * gelu_grad_f(fmaf(yh, ga.y, be.y)); o.y = kk.y * (dz - m1.y - yh * m2.y);
-                yh = (yv[k].z - mu.z) * is.z; dz = gv[k].z * gelu_grad_f(fmaf(yh, ga.z, be.z)); o.z = kk.z * (dz - m1.z - yh * m2.z);
-                yh = (yv[k].w - mu.w) * is.w; dz = gv[k].w * gelu_grad_f(fmaf(yh, ga.w, be.w)); o.w = kk.w * (dz - m1.w - yh * m2.w);
-                *reinterpret_cast<float4*>(dy + rr * C + c) = o;
-                am = amax4(am, o);
-            }
-        }
-    }
-    if (amax) block_amax_commit(am, amax);
 }
 
 // GLU backward, column-stationary (H % 4 == 0, H/4 <= 256): thread (cx, ry) owns a-columns 4cx.. and the matching gate columns;

@@ -403,6 +403,15 @@ class _Conv:
         return dw, db
 
 
+def _epilogue(kind, has_bn, act, slope, head, tail=()):
+    """(entry point, arguments before the stream) of a ConvSequence layer epilogue without gains, `kind` "fwd", "bwd",
+    "bwd_reduce" or "bwd_apply": bm_bn_gelu_skip_* (amax_out NULL) for a BatchNorm + GELU layer, else bm_bn_act_skip_* with
+    the activation code and slope.  head: the arguments up to C; tail: the ones after the activation's."""
+    if has_bn and act == ACT_GELU:
+        return "bm_bn_gelu_skip_" + kind, head + tail + ((None,) if kind in ("fwd", "bwd") else ())
+    return "bm_bn_act_skip_" + kind, head + (act, float(slope)) + tail
+
+
 # ----------------------------------------------------------------------------------------------------
 # The ConvSequence layers (bm/models/common.py:142-151) on channels-last activations: SimpleConv's encoder and the
 # stand-alone ConvSequence / DeepMel both run them through these two functions.
@@ -428,12 +437,9 @@ def _residual_branch_forward(plan: SequencePlan, k, p, x, y, mean, invstd, skip,
     src = y
     if rw is not None:
         a = _empty((B, T, cout), x)
-        if mean is not None and act == ACT_GELU:
-            call("bm_bn_gelu_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), None, ptr(a), rows, cout, None,
-                 st)
-        else:
-            call("bm_bn_act_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), None, ptr(a), rows, cout, act,
-                 slope, st)
+        name, args = _epilogue("fwd", mean is not None, act, slope,
+                               (ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), None, ptr(a), rows, cout))
+        call(name, *args, st)
         need_dy = nd.below[k] or any(nd.layer[k][:4])
         rconv = _Conv(rw, T, False, plan.use_tensor_cores, want_bwd=save and need_dy)
         y2 = _empty((B, T, cout), x)
@@ -551,12 +557,10 @@ def conv_stack_forward(plan: SequencePlan, x, conv0: _Conv, conv_p, glu_p, nd: "
         elif has_bn or act != ACT_NONE or skip:
             x_new = _empty((B, T, cout), x)
             gamma, beta = (gamma.contiguous(), beta.contiguous()) if has_bn else (None, None)
-            if has_bn and act == ACT_GELU:
-                call("bm_bn_gelu_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), ptr(x) if skip else None,
-                     ptr(x_new), rows, cout, None, st)
-            else:
-                call("bm_bn_act_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), ptr(x) if skip else None,
-                     ptr(x_new), rows, cout, act, float(plan.act_slope if plan.has_act[k] else bare_slope), st)
+            name, args = _epilogue("fwd", has_bn, act, plan.act_slope if plan.has_act[k] else bare_slope,
+                                   (ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), ptr(x) if skip else None, ptr(x_new),
+                                    rows, cout))
+            call(name, *args, st)
         if len(p) == 4:
             # kept: the conv input for its weight gradient, y for the activation backward, x_new for the GLU weight gradient
             rec = dict(x_in=x if nd.layer[k][0] else None, y=y if plan.has_act[k] and nd.layer_up(k) else None, mean=mean,
@@ -634,32 +638,26 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
             # Whether that all-reduce is issued depends on requires_grad flags only, never on data, so every rank issues
             # the same collectives in the same order (DESIGN 4.1).
             dgamma, dbeta = _empty((cout,), like), _empty((cout,), like)
-            gelu = rec["act"] == ACT_GELU
-            name = "bm_bn_gelu_skip_bwd" if gelu else "bm_bn_act_skip_bwd"
             gm, bt = gamma.contiguous(), beta.contiguous()
-            args = (ptr(g_act), ptr(rec["y"]), ptr(rec["mean"]), ptr(rec["invstd"]), ptr(gm), ptr(bt), rows, cout) + \
-                (() if gelu else (rec["act"], float(plan.act_slope)))
-            _reducing_call(name + "_reduce", like, (rows, cout), *args, ptr(sums), ptr(dgamma), ptr(dbeta), st)
+            head = (ptr(g_act), ptr(rec["y"]), ptr(rec["mean"]), ptr(rec["invstd"]), ptr(gm), ptr(bt), rows, cout)
+            name, args = _epilogue("bwd_reduce", True, rec["act"], plan.act_slope, head, (ptr(sums), ptr(dgamma), ptr(dbeta)))
+            _reducing_call(name, like, (rows, cout), *args, st)
             if n_cw or n_cb or nd.below[k]:
                 _sync_bn_sums(sums, cout, rows, group)
                 dy = _empty((B, T, cout), like)
-                call(name + "_apply", *args, ptr(sums), ptr(dy), st)
+                name, args = _epilogue("bwd_apply", True, rec["act"], plan.act_slope, head, (ptr(sums), ptr(dy)))
+                call(name, *args, st)
         elif rec["has_bn"]:
             # the batch statistics' backward reduces in training mode; in eval mode only for trainable gamma / beta (else
             # the BatchNorm + activation backward is one elementwise pass)
             reduce = plan.training or n_gamma or n_beta
             dy = _empty((B, T, cout), like)
             dgamma, dbeta = (_empty((cout,), like), _empty((cout,), like)) if reduce else (None, None)
-            if rec["act"] == ACT_GELU:
-                _reducing_call("bm_bn_gelu_skip_bwd", like, (rows, cout), ptr(g_act), ptr(rec["y"]), ptr(rec["mean"]),
-                               ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()),
-                               1 if plan.training else 0, rows, cout, ptr(sums if reduce else None), ptr(dy), ptr(dgamma),
-                               ptr(dbeta), None, st, reduces=reduce)
-            else:
-                _reducing_call("bm_bn_act_skip_bwd", like, (rows, cout), ptr(g_act), ptr(rec["y"]), ptr(rec["mean"]),
-                               ptr(rec["invstd"]), ptr(gamma.contiguous()), ptr(beta.contiguous()),
-                               1 if plan.training else 0, rows, cout, rec["act"], float(plan.act_slope),
-                               ptr(sums if reduce else None), ptr(dy), ptr(dgamma), ptr(dbeta), st, reduces=reduce)
+            name, args = _epilogue("bwd", True, rec["act"], plan.act_slope,
+                                   (ptr(g_act), ptr(rec["y"]), ptr(rec["mean"]), ptr(rec["invstd"]), ptr(gamma.contiguous()),
+                                    ptr(beta.contiguous()), 1 if plan.training else 0, rows, cout),
+                                   (ptr(sums if reduce else None), ptr(dy), ptr(dgamma), ptr(dbeta)))
+            _reducing_call(name, like, (rows, cout), *args, st, reduces=reduce)
         elif rec["act"] != ACT_NONE:
             dy = _empty((B, T, cout), like)
             call("bm_bn_act_skip_bwd", ptr(g_act), ptr(rec["y"]), None, None, None, None, 0, rows, cout, rec["act"],

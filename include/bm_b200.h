@@ -204,9 +204,10 @@ int bm_clip_loss_bwd(const float* probs, const float* inv_norm, const float* can
                      int Bc, long long KT, int target_offset, float* G, float* dest, int* status, bm_stream_t stream);
 
 /* ---- Stand-alone ConvSequence / DeepMel (SURVEY 8(f) row 3): bm/models/common.py:79-151, bm/models/features.py:15-35 --
- * Layer epilogue x_new = act(bn(y)) (+ x_old) over channels-last rows [rows, C] and its backward, for the cases the
- * brain encoder's fused BatchNorm+GELU kernels do not cover: act 0 = GELU, 1 = LeakyReLU(slope) (common.py:95),
- * 2 = none; mean == NULL = no BatchNorm (the layer then only applies the activation / the skip).
+ * Layer epilogue x_new = act(bn(y)) (+ x_old) over channels-last rows [rows, C] and its backward, for any activation:
+ * act 0 = GELU, 1 = LeakyReLU(slope) (common.py:95), 2 = none; mean == NULL = no BatchNorm (the layer then only applies the
+ * activation / the skip).  bm_bn_gelu_skip_*, bm_bn_act_skip_* and bm_bn_act_gain_skip_* are forms of one epilogue: where
+ * their contracts overlap (BatchNorm + GELU, no gain) they give the same bits.
  * bm_bn_act_skip_bwd: dy = d/dy of the above given g = dL/dx_new (the skip branch's gradient is g itself);
  * batch_stats=1: training-mode BatchNorm (dgamma, dbeta, fp64 sums [2C] scratch), 0: eval statistics. */
 int bm_bn_act_skip_fwd(const float* y, const float* mean, const float* invstd, const float* gamma, const float* beta,
@@ -226,7 +227,8 @@ int bm_bn_act_skip_bwd_apply(const float* g, const float* y, const float* mean, 
  * x_new = post[c] * ((boost * scale[c]) * branch) (+ x_old), branch = act(bn(y)) as in bm_bn_act_skip_fwd; scale [C]
  * (LayerScale's parameter, boost its factor 5) and post [C] (the depthwise 1x1 conv's weight) are each nullable (gain 1).
  * bm_bn_act_gain_skip_bwd: dy = d/dy of the branch given gain(g), g = dL/dx_new, with the BatchNorm cases of
- * bm_bn_act_skip_bwd, and in the same reduction pass S[c] = sum_rows g*branch (branch recomputed from y, fp64 per thread):
+ * bm_bn_act_skip_bwd, and in the same reduction pass S[c] = sum_rows g*branch (branch recomputed from y; fp32 per thread, fp64
+ * across threads and blocks, as the BatchNorm sums):
  * dscale = boost*post*S, dpost = (boost*scale)*S, each nullable (frozen: not reduced).  sums: fp64 scratch [3C], needed
  * when anything is reduced (a BatchNorm in training mode, dgamma / dbeta, dscale or dpost). */
 int bm_bn_act_gain_skip_fwd(const float* y, const float* mean, const float* invstd, const float* gamma, const float* beta,

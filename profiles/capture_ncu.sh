@@ -10,8 +10,8 @@ for n in $names; do
     conv|conv_glu|conv_acc) k=conv_pp_kernel; c=1;;
     wgrad) k=wgrad_pp_kernel; c=1;;
     scores_train) k=clip_scores_kernel; c=1;;
-    bn_bwd) k=bn_gelu_bwd; c=2;;
-    bn_fwd) k=bn_gelu_skip_fwd; c=1;;
+    bn_bwd) k=epi_bwd; c=2;;
+    bn_fwd) k=epi_fwd; c=1;;
   esac
   s=$((3 * c))
   timeout 300 ncu --set full --clock-control none --import-source on -k regex:$k -s $s -c $c -f -o gpurun_out/${tag}_${n} \

@@ -117,7 +117,7 @@ elif which == "scores":        # -k regex:clip_scores_kernel           (retrieva
     for _ in range(3):
         call("bm_clip_scores", ptr(est), ptr(cand), Bn, M, KT, 1, ptr(inv), ptr(out), None, ptr(ws), ws.numel(), ptr(status),
              stream())
-elif which in ("bn_bwd", "bn_fwd"):   # -k regex:bn_gelu_bwd_(reduce|apply)_cs_kernel | -k regex:bn_gelu_skip_fwd_cs_kernel
+elif which in ("bn_bwd", "bn_fwd"):   # -k regex:epi_bwd_(reduce|apply)_cs_kernel | -k regex:epi_fwd_cs_kernel
     rows = B * T
     dy, x, gy = (torch.randn(B, T, H, device=dev) for _ in range(3))
     gam, bet = torch.ones(H, device=dev), torch.zeros(H, device=dev)

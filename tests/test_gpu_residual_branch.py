@@ -58,9 +58,10 @@ def _close(got, ref, what):
 @pytest.mark.parametrize("C,rows", [(320, 1000), (10, 777)])
 @pytest.mark.parametrize("mode", ["bn_train", "bn_eval", "no_bn"])
 @pytest.mark.parametrize("act", [GELU, LRELU, NONE])
-@pytest.mark.parametrize("gains", ["scale", "post", "both"])
+@pytest.mark.parametrize("gains", ["scale", "post", "both", "none"])
 @pytest.mark.parametrize("det", [False, True])
 def test_gain_entry_points_against_fp64(C, rows, mode, act, gains, det):
+    """gains "none": scale and post NULL (gain 1) with dscale and dpost asked for: dpost = S, dscale = boost * S."""
     gen = torch.Generator(device=DEV).manual_seed(C + rows)
     r = lambda *s: torch.randn(*s, device=DEV, generator=gen)   # noqa: E731
     y, g, x_old = r(rows, C) * 2 + 0.5, r(rows, C), r(rows, C)
@@ -77,14 +78,17 @@ def test_gain_entry_points_against_fp64(C, rows, mode, act, gains, det):
         else:
             mean, invstd = 0.3 * r(C), 1 / (1 + r(C).abs())
         bn = (mean, invstd, gamma, beta)
-    ref = _gain_ref(y, g, bn, act, slope, scale, post, x_old, train)
+    ref_post = torch.ones(C, device=DEV) if gains == "none" else post
+    ref = _gain_ref(y, g, bn, act, slope, scale, ref_post, x_old, train)
+    if gains == "none":                     # the reference's post = 1 gives S as its gradient
+        ref = ref[:4] + (5.0 * ref[5], ref[5])
     st = stream()
     x_new = torch.empty_like(y)
     call("bm_bn_act_gain_skip_fwd", ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), ptr(x_old), ptr(x_new), rows, C,
          act, slope, ptr(scale), 5.0, ptr(post), st)
     _close(x_new, ref[0], "x_new")
     outs = [torch.empty_like(y)] + [torch.empty(C, device=DEV) if t is not None else None for t in ref[2:]]
-    sums = torch.empty(3 * C, device=DEV, dtype=torch.float64)
+    sums = torch.full((3 * C,), float("nan"), device=DEV, dtype=torch.float64)
     args = [ptr(g), ptr(y), ptr(mean), ptr(invstd), ptr(gamma), ptr(beta), int(train), rows, C, act, slope, ptr(scale), 5.0,
             ptr(post), ptr(sums)] + [ptr(t) for t in outs]
 
@@ -103,6 +107,42 @@ def test_gain_entry_points_against_fp64(C, rows, mode, act, gains, det):
         first = [t.clone() for t in outs if t is not None]
         run()
         assert all(torch.equal(a, b) for a, b in zip(first, [t for t in outs if t is not None]))
+
+
+@pytest.mark.parametrize("C,rows", [(320, 1000), (10, 777)])
+@pytest.mark.parametrize("train", [True, False])
+@pytest.mark.parametrize("det", [False, True])
+def test_epilogue_entry_points_agree_bitwise(C, rows, train, det):
+    """Where their contracts overlap -- BatchNorm + GELU without gains -- bm_bn_gelu_skip_*, bm_bn_act_skip_*(GELU) and
+    bm_bn_act_gain_skip_* with NULL gains run one layer epilogue: the same bits forward and backward, at a column-stationary
+    width (320) and a generic one (10)."""
+    gen = torch.Generator(device=DEV).manual_seed(C + rows + train)
+    r = lambda *s: torch.randn(*s, device=DEV, generator=gen)   # noqa: E731
+    y, g, x_old = r(rows, C) * 2 + 0.5, r(rows, C), r(rows, C)
+    mean, invstd, gamma, beta = 0.3 * r(C), 1 / (1 + r(C).abs()), 1 + 0.1 * r(C), 0.1 * r(C)
+    st = stream()
+    bn = [ptr(mean), ptr(invstd), ptr(gamma), ptr(beta)]
+    fwd = {"bm_bn_gelu_skip_fwd": [None], "bm_bn_act_skip_fwd": [GELU, 0.0],
+           "bm_bn_act_gain_skip_fwd": [GELU, 0.0, None, 5.0, None]}
+    bwd = {"bm_bn_gelu_skip_bwd": ([], [None]), "bm_bn_act_skip_bwd": ([GELU, 0.0], []),
+           "bm_bn_act_gain_skip_bwd": ([GELU, 0.0, None, 5.0, None], [None, None])}
+    results = []
+    for (fname, fextra), (bname, (act_args, tail)) in zip(fwd.items(), bwd.items()):
+        x_new, dy = torch.empty_like(y), torch.empty_like(y)
+        dgamma, dbeta = torch.empty(C, device=DEV), torch.empty(C, device=DEV)
+        call(fname, ptr(y), *bn, ptr(x_old), ptr(x_new), rows, C, *fextra, st)
+        sums = torch.empty(3 * C, device=DEV, dtype=torch.float64)
+        args = [ptr(g), ptr(y), *bn, int(train), rows, C, *act_args, ptr(sums), ptr(dy), ptr(dgamma), ptr(dbeta), *tail]
+        if det:
+            n = getattr(BF._lib.load(), bname + "_det_workspace")(rows, C)
+            ws = torch.full((n,), float("nan"), device=DEV)
+            call(bname + "_det", *args, ptr(ws), n, st)
+        else:
+            call(bname, *args, st)
+        results.append((x_new, dy, dgamma, dbeta))
+    for other in results[1:]:
+        for a, b, what in zip(results[0], other, ("x_new", "dy", "dgamma", "dbeta")):
+            assert torch.equal(a, b), what
 
 
 # ---- module level ------------------------------------------------------------------------------------------------
