@@ -20,8 +20,8 @@ import torch
 
 from . import _lib
 from ._lib import call, ptr, stream
-from .functional import (SequencePlan, _Conv, _Needs, _empty, _round_up, bn_sync_groups, conv_stack_backward,
-                         conv_stack_forward, layer_width, tc_status_tensor)
+from .functional import (SequencePlan, _Needs, _empty, bn_sync_groups, conv_stack_backward, conv_stack_forward,
+                         layer_width, stack_conv0, tc_status_tensor)
 
 
 def _present(plan: SequencePlan, k: int) -> tp.List[bool]:
@@ -81,13 +81,7 @@ class _ConvSequenceFn(torch.autograd.Function):
         status = tc_status_tensor(x_in.device)
 
         # channels-last input, zero-padded to a multiple of 64 channels when the first conv can use the tensor cores
-        Cp = _round_up(C0, 64)
-        if plan.skip and conv_p[0][0].shape[0] == C0:
-            Cp = C0                                         # layer 0 has a residual: its input keeps the true width
-        conv0 = _Conv(conv_p[0][0], T, False, tc, pad_cin_to=Cp, want_bwd=save and nd.below[0])
-        if not conv0.fwd_tc and Cp != C0:
-            Cp = C0
-            conv0 = _Conv(conv_p[0][0], T, False, False, want_bwd=save and nd.below[0])
+        conv0, Cp = stack_conv0(conv_p[0][0], T, C0, tc, plan.skip, save and nd.below[0])
         x = _empty((B, T, Cp), x_in)                               # the transpose writes the pad columns as zeros
         call("bm_transpose_nt_ld", ptr(x_in), B, C0, T, Cp, ptr(x), st)
 

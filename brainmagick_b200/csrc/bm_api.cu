@@ -12,6 +12,7 @@
 #include "retrieval.cuh"
 #include "prep.cuh"
 #include "convseq.cuh"
+#include "channel_join.cuh"
 
 namespace bm {
 thread_local char g_last_error[512] = "";
@@ -1499,6 +1500,65 @@ extern "C" int bm_transpose_nt_ld(const float* in, int Z, int N, int T, int ld_o
     transpose_nt_kernel<<<grid, dim3(32, 8), 0, ST(stream)>>>(in, out, N, T, ld_out, ld_out);
     BM_CHECK_LAUNCH();
     return 0;
+}
+
+// channel join / split (channel_join.cuh): the host describes each source once, the segments are laid out by column
+namespace {
+struct JoinSrc { float* p; int C, ld, cm, col; };
+
+int channel_join_launch(bool split, float* packed, int B, int T, int Cp, int n, const JoinSrc* src, cudaStream_t st) {
+    BM_CHECK_ARG(packed && B > 0 && T > 0 && Cp > 0 && n >= 1 && n <= 4 && B <= 65535);
+    int order[4];
+    for (int i = 0; i < n; ++i) {
+        const JoinSrc& s = src[i];
+        BM_CHECK_ARG(s.C > 0 && s.col >= 0 && s.col + s.C <= Cp && (s.cm == 0 || s.cm == 1));
+        BM_CHECK_ARG(split || s.p);                               // a NULL split destination is not wanted
+        BM_CHECK_ARG(!s.p || (s.cm ? s.ld >= T : s.ld >= s.C));
+        order[i] = i;
+    }
+    std::sort(order, order + n, [&](int x, int y) { return src[x].col < src[y].col; });
+    const bool packed_vec = (reinterpret_cast<uintptr_t>(packed) & 15) == 0 && Cp % 4 == 0;
+    JoinArgs a{};
+    a.T = T; a.Cp = Cp; a.packed = packed;
+    int tiles = 0, end = 0;
+    auto add = [&](float* p, int C, int ld, int cm, int col) {
+        JoinSeg& g = a.s[a.n++];
+        g.p = p; g.C = C; g.ld = ld; g.cm = cm; g.col = col; g.tile0 = tiles;
+        g.vec = !cm && packed_vec && C % 4 == 0 && col % 4 == 0 && (!p || (ld % 4 == 0 && (reinterpret_cast<uintptr_t>(p) & 15) == 0));
+        tiles += (C + (g.vec ? 128 : 32) - 1) / (g.vec ? 128 : 32);
+    };
+    for (int k = 0; k < n; ++k) {
+        const JoinSrc& s = src[order[k]];
+        BM_CHECK_ARG(s.col >= end);                              // column ranges do not overlap
+        if (!split && s.col > end) add(nullptr, s.col - end, 0, 0, end);
+        if (s.p) add(s.p, s.C, s.ld, s.cm, s.col);
+        end = s.col + s.C;
+    }
+    if (!split && end < Cp) add(nullptr, Cp - end, 0, 0, end);
+    if (a.n == 0) return 0;                                      // a split with every destination NULL
+    dim3 grid(tiles, (T + 31) / 32, B);
+    if (split) channel_join_kernel<true><<<grid, dim3(32, 8), 0, st>>>(a);
+    else channel_join_kernel<false><<<grid, dim3(32, 8), 0, st>>>(a);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+}  // namespace
+
+extern "C" int bm_channel_join(int B, int T, int Cp, int n, const float* src0, int C0, int ld0, int cm0, int col0,
+                               const float* src1, int C1, int ld1, int cm1, int col1, const float* src2, int C2, int ld2,
+                               int cm2, int col2, const float* src3, int C3, int ld3, int cm3, int col3, float* dst,
+                               bm_stream_t stream) {
+    const JoinSrc src[4] = {{const_cast<float*>(src0), C0, ld0, cm0, col0}, {const_cast<float*>(src1), C1, ld1, cm1, col1},
+                            {const_cast<float*>(src2), C2, ld2, cm2, col2}, {const_cast<float*>(src3), C3, ld3, cm3, col3}};
+    return channel_join_launch(false, dst, B, T, Cp, n, src, ST(stream));
+}
+
+extern "C" int bm_channel_split(const float* src, int B, int T, int Cp, int n, float* dst0, int C0, int ld0, int cm0,
+                                int col0, float* dst1, int C1, int ld1, int cm1, int col1, float* dst2, int C2, int ld2,
+                                int cm2, int col2, float* dst3, int C3, int ld3, int cm3, int col3, bm_stream_t stream) {
+    const JoinSrc dst[4] = {{dst0, C0, ld0, cm0, col0}, {dst1, C1, ld1, cm1, col1}, {dst2, C2, ld2, cm2, col2},
+                            {dst3, C3, ld3, cm3, col3}};
+    return channel_join_launch(true, const_cast<float*>(src), B, T, Cp, n, dst, ST(stream));
 }
 
 // weight gradient of a (dilated) conv / pointwise layer on the tensor cores: dW[m][n][tap] = sum_{b,t} dY[b,t,m] X[b,t+s,n]

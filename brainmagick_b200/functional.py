@@ -110,6 +110,11 @@ class EncoderPlan(SequencePlan):
     has_sub_emb: bool = False              # the last tensor argument is the [B, E] subject-embedding rows
     channel_mask: tp.Optional[torch.Tensor] = None   # [C] subsample_meg_channels mask (simpleconv.py:200-203), or None
     masked_meg: tp.Optional[torch.Tensor] = None     # [B,C,T] buffer that receives meg * channel_mask
+    # several input streams (simpleconv.py:150-196, 234-243).  This plan's own layers are encoder 0: "meg", or "concat"
+    # over every stream; `encoders` are the others, each with its own layer plan
+    streams: tp.Tuple[str, ...] = ()                 # the input streams other than "meg", in argument order
+    encoders: tp.Tuple[tp.Tuple[str, SequencePlan], ...] = ()
+    concatenate: bool = False
 
 
 def _empty(shape, like, dtype=torch.float32):
@@ -763,7 +768,9 @@ def _subject_bwd(g, x, subj_w, subject, shape, ld, want_dx, want_dw):
 def front_forward(plan: "EncoderPlan", meg, heads, il_w, il_b, subj_w, sub_emb, w0, nd: "_Needs", save: bool, status):
     """meg [B,C,T] -> (x [B,T,Dp] channels-last input of conv layer 0, conv0 = layer 0's prepared `_Conv` of weight w0 with
     its input padded to Dp, the record `front_backward` reads).  heads, (il_w, il_b), subj_w, sub_emb [B,E]: the stages'
-    parameters, None where a stage is absent.  `save`: a backward will run.
+    parameters, None where a stage is absent.  `save`: a backward will run.  w0 None (concatenate: layer 0 reads the
+    joined streams, whose width the caller pads): conv0 is None; x is still zero-padded to a multiple of 64 channels in
+    the complete chain on the tensor cores (rec["width"]: its valid columns, rec["pad_width"]: its row length).
 
     Kernel choice: the tensor-core stages run only in the complete chain (merger, initial_linear and subject layers, no
     subject embedding), each where its padded widths pass the shape gates; a complete chain whose initial_linear is not on
@@ -810,7 +817,9 @@ def front_forward(plan: "EncoderPlan", meg, heads, il_w, il_b, subj_w, sub_emb, 
         rec.update(emb=emb, att=att)
 
     conv0 = il_conv = None
-    if chain:
+    if chain and w0 is None and plan.use_tensor_cores:
+        Dp = _round_up(D, 64)        # concatenate: x0 padded as for layer 0, so the subject layers keep their tensor-core form
+    elif chain and w0 is not None:
         # x0 kept zero-padded to a multiple of 64 channels when the tensor-core conv follows
         Dp = _round_up(D, 64)
         conv0 = _Conv(w0, T, False, plan.use_tensor_cores, pad_cin_to=Dp, want_bwd=want_bwd0)
@@ -889,10 +898,11 @@ def front_forward(plan: "EncoderPlan", meg, heads, il_w, il_b, subj_w, sub_emb, 
             _subject_fwd(v, subj_w, plan.subject, x)
     if sub_emb is not None:                                    # ScaledEmbedding appended as channels (simpleconv.py:231-233)
         x = torch.cat([x, sub_emb[:, None, :].expand(B, T, sub_emb.shape[1])], dim=2).contiguous()
-    if conv0 is None:
+    if conv0 is None and w0 is not None:
         conv0 = _Conv(w0, T, False, plan.use_tensor_cores, want_bwd=want_bwd0)
     # u and v (the initial_linear and subject-layer inputs) are read by those stages' weight gradients only
-    rec.update(u=u if n_il_w else None, v=v if n_subj else None, il_conv=il_conv, widths=(O, IL, D), pads=(Op, ILp, Dp))
+    rec.update(u=u if n_il_w else None, v=v if n_subj else None, il_conv=il_conv, widths=(O, IL, D), pads=(Op, ILp, Dp),
+               width=D + (0 if sub_emb is None else sub_emb.shape[1]), pad_width=x.shape[2])
     return x, conv0, rec
 
 
@@ -1029,10 +1039,13 @@ def front_backward(plan: "EncoderPlan", rec, g, heads, il_w, subj_w, sub_emb, ne
 # The output head (simpleconv.py:185-193, 245): `final` = 1x1 Conv1d [2H,H] -> activation -> 1x1 ConvTranspose1d [2H,F] on
 # the channels-last output of the conv stack, handed out channel-major; with complex_out=False only the transpose.
 # ----------------------------------------------------------------------------------------------------
-def head_forward(plan: "EncoderPlan", x, w0, b0, w2, b2, nd: "_Needs", save: bool, B, T, status):
+def head_forward(plan: "EncoderPlan", x, w0, b0, w2, b2, nd: "_Needs", save: bool, B, T, status, want_g=None):
     """x [B,T,H] (the conv stack's output) -> (estimate [B,F,T], the record `head_backward` reads).  w0, b0, w2, b2: the
-    Conv1d and ConvTranspose1d parameters, all None without a head.  `save`: a backward will run.  The form is chosen here:
+    Conv1d and ConvTranspose1d parameters, all None without a head, w0 and b0 None with linear_out.  `save`: a backward
+    will run.  `want_g`: the gradient at x is needed (None: nd.below[-1]).  The form is chosen here:
       bare       no head: the stack already ends on out_channels, the estimate is its transpose;
+      linear     linear_out (simpleconv.py:182-184): the 1x1 ConvTranspose alone as a `_Conv`, storing channel-major from
+                 the tensor-core epilogue where the gates pass, else on FP32 FMA followed by a transpose;
       generic    an activation other than GELU: the two convs as `_Conv`s with the activation kernel between them, then a
                  transpose to channel-major;
       tc         GELU, and both convs pass the tensor-core gates both ways: the GELU and the channel-major store fused into
@@ -1041,17 +1054,29 @@ def head_forward(plan: "EncoderPlan", x, w0, b0, w2, b2, nd: "_Needs", save: boo
                  `bm_head_bwd_params`;
       fma        GELU, a conv gate fails: the FP32-FMA `bm_head_fwd` / `bm_head_bwd`."""
     st = stream()
-    if w0 is None:
+    if w2 is None:
         F = x.shape[2]
         est = _empty((B, F, T), x)
         call("bm_transpose_nt", ptr(x), B, T, F, ptr(est), st)
         return est, dict(form="bare", F=F)
+    n_w0, n_b0, n_w2, _ = nd.head
+    if want_g is None:
+        want_g = nd.below[-1]                        # the gradient at the head's input (the stack's output)
+    tc = plan.use_tensor_cores
+    if w0 is None:
+        H, F = w2.shape[0], w2.shape[1]
+        lin = _Conv(w2.permute(1, 0, 2).contiguous(), T, False, tc, want_bwd=save and want_g)    # as a conv: [F, H, 1]
+        est = _empty((B, F, T), x)
+        if lin.fwd_tc:
+            lin.run_tc(True, x, b2.contiguous(), None, B, T, 1, 0, 0, 1, est, None, None, None, status)
+        else:
+            est_cl = _empty((B, T, F), x)
+            lin.forward(x, b2.contiguous(), B, T, 1, est_cl, None, status)
+            call("bm_transpose_nt", ptr(est_cl), B, T, F, ptr(est), st)
+        return est, dict(form="linear", H=H, F=F, want_g=want_g, lin=lin, x_last=x if n_w2 else None)
     H, F = w0.shape[1], w2.shape[1]
     H2 = 2 * H
-    n_w0, n_b0, n_w2, _ = nd.head
-    want_g = nd.below[-1]                            # the gradient at the head's input (the stack's output)
     want_dh1 = want_g or n_w0 or n_b0                # ... and below the head's activation
-    tc = plan.use_tensor_cores
     head0 = _Conv(w0, T, False, tc, want_bwd=save and want_g)                                    # [2H, H, 1]
     head2 = _Conv(w2.permute(1, 0, 2).contiguous(), T, False, tc, want_bwd=save and want_dh1)    # as a conv: [F, 2H, 1]
     h1, q, est = _empty((B, T, H2), x), _empty((B, T, H2), x), _empty((B, F, T), x)
@@ -1091,6 +1116,22 @@ def head_backward(plan: "EncoderPlan", rec, dest, need, B, T, status, side, keep
         call("bm_transpose_nt", ptr(dest), B, rec["F"], T, ptr(g), st)
         return g, None, None, None, None
     H, F = rec["H"], rec["F"]
+    if form == "linear":
+        lin: _Conv = rec["lin"]
+        _, _, n_w2, n_b2 = need
+        dest_t = _empty((B, T, F), dest)
+        call("bm_transpose_nt", ptr(dest), B, F, T, ptr(dest_t), st)
+        dw2 = db2 = g = None
+        if n_w2 or n_b2:                              # the weight contraction on the side stream, in the ConvTranspose layout
+
+            def lin_wgrad():
+                dw, db = lin.backward_weight(dest_t, rec["x_last"], B, T, 1, dest, status, want_w=n_w2, want_b=n_b2)
+                return (None if dw is None else dw.permute(1, 0, 2).contiguous()), db
+            dw2, db2 = _on_side(side if n_w2 else None, keep_alive, lin_wgrad, dest_t, rec["x_last"])
+        if rec["want_g"]:
+            g = _empty((B, T, H), dest)
+            lin.backward_data(dest_t, None, B, T, 1, g, status)
+        return g, None, None, dw2, db2
     H2, rows = 2 * H, B * T
     n_w0, n_b0, n_w2, n_b2 = need
     want_g, want_dh1 = rec["want_g"], rec["want_dh1"]
@@ -1152,62 +1193,174 @@ def head_backward(plan: "EncoderPlan", rec, dest, need, B, T, status, side, keep
 class _Needs:
     """Which gradients a backward is asked for (`ctx.needs_input_grad`, fixed at forward time), stage by stage from the input.
     below[k]: the data gradient at the input of conv layer k is needed, i.e. `meg` or a parameter of an earlier stage
-    requires grad (below[depth]: at the input of the head)."""
+    requires grad (below[depth]: at the input of the head).  With several input streams `streams[i]` is the requires-grad
+    of stream plan.streams[i] and `enc[j]` the needs of encoder plan.encoders[j] (its front: its stream)."""
     front: tp.Tuple[bool, ...]                 # meg, heads, il_w, il_b, subj_w, sub_emb
     head: tp.Tuple[bool, ...]                  # w0, b0, w2, b2
     layer: tp.List[tp.Tuple[bool, ...]]        # conv_w, conv_b, gamma, beta (+ rewrite_w, rewrite_b, scale, post_skip_w)
     glu: tp.Dict[int, tp.Tuple[bool, ...]]     # glu_w, glu_b of the GLU block after layer k
     below: tp.List[bool]
+    streams: tp.Tuple[bool, ...] = ()
+    enc: tp.List["_Needs"] = dataclasses.field(default_factory=list)
 
     @staticmethod
     def of(needs_input_grad, plan: "EncoderPlan") -> "_Needs":
         n = [bool(v) for v in needs_input_grad]
-        depth = len(plan.dilations)
-        layer, at = [], 10
-        for k in range(depth):
-            layer.append(tuple(n[at:at + layer_width(plan, k)]))
-            at += layer_width(plan, k)
-        glu = {}
-        for k in range(depth):
-            if plan.glu_after[k]:
-                glu[k] = tuple(n[at:at + 2])
-                at += 2
         front = tuple(n[1:6]) + ((n[-1],) if plan.has_sub_emb else (False,))
-        below = [any(front)]
-        for k in range(depth):
-            below.append(below[-1] or any(layer[k]) or any(glu.get(k, ())))
-        return _Needs(front=front, head=tuple(n[6:10]), layer=layer, glu=glu, below=below)
+        layer, glu, at = _stack_needs(n, 10, plan)
+        streams = tuple(n[at:at + len(plan.streams)])
+        at += len(plan.streams)
+        below = _below(any(front) or (plan.concatenate and any(streams)), layer, glu)
+        enc = []
+        for name, sp in plan.encoders:
+            e_layer, e_glu, at = _stack_needs(n, at, sp)
+            own = streams[plan.streams.index(name)]
+            enc.append(_Needs(front=(own,), head=(), layer=e_layer, glu=e_glu, below=_below(own, e_layer, e_glu)))
+        return _Needs(front=front, head=tuple(n[6:10]), layer=layer, glu=glu, below=below, streams=streams, enc=enc)
 
     def layer_up(self, k: int) -> bool:
         """the gradient at layer k's output (below its GLU block) is needed"""
         return self.below[k] or any(self.layer[k])
 
 
+def _stack_needs(n, at, plan: SequencePlan):
+    """(layer, glu, next position) of the requires-grad flags n[at:] of one encoder's layer parameters"""
+    layer, glu = [], {}
+    for k in range(len(plan.dilations)):
+        layer.append(tuple(n[at:at + layer_width(plan, k)]))
+        at += layer_width(plan, k)
+    for k in range(len(plan.dilations)):
+        if plan.glu_after[k]:
+            glu[k] = tuple(n[at:at + 2])
+            at += 2
+    return layer, glu, at
+
+
+def _below(first, layer, glu):
+    below = [first]
+    for k in range(len(layer)):
+        below.append(below[-1] or any(layer[k]) or any(glu.get(k, ())))
+    return below
+
+
+def _stack_params(plan: SequencePlan, flat):
+    """(conv_p, glu_p, rest) of one encoder's parameters at the front of `flat` (see `_EncoderFn`)"""
+    conv_p, at = [], 0
+    for k in range(len(plan.dilations)):
+        conv_p.append(flat[at:at + layer_width(plan, k)])
+        at += layer_width(plan, k)
+    glu_p = {}
+    for k in range(len(plan.dilations)):
+        if plan.glu_after[k]:
+            glu_p[k] = flat[at:at + 2]
+            at += 2
+    return conv_p, glu_p, flat[at:]
+
+
+# ----------------------------------------------------------------------------------------------------
+# Several input streams (simpleconv.py:234-243): `bm_channel_join` places channel-major raw streams and channels-last
+# activations side by side in one channels-last tensor, `bm_channel_split` hands each column range's gradient back.
+# ----------------------------------------------------------------------------------------------------
+def _view_ptr(t):
+    """Device pointer of a channel-major [B, C, T] view whose channel stride is >= T and sample stride C * stride(1)"""
+    assert t.is_cuda, "brainmagick_b200 kernels need CUDA tensors (no CPU fallback)"
+    return _lib.c_void_p(t.data_ptr())
+
+
+def channel_major_operand(x):
+    """(x or a contiguous copy, its channel stride) for `bm_channel_join` / `bm_channel_split`: a view cropped in time (the
+    solver's offset crop) is read in place"""
+    B, C, T = x.shape
+    if x.is_contiguous():
+        return x, T
+    ld = x.stride(1)
+    if x.stride(2) == 1 and ld >= T and (B == 1 or x.stride(0) == C * ld):
+        return x, ld
+    return x.contiguous(), T
+
+
+def channel_join(parts, B, T, Cp, like):
+    """parts [(tensor, C, cm, col)], cm: the tensor is channel-major [B, C, T] (else channels-last [B, T, C]) -> [B, T, Cp]
+    channels-last, the parts in their columns and every other column zero"""
+    out = _empty((B, T, Cp), like)
+    args = []
+    for t, C, cm, col in parts:
+        if cm:
+            t, ld = channel_major_operand(t)
+            args += [ptr(t) if t.is_contiguous() else _view_ptr(t), C, ld, 1, col]
+        else:
+            args += [ptr(t), C, t.shape[2], 0, col]
+    args += [None, 0, 0, 0, 0] * (4 - len(parts))
+    call("bm_channel_join", B, T, Cp, len(parts), *args, ptr(out), stream())
+    return out
+
+
+def channel_split(g, parts):
+    """g [B, T, Cp] -> the tensors of parts [(C, cm, col, wanted[, ld])]: [B, C, T] if cm else [B, T, ld] (ld default C,
+    the columns past C zero), None where not wanted"""
+    B, T, Cp = g.shape
+    outs, args = [], []
+    for C, cm, col, wanted, *rest in parts:
+        ld = rest[0] if rest and not cm else (T if cm else C)
+        o = None
+        if wanted:
+            o = _empty((B, C, T), g) if cm else \
+                (torch.zeros((B, T, ld), device=g.device) if ld > C else _empty((B, T, C), g))
+        outs.append(o)
+        args += [ptr(o), C, ld, int(cm), col]
+    args += [None, 0, 0, 0, 0] * (4 - len(parts))
+    if any(o is not None for o in outs):
+        call("bm_channel_split", ptr(g), B, T, Cp, len(parts), *args, stream())
+    return outs
+
+
+def stack_conv0(w0, T, width, tc, skip, want_bwd, fit_wgrad=False):
+    """(layer 0's `_Conv`, Cp): its input zero-padded to Cp = a multiple of 64 channels when the tensor-core conv takes it
+    (a layer 0 with a residual keeps the true width), as the stand-alone ConvSequence pads its input.  `fit_wgrad`: pad
+    by up to two more 64-channel steps where that puts the layer's weight gradient on the tensor cores too (a joined
+    width such as 390 -> 448 misses the weight-gradient gate, 512 passes it)."""
+    if w0.shape[1] != width:
+        raise ValueError(f"layer 0 takes {w0.shape[1]} input channels, the input has {width}")
+    Cp = width if (skip and w0.shape[0] == width) else _round_up(width, 64)
+    if fit_wgrad and tc and Cp != width:
+        lib = _lib.load()
+        for extra in (0, 64, 128):
+            if lib.bm_tc_wgrad_supported(w0.shape[0], Cp + extra):
+                Cp += extra
+                break
+    conv0 = _Conv(w0, T, False, tc, pad_cin_to=Cp, want_bwd=want_bwd)
+    if not conv0.fwd_tc and Cp != width:
+        Cp = width
+        conv0 = _Conv(w0, T, False, False, want_bwd=want_bwd)
+    return conv0, Cp
+
+
 class _EncoderFn(torch.autograd.Function):
-    """inputs: plan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, then per layer k: (conv_w, conv_b, gamma, beta)
-    (+ (rewrite_w, rewrite_b, layer_scale, post_skip_w) on a layer with a residual-branch option, see `layer_width`) and,
-    appended in layer order, (glu_w, glu_b) for every layer followed by a GLU block.
+    """inputs: plan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, then per layer k of encoder 0: (conv_w, conv_b, gamma,
+    beta) (+ (rewrite_w, rewrite_b, layer_scale, post_skip_w) on a layer with a residual-branch option, see `layer_width`)
+    and, appended in layer order, (glu_w, glu_b) for every layer followed by a GLU block; then the input streams of
+    plan.streams, then the layer parameters of each encoder of plan.encoders laid out like encoder 0's, then the [B, E]
+    subject-embedding rows when plan.has_sub_emb.
+
+    Encoder 0 reads the front's output ("meg"), or with plan.concatenate the join of the front's output and the raw streams
+    in sorted key order ("concat"); every other encoder reads its raw stream.  With several encoders their outputs are
+    joined in sorted key order before the head (simpleconv.py:234-243).
 
     Only what requires grad is backpropagated: a frozen parameter's gradient is not computed, the backward stops at the
     deepest stage that still needs a data gradient, and the forward saves only what those gradients read (nothing when no
     tensor argument requires grad: it then issues the calls of a `torch.no_grad()` forward)."""
 
     @staticmethod
-    def forward(ctx, plan: EncoderPlan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, *layer_params):
-        depth = len(plan.dilations)
+    def forward(ctx, plan: EncoderPlan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, *params):
         sub_emb = None
         if plan.has_sub_emb:                     # [B, E] rows of the (scaled) subject embedding, appended by the caller
-            sub_emb, layer_params = layer_params[-1], layer_params[:-1]
-        conv_p, at = [], 0
-        for k in range(depth):
-            conv_p.append(layer_params[at:at + layer_width(plan, k)])
-            at += layer_width(plan, k)
-        glu_flat = layer_params[at:]
-        glu_p, gi = {}, 0
-        for k in range(depth):
-            if plan.glu_after[k]:
-                glu_p[k] = glu_flat[2 * gi:2 * gi + 2]
-                gi += 1
+            sub_emb, params = params[-1], params[:-1]
+        conv_p, glu_p, params = _stack_params(plan, params)
+        xs, params = params[:len(plan.streams)], params[len(plan.streams):]
+        enc_p = []
+        for _, sp in plan.encoders:
+            e_conv, e_glu, params = _stack_params(sp, params)
+            enc_p.append((e_conv, e_glu))
         st = stream()
         meg = meg.contiguous()
         B, C, T = meg.shape
@@ -1219,12 +1372,49 @@ class _EncoderFn(torch.autograd.Function):
         save = plan.keep_for_backward and any(ctx.needs_input_grad)
         status = tc_status_tensor(meg.device)
 
-        x, conv0, front = front_forward(plan, meg, heads, il_w, il_b, subj_w, sub_emb, conv_p[0][0], nd, save, status)
+        x, conv0, front = front_forward(plan, meg, heads, il_w, il_b, subj_w, sub_emb,
+                                        None if plan.concatenate else conv_p[0][0], nd, save, status)
+        join_in = None
+        if plan.concatenate:
+            # "concat" reads the streams joined in sorted key order, zero-padded for layer 0 as a stand-alone input
+            # the front's x keeps its tensor-core padding (rows of x.shape[2]); the join reads its valid columns
+            widths = dict(zip(plan.streams, (t.shape[1] for t in xs)), meg=front["width"])
+            cols, at = {}, 0
+            for name in sorted(widths):
+                cols[name] = at
+                at += widths[name]
+            conv0, Cp = stack_conv0(conv_p[0][0], T, at, plan.use_tensor_cores, plan.skip, save and nd.below[0],
+                                    fit_wgrad=True)
+            parts = [(x, widths["meg"], False, cols["meg"]) if name == "meg" else
+                     (xs[plan.streams.index(name)], widths[name], True, cols[name]) for name in sorted(widths)]
+            x = channel_join(parts, B, T, Cp, meg)
+            join_in = (widths, cols, front["pad_width"])
         x, layers = conv_stack_forward(plan, x, conv0, conv_p, glu_p, nd, save, B, T, status, bare_slope=0.0)
-        est, head = head_forward(plan, x, w0, b0, w2, b2, nd, save, B, T, status)
+        outs = {"concat" if plan.concatenate else "meg": x}
+        enc_layers = []
+        for (name, sp), (e_conv, e_glu), e_nd in zip(plan.encoders, enc_p, nd.enc):
+            xi = xs[plan.streams.index(name)]
+            c0, Cp = stack_conv0(e_conv[0][0], T, xi.shape[1], sp.use_tensor_cores, sp.skip, save and e_nd.below[0],
+                                 fit_wgrad=True)
+            x0 = channel_join([(xi, xi.shape[1], True, 0)], B, T, Cp, meg)
+            outs[name], e_layers = conv_stack_forward(sp, x0, c0, e_conv, e_glu, e_nd, save, B, T, status, bare_slope=0.0)
+            enc_layers.append((e_layers, Cp))
+        want_top = nd.below[-1] or any(e.below[-1] for e in nd.enc)
+        out_cols = None
+        if len(outs) > 1:
+            out_cols, at = {}, 0
+            for name in sorted(outs):
+                out_cols[name] = at
+                at += outs[name].shape[2]
+            x = channel_join([(outs[name], outs[name].shape[2], False, out_cols[name]) for name in sorted(outs)],
+                             B, T, at, meg)
+        est, head = head_forward(plan, x, w0, b0, w2, b2, nd, save, B, T, status, want_g=want_top)
         if save:
             ctx.plan, ctx.needs, ctx.dims = plan, nd, (B, T)
-            ctx.saved = dict(front=front, layers=layers, conv_p=conv_p, head=head, params=(heads, il_w, subj_w, sub_emb))
+            ctx.saved = dict(front=front, layers=layers, conv_p=conv_p, head=head, params=(heads, il_w, subj_w, sub_emb),
+                             enc=[(e_conv, e_layers, Cp) for (e_conv, _), (e_layers, Cp) in zip(enc_p, enc_layers)],
+                             widths={k: v.shape[2] for k, v in outs.items()}, out_cols=out_cols, join_in=join_in,
+                             stream_widths=[t.shape[1] for t in xs])
         return est
 
     @staticmethod
@@ -1245,31 +1435,64 @@ class _EncoderFn(torch.autograd.Function):
         side = _side_stream(dest.device) if (OVERLAP_WGRAD and plan.use_tensor_cores) else None
         ctx_keep: tp.List[tp.Any] = []
         g, *head_grads = head_backward(plan, s["head"], dest, nd.head, B, T, status, side, ctx_keep)
-        layer_grads, glu_grads, g = conv_stack_backward(plan, s["conv_p"], s["layers"], g, nd, B, T, status, side=side,
-                                                        keep_alive=ctx_keep)
+        name0 = "concat" if plan.concatenate else "meg"
+        g_enc = dict([(name0, g)] + [(name, None) for name, _ in plan.encoders])
+        if s["out_cols"] is not None and g is not None:     # the head's input gradient, split per encoder
+            wanted = dict([(name0, nd.below[-1])] + [(name, e.below[-1]) for (name, _), e in zip(plan.encoders, nd.enc)])
+            names = sorted(s["out_cols"])
+            g_enc = dict(zip(names, channel_split(g, [(s["widths"][n], False, s["out_cols"][n], wanted[n]) for n in names])))
+        layer_grads, glu_grads, g = conv_stack_backward(plan, s["conv_p"], s["layers"], g_enc[name0], nd, B, T, status,
+                                                        side=side, keep_alive=ctx_keep)
+        stream_grads = [None] * len(plan.streams)
+        enc_grads = []
+        for (name, sp), (e_conv, e_layers, Cp), e_nd in zip(plan.encoders, s["enc"], nd.enc):
+            e_lg, e_gg, e_g = conv_stack_backward(sp, e_conv, e_layers, g_enc[name], e_nd, B, T, status, side=side,
+                                                  keep_alive=ctx_keep)
+            enc_grads.append((e_lg, e_gg))
+            i = plan.streams.index(name)
+            if nd.streams[i]:                            # inputs[name].grad, channel-major
+                stream_grads[i] = channel_split(e_g, [(s["stream_widths"][i], True, 0, True)])[0]
         if ctx_keep:                                   # something ran on the side stream
             torch.cuda.current_stream().wait_stream(side)
         ctx_keep.clear()
+        if s["join_in"] is not None and nd.below[0]:    # "concat": the layer-0 input gradient back to the front and streams
+            widths, cols, meg_ld = s["join_in"]
+            wanted = dict(zip(plan.streams, nd.streams), meg=any(nd.front))
+            names = sorted(widths)
+            parts = channel_split(g, [(widths[n], n != "meg", cols[n], wanted[n], meg_ld) for n in names])
+            got = dict(zip(names, parts))
+            g = got["meg"]
+            stream_grads = [got[n] for n in plan.streams]
         dheads = d_il_w = d_il_b = d_subj = d_sub_emb = dmeg = None
-        if nd.below[0]:                                # else the sensor side is frozen and meg does not require grad
+        if any(nd.front):                              # else the sensor side is frozen and meg does not require grad
             dheads, d_il_w, d_il_b, d_subj, d_sub_emb, dmeg = front_backward(plan, s["front"], g, *s["params"], nd.front,
                                                                              status)
         grads = [None, dmeg, dheads, d_il_w, d_il_b, d_subj, *head_grads]
-        for k in range(depth):
-            grads.extend(layer_grads[k])
-        for k in range(depth):
-            if plan.glu_after[k]:
-                grads.extend(glu_grads[k])
+        _extend_stack_grads(grads, plan, layer_grads, glu_grads)
+        grads.extend(stream_grads)
+        for (_, sp), (e_lg, e_gg) in zip(plan.encoders, enc_grads):
+            _extend_stack_grads(grads, sp, e_lg, e_gg)
         if plan.has_sub_emb:
             grads.append(d_sub_emb)
         ctx.saved = None
         return tuple(grads)
 
 
-def encoder_forward(plan: EncoderPlan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, layer_params, sub_emb=None):
-    """`sub_emb` [B, E]: rows of the scaled subject embedding to append as channels (plan.has_sub_emb)."""
+def _extend_stack_grads(grads, plan: SequencePlan, layer_grads, glu_grads):
+    for k in range(len(plan.dilations)):
+        grads.extend(layer_grads[k])
+    for k in range(len(plan.dilations)):
+        if plan.glu_after[k]:
+            grads.extend(glu_grads[k])
+
+
+def encoder_forward(plan: EncoderPlan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, layer_params, sub_emb=None,
+                    streams=(), encoder_params=()):
+    """`sub_emb` [B, E]: rows of the scaled subject embedding to append as channels (plan.has_sub_emb).  `streams`: the
+    [B, C_s, T] tensors of plan.streams; `encoder_params`: the flat layer parameters of each encoder of plan.encoders."""
     extra = [] if sub_emb is None else [sub_emb]
-    return _EncoderFn.apply(plan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, *layer_params, *extra)
+    enc = [p for params in encoder_params for p in params]
+    return _EncoderFn.apply(plan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, *layer_params, *streams, *enc, *extra)
 
 
 # ----------------------------------------------------------------------------------------------------

@@ -13,6 +13,11 @@ or replaced by a subject embedding -- every row of the paper's ablation table (g
 The un-ablated configuration takes the fused tensor-core path; a missing sensor stage switches the sensor chain to
 its stage-by-stage form.  Options outside that family are accepted by the
 signature but raise NotImplementedError (SURVEY.md 8(f) row 4).
+
+Encoding models (bm/train.py:61-67) take more input streams than "meg", e.g. in_channels=dict(meg=C, features=F): the
+sensor front acts on "meg" (always required), every other stream enters its own encoder as is, and the encoder outputs
+are joined in sorted key order before the head -- `linear_out` (one 1x1 ConvTranspose) or `complex_out`; with
+`concatenate` one encoder "concat" reads the streams joined in sorted key order (simpleconv.py:150-196, 234-243).
 """
 from __future__ import annotations
 
@@ -92,11 +97,15 @@ class SimpleConv(nn.Module):
             raise ValueError("Channels and hidden keys must match "
                              f"({set(in_channels.keys())} and {set(hidden.keys())})")
         assert kernel_size % 2 == 1, "For padding to work, this must be verified"
+        if "meg" not in in_channels:
+            raise NotImplementedError("SimpleConv's sensor front is built around the 'meg' stream: in_channels needs it")
+        if len(in_channels) > 4:
+            raise NotImplementedError("SimpleConv joins at most 4 input streams (the channel-join kernel takes 4 sources); "
+                                      f"got {sorted(in_channels)}")
+        self._stream_channels = {name: c for name, c in in_channels.items() if name != "meg"}
         off_path = dict(
-            concatenate=concatenate, linear_out=linear_out, growth=growth != 1.,
-            dual_path=bool(dual_path), n_fft=n_fft is not None, dropout=dropout > 0.,
-            initial_depth=initial_depth != 1, initial_nonlin=initial_nonlin,
-            inputs=set(in_channels) != {"meg"})
+            growth=growth != 1., dual_path=bool(dual_path), n_fft=n_fft is not None, dropout=dropout > 0.,
+            initial_depth=initial_depth != 1, initial_nonlin=initial_nonlin)
         bad = [k for k, v in off_path.items() if v]
         if bad:
             raise NotImplementedError(
@@ -145,33 +154,46 @@ class SimpleConv(nn.Module):
             activation, make_act = None, (lambda: nn.LeakyReLU(relu_leakiness))    # ConvSequence builds the same module
         else:
             activation, make_act = nn.ReLU, nn.ReLU
-        sizes = [in_channels["meg"]] + [int(round(hidden["meg"] * growth ** k)) for k in range(depth)]
-        final_channels = sizes[-1]
+        self._streams = [name for name in in_channels if name != "meg"]      # the streams that enter their encoder as is
+        if concatenate:                          # simpleconv.py:150-153: one encoder over the streams joined by sorted key
+            in_channels = {"concat": sum(in_channels.values())}
+            hidden = {"concat": sum(hidden.values())}
+        sizes = {name: [in_channels[name]] + [int(round(hidden[name] * growth ** k)) for k in range(depth)]
+                 for name in in_channels}
+        final_channels = sum(s[-1] for s in sizes.values())
         seq_kw = {}
-        if complex_out:
+        if linear_out:                           # simpleconv.py:182-184
+            assert not complex_out
+            self.final = nn.ConvTranspose1d(final_channels, out_channels, 1, 1, 0)
+        elif complex_out:
             self.final = nn.Sequential(
                 nn.Conv1d(final_channels, 2 * final_channels, 1),
                 make_act(),
                 nn.ConvTranspose1d(2 * final_channels, out_channels, 1, 1, 0))
         else:
             # simpleconv.py:190-193: no head; the last convolution maps to out_channels, without BatchNorm / activation
+            assert len(sizes) == 1, "if no linear_out, there must be a single branch."
             self.final = None
             seq_kw["activation_on_last"] = False
-            sizes[-1] = out_channels
-        self.encoders = nn.ModuleDict({"meg": ConvSequence(
-            sizes, kernel=kernel_size, stride=1, leakiness=relu_leakiness, dropout=conv_dropout,
+            list(sizes.values())[0][-1] = out_channels
+        self.encoders = nn.ModuleDict({name: ConvSequence(
+            channels, kernel=kernel_size, stride=1, leakiness=relu_leakiness, dropout=conv_dropout,
             dropout_input=dropout_input, batch_norm=batch_norm, dilation_growth=dilation_growth, groups=groups,
             dilation_period=dilation_period, skip=skip, post_skip=post_skip, scale=scale, rewrite=rewrite, glu=glu,
-            glu_context=glu_context, glu_glu=glu_glu, activation=activation, **seq_kw)})
-        if not self.encoders["meg"].clip_conv_family:
+            glu_context=glu_context, glu_glu=glu_glu, activation=activation, **seq_kw) for name, channels in sizes.items()})
+        if not all(seq.clip_conv_family for seq in self.encoders.values()):
             raise NotImplementedError("SimpleConv's fused encoder needs batch_norm=True; "
                                       "see SURVEY.md 8(f) row 4")
         self._freq: tp.Optional[torch.Tensor] = None
         self.use_tensor_cores = True     # False forces the FP32-FMA kernels everywhere (debugging / A-B timing)
 
     # ------------------------------------------------------------------------------------------------
-    def _layer_params(self):
-        seq: ConvSequence = self.encoders["meg"]
+    def _encoder0(self) -> str:
+        """The encoder that follows the sensor front: "meg", or "concat" over every stream"""
+        return "concat" if self._concatenate else "meg"
+
+    @staticmethod
+    def _layer_params(seq: ConvSequence):
         out = []
         for k, block in enumerate(seq.sequence):
             conv = block[0]
@@ -186,8 +208,24 @@ class SimpleConv(nn.Module):
                 out += [glu[0].weight, glu[0].bias]
         return out
 
+    def _sequence_fields(self, seq: ConvSequence) -> dict:
+        """The `functional.SequencePlan` fields of one encoder"""
+        bn_buffers = [(blk[1].running_mean, blk[1].running_var) if seq.has_act[k] else None
+                      for k, blk in enumerate(seq.sequence)]
+        bn0 = seq.sequence[0][1]
+        if bn0.momentum is None:
+            raise NotImplementedError("BatchNorm cumulative-average mode (momentum=None)")
+        residual = seq.residual()
+        bn_groups = BF.bn_sync_groups([blk[1] if seq.has_act[k] else None for k, blk in enumerate(seq.sequence)], residual)
+        return dict(
+            dilations=list(seq.dilations), glu_after=seq.glu_after(), training=self.training, bn_eps=bn0.eps,
+            bn_momentum=bn0.momentum, bn_buffers=bn_buffers, keep_for_backward=torch.is_grad_enabled(),
+            use_tensor_cores=self.use_tensor_cores, skip=seq.skip, act_code=seq.act_code, act_slope=seq.act_slope,
+            has_act=list(seq.has_act), batch_norm=True, residual=residual, rewrite_slope=seq.rewrite_slope,
+            scale_boost=seq.scale_boost(), bn_groups=bn_groups)
+
     def _plan(self, meg: torch.Tensor, batch) -> BF.EncoderPlan:
-        seq: ConvSequence = self.encoders["meg"]
+        seq: ConvSequence = self.encoders[self._encoder0()]
         device = meg.device
         B, C, _ = meg.shape
         if self.merger is None:                 # no spatial attention: the layout tables are never read
@@ -198,32 +236,40 @@ class SimpleConv(nn.Module):
             pos, rec_of_sample, rec_order, rec_off = self.merger.position_getter.batch_layout(batch, C, device)
             if self._freq is None or self._freq.device != device:
                 self._freq = self.merger.embedding.frequencies().to(device)
-        bn_buffers = [(blk[1].running_mean, blk[1].running_var) if seq.has_act[k] else None
-                      for k, blk in enumerate(seq.sequence)]
-        bn0 = seq.sequence[0][1]
-        if bn0.momentum is None:
-            raise NotImplementedError("BatchNorm cumulative-average mode (momentum=None)")
-        residual = seq.residual()
-        bn_groups = BF.bn_sync_groups([blk[1] if seq.has_act[k] else None for k, blk in enumerate(seq.sequence)], residual)
+        fields = self._sequence_fields(seq)
+        encoders = tuple((name, BF.SequencePlan(**self._sequence_fields(self.encoders[name])))
+                         for name in self.encoders if name != self._encoder0())
         return BF.EncoderPlan(
-            dilations=list(seq.dilations), glu_after=seq.glu_after(), kernel_size=seq.kernel,
-            glu_kernel=seq.glu_kernel, training=self.training, bn_eps=bn0.eps, bn_momentum=bn0.momentum,
+            **fields, kernel_size=seq.kernel, glu_kernel=seq.glu_kernel,
             rec_positions=pos, rec_of_sample=rec_of_sample, rec_order=rec_order, rec_off=rec_off,
             subject=batch.subject_index.to(device=device, dtype=torch.int32).contiguous(),
             freq=self._freq, ban_centre=None if self.merger is None else self.merger.draw_ban_centre(device),
             ban_radius=0.0 if self.merger is None else float(self.merger.dropout),
-            bn_buffers=bn_buffers, keep_for_backward=torch.is_grad_enabled(),
-            use_tensor_cores=self.use_tensor_cores, skip=seq.skip, act_code=seq.act_code, act_slope=seq.act_slope,
-            has_act=list(seq.has_act), batch_norm=True, has_sub_emb=self.subject_embedding is not None,
-            residual=residual, rewrite_slope=seq.rewrite_slope, scale_boost=seq.scale_boost(), bn_groups=bn_groups)
+            has_sub_emb=self.subject_embedding is not None, streams=tuple(self._streams), encoders=encoders,
+            concatenate=self._concatenate)
 
     def forward(self, inputs, batch):
+        """inputs: {"meg": [B, C, T], and every other stream of in_channels: [B, C_s, T]}, CUDA fp32 tensors (a stream may
+        be a view, e.g. cropped in time); the sensor front (merger, initial_linear, subject layers / embedding) acts on
+        "meg", which is always required.  Gradients reach every parameter and each input tensor that requires grad."""
         meg = inputs["meg"]
         _require_cuda(meg)
         if meg.dtype != torch.float32:
             raise TypeError("brainmagick_b200.SimpleConv computes in fp32, like the reference")
         assert meg.shape[1] == self.n_input_channels, "number of MEG channels differs from in_channels['meg']"
         length = meg.shape[-1]
+        streams = []
+        for name in self._streams:
+            x = inputs[name]
+            _require_cuda(x)
+            if x.dtype != torch.float32 or x.dim() != 3:
+                raise TypeError(f"brainmagick_b200.SimpleConv: inputs[{name!r}] must be an fp32 [B, C, T] tensor")
+            if x.shape[0] != meg.shape[0] or x.shape[2] != length:
+                raise ValueError(f"inputs[{name!r}] has shape {tuple(x.shape)}; every stream needs meg's B and T")
+            if x.shape[1] != self._stream_channels[name]:
+                raise ValueError(f"inputs[{name!r}] has {x.shape[1]} channels; in_channels[{name!r}] is "
+                                 f"{self._stream_channels[name]}")
+            streams.append(x)
         plan = self._plan(meg, batch)
         if self.subsampled_meg_channels is not None:         # simpleconv.py:200-203, applied inside the encoder node
             if self._channel_mask is None or self._channel_mask.device != meg.device:
@@ -239,12 +285,18 @@ class SimpleConv(nn.Module):
         sub_emb = None
         if self.subject_embedding is not None:           # [B, E]; its gradient returns through torch's embedding backward
             sub_emb = self.subject_embedding(batch.subject_index.to(meg.device).long())
-        head = [None] * 4 if self.final is None else \
-            [self.final[0].weight, self.final[0].bias, self.final[2].weight, self.final[2].bias]
-        est = BF.encoder_forward(plan, meg, heads, il_w, il_b, subj_w, *head, self._layer_params(), sub_emb=sub_emb)
+        if self.final is None:
+            head = [None] * 4
+        elif isinstance(self.final, nn.ConvTranspose1d):    # linear_out
+            head = [None, None, self.final.weight, self.final.bias]
+        else:
+            head = [self.final[0].weight, self.final[0].bias, self.final[2].weight, self.final[2].bias]
+        est = BF.encoder_forward(plan, meg, heads, il_w, il_b, subj_w, *head,
+                                 self._layer_params(self.encoders[self._encoder0()]), sub_emb=sub_emb, streams=streams,
+                                 encoder_params=[self._layer_params(self.encoders[name]) for name, _ in plan.encoders])
         if self.training:
-            seq: ConvSequence = self.encoders["meg"]
-            for k, blk in enumerate(seq.sequence):   # nn.BatchNorm1d bookkeeping (running stats were updated on device)
-                if seq.has_act[k]:
-                    blk[1].num_batches_tracked += 1
+            for seq in self.encoders.values():   # nn.BatchNorm1d bookkeeping (running stats were updated on device)
+                for k, blk in enumerate(seq.sequence):
+                    if seq.has_act[k]:
+                        blk[1].num_batches_tracked += 1
         return est[:, :, :length]

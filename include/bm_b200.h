@@ -396,6 +396,20 @@ int bm_channel_mask(const float* x, const float* mask, int B, int C, int T, floa
 int bm_transpose_nt(const float* in, int Z, int N, int T, float* out, bm_stream_t stream);
 /* same with an output row stride ld_out >= N (pad columns written as zeros): meg [B,C,T] -> channels-last, channel-padded. */
 int bm_transpose_nt_ld(const float* in, int Z, int N, int T, int ld_out, float* out, bm_stream_t stream);
+/* Channel join of SimpleConv's input streams / encoder outputs (bm/models/simpleconv.py:234-243): dst [B,T,Cp]
+ * channels-last receives n (1..4) sources side by side, source i in columns [col_i, col_i + C_i) (ranges must not
+ * overlap); every column no source covers is written as zero.  Source i is channels-last (cm_i = 0: rows of stride
+ * ld_i >= C_i, an encoder output or the front's x0) or channel-major (cm_i = 1: [B, C_i, T] with channel stride ld_i >= T
+ * and sample stride C_i * ld_i, e.g. a raw input stream cropped in time), transposed on the way.  Slots i >= n are
+ * ignored.  An exact copy: deterministic, the same under TF32.  B <= 65535. */
+int bm_channel_join(int B, int T, int Cp, int n, const float* src0, int C0, int ld0, int cm0, int col0,
+                    const float* src1, int C1, int ld1, int cm1, int col1, const float* src2, int C2, int ld2, int cm2,
+                    int col2, const float* src3, int C3, int ld3, int cm3, int col3, float* dst, bm_stream_t stream);
+/* The reverse, for the gradients: src [B,T,Cp]; dst_i receives columns [col_i, col_i + C_i) in the layout (cm_i, ld_i)
+ * of bm_channel_join's sources.  dst_i NULL: that range is not wanted. */
+int bm_channel_split(const float* src, int B, int T, int Cp, int n, float* dst0, int C0, int ld0, int cm0, int col0,
+                     float* dst1, int C1, int ld1, int cm1, int col1, float* dst2, int C2, int ld2, int cm2, int col2,
+                     float* dst3, int C3, int ld3, int cm3, int col3, bm_stream_t stream);
 
 /* ---- Deterministic forms (torch.use_deterministic_algorithms(True) in the drop-in modules) -------------------------
  * Every `_det` entry point computes what its default form computes, with the same arguments plus (where noted) a
