@@ -33,6 +33,8 @@ SIGNATURES = {
     "bm_conv1d_fwd": [P, P, P, I, I, I, I, I, I, P, P, P],
     "bm_bn_stats_finalize": [P, L, F, F, P, P, P, P, I, P],
     "bm_bn_stats_finalize_counted": [P, F, F, P, P, P, P, I, P],
+    "bm_bn_stats_finalize_cumulative": [P, L, F, P, P, P, P, P, I, P],
+    "bm_bn_stats_finalize_counted_cumulative": [P, F, P, P, P, P, P, I, P],
     "bm_bn_eval_stats": [P, P, F, P, P, I, P],
     "bm_bn_gelu_skip_fwd": [P, P, P, P, P, P, P, L, I, P, P],
     "bm_bn_gelu_skip_bwd": [P, P, P, P, P, P, I, L, I, P, P, P, P, P, P],

@@ -20,8 +20,8 @@ import torch
 
 from . import _lib
 from ._lib import call, ptr, stream
-from .functional import (SequencePlan, _Needs, _empty, bn_sync_groups, conv_stack_backward, conv_stack_forward,
-                         layer_width, stack_conv0, tc_status_tensor)
+from .functional import (SequencePlan, _Needs, _empty, bn_count_batches, bn_plan_fields, bn_sync_groups,
+                         conv_stack_backward, conv_stack_forward, layer_width, stack_conv0, tc_status_tensor)
 
 
 def _present(plan: SequencePlan, k: int) -> tp.List[bool]:
@@ -140,40 +140,26 @@ def conv_sequence(module, x: torch.Tensor) -> torch.Tensor:
         raise TypeError("brainmagick_b200.ConvSequence computes in fp32, like the reference")
     _lib.load()
     params: tp.List[torch.Tensor] = []
-    bn_buffers: tp.List[tp.Any] = []
     bns: tp.List[tp.Any] = []
-    bn0 = None
     for k, block in enumerate(module.sequence):
         conv = block[0]
         params += [conv.weight, conv.bias]
         if module.has_act[k] and module.batch_norm:
             bn = block[1]
-            if bn0 is None:
-                bn0 = bn
             params += [bn.weight, bn.bias]
-            bn_buffers.append((bn.running_mean, bn.running_var))
             bns.append(bn)
         else:
-            bn_buffers.append(None)
             bns.append(None)
         params += [t for t in module.residual_params(k) if t is not None]
     for glu in module.glus:
         if glu is not None:
             params += [glu[0].weight, glu[0].bias]
-    if bn0 is not None and bn0.momentum is None:
-        raise NotImplementedError("BatchNorm cumulative-average mode (momentum=None)")
     residual = module.residual()
     plan = SequencePlan(
         dilations=list(module.dilations), glu_after=module.glu_after(), has_act=list(module.has_act),
         batch_norm=module.batch_norm, act_code=module.act_code, act_slope=module.act_slope, skip=module.skip,
-        training=module.training, bn_eps=bn0.eps if bn0 is not None else 0.0,
-        bn_momentum=bn0.momentum if bn0 is not None else 0.0, bn_buffers=bn_buffers,
-        use_tensor_cores=getattr(module, "use_tensor_cores", True), keep_for_backward=torch.is_grad_enabled(),
-        residual=residual, rewrite_slope=module.rewrite_slope, scale_boost=module.scale_boost(),
-        bn_groups=bn_sync_groups(bns, residual))
-    out = _ConvSequenceFn.apply(plan, x, *params)
-    if module.training and module.batch_norm:
-        for k, block in enumerate(module.sequence):       # nn.BatchNorm1d bookkeeping (running stats updated on device)
-            if module.has_act[k]:
-                block[1].num_batches_tracked += 1
-    return out
+        **bn_plan_fields(bns, module.training), use_tensor_cores=getattr(module, "use_tensor_cores", True),
+        keep_for_backward=torch.is_grad_enabled(), residual=residual, rewrite_slope=module.rewrite_slope,
+        scale_boost=module.scale_boost(), bn_groups=bn_sync_groups(bns, residual))
+    bn_count_batches(bns)           # nn.BatchNorm1d bookkeeping, ahead of the finalize kernels that read it
+    return _ConvSequenceFn.apply(plan, x, *params)

@@ -450,8 +450,18 @@ extern "C" int bm_bn_stats_finalize(const double* stats, long long n, float eps,
                                     bm_stream_t stream) {
     BM_CHECK_ARG(stats && mean && invstd && C > 0 && n > 0);
     BM_CHECK_ARG((running_mean == nullptr) == (running_var == nullptr));
-    bn_finalize_kernel<<<(C + 127) / 128, 128, 0, ST(stream)>>>(stats, (double)n, eps, momentum, running_mean,
+    bn_finalize_kernel<<<(C + 127) / 128, 128, 0, ST(stream)>>>(stats, (double)n, eps, momentum, nullptr, running_mean,
                                                                running_var, mean, invstd, C);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
+extern "C" int bm_bn_stats_finalize_cumulative(const double* stats, long long n, float eps,
+                                               const long long* num_batches_tracked, float* running_mean,
+                                               float* running_var, float* mean, float* invstd, int C, bm_stream_t stream) {
+    BM_CHECK_ARG(stats && num_batches_tracked && running_mean && running_var && mean && invstd && C > 0 && n > 0);
+    bn_finalize_kernel<<<(C + 127) / 128, 128, 0, ST(stream)>>>(stats, (double)n, eps, 0.f, num_batches_tracked,
+                                                               running_mean, running_var, mean, invstd, C);
     BM_CHECK_LAUNCH();
     return 0;
 }
@@ -460,8 +470,18 @@ extern "C" int bm_bn_stats_finalize_counted(const double* stats, float eps, floa
                                             float* running_var, float* mean, float* invstd, int C, bm_stream_t stream) {
     BM_CHECK_ARG(stats && mean && invstd && C > 0);
     BM_CHECK_ARG((running_mean == nullptr) == (running_var == nullptr));
-    bn_finalize_kernel<true><<<(C + 127) / 128, 128, 0, ST(stream)>>>(stats, 0.0, eps, momentum, running_mean, running_var,
-                                                                     mean, invstd, C);
+    bn_finalize_kernel<true><<<(C + 127) / 128, 128, 0, ST(stream)>>>(stats, 0.0, eps, momentum, nullptr, running_mean,
+                                                                     running_var, mean, invstd, C);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
+extern "C" int bm_bn_stats_finalize_counted_cumulative(const double* stats, float eps, const long long* num_batches_tracked,
+                                                       float* running_mean, float* running_var, float* mean, float* invstd,
+                                                       int C, bm_stream_t stream) {
+    BM_CHECK_ARG(stats && num_batches_tracked && running_mean && running_var && mean && invstd && C > 0);
+    bn_finalize_kernel<true><<<(C + 127) / 128, 128, 0, ST(stream)>>>(stats, 0.0, eps, 0.f, num_batches_tracked,
+                                                                     running_mean, running_var, mean, invstd, C);
     BM_CHECK_LAUNCH();
     return 0;
 }

@@ -87,13 +87,16 @@ __global__ void softmax_bwd_kernel(const float* __restrict__ w, const float* __r
 // stats[0:C] = sum y, stats[C:2C] = sum y^2 (fp64) over n = B*T rows  ->  mean, invstd (biased var),
 // running stats update with the unbiased variance (momentum), as nn.BatchNorm1d in training mode.
 // COUNTED: n is read from stats[2C] on the device (a SyncBatchNorm group's row count, all-reduced with the sums).
+// batches (nullable): the layer's num_batches_tracked, already incremented for this batch; momentum is then torch's
+// cumulative-average factor 1 / num_batches_tracked (momentum=None), computed here so that the host never reads the count.
 template <bool COUNTED = false>
 __global__ void bn_finalize_kernel(const double* __restrict__ stats, double n, float eps, float momentum,
-                                   float* running_mean, float* running_var, float* __restrict__ mean,
-                                   float* __restrict__ invstd, int C) {
+                                   const long long* __restrict__ batches, float* running_mean, float* running_var,
+                                   float* __restrict__ mean, float* __restrict__ invstd, int C) {
     int c = blockIdx.x * blockDim.x + threadIdx.x;
     if (c >= C) return;
     if (COUNTED) n = stats[2 * C];
+    if (batches) momentum = (float)(1.0 / (double)*batches);
     double m = stats[c] / n;
     double var = stats[C + c] / n - m * m;
     if (var < 0) var = 0;

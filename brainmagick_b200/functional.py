@@ -37,7 +37,10 @@ class SequencePlan:
     the residual add (common.py:123-130).  A layer with any of them takes `layer_width(plan, k)` = 8 parameters.
 
     `bn_groups[k]`: the process group layer k's BatchNorm takes its statistics over (an nn.SyncBatchNorm, see
-    `bn_sync_groups`), None where the layer uses its own rows (None: no layer syncs)."""
+    `bn_sync_groups`), None where the layer uses its own rows (None: no layer syncs).
+
+    `training`, `bn_eps`, `bn_momentum` hold for every BatchNorm layer unless `bn_layers` is set: then `bn_layers[k]` is
+    layer k's own mode and settings (None where the layer has no BatchNorm); see `bn_plan_fields` and `bn_layer`."""
     dilations: tp.List[int]
     glu_after: tp.List[bool]
     has_act: tp.List[bool]            # layer k ends with (BatchNorm +) activation (activation_on_last, common.py:112)
@@ -55,6 +58,51 @@ class SequencePlan:
     rewrite_slope: float = dataclasses.field(default=0.0, kw_only=True)
     scale_boost: float = dataclasses.field(default=5.0, kw_only=True)
     bn_groups: tp.Optional[tp.List[tp.Any]] = dataclasses.field(default=None, kw_only=True)
+    bn_layers: tp.Optional[tp.List[tp.Optional["BnLayer"]]] = dataclasses.field(default=None, kw_only=True)
+
+
+class BnLayer(tp.NamedTuple):
+    """One BatchNorm layer's mode and settings, as torch.nn.BatchNorm1d reads them from its own module."""
+    training: bool                    # batch statistics; running buffers and num_batches_tracked updated
+    eps: float
+    momentum: tp.Optional[float]      # None: cumulative average, factor 1 / num_batches_tracked computed on the device
+    num_batches_tracked: tp.Optional[torch.Tensor]   # the counter a cumulative-average layer's finalize reads
+
+
+def bn_plan_fields(bns, training: bool) -> dict:
+    """The SequencePlan fields `training`, `bn_eps`, `bn_momentum`, `bn_buffers` and `bn_layers` from layer k's BatchNorm
+    module bns[k] (None: the layer has none) in a module whose own mode is `training`.  Each layer follows its own module,
+    as torch does: batch statistics exactly when bn.training, and its own eps and momentum.  `bn_layers` stays None when
+    every layer has the module's mode and the first layer's eps and a numeric momentum: such a plan is the uniform one."""
+    present = [bn for bn in bns if bn is not None]
+    for bn in present:
+        if not bn.track_running_stats or bn.running_mean is None or bn.running_var is None:
+            raise NotImplementedError("BatchNorm without running statistics (track_running_stats=False)")
+    eps, momentum = (present[0].eps, present[0].momentum) if present else (0.0, 0.0)
+    layers = [None if bn is None else
+              BnLayer(bool(bn.training), float(bn.eps), None if bn.momentum is None else float(bn.momentum),
+                      bn.num_batches_tracked if bn.momentum is None and bn.training else None) for bn in bns]
+    uniform = momentum is not None and all(
+        layer is None or (layer.training == training and layer.eps == eps and layer.momentum == momentum)
+        for layer in layers)
+    return dict(training=training, bn_eps=eps, bn_momentum=0.0 if momentum is None else momentum,
+                bn_buffers=[None if bn is None else (bn.running_mean, bn.running_var) for bn in bns],
+                bn_layers=None if uniform else layers)
+
+
+def bn_layer(plan: SequencePlan, k: int) -> BnLayer:
+    """Layer k's BatchNorm mode and settings (the layer has a BatchNorm)."""
+    if plan.bn_layers is not None:
+        return plan.bn_layers[k]
+    return BnLayer(plan.training, plan.bn_eps, plan.bn_momentum, None)
+
+
+def bn_count_batches(bns) -> None:
+    """nn.BatchNorm1d's bookkeeping on the device: num_batches_tracked += 1 on every layer in training mode.  Called before
+    the layers run, as torch does, so that a cumulative-average finalize reads the incremented count on the same stream."""
+    for bn in bns:
+        if bn is not None and bn.training:
+            bn.num_batches_tracked.add_(1)
 
 
 def bn_sync_groups(bns, residual=None):
@@ -76,6 +124,23 @@ def bn_sync_groups(bns, residual=None):
             raise NotImplementedError("SyncBatchNorm on a ConvSequence layer with a LayerScale (scale) or post_skip gain")
         groups.append(group)
     return groups if any(g is not None for g in groups) else None
+
+
+def _bn_finalize(stats, rows, group, layer: BnLayer, rm, rv, mean, invstd, C, st):
+    """Batch statistics -> mean, invstd and the running-buffer update of one training-mode BatchNorm layer: the `_counted`
+    forms for a syncing layer (its row count is in stats[2C]), the `_cumulative` forms for momentum=None."""
+    if group is not None and layer.momentum is None:
+        call("bm_bn_stats_finalize_counted_cumulative", ptr(stats), float(layer.eps), ptr(layer.num_batches_tracked),
+             ptr(rm), ptr(rv), ptr(mean), ptr(invstd), C, st)
+    elif group is not None:
+        call("bm_bn_stats_finalize_counted", ptr(stats), float(layer.eps), float(layer.momentum), ptr(rm), ptr(rv),
+             ptr(mean), ptr(invstd), C, st)
+    elif layer.momentum is None:
+        call("bm_bn_stats_finalize_cumulative", ptr(stats), rows, float(layer.eps), ptr(layer.num_batches_tracked),
+             ptr(rm), ptr(rv), ptr(mean), ptr(invstd), C, st)
+    else:
+        call("bm_bn_stats_finalize", ptr(stats), rows, float(layer.eps), float(layer.momentum), ptr(rm), ptr(rv),
+             ptr(mean), ptr(invstd), C, st)
 
 
 def _sync_bn_sums(buf, C, rows, group):
@@ -485,8 +550,9 @@ def _residual_branch_backward(plan: SequencePlan, k, p, rec, g, nd: "_Needs", B,
         act, slope = rec["act"], (plan.act_slope if plan.has_act[k] else 0.0)
         want_dsrc = need_dy
     dsrc = dgamma = dbeta = dls = dps = None
+    batch_stats = mean is not None and bn_layer(plan, k).training
     if rec["gain"] and (want_dsrc or n_ls or n_ps):
-        bn_reduce = mean is not None and (plan.training or n_gamma or n_beta)
+        bn_reduce = mean is not None and (batch_stats or n_gamma or n_beta)
         if bn_reduce:
             dgamma, dbeta = _empty((cout,), like), _empty((cout,), like)
         dls = _empty((cout,), like) if n_ls else None
@@ -494,7 +560,7 @@ def _residual_branch_backward(plan: SequencePlan, k, p, rec, g, nd: "_Needs", B,
         dsrc = _empty((B, T, cout), like)
         reduce = bool(bn_reduce or n_ls or n_ps)
         _reducing_call("bm_bn_act_gain_skip_bwd", like, (rows, cout), ptr(g), ptr(src), ptr(mean), ptr(invstd), ptr(gm),
-                       ptr(bt), 1 if plan.training else 0, rows, cout, act, float(slope), ptr(ls), float(plan.scale_boost),
+                       ptr(bt), 1 if batch_stats else 0, rows, cout, act, float(slope), ptr(ls), float(plan.scale_boost),
                        ptr(ps), ptr(sums3 if reduce else None), ptr(dsrc), ptr(dgamma), ptr(dbeta), ptr(dls), ptr(dps), st,
                        reduces=reduce)
     elif not rec["gain"] and want_dsrc:                     # a rewrite without gain: the LeakyReLU backward alone
@@ -535,19 +601,17 @@ def conv_stack_forward(plan: SequencePlan, x, conv0: _Conv, conv_p, glu_p, nd: "
             mean, invstd = _empty((cout,), x), _empty((cout,), x)
             rm, rv = plan.bn_buffers[k]
             group = plan.bn_groups[k] if plan.bn_groups else None
-            if plan.training and group is not None:
-                # SyncBatchNorm: one all-reduce per layer, issued whatever the data, so every rank issues the same ones
+            layer = bn_layer(plan, k)
+            if layer.training:
                 conv.forward(x, b.contiguous(), B, T, plan.dilations[k], y, stats, status)
-                _sync_bn_sums(stats, cout, rows, group)
-                call("bm_bn_stats_finalize_counted", ptr(stats), float(plan.bn_eps), float(plan.bn_momentum), ptr(rm),
-                     ptr(rv), ptr(mean), ptr(invstd), cout, st)
-            elif plan.training:
-                conv.forward(x, b.contiguous(), B, T, plan.dilations[k], y, stats, status)
-                call("bm_bn_stats_finalize", ptr(stats), rows, float(plan.bn_eps), float(plan.bn_momentum),
-                     ptr(rm), ptr(rv), ptr(mean), ptr(invstd), cout, st)
+                if group is not None:
+                    # SyncBatchNorm: one all-reduce per layer, issued whatever the data, so every rank issues the same ones
+                    _sync_bn_sums(stats, cout, rows, group)
+                _bn_finalize(stats, rows, group, layer, rm, rv, mean, invstd, cout, st)
             else:
+                # eval mode (the module's, or this layer's alone): the running statistics, no statistics epilogue
                 conv.forward(x, b.contiguous(), B, T, plan.dilations[k], y, None, status)
-                call("bm_bn_eval_stats", ptr(rm), ptr(rv), float(plan.bn_eps), ptr(mean), ptr(invstd), cout, st)
+                call("bm_bn_eval_stats", ptr(rm), ptr(rv), float(layer.eps), ptr(mean), ptr(invstd), cout, st)
         else:
             conv.forward(x, b.contiguous(), B, T, plan.dilations[k], y, None, status)
         skip = plan.skip and conv.cin_true == cout
@@ -635,6 +699,7 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
                 layer_grads[k] = (None, None, None, None) + opt_grads
                 continue
         group = plan.bn_groups[k] if plan.bn_groups else None
+        batch_stats = rec["has_bn"] and bn_layer(plan, k).training
         if dy is not None:
             pass                                    # the gain kernel ran the BatchNorm / activation backward
         elif rec["has_bn"] and group is not None:
@@ -655,12 +720,12 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
         elif rec["has_bn"]:
             # the batch statistics' backward reduces in training mode; in eval mode only for trainable gamma / beta (else
             # the BatchNorm + activation backward is one elementwise pass)
-            reduce = plan.training or n_gamma or n_beta
+            reduce = batch_stats or n_gamma or n_beta
             dy = _empty((B, T, cout), like)
             dgamma, dbeta = (_empty((cout,), like), _empty((cout,), like)) if reduce else (None, None)
             name, args = _epilogue("bwd", True, rec["act"], plan.act_slope,
                                    (ptr(g_act), ptr(rec["y"]), ptr(rec["mean"]), ptr(rec["invstd"]), ptr(gamma.contiguous()),
-                                    ptr(beta.contiguous()), 1 if plan.training else 0, rows, cout),
+                                    ptr(beta.contiguous()), 1 if batch_stats else 0, rows, cout),
                                    (ptr(sums if reduce else None), ptr(dy), ptr(dgamma), ptr(dbeta)))
             _reducing_call(name, like, (rows, cout), *args, st, reduces=reduce)
         elif rec["act"] != ACT_NONE:
@@ -673,7 +738,7 @@ def conv_stack_backward(plan: SequencePlan, conv_p, layers, g, nd: "_Needs", B, 
             dy = g.clone() if (rec["skip"] and nd.below[k]) else g
         # with a training-mode BatchNorm behind the conv, sum(dy) is exactly 0: no bias reduction (a SyncBatchNorm's is 0
         # summed over the group only)
-        dcw, dcb = weight_grad(conv, dy, rec["x_in"], plan.dilations[k], rec["has_bn"] and plan.training and group is None,
+        dcw, dcb = weight_grad(conv, dy, rec["x_in"], plan.dilations[k], batch_stats and group is None,
                                want=(n_cw, n_cb))
         if not nd.below[k]:
             pass

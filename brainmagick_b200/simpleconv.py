@@ -208,21 +208,20 @@ class SimpleConv(nn.Module):
                 out += [glu[0].weight, glu[0].bias]
         return out
 
+    @staticmethod
+    def _bns(seq: ConvSequence) -> list:
+        """layer k's BatchNorm module, None on the bare last layer"""
+        return [blk[1] if seq.has_act[k] else None for k, blk in enumerate(seq.sequence)]
+
     def _sequence_fields(self, seq: ConvSequence) -> dict:
         """The `functional.SequencePlan` fields of one encoder"""
-        bn_buffers = [(blk[1].running_mean, blk[1].running_var) if seq.has_act[k] else None
-                      for k, blk in enumerate(seq.sequence)]
-        bn0 = seq.sequence[0][1]
-        if bn0.momentum is None:
-            raise NotImplementedError("BatchNorm cumulative-average mode (momentum=None)")
         residual = seq.residual()
-        bn_groups = BF.bn_sync_groups([blk[1] if seq.has_act[k] else None for k, blk in enumerate(seq.sequence)], residual)
+        bns = self._bns(seq)
         return dict(
-            dilations=list(seq.dilations), glu_after=seq.glu_after(), training=self.training, bn_eps=bn0.eps,
-            bn_momentum=bn0.momentum, bn_buffers=bn_buffers, keep_for_backward=torch.is_grad_enabled(),
-            use_tensor_cores=self.use_tensor_cores, skip=seq.skip, act_code=seq.act_code, act_slope=seq.act_slope,
-            has_act=list(seq.has_act), batch_norm=True, residual=residual, rewrite_slope=seq.rewrite_slope,
-            scale_boost=seq.scale_boost(), bn_groups=bn_groups)
+            dilations=list(seq.dilations), glu_after=seq.glu_after(), **BF.bn_plan_fields(bns, self.training),
+            keep_for_backward=torch.is_grad_enabled(), use_tensor_cores=self.use_tensor_cores, skip=seq.skip,
+            act_code=seq.act_code, act_slope=seq.act_slope, has_act=list(seq.has_act), batch_norm=True, residual=residual,
+            rewrite_slope=seq.rewrite_slope, scale_boost=seq.scale_boost(), bn_groups=BF.bn_sync_groups(bns, residual))
 
     def _plan(self, meg: torch.Tensor, batch) -> BF.EncoderPlan:
         seq: ConvSequence = self.encoders[self._encoder0()]
@@ -271,6 +270,8 @@ class SimpleConv(nn.Module):
                                  f"{self._stream_channels[name]}")
             streams.append(x)
         plan = self._plan(meg, batch)
+        for seq in self.encoders.values():      # nn.BatchNorm1d bookkeeping, ahead of the finalize kernels that read it
+            BF.bn_count_batches(self._bns(seq))
         if self.subsampled_meg_channels is not None:         # simpleconv.py:200-203, applied inside the encoder node
             if self._channel_mask is None or self._channel_mask.device != meg.device:
                 mask = torch.zeros(self.n_input_channels)
@@ -294,9 +295,4 @@ class SimpleConv(nn.Module):
         est = BF.encoder_forward(plan, meg, heads, il_w, il_b, subj_w, *head,
                                  self._layer_params(self.encoders[self._encoder0()]), sub_emb=sub_emb, streams=streams,
                                  encoder_params=[self._layer_params(self.encoders[name]) for name, _ in plan.encoders])
-        if self.training:
-            for seq in self.encoders.values():   # nn.BatchNorm1d bookkeeping (running stats were updated on device)
-                for k, blk in enumerate(seq.sequence):
-                    if seq.has_act[k]:
-                        blk[1].num_batches_tracked += 1
         return est[:, :, :length]

@@ -116,6 +116,16 @@ int bm_bn_stats_finalize(const double* stats, long long n, float eps, float mome
  * and row count are all-reduced over the group in one buffer without a host read of the count. */
 int bm_bn_stats_finalize_counted(const double* stats, float eps, float momentum, float* running_mean, float* running_var,
                                  float* mean, float* invstd, int C, bm_stream_t stream);
+/* Cumulative-average forms of the two above (nn.BatchNorm1d with momentum=None): the running statistics are updated with
+ * factor 1 / num_batches_tracked, read on the device from the layer's int64 counter, which the caller has already
+ * incremented for this batch on the same stream (torch's order: increment, then factor).  The host never reads the count.
+ * running_mean / running_var are required. */
+int bm_bn_stats_finalize_cumulative(const double* stats, long long n, float eps, const long long* num_batches_tracked,
+                                    float* running_mean, float* running_var, float* mean, float* invstd, int C,
+                                    bm_stream_t stream);
+int bm_bn_stats_finalize_counted_cumulative(const double* stats, float eps, const long long* num_batches_tracked,
+                                            float* running_mean, float* running_var, float* mean, float* invstd, int C,
+                                            bm_stream_t stream);
 int bm_bn_eval_stats(const float* running_mean, const float* running_var, float eps, float* mean, float* invstd,
                      int C, bm_stream_t stream);
 /* x_new = GELU(gamma*(y-mean)*invstd + beta) (+ x_old if not NULL); rows = B*T.
