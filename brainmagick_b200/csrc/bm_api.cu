@@ -369,6 +369,8 @@ static int sensor_chain_bwd(const float* dx0, const float* meg, const float* il_
     BM_CHECK_ARG(dx0 && ld_x0 >= D);
     BM_CHECK_ARG((dv || !(du || d_il_w || d_il_b)) && (du || !d_weights));
     BM_CHECK_ARG(!d_weights || (meg && rec_order && rec_off));
+    // a short workspace is refused before any stage is enqueued, not after the subject-layer backward has written dv
+    if (det && (d_il_w || d_il_b)) BM_CHECK_WS(bm_initial_linear_bwd_det_workspace(B, T, O, IL));
     // the subject and sensor-mix gradients reduce each segment inside one CTA: already fixed-order
     int rc = 0;
     if (dv || d_subj_w)
