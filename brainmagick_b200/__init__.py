@@ -15,9 +15,9 @@ if "CUDA_DEVICE_MAX_CONNECTIONS" not in _os.environ and not _torch.cuda.is_initi
 
 from .simpleconv import SimpleConv  # noqa: F401,E402
 from .losses import ClipLoss  # noqa: F401,E402
-from .common import ChannelMerger, ConvSequence, FourierEmb, PositionGetter, SubjectLayers  # noqa: F401
+from .common import ChannelMerger, ConvSequence, FourierEmb, PositionGetter, StaticBatch, SubjectLayers  # noqa: F401
 from .features import DeepMel  # noqa: F401
 from .norm import BatchScaler, ScaleReject  # noqa: F401
 
 __all__ = ["SimpleConv", "ClipLoss", "ChannelMerger", "ConvSequence", "FourierEmb", "PositionGetter",
-           "SubjectLayers", "DeepMel", "BatchScaler", "ScaleReject"]
+           "StaticBatch", "SubjectLayers", "DeepMel", "BatchScaler", "ScaleReject"]

@@ -67,6 +67,7 @@ SIGNATURES = {
     "bm_transpose_nt_ld": [P, I, I, I, I, P, P],
     "bm_channel_join": [I, I, I, I] + [P, I, I, I, I] * 4 + [P, P],
     "bm_channel_split": [P, I, I, I, I] + [P, I, I, I, I] * 4 + [P],
+    "bm_check_all_true": [P, L, I, P, P],
     "bm_tc_wgrad_supported": [I, I],
     "bm_tc_wgrad": [P, P, I, I, I, I, I, I, I, P, P, P, P, P],
     "bm_tc_wgrad_conv_supported": [I, I, I, I],

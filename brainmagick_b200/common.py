@@ -78,6 +78,14 @@ class PositionGetter:
     # ---- fused-path helper: one row per recording present in the batch -------------------------------
     def batch_layout(self, batch, n_channels: int, device):
         """-> rec_positions [R,C,2] (device), rec_of_sample [B] int32, rec_order [B] int32, rec_off [R+1] int32."""
+        table, rows, order, off = self.batch_layout_host(batch, n_channels)
+        to = dict(device=device, non_blocking=True)
+        return (table.to(**to), torch.from_numpy(rows).to(**to), torch.from_numpy(order).to(**to),
+                torch.from_numpy(off).to(**to))
+
+    def batch_layout_host(self, batch, n_channels: int):
+        """`batch_layout` on the host: (rec_positions [R,C,2] fp32 tensor, rec_of_sample [B], rec_order [B] and
+        rec_off [R+1] int32 numpy arrays); rows are the recordings in ascending recording_index."""
         rec_ids = [r.recording_index for r in batch._recordings]
         uniq = sorted(set(rec_ids))
         row_of = {rid: i for i, rid in enumerate(uniq)}
@@ -92,9 +100,99 @@ class PositionGetter:
         order = np.argsort(rows, kind="stable").astype(np.int32)
         off = np.zeros(len(uniq) + 1, dtype=np.int32)
         np.cumsum(np.bincount(rows, minlength=len(uniq)), out=off[1:])
-        to = dict(device=device, non_blocking=True)
-        return (table.to(**to), torch.from_numpy(rows).to(**to), torch.from_numpy(order).to(**to),
-                torch.from_numpy(off).to(**to))
+        return table, rows, order, off
+
+
+class StaticBatch:
+    """A batch of fixed shape whose sensor layout lives in device buffers, for training / evaluation steps captured in a CUDA
+    graph (torch.cuda.graph): the graph reads these buffers, and the caller refills them with `fill_` before each replay.
+    `SimpleConv.forward` and `ChannelMerger.forward` take it in place of a reference batch, in eager mode too.
+
+    Buffers (on `device`, fixed addresses): subject_index [B] int32, rec_positions [R_max, C, 2] fp32 (one row per recording
+    slot), rec_of_sample [B] and rec_order [B] int32, rec_off [R_max + 1] int32 (CSR offsets of the samples of each slot).
+    A batch with R < R_max recordings fills slots 0..R-1 exactly as `PositionGetter.batch_layout` lays out a reference batch;
+    slots R..R_max-1 repeat slot 0's positions and own empty segments (rec_off[r] = B).  Their attention weights are
+    therefore finite (an all-INVALID row would be a softmax over -inf only: NaN, and NaN * 0 poisons the heads' gradient)
+    and their weight gradients are exact zeros."""
+
+    def __init__(self, batch_size: int, n_channels: int, max_recordings: int, device):
+        if min(batch_size, n_channels, max_recordings) < 1:
+            raise ValueError(f"StaticBatch needs batch_size, n_channels and max_recordings >= 1, got "
+                             f"{batch_size}, {n_channels}, {max_recordings}")
+        self.batch_size, self.n_channels, self.max_recordings = int(batch_size), int(n_channels), int(max_recordings)
+        self.device = torch.device(device)
+        if self.device.type == "cuda" and self.device.index is None:
+            self.device = torch.device("cuda", torch.cuda.current_device())
+        B, C, R = self.batch_size, self.n_channels, self.max_recordings
+        sizes = dict(rec_positions=R * C * 2, subject_index=B, rec_of_sample=B, rec_order=B, rec_off=R + 1)
+        cuda = self.device.type == "cuda"
+        # every field is 4 bytes wide: one int32 staging buffer (pinned) and one device buffer, sent with one copy
+        total = sum(sizes.values())
+        self._stage = torch.zeros(total, dtype=torch.int32, pin_memory=cuda)
+        self._buffer = torch.zeros(total, dtype=torch.int32, device=self.device)
+        self._staged, at = {}, 0
+        for name, n in sizes.items():
+            host, dev = self._stage[at:at + n], self._buffer[at:at + n]
+            if name == "rec_positions":
+                host, dev = host.view(torch.float32).view(R, C, 2), dev.view(torch.float32).view(R, C, 2)
+            self._staged[name] = host
+            setattr(self, name, dev)
+            at += n
+        self._copied = torch.cuda.Event() if cuda else None   # recorded after the last copy out of the staging buffer
+        self._copy_pending = False
+        self._position_getter = PositionGetter()
+
+    def layout(self):
+        """(rec_positions, rec_of_sample, rec_order, rec_off): the device buffers, as `PositionGetter.batch_layout` returns."""
+        return self.rec_positions, self.rec_of_sample, self.rec_order, self.rec_off
+
+    def check(self, meg: torch.Tensor) -> None:
+        """Raises ValueError unless meg [B, C, T] has this batch's B and C and lives on its device."""
+        if meg.shape[0] != self.batch_size or meg.shape[1] != self.n_channels or meg.device != self.device:
+            raise ValueError(f"input of shape {tuple(meg.shape)} on {meg.device} for a StaticBatch of batch_size "
+                             f"{self.batch_size}, n_channels {self.n_channels} on {self.device}")
+
+    def fill_(self, batch) -> "StaticBatch":
+        """Refill the buffers from a reference-style batch (`subject_index`, `_recordings`, `meg`): the layout is computed on
+        the host by `PositionGetter.batch_layout_host`, then everything goes to the device in one non-blocking copy from the
+        pinned staging buffer, on the current stream (a CUDA subject_index is copied device to device on the same stream).
+        Waits first for the previous copy out of the staging buffer.  Not allowed while a CUDA graph is being captured.
+
+        In eager use the autograd graph of a step keeps references to these buffers until its backward has run: call
+        `fill_` for the next batch only after the backward of the step that read the previous contents (not ahead of it
+        to prefetch, nor between the forwards of accumulated steps), or that backward reads the new layout."""
+        from . import functional as BF
+        if BF.capturing():
+            raise RuntimeError("StaticBatch.fill_ copies from host memory: call it before a replay, not inside the capture")
+        B, C, R_max = self.batch_size, self.n_channels, self.max_recordings
+        subject = batch.subject_index.reshape(-1)
+        meg = getattr(batch, "meg", None)
+        if len(batch._recordings) != B or subject.numel() != B or (meg is not None and meg.shape[0] != B):
+            raise ValueError(f"a batch of {len(batch._recordings)} samples for a StaticBatch of batch_size {B}")
+        if meg is not None and meg.shape[1] != C:
+            raise ValueError(f"a batch of {meg.shape[1]} channels for a StaticBatch of n_channels {C}")
+        table, rows, order, off = self._position_getter.batch_layout_host(batch, C)
+        R = table.shape[0]
+        if R > R_max:
+            raise ValueError(f"a batch of {R} distinct recordings for a StaticBatch of max_recordings {R_max}")
+        if self._copy_pending:
+            self._copied.synchronize()          # the previous copy may still be reading the staging buffer
+        st = self._staged
+        st["rec_positions"][:R] = table
+        st["rec_positions"][R:] = table[0]
+        st["rec_of_sample"].numpy()[:] = rows
+        st["rec_order"].numpy()[:] = order
+        st["rec_off"].numpy()[:R + 1] = off
+        st["rec_off"][R + 1:] = B
+        if not subject.is_cuda:
+            st["subject_index"].copy_(subject)
+        self._buffer.copy_(self._stage, non_blocking=True)
+        if subject.is_cuda:
+            self.subject_index.copy_(subject)
+        if self._copied is not None:
+            self._copied.record(torch.cuda.current_stream(self.device))    # the stream the copies above ran on
+            self._copy_pending = True
+        return self
 
 
 class FourierEmb(nn.Module):
@@ -145,6 +243,7 @@ class ChannelMerger(nn.Module):
         self.usage_penalty = usage_penalty
         self._penalty = torch.tensor(0.)
         self.ban_centre_override: tp.Optional[torch.Tensor] = None   # test hook: inject the per-forward centre
+        self._freq: tp.Optional[torch.Tensor] = None                 # `frequencies(device)`'s copy
 
     @property
     def training_penalty(self):
@@ -159,15 +258,32 @@ class ChannelMerger(nn.Module):
             return self.ban_centre_override.to(device=device, dtype=torch.float32).contiguous()
         return torch.rand(2, device=device)
 
+    def frequencies(self, device) -> torch.Tensor:
+        """The embedding's frequency table (`FourierEmb.frequencies`) on `device`, copied there once: a step captured in a
+        CUDA graph copies nothing from the host."""
+        if self._freq is None or self._freq.device != torch.device(device):
+            self._freq = self.embedding.frequencies().to(device)
+        return self._freq
+
+    def batch_layout(self, batch, meg: torch.Tensor):
+        """(rec_positions, rec_of_sample, rec_order, rec_off) of `batch` for the input meg [B, C, T]: a StaticBatch's device
+        buffers as they are, else the reference batch's layout built on the host and copied to meg's device."""
+        from . import functional as BF
+        if isinstance(batch, StaticBatch):
+            batch.check(meg)
+            return batch.layout()
+        if BF.capturing():
+            raise RuntimeError("a reference batch's sensor layout is built on the host and copied to the device on every "
+                               "forward, which a CUDA graph capture cannot hold: pass a brainmagick_b200.StaticBatch")
+        return self.position_getter.batch_layout(batch, meg.shape[1], meg.device)
+
     def forward(self, meg, batch):
         """Stand-alone call (bm/models/common.py:334-362): [B, C, T] -> [B, chout, T].  Inside SimpleConv the merger is
         fused into the encoder; this runs the same stage kernels for callers that use the module on its own."""
         from . import functional as BF
         _require_cuda_fp32(meg, "ChannelMerger")
-        B, C, T = meg.shape
-        pos, rec_of_sample, rec_order, rec_off = self.position_getter.batch_layout(batch, C, meg.device)
-        freq = self.embedding.frequencies().to(meg.device)
-        return BF.channel_merger_forward(meg, self.heads, pos, rec_of_sample, rec_order, rec_off, freq,
+        pos, rec_of_sample, rec_order, rec_off = self.batch_layout(batch, meg)
+        return BF.channel_merger_forward(meg, self.heads, pos, rec_of_sample, rec_order, rec_off, self.frequencies(meg.device),
                                          self.draw_ban_centre(meg.device), float(self.dropout))
 
 

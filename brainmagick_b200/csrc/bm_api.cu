@@ -1583,6 +1583,15 @@ extern "C" int bm_channel_split(const float* src, int B, int T, int Cp, int n, f
     return channel_join_launch(true, const_cast<float*>(src), B, T, Cp, n, dst, ST(stream));
 }
 
+extern "C" int bm_check_all_true(const unsigned char* mask, long long n, int code, int* status, bm_stream_t stream) {
+    BM_CHECK_ARG(status && n >= 0 && (mask || n == 0) && code != 0);
+    if (n == 0) return 0;
+    const bool vec = aligned16(mask);
+    check_all_true_kernel<<<ew_grid(vec ? (n + 15) / 16 : n), 256, 0, ST(stream)>>>(mask, n, vec, code, status);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
 // weight gradient of a (dilated) conv / pointwise layer on the tensor cores: dW[m][n][tap] = sum_{b,t} dY[b,t,m] X[b,t+s,n]
 extern "C" int bm_tc_wgrad_supported(int M, int N) { return tc::wgrad_tc_supported(M, N) ? 1 : 0; }
 extern "C" long long bm_tc_wgrad_workspace(int B, int M, int N, int Kw) {

@@ -531,4 +531,29 @@ inline int ew_grid(long long total, int block = 256, int per_thread = 1) {
     return (int)g;
 }
 
+// ------------------------------------------------------------------------------------------------
+// ClipLoss's `assert mask.all()` (bm/losses.py:110) without a host read: status <- code (if still 0) when any of the n
+// bytes of `mask` is 0.  `vec`: mask is 16-byte aligned, read as uint4 (the last n % 16 bytes one by one).
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool has_zero_byte(unsigned w) { return ((w - 0x01010101u) & ~w & 0x80808080u) != 0u; }
+
+__global__ void check_all_true_kernel(const unsigned char* __restrict__ mask, long long n, bool vec, int code,
+                                      int* __restrict__ status) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    bool bad = false;
+    long long tail = 0;
+    if (vec) {
+        const long long nv = n >> 4;
+        const uint4* m4 = reinterpret_cast<const uint4*>(mask);
+        for (long long i = tid; i < nv; i += stride) {
+            const uint4 w = __ldg(m4 + i);
+            bad |= has_zero_byte(w.x) | has_zero_byte(w.y) | has_zero_byte(w.z) | has_zero_byte(w.w);
+        }
+        tail = nv << 4;
+    }
+    for (long long i = tail + tid; i < n; i += stride) bad |= mask[i] == 0;
+    if (__syncthreads_or(bad) && threadIdx.x == 0) atomicCAS(status, 0, code);
+}
+
 }  // namespace bm

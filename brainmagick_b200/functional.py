@@ -123,6 +123,9 @@ def bn_sync_groups(bns, residual=None):
         if group is not None and residual is not None and (residual[k][1] or residual[k][2]):
             raise NotImplementedError("SyncBatchNorm on a ConvSequence layer with a LayerScale (scale) or post_skip gain")
         groups.append(group)
+    if any(g is not None for g in groups) and capturing():
+        raise RuntimeError("a SyncBatchNorm layer with more than one rank all-reduces its statistics, which a CUDA graph "
+                           "capture of the step cannot hold; capture on one rank or use nn.BatchNorm1d")
     return groups if any(g is not None for g in groups) else None
 
 
@@ -197,8 +200,12 @@ def tc_status_tensor(device) -> torch.Tensor:
     return _status[device]
 
 
+MASK_NOT_ALL_TRUE = 903   # status code of bm_check_all_true: a ClipLoss mask with a False entry (900-902: the kernels' own)
+
+
 def check_tc_status(device=None) -> None:
-    """Synchronising check (tests, bench, end of epoch): raises if a tensor-core kernel reported a timeout."""
+    """Synchronising check (tests, bench, end of epoch): raises if a kernel reported a bad subject index, a ClipLoss mask that
+    is not all true (checked on the device in a captured step), or a tensor-core pipeline timeout."""
     for dev, t in _status.items():
         if device is None or torch.device(device) == dev:
             code = int(t.item())
@@ -206,8 +213,27 @@ def check_tc_status(device=None) -> None:
                 t.zero_()
                 raise IndexError(f"a subject / recording index is outside the weight sets of the per-sample 1x1 layer on {dev} "
                                  "(bm/models/common.py:57 raises there too)")
+            if code == MASK_NOT_ALL_TRUE:
+                t.zero_()
+                raise AssertionError(f"mask is not supported for now (a ClipLoss mask with a False entry on {dev})")
             if code != 0:
                 raise _lib.BmB200Error(f"a tensor-core kernel reported a pipeline timeout (barrier code {code}) on {dev}")
+
+
+def capturing() -> bool:
+    """True while the current CUDA stream is being captured into a CUDA graph (torch.cuda.graph): then no step may read
+    device memory on the host, copy from host memory or run a collective.  The one place the host code asks."""
+    return torch.cuda.is_initialized() and torch.cuda.is_current_stream_capturing()
+
+
+def check_all_true(mask: torch.Tensor, code: int = MASK_NOT_ALL_TRUE) -> None:
+    """Enqueue `assert mask.all()` on the device (bm_check_all_true): a False entry sets the status word to `code`, which
+    the next check_tc_status() raises."""
+    m = mask.detach()
+    if m.dtype not in (torch.bool, torch.uint8):
+        m = m != 0
+    m = m.contiguous()
+    call("bm_check_all_true", ptr(m), m.numel(), int(code), ptr(tc_status_tensor(m.device)), stream())
 
 
 OVERLAP_WGRAD = True   # weight-gradient kernels on a side stream, concurrent with the data-gradient kernels of the layer

@@ -101,7 +101,14 @@ class ClipLoss(torch.nn.Module):
     def _check_mask(self, mask) -> None:
         """losses.py:110 `assert mask.all()`: on a CUDA mask that is a device->host sync per call.  The verdict is kept per
         mask tensor OBJECT (weak reference + version counter), so a caller that reuses one all-true mask pays it once; a fresh
-        mask per batch (what bm/solver.py passes) is checked every time, exactly like the reference."""
+        mask per batch (what bm/solver.py passes) is checked every time, exactly like the reference.
+
+        While the step is captured in a CUDA graph the host cannot read the mask, and a replay changes its content without
+        running any Python: the check is then enqueued on the device on every call (`functional.check_all_true`), and a
+        False entry raises at the next `functional.check_tc_status()`."""
+        if BF.capturing():
+            BF.check_all_true(mask)
+            return
         seen = self._mask_ok
         if seen is not None and seen[0]() is mask and seen[1] == mask._version:
             return
@@ -109,6 +116,9 @@ class ClipLoss(torch.nn.Module):
         self._mask_ok = (weakref.ref(mask), mask._version)
 
     def forward(self, estimate, candidate, mask=None):
+        if self.global_negatives and BF.capturing() and distrib.world_size() > 1:
+            raise RuntimeError("ClipLoss(global_negatives=True) all-gathers the candidates over the ranks, which a CUDA graph "
+                               "capture of the step cannot hold; capture on one rank or without global_negatives")
         self._check_mask(mask)
         assert estimate.size(0) <= candidate.size(0), "need at least as many targets as estimates"
         pre, self._prefetched = self._prefetched, None

@@ -28,7 +28,7 @@ import torch
 from torch import nn
 
 from . import functional as BF
-from .common import ChannelMerger, ConvSequence, ScaledEmbedding, SubjectLayers, require_library
+from .common import ChannelMerger, ConvSequence, ScaledEmbedding, StaticBatch, SubjectLayers, require_library
 
 
 def _require_cuda(meg: torch.Tensor) -> None:
@@ -184,7 +184,7 @@ class SimpleConv(nn.Module):
         if not all(seq.clip_conv_family for seq in self.encoders.values()):
             raise NotImplementedError("SimpleConv's fused encoder needs batch_norm=True; "
                                       "see SURVEY.md 8(f) row 4")
-        self._freq: tp.Optional[torch.Tensor] = None
+        self._unused_layout: tp.Dict[tuple, tuple] = {}     # merger=False: placeholder layout tables per (device, B, C)
         self.use_tensor_cores = True     # False forces the FP32-FMA kernels everywhere (debugging / A-B timing)
 
     # ------------------------------------------------------------------------------------------------
@@ -228,13 +228,19 @@ class SimpleConv(nn.Module):
         device = meg.device
         B, C, _ = meg.shape
         if self.merger is None:                 # no spatial attention: the layout tables are never read
-            pos = torch.zeros(1, C, 2, device=device)
-            rec_of_sample = rec_order = torch.zeros(B, dtype=torch.int32, device=device)
-            rec_off = torch.tensor([0, B], dtype=torch.int32, device=device)
+            if isinstance(batch, StaticBatch):
+                batch.check(meg)
+            key = (device, B, C)
+            if key not in self._unused_layout:  # made once: a captured step copies nothing from the host
+                zeros = torch.zeros(B, dtype=torch.int32, device=device)
+                self._unused_layout[key] = (torch.zeros(1, C, 2, device=device), zeros, zeros,
+                                            torch.tensor([0, B], dtype=torch.int32, device=device))
+            pos, rec_of_sample, rec_order, rec_off = self._unused_layout[key]
         else:
-            pos, rec_of_sample, rec_order, rec_off = self.merger.position_getter.batch_layout(batch, C, device)
-            if self._freq is None or self._freq.device != device:
-                self._freq = self.merger.embedding.frequencies().to(device)
+            pos, rec_of_sample, rec_order, rec_off = self.merger.batch_layout(batch, meg)
+        if not isinstance(batch, StaticBatch) and not batch.subject_index.is_cuda and BF.capturing():
+            raise RuntimeError("the batch's subject_index is on the host, and a CUDA graph capture cannot copy it: pass a "
+                               "brainmagick_b200.StaticBatch or a batch whose subject_index is a CUDA tensor")
         fields = self._sequence_fields(seq)
         encoders = tuple((name, BF.SequencePlan(**self._sequence_fields(self.encoders[name])))
                          for name in self.encoders if name != self._encoder0())
@@ -242,7 +248,8 @@ class SimpleConv(nn.Module):
             **fields, kernel_size=seq.kernel, glu_kernel=seq.glu_kernel,
             rec_positions=pos, rec_of_sample=rec_of_sample, rec_order=rec_order, rec_off=rec_off,
             subject=batch.subject_index.to(device=device, dtype=torch.int32).contiguous(),
-            freq=self._freq, ban_centre=None if self.merger is None else self.merger.draw_ban_centre(device),
+            freq=None if self.merger is None else self.merger.frequencies(device),
+            ban_centre=None if self.merger is None else self.merger.draw_ban_centre(device),
             ban_radius=0.0 if self.merger is None else float(self.merger.dropout),
             has_sub_emb=self.subject_embedding is not None, streams=tuple(self._streams), encoders=encoders,
             concatenate=self._concatenate)
@@ -250,7 +257,9 @@ class SimpleConv(nn.Module):
     def forward(self, inputs, batch):
         """inputs: {"meg": [B, C, T], and every other stream of in_channels: [B, C_s, T]}, CUDA fp32 tensors (a stream may
         be a view, e.g. cropped in time); the sensor front (merger, initial_linear, subject layers / embedding) acts on
-        "meg", which is always required.  Gradients reach every parameter and each input tensor that requires grad."""
+        "meg", which is always required.  Gradients reach every parameter and each input tensor that requires grad.
+        batch: a reference-style batch (`subject_index`, `_recordings`), or a `StaticBatch` whose device buffers are used as
+        they are -- what a step captured in a CUDA graph needs (DESIGN.md, "CUDA graph capture")."""
         meg = inputs["meg"]
         _require_cuda(meg)
         if meg.dtype != torch.float32:

@@ -420,6 +420,10 @@ int bm_channel_join(int B, int T, int Cp, int n, const float* src0, int C0, int 
 int bm_channel_split(const float* src, int B, int T, int Cp, int n, float* dst0, int C0, int ld0, int cm0, int col0,
                      float* dst1, int C1, int ld1, int cm1, int col1, float* dst2, int C2, int ld2, int cm2, int col2,
                      float* dst3, int C3, int ld3, int cm3, int col3, bm_stream_t stream);
+/* ClipLoss's `assert mask.all()` (bm/losses.py:110) on the device, for a step captured in a CUDA graph where the host cannot
+ * read the mask: *status <- code (code != 0; only if *status is still 0) when any of the n bytes of `mask` (a bool tensor)
+ * is 0.  Nothing is written otherwise; n = 0 enqueues nothing.  The caller raises at its next read of the status word. */
+int bm_check_all_true(const unsigned char* mask, long long n, int code, int* status, bm_stream_t stream);
 
 /* ---- Deterministic forms (torch.use_deterministic_algorithms(True) in the drop-in modules) -------------------------
  * Every `_det` entry point computes what its default form computes, with the same arguments plus (where noted) a
