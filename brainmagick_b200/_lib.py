@@ -2,8 +2,10 @@
 or a call fails, this raises."""
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import os
+import threading
 from ctypes import c_float, c_int, c_longlong, c_void_p
 
 import torch
@@ -131,6 +133,8 @@ TF32_FORMS = ("bm_tc_conv1d", "bm_tc_conv1d_persistent", "bm_tc_pointwise_sel", 
               "bm_tc_wgrad_conv", "bm_tc_wgrad_grouped", "bm_clip_scores", "bm_clip_scores_det", "bm_clip_loss_fwd",
               "bm_clip_loss_fwd_det", "bm_clip_loss_bwd", "bm_clip_loss_bwd_cand", "bm_clip_scores_bwd")
 SIGNATURES.update({name + "_tf32": SIGNATURES[name] for name in TF32_FORMS})
+# bf16 forms (bf16() below): the same entry points, the default form's arguments
+SIGNATURES.update({name + "_bf16": SIGNATURES[name] for name in TF32_FORMS})
 
 
 _lib = None
@@ -198,6 +202,32 @@ def tf32() -> bool:
     cuDNN's conv flag is deliberately not read: it defaults to TF32, and the library's default stays 3xTF32.  Read per call;
     the one place the host code asks."""
     return torch.backends.cuda.matmul.fp32_precision == "tf32"
+
+
+_recorded = threading.local()          # .bf16: the mode an autograd node's backward replays (recorded_bf16), or None
+
+
+def bf16() -> bool:
+    """True when every tensor-core contraction should take its bf16 (`_bf16`) form: exactly when torch.autocast is enabled
+    for CUDA with dtype torch.bfloat16 (an fp16 autocast, or a nested `autocast(enabled=False)`, leaves it False).  Inside
+    `recorded_bf16(mode)` it is `mode` instead.  Read per call; the one place the host code asks."""
+    mode = getattr(_recorded, "bf16", None)
+    if mode is not None:
+        return mode
+    return torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == torch.bfloat16
+
+
+@contextlib.contextmanager
+def recorded_bf16(mode: bool):
+    """Runs the body with bf16() == `mode`.  Autocast is thread-local and torch runs the backward outside it, so each
+    autograd node records bf16() in its forward and runs its backward (side-stream weight gradients included) inside
+    recorded_bf16 of that record."""
+    saved = getattr(_recorded, "bf16", None)
+    _recorded.bf16 = bool(mode)
+    try:
+        yield
+    finally:
+        _recorded.bf16 = saved
 
 
 def launch_count() -> int:

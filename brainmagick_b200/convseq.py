@@ -21,7 +21,8 @@ import torch
 from . import _lib
 from ._lib import call, ptr, stream
 from .functional import (SequencePlan, _Needs, _empty, bn_count_batches, bn_plan_fields, bn_sync_groups,
-                         conv_stack_backward, conv_stack_forward, layer_width, stack_conv0, tc_status_tensor)
+                         conv_stack_backward, conv_stack_forward, layer_width, replays_bf16, stack_conv0,
+                         tc_status_tensor)
 
 
 def _present(plan: SequencePlan, k: int) -> tp.List[bool]:
@@ -66,6 +67,7 @@ class _ConvSequenceFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, plan: SequencePlan, x_in, *params):
+        ctx.bf16 = _lib.bf16()                   # the mode the backward replays
         depth = len(plan.dilations)
         it = iter(params)
         conv_p = []
@@ -98,6 +100,7 @@ class _ConvSequenceFn(torch.autograd.Function):
 
     @staticmethod
     @torch.autograd.function.once_differentiable
+    @replays_bf16
     def backward(ctx, dout):
         plan: SequencePlan = ctx.plan
         s = ctx.saved

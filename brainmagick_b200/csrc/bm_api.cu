@@ -24,14 +24,16 @@ using namespace bm;
 
 #define ST(s) reinterpret_cast<cudaStream_t>(s)
 
-// ---- TF32 forms (the `_tf32` entry points) -----------------------------------------------------------------------------
+// ---- TF32 and bf16 forms (the `_tf32` and `_bf16` entry points) ---------------------------------------------------------
 // Every entry point that runs a tensor-core contraction is a static implementation whose first argument is the engine's
-// pass count (tc_common.cuh).  BM_TC_FORMS defines over it the default entry point (3xTF32) and its `_tf32` twin
-// (single-pass TF32: each fp32 operand element rounded once to tf32), with identical arguments.
+// operand mode (tc_common.cuh).  BM_TC_FORMS defines over it the default entry point (3xTF32), its `_tf32` twin
+// (single-pass TF32: each fp32 operand element rounded once to tf32) and its `_bf16` twin (each fp32 operand element
+// rounded once to bf16), with identical arguments.
 #define BM_ARGS(...) __VA_ARGS__
 #define BM_TC_FORMS(name, impl, params, args)                                                                            \
-    extern "C" int name params { return impl(3, BM_ARGS args); }                                                          \
-    extern "C" int name##_tf32 params { return impl(1, BM_ARGS args); }
+    extern "C" int name params { return impl(tc::TC_3XTF32, BM_ARGS args); }                                              \
+    extern "C" int name##_tf32 params { return impl(tc::TC_TF32, BM_ARGS args); }                                         \
+    extern "C" int name##_bf16 params { return impl(tc::TC_BF16, BM_ARGS args); }
 
 extern "C" const char* bm_last_error(void) { return bm::g_last_error; }
 extern "C" int bm_abi_version(void) { return 1; }
@@ -1444,12 +1446,13 @@ extern "C" int bm_tc_weight_split(const float* w, int Cout, int Cin, int Kw, flo
     return 0;
 }
 
-// passes = 1 (the _tf32 form): w_hi alone is read, w_lo may be NULL
+// passes = 1 (the _tf32 form): w_hi alone is read, w_lo may be NULL; TC_BF16 (the _bf16 form): w_hi + w_lo is read,
+// w_lo may be NULL (w_hi then holds the raw fp32 weights)
 static int tc_conv1d(int passes, const float* x, const float* w_hi, const float* w_lo, const float* bias, const float* addend,
                      int B, int T, int Cin, int Ntot, int Kw, int dilation, int sign, int glu, int act, int out_tmajor,
                      float* y, float* aux, float* glu_out, double* stats, int* status, bm_stream_t stream) {
     BM_CHECK_ARG(stats == nullptr);      // BatchNorm statistics in the epilogue: bm_tc_conv1d_persistent / bm_tc_conv1d_f16
-    BM_CHECK_ARG(x && w_hi && (w_lo || passes == 1) && B > 0 && T > 0 && dilation >= 1 && (sign == 1 || sign == -1));
+    BM_CHECK_ARG(x && w_hi && (w_lo || passes != 3) && B > 0 && T > 0 && dilation >= 1 && (sign == 1 || sign == -1));
     BM_CHECK_ARG(glu ? (glu_out != nullptr) : (y != nullptr));
     BM_CHECK_ARG(B <= 65535);
     BM_CHECK_ARG(!(glu && (act || out_tmajor || aux)));
@@ -1740,7 +1743,7 @@ extern "C" int bm_tc_conv1d_f16(const float* x, const float* x_amax, const void*
 //   y[b,t,n] = sum_k x[b,t,k] W[wsel[b]][n][k];  w_hi/w_lo are the tf32-split K-major weight sets [S][Ntot][Cin]
 static int tc_pointwise_sel(int passes, const float* x, const float* w_hi, const float* w_lo, const int* wsel, int n_sets,
                             int B, int T, int Cin, int Ntot, float* y, int* status, bm_stream_t stream) {
-    BM_CHECK_ARG(x && w_hi && (w_lo || passes == 1) && wsel && y && n_sets > 0 && B > 0 && B <= 65535 && T > 0);
+    BM_CHECK_ARG(x && w_hi && (w_lo || passes != 3) && wsel && y && n_sets > 0 && B > 0 && B <= 65535 && T > 0);
     BM_CHECK_ARG(tc::conv_tc_supported(T, Cin, Ntot, 1, 0));
     tc::ConvOp o = tc::conv_op_defaults();
     o.x = x; o.w = w_hi; o.w_lo32 = passes == 1 ? nullptr : w_lo; o.passes = passes;
@@ -1758,7 +1761,7 @@ BM_TC_FORMS(bm_tc_pointwise_sel, tc_pointwise_sel,
 static int tc_sensor_mix_bwd_data(int passes, const float* du, const float* w_hi, const float* w_lo, const int* wsel,
                                   int n_sets, const float* mask, int B, int T, int Op, int Cp, int C, float* dmeg, int* status,
                                   bm_stream_t stream) {
-    BM_CHECK_ARG(du && w_hi && (w_lo || passes == 1) && wsel && dmeg && n_sets > 0 && B > 0 && T > 0 && C > 0 && C <= Cp);
+    BM_CHECK_ARG(du && w_hi && (w_lo || passes != 3) && wsel && dmeg && n_sets > 0 && B > 0 && T > 0 && C > 0 && C <= Cp);
     BM_CHECK_ARG(tc::conv_tc_supported(T, Op, Cp, 1, 0));
     tc::SensorMixBwdOp o;
     memset(&o, 0, sizeof(o));

@@ -1,5 +1,6 @@
 // K6: ClipLoss.get_scores (bm/losses.py:91-94) as ONE split-K tensor-core GEMM (3xTF32 wgmma engine of tc_common.cuh, or
-// its single-pass TF32 form: passes = 1; the candidate norms stay fp64 sums of squares of the fp32 values either way)
+// its single-pass TF32 form: passes = 1, or its bf16 form: passes = TC_BF16; the candidate norms stay fp64 sums of squares
+// of the fp32 values either way)
 // followed by ONE finalize kernel (split reduction + 1/norm scale + row softmax / cross-entropy + batch mean,
 // bm/losses.py:97-114).
 //

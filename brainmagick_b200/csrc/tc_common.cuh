@@ -1,5 +1,6 @@
 // Hopper (sm_90a) tensor-core engine shared by the conv / weight-gradient / CLIP kernels: one 3xTF32 wgmma GEMM
-// (or, with the compile-time pass count PASSES = 1, its single-pass TF32 form: see below)
+// (or, with the compile-time operand mode PASSES = 1, its single-pass TF32 form, or with PASSES = TC_BF16 its bf16 form:
+// see below)
 //
 //     D[m][n] = sum_k A[m][k] * B[n][k]        (fp32 operands, fp32-faithful result)
 //
@@ -30,8 +31,13 @@
 // operand element is rounded once to tf32 (round to nearest, ties away from zero: the `hi` piece of the split), the stages
 // hold no lo tiles, and ONE wgmma per k8 replaces the three.  The per-block fresh register tile and its round-to-nearest
 // adds into the running sum are kept, so the accumulation bias bound and the fixed reduction order do not change.
+// PASSES = TC_BF16 is the bf16 form of the `_bf16` entry points (torch.autocast with dtype bfloat16): every fp32 operand
+// element is rounded once to bf16 (round to nearest even, cvt.rn.bf16x2.f32), the stages hold bf16 tiles of 64-byte rows
+// with the 64-byte swizzle, and two wgmma.k16.bf16 per K block of 32 replace the tf32 MMAs.  Products of bf16 values are
+// exact in fp32, and the per-block fresh tile and its round-to-nearest adds are kept here too.
 #pragma once
 #include <cuda.h>
+#include <cuda_bf16.h>
 #include <algorithm>
 #include <type_traits>
 #include "common.cuh"
@@ -63,6 +69,11 @@ inline int ensure_dyn_smem(const void* func, int bytes) {
 
 namespace tc {
 
+// The operand modes of the main loops, carried by their template argument PASSES and the launchers' `passes`:
+// TC_3XTF32 (three tf32 passes, the default forms), TC_TF32 (one tf32 pass, the `_tf32` forms) and TC_BF16 (one bf16
+// pass, the `_bf16` forms)
+constexpr int TC_3XTF32 = 3, TC_TF32 = 1, TC_BF16 = 2;
+
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
@@ -78,6 +89,14 @@ __device__ __forceinline__ void tf32_split(float x, float& hi, float& lo) {
     hi = __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xFFFFE000u);
     lo = x - hi;
 }
+// (lo, hi) -> two bf16 in one register, each rounded to nearest even, lo in the low half (the K order of a fragment)
+__device__ __forceinline__ uint32_t bf16x2_rn(float lo, float hi) {
+    uint32_t r;
+    asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
+    return r;
+}
+// four consecutive K elements as bf16, rounded to nearest even (8 bytes: x at the lowest address)
+__device__ __forceinline__ uint2 bf16x4_rn(float4 v) { return make_uint2(bf16x2_rn(v.x, v.y), bf16x2_rn(v.z, v.w)); }
 
 // ---------------------------------------------------------------------------------------------------
 // wgmma
@@ -89,6 +108,16 @@ __device__ __forceinline__ uint64_t wgmma_desc_k_sw128(uint32_t smem_addr) {
     d |= (uint64_t)1 << 16;                              // leading byte offset (unused for swizzled K-major)
     d |= (uint64_t)(1024 >> 4) << 32;                    // stride byte offset: next 8-row group
     d |= (uint64_t)1 << 62;                              // SWIZZLE_128B
+    return d;
+}
+// K-major bf16 operand tile, rows of exactly 64 bytes (32 bf16), 64-byte swizzle (16-byte chunk c of row r at chunk
+// c ^ ((r >> 1) & 3)), 8-row groups 512 B apart; the tile starts 1 KB-aligned and a k16 step adds 32 bytes
+__device__ __forceinline__ uint64_t wgmma_desc_k_sw64(uint32_t smem_addr) {
+    uint64_t d = 0;
+    d |= (uint64_t)((smem_addr & 0x3FFFFu) >> 4);        // start address
+    d |= (uint64_t)1 << 16;                              // leading byte offset (unused for swizzled K-major)
+    d |= (uint64_t)(512 >> 4) << 32;                     // stride byte offset: next 8-row group
+    d |= (uint64_t)2 << 62;                              // SWIZZLE_64B
     return d;
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -204,6 +233,118 @@ __device__ __forceinline__ void wgmma_tf32_rs(float* d, const float* a, uint64_t
     static_assert(BN == 128 || BN == 160, "engine tile widths: 128, 160");
     if constexpr (BN == 128) wgmma_tf32_rs_m64n128(d, a, bdesc, accumulate);
     else wgmma_tf32_rs_m64n160(d, a, bdesc, accumulate);
+}
+
+// The bf16 forms (TC_BF16): K = 16 per MMA, bf16 inputs, fp32 accumulators.  Shared-memory operands are K-major tiles of
+// 64-byte rows (32 bf16: one K block) with the 64-byte swizzle (wgmma_desc_k_sw64); a register A fragment is 4 x 32 bits,
+// each two bf16 of one row, the lower K index in the low half: register e of warp w holds row 16 w + lane/4 (+8 for e = 1,
+// 3), K columns 2 (lane % 4) + {0, 1} (+8 for e = 2, 3).
+__device__ __forceinline__ void wgmma_bf16_m64n128(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+
+__device__ __forceinline__ void wgmma_bf16_m64n160(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %82, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n160k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
+        "%80, %81, p, 1, 1, 0, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]),
+          "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]),
+          "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+
+__device__ __forceinline__ void wgmma_bf16_rs_m64n128(float* d, const uint32_t* a, uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %69, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]),
+          "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+
+__device__ __forceinline__ void wgmma_bf16_rs_m64n160(float* d, const uint32_t* a, uint64_t bdesc, int accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %85, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n160k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, "
+        "%32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, "
+        "%48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, "
+        "%64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79}, "
+        "{%80, %81, %82, %83}, %84, p, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]),
+          "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]),
+          "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]),
+          "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]),
+          "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]),
+          "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]),
+          "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]),
+          "l"(bdesc), "r"(accumulate)
+        : "memory");
+}
+template <int BN>
+__device__ __forceinline__ void wgmma_bf16(float* d, uint64_t adesc, uint64_t bdesc, int accumulate) {
+    static_assert(BN == 128 || BN == 160, "engine tile widths: 128, 160");
+    if constexpr (BN == 128) wgmma_bf16_m64n128(d, adesc, bdesc, accumulate);
+    else wgmma_bf16_m64n160(d, adesc, bdesc, accumulate);
+}
+template <int BN>
+__device__ __forceinline__ void wgmma_bf16_rs(float* d, const uint32_t* a, uint64_t bdesc, int accumulate) {
+    static_assert(BN == 128 || BN == 160, "engine tile widths: 128, 160");
+    if constexpr (BN == 128) wgmma_bf16_rs_m64n128(d, a, bdesc, accumulate);
+    else wgmma_bf16_rs_m64n160(d, a, bdesc, accumulate);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -322,10 +463,13 @@ struct HcProbe {
 // ---------------------------------------------------------------------------------------------------
 constexpr int HG_BM = 128, HG_BN = 128, HG_BK = 32, HG_THREADS = 256;
 constexpr int HG_TILE_BYTES = 128 * HG_BK * 4;                        // 16 KB: 128 rows x 32 fp32
-// one stage: A hi | A lo (128 rows each) | B hi | B lo (BN rows each), the lo tiles only when PASSES = 3; double-buffered,
-// 1 KB alignment slack
+// one K block of a K-major operand tile of `rows` rows in shared memory: 32 tf32 (128-byte rows) or, for TC_BF16, 32 bf16
+// (64-byte rows)
+template <int PASSES> constexpr int hg_tile_bytes(int rows) { return rows * HG_BK * (PASSES == TC_BF16 ? 2 : 4); }
+// one stage: A hi | A lo (128 rows each) | B hi | B lo (BN rows each), the lo tiles only when PASSES = 3 (TC_BF16: A and
+// B as bf16); double-buffered, 1 KB alignment slack
 template <int BN, int PASSES> constexpr int hg_stage_bytes() {
-    return (PASSES == 3 ? 2 : 1) * (HG_TILE_BYTES + BN * HG_BK * 4);
+    return (PASSES == 3 ? 2 : 1) * (hg_tile_bytes<PASSES>(HG_BM) + hg_tile_bytes<PASSES>(BN));
 }
 template <int BN, int PASSES> constexpr int hg_smem_bytes() { return 2 * hg_stage_bytes<BN, PASSES>() + 1024; }
 
@@ -340,7 +484,9 @@ inline int hg_pick_bn(long long n) {
 //   K-contiguous operand (Op::A_KCONTIG / B_KCONTIG):  v4(cta, kb, row, q) = elements k = 4q .. 4q+3 of tile row `row`
 //   M/N-contiguous operand:                            v4(cta, kb, k, q)   = tile rows 4q .. 4q+3 at reduction index k
 // Out-of-range elements (padding, tails, other samples) are returned as zeros.  store<PASSES> writes the tf32 pieces of a
-// float4 into the hi and lo tiles (PASSES = 3) or its rounded value into the hi tile alone (PASSES = 1: `lo` is not touched).
+// float4 into the hi and lo tiles (PASSES = 3) or its rounded value into the hi tile alone (PASSES = 1: `lo` is not touched;
+// TC_BF16: rounded to bf16 into the 64-byte-row layout of wgmma_desc_k_sw64, 8 bytes per float4 of a K-contiguous operand,
+// 2 bytes per element of a transposed one).
 template <bool KCONTIG, int ROWS>
 struct HgSlot {
     static constexpr int N4 = ROWS / 32;       // float4 moved per thread per tile
@@ -356,7 +502,19 @@ struct HgSlot {
     }
     template <int PASSES>
     __device__ static void store(uint8_t* hi, uint8_t* lo, int i, int q, float4 v) {
-        if (KCONTIG) {
+        if constexpr (PASSES == TC_BF16) {
+            if (KCONTIG) {                             // row i, K elements 4q .. 4q+3: chunk q / 2, half q & 1
+                *reinterpret_cast<uint2*>(hi + i * 64 + (((q >> 1) ^ ((i >> 1) & 3)) << 4) + (q & 1) * 8) = bf16x4_rn(v);
+            } else {                                   // rows 4q .. 4q+3, K element i
+                const float e[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+                for (int c = 0; c < 4; ++c) {
+                    const int r = 4 * q + c;
+                    *reinterpret_cast<__nv_bfloat16*>(hi + r * 64 + (((i >> 3) ^ ((r >> 1) & 3)) << 4) + (i & 7) * 2) =
+                        __float2bfloat16_rn(e[c]);
+                }
+            }
+        } else if (KCONTIG) {
             float4 h, l;
             tf32_split(v.x, h.x, l.x); tf32_split(v.y, h.y, l.y); tf32_split(v.z, h.z, l.z); tf32_split(v.w, h.w, l.w);
             const int off = i * 128 + ((q ^ (i & 7)) << 4);
@@ -388,9 +546,10 @@ __device__ __forceinline__ int hg_col(int i) { return 8 * (i >> 2) + 2 * (thread
 
 template <class Op, int BN, int PASSES>
 __global__ void __launch_bounds__(HG_THREADS, 1) hg_gemm_kernel(const __grid_constant__ Op op) {
-    static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or single-pass TF32");
-    constexpr int NACC = BN / 2, STAGE = hg_stage_bytes<BN, PASSES>(), B_TILE = BN * HG_BK * 4;
-    constexpr int A_LO = HG_TILE_BYTES, B_HI = (PASSES == 3 ? 2 : 1) * HG_TILE_BYTES;   // tile offsets in a stage
+    static_assert(PASSES == TC_3XTF32 || PASSES == TC_TF32 || PASSES == TC_BF16, "3xTF32, single-pass TF32 or bf16");
+    constexpr int NACC = BN / 2, STAGE = hg_stage_bytes<BN, PASSES>(), B_TILE = hg_tile_bytes<PASSES>(BN);
+    constexpr int A_TILE = hg_tile_bytes<PASSES>(HG_BM);
+    constexpr int A_LO = A_TILE, B_HI = (PASSES == 3 ? 2 : 1) * A_TILE;                 // tile offsets in a stage
     extern __shared__ uint8_t smem_raw[];
     const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base_u32 - smem_u32(smem_raw));
@@ -444,20 +603,26 @@ __global__ void __launch_bounds__(HG_THREADS, 1) hg_gemm_kernel(const __grid_con
         const int s = kb & 1;
         if (kb + 1 < nkb) fetch(kb + 1);
         const uint32_t st = base_u32 + s * STAGE;
-        const uint32_t a_hi = st + wg * (HG_TILE_BYTES / 2), a_lo = a_hi + A_LO;
+        const uint32_t a_hi = st + wg * (A_TILE / 2), a_lo = a_hi + A_LO;
         const uint32_t b_hi = st + B_HI, b_lo = b_hi + B_TILE;
         wgmma_fence();
+        if constexpr (PASSES == TC_BF16) {
 #pragma unroll
-        for (int kk = 0; kk < HG_BK / 8; ++kk) {
-            const uint32_t off = kk * 32;                  // 8 tf32 = 32 bytes along K inside the swizzle span
-            const uint64_t dah = wgmma_desc_k_sw128(a_hi + off), dbh = wgmma_desc_k_sw128(b_hi + off);
-            if constexpr (PASSES == 3) {
-                const uint64_t dal = wgmma_desc_k_sw128(a_lo + off), dbl = wgmma_desc_k_sw128(b_lo + off);
-                wgmma_tf32<BN>(part, dal, dbh, kk != 0);
-                wgmma_tf32<BN>(part, dah, dbl, 1);
-                wgmma_tf32<BN>(part, dah, dbh, 1);
-            } else {
-                wgmma_tf32<BN>(part, dah, dbh, kk != 0);
+            for (int kk = 0; kk < HG_BK / 16; ++kk)       // 16 bf16 = 32 bytes along K inside the 64-byte swizzle span
+                wgmma_bf16<BN>(part, wgmma_desc_k_sw64(a_hi + kk * 32), wgmma_desc_k_sw64(b_hi + kk * 32), kk != 0);
+        } else {
+#pragma unroll
+            for (int kk = 0; kk < HG_BK / 8; ++kk) {
+                const uint32_t off = kk * 32;              // 8 tf32 = 32 bytes along K inside the swizzle span
+                const uint64_t dah = wgmma_desc_k_sw128(a_hi + off), dbh = wgmma_desc_k_sw128(b_hi + off);
+                if constexpr (PASSES == 3) {
+                    const uint64_t dal = wgmma_desc_k_sw128(a_lo + off), dbl = wgmma_desc_k_sw128(b_lo + off);
+                    wgmma_tf32<BN>(part, dal, dbh, kk != 0);
+                    wgmma_tf32<BN>(part, dah, dbl, 1);
+                    wgmma_tf32<BN>(part, dah, dbh, 1);
+                } else {
+                    wgmma_tf32<BN>(part, dah, dbh, kk != 0);
+                }
             }
         }
         wgmma_commit();
@@ -483,9 +648,10 @@ inline int hg_run(const Op& op, dim3 grid, cudaStream_t st, const char* who) {
     if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", who, cudaGetErrorString(e));
     return 0;
 }
-// passes: 3 (3xTF32) or 1 (single-pass TF32)
+// passes: TC_3XTF32, TC_TF32 or TC_BF16
 template <int BN, class Op>
 inline int hg_launch(const Op& op, dim3 grid, int passes, cudaStream_t st, const char* who) {
+    if (passes == TC_BF16) return hg_run<BN, TC_BF16>(op, grid, st, who);
     return passes == 1 ? hg_run<BN, 1>(op, grid, st, who) : hg_run<BN, 3>(op, grid, st, who);
 }
 // the same with the tile width of hg_pick_bn
@@ -516,6 +682,11 @@ inline int hg_launch_bn(int bn, const Op& op, dim3 grid, int passes, cudaStream_
 // read by the wgmmas (the register-staged loop also wrote A hi/lo and read A twice per MMA).
 // PASSES = 1 (single-pass TF32): the producer stores B's rounded value alone (the pre-split format reads only its hi
 // piece), the consumers round A in registers with cvt.rna and issue one wgmma per k8; B traffic: 20 KB written + 40 KB read.
+// TC_BF16 (the bf16 form): the stage keeps the raw fp32 A tile that TMA writes (TMA cannot round) and B as bf16 in 64-byte
+// rows with the 64-byte swizzle (wgmma_desc_k_sw64: 32 bf16 = one K block per row, so the 32-wide blocks, the stage count
+// and the ring are unchanged).  The producer rounds B to bf16 on its store (the pre-split format: hi + lo, rounded once),
+// the consumers convert their fp32 A fragment to bf16x2 registers and issue one k16 wgmma per 16 K; B traffic: 10 KB
+// written + 20 KB read per block at BN = 160.
 constexpr int HC_THREADS = 384, HC_CONSUMERS = 256, HC_STAGES = 3;
 constexpr int HC_PRODUCER_REGS = 104, HC_CONSUMER_REGS = 200;    // 104 * 128 + 200 * 256 = 168 * 384 registers
 // __launch_bounds__(HC_THREADS, 1) compiles the kernels for 168 registers per thread (65 536 / 384, rounded down to a
@@ -524,9 +695,11 @@ constexpr int HC_PRODUCER_REGS = 104, HC_CONSUMER_REGS = 200;    // 104 * 128 + 
 static_assert(HC_PRODUCER_REGS * 128 + HC_CONSUMER_REGS * HC_CONSUMERS <= (65536 / HC_THREADS) / 8 * 8 * HC_THREADS,
               "the producer / consumer register split must fit in the registers the CTA is launched with");
 constexpr int HC_ERR_FULL = 901, HC_ERR_EMPTY = 902;           // status codes of a timed-out consumer / producer wait
-// one stage: A raw fp32 (128 rows) | B hi | B lo (BN rows each; no lo tile when PASSES = 1), every tile 1 KB-aligned for
-// the 128-byte swizzle
-template <int BN, int PASSES> constexpr int hc_stage_bytes() { return HG_TILE_BYTES + (PASSES == 3 ? 2 : 1) * BN * HG_BK * 4; }
+// one stage: A raw fp32 (128 rows) | B hi | B lo (BN rows each; no lo tile when PASSES = 1, B as bf16 when TC_BF16),
+// every tile 1 KB-aligned for the swizzle
+template <int BN, int PASSES> constexpr int hc_stage_bytes() {
+    return HG_TILE_BYTES + (PASSES == 3 ? 2 : 1) * hg_tile_bytes<PASSES>(BN);
+}
 template <int BN, int PASSES> constexpr int hc_smem_bytes() { return HC_STAGES * hc_stage_bytes<BN, PASSES>() + 1024; }
 
 // index of a consumer thread in [0, 256) and a barrier over the consumer warpgroups only (the producer does not take part)
@@ -552,13 +725,29 @@ struct HcBars {
 // into tf32 hi/lo in registers (PASSES = 1: rounded once with cvt.rna) and multiplied with the stage's B tiles at b_hi
 // (hi) and b_hi + BN x 32 x 4 (lo): lo*hi + hi*lo + hi*hi per k8 into a fresh `part` tile (PASSES = 1: one wgmma per k8);
 // once the MMAs have drained, release() hands the stage back and `part` is added into `acc` with round-to-nearest FADDs.
+// TC_BF16: a(kk, e) is read as a float2 instead -- the fp32 elements of fragment register e of k16 step kk in the layout of
+// wgmma_bf16_rs (row r0 + 8 (e & 1), K columns 16 kk + 8 (e >> 1) + 2 tq + {0, 1}) -- rounded to bf16x2 with
+// cvt.rn and multiplied with the bf16 B tile at b_hi, one wgmma per k16.
 // The two warpgroups issue their blocks concurrently: their 2 x 12 MMAs then take ~1900 clocks per block at BN = 160, the
 // tensor floor; issuing them one warpgroup after the other measured slower (DESIGN §4.2).
 template <int BN, int PASSES, class LoadA, class Release>
 __device__ __forceinline__ void hc_consume_block(float* acc, float* part, uint32_t b_hi, const LoadA& a,
                                                  const Release& release, HcProbe& pr) {
     constexpr int NACC = BN / 2, B_TILE = BN * HG_BK * 4;
-    if constexpr (PASSES == 3) {
+    if constexpr (PASSES == TC_BF16) {
+        uint32_t r[2][4];                           // [k16][fragment register]: two bf16 each
+#pragma unroll
+        for (int kk = 0; kk < HG_BK / 16; ++kk)
+#pragma unroll
+            for (int e = 0; e < 4; ++e) {
+                const float2 v = a(kk, e);
+                r[kk][e] = bf16x2_rn(v.x, v.y);
+            }
+        pr.mark(HP_SPLIT_ADD);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < HG_BK / 16; ++kk) wgmma_bf16_rs<BN>(part, r[kk], wgmma_desc_k_sw64(b_hi + kk * 32), kk != 0);
+    } else if constexpr (PASSES == 3) {
         float hi[4][4], lo[4][4];                   // [k8][fragment element]
 #pragma unroll
         for (int kk = 0; kk < HG_BK / 8; ++kk)
@@ -598,9 +787,9 @@ __device__ __forceinline__ void hc_consume_block(float* acc, float* part, uint32
 template <class Op, int BN, int PASSES>
 __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_constant__ Op op,
                                                                const __grid_constant__ CUtensorMap xmap, int tiles) {
-    static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or single-pass TF32");
+    static_assert(PASSES == TC_3XTF32 || PASSES == TC_TF32 || PASSES == TC_BF16, "3xTF32, single-pass TF32 or bf16");
     const uint32_t t_start = HcProbe::now();        // the probe's CTA start (BM_HC_PHASES)
-    constexpr int NACC = BN / 2, STAGE = hc_stage_bytes<BN, PASSES>(), B_TILE = BN * HG_BK * 4;
+    constexpr int NACC = BN / 2, STAGE = hc_stage_bytes<BN, PASSES>(), B_TILE = hg_tile_bytes<PASSES>(BN);
     extern __shared__ uint8_t smem_raw[];
     __shared__ HcBars bars;
     const uint32_t base_u32 = (smem_u32(smem_raw) + 1023u) & ~1023u;
@@ -688,6 +877,9 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_con
         bool ok;
         if constexpr (PASSES == 1)                      // raw or the hi piece of the split (rounding it again changes nothing);
             ok = produce(std::integral_constant<int, Op::B_RAW>());     // the launcher refuses the fp16 pieces
+        else if constexpr (PASSES == TC_BF16)          // raw, or hi + lo of the split rounded once (no fp16 pieces either)
+            ok = f == Op::B_RAW ? produce(std::integral_constant<int, Op::B_RAW>())
+                                : produce(std::integral_constant<int, Op::B_SPLIT>());
         else
             ok = f == Op::B_RAW     ? produce(std::integral_constant<int, Op::B_RAW>())
                  : f == Op::B_SPLIT ? produce(std::integral_constant<int, Op::B_SPLIT>())
@@ -706,6 +898,9 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_con
     // 32 row + 4 (c ^ grp) + tq of the swizzled tile, i.e. (w0 ^ 4 c) + 256 (e & 1) with w0 = 32 r0 + 4 grp + tq (bits 2-4
     // of w0 hold grp alone), one register for all 16 addresses.
     const int w0 = 32 * r0 + 4 * grp + tq;
+    // TC_BF16: the float2 of register e of k16 step kk is at word (wb ^ 4 (4 kk + 2 (e >> 1))) + 256 (e & 1): the chunk
+    // bit tq / 2 joins grp in bits 2-4, which the XOR with the even chunk offset leaves in place
+    const int wb = 32 * r0 + 4 * ((tq >> 1) ^ grp) + 2 * (tq & 1);
     float acc[NACC], part[NACC];
     // The ring position, packed into one register (the consumers' registers are taken by acc, part and the A fragment):
     // the stage (bits 0-1), the round through the ring mod 2 = the parity of the stage's full-barrier phase (bit 2) and the
@@ -725,7 +920,12 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hc_conv_kernel(const __grid_con
             const float* at = reinterpret_cast<const float*>(smem + s * STAGE);
             hc_consume_block<BN, PASSES>(
                 acc, part, base_u32 + s * STAGE + HG_TILE_BYTES,
-                [&](int kk, int e) { return at[(w0 ^ (4 * (2 * kk + (e >> 1)))) + 256 * (e & 1)]; },
+                [&](int kk, int e) {
+                    if constexpr (PASSES == TC_BF16)        // 16-byte chunk 4 kk + 2 (e >> 1) + tq / 2, words 2 (tq & 1) + {0, 1}
+                        return *reinterpret_cast<const float2*>(at + ((wb ^ (4 * (4 * kk + 2 * (e >> 1)))) + 256 * (e & 1)));
+                    else
+                        return at[(w0 ^ (4 * (2 * kk + (e >> 1)))) + 256 * (e & 1)];
+                },
                 [&] {
                     __syncwarp();
                     if (lane == 0) mbar_arrive(bars.empty(s));
@@ -790,12 +990,17 @@ inline int hc_launch(const Op& op, long long tiles, cudaStream_t st, const char*
     if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", who, cudaGetErrorString(e));
     return 0;
 }
-// the tile width of hg_pick_bn and the pass count op.passes (3 or 1; the fp16-piece weights only with 3)
+// the tile width of hg_pick_bn and the operand mode op.passes (TC_3XTF32, TC_TF32 or TC_BF16; the fp16-piece weights
+// only with TC_3XTF32)
 template <class Op>
 inline int hc_launch_bn(int bn, const Op& op, long long tiles, cudaStream_t st, const char* who) {
     if (op.passes == 1) {
         if (!op.w) return set_error(2, "%s: the single-pass form takes fp32 weights%s", who);
         return bn == 160 ? hc_launch<160, 1>(op, tiles, st, who) : hc_launch<128, 1>(op, tiles, st, who);
+    }
+    if (op.passes == TC_BF16) {
+        if (!op.w) return set_error(2, "%s: the bf16 form takes fp32 weights%s", who);
+        return bn == 160 ? hc_launch<160, TC_BF16>(op, tiles, st, who) : hc_launch<128, TC_BF16>(op, tiles, st, who);
     }
     return bn == 160 ? hc_launch<160, 3>(op, tiles, st, who) : hc_launch<128, 3>(op, tiles, st, who);
 }
@@ -839,6 +1044,8 @@ inline int hc_launch_bn(int bn, const Op& op, long long tiles, cudaStream_t st, 
 //     distinct.
 // (Plain c = s0 + 2 s1 + 4 s2 would leave the stores 4-way conflicted, since m & 7 sees only c's low bit; s2 feeding both
 // c and a is what spreads both sides.)
+// TC_BF16: the same sub-blocks and loads; per m one 8-byte store of the 4 p rounded to bf16, into the 64-byte-row B tile of
+// wgmma_desc_k_sw64 (byte 64 m + 16 ((p / 8) ^ ((m / 2) & 3)) + 2 (p & 7)).
 template <int BN, int PASSES>
 struct HwTranspose {
     static constexpr int NSUB = 2 * BN, NJ = (NSUB + 127) / 128;     // sub-blocks per block, per thread (the last partly)
@@ -850,7 +1057,10 @@ struct HwTranspose {
             const int c = (s & 1) | ((s >> 1) & 2) | ((s >> 2) & 4);
             const int a = ((s >> 1) & 1) | (((s >> 1) ^ (s >> 2)) & 2) | ((s >> 3) & 4);
             ro[j] = box * (32 * 128) + a * 512 + ((c ^ 4 * (a & 1)) << 4);     // row 4 a, chunk c ^ (4 a & 7)
-            bo[j] = (32 * box + 4 * c) * 128 + ((a ^ 4 * (c & 1)) << 4);      // row 4 c, chunk a ^ (4 c & 7)
+            if constexpr (PASSES == TC_BF16)                                   // row 4 c, chunk (a / 2) ^ 2 (c & 1), half a & 1
+                bo[j] = (32 * box + 4 * c) * 64 + (((a >> 1) ^ 2 * (c & 1)) << 4) + 8 * (a & 1);
+            else
+                bo[j] = (32 * box + 4 * c) * 128 + ((a ^ 4 * (c & 1)) << 4);  // row 4 c, chunk a ^ (4 c & 7)
         }
     }
     __device__ void run(const uint8_t* raw, uint8_t* hi, uint8_t* lo, int t) const {
@@ -862,6 +1072,13 @@ struct HwTranspose {
             for (int i = 0; i < 4; ++i) {
                 const float4 r = *reinterpret_cast<const float4*>(raw + ((ro[j] + 128 * i) ^ (i << 4)));
                 v[i][0] = r.x; v[i][1] = r.y; v[i][2] = r.z; v[i][3] = r.w;
+            }
+            if constexpr (PASSES == TC_BF16) {
+#pragma unroll
+                for (int e = 0; e < 4; ++e)                            // row 4 c + e: chunk bit 0 ^= e / 2
+                    *reinterpret_cast<uint2*>(hi + ((bo[j] + 64 * e) ^ ((e >> 1) << 4))) =
+                        bf16x4_rn(make_float4(v[0][e], v[1][e], v[2][e], v[3][e]));
+                continue;
             }
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
@@ -877,6 +1094,7 @@ struct HwTranspose {
 };
 // a barrier over the producer warpgroup's 128 threads only (id 2: hc_consumer_sync uses 1)
 __device__ __forceinline__ void hw_producer_sync() { asm volatile("bar.sync 2, 128;" ::: "memory"); }
+// the stages and 2 raw fp32 dY staging slots
 template <int BN, int PASSES> constexpr int hw_smem_bytes() { return hc_smem_bytes<BN, PASSES>() + 2 * BN * HG_BK * 4; }
 
 // bits a .. b-1 of a 32-bit mask (clamped to [0, 32))
@@ -890,11 +1108,11 @@ template <class Op, int BN, int PASSES>
 __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_constant__ Op op,
                                                                 const __grid_constant__ CUtensorMap xmap,
                                                                 const __grid_constant__ CUtensorMap ymap) {
-    static_assert(PASSES == 3 || PASSES == 1, "3xTF32 or single-pass TF32");
-    constexpr int NACC = BN / 2, STAGE = hc_stage_bytes<BN, PASSES>(), B_TILE = BN * HG_BK * 4;
+    static_assert(PASSES == TC_3XTF32 || PASSES == TC_TF32 || PASSES == TC_BF16, "3xTF32, single-pass TF32 or bf16");
+    constexpr int NACC = BN / 2, STAGE = hc_stage_bytes<BN, PASSES>(), B_TILE = hg_tile_bytes<PASSES>(BN);
     const uint32_t t_start = HcProbe::now();        // the probe's CTA start (BM_HC_PHASES)
     constexpr int BOX_BYTES = HG_BK * HG_BK * 4;                 // one [32 p][32 channels] box of A or dY
-    constexpr int RAW = HC_STAGES * STAGE;                       // the dY staging ring: 2 slots of B_TILE bytes
+    constexpr int RAW = HC_STAGES * STAGE, SLOT = BN * HG_BK * 4;   // the dY staging ring: 2 slots of raw fp32
     extern __shared__ uint8_t smem_raw[];
     __shared__ HcBars bars;
     __shared__ uint64_t dy_bars[2];                              // one per staging slot: thread 0's arrival + the TMA bytes
@@ -923,8 +1141,8 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
         }
         const HwTranspose<BN, PASSES> tr(tid);
         auto stage_dy = [&](int kb) {                    // thread 0: block kb's dY boxes into staging slot kb & 1
-            const uint32_t bar = smem_u32(&dy_bars[kb & 1]), slot = base_u32 + RAW + (kb & 1) * B_TILE;
-            mbar_expect_tx(bar, B_TILE);
+            const uint32_t bar = smem_u32(&dy_bars[kb & 1]), slot = base_u32 + RAW + (kb & 1) * SLOT;
+            mbar_expect_tx(bar, SLOT);
 #pragma unroll
             for (int j = 0; j < BN / 32; ++j) {
                 const int2 c = op.b_box(cta, kb, j);
@@ -957,7 +1175,7 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
             }
             pr.mark(HP_B_LOAD);
             uint8_t* bh = smem + s * STAGE + HG_TILE_BYTES;
-            tr.run(smem + RAW + (kb & 1) * B_TILE, bh, bh + B_TILE, tid);
+            tr.run(smem + RAW + (kb & 1) * SLOT, bh, bh + B_TILE, tid);
             fence_proxy_async();                               // the generic-proxy stores, before the wgmmas read them
             mbar_arrive(full);
             hw_producer_sync();                                // every read of this staging slot, before its next TMA
@@ -983,6 +1201,16 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
         const int c = (r0 & 31) + 8 * (e & 1), kq = tq + 4 * (e >> 1);
         off[e] = (r0 >> 5) * (BOX_BYTES / 4) + kq * 32 + (((c >> 2) ^ kq) << 2) + (c & 3);
     }
+    // TC_BF16: word offset of the pair element i of fragment register e (row r0 + 8 (e & 1), k = 2 tq + i + 8 (e >> 1))
+    // at kk = 0, indexed [e & 1][i]; e >> 1 adds 8 rows of the box and a k16 step kk 16
+    int offb[2][2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int i = 0; i < 2; ++i) {
+            const int c = (r0 & 31) + 8 * h, kq = 2 * tq + i;
+            offb[h][i] = (r0 >> 5) * (BOX_BYTES / 4) + kq * 32 + (((c >> 2) ^ kq) << 2) + (c & 3);
+        }
     float acc[NACC], part[NACC];
 #pragma unroll
     for (int i = 0; i < NACC; ++i) acc[i] = 0.f;
@@ -992,7 +1220,8 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
         // rows k of this block that contribute: t0 + k in [tlo, thi), or in [tlo + T, thi + T) past the sample's end,
         // and p < R
         const int p = p0 + kb * HG_BK;
-        const uint32_t live = ((hw_bits(tlo - t0, thi - t0) | hw_bits(tlo + T - t0, thi + T - t0)) & hw_bits(0, op.R - p)) >> tq;
+        const uint32_t live = ((hw_bits(tlo - t0, thi - t0) | hw_bits(tlo + T - t0, thi + T - t0)) & hw_bits(0, op.R - p)) >>
+                              (PASSES == TC_BF16 ? 2 * tq : tq);
         t0 += HG_BK;
         if (t0 >= T) t0 -= T;
         if (!mbar_wait(bars.full(s), use & 1)) {
@@ -1005,8 +1234,14 @@ __global__ void __launch_bounds__(HC_THREADS, 1) hw_wgrad_kernel(const __grid_co
         hc_consume_block<BN, PASSES>(
             acc, part, base_u32 + s * STAGE + HG_TILE_BYTES,
             [&](int kk, int e) {
-                const float v = at[off[e] + 8 * 32 * kk];
-                return (live >> (8 * kk + 4 * (e >> 1))) & 1 ? v : 0.f;
+                if constexpr (PASSES == TC_BF16) {
+                    const int d = 8 * 32 * (e >> 1) + 16 * 32 * kk, k = 16 * kk + 8 * (e >> 1);
+                    const float v0 = at[offb[e & 1][0] + d], v1 = at[offb[e & 1][1] + d];
+                    return make_float2((live >> k) & 1 ? v0 : 0.f, (live >> (k + 1)) & 1 ? v1 : 0.f);
+                } else {
+                    const float v = at[off[e] + 8 * 32 * kk];
+                    return (live >> (8 * kk + 4 * (e >> 1))) & 1 ? v : 0.f;
+                }
             },
             [&] {
                 __syncwarp();
@@ -1038,9 +1273,11 @@ inline int hw_launch(const Op& op, dim3 grid, cudaStream_t st, const char* who) 
     if (e != cudaSuccess) return set_error(3, "%s: launch failed: %s", who, cudaGetErrorString(e));
     return 0;
 }
-// tile width 160 or 128 (hg_pick_bn), passes 3 or 1
+// tile width 160 or 128 (hg_pick_bn), passes TC_3XTF32, TC_TF32 or TC_BF16
 template <class Op>
 inline int hw_launch_bn(int bn, const Op& op, dim3 grid, int passes, cudaStream_t st, const char* who) {
+    if (passes == TC_BF16)
+        return bn == 160 ? hw_launch<160, TC_BF16>(op, grid, st, who) : hw_launch<128, TC_BF16>(op, grid, st, who);
     if (passes == 1) return bn == 160 ? hw_launch<160, 1>(op, grid, st, who) : hw_launch<128, 1>(op, grid, st, who);
     return bn == 160 ? hw_launch<160, 3>(op, grid, st, who) : hw_launch<128, 3>(op, grid, st, who);
 }

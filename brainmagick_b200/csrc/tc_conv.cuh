@@ -1,5 +1,6 @@
 // K3/K4/K5 on the Hopper tensor cores: dilated Conv1d (and its data gradient, and the 1x1 head / subject layers) as an
-// implicit GEMM on the 3xTF32 wgmma engine of tc_common.cuh (or its single-pass TF32 form: ConvOp::passes = 1).
+// implicit GEMM on the 3xTF32 wgmma engine of tc_common.cuh (or its single-pass TF32 form: ConvOp::passes = 1, or its bf16
+// form: ConvOp::passes = TC_BF16).
 //
 //   y[b, t, n] = bias[n] + sum_{tap} sum_{k} x[b, t + shift(tap), k] * W[wset(b)][tap][n][k]      (channels-last x, y)
 //
@@ -60,7 +61,8 @@ struct ConvOp {
     unsigned int* out_amax;               // max |GELU / GLU output| (float bits) or null
     int act, out_tmajor;
     int* err;
-    int passes;                           // 3: 3xTF32, 1: single-pass TF32 (reads w alone; not with the fp16 pieces)
+    int passes;                           // 3: 3xTF32, 1: single-pass TF32 (reads w alone), TC_BF16: bf16 (w + w_lo32
+                                          // rounded once); not with the fp16 pieces
 
     struct Cta { int b, t0, n_tile, wbase; float w_inv; };
     template <int BN> __device__ Cta cta(int tile) const {

@@ -1,5 +1,5 @@
 // ClipLoss backward contractions (bm/losses.py:91-114 differentiated, SURVEY.md A.6) on the 3xTF32 wgmma engine (or its
-// single-pass TF32 form: passes = 1):
+// single-pass TF32 / bf16 forms: passes = 1 / TC_BF16):
 //
 //     D[m][n] = sum_k A[m][k] * B[k][n]        A [M][K] row-major (K contiguous), B [K][N] row-major (N contiguous)
 //

@@ -1,4 +1,5 @@
-// Weight gradients on the tensor cores (3xTF32 wgmma engine of tc_common.cuh, or its single-pass TF32 form: passes = 1):
+// Weight gradients on the tensor cores (3xTF32 wgmma engine of tc_common.cuh, or its single-pass TF32 / bf16 forms:
+// passes = 1 / TC_BF16):
 // for one tap shift s
 //
 //     P[ks][m][n] = sum_{b in split ks} sum_t  dY[b, t, m] * X[b, t + s, n]          (dY, X channels-last)

@@ -8,12 +8,14 @@ flashy.distrib.sync_model expect), and on `meg` when it requires grad (gradient-
 
 Kernel selection is by shape only: contractions whose channel counts fit the tensor-core tiling (K % 32 == 0 and an
 N tile of 64..160 dividing N -- every layer of the real clip_conv model) run on the tensor-core kernels
-(3xTF32, `bm_tc_*`; single-pass TF32 when PyTorch's float32 matmul precision allows TF32, see `_tc_call`); other shapes
+(3xTF32, `bm_tc_*`; single-pass TF32 when PyTorch's float32 matmul precision allows TF32, bf16 operands under bf16
+autocast, see `_tc_call`); other shapes
 (the tiny unit-test models) run on the FP32-FMA kernels of the same library.
 """
 from __future__ import annotations
 
 import dataclasses
+import functools
 import typing as tp
 
 import torch
@@ -294,19 +296,32 @@ def _reducing_call(name, like, ws_dims, *args, reduces=True):
     return call(name + "_det", *args[:-1], ptr(ws), ws.numel(), args[-1])
 
 
-# ---- TF32 forms -----------------------------------------------------------------------------------------------------
+# ---- TF32 and bf16 forms ---------------------------------------------------------------------------------------------
 # Under TF32 matmul precision (`_lib.tf32()`: torch.set_float32_matmul_precision("high"), matmul.allow_tf32 = True, ...) every
-# tensor-core contraction takes its single-pass `_tf32` form (include/bm_b200.h), with the same arguments.  The FP32-FMA
-# kernels stay exact (TF32 is permitted, not required) and the fp16-piece entry points keep their one form.
+# tensor-core contraction takes its single-pass `_tf32` form (include/bm_b200.h), with the same arguments.  Under
+# torch.autocast("cuda", dtype=torch.bfloat16) (`_lib.bf16()`, recorded by each autograd node's forward for its backward)
+# it takes its `_bf16` form instead, whatever the TF32 flag says.  The FP32-FMA kernels stay exact (TF32 and bf16 are
+# permitted, not required) and the fp16-piece entry points keep their one form.
 _DET_SAME_ARGS = ("bm_clip_scores", "bm_clip_loss_fwd")      # tensor-core entry points with a `_det` form of the same arguments
 
 
+def replays_bf16(backward):
+    """An autograd node's backward, run with the bf16 mode its forward recorded in `ctx.bf16` (`_lib.recorded_bf16`)."""
+    @functools.wraps(backward)
+    def run(ctx, *grads):
+        with _lib.recorded_bf16(ctx.bf16):
+            return backward(ctx, *grads)
+    return run
+
+
 def _tc_call(name, *args):
-    """call(name[_det][_tf32], *args) for a tensor-core entry point: its `_det` form under the determinism flag where it has
-    one, then the `_tf32` form under TF32 matmul precision."""
+    """call(name[_det][_bf16 | _tf32], *args) for a tensor-core entry point: its `_det` form under the determinism flag where
+    it has one, then the `_bf16` form under bf16 autocast, else the `_tf32` form under TF32 matmul precision."""
     if name in _DET_SAME_ARGS and _lib.deterministic():
         name += "_det"
-    if _lib.tf32():
+    if _lib.bf16():
+        name += "_bf16"
+    elif _lib.tf32():
         name += "_tf32"
     return call(name, *args)
 
@@ -1443,6 +1458,7 @@ class _EncoderFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, plan: EncoderPlan, meg, heads, il_w, il_b, subj_w, w0, b0, w2, b2, *params):
+        ctx.bf16 = _lib.bf16()                   # the mode the backward replays
         sub_emb = None
         if plan.has_sub_emb:                     # [B, E] rows of the (scaled) subject embedding, appended by the caller
             sub_emb, params = params[-1], params[:-1]
@@ -1510,6 +1526,7 @@ class _EncoderFn(torch.autograd.Function):
 
     @staticmethod
     @torch.autograd.function.once_differentiable
+    @replays_bf16
     def backward(ctx, dest):
         plan: EncoderPlan = ctx.plan
         s = ctx.saved
@@ -1635,6 +1652,7 @@ class _ClipScoresFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, estimate, candidate, want_probs: bool):
+        ctx.bf16 = _lib.bf16()                   # the mode the backward replays
         _check_clip_operands(estimate, candidate)
         est, cand = estimate.contiguous(), candidate.contiguous()
         Bn, Bc = est.shape[0], cand.shape[0]
@@ -1652,6 +1670,7 @@ class _ClipScoresFn(torch.autograd.Function):
 
     @staticmethod
     @torch.autograd.function.once_differentiable
+    @replays_bf16
     def backward(ctx, gout):
         est, cand, inv, scores, probs = ctx.saved_tensors
         Bn, Bc, KT, est_shape, cand_shape = ctx.meta
@@ -1704,6 +1723,7 @@ def clip_scores_prenormed(estimates: torch.Tensor, candidates: torch.Tensor, inv
 class _ClipLossFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, estimate, candidate, target_offset: int):
+        ctx.bf16 = _lib.bf16()                   # the mode the backward replays
         _check_clip_operands(estimate, candidate)
         est = estimate.contiguous()
         cand = candidate.contiguous()
@@ -1726,6 +1746,7 @@ class _ClipLossFn(torch.autograd.Function):
 
     @staticmethod
     @torch.autograd.function.once_differentiable
+    @replays_bf16
     def backward(ctx, gout):
         probs, inv, cand = ctx.saved_tensors[:3]
         Bn, Bc, KT, off, shape, cand_shape = ctx.meta

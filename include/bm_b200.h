@@ -555,6 +555,62 @@ int bm_clip_scores_bwd_tf32(const float* dscores, const float* scores, const flo
                             const float* cand, int Bn, int Bc, long long KT, float* G, float* coef, float* dest,
                             float* dcand, int* status, bm_stream_t stream);
 
+
+/* ---- bf16 forms (torch.autocast(dtype=torch.bfloat16) in the drop-in modules) -----------------------------------------
+ * Every `_bf16` entry point takes its default form's arguments and computes its contraction with bf16 operands and fp32
+ * accumulation: each fp32 operand element is rounded once to bf16 (round to nearest even: cvt.rn.bf16x2.f32; a weight
+ * that arrives as the two tf32 pieces of bm_tc_weight_split is rounded as hi + lo), the products of bf16 values are exact
+ * in fp32, and they are accumulated in fp32 exactly as in the default form (a fresh register tile per 32-wide K block,
+ * added into the running sum with round-to-nearest adds), so the result is within ~1e-5 relative of an fp64 contraction of
+ * the rounded operands however long K is, and the fixed reduction order of the `_det` forms is kept.  Inputs, outputs and
+ * workspaces stay fp32: no new storage format.  Everything outside the contraction is unchanged, as for the TF32 forms:
+ * epilogues, the CLIP candidate norms, softmax and the FP32-FMA kernels of the shapes outside the tensor-core gates.  The
+ * forms that take w_hi / w_lo accept w_lo == NULL (w_hi then holds the raw fp32 weights).  bm_clip_scores_det_bf16 /
+ * bm_clip_loss_fwd_det_bf16 combine both forms: repeated calls are bitwise identical.  The fp16-piece entry points
+ * (`*_f16`) have no bf16 form.
+ * The drop-in modules take these forms exactly when torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda")
+ * == torch.bfloat16 hold at the forward of the autograd node that issues the call; its backward uses the mode its forward
+ * recorded.  An fp16 autocast or a nested autocast(enabled=False) leaves every call as without autocast, and bf16 takes
+ * precedence over PyTorch's TF32 matmul flag. */
+int bm_tc_conv1d_bf16(const float* x, const float* w_hi, const float* w_lo, const float* bias, const float* addend,
+                      int B, int T, int Cin, int Ntot, int Kw, int dilation, int sign, int glu, int act, int out_tmajor,
+                      float* y, float* aux, float* glu_out, double* stats, int* status, bm_stream_t stream);
+int bm_tc_conv1d_persistent_bf16(const float* x, const float* w_raw, const float* bias, int accumulate, int B, int T,
+                                 int Cin, int Ntot, int Kw, int dilation, int sign, int glu, int act, int out_tmajor,
+                                 float* y, float* aux, float* glu_out, double* stats, int* status, bm_stream_t stream);
+int bm_tc_pointwise_sel_bf16(const float* x, const float* w_hi, const float* w_lo, const int* wsel, int n_sets, int B,
+                             int T, int Cin, int Ntot, float* y, int* status, bm_stream_t stream);
+int bm_tc_sensor_mix_bwd_data_bf16(const float* du, const float* w_hi, const float* w_lo, const int* wsel, int n_sets,
+                                   const float* mask, int B, int T, int Op, int Cp, int C, float* dmeg, int* status,
+                                   bm_stream_t stream);
+int bm_tc_wgrad_bf16(const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw, int dilation,
+                     float* workspace, float* dw, float* dbias, int* status, bm_stream_t stream);
+int bm_tc_wgrad_conv_bf16(const float* dy, const float* x, int B, int T, int M, int N, int Ntrue, int Kw, int dilation,
+                          float* workspace, float* dw, int* status, bm_stream_t stream);
+int bm_tc_wgrad_grouped_bf16(const float* dy, const float* x, const int* order, const int* seg_off, int G, int B, int T,
+                             int M, int N, float* out, int* status, bm_stream_t stream);
+int bm_clip_scores_bf16(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
+                        float* inv_norm, float* scores, float* probs, float* workspace, long long workspace_floats,
+                        int* status, bm_stream_t stream);
+int bm_clip_scores_det_bf16(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
+                            float* inv_norm, float* scores, float* probs, float* workspace, long long workspace_floats,
+                            int* status, bm_stream_t stream);
+int bm_clip_loss_fwd_bf16(const float* est, const float* cand, int Bn, int Bc, long long KT, int target_offset,
+                          float* inv_norm, float* scores, float* probs, float* row_loss, float* loss, float* workspace,
+                          long long workspace_floats, int* status, bm_stream_t stream);
+int bm_clip_loss_fwd_det_bf16(const float* est, const float* cand, int Bn, int Bc, long long KT, int target_offset,
+                              float* inv_norm, float* scores, float* probs, float* row_loss, float* loss,
+                              float* workspace, long long workspace_floats, int* status, bm_stream_t stream);
+int bm_clip_loss_bwd_bf16(const float* probs, const float* inv_norm, const float* cand, const float* gout, int Bn,
+                          int Bc, long long KT, int target_offset, float* G, float* dest, int* status,
+                          bm_stream_t stream);
+int bm_clip_loss_bwd_cand_bf16(const float* probs, const float* scores, const float* inv_norm, const float* est,
+                               const float* cand, const float* gout, int Bn, int Bc, long long KT, int target_offset,
+                               float* G, float* coef, float* dcand, int* status, bm_stream_t stream);
+int bm_clip_scores_bwd_bf16(const float* dscores, const float* scores, const float* inv_norm, const float* est,
+                            const float* cand, int Bn, int Bc, long long KT, float* G, float* coef, float* dest,
+                            float* dcand, int* status, bm_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
