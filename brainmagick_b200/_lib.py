@@ -70,6 +70,9 @@ SIGNATURES = {
     "bm_channel_join": [I, I, I, I] + [P, I, I, I, I] * 4 + [P, P],
     "bm_channel_split": [P, I, I, I, I] + [P, I, I, I, I] * 4 + [P],
     "bm_check_all_true": [P, L, I, P, P],
+    "bm_masked_loss_workspace": [I, I, I],         # returns long long floats, like the `_det_workspace` queries
+    "bm_masked_loss_fwd": [I, P, L, L, P, L, L, P, L, L, L, I, I, I, P, L, P, P, P],
+    "bm_masked_loss_bwd": [I, P, P, P, L, L, P, L, L, P, L, L, L, I, I, I, P, P, P],
     "bm_tc_wgrad_supported": [I, I],
     "bm_tc_wgrad": [P, P, I, I, I, I, I, I, I, P, P, P, P, P],
     "bm_tc_wgrad_conv_supported": [I, I, I, I],
@@ -168,7 +171,7 @@ def load():
     lib.bm_clip_workspace.argtypes = [I, I, L]
     for name, argtypes in SIGNATURES.items():
         fn = getattr(lib, name)          # AttributeError if the symbol is not exported
-        fn.restype = c_longlong if name.endswith("_det_workspace") else c_int
+        fn.restype = c_longlong if name.endswith("_workspace") else c_int
         fn.argtypes = argtypes
     _lib = lib
     return lib

@@ -13,6 +13,7 @@
 #include "prep.cuh"
 #include "convseq.cuh"
 #include "channel_join.cuh"
+#include "masked_loss.cuh"
 
 namespace bm {
 thread_local char g_last_error[512] = "";
@@ -1591,6 +1592,47 @@ extern "C" int bm_check_all_true(const unsigned char* mask, long long n, int cod
     if (n == 0) return 0;
     const bool vec = aligned16(mask);
     check_all_true_kernel<<<ew_grid(vec ? (n + 15) / 16 : n), 256, 0, ST(stream)>>>(mask, n, vec, code, status);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
+// masked L1 / L2 loss (bm/losses.py:11-26): fixed-grid fp64 partials, a one-CTA finalize, an elementwise backward
+extern "C" long long bm_masked_loss_workspace(int B, int C, int T) {
+    return (B < 0 || C < 0 || T < 0) ? 0 : 4ll * ml_blocks((long long)B * C);      // (sum, count) fp64 per CTA
+}
+extern "C" int bm_masked_loss_fwd(int kind, const float* est, long long est_sb, long long est_sc, const float* out,
+                                  long long out_sb, long long out_sc, const unsigned char* mask, long long mask_sb,
+                                  long long mask_sc, long long mask_st, int B, int C, int T, float* workspace,
+                                  long long workspace_floats, float* loss, float* inv_n, bm_stream_t stream) {
+    BM_CHECK_ARG((kind == ML_L1 || kind == ML_L2) && B >= 0 && C >= 0 && T >= 0 && loss && inv_n);
+    BM_CHECK_ARG(((long long)B * C * T == 0) || (est && out && mask));
+    BM_CHECK_WS(bm_masked_loss_workspace(B, C, T));
+    const long long rows = (long long)B * C * (T > 0);
+    const MlOperands p{est, est_sb, est_sc, out, out_sb, out_sc, mask, mask_sb, mask_sc, mask_st, C, T};
+    const int nb = ml_blocks(rows);
+    double* part = reinterpret_cast<double*>(workspace);
+    if (kind == ML_L1) masked_loss_partials_kernel<ML_L1><<<nb, ML_THREADS, 0, ST(stream)>>>(p, rows, part);
+    else masked_loss_partials_kernel<ML_L2><<<nb, ML_THREADS, 0, ST(stream)>>>(p, rows, part);
+    BM_CHECK_LAUNCH();
+    masked_loss_finalize_kernel<<<1, ML_FINAL_THREADS, 0, ST(stream)>>>(part, nb, loss, inv_n);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+extern "C" int bm_masked_loss_bwd(int kind, const float* gout, const float* inv_n, const float* est, long long est_sb,
+                                  long long est_sc, const float* out, long long out_sb, long long out_sc,
+                                  const unsigned char* mask, long long mask_sb, long long mask_sc, long long mask_st, int B,
+                                  int C, int T, float* d_est, float* d_out, bm_stream_t stream) {
+    BM_CHECK_ARG((kind == ML_L1 || kind == ML_L2) && B >= 0 && C >= 0 && T >= 0 && gout && inv_n);
+    const long long rows = (long long)B * C;
+    if (rows * T == 0 || (!d_est && !d_out)) return 0;
+    BM_CHECK_ARG(est && out && mask);
+    const MlOperands p{est, est_sb, est_sc, out, out_sb, out_sc, mask, mask_sb, mask_sc, mask_st, C, T};
+    const bool vec_out = T % 4 == 0 && aligned16(d_est, d_out);
+    const int grid = ew_grid(rows * ((T + 3) / 4), ML_THREADS);
+    if (kind == ML_L1)
+        masked_loss_bwd_kernel<ML_L1><<<grid, ML_THREADS, 0, ST(stream)>>>(p, rows, gout, inv_n, d_est, d_out, vec_out);
+    else
+        masked_loss_bwd_kernel<ML_L2><<<grid, ML_THREADS, 0, ST(stream)>>>(p, rows, gout, inv_n, d_est, d_out, vec_out);
     BM_CHECK_LAUNCH();
     return 0;
 }

@@ -1773,6 +1773,86 @@ def clip_loss(estimate, candidate, target_offset: int = 0):
 
 
 # ----------------------------------------------------------------------------------------------------
+# L1Loss / L2Loss (bm/losses.py:11-26): torch's L1Loss / MSELoss over estimate[mask.expand_as(estimate)] and the same
+# entries of output, without the boolean indexing: the kernels read the mask through its broadcast strides, so the True
+# count never reaches the host, and the operands are read in place (the encode task's estimate[..., limit:] included).
+# ----------------------------------------------------------------------------------------------------
+MASKED_L1, MASKED_L2 = 0, 1      # `kind` of bm_masked_loss_fwd / _bwd
+
+
+def _require_cuda_operands(*ts) -> None:
+    if not all(t.is_cuda for t in ts):
+        raise RuntimeError("brainmagick_b200 L1Loss / L2Loss run on CUDA (sm_90a) only; there is no CPU fallback: got "
+                           f"{', '.join(str(t.device) for t in ts)}")
+
+
+def _bct(t: torch.Tensor, unit_t: bool = True) -> torch.Tensor:
+    """t as a [B, C, T] view (leading dimensions of size 1 added); `unit_t`: with t-stride 1, a copy only when the last
+    dimension is not unit-stride (the mask keeps its broadcast strides)"""
+    if t.dim() > 3:
+        raise ValueError(f"brainmagick_b200 L1Loss / L2Loss take [B, C, T] operands, got {t.dim()} dimensions")
+    while t.dim() < 3:
+        t = t.unsqueeze(0)
+    if unit_t and t.shape[2] > 1 and t.stride(2) != 1:
+        t = t.contiguous()
+    return t
+
+
+def _strides(t: torch.Tensor):
+    return [int(s) for s in t.stride()]
+
+
+class _MaskedLossFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, kind: int, estimate, output, mask):
+        est, out, m = _bct(estimate), _bct(output), _bct(mask, unit_t=False)
+        B, C, T = est.shape
+        loss, inv_n = _empty((1,), est), _empty((1,), est)
+        ws = _empty((max(int(_lib.load().bm_masked_loss_workspace(B, C, T)), 2),), est)
+        call("bm_masked_loss_fwd", kind, _view_ptr(est), *_strides(est)[:2], _view_ptr(out), *_strides(out)[:2],
+             _view_ptr(m), *_strides(m), B, C, T, ptr(ws), ws.numel(), ptr(loss), ptr(inv_n), stream())
+        ctx.save_for_backward(est, out, m, inv_n)
+        ctx.kind, ctx.shape = kind, estimate.shape
+        return loss.reshape(())
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gout):
+        est, out, m, inv_n = ctx.saved_tensors
+        B, C, T = est.shape
+        want_est, want_out = ctx.needs_input_grad[1:3]
+        d_est = _empty((B, C, T), est) if want_est else None
+        d_out = _empty((B, C, T), est) if want_out else None
+        if want_est or want_out:
+            g = gout.reshape(1).contiguous().float()
+            call("bm_masked_loss_bwd", ctx.kind, ptr(g), ptr(inv_n), _view_ptr(est), *_strides(est)[:2], _view_ptr(out),
+                 *_strides(out)[:2], _view_ptr(m), *_strides(m), B, C, T, ptr(d_est), ptr(d_out), stream())
+        return (None, None if d_est is None else d_est.view(ctx.shape),
+                None if d_out is None else d_out.view(ctx.shape), None)
+
+
+def masked_loss(kind: int, estimate: torch.Tensor, output: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
+    """L1Loss (kind MASKED_L1) / L2Loss (MASKED_L2).forward: the mean of |e - o| or (e - o)^2 over the entries where
+    `mask` (bool, broadcast to estimate's shape) is True; NaN when there is none.  fp32 CUDA operands."""
+    if mask is None:
+        raise TypeError("L1Loss / L2Loss need a bool mask that broadcasts to the estimate (bm/losses.py:13 expands it); "
+                        "got None")
+    _require_cuda_operands(estimate, output, mask)
+    if estimate.dtype != torch.float32 or output.dtype != torch.float32:
+        raise TypeError(f"L1Loss / L2Loss kernels are fp32 (the reference trains in fp32): got {estimate.dtype} / "
+                        f"{output.dtype}")
+    if mask.dtype != torch.bool:
+        raise TypeError(f"L1Loss / L2Loss take a bool mask, got {mask.dtype}")
+    if not (estimate.device == output.device == mask.device):
+        raise RuntimeError(f"estimate on {estimate.device}, output on {output.device}, mask on {mask.device}")
+    mask = mask.expand_as(estimate)          # RuntimeError when it does not broadcast, as in the reference
+    if output.shape != estimate.shape:       # the reference's output[mask] raises IndexError
+        raise IndexError(f"The shape of the mask {list(mask.shape)} does not match the shape of the indexed tensor "
+                         f"{list(output.shape)}")
+    return _MaskedLossFn.apply(kind, estimate, output, mask)
+
+
+# ----------------------------------------------------------------------------------------------------
 # Stand-alone ChannelMerger.forward / SubjectLayers.forward (bm/models/common.py:334-362, 55-58): inside SimpleConv both are
 # fused into the encoder; called on their own (analysis notebooks, user code) they run the same stage kernels.  Channel-major
 # tensors in and out, like the reference; gradients flow to the parameters and to the input (`meg` / `x`).

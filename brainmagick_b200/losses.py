@@ -1,4 +1,8 @@
-"""Drop-in `ClipLoss` (reference: bm/losses.py:29-114): same constructor, `forward(estimate, candidate, mask)`,
+"""Drop-in `L1Loss` / `L2Loss` (reference: bm/losses.py:11-26): no constructor arguments, `forward(estimate, output, mask)`,
+the mean absolute / squared error over the entries where the broadcast mask is True, in CUDA through the C ABI
+(`functional.masked_loss`) with no host read, so a step that uses them can be captured in a CUDA graph.
+
+Drop-in `ClipLoss` (reference: bm/losses.py:29-114): same constructor, `forward(estimate, candidate, mask)`,
 `get_scores`, `get_probabilities`, `trim_samples`.  Scores, softmax / cross-entropy and their gradients run in
 CUDA through the C ABI (`functional.clip_loss`, `functional.clip_scores`, and `functional.clip_scores_grad` when the
 scores are differentiated, e.g. for gradient-based attribution).
@@ -22,6 +26,23 @@ from . import distrib
 
 def _wants_grad(estimates, candidates) -> bool:
     return torch.is_grad_enabled() and (estimates.requires_grad or candidates.requires_grad)
+
+
+class _MaskedLoss(torch.nn.Module):
+    _kind: int
+
+    def forward(self, estimate, output, mask=None):
+        return BF.masked_loss(self._kind, estimate, output, mask)
+
+
+class L1Loss(_MaskedLoss):
+    """torch.nn.L1Loss() over estimate[mask.expand_as(estimate)] and output[...] (bm/losses.py:17-20)"""
+    _kind = BF.MASKED_L1
+
+
+class L2Loss(_MaskedLoss):
+    """torch.nn.MSELoss() over estimate[mask.expand_as(estimate)] and output[...] (bm/losses.py:23-26)"""
+    _kind = BF.MASKED_L2
 
 
 class ClipLoss(torch.nn.Module):

@@ -425,6 +425,28 @@ int bm_channel_split(const float* src, int B, int T, int Cp, int n, float* dst0,
  * is 0.  Nothing is written otherwise; n = 0 enqueues nothing.  The caller raises at its next read of the status word. */
 int bm_check_all_true(const unsigned char* mask, long long n, int code, int* status, bm_stream_t stream);
 
+/* ---- Masked regression losses L1Loss / L2Loss (bm/losses.py:11-26) ---------------------------------------------------
+ * kind 0 (L1): loss = mean |est - out|, kind 1 (L2): loss = mean (est - out)^2, both over the N entries (b, c, t) where
+ * mask[b, c, t] != 0 -- torch.nn.L1Loss() / MSELoss() of est[mask] and out[mask].
+ * est and out are [B, C, T] fp32 with t-stride 1 and (b, c) strides est_sb / est_sc and out_sb / out_sc in elements, at any
+ * element offset (a view cropped in time is read in place); mask is one byte per entry read at
+ * mask[b*mask_sb + c*mask_sc + t*mask_st] (stride 0 along a broadcast dimension).
+ * bm_masked_loss_fwd: loss [1] and inv_n [1] = 1 / N on the device; N = 0 gives loss NaN (the mean of nothing).  The sum is
+ * taken in fp64 in a fixed order on a grid set by the shape and the SM count: bitwise repeatable, no atomics.  workspace:
+ * bm_masked_loss_workspace(B, C, T) floats of caller-owned scratch, 8-byte aligned.
+ * bm_masked_loss_bwd: gout [1] the loss's upstream gradient and inv_n [1] from the forward, both read on the device ->
+ * d_est = sign(est - out) gout inv_n (L1; sign(0) = 0) or 2 (est - out) gout inv_n (L2) where the mask is set, 0 elsewhere,
+ * and d_out = -d_est, each a contiguous [B, C, T] buffer or NULL (not computed). */
+long long bm_masked_loss_workspace(int B, int C, int T);
+int bm_masked_loss_fwd(int kind, const float* est, long long est_sb, long long est_sc, const float* out, long long out_sb,
+                       long long out_sc, const unsigned char* mask, long long mask_sb, long long mask_sc, long long mask_st,
+                       int B, int C, int T, float* workspace, long long workspace_floats, float* loss, float* inv_n,
+                       bm_stream_t stream);
+int bm_masked_loss_bwd(int kind, const float* gout, const float* inv_n, const float* est, long long est_sb, long long est_sc,
+                       const float* out, long long out_sb, long long out_sc, const unsigned char* mask, long long mask_sb,
+                       long long mask_sc, long long mask_st, int B, int C, int T, float* d_est, float* d_out,
+                       bm_stream_t stream);
+
 /* ---- Deterministic forms (torch.use_deterministic_algorithms(True) in the drop-in modules) -------------------------
  * Every `_det` entry point computes what its default form computes, with the same arguments plus (where noted) a
  * caller-owned workspace of bm_<op>_det_workspace(dims) floats, 8-byte aligned, checked against `workspace_floats`.  Its
