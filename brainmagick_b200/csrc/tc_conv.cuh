@@ -441,17 +441,22 @@ __global__ void weight_split_kernel(const float* __restrict__ W, float* __restri
 
 // The fp16 pieces of bm_tc_conv1d_f16's weights: w*s = hi + lo (11 + 11 significant bits) with s = f16_scale_of(amax).
 // largest |x| of a tensor into `cell` (a float whose bits compare like an unsigned integer because it is non-negative);
-// NaNs are ignored by fmaxf, +-inf gives inf (=> scale 1: the conv then propagates the non-finite values like fp32 would)
+// NaNs are ignored by fmaxf, +-inf gives inf (=> scale 1: the conv then propagates the non-finite values like fp32 would).
+// x need only be float-aligned (the generic epilogue and GLU forms run on misaligned views): the `head` elements before its
+// first 16-byte boundary and the tail after the last whole float4 are read one by one.
 __global__ void __launch_bounds__(256) amax_kernel(const float* __restrict__ x, long long n, unsigned int* __restrict__ cell) {
     float m = 0.f;
-    const long long n4 = n >> 2;
-    const float4* x4 = reinterpret_cast<const float4*>(x);
+    const long long head = min(n, (long long)(((16 - (reinterpret_cast<uintptr_t>(x) & 15)) & 15) >> 2));
+    const long long n4 = (n - head) >> 2;
+    const float4* x4 = reinterpret_cast<const float4*>(x + head);
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
         const float4 v = __ldg(x4 + i);
         m = fmaxf(fmaxf(m, fmaxf(fabsf(v.x), fabsf(v.y))), fmaxf(fabsf(v.z), fabsf(v.w)));
     }
-    if (blockIdx.x == 0)
-        for (long long i = (n4 << 2) + threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(x[i]));
+    if (blockIdx.x == 0) {
+        for (long long i = threadIdx.x; i < head; i += blockDim.x) m = fmaxf(m, fabsf(x[i]));
+        for (long long i = head + (n4 << 2) + threadIdx.x; i < n; i += blockDim.x) m = fmaxf(m, fabsf(x[i]));
+    }
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
     __shared__ float wm[8];
