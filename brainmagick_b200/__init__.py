@@ -1,8 +1,9 @@
 """brainmagick_b200: H100-native (sm_90a) drop-in for brainmagick's contrastive training step --
 `SimpleConv` (bm/models/simpleconv.py) and `ClipLoss` (bm/losses.py) behind the reference's module surface, with the
-masked regression losses `L1Loss` / `L2Loss` of encoding models and the regression baseline -- and for the
-callers either side of it: batch preparation (`norm`: bm/norm.py), the DeepMel feature model (`features`:
-bm/models/features.py) and the retrieval evaluation (`retrieval`: scripts/run_eval_probs.py, bm/wer.py)."""
+masked regression losses `L1Loss` / `L2Loss` of encoding models and the regression baseline and the decoding loss
+`FeatureDecodingLoss` -- and for the callers either side of it: batch preparation (`norm`: bm/norm.py), the DeepMel
+feature model (`features`: bm/models/features.py) and the retrieval evaluation (`retrieval`: scripts/run_eval_probs.py,
+bm/wer.py)."""
 import os as _os
 
 import torch as _torch
@@ -15,10 +16,10 @@ if "CUDA_DEVICE_MAX_CONNECTIONS" not in _os.environ and not _torch.cuda.is_initi
     _os.environ["CUDA_DEVICE_MAX_CONNECTIONS"] = "32"
 
 from .simpleconv import SimpleConv  # noqa: F401,E402
-from .losses import ClipLoss, L1Loss, L2Loss  # noqa: F401,E402
+from .losses import ClipLoss, FeatureDecodingLoss, L1Loss, L2Loss  # noqa: F401,E402
 from .common import ChannelMerger, ConvSequence, FourierEmb, PositionGetter, StaticBatch, SubjectLayers  # noqa: F401
 from .features import DeepMel  # noqa: F401
 from .norm import BatchScaler, ScaleReject  # noqa: F401
 
-__all__ = ["SimpleConv", "ClipLoss", "L1Loss", "L2Loss", "ChannelMerger", "ConvSequence", "FourierEmb", "PositionGetter",
-           "StaticBatch", "SubjectLayers", "DeepMel", "BatchScaler", "ScaleReject"]
+__all__ = ["SimpleConv", "ClipLoss", "L1Loss", "L2Loss", "FeatureDecodingLoss", "ChannelMerger", "ConvSequence",
+           "FourierEmb", "PositionGetter", "StaticBatch", "SubjectLayers", "DeepMel", "BatchScaler", "ScaleReject"]

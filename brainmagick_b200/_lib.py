@@ -73,6 +73,9 @@ SIGNATURES = {
     "bm_masked_loss_workspace": [I, I, I],         # returns long long floats, like the `_det_workspace` queries
     "bm_masked_loss_fwd": [I, P, L, L, P, L, L, P, L, L, L, I, I, I, P, L, P, P, P],
     "bm_masked_loss_bwd": [I, P, P, P, L, L, P, L, L, P, L, L, L, I, I, I, P, P, P],
+    "bm_decoding_loss_workspace": [I, I, I],
+    "bm_decoding_loss_fwd": [P, L, L, P, L, L, P, L, L, L, I, I, P, I, P, P, P, L, P, P, P, P, P],
+    "bm_decoding_loss_bwd": [P, P, P, P, L, L, P, L, L, P, L, L, L, I, I, I, I, P, I, P, P, P, P],
     "bm_tc_wgrad_supported": [I, I],
     "bm_tc_wgrad": [P, P, I, I, I, I, I, I, I, P, P, P, P, P],
     "bm_tc_wgrad_conv_supported": [I, I, I, I],

@@ -14,6 +14,7 @@
 #include "convseq.cuh"
 #include "channel_join.cuh"
 #include "masked_loss.cuh"
+#include "decoding_loss.cuh"
 
 namespace bm {
 thread_local char g_last_error[512] = "";
@@ -1633,6 +1634,49 @@ extern "C" int bm_masked_loss_bwd(int kind, const float* gout, const float* inv_
         masked_loss_bwd_kernel<ML_L1><<<grid, ML_THREADS, 0, ST(stream)>>>(p, rows, gout, inv_n, d_est, d_out, vec_out);
     else
         masked_loss_bwd_kernel<ML_L2><<<grid, ML_THREADS, 0, ST(stream)>>>(p, rows, gout, inv_n, d_est, d_out, vec_out);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
+// FeatureDecodingLoss (bm/losses.py:117-173): fixed-grid fp64 partials per (CTA, feature), a one-CTA finalize, one
+// backward pass over every gradient row
+extern "C" long long bm_decoding_loss_workspace(int B, int T, int F) {
+    if (B < 0 || T < 0 || F < 1 || F > FD_MAX_FEATURES) return 0;
+    const long long nb = fd_blocks(B, T);
+    return 4 * nb * F + nb + (nb & 1);              // (sum, count) fp64 per (CTA, feature), then one flag word per CTA
+}
+extern "C" int bm_decoding_loss_fwd(const float* est, long long est_sb, long long est_sc, const float* out, long long out_sb,
+                                    long long out_sc, const unsigned char* mask, long long mask_sb, long long mask_sc,
+                                    long long mask_st, int B, int T, const int* table, int F, const float* weights,
+                                    float* lse, float* workspace, long long workspace_floats, float* loss, float* scale,
+                                    int* flag, int* status, bm_stream_t stream) {
+    BM_CHECK_ARG(B >= 0 && T >= 0 && F >= 1 && F <= FD_MAX_FEATURES && table && loss && scale && flag);
+    BM_CHECK_ARG(((long long)B * T == 0) || (est && out && mask && lse));
+    BM_CHECK_WS(bm_decoding_loss_workspace(B, T, F));
+    const int nb = fd_blocks(B, T);
+    const FdOperands p{est, est_sb, est_sc, out, out_sb, out_sc, mask, mask_sb, mask_sc, mask_st, table, weights, F, B, T};
+    double* part = reinterpret_cast<double*>(workspace);
+    int* cta_flags = reinterpret_cast<int*>(workspace + 4ll * nb * F);
+    decoding_loss_partials_kernel<<<nb, FD_THREADS, 0, ST(stream)>>>(p, part, cta_flags, lse);
+    BM_CHECK_LAUNCH();
+    decoding_loss_finalize_kernel<<<1, ML_FINAL_THREADS, 0, ST(stream)>>>(part, cta_flags, nb, table, F, loss, scale, flag,
+                                                                           status);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+extern "C" int bm_decoding_loss_bwd(const float* gout, const float* scale, const float* lse, const float* est,
+                                    long long est_sb, long long est_sc, const float* out, long long out_sb, long long out_sc,
+                                    const unsigned char* mask, long long mask_sb, long long mask_sc, long long mask_st, int B,
+                                    int T, int est_C, int out_C, const int* table, int F, const float* weights, float* d_est,
+                                    float* d_out, bm_stream_t stream) {
+    BM_CHECK_ARG(B >= 0 && T >= 0 && est_C >= 0 && out_C >= 0 && F >= 1 && F <= FD_MAX_FEATURES && gout && scale && table);
+    if ((long long)B * T == 0 || (!d_est && !d_out)) return 0;
+    BM_CHECK_ARG(est && out && mask && lse);
+    const FdOperands p{est, est_sb, est_sc, out, out_sb, out_sc, mask, mask_sb, mask_sc, mask_st, table, weights, F, B, T};
+    const bool vec_out = T % 4 == 0 && aligned16(d_est, d_out);
+    const long long rows = (long long)B * ((d_est ? est_C : 0) + (d_out ? out_C : 0));
+    decoding_loss_bwd_kernel<<<ew_grid(rows * ((T + 3) / 4), FD_THREADS), FD_THREADS, 0, ST(stream)>>>(
+        p, est_C, out_C, gout, scale, lse, d_est, d_out, vec_out);
     BM_CHECK_LAUNCH();
     return 0;
 }

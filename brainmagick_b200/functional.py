@@ -203,11 +203,14 @@ def tc_status_tensor(device) -> torch.Tensor:
 
 
 MASK_NOT_ALL_TRUE = 903   # status code of bm_check_all_true: a ClipLoss mask with a False entry (900-902: the kernels' own)
+# status codes of bm_decoding_loss_fwd (FeatureDecodingLoss): no mask entry set, a class target >= K, a bad negative target
+DECODING_NO_MASK, DECODING_TARGET_TOO_LARGE, DECODING_TARGET_NEGATIVE = 904, 905, 906
 
 
 def check_tc_status(device=None) -> None:
     """Synchronising check (tests, bench, end of epoch): raises if a kernel reported a bad subject index, a ClipLoss mask that
-    is not all true (checked on the device in a captured step), or a tensor-core pipeline timeout."""
+    is not all true or a FeatureDecodingLoss data error (both checked on the device in a captured step), or a tensor-core
+    pipeline timeout."""
     for dev, t in _status.items():
         if device is None or torch.device(device) == dev:
             code = int(t.item())
@@ -218,6 +221,9 @@ def check_tc_status(device=None) -> None:
             if code == MASK_NOT_ALL_TRUE:
                 t.zero_()
                 raise AssertionError(f"mask is not supported for now (a ClipLoss mask with a False entry on {dev})")
+            if code in (DECODING_NO_MASK, DECODING_TARGET_TOO_LARGE, DECODING_TARGET_NEGATIVE):
+                t.zero_()
+                raise _decoding_error(code, f"on {dev}")
             if code != 0:
                 raise _lib.BmB200Error(f"a tensor-core kernel reported a pipeline timeout (barrier code {code}) on {dev}")
 
@@ -1850,6 +1856,93 @@ def masked_loss(kind: int, estimate: torch.Tensor, output: torch.Tensor, mask: t
         raise IndexError(f"The shape of the mask {list(mask.shape)} does not match the shape of the indexed tensor "
                          f"{list(output.shape)}")
     return _MaskedLossFn.apply(kind, estimate, output, mask)
+
+
+# ----------------------------------------------------------------------------------------------------
+# FeatureDecodingLoss (bm/losses.py:117-173): per feature of the builder, F.mse_loss over the masked entries of a regression
+# feature's channels or torch's weighted cross-entropy over the masked (b, t) of a categorical one, summed in feature order.
+# One forward call (partials + finalize) and one backward call (every row of both gradients) whatever the features; the
+# mask is never indexed on the host and the operands are read in place.  The feature table and the class weights are the
+# module's (losses.FeatureDecodingLoss), built once per device.
+# ----------------------------------------------------------------------------------------------------
+DECODING_REGRESSION, DECODING_CATEGORICAL = 0, 1     # `kind` column of the bm_decoding_loss_* feature table
+DECODING_TABLE_WIDTH = 6                             # (kind, est_start, width, out_start, weight_offset, lse_slot)
+DECODING_MAX_FEATURES = 15                           # features of one loss: the flag word's bits
+
+
+def _decoding_error(code: int, where: str) -> Exception:
+    """The exception the reference raises for a bm_decoding_loss_fwd error code"""
+    if code == DECODING_NO_MASK:
+        return AssertionError(f"FeatureDecodingLoss: mask.any() is False, no entry is masked in ({where})")
+    if code == DECODING_TARGET_TOO_LARGE:
+        return AssertionError(f"FeatureDecodingLoss: output contains a category >= the feature's output_dim, or NaN ({where})")
+    return IndexError(f"FeatureDecodingLoss: Target out of bounds: a masked class target is negative and not the "
+                      f"ignore_index -100 ({where})")
+
+
+def _require_cuda_decoding(*ts) -> None:
+    if not all(t.is_cuda for t in ts):
+        raise RuntimeError("brainmagick_b200 FeatureDecodingLoss runs on CUDA (sm_90a) only; there is no CPU fallback: got "
+                           f"{', '.join(str(t.device) for t in ts)}")
+
+
+def _mask_strides(m: torch.Tensor):
+    """a [B, C, T] mask's strides, 0 along every dimension of size 1 (it broadcasts there)"""
+    return [int(s) if n > 1 else 0 for s, n in zip(m.stride(), m.shape)]
+
+
+class _DecodingLossFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, table, n_cat: int, weights, flag, estimate, output, mask):
+        est, out = _bct(estimate), _bct(output)
+        B, _, T = est.shape
+        F = table.shape[0]
+        lse = _empty((max(n_cat * B * T, 1),), est)
+        loss, scale = _empty((1,), est), _empty((F,), est)
+        ws = _empty((max(int(_lib.load().bm_decoding_loss_workspace(B, T, F)), 2),), est)
+        status = tc_status_tensor(est.device)        # created eagerly: a captured step only writes it
+        call("bm_decoding_loss_fwd", _view_ptr(est), *_strides(est)[:2], _view_ptr(out), *_strides(out)[:2], _view_ptr(mask),
+             *_mask_strides(mask), B, T, ptr(table), F, ptr(weights), ptr(lse), ptr(ws), ws.numel(), ptr(loss), ptr(scale),
+             ptr(flag), ptr(status) if capturing() else None, stream())
+        ctx.save_for_backward(est, out, mask, table, weights, lse, scale)
+        ctx.shapes = (estimate.shape, output.shape)
+        return loss.reshape(())
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gout):
+        est, out, mask, table, weights, lse, scale = ctx.saved_tensors
+        B, Ce, T = est.shape
+        Co = out.shape[1]
+        want_est, want_out = ctx.needs_input_grad[4:6]
+        d_est = _empty((B, Ce, T), est) if want_est else None
+        d_out = _empty((B, Co, T), est) if want_out else None
+        if want_est or want_out:
+            g = gout.reshape(1).contiguous().float()
+            call("bm_decoding_loss_bwd", ptr(g), ptr(scale), ptr(lse), _view_ptr(est), *_strides(est)[:2], _view_ptr(out),
+                 *_strides(out)[:2], _view_ptr(mask), *_mask_strides(mask), B, T, Ce, Co, ptr(table), table.shape[0],
+                 ptr(weights), ptr(d_est), ptr(d_out), stream())
+        return (None, None, None, None, None if d_est is None else d_est.view(ctx.shapes[0]),
+                None if d_out is None else d_out.view(ctx.shapes[1]), None)
+
+
+def decoding_loss(table: torch.Tensor, n_cat: int, weights: tp.Optional[torch.Tensor], estimate: torch.Tensor,
+                  output: torch.Tensor, mask: torch.Tensor) -> tp.Tuple[torch.Tensor, torch.Tensor]:
+    """FeatureDecodingLoss.forward on checked operands: `table` the int32 [F, DECODING_TABLE_WIDTH] feature table on the
+    operands' device, `n_cat` its categorical features, `weights` the fp32 class weights its weight offsets index (None:
+    unweighted), estimate [B, F_out, T] and output [B, F, T] fp32 with t-stride 1 where T > 1, mask bool [B, 1 or width, T]
+    (broadcast views allowed).  -> (loss, flag): flag the int32 [1] word bm_decoding_loss_fwd writes (0: no error), which the
+    caller reads in an eager step; a captured step gets the error code in the status word instead."""
+    _require_cuda_decoding(estimate, output, mask)
+    if estimate.dtype != torch.float32 or output.dtype != torch.float32:
+        raise TypeError(f"FeatureDecodingLoss kernels are fp32 (the reference trains in fp32): got {estimate.dtype} / "
+                        f"{output.dtype}")
+    if mask.dtype != torch.bool:
+        raise TypeError(f"FeatureDecodingLoss takes a bool mask, got {mask.dtype}")
+    if not (estimate.device == output.device == mask.device):
+        raise RuntimeError(f"estimate on {estimate.device}, output on {output.device}, mask on {mask.device}")
+    flag = _empty((1,), estimate, torch.int32)
+    return _DecodingLossFn.apply(table, n_cat, weights, flag, estimate, output, mask), flag
 
 
 # ----------------------------------------------------------------------------------------------------

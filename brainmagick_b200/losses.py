@@ -1,4 +1,8 @@
-"""Drop-in `L1Loss` / `L2Loss` (reference: bm/losses.py:11-26): no constructor arguments, `forward(estimate, output, mask)`,
+"""Drop-in `FeatureDecodingLoss` (reference: bm/losses.py:117-173): same constructor `(used_features, scaler)`,
+`forward(estimate, output, mask)`, the sum over the features of a masked MSE (regression features) or a class-weighted
+cross-entropy (categorical ones), in CUDA through the C ABI (`functional.decoding_loss`); see the class.
+
+Drop-in `L1Loss` / `L2Loss` (reference: bm/losses.py:11-26): no constructor arguments, `forward(estimate, output, mask)`,
 the mean absolute / squared error over the entries where the broadcast mask is True, in CUDA through the C ABI
 (`functional.masked_loss`) with no host read, so a step that uses them can be captured in a CUDA graph.
 
@@ -16,6 +20,7 @@ grad (a trainable feature model) the gather is differentiable (reduce-scatter of
 """
 from __future__ import annotations
 
+import typing as tp
 import weakref
 
 import torch
@@ -43,6 +48,131 @@ class L1Loss(_MaskedLoss):
 class L2Loss(_MaskedLoss):
     """torch.nn.MSELoss() over estimate[mask.expand_as(estimate)] and output[...] (bm/losses.py:23-26)"""
     _kind = BF.MASKED_L2
+
+
+class _DecodedFeature(tp.NamedTuple):
+    name: str
+    categorical: bool
+    est_start: int
+    est_width: int          # the feature's output_dimension (K for a categorical feature)
+    out_start: int
+    out_width: int          # the feature's dimension
+
+
+class FeatureDecodingLoss(torch.nn.Module):
+    """Drop-in `FeatureDecodingLoss(used_features, scaler)` (bm/losses.py:117-173), the solver's `regression_classification`
+    loss: per feature of `used_features`, in order, F.mse_loss over the masked entries of a regression feature or
+    F.cross_entropy over the masked (b, t) of a categorical one -- weighted by `scaler.get_categorical_feature_weights(name)`
+    when a scaler is given -- added up as `loss += ...`.
+
+    `used_features` is duck-typed like the reference's FeaturesBuilder (`values()` of features with `name`, `categorical`,
+    `dimension`, `output_dimension`; `get_slice(name, model_output)`, `dimension`, `output_dimension`) and `scaler` like
+    its BatchScaler or this package's (`get_categorical_feature_weights`, and `feature_scalers[name].categories_count_`).
+    The feature table is built once per device, the class weights once per device and again whenever a feature's
+    `categories_count_` is replaced or changed in place.  An eager step reads one flag word to raise the reference's errors;
+    a captured step reads nothing and reports them through `functional.check_tc_status()`."""
+
+    def __init__(self, used_features, scaler):
+        super().__init__()
+        self.used_features = used_features
+        self.scaler = scaler
+        self._plan: tp.Optional[tp.List[_DecodedFeature]] = None
+        self._tables: tp.Dict[torch.device, torch.Tensor] = {}
+        self._weights: tp.Dict[torch.device, tp.Tuple[tp.Tuple, torch.Tensor]] = {}
+
+    def _features(self) -> tp.List[_DecodedFeature]:
+        if self._plan is None:
+            plan = []
+            for feature in self.used_features.values():
+                est_sl = self.used_features.get_slice(feature.name, model_output=True)
+                out_sl = self.used_features.get_slice(feature.name)
+                plan.append(_DecodedFeature(feature.name, bool(feature.categorical), est_sl.start, est_sl.stop - est_sl.start,
+                                            out_sl.start, out_sl.stop - out_sl.start))
+            if not 1 <= len(plan) <= BF.DECODING_MAX_FEATURES:
+                raise NotImplementedError(f"FeatureDecodingLoss takes 1 to {BF.DECODING_MAX_FEATURES} features, got "
+                                          f"{len(plan)}")
+            self._plan = plan
+        return self._plan
+
+    def _table(self, device) -> torch.Tensor:
+        table = self._tables.get(device)
+        if table is None:
+            if BF.capturing():
+                raise RuntimeError("FeatureDecodingLoss copies its feature table to the device on the first call: run one "
+                                   "eager step on this device before capturing")
+            rows, woff, slot = [], 0, 0
+            for f in self._features():
+                if f.categorical:
+                    rows.append([BF.DECODING_CATEGORICAL, f.est_start, f.est_width, f.out_start,
+                                 woff if self.scaler is not None else -1, slot])
+                    woff, slot = woff + f.est_width, slot + 1
+                else:
+                    rows.append([BF.DECODING_REGRESSION, f.est_start, f.est_width, f.out_start, -1, -1])
+            table = self._tables[device] = torch.tensor(rows, dtype=torch.int32).to(device)
+        return table
+
+    def _count_token(self, name):
+        """what identifies the class counts the weights of feature `name` come from: the tensor and its version"""
+        counts = getattr(getattr(self.scaler, "feature_scalers", {}).get(name), "categories_count_", None)
+        return None if counts is None else (counts, counts._version)
+
+    def _class_weights(self, device) -> tp.Optional[torch.Tensor]:
+        if self.scaler is None:
+            return None
+        cats = [f for f in self._features() if f.categorical]
+        tokens = tuple(self._count_token(f.name) for f in cats)
+        cached = self._weights.get(device)
+        if cached is not None and all(a is b or (a is not None and b is not None and a[0] is b[0] and a[1] == b[1])
+                                      for a, b in zip(cached[0], tokens)):
+            return cached[1]
+        if BF.capturing():
+            raise RuntimeError("FeatureDecodingLoss copies the class weights to the device when they are first used or "
+                               "the scaler's category counts change: run one eager step before capturing")
+        parts = []
+        for f in cats:
+            w = self.scaler.get_categorical_feature_weights(f.name)
+            if w.dim() != 1 or w.numel() != f.est_width:     # F.cross_entropy's check
+                raise RuntimeError(f"weight tensor should be defined either for all {f.est_width} classes or no classes "
+                                   f"but got weight tensor of shape: {list(w.shape)}")
+            parts.append(w.detach().to(device=device, dtype=torch.float32))
+        weights = torch.cat(parts) if parts else torch.zeros(1, device=device)
+        self._weights[device] = (tokens, weights)
+        return weights
+
+    def forward(self, estimate, output, mask=None):
+        uf = self.used_features
+        assert estimate.shape[1] == uf.output_dimension and output.shape[1] == uf.dimension, \
+            "Invalid features dim received. Are you using the correct features for the loss?"
+        if mask is None:
+            raise TypeError("FeatureDecodingLoss needs a bool mask (bm/losses.py:141 expands it); got None")
+        if estimate.dim() != 3 or output.dim() != 3:
+            raise ValueError(f"FeatureDecodingLoss takes [B, C, T] operands, got {estimate.dim()} and {output.dim()} "
+                             "dimensions")
+        plan = self._features()
+        for f in plan:                                       # the reference's shape errors, in its order
+            feature_mask = mask.expand_as(estimate[:, f.est_start:f.est_start + f.est_width])    # RuntimeError
+            if f.categorical:
+                assert f.out_width == 1, "Supporting only single categorical cross entropy for now."
+                if mask.dim() != 3 or mask.shape[1] != 1 or \
+                        (mask.shape[0], mask.shape[2]) != (output.shape[0], output.shape[2]):
+                    raise IndexError(f"The shape of the mask {list(mask.transpose(-1, -2).shape)} does not match the "
+                                     f"shape of the indexed tensor {[output.shape[0], output.shape[2], 1]}")
+            elif output[:, f.out_start:f.out_start + f.out_width].shape != feature_mask.shape:
+                raise IndexError(f"The shape of the mask {list(feature_mask.shape)} does not match the shape of the "
+                                 f"indexed tensor {list(output[:, f.out_start:f.out_start + f.out_width].shape)}")
+        m = mask
+        while m.dim() < 3:
+            m = m.unsqueeze(0)
+        m = m.expand(estimate.shape[0], m.shape[1], estimate.shape[2])
+        device = estimate.device
+        loss, flag = BF.decoding_loss(self._table(device), sum(f.categorical for f in plan), self._class_weights(device),
+                                      estimate, output, m)
+        if not BF.capturing():
+            code = int(flag.item())                          # the one host read of an eager step
+            if code:
+                f = plan[code >> 16]
+                raise BF._decoding_error(code & 0xFFFF, f"feature {f.name!r}, output_dim {f.est_width}")
+        return loss
 
 
 class ClipLoss(torch.nn.Module):

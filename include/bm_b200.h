@@ -447,6 +447,36 @@ int bm_masked_loss_bwd(int kind, const float* gout, const float* inv_n, const fl
                        long long mask_sc, long long mask_st, int B, int C, int T, float* d_est, float* d_out,
                        bm_stream_t stream);
 
+/* ---- FeatureDecodingLoss (bm/losses.py:117-173) --------------------------------------------------------------------
+ * loss = the sum, in feature order, of one fp32 term per feature f = 0..F-1 of a device table of 6 ints per feature:
+ * (kind, est_start, width, out_start, weight_offset, lse_slot).
+ *   kind 0 (regression): mean (est - out)^2 over the masked entries of est channels [est_start, est_start + width) and out
+ *     channels [out_start, out_start + width), the mask's channel c - est_start (mask_sc 0: one channel for all).
+ *   kind 1 (categorical, K = width): torch's F.cross_entropy of the logits est[b, est_start + k, t], k < K, against the
+ *     target (long) out[b, out_start, t] over the (b, t) where mask[b, 0, t] != 0: sum w_y (lse - z_y) / sum w_y with
+ *     w = weights[weight_offset + y] (weight_offset -1: w = 1), ignore_index -100.  lse_slot s: the forward stores the
+ *     log-sum-exp of every (b, t) at lse[(s * B + b) * T + t].
+ * est and out are fp32 with t-stride 1 and (b, c) strides in elements, at any element offset; mask is one byte per entry
+ * read at mask[b*mask_sb + c*mask_sc + t*mask_st].  1 <= F <= 15.
+ * bm_decoding_loss_fwd: loss [1] and scale [F] (2 / N_f, or 1 / W_f) on the device; partials in fp64 in a fixed order on a
+ * grid set by the shape and the SM count: bitwise repeatable, no atomics.  flag [1] <- 0, or the reference's first error
+ * as code | (feature << 16): 904 no mask entry is set (assert mask.any()), 905 a categorical target >= K or NaN at any
+ * (b, t) (assert K > output[:, start].max()), 906 a masked target that is negative and not -100 (torch's "target out of
+ * bounds").  status (NULL: none) <- the code if it is still 0.  A bad target contributes nothing and indexes nothing.
+ * workspace: bm_decoding_loss_workspace(B, T, F) floats of caller-owned scratch, 8-byte aligned.
+ * bm_decoding_loss_bwd: gout [1], scale and lse from the forward -> d_est [B, est_C, T] (regression: 2 (est - out) gout /
+ * N_f; categorical: gout w_y / W_f (softmax - onehot(y)); 0 where the mask is 0, at ignored or bad targets and on channels
+ * no feature holds) and d_out [B, out_C, T] (regression: -d_est of the channel; 0 elsewhere), contiguous, or NULL. */
+long long bm_decoding_loss_workspace(int B, int T, int F);
+int bm_decoding_loss_fwd(const float* est, long long est_sb, long long est_sc, const float* out, long long out_sb,
+                         long long out_sc, const unsigned char* mask, long long mask_sb, long long mask_sc, long long mask_st,
+                         int B, int T, const int* table, int F, const float* weights, float* lse, float* workspace,
+                         long long workspace_floats, float* loss, float* scale, int* flag, int* status, bm_stream_t stream);
+int bm_decoding_loss_bwd(const float* gout, const float* scale, const float* lse, const float* est, long long est_sb,
+                         long long est_sc, const float* out, long long out_sb, long long out_sc, const unsigned char* mask,
+                         long long mask_sb, long long mask_sc, long long mask_st, int B, int T, int est_C, int out_C,
+                         const int* table, int F, const float* weights, float* d_est, float* d_out, bm_stream_t stream);
+
 /* ---- Deterministic forms (torch.use_deterministic_algorithms(True) in the drop-in modules) -------------------------
  * Every `_det` entry point computes what its default form computes, with the same arguments plus (where noted) a
  * caller-owned workspace of bm_<op>_det_workspace(dims) floats, 8-byte aligned, checked against `workspace_floats`.  Its
