@@ -2,8 +2,8 @@
 `SimpleConv` (bm/models/simpleconv.py) and `ClipLoss` (bm/losses.py) behind the reference's module surface, with the
 masked regression losses `L1Loss` / `L2Loss` of encoding models and the regression baseline and the decoding loss
 `FeatureDecodingLoss` -- and for the callers either side of it: batch preparation (`norm`: bm/norm.py), the DeepMel
-feature model (`features`: bm/models/features.py) and the retrieval evaluation (`retrieval`: scripts/run_eval_probs.py,
-bm/wer.py)."""
+feature model (`features`: bm/models/features.py), the retrieval evaluation (`retrieval`: scripts/run_eval_probs.py,
+bm/wer.py) and the test-stage metrics (`metrics`: bm/metrics.py)."""
 import os as _os
 
 import torch as _torch
@@ -20,6 +20,7 @@ from .losses import ClipLoss, FeatureDecodingLoss, L1Loss, L2Loss  # noqa: F401,
 from .common import ChannelMerger, ConvSequence, FourierEmb, PositionGetter, StaticBatch, SubjectLayers  # noqa: F401
 from .features import DeepMel  # noqa: F401
 from .norm import BatchScaler, ScaleReject  # noqa: F401
+from . import metrics  # noqa: F401,E402
 
 __all__ = ["SimpleConv", "ClipLoss", "L1Loss", "L2Loss", "FeatureDecodingLoss", "ChannelMerger", "ConvSequence",
            "FourierEmb", "PositionGetter", "StaticBatch", "SubjectLayers", "DeepMel", "BatchScaler", "ScaleReject"]

@@ -6,14 +6,14 @@ import contextlib
 import ctypes
 import os
 import threading
-from ctypes import c_float, c_int, c_longlong, c_void_p
+from ctypes import c_double, c_float, c_int, c_longlong, c_void_p
 
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libbm_b200.so")
 
-P, I, L, F = c_void_p, c_int, c_longlong, c_float
+P, I, L, F, D = c_void_p, c_int, c_longlong, c_float, c_double
 
 # name -> argtypes, in the order of include/bm_b200.h
 SIGNATURES = {
@@ -76,6 +76,9 @@ SIGNATURES = {
     "bm_decoding_loss_workspace": [I, I, I],
     "bm_decoding_loss_fwd": [P, L, L, P, L, L, P, L, L, L, I, I, P, I, P, P, P, L, P, P, P, P, P],
     "bm_decoding_loss_bwd": [P, P, P, P, L, L, P, L, L, P, L, L, L, I, I, I, I, P, I, P, P, P, P],
+    "bm_metric_workspace": [I, I, I],
+    "bm_metric_update": [I, I, P, L, L, L, P, L, L, L, P, L, L, L, I, I, I, I, I, P, P, I, P, L, P],
+    "bm_metric_finalize": [I, P, I, I, D, P, I, P, P],
     "bm_tc_wgrad_supported": [I, I],
     "bm_tc_wgrad": [P, P, I, I, I, I, I, I, I, P, P, P, P, P],
     "bm_tc_wgrad_conv_supported": [I, I, I, I],

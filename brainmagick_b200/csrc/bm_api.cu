@@ -15,6 +15,7 @@
 #include "channel_join.cuh"
 #include "masked_loss.cuh"
 #include "decoding_loss.cuh"
+#include "metrics.cuh"
 
 namespace bm {
 thread_local char g_last_error[512] = "";
@@ -1679,6 +1680,74 @@ extern "C" int bm_decoding_loss_bwd(const float* gout, const float* scale, const
         p, est_C, out_C, gout, scale, lse, d_est, d_out, vec_out);
     BM_CHECK_LAUNCH();
     return 0;
+}
+
+// Test metrics (bm/metrics.py): per-column fp64 sums over dim 0 into device accumulators, and one finalize per get()
+namespace {
+template <typename S>
+int metric_update_launch(int kind, const MtOperands& p, int splits, double* acc, int* seen, int parity, double* part,
+                         cudaStream_t st) {
+    const long long cols = (long long)p.C * p.T;
+    const dim3 grid((unsigned)((cols + MT_THREADS - 1) / MT_THREADS), (unsigned)splits);
+    switch (kind) {
+        case MT_CORRELATION: metric_update_kernel<S, MT_CORRELATION><<<grid, MT_THREADS, 0, st>>>(p, splits, acc, seen, parity, part); break;
+        case MT_L1: metric_update_kernel<S, MT_L1><<<grid, MT_THREADS, 0, st>>>(p, splits, acc, seen, parity, part); break;
+        case MT_L2: metric_update_kernel<S, MT_L2><<<grid, MT_THREADS, 0, st>>>(p, splits, acc, seen, parity, part); break;
+        default: metric_update_kernel<S, MT_ACCURACY><<<grid, MT_THREADS, 0, st>>>(p, splits, acc, seen, parity, part); break;
+    }
+    BM_CHECK_LAUNCH();
+    if (splits > 1) {
+        if (kind == MT_CORRELATION)
+            metric_combine_kernel<6><<<grid.x, MT_THREADS, 0, st>>>(part, splits, cols, acc, seen, parity);
+        else
+            metric_combine_kernel<2><<<grid.x, MT_THREADS, 0, st>>>(part, splits, cols, acc, seen, parity);
+        BM_CHECK_LAUNCH();
+    }
+    return 0;
+}
+template <typename O>
+int metric_finalize_launch(int kind, const double* acc, long long cols, double tol, void* out, int* flag, cudaStream_t st) {
+    if (kind == MT_CORRELATION)
+        metric_finalize_kernel<O, MT_CORRELATION><<<1, MT_FINAL_THREADS, 0, st>>>(acc, cols, tol, static_cast<O*>(out), flag);
+    else
+        metric_finalize_kernel<O, MT_L1><<<1, MT_FINAL_THREADS, 0, st>>>(acc, cols, tol, static_cast<O*>(out), flag);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+}  // namespace
+
+extern "C" long long bm_metric_workspace(int N, int C, int T) {
+    if (N < 0 || C < 0 || T < 0) return 0;
+    const long long cols = (long long)C * T;
+    const int s = mt_splits(N, cols);
+    return s > 1 ? 2ll * MT_MAX_PLANES * s * cols : 0;      // fp64 partials: NP planes per split
+}
+extern "C" int bm_metric_update(int kind, int dtype, const void* left, long long left_sn, long long left_sc,
+                                long long left_st, const void* right, long long right_sn, long long right_sc,
+                                long long right_st, const unsigned char* mask, long long mask_sn, long long mask_sc,
+                                long long mask_st, int mask_n, int N, int C, int T, int K, double* acc, int* seen,
+                                int parity, float* workspace, long long workspace_floats, bm_stream_t stream) {
+    BM_CHECK_ARG(kind >= MT_CORRELATION && kind <= MT_ACCURACY && (dtype == 0 || dtype == 1));
+    BM_CHECK_ARG(N >= 0 && C >= 0 && T >= 0 && (mask_n == 1 || mask_n == N) && (parity == 0 || parity == 1));
+    BM_CHECK_ARG(kind != MT_ACCURACY || (C == 1 && K >= 1));
+    const long long cols = (long long)C * T;
+    if (cols == 0) return 0;                                // an empty slice or time crop: nothing to add
+    BM_CHECK_ARG(acc && seen && left && right && mask);
+    const int splits = mt_splits(N, cols);
+    if (splits > 1) BM_CHECK_WS(bm_metric_workspace(N, C, T));
+    const MtOperands p{left, left_sn, left_sc, left_st, right, right_sn, right_sc, right_st, mask, mask_sn, mask_sc, mask_st,
+                       mask_n, N, C, T, K};
+    double* part = reinterpret_cast<double*>(workspace);
+    return dtype == 0 ? metric_update_launch<float>(kind, p, splits, acc, seen, parity, part, ST(stream))
+                      : metric_update_launch<double>(kind, p, splits, acc, seen, parity, part, ST(stream));
+}
+extern "C" int bm_metric_finalize(int kind, const double* acc, int C, int T, double tol, void* out, int out_dtype, int* flag,
+                                  bm_stream_t stream) {
+    BM_CHECK_ARG(kind >= MT_CORRELATION && kind <= MT_ACCURACY && (out_dtype == 0 || out_dtype == 1));
+    const long long cols = (long long)C * T;
+    BM_CHECK_ARG(C >= 0 && T >= 0 && flag && (cols == 0 || (acc && out)));
+    return out_dtype == 0 ? metric_finalize_launch<float>(kind, acc, cols, tol, out, flag, ST(stream))
+                          : metric_finalize_launch<double>(kind, acc, cols, tol, out, flag, ST(stream));
 }
 
 // weight gradient of a (dilated) conv / pointwise layer on the tensor cores: dW[m][n][tap] = sum_{b,t} dY[b,t,m] X[b,t+s,n]

@@ -1946,6 +1946,87 @@ def decoding_loss(table: torch.Tensor, n_cat: int, weights: tp.Optional[torch.Te
 
 
 # ----------------------------------------------------------------------------------------------------
+# Test metrics (bm/metrics.py): each update adds its per-column sums over dim 0 into fp64 accumulators on the device in one
+# bm_metric_update call (one or two launches, set by the shape); get() is one bm_metric_finalize call and one flag word.
+# The operands and the mask are read in place through their strides.  The metric objects are in metrics.py.
+# ----------------------------------------------------------------------------------------------------
+METRIC_CORRELATION, METRIC_L1, METRIC_L2, METRIC_ACCURACY = 0, 1, 2, 3
+# bits of bm_metric_finalize's flag word
+METRIC_LEFT_UNSTABLE, METRIC_LEFT_NAN, METRIC_RIGHT_UNSTABLE, METRIC_RIGHT_NAN, METRIC_RESULT_NAN, METRIC_COUNTED = \
+    1, 2, 4, 8, 16, 32
+_METRIC_DTYPES = {torch.float32: 0, torch.float64: 1}
+
+
+def metric_planes(kind: int) -> int:
+    """fp64 accumulator planes of a metric kind: (Σ l·r·m, Σ l·m, Σ r·m, Σ (l·m)², Σ (r·m)², count) or (sum, count)"""
+    return 6 if kind == METRIC_CORRELATION else 2
+
+
+def _require_cuda_metric(*ts) -> None:
+    if not all(t.is_cuda for t in ts):
+        raise RuntimeError("brainmagick_b200 test metrics run on CUDA (sm_90a) only; there is no CPU fallback: got "
+                           f"{', '.join(str(t.device) for t in ts)}")
+
+
+def _nct(t: torch.Tensor) -> torch.Tensor:
+    """a [N, C, T] operand as it is, a [N, D] one as the view [N, D, 1]"""
+    if t.dim() not in (2, 3):
+        raise ValueError(f"brainmagick_b200 test metrics take [N, C, T] or [N, D] tensors, got {t.dim()} dimensions")
+    return t if t.dim() == 3 else t.unsqueeze(-1)
+
+
+def metric_operands(kind: int, left: torch.Tensor, right: torch.Tensor, mask: torch.Tensor) -> None:
+    """Raises what the reference (or this port) raises for these sliced operands, before anything is allocated"""
+    if left.is_complex() or right.is_complex():
+        raise NotImplementedError("brainmagick_b200 test metrics take real operands (no CUDA model here is complex)")
+    if mask.dtype != torch.bool:
+        raise TypeError(f"brainmagick_b200 test metrics take a bool mask, got {mask.dtype}")
+    _require_cuda_metric(left, right, mask)
+    if left.dtype not in _METRIC_DTYPES or right.dtype != left.dtype:
+        raise TypeError(f"brainmagick_b200 test metrics take fp32 or fp64 operands of one dtype, got {left.dtype} / "
+                        f"{right.dtype}")
+    if not (left.device == right.device == mask.device):
+        raise RuntimeError(f"left on {left.device}, right on {right.device}, mask on {mask.device}")
+    if not (left.dim() == right.dim() == mask.dim()) or left.dim() not in (2, 3):
+        raise RuntimeError(f"the operands and the mask must all be [N, C, T] or all [N, D]: got {tuple(left.shape)}, "
+                           f"{tuple(right.shape)}, {tuple(mask.shape)}")
+    if kind == METRIC_ACCURACY:
+        want = (left.shape[0], 1) + tuple(left.shape[2:])
+        if tuple(mask.shape) != want or tuple(right.shape) != want:   # preds[~mask], expected[~mask] in the reference
+            raise IndexError(f"ClassificationAcc takes targets and a mask of the predictions' shape {want}: got "
+                             f"{tuple(right.shape)} and {tuple(mask.shape)}")
+        if left.shape[1] == 0:
+            raise IndexError("ClassificationAcc: argmax over zero class channels")
+    else:
+        if left.shape != right.shape:
+            raise RuntimeError(f"left {tuple(left.shape)} and right {tuple(right.shape)} differ")
+        if any(m not in (1, n) for m, n in zip(mask.shape, left.shape)):
+            raise RuntimeError(f"the mask {tuple(mask.shape)} does not broadcast to {tuple(left.shape)}")
+
+
+def metric_update(kind: int, left: torch.Tensor, right: torch.Tensor, mask: torch.Tensor, acc: torch.Tensor,
+                  seen: torch.Tensor, parity: int) -> None:
+    """One update of a metric's accumulators on operands metric_operands() accepted: `acc` fp64 [metric_planes(kind), cols]
+    (cols = C*T, T for the accuracy), `seen` the int32 [2] ping-pong word read at `parity` (the caller flips it after the
+    call).  Reads nothing on the host."""
+    l, r, m = _nct(left), _nct(right), _nct(mask)
+    N, C, T = l.shape
+    K, C = (C, 1) if kind == METRIC_ACCURACY else (0, C)
+    ws = _empty((max(int(_lib.load().bm_metric_workspace(N, C, T)), 2),), l)
+    call("bm_metric_update", kind, _METRIC_DTYPES[l.dtype], _view_ptr(l), *_strides(l), _view_ptr(r), *_strides(r),
+         _view_ptr(m), *_mask_strides(m), m.shape[0], N, C, T, K, ptr(acc), ptr(seen), parity, ptr(ws), ws.numel(),
+         stream())
+
+
+def metric_finalize(kind: int, acc: torch.Tensor, cols: int, tol: float, dtype: torch.dtype):
+    """get() of a metric's accumulators -> (out [cols] in `dtype`, flag int32 [1] of METRIC_* bits), both on the device"""
+    out = _empty((cols,), acc, dtype)
+    flag = _empty((1,), acc, torch.int32)
+    call("bm_metric_finalize", kind, ptr(acc), 1, cols, float(tol), ptr(out), _METRIC_DTYPES[dtype], ptr(flag), stream())
+    return out, flag
+
+
+# ----------------------------------------------------------------------------------------------------
 # Stand-alone ChannelMerger.forward / SubjectLayers.forward (bm/models/common.py:334-362, 55-58): inside SimpleConv both are
 # fused into the encoder; called on their own (analysis notebooks, user code) they run the same stage kernels.  Channel-major
 # tensors in and out, like the reference; gradients flow to the parameters and to the input (`meg` / `x`).

@@ -477,6 +477,34 @@ int bm_decoding_loss_bwd(const float* gout, const float* scale, const float* lse
                          long long mask_sb, long long mask_sc, long long mask_st, int B, int T, int est_C, int out_C,
                          const int* table, int F, const float* weights, float* d_est, float* d_out, bm_stream_t stream);
 
+/* ---- Test metrics (bm/metrics.py: OnlineCorrelation, L1Reg, L2Reg, ClassificationAcc) --------------------------------
+ * kind 0 correlation, 1 L1Reg, 2 L2Reg, 3 ClassificationAcc.  dtype / out_dtype 0 fp32, 1 fp64.
+ * bm_metric_update adds one update's per-column sums over n < N into acc, fp64 [NP, C*T] on the device (NP = 6 for the
+ * correlation: Σ l·r·m, Σ l·m, Σ r·m, Σ (l·m)², Σ (r·m)², count; NP = 2 otherwise: the sum, count), column c*T + t:
+ *   kinds 0-2: left and right [N, C, T] read at left[n*left_sn + c*left_sc + t*left_st] (the same for right), any element
+ *     offset; L1Reg sums |(l - r)·m|, L2Reg ((l - r)·m)², l - r formed in the operands' dtype.
+ *   kind 3 (C = 1): the first index of the maximum (NaN maximal) over the K channels left[n*left_sn + k*left_sc +
+ *     t*left_st] compared, as fp64 values, with right[n*right_sn + t*right_st]; the sum counts the equal masked (n, t).
+ * m is the mask byte mask[n*mask_sn + c*mask_sc + t*mask_st] (stride 0 along a broadcast dimension) as 0 or 1, multiplied
+ * in (a masked-out inf or NaN still gives NaN).  The count adds the mask over its own first dimension mask_n (1 or N).
+ * seen [2] int32 on the device: the update reads seen[parity]; while it is 0 the accumulators are overwritten instead of
+ * added to.  It stores 1 into seen[parity ^ 1] when seen[parity] is set or a mask entry was True, and nothing else; the
+ * caller flips parity after every update.  Sums are fp64 FMAs in a fixed row order; when the columns do not fill the GPU
+ * the rows are split into a fixed number of chunks (shape and SM count only) whose partials are added in order by a second
+ * launch: one or two launches per update, bitwise repeatable, no atomics.  workspace: bm_metric_workspace(N, C, T) floats
+ * of caller-owned scratch, 8-byte aligned (0: none needed; NULL is then accepted).  C*T = 0 (an empty slice or time
+ * crop) launches nothing, reads no pointer and leaves seen as it is.
+ * bm_metric_finalize: out [C*T] in out_dtype -- the correlation (the reference's get() formula, order and tol) or sum /
+ * count -- and flag [1]: bit 1 left norm² < -tol, 2 a left norm² is NaN, 4 and 8 the same for the right, 16 a NaN result,
+ * 32 a nonzero count.  With C*T = 0, acc and out may be NULL and flag gets 0. */
+long long bm_metric_workspace(int N, int C, int T);
+int bm_metric_update(int kind, int dtype, const void* left, long long left_sn, long long left_sc, long long left_st,
+                     const void* right, long long right_sn, long long right_sc, long long right_st, const unsigned char* mask,
+                     long long mask_sn, long long mask_sc, long long mask_st, int mask_n, int N, int C, int T, int K,
+                     double* acc, int* seen, int parity, float* workspace, long long workspace_floats, bm_stream_t stream);
+int bm_metric_finalize(int kind, const double* acc, int C, int T, double tol, void* out, int out_dtype, int* flag,
+                       bm_stream_t stream);
+
 /* ---- Deterministic forms (torch.use_deterministic_algorithms(True) in the drop-in modules) -------------------------
  * Every `_det` entry point computes what its default form computes, with the same arguments plus (where noted) a
  * caller-owned workspace of bm_<op>_det_workspace(dims) floats, 8-byte aligned, checked against `workspace_floats`.  Its
