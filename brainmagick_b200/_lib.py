@@ -79,6 +79,9 @@ SIGNATURES = {
     "bm_metric_workspace": [I, I, I],
     "bm_metric_update": [I, I, P, L, L, L, P, L, L, L, P, L, L, L, I, I, I, I, I, P, P, I, P, L, P],
     "bm_metric_finalize": [I, P, I, I, D, P, I, P, P],
+    "bm_svd_table": [I, P, P, P, P, I, I, P, P],
+    "bm_svd_penalty_fwd": [P, I, I, I, L, L, P, P, P, D, P, P],
+    "bm_svd_penalty_bwd": [P, I, I, I, L, L, L, P, P, P, P, D, P, P],
     "bm_tc_wgrad_supported": [I, I],
     "bm_tc_wgrad": [P, P, I, I, I, I, I, I, I, P, P, P, P, P],
     "bm_tc_wgrad_conv_supported": [I, I, I, I],

@@ -17,6 +17,7 @@ from __future__ import annotations
 import dataclasses
 import functools
 import typing as tp
+import weakref
 
 import torch
 import torch.distributed as dist
@@ -2024,6 +2025,115 @@ def metric_finalize(kind: int, acc: torch.Tensor, cols: int, tol: float, dtype: 
     flag = _empty((1,), acc, torch.int32)
     call("bm_metric_finalize", kind, ptr(acc), 1, cols, float(tol), ptr(out), _METRIC_DTYPES[dtype], ptr(flag), stream())
     return out, flag
+
+
+# ----------------------------------------------------------------------------------------------------
+# Spectral-norm penalty (bm/svd.py: svd_penalty): the estimate of every selected weight's top squared singular value by
+# randomized subspace iteration, summed, in one bm_svd_penalty_fwd call (a fixed number of grouped launches whatever the
+# number of weights) and its gradient in one bm_svd_penalty_bwd call.  The weights are read in place; the draws are torch's.
+# The weight table is built on an eager call and kept per (weights, shapes, grad flags, q, niter, device), so a captured
+# call copies nothing from the host.  A table is kept while its weights live: a graph captured with it reads it on every
+# replay, so it is dropped only once its first weight is gone or has moved.  The drop-in function is in svd.py.
+# ----------------------------------------------------------------------------------------------------
+SVD_MAX_DIM = 32                      # largest projection dimension q of the kernels
+
+
+class SvdPlan(tp.NamedTuple):
+    table: torch.Tensor               # int64 [W, 12] on the weights' device (bm_svd_table)
+    q: int
+    niter: int
+    ws_floats: int
+    ws64_doubles: int
+    r_offsets: tp.List[tp.Tuple[int, int]]     # per weight: (offset, rows) of its [rows, q] draw in the draw buffer
+    r_floats: int
+    g_offsets: tp.List[int]                    # per weight: offset of its gradient block, -1 when it gets none
+    g_floats: int
+    tiles: tp.Tuple[int, int, int]             # tiles_m, tiles_n, tiles_w
+
+
+_svd_plans: tp.Dict[tuple, tp.Tuple[SvdPlan, "weakref.ref[torch.Tensor]"]] = {}    # key -> (plan, its first weight)
+
+
+def _require_cuda_svd(weights) -> None:
+    if not all(p.is_cuda for p in weights):
+        raise RuntimeError("brainmagick_b200 svd_penalty runs on CUDA (sm_90a) only; there is no CPU fallback: got "
+                           f"{', '.join(sorted({str(p.device) for p in weights}))}")
+
+
+def svd_plan(weights: tp.Sequence[torch.Tensor], q: int, niter: int) -> SvdPlan:
+    """The table and buffer sizes of these weights (contiguous fp32 on one device) at (q, niter): built once, on an eager
+    call, then returned from the cache without touching the host."""
+    key = (tuple((p.data_ptr(), tuple(p.shape), p.requires_grad) for p in weights), q, niter, weights[0].device)
+    cached = _svd_plans.get(key)
+    if cached is not None:
+        return cached[0]
+    if capturing():
+        raise RuntimeError("svd_penalty: these weights' table is built on an eager call: run one eager step on this device "
+                           "before capturing")
+    for k in [k for k, (_, ref) in _svd_plans.items() if ref() is None or ref().data_ptr() != k[0][0][0]]:
+        del _svd_plans[k]                                # tables of weights that are gone or have moved
+    W = len(weights)
+    ptrs = torch.tensor([p.data_ptr() for p in weights], dtype=torch.int64)
+    rows = torch.tensor([p.shape[0] for p in weights], dtype=torch.int64)
+    cols = torch.tensor([p.numel() // p.shape[0] for p in weights], dtype=torch.int64)
+    grad = torch.tensor([int(p.requires_grad) for p in weights], dtype=torch.int32)
+    table = torch.empty((W, 12), dtype=torch.int64)
+    sizes = torch.empty((7,), dtype=torch.int64)
+    lib = _lib.load()
+    if lib.bm_svd_table(W, ptrs.data_ptr(), rows.data_ptr(), cols.data_ptr(), grad.data_ptr(), q, niter, table.data_ptr(),
+                        sizes.data_ptr()) != 0:
+        raise _lib.BmB200Error(f"bm_svd_table failed: {lib.bm_last_error().decode()}")
+    ws, ws64, r, g, tm, tn, tw = (int(v) for v in sizes.tolist())
+    t = table.tolist()
+    plan = SvdPlan(table.to(weights[0].device), q, niter, max(ws, 2), max(ws64, 1),
+                   [(row[7], min(row[1], row[2])) for row in t], r, [row[8] for row in t], g, (tm, tn, tw))
+    _svd_plans[key] = (plan, weakref.ref(weights[0]))
+    return plan
+
+
+def svd_draws(plan: SvdPlan, like: torch.Tensor) -> torch.Tensor:
+    """Every weight's draw R [min(m, n), q] from torch's generator, one normal_ per weight in weight order -- what
+    torch.randn(min(m, n), q) inside each torch.svd_lowrank call draws -- into one fp32 buffer"""
+    R = _empty((max(plan.r_floats, 1),), like)
+    for off, n in plan.r_offsets:
+        R[off:off + n * plan.q].view(n, plan.q).normal_()
+    return R
+
+
+class _SvdPenaltyFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, plan: SvdPlan, proba: float, R, *weights):
+        ws = _empty((plan.ws_floats,), R)
+        ws64 = _empty((plan.ws64_doubles,), R, torch.float64)
+        out = _empty((1,), R)
+        tm, tn, _ = plan.tiles
+        call("bm_svd_penalty_fwd", ptr(plan.table), len(weights), plan.q, plan.niter, tm, tn, ptr(R), ptr(ws), ptr(ws64),
+             float(proba), ptr(out), stream())
+        ctx.save_for_backward(R, ws, ws64, *weights)
+        ctx.plan, ctx.proba = plan, proba
+        return out.reshape(())
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    def backward(ctx, gout):
+        R, ws, ws64, *weights = ctx.saved_tensors
+        plan = ctx.plan
+        grad = _empty((max(plan.g_floats, 1),), R)
+        g = gout.reshape(1).contiguous().float()
+        call("bm_svd_penalty_bwd", ptr(plan.table), len(weights), plan.q, plan.niter, *plan.tiles, ptr(R), ptr(ws), ptr(ws64),
+             ptr(g), float(ctx.proba), ptr(grad), stream())
+        grads = [grad[off:off + p.numel()].view(p.shape) if off >= 0 and need else None
+                 for p, off, need in zip(weights, plan.g_offsets, ctx.needs_input_grad[3:])]
+        return (None, None, None, *grads)
+
+
+def svd_penalty(weights: tp.Sequence[torch.Tensor], q: int, niter: int, proba: float) -> torch.Tensor:
+    """Σ over `weights` of torch.svd_lowrank(p.view(p.shape[0], -1), q, niter)[1][0] ** 2, divided by proba, as a 0-dim fp32
+    tensor on their device; differentiable in every weight that requires grad.  The weights are contiguous fp32 CUDA
+    tensors on one device (checked by the caller).  The draws come from torch's CUDA generator, one per weight in order."""
+    plan = svd_plan(weights, q, niter)
+    R = svd_draws(plan, weights[0])
+    return _SvdPenaltyFn.apply(plan, float(proba), R, *weights)
 
 
 # ----------------------------------------------------------------------------------------------------

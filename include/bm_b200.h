@@ -505,6 +505,33 @@ int bm_metric_update(int kind, int dtype, const void* left, long long left_sn, l
 int bm_metric_finalize(int kind, const double* acc, int C, int T, double tol, void* out, int out_dtype, int* flag,
                        bm_stream_t stream);
 
+/* ---- Spectral-norm penalty (bm/svd.py: svd_penalty) -----------------------------------------------------------------
+ * For W weights, each the row-major fp32 matrix P [rows_p, cols_p] (a weight viewed as [shape[0], -1]) read in place in its
+ * tall orientation A [m, n], m >= n (A = Pᵀ when rows_p < cols_p): the estimate λ of torch.svd_lowrank(P, q, niter)'s
+ * S[0]², i.e. the top eigenvalue of Qᵀ A Aᵀ Q where Q spans A (AᵀA)^niter R for the draw R [n, q] (randomized subspace
+ * iteration with an orthonormalisation after every product; only the spans enter); when n <= q the span is A's whole range
+ * and λ is σ₁(A)² exactly.  Columns of a panel whose Cholesky pivot is at or below 1e-8 of its Gram matrix's largest
+ * diagonal are dropped, so a weight of rank below q gives a finite value and gradient (DESIGN §4.10).  Everything is FP32
+ * FMA with fp64 Gram matrices and eigenproblems, whatever the TF32 flag or autocast; no atomics and a fixed order everywhere, so repeated calls are bitwise identical.  q = 1..32, niter >= 0.
+ * bm_svd_table (host only, no launch) fills table int64 [W, 12] from the weights' device addresses ptrs, shapes and grad
+ * flags (nonzero: the weight gets a gradient), and sizes int64 [7]: the float workspace, the double workspace, the draw
+ * buffer R and the gradient buffer in elements, then the grouped tile counts tiles_m, tiles_n and tiles_w.  The caller
+ * copies the table to the device once and passes it, with those counts, to every call for the same weights and settings.
+ * Weight i's draw is R[table[i][7] ...] as an [n_i, q] row-major block, n_i = min(rows_p, cols_p).
+ * bm_svd_penalty_fwd: out [1] fp32 = Σ λ_i / proba (fp64 sum in weight order), all on the device; it leaves in ws / ws64
+ * (sizes[0] floats / sizes[1] doubles, caller-owned) what the backward of the same call reads.  13 launches at niter = 2
+ * (2 niter + 5 at most, fewer when no weight has n > q), whatever W.
+ * bm_svd_penalty_bwd: after the forward with the same buffers, writes the gradient gout[0] / proba · dλ_i/dP_i of every
+ * weight with a gradient into grad (sizes[3] floats; weight i's [rows_p, cols_p] block at table[i][8]), every element once:
+ * for n <= q 2 σ₁ u₁ v₁ᵀ, else the derivative through the spans (DESIGN §4.10).  At most 2 niter + 5 launches, whatever W. */
+int bm_svd_table(int W, const long long* ptrs, const long long* rows_p, const long long* cols_p, const int* grad, int q,
+                 int niter, long long* table, long long* sizes);
+int bm_svd_penalty_fwd(const long long* table, int W, int q, int niter, long long tiles_m, long long tiles_n, const float* R,
+                       float* ws, double* ws64, double proba, float* out, bm_stream_t stream);
+int bm_svd_penalty_bwd(const long long* table, int W, int q, int niter, long long tiles_m, long long tiles_n,
+                       long long tiles_w, const float* R, float* ws, const double* ws64, const float* gout, double proba,
+                       float* grad, bm_stream_t stream);
+
 /* ---- Deterministic forms (torch.use_deterministic_algorithms(True) in the drop-in modules) -------------------------
  * Every `_det` entry point computes what its default form computes, with the same arguments plus (where noted) a
  * caller-owned workspace of bm_<op>_det_workspace(dims) floats, 8-byte aligned, checked against `workspace_floats`.  Its
