@@ -3,8 +3,8 @@
 masked regression losses `L1Loss` / `L2Loss` of encoding models and the regression baseline and the decoding loss
 `FeatureDecodingLoss` -- and for the callers either side of it: batch preparation (`norm`: bm/norm.py), the DeepMel
 feature model (`features`: bm/models/features.py), the retrieval evaluation (`retrieval`: scripts/run_eval_probs.py,
-bm/wer.py), the test-stage metrics (`metrics`: bm/metrics.py) and the solver's spectral penalty (`svd_penalty`:
-bm/svd.py)."""
+bm/wer.py), the test-stage metrics (`metrics`: bm/metrics.py), the solver's spectral penalty (`svd_penalty`:
+bm/svd.py) and its contrastive negative pool (`NegativePool`: bm/solver.py)."""
 import os as _os
 
 import torch as _torch
@@ -23,7 +23,8 @@ from .features import DeepMel  # noqa: F401
 from .norm import BatchScaler, ScaleReject  # noqa: F401
 from . import metrics  # noqa: F401,E402
 from .svd import svd_penalty  # noqa: F401,E402
+from .negatives import NegativePool, PooledCandidates  # noqa: F401,E402
 
 __all__ = ["SimpleConv", "ClipLoss", "L1Loss", "L2Loss", "FeatureDecodingLoss", "ChannelMerger", "ConvSequence",
            "FourierEmb", "PositionGetter", "StaticBatch", "SubjectLayers", "DeepMel", "BatchScaler", "ScaleReject",
-           "svd_penalty"]
+           "svd_penalty", "NegativePool", "PooledCandidates"]

@@ -52,6 +52,8 @@ SIGNATURES = {
     "bm_clip_scores": [P, P, I, I, L, I, P, P, P, P, L, P, P],
     "bm_clip_loss_fwd": [P, P, I, I, L, I, P, P, P, P, P, P, L, P, P],
     "bm_clip_loss_bwd": [P, P, P, P, I, I, L, I, P, P, P, P],
+    "bm_clip_loss_fwd_pooled": [P, P, I, P, P, I, I, L, I, P, P, P, P, P, P, L, P, P],
+    "bm_clip_loss_bwd_pooled": [P, P, P, I, P, P, P, I, I, L, I, P, P, P, P],
     "bm_set_debug_flags": [I],
     "bm_set_debug_buffer": [P],
     "bm_tc_conv_supported": [I, I, I, I, I],
@@ -100,6 +102,7 @@ SIGNATURES = {
     "bm_scale_clamp_crop": [P, P, P, P, I, I, I, I, I, F, I, I, P, P, P],
     "bm_reject_compact": [P, P, L, F, I, P, P, P, P],
     "bm_gather_rows": [P, P, I, L, P, P],
+    "bm_scatter_rows": [P, P, I, L, P, P],
     "bm_bn_act_skip_fwd": [P, P, P, P, P, P, P, L, I, I, F, P],
     "bm_bn_act_skip_bwd": [P, P, P, P, P, P, I, L, I, I, F, P, P, P, P, P],
     "bm_bn_act_skip_bwd_reduce": [P, P, P, P, P, P, L, I, I, F, P, P, P, P],
@@ -139,11 +142,13 @@ SIGNATURES = {
     "bm_candidate_inv_norms_det": [P, I, L, P, P, P],
     "bm_clip_scores_det": [P, P, I, I, L, I, P, P, P, P, L, P, P],
     "bm_clip_loss_fwd_det": [P, P, I, I, L, I, P, P, P, P, P, P, L, P, P],
+    "bm_clip_loss_fwd_pooled_det": [P, P, I, P, P, I, I, L, I, P, P, P, P, P, P, L, P, P],
 }
 # single-pass TF32 forms (tf32() below): the default form's arguments
 TF32_FORMS = ("bm_tc_conv1d", "bm_tc_conv1d_persistent", "bm_tc_pointwise_sel", "bm_tc_sensor_mix_bwd_data", "bm_tc_wgrad",
               "bm_tc_wgrad_conv", "bm_tc_wgrad_grouped", "bm_clip_scores", "bm_clip_scores_det", "bm_clip_loss_fwd",
-              "bm_clip_loss_fwd_det", "bm_clip_loss_bwd", "bm_clip_loss_bwd_cand", "bm_clip_scores_bwd")
+              "bm_clip_loss_fwd_det", "bm_clip_loss_bwd", "bm_clip_loss_bwd_cand", "bm_clip_scores_bwd",
+              "bm_clip_loss_fwd_pooled", "bm_clip_loss_fwd_pooled_det", "bm_clip_loss_bwd_pooled")
 SIGNATURES.update({name + "_tf32": SIGNATURES[name] for name in TF32_FORMS})
 # bf16 forms (bf16() below): the same entry points, the default form's arguments
 SIGNATURES.update({name + "_bf16": SIGNATURES[name] for name in TF32_FORMS})

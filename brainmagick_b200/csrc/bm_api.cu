@@ -1225,6 +1225,59 @@ BM_TC_FORMS(bm_clip_loss_bwd, clip_loss_bwd,
              int target_offset, float* G, float* dest, int* status, bm_stream_t stream),
             (probs, inv_norm, cand, gout, Bn, Bc, KT, target_offset, G, dest, status, stream))
 
+// ---- pooled candidates (negatives.py): candidate o is cand[o] for o < Bb, else arena[slots[o - Bb]] ----------------------
+namespace {
+int check_pooled(const float* cand, int Bb, const float* arena, const int* slots, int Bn, int Bc, long long KT) {
+    BM_CHECK_ARG(cand && Bn > 0 && Bb >= 0 && Bb <= Bc && (Bb == Bc || (arena && slots)));
+    BM_CHECK_ARG(tc::clip_tc_supported(Bn, Bc, KT));
+    return 0;
+}
+
+int clip_loss_fwd_pooled(int passes, bool det, const float* est, const float* cand, int Bb, const float* arena,
+                         const int* slots, int Bn, int Bc, long long KT, int target_offset, float* inv_norm, float* scores,
+                         float* probs, float* row_loss, float* loss, float* workspace, long long workspace_floats, int* status,
+                         bm_stream_t stream) {
+    if (int rc = check_pooled(cand, Bb, arena, slots, Bn, Bc, KT)) return rc;
+    BM_CHECK_ARG(est && inv_norm && scores && probs && row_loss && loss && workspace);
+    BM_CHECK_ARG(target_offset >= 0 && target_offset + Bn <= Bc);
+    BM_CHECK_ARG(workspace_floats >= bm_clip_workspace(Bn, Bc, KT));
+    BM_CHECK_ARG((reinterpret_cast<uintptr_t>(workspace) & 7) == 0);
+    return tc::launch_clip_scores(est, cand, Bn, Bc, KT, 0, target_offset, inv_norm, scores, probs, row_loss, loss,
+                                  workspace, passes, status, ST(stream), det, Bb, arena, Bb < Bc ? slots : nullptr);
+}
+
+int clip_loss_bwd_pooled(int passes, const float* probs, const float* inv_norm, const float* cand, int Bb, const float* arena,
+                         const int* slots, const float* gout, int Bn, int Bc, long long KT, int target_offset, float* G,
+                         float* dest, int* status, bm_stream_t stream) {
+    (void)status;
+    if (int rc = check_pooled(cand, Bb, arena, slots, Bn, Bc, KT)) return rc;
+    BM_CHECK_ARG(probs && inv_norm && gout && G && dest);
+    cudaStream_t st = ST(stream);
+    const int ldg = (Bc + 3) / 4 * 4;
+    clip_ce_bwd_padded_kernel<<<ew_grid((long long)Bn * ldg), 256, 0, st>>>(probs, inv_norm, gout, Bn, Bc, ldg,
+                                                                            target_offset, G);
+    BM_CHECK_LAUNCH();
+    return tc::launch_gemm_nt_pooled(G, ldg, cand, Bb, arena, slots, Bc, dest, Bn, (int)KT, passes, st);
+}
+}  // namespace
+
+#define BM_CLIP_LOSS_FWD_POOLED_PARAMS                                                                                   \
+    (const float* est, const float* cand, int Bb, const float* arena, const int* slots, int Bn, int Bc, long long KT,   \
+     int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss, float* loss, float* workspace,   \
+     long long workspace_floats, int* status, bm_stream_t stream)
+#define BM_CLIP_LOSS_FWD_POOLED_ARGS(det)                                                                                \
+    (det, est, cand, Bb, arena, slots, Bn, Bc, KT, target_offset, inv_norm, scores, probs, row_loss, loss, workspace,   \
+     workspace_floats, status, stream)
+BM_TC_FORMS(bm_clip_loss_fwd_pooled, clip_loss_fwd_pooled, BM_CLIP_LOSS_FWD_POOLED_PARAMS,
+            BM_CLIP_LOSS_FWD_POOLED_ARGS(false))
+BM_TC_FORMS(bm_clip_loss_fwd_pooled_det, clip_loss_fwd_pooled, BM_CLIP_LOSS_FWD_POOLED_PARAMS,
+            BM_CLIP_LOSS_FWD_POOLED_ARGS(true))
+BM_TC_FORMS(bm_clip_loss_bwd_pooled, clip_loss_bwd_pooled,
+            (const float* probs, const float* inv_norm, const float* cand, int Bb, const float* arena, const int* slots,
+             const float* gout, int Bn, int Bc, long long KT, int target_offset, float* G, float* dest, int* status,
+             bm_stream_t stream),
+            (probs, inv_norm, cand, Bb, arena, slots, gout, Bn, Bc, KT, target_offset, G, dest, status, stream))
+
 // =================================================================================================
 // Stand-alone ConvSequence epilogues (the forms of epi_fwd / epi_bwd above) + candidate-side ClipLoss gradient (SURVEY 8(f)
 // row 3: DeepMel)
@@ -1429,6 +1482,14 @@ extern "C" int bm_gather_rows(const float* x, const int* rows, int n_rows, long 
                               bm_stream_t stream) {
     BM_CHECK_ARG(x && rows && y && n_rows > 0 && row_elems > 0);
     gather_rows_kernel<<<ew_grid((long long)n_rows * row_elems), 256, 0, ST(stream)>>>(x, rows, n_rows, row_elems, y);
+    BM_CHECK_LAUNCH();
+    return 0;
+}
+
+extern "C" int bm_scatter_rows(const float* x, const int* rows, int n_rows, long long row_elems, float* y,
+                               bm_stream_t stream) {
+    BM_CHECK_ARG(x && rows && y && n_rows > 0 && row_elems > 0);
+    scatter_rows_kernel<<<ew_grid((long long)n_rows * row_elems), 256, 0, ST(stream)>>>(x, rows, n_rows, row_elems, y);
     BM_CHECK_LAUNCH();
     return 0;
 }

@@ -244,9 +244,8 @@ __global__ void weight_prep_kernel(const float* __restrict__ W, float* __restric
 // ------------------------------------------------------------------------------------------------
 // ss[o] += sum_k cand[o][k]^2 (fp64 atomics; grid = (rows, splits)).  With one split, every slot receives exactly one add
 // onto its zero: the deterministic form.
-__global__ void row_sumsq_kernel(const float* __restrict__ X, double* __restrict__ ss, long long K) {
+__device__ __forceinline__ void row_sumsq_row(const float* __restrict__ x, double* __restrict__ ss, long long K) {
     __shared__ double red[32];
-    const float* x = X + (long long)blockIdx.x * K;
     long long chunk = (K + gridDim.y - 1) / gridDim.y;
     long long k0 = (long long)blockIdx.y * chunk, k1 = min(K, k0 + chunk);
     float s = 0.f;
@@ -266,6 +265,15 @@ __global__ void row_sumsq_kernel(const float* __restrict__ X, double* __restrict
         v = warp_sum_d(v);
         if (threadIdx.x == 0) atomicAdd(ss + blockIdx.x, v);
     }
+}
+__global__ void row_sumsq_kernel(const float* __restrict__ X, double* __restrict__ ss, long long K) {
+    row_sumsq_row(X + (long long)blockIdx.x * K, ss, K);
+}
+// the same over pooled candidates: row o is X[o] for o < Bb (the batch), else arena[slots[o - Bb]] (the negative pool)
+__global__ void row_sumsq_pooled_kernel(const float* __restrict__ X, int Bb, const float* __restrict__ arena,
+                                        const int* __restrict__ slots, double* __restrict__ ss, long long K) {
+    const int o = blockIdx.x;
+    row_sumsq_row(o < Bb ? X + (long long)o * K : arena + (long long)slots[o - Bb] * K, ss, K);
 }
 
 // inv_norm[o] = 1 / (1e-8 + sqrt(ss[o]))    (losses.py:91)
@@ -342,6 +350,25 @@ __global__ void clip_ce_bwd_kernel(const float* __restrict__ probs, const float*
         float v = gs * p * inv_norm[o];
         if (transposed) G[(long long)o * Bn + b] = v;
         else G[i] = v;
+    }
+}
+
+// clip_ce_bwd_kernel's G [Bn][Bc] in rows of ld >= Bc floats, the columns Bc..ld-1 zero (the pooled backward's GEMM reads
+// G in float4 steps along the candidates)
+__global__ void clip_ce_bwd_padded_kernel(const float* __restrict__ probs, const float* __restrict__ inv_norm,
+                                          const float* __restrict__ gout, int Bn, int Bc, int ld, int target_offset,
+                                          float* __restrict__ G) {
+    long long total = (long long)Bn * ld;
+    float gs = gout[0] / (float)Bn;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        int b = (int)(i / ld), o = (int)(i - (long long)b * ld);
+        float v = 0.f;
+        if (o < Bc) {
+            float p = probs[(long long)b * Bc + o] - (o == b + target_offset ? 1.f : 0.f);
+            v = gs * p * inv_norm[o];
+        }
+        G[i] = v;
     }
 }
 

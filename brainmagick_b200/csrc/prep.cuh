@@ -109,4 +109,16 @@ __global__ void gather_rows_kernel(const float* __restrict__ x, const int* __res
     }
 }
 
+// y[rows[i]][:] = x[i][:], the inverse of gather_rows_kernel: a batch written into free rows of the negative pool's
+// device storage (the rows must be distinct)
+__global__ void scatter_rows_kernel(const float* __restrict__ x, const int* __restrict__ rows, int n_rows,
+                                    long long row_elems, float* __restrict__ y) {
+    const long long total = (long long)n_rows * row_elems;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const long long r = i / row_elems, e = i - r * row_elems;
+        y[(long long)rows[r] * row_elems + e] = x[i];
+    }
+}
+
 }  // namespace bm

@@ -56,6 +56,20 @@ struct ClipOp {
     }
 };
 
+// ClipOp over pooled candidates: candidate n is C + n*KT for n < Bb (the batch rows, read in place), else
+// arena + slots[n - Bb]*KT (a row of the negative pool's device storage); one more load per row than ClipOp
+struct ClipPooledOp : ClipOp {
+    const float* arena; const int* slots;
+    int Bb;
+    __device__ float4 b4(const Cta& c, int kb, int r, int q) const {
+        const int n = c.n0 + r;
+        const long long k = (long long)(c.c0 + kb) * HG_BK + 4 * q;
+        if (n >= Bc || k >= KT) return make_float4(0.f, 0.f, 0.f, 0.f);
+        const float* row = n < Bb ? C + n * KT : arena + __ldg(slots + (n - Bb)) * KT;
+        return __ldg(reinterpret_cast<const float4*>(row + k));
+    }
+};
+
 // ---- finalize: fixed-order reduction of the K slices, 1/norm, scores, optional softmax / cross-entropy / batch mean ----
 // one block per estimate row b.  `counter` (zeroed by the launcher) elects the last block, which averages row_loss in a
 // fixed order.
@@ -163,10 +177,12 @@ inline long long clip_ws_floats(int Bn, int Bc, long long KT) {
     return n + 2ll * g.ks * Bc + 2;
 }
 
-// scores [Bn][Bc] (+ inv_norm when !norms_given, + probs / row_loss / loss when requested)
+// scores [Bn][Bc] (+ inv_norm when !norms_given, + probs / row_loss / loss when requested).  slots != NULL: pooled
+// candidates (ClipPooledOp): candidates Bb..Bc-1 are the arena rows slots[0..Bc-Bb-1]
 inline int launch_clip_scores(const float* est, const float* cand, int Bn, int Bc, long long KT, int norms_given,
                               int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss,
-                              float* loss, float* ws, int passes, int* err, cudaStream_t st, bool det = false) {
+                              float* loss, float* ws, int passes, int* err, cudaStream_t st, bool det = false,
+                              int Bb = 0, const float* arena = nullptr, const int* slots = nullptr) {
     (void)err;
     const ClipGeom g = clip_geometry(Bn, Bc, KT);
     long long nP = (long long)g.ks * Bn * Bc;
@@ -183,15 +199,23 @@ inline int launch_clip_scores(const float* est, const float* cand, int Bn, int B
         int splits = (int)((KT + 65535) / 65536);
         if (splits > 32) splits = 32;
         if (det) splits = 1;                                      // one add per slot: independent of block order
-        row_sumsq_kernel<<<dim3(Bc, splits), 256, 0, st>>>(cand, ssp, KT);
+        if (slots) row_sumsq_pooled_kernel<<<dim3(Bc, splits), 256, 0, st>>>(cand, Bb, arena, slots, ssp, KT);
+        else row_sumsq_kernel<<<dim3(Bc, splits), 256, 0, st>>>(cand, ssp, KT);
         ++g_launches;
         cudaError_t e = cudaGetLastError();
         if (e != cudaSuccess) return set_error(3, "%s: norm launch failed: %s", __func__, cudaGetErrorString(e));
     }
-    ClipOp o;
-    o.E = est; o.C = cand; o.Bn = Bn; o.Bc = Bc; o.chunks = g.chunks; o.per_split = g.per_split; o.KT = KT; o.P = ws;
-    if (int rc = hg_launch<HG_BN>(o, dim3((Bc + HG_BN - 1) / HG_BN, (Bn + HG_BM - 1) / HG_BM, g.ks), passes, st, __func__))
-        return rc;
+    const dim3 grid((Bc + HG_BN - 1) / HG_BN, (Bn + HG_BM - 1) / HG_BM, g.ks);
+    if (slots) {
+        ClipPooledOp o;
+        o.E = est; o.C = cand; o.Bn = Bn; o.Bc = Bc; o.chunks = g.chunks; o.per_split = g.per_split; o.KT = KT; o.P = ws;
+        o.arena = arena; o.slots = slots; o.Bb = Bb;
+        if (int rc = hg_launch<HG_BN>(o, grid, passes, st, __func__)) return rc;
+    } else {
+        ClipOp o;
+        o.E = est; o.C = cand; o.Bn = Bn; o.Bc = Bc; o.chunks = g.chunks; o.per_split = g.per_split; o.KT = KT; o.P = ws;
+        if (int rc = hg_launch<HG_BN>(o, grid, passes, st, __func__)) return rc;
+    }
     clip_finalize_kernel<<<Bn, 256, 0, st>>>(ws, ssp, g.ks, Bn, Bc, target_offset, inv_norm, scores, probs, row_loss,
                                              loss, counter);
     ++g_launches;

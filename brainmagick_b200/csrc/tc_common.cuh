@@ -39,30 +39,29 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <algorithm>
+#include <array>
 #include <type_traits>
+#include <utility>
+#include <vector>
 #include "common.cuh"
 
 namespace bm {
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device): the attribute is per device, so a
-// process-wide flag would leave a second device of the same process without it.
+// process-wide flag would leave a second device of the same process without it.  The table grows with the kernels a
+// process launches: every instantiation of the tensor-core loops can reach it, so no fixed count bounds them.
 inline int ensure_dyn_smem(const void* func, int bytes) {
-    constexpr int kMaxDev = 64, kMaxFn = 32;
-    static const void* fns[kMaxFn];
-    static bool done[kMaxFn][kMaxDev];
-    static int nfn = 0;
+    constexpr int kMaxDev = 64;
+    static std::vector<std::pair<const void*, std::array<bool, kMaxDev>>> done;
     int dev = 0;
     cudaGetDevice(&dev);
-    int f = 0;
-    while (f < nfn && fns[f] != func) ++f;
-    if (f == nfn) {
-        if (nfn == kMaxFn) return set_error(3, "%s: too many kernels%s", __func__);
-        fns[nfn++] = func;
-    }
-    if (dev >= 0 && dev < kMaxDev && done[f][dev]) return 0;
+    size_t f = 0;
+    while (f < done.size() && done[f].first != func) ++f;
+    if (f == done.size()) done.push_back({func, {}});
+    if (dev >= 0 && dev < kMaxDev && done[f].second[dev]) return 0;
     cudaError_t e = cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
     if (e != cudaSuccess) return set_error(3, "%s: cudaFuncSetAttribute: %s", __func__, cudaGetErrorString(e));
-    if (dev >= 0 && dev < kMaxDev) done[f][dev] = true;
+    if (dev >= 0 && dev < kMaxDev) done[f].second[dev] = true;
     return 0;
 }
 

@@ -34,6 +34,19 @@ struct GemmNTOp {
     }
 };
 
+// dE = G C over pooled candidates (ClipPooledOp's rows): B row kk is B + kk*N for kk < Bb, else arena + slots[kk - Bb]*N,
+// and zero for Bc <= kk < K (K: G's row pitch, Bc rounded up to a multiple of 4 floats)
+struct GemmNTPooledOp : GemmNTOp {
+    const float* arena; const int* slots;
+    int Bb, Bc;
+    __device__ float4 b4(const Cta& c, int kb, int k, int q) const {
+        const int kk = kb * HG_BK + k, n = c.n0 + 4 * q;
+        if (kk >= Bc || n >= N) return make_float4(0.f, 0.f, 0.f, 0.f);
+        const float* row = kk < Bb ? B + (long long)kk * N : arena + (long long)__ldg(slots + (kk - Bb)) * N;
+        return __ldg(reinterpret_cast<const float4*>(row + n));
+    }
+};
+
 inline bool gemm_nt_pp_supported(int M, int N, int K) {
     return M > 0 && N >= 32 && K >= 8 && K % 4 == 0 && N % 4 == 0;
 }
@@ -43,6 +56,15 @@ inline int launch_gemm_nt_pp(const float* A, const float* B, float* D, int M, in
                              cudaStream_t st) {
     (void)err;
     GemmNTOp o{A, B, D, M, N, K};
+    return hg_launch<HG_BN>(o, dim3((N + HG_BN - 1) / HG_BN, (M + HG_BM - 1) / HG_BM, 1), passes, st, __func__);
+}
+
+// D [M][N] = G [M][ldg] * pooled candidates [Bc][N] (GemmNTPooledOp); ldg % 4 == 0, the columns Bc..ldg-1 of G zero
+inline int launch_gemm_nt_pooled(const float* G, int ldg, const float* cand, int Bb, const float* arena, const int* slots,
+                                 int Bc, float* D, int M, int N, int passes, cudaStream_t st) {
+    GemmNTPooledOp o;
+    o.A = G; o.B = cand; o.D = D; o.M = M; o.N = N; o.K = ldg;
+    o.arena = arena; o.slots = slots; o.Bb = Bb; o.Bc = Bc;
     return hg_launch<HG_BN>(o, dim3((N + HG_BN - 1) / HG_BN, (M + HG_BM - 1) / HG_BM, 1), passes, st, __func__);
 }
 

@@ -309,7 +309,8 @@ def _reducing_call(name, like, ws_dims, *args, reduces=True):
 # torch.autocast("cuda", dtype=torch.bfloat16) (`_lib.bf16()`, recorded by each autograd node's forward for its backward)
 # it takes its `_bf16` form instead, whatever the TF32 flag says.  The FP32-FMA kernels stay exact (TF32 and bf16 are
 # permitted, not required) and the fp16-piece entry points keep their one form.
-_DET_SAME_ARGS = ("bm_clip_scores", "bm_clip_loss_fwd")      # tensor-core entry points with a `_det` form of the same arguments
+# tensor-core entry points with a `_det` form of the same arguments
+_DET_SAME_ARGS = ("bm_clip_scores", "bm_clip_loss_fwd", "bm_clip_loss_fwd_pooled")
 
 
 def replays_bf16(backward):
@@ -1777,6 +1778,61 @@ class _ClipLossFn(torch.autograd.Function):
 
 def clip_loss(estimate, candidate, target_offset: int = 0):
     return _ClipLossFn.apply(estimate, candidate, target_offset)
+
+
+def clip_pooled_supported(KT: int) -> bool:
+    """Whether the pooled CLIP entry points take rows of KT floats (the tensor-core forms' 16-byte row pitch)."""
+    return KT >= 32 and KT % 4 == 0 and KT < (1 << 31)
+
+
+class _ClipLossPooledFn(torch.autograd.Function):
+    """ClipLoss.forward over a negatives.PooledCandidates: the candidates are read where they lie (the batch rows in
+    place, the pool rows in the pool's device storage through the slot table).  The candidates carry no gradient, as in
+    the reference, which builds them under no_grad.  The node keeps the PooledCandidates, and with it the lease on its
+    slots, until its backward has run."""
+
+    @staticmethod
+    def forward(ctx, estimate, pooled):
+        ctx.bf16 = _lib.bf16()                   # the mode the backward replays
+        _check_clip_operands(estimate, pooled.batch)
+        est = estimate.contiguous()
+        Bn, Bc, Bb = est.shape[0], len(pooled), pooled.batch.shape[0]
+        KT = est[0].numel()
+        assert pooled.row_elems == KT, f"estimate rows of {KT} values, candidate rows of {pooled.row_elems}"
+        inv = _empty((Bc,), est)
+        scores = _empty((Bn, Bc), est)
+        probs = _empty((Bn, Bc), est)
+        row_loss = _empty((Bn,), est)
+        loss = _empty((1,), est)
+        ws = _clip_workspace(est, Bn, Bc, KT)
+        _tc_call("bm_clip_loss_fwd_pooled", ptr(est), ptr(pooled.batch), Bb, ptr(pooled.storage), ptr(pooled.slots), Bn, Bc,
+                 KT, 0, ptr(inv), ptr(scores), ptr(probs), ptr(row_loss), ptr(loss), ptr(ws), ws.numel(),
+                 ptr(tc_status_tensor(est.device)), stream())
+        ctx.save_for_backward(probs, inv)
+        ctx.pooled = pooled
+        ctx.meta = (Bn, Bc, Bb, KT, est.shape)
+        return loss.reshape(())
+
+    @staticmethod
+    @torch.autograd.function.once_differentiable
+    @replays_bf16
+    def backward(ctx, gout):
+        probs, inv = ctx.saved_tensors
+        pooled, ctx.pooled = ctx.pooled, None    # the lease on the slots ends here
+        Bn, Bc, Bb, KT, shape = ctx.meta
+        gout = gout.reshape(1).contiguous().float()
+        G = _empty((Bn, _round_up(Bc, 4)), probs)
+        dest = _empty(shape, probs)
+        _tc_call("bm_clip_loss_bwd_pooled", ptr(probs), ptr(inv), ptr(pooled.batch), Bb, ptr(pooled.storage),
+                 ptr(pooled.slots), ptr(gout), Bn, Bc, KT, 0, ptr(G), ptr(dest), ptr(tc_status_tensor(probs.device)),
+                 stream())
+        return dest, None
+
+
+def clip_loss_pooled(estimate, pooled):
+    """ClipLoss.forward over a negatives.PooledCandidates (targets: the first Bn candidates); needs
+    clip_pooled_supported(KT)."""
+    return _ClipLossPooledFn.apply(estimate, pooled)
 
 
 # ----------------------------------------------------------------------------------------------------

@@ -27,6 +27,7 @@ import torch
 
 from . import functional as BF
 from . import distrib
+from .negatives import PooledCandidates
 
 
 def _wants_grad(estimates, candidates) -> bool:
@@ -267,6 +268,19 @@ class ClipLoss(torch.nn.Module):
         self._mask_ok = (weakref.ref(mask), mask._version)
 
     def forward(self, estimate, candidate, mask=None):
+        if isinstance(candidate, PooledCandidates):
+            if self.global_negatives and distrib.world_size() > 1:
+                raise NotImplementedError("ClipLoss(global_negatives=True) over a negative pool: the reference's pool is "
+                                          "local to each GPU, and mixing pools across ranks has no reference meaning")
+            if BF.capturing():
+                raise RuntimeError("ClipLoss over a negative pool cannot be captured in a CUDA graph: the slot table is "
+                                   "built on the host and the candidate count grows while the pool fills")
+            if self._window(estimate.shape[-1]) == (0, estimate.shape[-1]) and not (self.pool or self.center) \
+                    and BF.clip_pooled_supported(candidate.row_elems):
+                self._check_mask(mask)
+                assert estimate.size(0) <= candidate.size(0), "need at least as many targets as estimates"
+                return BF.clip_loss_pooled(estimate, candidate)
+            candidate = candidate.materialize()
         if self.global_negatives and BF.capturing() and distrib.world_size() > 1:
             raise RuntimeError("ClipLoss(global_negatives=True) all-gathers the candidates over the ranks, which a CUDA graph "
                                "capture of the step cannot hold; capture on one rank or without global_negatives")

@@ -212,6 +212,19 @@ int bm_clip_loss_fwd(const float* est, const float* cand, int Bn, int Bc, long l
 /* dL/dest [Bn,KT] = gout * ((probs - onehot)/Bn * inv_norm) @ cand ; G [Bn,Bc] scratch; gout [1] on device. */
 int bm_clip_loss_bwd(const float* probs, const float* inv_norm, const float* cand, const float* gout, int Bn,
                      int Bc, long long KT, int target_offset, float* G, float* dest, int* status, bm_stream_t stream);
+/* The same over pooled candidates (the solver's `optim.negatives` pool, bm/solver.py:358-371): candidate o is cand[o] for
+ * o < Bb (the batch, read in place) and arena[slots[o - Bb]] for Bb <= o < Bc (a row of the pool's device storage, slots
+ * int32 [Bc - Bb] on the device; arena and slots may be NULL when Bb == Bc).  The contiguous forms' arithmetic, bit for bit:
+ * the forward runs the same kernels with one more load per pool row; the backward always runs the wgmma GEMM of
+ * bm_clip_loss_bwd's Bn >= 192 form, over G [Bn, ldg] scratch with ldg = Bc rounded up to a multiple of 4 (zero columns).
+ * Requires KT % 4 == 0 and KT >= 32.  The `_det`, `_tf32` and `_bf16` forms are those of bm_clip_loss_fwd. */
+int bm_clip_loss_fwd_pooled(const float* est, const float* cand, int Bb, const float* arena, const int* slots, int Bn,
+                            int Bc, long long KT, int target_offset, float* inv_norm, float* scores, float* probs,
+                            float* row_loss, float* loss, float* workspace, long long workspace_floats, int* status,
+                            bm_stream_t stream);
+int bm_clip_loss_bwd_pooled(const float* probs, const float* inv_norm, const float* cand, int Bb, const float* arena,
+                            const int* slots, const float* gout, int Bn, int Bc, long long KT, int target_offset, float* G,
+                            float* dest, int* status, bm_stream_t stream);
 
 /* ---- Stand-alone ConvSequence / DeepMel (SURVEY 8(f) row 3): bm/models/common.py:79-151, bm/models/features.py:15-35 --
  * Layer epilogue x_new = act(bn(y)) (+ x_old) over channels-last rows [rows, C] and its backward, for any activation:
@@ -299,13 +312,15 @@ int bm_rowdot_scaled(const float* a, const float* c, int Bn, long long K, float*
  *   pattern of max |op(x)| over the whole uncropped sample (what ScaleReject tests, norm.py:334).
  * bm_reject_compact: keep[b] = !(peak > limit) && (mask == NULL || any(mask[b])) (norm.py:335-339);
  *   keep_rows = kept sample indices in order, n_keep[0] their count.
- * bm_gather_rows: y[i] = x[rows[i]] over rows of row_elems floats (batch[keep], norm.py:340). */
+ * bm_gather_rows: y[i] = x[rows[i]] over rows of row_elems floats (batch[keep], norm.py:340).
+ * bm_scatter_rows: y[rows[i]] = x[i], its inverse (rows distinct): a batch written into free rows of the negative pool. */
 int bm_scale_clamp_crop(const float* x, const int* slot, const float* center, const float* scale, int B, int C, int T,
                         int t0, int T_out, float limit, int clip, int inverse, float* y, unsigned int* peak_bits,
                         bm_stream_t stream);
 int bm_reject_compact(const unsigned int* peak_bits, const unsigned char* mask, long long mask_elems, float limit,
                       int B, unsigned char* keep, int* keep_rows, int* n_keep, bm_stream_t stream);
 int bm_gather_rows(const float* x, const int* rows, int n_rows, long long row_elems, float* y, bm_stream_t stream);
+int bm_scatter_rows(const float* x, const int* rows, int n_rows, long long row_elems, float* y, bm_stream_t stream);
 
 /* ---- tensor-core (wgmma) versions of K3/K4: 3xTF32 implicit-GEMM conv ------------------------------------
  * Same arithmetic contract as bm_conv1d_fwd / bm_conv1d_bwd_data / bm_conv1d_glu_fwd (fp32-faithful: every
@@ -611,6 +626,9 @@ int bm_clip_scores_det(const float* est, const float* cand, int Bn, int Bc, long
 int bm_clip_loss_fwd_det(const float* est, const float* cand, int Bn, int Bc, long long KT, int target_offset,
                          float* inv_norm, float* scores, float* probs, float* row_loss, float* loss, float* workspace,
                          long long workspace_floats, int* status, bm_stream_t stream);
+int bm_clip_loss_fwd_pooled_det(const float* est, const float* cand, int Bb, const float* arena, const int* slots, int Bn,
+        int Bc, long long KT, int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss, float* loss,
+        float* workspace, long long workspace_floats, int* status, bm_stream_t stream);
 
 /* ---- TF32 forms (PyTorch's TF32 matmul precision in the drop-in modules) -------------------------------------------
  * Every `_tf32` entry point takes its default form's arguments and computes its contraction in single-pass TF32 instead of
@@ -661,6 +679,15 @@ int bm_clip_loss_bwd_cand_tf32(const float* probs, const float* scores, const fl
 int bm_clip_scores_bwd_tf32(const float* dscores, const float* scores, const float* inv_norm, const float* est,
                             const float* cand, int Bn, int Bc, long long KT, float* G, float* coef, float* dest,
                             float* dcand, int* status, bm_stream_t stream);
+int bm_clip_loss_fwd_pooled_tf32(const float* est, const float* cand, int Bb, const float* arena, const int* slots, int Bn,
+        int Bc, long long KT, int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss, float* loss,
+        float* workspace, long long workspace_floats, int* status, bm_stream_t stream);
+int bm_clip_loss_fwd_pooled_det_tf32(const float* est, const float* cand, int Bb, const float* arena, const int* slots, int Bn,
+        int Bc, long long KT, int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss, float* loss,
+        float* workspace, long long workspace_floats, int* status, bm_stream_t stream);
+int bm_clip_loss_bwd_pooled_tf32(const float* probs, const float* inv_norm, const float* cand, int Bb, const float* arena,
+        const int* slots, const float* gout, int Bn, int Bc, long long KT, int target_offset, float* G, float* dest,
+        int* status, bm_stream_t stream);
 
 
 /* ---- bf16 forms (torch.autocast(dtype=torch.bfloat16) in the drop-in modules) -----------------------------------------
@@ -717,6 +744,15 @@ int bm_clip_loss_bwd_cand_bf16(const float* probs, const float* scores, const fl
 int bm_clip_scores_bwd_bf16(const float* dscores, const float* scores, const float* inv_norm, const float* est,
                             const float* cand, int Bn, int Bc, long long KT, float* G, float* coef, float* dest,
                             float* dcand, int* status, bm_stream_t stream);
+int bm_clip_loss_fwd_pooled_bf16(const float* est, const float* cand, int Bb, const float* arena, const int* slots, int Bn,
+        int Bc, long long KT, int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss, float* loss,
+        float* workspace, long long workspace_floats, int* status, bm_stream_t stream);
+int bm_clip_loss_fwd_pooled_det_bf16(const float* est, const float* cand, int Bb, const float* arena, const int* slots, int Bn,
+        int Bc, long long KT, int target_offset, float* inv_norm, float* scores, float* probs, float* row_loss, float* loss,
+        float* workspace, long long workspace_floats, int* status, bm_stream_t stream);
+int bm_clip_loss_bwd_pooled_bf16(const float* probs, const float* inv_norm, const float* cand, int Bb, const float* arena,
+        const int* slots, const float* gout, int Bn, int Bc, long long KT, int target_offset, float* G, float* dest,
+        int* status, bm_stream_t stream);
 
 #ifdef __cplusplus
 }
