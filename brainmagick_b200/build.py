@@ -1,18 +1,22 @@
 """Builds libbm_b200.so in-tree with nvcc for sm_90a (H100) (cross-compiles without a GPU)."""
 from __future__ import annotations
 
+import concurrent.futures
 import hashlib
 import os
 import subprocess
 import sys
+import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libbm_b200.so")
 STAMP = LIB + ".sha256"        # digest of the sources the library was built from (git-ignored, travels with the .so)
-SOURCES = ["bm_api.cu"]
+# one translation unit per subsystem, compiled in parallel; no relocatable device code, so each keeps its own kernels
+SOURCES = ["api.cu", "gemm_simt.cu", "front_api.cu", "convseq_api.cu", "tc_conv_api.cu", "clip_api.cu", "losses_api.cu",
+           "svd_api.cu", "prep_api.cu"]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
-              "-Xcompiler", "-fPIC", "-shared", "--expt-relaxed-constexpr"]
+              "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr"]
 
 
 def _source_digest() -> str:
@@ -36,18 +40,34 @@ def is_current() -> bool:
         return f.read().strip() == _source_digest()
 
 
+def compile_library(out: str, extra_flags: list[str] = (), verbose: bool = False, csrc: str = CSRC) -> str:
+    """Compiles every SOURCES translation unit of `csrc` with `nvcc -c` in parallel, then links them with one
+    `nvcc -shared` into `out`.  The objects live in a temporary directory: the tree receives the library alone."""
+    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
+    name = os.path.basename(out)
+
+    def run(cmd):
+        res = subprocess.run(cmd, capture_output=True, text=True)
+        if res.returncode != 0:
+            sys.stderr.write(res.stdout + res.stderr)
+            raise RuntimeError(f"nvcc failed building {name}")
+        if verbose:
+            sys.stderr.write(res.stderr)
+
+    with tempfile.TemporaryDirectory() as tmp:
+        objs = [os.path.join(tmp, os.path.splitext(s)[0] + ".o") for s in SOURCES]
+        cmds = [[nvcc] + NVCC_FLAGS + list(extra_flags) + ["-c", os.path.join(csrc, s), "-o", o]
+                for s, o in zip(SOURCES, objs)]
+        with concurrent.futures.ThreadPoolExecutor(max_workers=min(len(cmds), os.cpu_count() or 1)) as pool:
+            list(pool.map(run, cmds))
+        run([nvcc, "-shared"] + objs + ["-o", out, "-lcudart"])
+    return out
+
+
 def build_library(force: bool = False, verbose: bool = False) -> str:
     if not force and is_current():
         return LIB
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc] + NVCC_FLAGS + (["-Xptxas", "-v"] if verbose else []) + \
-        [os.path.join(CSRC, s) for s in SOURCES] + ["-o", LIB, "-lcudart"]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if res.returncode != 0:
-        sys.stderr.write(res.stdout + res.stderr)
-        raise RuntimeError("nvcc failed building libbm_b200.so")
-    if verbose:
-        sys.stderr.write(res.stderr)
+    compile_library(LIB, (["-Xptxas", "-v"] if verbose else []), verbose)
     with open(STAMP, "w") as f:
         f.write(_source_digest() + "\n")
     return LIB

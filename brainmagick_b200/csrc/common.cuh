@@ -103,4 +103,16 @@ inline int num_sms() {
     return n;
 }
 
+inline bool aligned16(const void* a, const void* b = nullptr, const void* c = nullptr) {
+    return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) == 0;
+}
+
+inline int ew_grid(long long total, int block = 256, int per_thread = 1) {
+    long long g = (total / per_thread + block - 1) / block;
+    long long cap = (long long)num_sms() * 16;
+    if (g > cap) g = cap;
+    if (g < 1) g = 1;
+    return (int)g;
+}
+
 }  // namespace bm

@@ -1,6 +1,6 @@
 // The ConvSequence layer epilogue (bm/models/common.py:65-76,79-151) of every convolution layer -- SimpleConv's encoder,
-// the stand-alone ConvSequence and the DeepMel feature model (bm/models/features.py:15-35) -- and the candidate-side gradient
-// of ClipLoss that a trainable feature model needs (bm/losses.py:91-94 differentiated w.r.t. `candidates`).
+// the stand-alone ConvSequence and the DeepMel feature model (bm/models/features.py:15-35) -- and the other elementwise
+// kernels of the FP32-FMA layers (convseq_api.cu): BatchNorm eval statistics, GLU and GELU backward, conv weight re-layout.
 //
 // Epilogue over channels-last rows [rows, C]: branch = act(bn(y)) with bn(y) = ((y - mean) * invstd) * gamma + beta (or y
 // itself without a BatchNorm), x_new = post[c] * ((boost * scale[c]) * branch) (+ x_old) with the residual gains (LayerScale,
@@ -394,28 +394,87 @@ __global__ void epi_bwd_apply_kernel(const float* __restrict__ g, const float* _
     }
 }
 
-// ---- ClipLoss, gradient w.r.t. the candidates -----------------------------------------------------------------
-// scores[b][o] = inv_o <e_b, c_o>, inv_o = 1/(1e-8 + ||c_o||)   (losses.py:91-94).  With G = dL/d<e_b, c_o> (the matrix
-// clip_ce_bwd_kernel builds), dL/dc_o = sum_b G[b][o] e_b  -  coef_o c_o,
-//   coef_o = (sum_b G[b][o] scores[b][o]) / ||c_o||      (the derivative of inv_o; 0 for a zero candidate, as autograd's
-//                                                          norm backward defines it)
-__global__ void clip_cand_coef_kernel(const float* __restrict__ G, const float* __restrict__ scores,
-                                      const float* __restrict__ inv_norm, int Bn, int Bc, float* __restrict__ coef) {
-    int o = blockIdx.x * blockDim.x + threadIdx.x;
-    if (o >= Bc) return;
-    float acc = 0.f;
-    for (int b = 0; b < Bn; ++b) acc = fmaf(G[(long long)b * Bc + o], scores[(long long)b * Bc + o], acc);
-    float norm = 1.f / inv_norm[o] - 1e-8f;
-    coef[o] = norm > 0.f ? acc / norm : 0.f;
+// eval mode: mean = running_mean, invstd = 1/sqrt(running_var + eps)
+__global__ void bn_eval_stats_kernel(const float* __restrict__ rm, const float* __restrict__ rv, float eps,
+                                     float* __restrict__ mean, float* __restrict__ invstd, int C) {
+    int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= C) return;
+    mean[c] = rm[c];
+    invstd[c] = 1.f / sqrtf(rv[c] + eps);
 }
 
-// dcand[o][k] -= coef[o] * cand[o][k]
-__global__ void clip_cand_correct_kernel(const float* __restrict__ cand, const float* __restrict__ coef, long long KT,
-                                         long long total, float* __restrict__ dcand) {
+// ------------------------------------------------------------------------------------------------
+// GLU backward (common.py:133-138): h = [a | b] per row (2H columns), out = a*sigmoid(b)
+// ------------------------------------------------------------------------------------------------
+__global__ void glu_bwd_kernel(const float* __restrict__ g, const float* __restrict__ h, float* __restrict__ dh,
+                               long long rows, int H) {
+    long long total = rows * H;
     for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
          i += (long long)gridDim.x * blockDim.x) {
-        const int o = (int)(i / KT);
-        dcand[i] = fmaf(-coef[o], cand[i], dcand[i]);
+        long long r = i / H;
+        int c = (int)(i - r * H);
+        float a = h[r * 2 * H + c], b = h[r * 2 * H + H + c];
+        float s = sigmoid_f(b);
+        float gg = g[i];
+        dh[r * 2 * H + c] = gg * s;
+        dh[r * 2 * H + H + c] = gg * a * s * (1.f - s);
+    }
+}
+
+// dh = dq * GELU'(h)   (head, simpleconv.py:185-189)
+__global__ void gelu_bwd_kernel(const float* __restrict__ dq, const float* __restrict__ h, float* __restrict__ dh,
+                                long long total) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x)
+        dh[i] = dq[i] * gelu_grad_f(h[i]);
+}
+
+// ------------------------------------------------------------------------------------------------
+// conv weight re-layout: W[o][i][j] -> Wf[j][i][o] (forward B operand) and Wb[j][o][i] (data-gradient B operand)
+// ------------------------------------------------------------------------------------------------
+__global__ void weight_prep_kernel(const float* __restrict__ W, float* __restrict__ Wf, float* __restrict__ Wb,
+                                   int O, int I, int Kw) {
+    long long total = (long long)O * I * Kw;
+    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
+         idx += (long long)gridDim.x * blockDim.x) {
+        int j = (int)(idx % Kw);
+        long long oi = idx / Kw;
+        int i = (int)(oi % I), o = (int)(oi / I);
+        float v = W[idx];
+        if (Wf) Wf[((long long)j * I + i) * O + o] = v;
+        if (Wb) Wb[((long long)j * O + o) * I + i] = v;
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// float4 versions (C % 4 == 0, 16-byte aligned rows): one thread owns 4 consecutive channels
+// ------------------------------------------------------------------------------------------------
+__global__ void glu_bwd_v4_kernel(const float4* __restrict__ g, const float4* __restrict__ h, float4* __restrict__ dh,
+                                  long long rows, int H) {
+    const int H4 = H >> 2;
+    long long total = rows * H4;
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const long long r = i / H4;
+        const int c4 = (int)(i - r * H4);
+        const float4 a = h[r * 2 * H4 + c4], b = h[r * 2 * H4 + H4 + c4], gg = g[i];
+        float4 da, db;
+        float s;
+        s = sigmoid_f(b.x); da.x = gg.x * s; db.x = gg.x * a.x * s * (1.f - s);
+        s = sigmoid_f(b.y); da.y = gg.y * s; db.y = gg.y * a.y * s * (1.f - s);
+        s = sigmoid_f(b.z); da.z = gg.z * s; db.z = gg.z * a.z * s * (1.f - s);
+        s = sigmoid_f(b.w); da.w = gg.w * s; db.w = gg.w * a.w * s * (1.f - s);
+        dh[r * 2 * H4 + c4] = da;
+        dh[r * 2 * H4 + H4 + c4] = db;
+    }
+}
+
+__global__ void gelu_bwd_v4_kernel(const float4* __restrict__ dq, const float4* __restrict__ h, float4* __restrict__ dh,
+                                   long long total4) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total4;
+         i += (long long)gridDim.x * blockDim.x) {
+        const float4 d = dq[i], x = h[i];
+        dh[i] = make_float4(d.x * gelu_grad_f(x.x), d.y * gelu_grad_f(x.y), d.z * gelu_grad_f(x.z), d.w * gelu_grad_f(x.w));
     }
 }
 

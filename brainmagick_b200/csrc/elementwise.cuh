@@ -1,85 +1,11 @@
-// HBM-bound kernels of the hot path: everything that is not a contraction.
+// HBM-bound kernels of the FP32-FMA layers: BatchNorm finalize, column reductions and the column-stationary GLU backward.
+// Templates only: front_api.cu and convseq_api.cu both include this header.
 // Activations are channels-last [B, T, C] inside the encoder (rows = B*T), so a warp always walks
 // contiguous channels; per-channel parameters are read through the read-only path.
 #pragma once
 #include "common.cuh"
 
 namespace bm {
-
-// ------------------------------------------------------------------------------------------------
-// K1 pieces: Fourier embedding of sensor positions and the masked softmax (common.py:254-271,339-357)
-// ------------------------------------------------------------------------------------------------
-// emb[rc][k*n+l] = cos(loc), emb[rc][P/2 + k*n+l] = sin(loc), loc = (x+margin)*f[k] + (y+margin)*f[l]
-// `freq` is the table 2*pi*arange(n)/(1+2*margin) built by the host with the reference's own op order, and
-// the products/sum are rounded separately (no FMA contraction) so that `loc` is bit-identical to torch's.
-__global__ void fourier_emb_kernel(const float* __restrict__ pos, const float* __restrict__ freq, float margin,
-                                   int RC, int n, float* __restrict__ emb) {
-    const int P2 = n * n;
-    long long total = (long long)RC * P2;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        int rc = (int)(idx / P2);
-        int kl = (int)(idx - (long long)rc * P2);
-        int k = kl / n, l = kl - k * n;
-        float x = __fadd_rn(pos[2 * rc], margin), y = __fadd_rn(pos[2 * rc + 1], margin);
-        float loc = __fadd_rn(__fmul_rn(x, freq[k]), __fmul_rn(y, freq[l]));
-        float s, c;
-        sincosf(loc, &s, &c);
-        emb[(long long)rc * 2 * P2 + kl] = c;
-        emb[(long long)rc * 2 * P2 + P2 + kl] = s;
-    }
-}
-
-// in-place softmax over c of scores[r][o][:] with -inf on invalid (pos == INVALID) and banned sensors
-// (||pos - centre|| <= radius, training only).  One warp per (r, o) row.
-__global__ void masked_softmax_kernel(float* __restrict__ w, const float* __restrict__ pos,
-                                      const float* __restrict__ centre, float radius, float invalid, int R, int O,
-                                      int C) {
-    int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    int lane = threadIdx.x & 31;
-    if (row >= R * O) return;
-    int r = row / O;
-    float* s = w + (long long)row * C;
-    const float* pr = pos + (long long)r * C * 2;
-    float cx = 0.f, cy = 0.f;
-    if (centre) { cx = centre[0]; cy = centre[1]; }
-    float mx = -INFINITY;
-    for (int c = lane; c < C; c += 32) {
-        float x = pr[2 * c], y = pr[2 * c + 1];
-        bool masked = (x == invalid) && (y == invalid);
-        if (centre) {
-            float dx = x - cx, dy = y - cy;
-            masked = masked || (sqrtf(__fadd_rn(__fmul_rn(dx, dx), __fmul_rn(dy, dy))) <= radius);
-        }
-        float v = masked ? -INFINITY : s[c];
-        s[c] = v;
-        mx = fmaxf(mx, v);
-    }
-    mx = warp_max(mx);
-    float sum = 0.f;
-    for (int c = lane; c < C; c += 32) {
-        float e = expf(s[c] - mx);
-        s[c] = e;
-        sum += e;
-    }
-    sum = warp_sum(sum);
-    float inv = 1.f / sum;
-    for (int c = lane; c < C; c += 32) s[c] *= inv;
-}
-
-// dscore = w * (dw - sum_c w*dw)   (softmax backward, one warp per row)
-__global__ void softmax_bwd_kernel(const float* __restrict__ w, const float* __restrict__ dw,
-                                   float* __restrict__ ds, int rows, int C) {
-    int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
-    int lane = threadIdx.x & 31;
-    if (row >= rows) return;
-    const float* wr = w + (long long)row * C;
-    const float* dr = dw + (long long)row * C;
-    float dot = 0.f;
-    for (int c = lane; c < C; c += 32) dot += wr[c] * dr[c];
-    dot = warp_sum(dot);
-    for (int c = lane; c < C; c += 32) ds[(long long)row * C + c] = wr[c] * (dr[c] - dot);
-}
 
 // ------------------------------------------------------------------------------------------------
 // BatchNorm1d statistics (common.py:118-120); the layer epilogue that applies them is in convseq.cuh
@@ -107,41 +33,6 @@ __global__ void bn_finalize_kernel(const double* __restrict__ stats, double n, f
         double unb = n > 1 ? var * n / (n - 1) : var;
         running_var[c] = (1.f - momentum) * running_var[c] + momentum * (float)unb;
     }
-}
-
-// eval mode: mean = running_mean, invstd = 1/sqrt(running_var + eps)
-__global__ void bn_eval_stats_kernel(const float* __restrict__ rm, const float* __restrict__ rv, float eps,
-                                     float* __restrict__ mean, float* __restrict__ invstd, int C) {
-    int c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= C) return;
-    mean[c] = rm[c];
-    invstd[c] = 1.f / sqrtf(rv[c] + eps);
-}
-
-// ------------------------------------------------------------------------------------------------
-// GLU backward (common.py:133-138): h = [a | b] per row (2H columns), out = a*sigmoid(b)
-// ------------------------------------------------------------------------------------------------
-__global__ void glu_bwd_kernel(const float* __restrict__ g, const float* __restrict__ h, float* __restrict__ dh,
-                               long long rows, int H) {
-    long long total = rows * H;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-         i += (long long)gridDim.x * blockDim.x) {
-        long long r = i / H;
-        int c = (int)(i - r * H);
-        float a = h[r * 2 * H + c], b = h[r * 2 * H + H + c];
-        float s = sigmoid_f(b);
-        float gg = g[i];
-        dh[r * 2 * H + c] = gg * s;
-        dh[r * 2 * H + H + c] = gg * a * s * (1.f - s);
-    }
-}
-
-// dh = dq * GELU'(h)   (head, simpleconv.py:185-189)
-__global__ void gelu_bwd_kernel(const float* __restrict__ dq, const float* __restrict__ h, float* __restrict__ dh,
-                                long long total) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-         i += (long long)gridDim.x * blockDim.x)
-        dh[i] = dq[i] * gelu_grad_f(h[i]);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -219,234 +110,6 @@ __global__ void rowsum_cm_kernel(const float* __restrict__ X, float* __restrict_
     if (lane == 0) {
         if (DET) out[row] = s;
         else atomicAdd(out + (int)(row % N), s);
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// conv weight re-layout: W[o][i][j] -> Wf[j][i][o] (forward B operand) and Wb[j][o][i] (data-gradient B operand)
-// ------------------------------------------------------------------------------------------------
-__global__ void weight_prep_kernel(const float* __restrict__ W, float* __restrict__ Wf, float* __restrict__ Wb,
-                                   int O, int I, int Kw) {
-    long long total = (long long)O * I * Kw;
-    for (long long idx = blockIdx.x * (long long)blockDim.x + threadIdx.x; idx < total;
-         idx += (long long)gridDim.x * blockDim.x) {
-        int j = (int)(idx % Kw);
-        long long oi = idx / Kw;
-        int i = (int)(oi % I), o = (int)(oi / I);
-        float v = W[idx];
-        if (Wf) Wf[((long long)j * I + i) * O + o] = v;
-        if (Wb) Wb[((long long)j * O + o) * I + i] = v;
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// ClipLoss pieces (losses.py:91-114)
-// ------------------------------------------------------------------------------------------------
-// ss[o] += sum_k cand[o][k]^2 (fp64 atomics; grid = (rows, splits)).  With one split, every slot receives exactly one add
-// onto its zero: the deterministic form.
-__device__ __forceinline__ void row_sumsq_row(const float* __restrict__ x, double* __restrict__ ss, long long K) {
-    __shared__ double red[32];
-    long long chunk = (K + gridDim.y - 1) / gridDim.y;
-    long long k0 = (long long)blockIdx.y * chunk, k1 = min(K, k0 + chunk);
-    float s = 0.f;
-    double acc = 0.0;
-    int cnt = 0;
-    for (long long k = k0 + threadIdx.x; k < k1; k += blockDim.x) {
-        float v = x[k];
-        s = fmaf(v, v, s);
-        if (++cnt == 64) { acc += (double)s; s = 0.f; cnt = 0; }
-    }
-    acc += (double)s;
-    acc = warp_sum_d(acc);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = acc;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        double v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.0;
-        v = warp_sum_d(v);
-        if (threadIdx.x == 0) atomicAdd(ss + blockIdx.x, v);
-    }
-}
-__global__ void row_sumsq_kernel(const float* __restrict__ X, double* __restrict__ ss, long long K) {
-    row_sumsq_row(X + (long long)blockIdx.x * K, ss, K);
-}
-// the same over pooled candidates: row o is X[o] for o < Bb (the batch), else arena[slots[o - Bb]] (the negative pool)
-__global__ void row_sumsq_pooled_kernel(const float* __restrict__ X, int Bb, const float* __restrict__ arena,
-                                        const int* __restrict__ slots, double* __restrict__ ss, long long K) {
-    const int o = blockIdx.x;
-    row_sumsq_row(o < Bb ? X + (long long)o * K : arena + (long long)slots[o - Bb] * K, ss, K);
-}
-
-// inv_norm[o] = 1 / (1e-8 + sqrt(ss[o]))    (losses.py:91)
-__global__ void inv_norm_kernel(const double* __restrict__ ss, float* __restrict__ inv, int n) {
-    int i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i < n) inv[i] = 1.f / (1e-8f + (float)sqrt(ss[i]));
-}
-
-// per row b: lse, row_loss[b] = lse - s[b][b+off]; optional probs = softmax(s)   (one block per row)
-__global__ void clip_ce_rows_kernel(const float* __restrict__ scores, int Bn, int Bc, int target_offset,
-                                    float* __restrict__ row_loss, float* __restrict__ probs) {
-    __shared__ float red[32];
-    __shared__ float bcast;
-    int b = blockIdx.x;
-    const float* s = scores + (long long)b * Bc;
-    float mx = -INFINITY;
-    for (int o = threadIdx.x; o < Bc; o += blockDim.x) mx = fmaxf(mx, s[o]);
-    mx = warp_max(mx);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = mx;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : -INFINITY;
-        v = warp_max(v);
-        if (threadIdx.x == 0) bcast = v;
-    }
-    __syncthreads();
-    mx = bcast;
-    __syncthreads();
-    float sum = 0.f;
-    for (int o = threadIdx.x; o < Bc; o += blockDim.x) sum += expf(s[o] - mx);
-    sum = warp_sum(sum);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = sum;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        float v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.f;
-        v = warp_sum(v);
-        if (threadIdx.x == 0) bcast = v;
-    }
-    __syncthreads();
-    sum = bcast;
-    if (row_loss && threadIdx.x == 0) row_loss[b] = (logf(sum) + mx) - s[b + target_offset];
-    if (probs) {
-        float inv = 1.f / sum;
-        for (int o = threadIdx.x; o < Bc; o += blockDim.x) probs[(long long)b * Bc + o] = expf(s[o] - mx) * inv;
-    }
-}
-
-// loss = mean(row_loss)  (single block, deterministic order)
-__global__ void mean_kernel(const float* __restrict__ x, int n, float* __restrict__ out) {
-    __shared__ double red[32];
-    double s = 0.0;
-    for (int i = threadIdx.x; i < n; i += blockDim.x) s += (double)x[i];
-    s = warp_sum_d(s);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        double v = threadIdx.x < (blockDim.x >> 5) ? red[threadIdx.x] : 0.0;
-        v = warp_sum_d(v);
-        if (threadIdx.x == 0) out[0] = (float)(v / n);
-    }
-}
-
-// G[b][o] = gout * (softmax(s)[b][o] - [o == b+off]) / Bn * inv_norm[o]    (A.6 of SURVEY.md)
-// transposed != 0: G is written as [Bc][Bn] (the dY operand layout of the tensor-core dE GEMM)
-__global__ void clip_ce_bwd_kernel(const float* __restrict__ probs, const float* __restrict__ inv_norm,
-                                   const float* __restrict__ gout, int Bn, int Bc, int target_offset,
-                                   float* __restrict__ G, int transposed) {
-    long long total = (long long)Bn * Bc;
-    float gs = gout[0] / (float)Bn;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-         i += (long long)gridDim.x * blockDim.x) {
-        int b = (int)(i / Bc), o = (int)(i - (long long)b * Bc);
-        float p = probs[i] - (o == b + target_offset ? 1.f : 0.f);
-        float v = gs * p * inv_norm[o];
-        if (transposed) G[(long long)o * Bn + b] = v;
-        else G[i] = v;
-    }
-}
-
-// clip_ce_bwd_kernel's G [Bn][Bc] in rows of ld >= Bc floats, the columns Bc..ld-1 zero (the pooled backward's GEMM reads
-// G in float4 steps along the candidates)
-__global__ void clip_ce_bwd_padded_kernel(const float* __restrict__ probs, const float* __restrict__ inv_norm,
-                                          const float* __restrict__ gout, int Bn, int Bc, int ld, int target_offset,
-                                          float* __restrict__ G) {
-    long long total = (long long)Bn * ld;
-    float gs = gout[0] / (float)Bn;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-         i += (long long)gridDim.x * blockDim.x) {
-        int b = (int)(i / ld), o = (int)(i - (long long)b * ld);
-        float v = 0.f;
-        if (o < Bc) {
-            float p = probs[(long long)b * Bc + o] - (o == b + target_offset ? 1.f : 0.f);
-            v = gs * p * inv_norm[o];
-        }
-        G[i] = v;
-    }
-}
-
-// G[b][o] = dscores[b][o] * inv_norm[o]: the same G for an arbitrary upstream gradient of the scores (get_scores backward);
-// transposed as in clip_ce_bwd_kernel
-__global__ void clip_scores_grad_kernel(const float* __restrict__ dscores, const float* __restrict__ inv_norm, int Bn, int Bc,
-                                        float* __restrict__ G, int transposed) {
-    long long total = (long long)Bn * Bc;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-         i += (long long)gridDim.x * blockDim.x) {
-        int b = (int)(i / Bc), o = (int)(i - (long long)b * Bc);
-        float v = dscores[i] * inv_norm[o];
-        if (transposed) G[(long long)o * Bn + b] = v;
-        else G[i] = v;
-    }
-}
-
-// y[b][c][t] = x[b][c][t] * mask[c]   (simpleconv.py:200-203: `subsample_meg_channels` zeroes the sensors not drawn)
-__global__ void channel_mask_kernel(const float* __restrict__ x, const float* __restrict__ mask, float* __restrict__ y,
-                                    int C, int T, long long total) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-         i += (long long)gridDim.x * blockDim.x) {
-        const int c = (int)((i / T) % C);
-        y[i] = x[i] * mask[c];
-    }
-}
-
-// in [Z][N][T] -> out [Z][T][N]   (32x32 tiles through shared memory, both sides coalesced)
-__global__ void transpose_nt_kernel(const float* __restrict__ in, float* __restrict__ out, int N, int T, int ld_out,
-                                    int n_store) {
-    // n_store = N: plain transpose; n_store = ld_out > N: the pad columns [N, ld_out) are written as zeros
-    __shared__ float tile[32][33];
-    const long long zoff = (long long)blockIdx.z * N * T;
-    const long long zout = (long long)blockIdx.z * T * ld_out;
-    int t = blockIdx.x * 32 + threadIdx.x;
-#pragma unroll
-    for (int i = threadIdx.y; i < 32; i += 8) {
-        int n = blockIdx.y * 32 + i;
-        tile[i][threadIdx.x] = (n < N && t < T) ? in[zoff + (long long)n * T + t] : 0.f;
-    }
-    __syncthreads();
-    int n = blockIdx.y * 32 + threadIdx.x;
-#pragma unroll
-    for (int i = threadIdx.y; i < 32; i += 8) {
-        int tt = blockIdx.x * 32 + i;
-        if (n < n_store && tt < T) out[zout + (long long)tt * ld_out + n] = tile[threadIdx.x][i];
-    }
-}
-
-// ------------------------------------------------------------------------------------------------
-// float4 versions (C % 4 == 0, 16-byte aligned rows): one thread owns 4 consecutive channels
-// ------------------------------------------------------------------------------------------------
-__global__ void glu_bwd_v4_kernel(const float4* __restrict__ g, const float4* __restrict__ h, float4* __restrict__ dh,
-                                  long long rows, int H) {
-    const int H4 = H >> 2;
-    long long total = rows * H4;
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
-         i += (long long)gridDim.x * blockDim.x) {
-        const long long r = i / H4;
-        const int c4 = (int)(i - r * H4);
-        const float4 a = h[r * 2 * H4 + c4], b = h[r * 2 * H4 + H4 + c4], gg = g[i];
-        float4 da, db;
-        float s;
-        s = sigmoid_f(b.x); da.x = gg.x * s; db.x = gg.x * a.x * s * (1.f - s);
-        s = sigmoid_f(b.y); da.y = gg.y * s; db.y = gg.y * a.y * s * (1.f - s);
-        s = sigmoid_f(b.z); da.z = gg.z * s; db.z = gg.z * a.z * s * (1.f - s);
-        s = sigmoid_f(b.w); da.w = gg.w * s; db.w = gg.w * a.w * s * (1.f - s);
-        dh[r * 2 * H4 + c4] = da;
-        dh[r * 2 * H4 + H4 + c4] = db;
-    }
-}
-
-__global__ void gelu_bwd_v4_kernel(const float4* __restrict__ dq, const float4* __restrict__ h, float4* __restrict__ dh,
-                                   long long total4) {
-    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total4;
-         i += (long long)gridDim.x * blockDim.x) {
-        const float4 d = dq[i], x = h[i];
-        dh[i] = make_float4(d.x * gelu_grad_f(x.x), d.y * gelu_grad_f(x.y), d.z * gelu_grad_f(x.z), d.w * gelu_grad_f(x.w));
     }
 }
 
@@ -546,41 +209,5 @@ __global__ void reduce_rows_kernel(const T* __restrict__ part, long long n, int 
     out[c] = s;
 }
 
-inline bool aligned16(const void* a, const void* b = nullptr, const void* c = nullptr) {
-    return ((reinterpret_cast<uintptr_t>(a) | reinterpret_cast<uintptr_t>(b) | reinterpret_cast<uintptr_t>(c)) & 15) == 0;
-}
-
-inline int ew_grid(long long total, int block = 256, int per_thread = 1) {
-    long long g = (total / per_thread + block - 1) / block;
-    long long cap = (long long)num_sms() * 16;
-    if (g > cap) g = cap;
-    if (g < 1) g = 1;
-    return (int)g;
-}
-
-// ------------------------------------------------------------------------------------------------
-// ClipLoss's `assert mask.all()` (bm/losses.py:110) without a host read: status <- code (if still 0) when any of the n
-// bytes of `mask` is 0.  `vec`: mask is 16-byte aligned, read as uint4 (the last n % 16 bytes one by one).
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ bool has_zero_byte(unsigned w) { return ((w - 0x01010101u) & ~w & 0x80808080u) != 0u; }
-
-__global__ void check_all_true_kernel(const unsigned char* __restrict__ mask, long long n, bool vec, int code,
-                                      int* __restrict__ status) {
-    const long long stride = (long long)gridDim.x * blockDim.x;
-    const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-    bool bad = false;
-    long long tail = 0;
-    if (vec) {
-        const long long nv = n >> 4;
-        const uint4* m4 = reinterpret_cast<const uint4*>(mask);
-        for (long long i = tid; i < nv; i += stride) {
-            const uint4 w = __ldg(m4 + i);
-            bad |= has_zero_byte(w.x) | has_zero_byte(w.y) | has_zero_byte(w.z) | has_zero_byte(w.w);
-        }
-        tail = nv << 4;
-    }
-    for (long long i = tail + tid; i < n; i += stride) bad |= mask[i] == 0;
-    if (__syncthreads_or(bad) && threadIdx.x == 0) atomicCAS(status, 0, code);
-}
 
 }  // namespace bm

@@ -121,4 +121,61 @@ __global__ void scatter_rows_kernel(const float* __restrict__ x, const int* __re
     }
 }
 
+// y[b][c][t] = x[b][c][t] * mask[c]   (simpleconv.py:200-203: `subsample_meg_channels` zeroes the sensors not drawn)
+__global__ void channel_mask_kernel(const float* __restrict__ x, const float* __restrict__ mask, float* __restrict__ y,
+                                    int C, int T, long long total) {
+    for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < total;
+         i += (long long)gridDim.x * blockDim.x) {
+        const int c = (int)((i / T) % C);
+        y[i] = x[i] * mask[c];
+    }
+}
+
+// in [Z][N][T] -> out [Z][T][N]   (32x32 tiles through shared memory, both sides coalesced)
+__global__ void transpose_nt_kernel(const float* __restrict__ in, float* __restrict__ out, int N, int T, int ld_out,
+                                    int n_store) {
+    // n_store = N: plain transpose; n_store = ld_out > N: the pad columns [N, ld_out) are written as zeros
+    __shared__ float tile[32][33];
+    const long long zoff = (long long)blockIdx.z * N * T;
+    const long long zout = (long long)blockIdx.z * T * ld_out;
+    int t = blockIdx.x * 32 + threadIdx.x;
+#pragma unroll
+    for (int i = threadIdx.y; i < 32; i += 8) {
+        int n = blockIdx.y * 32 + i;
+        tile[i][threadIdx.x] = (n < N && t < T) ? in[zoff + (long long)n * T + t] : 0.f;
+    }
+    __syncthreads();
+    int n = blockIdx.y * 32 + threadIdx.x;
+#pragma unroll
+    for (int i = threadIdx.y; i < 32; i += 8) {
+        int tt = blockIdx.x * 32 + i;
+        if (n < n_store && tt < T) out[zout + (long long)tt * ld_out + n] = tile[threadIdx.x][i];
+    }
+}
+
+// ------------------------------------------------------------------------------------------------
+// ClipLoss's `assert mask.all()` (bm/losses.py:110) without a host read: status <- code (if still 0) when any of the n
+// bytes of `mask` is 0.  `vec`: mask is 16-byte aligned, read as uint4 (the last n % 16 bytes one by one).
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ bool has_zero_byte(unsigned w) { return ((w - 0x01010101u) & ~w & 0x80808080u) != 0u; }
+
+__global__ void check_all_true_kernel(const unsigned char* __restrict__ mask, long long n, bool vec, int code,
+                                      int* __restrict__ status) {
+    const long long stride = (long long)gridDim.x * blockDim.x;
+    const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+    bool bad = false;
+    long long tail = 0;
+    if (vec) {
+        const long long nv = n >> 4;
+        const uint4* m4 = reinterpret_cast<const uint4*>(mask);
+        for (long long i = tid; i < nv; i += stride) {
+            const uint4 w = __ldg(m4 + i);
+            bad |= has_zero_byte(w.x) | has_zero_byte(w.y) | has_zero_byte(w.z) | has_zero_byte(w.w);
+        }
+        tail = nv << 4;
+    }
+    for (long long i = tail + tid; i < n; i += stride) bad |= mask[i] == 0;
+    if (__syncthreads_or(bad) && threadIdx.x == 0) atomicCAS(status, 0, code);
+}
+
 }  // namespace bm

@@ -15,7 +15,7 @@
 //   deterministic form (`det`) computes each candidate's sum in one block, which adds onto its zeroed slot exactly once.
 #pragma once
 #include "tc_common.cuh"
-#include "elementwise.cuh"
+#include "clip.cuh"
 
 namespace bm {
 namespace tc {

@@ -398,7 +398,8 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
 // Compiled only with -DBM_HC_PHASES (the shipped library never is: every method below is then empty).  Thread 0 of each
 // warpgroup sums the SM clocks (%clock) spent in each phase over its CTA and adds them to g_hc_phases[kernel][phase]
 // (kernel 0: hc_conv_kernel, 1: hw_wgrad_kernel), which bm_hc_phases() reads back.  Consumer phases are summed over both
-// consumer warpgroups.
+// consumer warpgroups.  Each translation unit that includes this header gets its own copy of the counters: both kernels
+// and bm_hc_phases() live in tc_conv_api.cu.
 enum HcPhase {
     HP_FULL_WAIT,      // consumer: waiting on the full barrier
     HP_SPLIT_ADD,      // consumer: A fragment split + stage release + acc += part

@@ -13,12 +13,11 @@
 // pieces of a power-of-two-scaled copy (bm_tc_weight_split_f16); the pieces are summed back on load (fp16: ~22 significant
 // bits of the weight, the precision the pieces carry).  Fused epilogue: bias, addend (skip gradient / in-place accumulate),
 // pre-activation copy, exact GELU, channel-major store, GLU, BatchNorm column statistics (fp64), max |output|.
-// Every conv entry point of bm_api.cu fills its op and launches it through launch_conv.
+// Every conv entry point of tc_conv_api.cu fills its op and launches it through launch_conv.
 #pragma once
 #include <cuda_fp16.h>
 #include <cstring>
 #include "tc_common.cuh"
-#include "elementwise.cuh"
 
 namespace bm {
 namespace tc {
@@ -503,7 +502,7 @@ __global__ void __launch_bounds__(256) weight_split_f16_kernel(const float* __re
     }
 }
 
-inline int launch_amax(const float* x, long long n, float* cell, cudaStream_t st) {
+int launch_amax(const float* x, long long n, float* cell, cudaStream_t st) {
     cudaError_t e = cudaMemsetAsync(cell, 0, 4, st);
     if (e != cudaSuccess) return set_error(3, "%s: memset: %s", __func__, cudaGetErrorString(e));
     long long blocks = (n / 4 + 255) / 256;

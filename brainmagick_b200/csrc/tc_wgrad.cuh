@@ -10,8 +10,8 @@
 // `wgrad_reduce_kernel` sums the batch slices in a fixed order (deterministic) into the nn.Conv1d layout [m][n][tap];
 // "direct" calls (one tap, one slice) write the output itself, and the grouped form writes one plane per group.
 #pragma once
+#include "../../include/bm_b200.h"
 #include "tc_common.cuh"
-#include "elementwise.cuh"
 
 namespace bm {
 namespace tc {
@@ -40,7 +40,7 @@ inline int wgrad_pick_nh(int N) {
         if (N % (2 * nh) == 0) return nh;
     return 0;
 }
-inline bool wgrad_tc_supported(int M, int N) { return wgrad_pick_nh(N) != 0 && M >= 32 && (M % 4) == 0; }
+bool wgrad_tc_supported(int M, int N) { return wgrad_pick_nh(N) != 0 && M >= 32 && (M % 4) == 0; }
 inline void wgrad_geometry(int B, int M, int N, int taps, int* nh, int* mblocks, int* ksplit, int* bchunk) {
     *nh = wgrad_pick_nh(N);
     *mblocks = (M + WG_BM - 1) / WG_BM;
@@ -106,8 +106,8 @@ struct WgradOp {
 };
 
 // dY [B,T,M], X [B,T,N] -> dW [M][Ntrue][taps]; ws: wgrad_workspace_floats() floats
-inline int launch_wgrad_tc(const float* dY, const float* X, int B, int T, int M, int N, int Ntrue, int taps,
-                           int dilation, float* ws, float* dW, int passes, cudaStream_t st, float* dbias = nullptr) {
+int launch_wgrad_tc(const float* dY, const float* X, int B, int T, int M, int N, int Ntrue, int taps, int dilation,
+                    float* ws, float* dW, int passes, cudaStream_t st, float* dbias) {
     int nh, mblocks, ksplit, bchunk;
     wgrad_geometry(B, M, N, taps, &nh, &mblocks, &ksplit, &bchunk);
     if (nh == 0) return set_error(2, "%s: unsupported N%s", __func__);
@@ -121,15 +121,8 @@ inline int launch_wgrad_tc(const float* dY, const float* X, int B, int T, int M,
     o.plane = (long long)(direct ? M : Mpad) * N;
     o.rows = direct ? M : Mpad;
     if (int rc = hg_launch_bn(bn, o, dim3(o.ntiles * taps, mblocks, ksplit), passes, st, __func__)) return rc;
-    if (dbias) {               // bias gradient sum_{b,t} dY[b,t,m]
-        cudaError_t em = cudaMemsetAsync(dbias, 0, sizeof(float) * M, st);
-        if (em != cudaSuccess) return set_error(3, "%s: memset: %s", __func__, cudaGetErrorString(em));
-        const long long rows = (long long)B * T;
-        colsum_cl_kernel<<<dim3((unsigned)((rows + 255) / 256), (M + 127) / 128), 128, 0, st>>>(dY, dbias, rows, M, 256);
-        ++g_launches;
-        cudaError_t e = cudaGetLastError();
-        if (e != cudaSuccess) return set_error(3, "%s: bias launch failed: %s", __func__, cudaGetErrorString(e));
-    }
+    if (dbias)                 // bias gradient sum_{b,t} dY[b,t,m]
+        if (int rc = bm_col_sum(dY, (long long)B * T, M, dbias, st)) return rc;
     if (direct) return 0;
     wgrad_reduce_kernel<<<ew_grid((long long)M * Ntrue * taps), 256, 0, st>>>(ws, dW, taps, ksplit, Mpad, M, N, Ntrue);
     ++g_launches;

@@ -30,7 +30,6 @@ import argparse
 import ctypes
 import json
 import os
-import subprocess
 import sys
 import tempfile
 
@@ -60,14 +59,7 @@ NSETS = 4
 
 
 def compile_probe(csrc, outdir):
-    lib = os.path.join(outdir, "libbm_b200_phases.so")
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc] + build.NVCC_FLAGS + ["-DBM_HC_PHASES", os.path.join(csrc, "bm_api.cu"), "-o", lib, "-lcudart"]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if res.returncode != 0:
-        sys.stderr.write(res.stdout + res.stderr)
-        raise RuntimeError("nvcc failed building the probe library")
-    return lib
+    return build.compile_library(os.path.join(outdir, "libbm_b200_phases.so"), ["-DBM_HC_PHASES"], csrc=csrc)
 
 
 def conv_call(name, suffix, dev):

@@ -1,6 +1,7 @@
 """GPU: every C entry point that is not a contraction -- the ConvSequence layer epilogue (csrc/convseq.cuh), the BatchNorm
 finalize, the column reductions, the GLU / GELU backward, the attention pieces, the layouts and the ClipLoss norms
-(csrc/elementwise.cuh) -- against a plain fp64 reference, element by element, on each of its kernel forms.
+(csrc/elementwise.cuh, front.cuh, prep.cuh, clip.cuh) -- against a plain fp64 reference, element by element, on each of its
+kernel forms.
 
 The reference is computed in fp64 from the fp32 operands the kernel read.  Each output is held to a componentwise bound
 

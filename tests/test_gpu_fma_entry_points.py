@@ -40,7 +40,7 @@ def _sms():
 
 
 def _split(B, tiles):
-    """(nseg, zchunk) of the split-batch weight-gradient GEMMs (bm_api.cu pick_chunks)"""
+    """(nseg, zchunk) of the split-batch weight-gradient GEMMs (csrc/api.cuh pick_chunks)"""
     want = min(max(1, -(-2 * _sms() // tiles)), B)
     zchunk = -(-B // want)
     return -(-B // zchunk), zchunk
